@@ -11,7 +11,7 @@ reached through the C ABI of include/dfb200.h.  There is no CPU fallback.
 from . import libdf  # noqa: F401
 from .config import ModelConfig, load_config  # noqa: F401
 from .dropin import install_dropin  # noqa: F401
-from .enhance import df_features, enhance, enhance_device, init_df  # noqa: F401
+from .enhance import df_features, enhance, enhance_batch, enhance_device, enhance_device_ragged, init_df  # noqa: F401
 from .model import DfNet, load_model  # noqa: F401
 from .streaming import DfStream  # noqa: F401
 

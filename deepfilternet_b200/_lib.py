@@ -84,6 +84,8 @@ SIGNATURES = {
     "dfb_enhance": (_I, [_VP, _VP, _VP, _I64, _I64, _I, _F, _VP, _VP]),
     "dfb_enhance_host": (_I, [_VP, _VP, _VP, _I64, _I64, _I, _F, _VP]),
     "dfb_enhance_out_len": (_I64, [_VP, _I64, _I]),
+    "dfb_enhance_ragged": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP]),
+    "dfb_enhance_ragged_host": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP]),
     "dfb_model_workspace_bytes": (_I64, [_VP]),
     "dfb_stream_create": (_I, [C.POINTER(_VP), _VP, _VP, _I64, _F]),
     "dfb_stream_free": (None, [_VP]),

@@ -119,6 +119,11 @@ struct DspTables {
     int fft, hop, F, E;
 };
 
+// One stream of a ragged batch (dfb_enhance_ragged), in the executor's order (longest first): its samples are
+// audio[in_off, in_off + len), its result out[out_off, out_off + out_len), and it has Tf STFT frames.  Kernels that take a
+// table index their rows with it; a null table means every row has the call's common length.
+struct RaggedRow { int64_t in_off, len, out_off, out_len, Tf; };
+
 // Parameters of the fused apply + synthesis kernel (dfb_dsp.cu).
 // mode 0: plain ISTFT; 1: DeepFilterNet3 (DF on the noisy spectrum); 2: DeepFilterNet2 (DF on the
 // masked spectrum).
@@ -155,6 +160,12 @@ struct ApplyParams {
     const float *init_tail;  // [hop] or null
     float *final_tail;       // [hop] or null
     int carry;
+    // ragged batch (or null): row b reads rows[b] for its output row and its end.  Window frame t is absolute frame w0 + t;
+    // spectrum rows >= rows[b].Tf - w0 do not exist, and the stream synthesises frames up to rows[b].Tf - w0 when that is
+    // <= Tf (it ends in this window), else up to t_emit
+    const RaggedRow *rows;
+    int64_t w0;
+    int t_emit;
 };
 
 }  // namespace dfb
@@ -162,8 +173,9 @@ struct ApplyParams {
 struct dfb_state;
 namespace dfb {
 // frame window of launch_analysis: frames [t_begin, t_begin + nf) of a signal of T samples per row (row pitch row_stride,
-// 0 = T) go to rows out_t0 ... of buffers holding Tbuf frames per stream
-struct AnaWindow { int t_begin, nf, out_t0, Tbuf; int64_t row_stride; };
+// 0 = T) go to rows out_t0 ... of buffers holding Tbuf frames per stream.  rows (ragged batch, or null): stream b starts
+// at audio + rows[b].in_off and its samples >= rows[b].len read as zero
+struct AnaWindow { int t_begin, nf, out_t0, Tbuf; int64_t row_stride; const RaggedRow *rows = nullptr; };
 int launch_analysis(dfb_state *st, const float *d_audio, int64_t C, int64_t T, float *d_spec, float *d_erb_db,
                     cudaStream_t s, const float *d_init_mem = nullptr, const AnaWindow *w = nullptr);
 // Ts: frames per stream in the buffers (0 = Tf; pointers pre-offset to the first frame); *_state_out: EMA states after

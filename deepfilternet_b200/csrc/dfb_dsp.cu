@@ -145,10 +145,14 @@ __device__ __forceinline__ void warp_fft480_twptr(LoadF load, const float2 *tw_l
 // Frame window: the grid covers frames [t_begin, t_begin + nf) of every stream (time-chunked execution); their rows
 // go to out_t0 ... of spec / erb_db buffers that hold Tbuf frames per stream.  The whole-signal call is
 // (t_begin, nf, out_t0, Tbuf) = (0, Tf, 0, Tf).
+// Ragged batch (rows != null): stream b starts at audio + rows[b].in_off and reads zeros from sample rows[b].len on, so the
+// `pad` zeros of enhance() are implicit and no padded copy of the input is needed (RG: its own instantiation, so that the
+// equal-length kernel is compiled as without it).
+template <bool RG>
 __global__ void __launch_bounds__(32 * kAnaWarps, 4)
 k_analysis(const float *__restrict__ audio, int64_t T, int Tf, float2 *__restrict__ spec,
            float *__restrict__ erb_db, DspTables tb, const float *__restrict__ init_mem, int t_begin, int nf, int out_t0,
-           int Tbuf) {
+           int Tbuf, const RaggedRow *__restrict__ rows) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float *s_stage = reinterpret_cast<float *>(smem_raw);                    // (W + 1) * hop
     float *s_win = s_stage + (kAnaWarps + 1) * kHop;                         // fft
@@ -157,8 +161,8 @@ k_analysis(const float *__restrict__ audio, int64_t T, int Tf, float2 *__restric
     float2 *s_buf = s_twa + kN2 * kN1;                                       // W * kTileFloat2
     const int b = blockIdx.y, tl0 = blockIdx.x * kAnaWarps, t0 = t_begin + tl0;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const float *x = audio + (int64_t)b * T;
-    const int64_t s_end = (int64_t)Tf * kHop;
+    const float *x = audio + (RG ? rows[b].in_off : (int64_t)b * T);
+    const int64_t s_end = RG ? min((int64_t)Tf * kHop, rows[b].len) : (int64_t)Tf * kHop;
     // stage samples [(t0-1)*hop, (t0+W)*hop); zeros before the stream start (analysis_mem = 0).  All 17 loads of a thread
     // are issued into registers before the first store: as a load / store loop with the bounds checks inside, the compiler
     // kept them in program order -- 17 dependent round trips to L2 / HBM per CTA.
@@ -525,8 +529,8 @@ __device__ __forceinline__ float pf_gain_spec(float2 y, float2 x, float beta) {
 }
 
 __device__ __forceinline__ float2 apply_bin(const ApplyParams &p, const DspTables &tb, const float2 *srow0,
-                                            const float *mrow0, const float *crow, int t, int k) {
-    // srow0 / mrow0: row pointers of frame 0 of this stream
+                                            const float *mrow0, const float *crow, int t, int k, int Tv) {
+    // srow0 / mrow0: row pointers of frame 0 of this stream; spectrum rows >= Tv do not exist
     float2 x = srow0[(int64_t)t * kF + k];
     float2 y;
     if (p.mode == 0) return x;
@@ -542,7 +546,7 @@ __device__ __forceinline__ float2 apply_bin(const ApplyParams &p, const DspTable
         float yr = 0.f, yi = 0.f;
         for (int o = 0; o < p.order; o++) {
             int tt = t + o - (p.order - 1 - p.lookahead);
-            if (tt < 0 || tt >= (p.Tv ? p.Tv : p.Tf)) continue;
+            if (tt < 0 || tt >= Tv) continue;
             float2 s = srow0[(int64_t)tt * kF + k];
             if (p.mode == 2 && tt < (p.mc_T ? p.mc_T : p.Tf)) {
                 float g = mrow0[(int64_t)tt * tb.E + band];
@@ -584,8 +588,19 @@ __global__ void __launch_bounds__(32 * kSynWarps) k_apply_synthesis_generic(Appl
     __syncthreads();
     const int syn_chunk = p.frames_per_warp ? p.frames_per_warp : kSynChunk;
     const int t0 = (blockIdx.x * kSynWarps + warp) * syn_chunk;
-    if (t0 >= p.Tf) return;
-    const int t1 = min(t0 + syn_chunk, p.Tf);
+    int Te = p.Tf, Tv = p.Tv ? p.Tv : p.Tf;     // frames this stream synthesises / spectrum rows that exist
+    float *orow = p.audio ? p.audio + (int64_t)b * p.out_stride : nullptr;
+    int64_t out_len = p.out_len;
+    if (p.rows) {
+        const RaggedRow r = p.rows[b];
+        const int tfb = (int)(r.Tf - p.w0);
+        Te = tfb <= p.Tf ? tfb : p.t_emit;
+        Tv = min(Tv, tfb);
+        if (orow) orow = p.audio + r.out_off;
+        out_len = r.out_len;
+    }
+    if (t0 >= Te) return;
+    const int t1 = min(t0 + syn_chunk, Te);
     const float2 *srow0 = p.spec + (int64_t)b * (p.spec_T ? p.spec_T : p.Tf) * kF;
     const int mcT = p.mc_T ? p.mc_T : p.Tf;
     const float *mrow0 = p.m ? p.m + (int64_t)b * mcT * tb.E : nullptr;
@@ -604,8 +619,8 @@ __global__ void __launch_bounds__(32 * kSynWarps) k_apply_synthesis_generic(Appl
         for (int j = 0; j < 8; j++) {
             int k = lane + 32 * j;
             if (k <= 240) {
-                float2 xk = apply_bin(p, tb, srow0, mrow0, crow, t, k);
-                float2 xnk = apply_bin(p, tb, srow0, mrow0, crow, t, kC - k);
+                float2 xk = apply_bin(p, tb, srow0, mrow0, crow, t, k, Tv);
+                float2 xnk = apply_bin(p, tb, srow0, mrow0, crow, t, kC - k, Tv);
                 if (p.spec_out && t >= t0) {
                     float2 *orow = p.spec_out + ((int64_t)b * p.Tf + t) * kF;
                     orow[k] = xk;
@@ -632,14 +647,13 @@ __global__ void __launch_bounds__(32 * kSynWarps) k_apply_synthesis_generic(Appl
                 nat[n] = make_float2(v.x * w.x, v.y * w.y);
             }
             __syncwarp();
-            float *orow = p.audio + (int64_t)b * p.out_stride;
 #pragma unroll
             for (int j = 0; j < 15; j++) {
                 int i = lane + 32 * j;
                 float o = yb[i] + tail[j];      // lib.rs:407-411
                 tail[j] = yb[kHop + i];         // lib.rs:423-426 (hop == fft/2)
                 int64_t g = (int64_t)t * kHop + i - p.out_offset;
-                if (t >= t0 && t >= p.t_first && g >= 0 && g < p.out_len) orow[g] = o;
+                if (t >= t0 && t >= p.t_first && g >= 0 && g < out_len) orow[g] = o;
             }
         }
         __syncwarp();
@@ -655,7 +669,8 @@ __global__ void __launch_bounds__(32 * kSynWarps) k_apply_synthesis_generic(Appl
 // bins lives in registers as a 5-deep shift register (one new look-ahead value per bin and frame instead of
 // five reloads), the band gains come from one register per lane via warp shuffles, and all global loads of
 // a frame are issued up front, coalesced (256-byte rows), before any use.
-template <int ORDER, int NDFJ, int MINB>
+// RG: ragged batch (p.rows), a separate instantiation so that the equal-length path compiles exactly as without it.
+template <int ORDER, int NDFJ, int MINB, bool RG>
 __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyParams p, DspTables tb) {
     __shared__ __align__(16) float s_win[kFft];
     __shared__ __align__(16) float2 s_tw960[241];
@@ -669,10 +684,19 @@ __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyP
     __syncthreads();
     const int syn_chunk = p.frames_per_warp ? p.frames_per_warp : kSynChunk;
     const int t0 = (blockIdx.x * kSynWarps + warp) * syn_chunk;
-    if (t0 >= p.Tf) return;
-    const int t1 = min(t0 + syn_chunk, p.Tf);
     const int Tf = p.Tf, L = p.lookahead, back = ORDER - 1 - L;
-    const int Tv = p.Tv ? p.Tv : Tf;                       // spectrum rows >= Tv do not exist (end of the stream)
+    int Te = Tf, Tv = p.Tv ? p.Tv : Tf;                    // frames synthesised; spectrum rows >= Tv do not exist (end of the stream)
+    int64_t orow0 = (int64_t)b * p.out_stride, out_len = p.out_len;
+    if constexpr (RG) {                                    // ragged batch: this stream's own end and output row
+        const RaggedRow r = p.rows[b];
+        const int tfb = (int)(r.Tf - p.w0);
+        Te = tfb <= Tf ? tfb : p.t_emit;
+        Tv = min(Tv, tfb);
+        orow0 = r.out_off;
+        out_len = r.out_len;
+    }
+    if (t0 >= Te) return;
+    const int t1 = min(t0 + syn_chunk, Te);
     const float2 *srow0 = p.spec + (int64_t)b * (p.spec_T ? p.spec_T : Tf) * kF;
     const int mcT = p.mc_T ? p.mc_T : Tf;                  // m / coefs rows per stream
     const float *mrow0 = p.m + (int64_t)b * mcT * 32;
@@ -803,14 +827,14 @@ __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyP
                 nat[n] = make_float2(v.x * w.x, v.y * w.y);
             }
             __syncwarp();
-            float *orow = p.audio + (int64_t)b * p.out_stride;
+            float *orow = p.audio + orow0;
 #pragma unroll
             for (int j = 0; j < 15; j++) {
                 int i = lane + 32 * j;
                 float o = yb[i] + tail[j];      // lib.rs:407-411
                 tail[j] = yb[kHop + i];         // lib.rs:423-426 (hop == fft/2)
                 int64_t g = (int64_t)t * kHop + i - p.out_offset;
-                if (t >= t0 && t >= p.t_first && g >= 0 && g < p.out_len) orow[g] = o;
+                if (t >= t0 && t >= p.t_first && g >= 0 && g < out_len) orow[g] = o;
             }
         }
         __syncwarp();
@@ -975,7 +999,8 @@ extern "C" int dfb_state_create(dfb_state **out, int device, int sr, int fft_siz
     st->tb.band_of_bin = (const unsigned char *)(d + o_bob);
     st->tb.wnorm = 1.f / ((float)((int64_t)fft_size * fft_size) / (float)(2 * hop_size));  // lib.rs:133
     st->tb.fft = fft_size; st->tb.hop = hop_size; st->tb.F = F; st->tb.E = nb_erb;
-    cudaFuncSetAttribute(k_analysis, cudaFuncAttributeMaxDynamicSharedMemorySize, kAnaSmem);
+    cudaFuncSetAttribute(k_analysis<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAnaSmem);
+    cudaFuncSetAttribute(k_analysis<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAnaSmem);
     if (cudaStreamCreateWithFlags(&st->stream, cudaStreamNonBlocking) != cudaSuccess) {
         cudaFree(d);
         delete st;
@@ -1024,8 +1049,13 @@ int launch_analysis(dfb_state *st, const float *d_audio, int64_t C, int64_t T, f
     if (nf <= 0) return DFB_OK;
     dim3 grid((unsigned)((nf + kAnaWarps - 1) / kAnaWarps), (unsigned)C);
     DFB_PROF("k_analysis", s);
-    k_analysis<<<grid, 32 * kAnaWarps, kAnaSmem, s>>>(d_audio, w && w->row_stride ? w->row_stride : T, (int)Tf, (float2 *)d_spec,
-                                                     d_erb_db, st->tb, d_init_mem, t_begin, nf, out_t0, Tbuf);
+    const int64_t stride = w && w->row_stride ? w->row_stride : T;
+    if (w && w->rows)
+        k_analysis<true><<<grid, 32 * kAnaWarps, kAnaSmem, s>>>(d_audio, stride, (int)Tf, (float2 *)d_spec, d_erb_db, st->tb, d_init_mem,
+                                                              t_begin, nf, out_t0, Tbuf, w->rows);
+    else
+        k_analysis<false><<<grid, 32 * kAnaWarps, kAnaSmem, s>>>(d_audio, stride, (int)Tf, (float2 *)d_spec, d_erb_db, st->tb, d_init_mem,
+                                                               t_begin, nf, out_t0, Tbuf, nullptr);
     DFB_LAUNCH_CHECK();
     return DFB_OK;
 }
@@ -1069,10 +1099,13 @@ int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaS
         return fail(DFB_ERR_UNSUPPORTED, "LSNR stage gating is built for the DeepFilterNet3 apply kernel only");
     DFB_PROF("k_apply_synthesis", s);
     static const int minb = getenv("DFB_APPLY_MINB") ? atoi(getenv("DFB_APPLY_MINB")) : 2;  // 2 CTAs/SM without spills measured fastest
-    if (p.mode != 0 && p.order == 5 && p.nb_df == 96 && st->tb.E == 32 && p.m && p.coefs && minb == 3)
-        k_apply_synthesis<5, 3, 3><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
-    else if (p.mode != 0 && p.order == 5 && p.nb_df == 96 && st->tb.E == 32 && p.m && p.coefs && minb == 2)
-        k_apply_synthesis<5, 3, 2><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
+    const bool special = p.mode != 0 && p.order == 5 && p.nb_df == 96 && st->tb.E == 32 && p.m && p.coefs;
+    if (special && p.rows)
+        k_apply_synthesis<5, 3, 2, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
+    else if (special && minb == 3)
+        k_apply_synthesis<5, 3, 3, false><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
+    else if (special && minb == 2)
+        k_apply_synthesis<5, 3, 2, false><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
     else
         k_apply_synthesis_generic<<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
     DFB_LAUNCH_CHECK();

@@ -16,6 +16,7 @@
 #include <cooperative_groups.h>
 #include <cuda_bf16.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <functional>
@@ -58,10 +59,12 @@ k_conv_in(const float *__restrict__ x, const float *__restrict__ w /*[kt][3][CIN
           float *__restrict__ out, int T, int F, int kt, int lookahead, int Tsx /* frames per stream in x */,
           int Tx /* feature frames that exist; beyond = end of the stream = zero */,
           int tp_min /* 0: the features are shifted by the look-ahead, then padded causally (DeepFilterNet2 / 3, pad_feat);
-                        -lookahead: the conv itself pads (kt-1-la, la) around the unshifted features (DeepFilterNet v1) */) {
+                        -lookahead: the conv itself pads (kt-1-la, la) around the unshifted features (DeepFilterNet v1) */,
+          const RaggedRow *__restrict__ rg /* ragged batch: stream b's features end at its own frame count */, int64_t w0 /* absolute frame of window row 0 */) {
     extern __shared__ float s_in[];  // [(kInFrames + kt - 1)][(F + 2) * CIN]
     const int b = blockIdx.y, t0 = blockIdx.x * kInFrames;
     const int rows = kInFrames + kt - 1, ld = (F + 2) * CIN;
+    if (rg) Tx = min(Tx, (int)(rg[b].Tf - w0));
     for (int i = threadIdx.x; i < rows * ld; i += blockDim.x) {
         int r = i / ld, j = i - r * ld;
         int f = j / CIN - 1, ci = j - (f + 1) * CIN;
@@ -815,8 +818,9 @@ using namespace dfb;
 
 
 struct GruLayerW { const float *w_ih_t, *w_hh, *b_ih, *b_hh; int in_dim; };
-// carried hidden states of one GRU stack between time chunks: h = [layers][B][H]; t0 = first frame the recurrences run
-struct GruChunk { float *h; bool have_state; int t0; };
+// carried hidden states of one GRU stack between time chunks: h = [layers][Bs][H]; t0 = first frame the recurrences run.
+// Bs is the stream count the state was allocated for: a chunk may run only a prefix B <= Bs of the streams (ragged batch)
+struct GruChunk { float *h; bool have_state; int t0; int Bs; };
 
 struct dfb_model {
     int device;
@@ -1092,7 +1096,7 @@ int run_gru(dfb_model *m, cudaStream_t s, const char *name, int layers, int H, c
         }
         if (rc) return rc;
         float *dst = (l == layers - 1) ? y : tmp_h;
-        float *hs = ck && ck->h ? ck->h + (int64_t)l * B * H : nullptr;   // carried state of this layer [B][H]
+        float *hs = ck && ck->h ? ck->h + (int64_t)l * ck->Bs * H : nullptr;   // carried state of this layer [Bs][H], rows [0, B)
         GruWindow gw{ck && ck->have_state ? hs : nullptr, hs, t0, T};
         GruParams p{xproj, w_hh, b_hh, (l == layers - 1) ? res_last : nullptr, dst, B, Tn, 0, m->gru_dbg, gw.h0, gw.hT, t0, T};
         if (tc_gru) {
@@ -1238,6 +1242,9 @@ struct ChunkCtx {
     int dec_tail_n;                // frames of dec_tail that are valid
     int lane;                      // which of the model's two stream / event sets (and arenas) this chunk runs on
     cudaEvent_t wait_dec;          // previous chunk finished (its decoder states / tails are final) or null
+    int Bs;                        // streams the GRU states were allocated for (layer stride); the window runs rows [0, B)
+    const RaggedRow *rows;         // ragged batch: per-stream frame counts (features end at rows[b].Tf), or null
+    int64_t W0;                    // absolute frame of window row 0
 };
 constexpr int kHalo = 8;           // >= temporal receptive field of every feed-forward chain of the shipped models
 
@@ -1281,9 +1288,11 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
                         float *d_m, float *d_coefs, float *d_lsnr, float *d_alpha, cudaStream_t s_in, ChunkCtx *cx) {
     const dfb_model_config &c = m->cfg;
     const int Tsx = cx ? cx->Tsx : T, Tx = cx ? cx->Tx : T;
-    GruChunk ck_enc{cx ? cx->h_enc : nullptr, cx && cx->have_state, cx ? cx->Rc : 0};
-    GruChunk ck_erb{cx ? cx->h_erb : nullptr, cx && cx->have_state, cx ? cx->Rc : 0};
-    GruChunk ck_df{cx ? cx->h_df : nullptr, cx && cx->have_state, cx ? cx->Rc : 0};
+    GruChunk ck_enc{cx ? cx->h_enc : nullptr, cx && cx->have_state, cx ? cx->Rc : 0, cx ? cx->Bs : B};
+    GruChunk ck_erb{cx ? cx->h_erb : nullptr, cx && cx->have_state, cx ? cx->Rc : 0, cx ? cx->Bs : B};
+    GruChunk ck_df{cx ? cx->h_df : nullptr, cx && cx->have_state, cx ? cx->Rc : 0, cx ? cx->Bs : B};
+    const RaggedRow *rows = cx ? cx->rows : nullptr;
+    const int64_t W0 = cx ? cx->W0 : 0;
     // DFB_SERIAL=1: everything on the caller's stream (profiling: per-kernel times without overlap)
     static const bool serial = getenv("DFB_SERIAL") && atoi(getenv("DFB_SERIAL"));
     dfb_model::Lane &L = m->lanes[cx ? cx->lane : 0];
@@ -1367,7 +1376,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         dim3 grid((unsigned)((T + kInFrames - 1) / kInFrames), (unsigned)B);
         int smem = (kInFrames + c.inp_kt - 1) * (E + 2) * 4;
         DFB_PROF("k_conv_in[erb_conv0]", s);
-        k_conv_in<1><<<grid, 256, smem, s>>>(d_feat_erb, w, bb, f.e0, T, E, c.inp_kt, c.conv_lookahead, Tsx, Tx, 0);
+        k_conv_in<1><<<grid, 256, smem, s>>>(d_feat_erb, w, bb, f.e0, T, E, c.inp_kt, c.conv_lookahead, Tsx, Tx, 0, rows, W0);
         DFB_LAUNCH_CHECK();
     }
     const float *pw_sw = nullptr;  // set by blk(): swizzled BF16 hi | lo image of the [C_out][C_in] 1x1 weights (tensor-core path)
@@ -1399,7 +1408,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
             dim3 grid((unsigned)((T + kInFrames - 1) / kInFrames), (unsigned)B);
             int smem = (kInFrames + c.inp_kt - 1) * (Fd + 2) * 2 * 4;
             DFB_PROF("k_conv_in[df_conv0]", sa);
-            k_conv_in<2><<<grid, 256, smem, sa>>>(d_feat_spec, w, bb, f.c0, T, Fd, c.inp_kt, c.conv_lookahead, Tsx, Tx, 0);
+            k_conv_in<2><<<grid, 256, smem, sa>>>(d_feat_spec, w, bb, f.c0, T, Fd, c.inp_kt, c.conv_lookahead, Tsx, Tx, 0, rows, W0);
             DFB_LAUNCH_CHECK();
             DFB_CUDA(cudaEventRecord(L.ev_c0, sa));
         }
@@ -1687,13 +1696,14 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
         const int la = c.conv_lookahead > 0 ? 1 : 0;
         {
             DFB_PROF("k_conv_in[erb_conv0]", s);
-            k_conv_in<1><<<grid, 256, (kInFrames + c.inp_kt - 1) * (E + 2) * 4, s>>>(d_feat_erb, w, bb, f.e0, T, E, c.inp_kt, la, Tsx, Tx, -la);
+            k_conv_in<1><<<grid, 256, (kInFrames + c.inp_kt - 1) * (E + 2) * 4, s>>>(d_feat_erb, w, bb, f.e0, T, E, c.inp_kt, la, Tsx, Tx, -la,
+                                                                                      nullptr, 0);
             DFB_LAUNCH_CHECK();
         }
         if ((rc = need(m, "enc.df_conv0.w", c.inp_kt * 3 * 2 * kCh, &w)) || (rc = need(m, "enc.df_conv0.b", kCh, &bb))) return rc;
         DFB_PROF("k_conv_in[df_conv0]", sa);
         k_conv_in<2><<<grid, 256, (kInFrames + c.inp_kt - 1) * (Fd + 2) * 2 * 4, sa>>>(d_feat_spec, w, bb, f.c0, T, Fd, c.inp_kt, c.conv_lookahead,
-                                                                                      Tsx, Tx, -c.conv_lookahead);
+                                                                                      Tsx, Tx, -c.conv_lookahead, nullptr, 0);
         DFB_LAUNCH_CHECK();
     }
     if ((rc = block(sa, "enc.df_conv1", DW_S2, f.c0, Fd, f.c1, Fd / 2, kt, 0, nullptr))) return rc;
@@ -1723,7 +1733,7 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
         unsigned short *ch = x_hi, *cl = x_lo;
         for (int l = 0; l < layers; l++) {
             const std::string nm = std::string(name) + ".g" + std::to_string(l);
-            GruChunk ck{hbase ? hbase + (int64_t)l * B * H : nullptr, false, 0};
+            GruChunk ck{hbase ? hbase + (int64_t)l * B * H : nullptr, false, 0, B};
             bool ok = false;
             int r = run_gru(m, st, nm.c_str(), 1, H, cur, H, nullptr, y[l], xproj, nullptr, B, T, ch, cl, f.scr_hi, f.scr_lo, 0, y_hi[l], y_lo[l], &ok,
                             hbase ? &ck : nullptr);
@@ -1998,10 +2008,15 @@ struct ChunkIO {
     int64_t out_sample0;      // absolute synthesis sample (frame * hop + i) that lands at out[0]
     float atten_lim;
     const float *lsnr_th;     // {min_db_thresh, max_db_erb_thresh, max_db_df_thresh} (tract.rs:658-672) or null: no gating
+    // ragged batch (dfb_enhance_ragged): per-stream input / output rows and frame counts (device table, streams sorted
+    // longest first), and how many of them still have frames in this chunk (a prefix); null / 0: all S.B streams alike
+    const RaggedRow *rows = nullptr;
+    int nb = 0;
 };
 
 // One chunk: analyse frames [S.a1, a1n), run the DNN over [S.d1, d1n), emit audio of frames [S.e1, e1n).
-// Tf_end: total frames of the stream when known (features / spectrum beyond it are zero), else -1.
+// Ragged batch (io.rows): only the first io.nb streams run; a stream whose frame count Tf_b is <= d1n ends in this chunk:
+// its features and spectrum beyond Tf_b do not exist and it emits all of its frames up to Tf_b.
 // lane / pipelined: consecutive chunks of a batch call alternate between the model's two lanes (stream sets + arenas);
 // chunk c starts when chunk c - 1 has finished its ENCODER phase and its decoder phase waits for chunk c - 1 to finish
 // entirely, so encoder(c) overlaps decoder(c - 1).  `s` is the stream the chunk is enqueued on (the lane's main stream
@@ -2014,7 +2029,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     if (have_prev) DFB_CUDA(cudaStreamWaitEvent(s, P.ev_fork, 0));   // previous chunk: features + encoder phase done
     const dfb_model_config &c = m->cfg;
     const ChunkGeom g = chunk_geom(c);
-    const int B = S.B, E = c.nb_erb, Fd = c.nb_df, O2 = 2 * c.df_order, F = st->tb.F, hop = st->hop, ED = E / 4 * kCh;
+    const int B = io.nb > 0 ? io.nb : S.B, E = c.nb_erb, Fd = c.nb_df, O2 = 2 * c.df_order, F = st->tb.F, hop = st->hop, ED = E / 4 * kCh;
     const int64_t W0 = S.d1 > kHalo ? S.d1 - kHalo : 0;
     const int Rc = (int)(S.d1 - W0), Tw = (int)(d1n - W0), Tsb = Tw + g.Lmax;
     const int n_hist = (int)(S.a1 - W0);                 // feature frames of the window that are already known
@@ -2037,7 +2052,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
         (rc = load_tail(s, fs, Tsb, (size_t)2 * Fd, n_hist, S.t_fs, g.Hf, 0, B)))
         return rc;
     if (n_new > 0) {
-        AnaWindow w{(int)(S.a1 - io.audio_frame0), n_new, n_hist, Tsb, io.audio_stride};
+        AnaWindow w{(int)(S.a1 - io.audio_frame0), n_new, n_hist, Tsb, io.audio_stride, io.rows};
         if ((rc = launch_analysis(st, io.audio, B, io.audio_T, spec, fe, s, io.init_mem, &w))) return rc;
         if ((rc = launch_feat_norm(fe + (size_t)n_hist * E, E, E, spec + (size_t)n_hist * 2 * F, Fd, F, B, n_new, c.norm_alpha,
                                    S.started ? S.erb_state : nullptr, S.started ? S.unit_state : nullptr, fe + (size_t)n_hist * E,
@@ -2058,7 +2073,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     // ---- DNN over the window
     if (run_dnn) {
     ChunkCtx cx{Rc, Tsb, Tv, S.h_enc, S.h_erb, S.h_df, S.dnn_started, c.conv_kt > 1 ? S.t_dec : nullptr, S.n_dec, lane,
-                have_prev ? P.ev_done : nullptr};
+                have_prev ? P.ev_done : nullptr, S.B, io.rows, W0};
     if ((rc = forward_impl(m, arena, fe, fs, B, Tw, mm, cc, ll, aa, s, &cx))) return rc;
     S.n_dec = cx.dec_tail_n;
     S.dnn_started = true;
@@ -2071,8 +2086,8 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
         if (ll && (rc = load_tail(s, ll, Tw, 1, n, S.t_l, kMcTail, Rc - n, B))) return rc;
     }
     }
-    // ---- apply + synthesis of frames [e0, e1n)
-    if (run_dnn && e1n > S.e1) {
+    // ---- apply + synthesis of frames [e0, e1n) (ragged: a stream that ends in this chunk emits up to its end)
+    if (run_dnn && (e1n > S.e1 || io.rows)) {
         dfb::ApplyParams p{};
         p.spec = (const float2 *)spec; p.m = mm; p.coefs = cc; p.audio = io.out; p.spec_out = nullptr;
         p.out_stride = io.out_stride; p.out_len = io.out_len;
@@ -2083,6 +2098,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
         p.alpha = aa;
         apply_options(m, p);
         if (ll) { p.lsnr = ll; p.th_min = io.lsnr_th[0]; p.th_erb = io.lsnr_th[1]; p.th_df = io.lsnr_th[2]; }
+        if (io.rows) { p.rows = io.rows; p.w0 = W0; p.t_emit = p.Tf; p.Tf = Tw; }   // the grid covers every stream's end
         if ((rc = launch_apply_synthesis(st, p, B, s))) return rc;
     }
     // ---- carry
@@ -2124,17 +2140,22 @@ static int pick_chunk(const dfb_model *m, const dfb_state *st, int64_t B, int64_
 // `before` / `after` are called around every chunk with the sample ranges it reads / has written).
 struct ChunkHooks {
     // analysis of this chunk reads input samples [x0, x1) of every stream; output samples [y0, y1) have been written
-    // `cs` is the stream the chunk's compute is enqueued on (must wait for the input / produces the output)
-    std::function<int(int64_t x0, int64_t x1, cudaStream_t cs)> before;
-    std::function<int(int64_t y0, int64_t y1, cudaStream_t cs)> after;
+    // `cs` is the stream the chunk's compute is enqueued on (must wait for the input / produces the output).
+    // Ragged batch: only the first `na` streams take part in the chunk, and those whose frame count is <= d1 (the chunk's
+    // last DNN frame) have ended in it: they have written all of their output, beyond y1.
+    std::function<int(int64_t x0, int64_t x1, int64_t na, cudaStream_t cs)> before;
+    std::function<int(int64_t y0, int64_t y1, int64_t d1, int64_t na, cudaStream_t cs)> after;
 };
 
+// rows / tfs (ragged batch, or null): the group's device table and its streams' frame counts on the host, longest first;
+// the signal is then read through the table (d_x is the base pointer) and Tp only bounds the longest stream's frames.
 static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, int64_t nb, int64_t Tp, int64_t in_valid, int pad,
-                         float lim, float *d_out, int64_t out_len, int tc, bool pipelined, cudaStream_t s, const ChunkHooks *hooks) {
+                         float lim, float *d_out, int64_t out_len, int tc, bool pipelined, cudaStream_t s, const ChunkHooks *hooks,
+                         const RaggedRow *rows = nullptr, const int64_t *tfs = nullptr) {
     const dfb_model_config &c = m->cfg;
     const ChunkGeom g = chunk_geom(c);
     const int hop = st->hop, fft = st->fft;
-    const int64_t Tf = Tp / hop;
+    const int64_t Tf = tfs ? tfs[0] : Tp / hop;
     size_t off[16];
     const size_t nstate = state_floats(c, st, (int)nb, off);
     float *slab = m->aux_arena.take<float>(nstate);
@@ -2167,19 +2188,21 @@ static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, int64_t 
         const int64_t e1n = d1n == Tf ? Tf : d1n - g.lag;
         const int lane = pipelined ? (chunk & 1) : 0;
         cudaStream_t cs = pipelined ? m->lanes[lane].main : s;
+        int64_t na = nb;   // streams with frames left: a prefix, since the ragged table is sorted longest first
+        if (tfs) while (na > 1 && tfs[na - 1] <= S.d1) na--;
         if (hooks && hooks->before) {
             int64_t x0 = S.a1 * hop, x1 = a1n * hop;
             if (x1 > in_valid) x1 = in_valid;
-            if (x0 < x1 && (rc = hooks->before(x0, x1, cs))) break;
+            if (x0 < x1 && (rc = hooks->before(x0, x1, na, cs))) break;
         }
         const int64_t e0 = S.e1;
-        ChunkIO io{d_x, Tp, Tp, 0, nullptr, d_out, out_len, out_len, delay, lim, nullptr};
+        ChunkIO io{d_x, Tp, Tp, 0, nullptr, d_out, out_len, out_len, delay, lim, nullptr, rows, (int)na};
         if ((rc = run_chunk(m, st, S, io, a1n, d1n, e1n > S.e1 ? e1n : S.e1, cs, lane, pipelined))) break;
         if (hooks && hooks->after) {
             int64_t y0 = e0 * hop - delay, y1 = S.e1 * hop - delay;
             if (y0 < 0) y0 = 0;
             if (y1 > out_len) y1 = out_len;
-            if (y0 < y1 && (rc = hooks->after(y0, y1, cs))) break;
+            if ((y0 < y1 || rows) && (rc = hooks->after(y0, y1, d1n, na, cs))) break;
         }
         last_lane = lane;
         chunk++;
@@ -2298,7 +2321,7 @@ extern "C" int dfb_enhance_host(dfb_model *m, dfb_state *st, const float *h_audi
         if (pad)  // zero tail of the padded rows (enhance.py:233)
             DFB_CUDA(cudaMemset2DAsync(d_in + T, sizeof(float) * Tp, 0, sizeof(float) * (Tp - T), nb, sh));
         ChunkHooks hooks;
-        hooks.before = [&](int64_t x0, int64_t x1, cudaStream_t cs) -> int {
+        hooks.before = [&](int64_t x0, int64_t x1, int64_t, cudaStream_t cs) -> int {
             if (x1 > T) x1 = T;
             if (x0 < x1)
                 DFB_CUDA(cudaMemcpy2DAsync(d_in + x0, sizeof(float) * Tp, hx + x0, sizeof(float) * T, sizeof(float) * (x1 - x0), nb,
@@ -2308,7 +2331,7 @@ extern "C" int dfb_enhance_host(dfb_model *m, dfb_state *st, const float *h_audi
             DFB_CUDA(cudaStreamWaitEvent(cs, e, 0));
             return DFB_OK;
         };
-        hooks.after = [&](int64_t y0, int64_t y1, cudaStream_t cs) -> int {
+        hooks.after = [&](int64_t y0, int64_t y1, int64_t, int64_t, cudaStream_t cs) -> int {
             cudaEvent_t e = new_event();
             DFB_CUDA(cudaEventRecord(e, cs));
             DFB_CUDA(cudaStreamWaitEvent(sd, e, 0));
@@ -2326,6 +2349,193 @@ extern "C" int dfb_enhance_host(dfb_model *m, dfb_state *st, const float *h_audi
     if (rc) return rc;
     if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess)
         return fail(DFB_ERR_CUDA, "enhance_host failed: %s", cudaGetErrorString(e1 != cudaSuccess ? e1 : (e2 != cudaSuccess ? e2 : e3)));
+    return DFB_OK;
+}
+
+// ============================================================== ragged batch ====
+// B streams of different lengths in one call, each exactly as if enhanced alone.  The streams are sorted by frame count,
+// longest first, and stream groups are cut from that order.  Inside a group the chunk loop above runs only the prefix of
+// streams that still have frames (the others have ended: their padded frames are never computed), and the kernels that
+// look past the current frame -- analysis, the input convs' feature look-ahead, apply + synthesis -- read each stream's
+// own end from a small table (RaggedRow) in the aux arena.  Zero-padding the batch to its longest stream would NOT be
+// equivalent: the padded frames would exist, with features far from zero, and change the mask and deep filter of every
+// padded stream's last look-ahead frames.  DeepFilterNet v1 runs one window per signal with the end padding applied inside
+// every layer (forward_v1): its streams go through dfb_enhance in sets of equal length instead, which is exact but not
+// compacted.
+
+// Validates the call and returns its streams in executor order (frame count descending; ties keep the input order).
+static int ragged_plan(const dfb_state *st, int64_t in_numel, const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad,
+                       int64_t out_numel, const int64_t *out_offsets, std::vector<RaggedRow> &rows) {
+    if (!in_offsets || !lengths || !out_offsets) return fail(DFB_ERR_INVALID, "null argument");
+    if (B <= 0) return fail(DFB_ERR_INVALID, "empty batch");
+    rows.resize((size_t)B);
+    for (int64_t b = 0; b < B; b++) {
+        const int64_t len = lengths[b], io = in_offsets[b], oo = out_offsets[b];
+        if (len <= 0) return fail(DFB_ERR_INVALID, "stream %lld has length %lld", (long long)b, (long long)len);
+        const int64_t tf = (pad ? len + st->fft : len) / st->hop, ol = dfb_enhance_out_len(st, len, pad);
+        if (tf <= 0) return fail(DFB_ERR_INVALID, "stream %lld is shorter than one hop", (long long)b);
+        if (io < 0 || io > in_numel - len)
+            return fail(DFB_ERR_INVALID, "stream %lld reaches outside the input (%lld samples)", (long long)b, (long long)in_numel);
+        if (oo < 0 || oo > out_numel - ol)
+            return fail(DFB_ERR_INVALID, "stream %lld reaches outside the output (%lld samples)", (long long)b, (long long)out_numel);
+        rows[(size_t)b] = RaggedRow{io, len, oo, ol, tf};
+    }
+    std::stable_sort(rows.begin(), rows.end(), [](const RaggedRow &a, const RaggedRow &b) { return a.Tf > b.Tf; });
+    return DFB_OK;
+}
+
+// DeepFilterNet v1: every set of equal-length streams is gathered into a [n][len] batch and enhanced by dfb_enhance
+// (device) / dfb_enhance_host (host).
+static int ragged_v1(dfb_model *m, dfb_state *st, std::vector<RaggedRow> rows, const float *audio, float *out, int pad,
+                     float atten_lim_db, cudaStream_t s, bool host) {
+    std::stable_sort(rows.begin(), rows.end(), [](const RaggedRow &a, const RaggedRow &b) { return a.len > b.len; });
+    int rc = DFB_OK;
+    for (size_t i = 0; i < rows.size() && !rc;) {
+        size_t j = i;
+        while (j < rows.size() && rows[j].len == rows[i].len) j++;
+        const int64_t n = (int64_t)(j - i), len = rows[i].len, ol = rows[i].out_len;
+        const size_t in_b = sizeof(float) * len, out_b = sizeof(float) * ol;
+        if (host) {
+            std::vector<float> x((size_t)(n * len)), y((size_t)(n * ol));
+            for (int64_t k = 0; k < n; k++) memcpy(x.data() + k * len, audio + rows[i + k].in_off, in_b);
+            rc = dfb_enhance_host(m, st, x.data(), n, len, pad, atten_lim_db, y.data());
+            for (int64_t k = 0; k < n && !rc; k++) memcpy(out + rows[i + k].out_off, y.data() + k * ol, out_b);
+        } else {
+            float *x = nullptr, *y = nullptr;
+            DFB_CUDA(cudaMallocAsync(&x, in_b * n, s));
+            DFB_CUDA(cudaMallocAsync(&y, out_b * n, s));
+            for (int64_t k = 0; k < n; k++) DFB_CUDA(cudaMemcpyAsync(x + k * len, audio + rows[i + k].in_off, in_b, cudaMemcpyDeviceToDevice, s));
+            rc = dfb_enhance(m, st, x, n, len, pad, atten_lim_db, y, s);
+            for (int64_t k = 0; k < n && !rc; k++)
+                DFB_CUDA(cudaMemcpyAsync(out + rows[i + k].out_off, y + k * ol, out_b, cudaMemcpyDeviceToDevice, s));
+            cudaFreeAsync(x, s);
+            cudaFreeAsync(y, s);
+        }
+        i = j;
+    }
+    return rc;
+}
+
+// Plan shared by both entry points: chunk length, stream group size and the aux arena (state slab + table of one group).
+static int ragged_reserve(dfb_model *m, dfb_state *st, int64_t B, int64_t Tf, int min_chunks, int64_t *group, int *tc, bool *pipelined) {
+    int rc = enhance_plan(m, st, B, Tf, min_chunks, group, tc, pipelined);
+    if (rc) return rc;
+    size_t off[16];
+    return m->aux_arena.reserve(state_floats(m->cfg, st, (int)*group, off) * sizeof(float) + (size_t)*group * sizeof(RaggedRow) + 8192);
+}
+
+extern "C" int dfb_enhance_ragged(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
+                                  const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
+                                  const int64_t *out_offsets, void *stream) {
+    if (!m || !st || !d_audio || !d_out) return fail(DFB_ERR_INVALID, "null argument");
+    if (int rcs = check_state(m, st)) return rcs;
+    std::vector<RaggedRow> rows;
+    int rc = ragged_plan(st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rows);
+    if (rc) return rc;
+    DFB_CUDA(cudaSetDevice(m->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    if (m->cfg.model_kind == 1) return ragged_v1(m, st, std::move(rows), d_audio, d_out, pad, atten_lim_db, s, false);
+    const int hop = st->hop;
+    int64_t group = 0;
+    int tc = 0;
+    bool pipelined = false;
+    std::vector<int64_t> tfs(rows.size());
+    int64_t true_frames = 0;
+    for (size_t i = 0; i < rows.size(); i++) { tfs[i] = rows[i].Tf; true_frames += tfs[i]; }
+    int dev_chunks = m->dev_chunks > 0 ? m->dev_chunks : (B <= 8 ? 3 : (B <= 256 ? 2 : 1));   // as dfb_enhance
+    // ended streams drop out at chunk boundaries only: with a spread of lengths, shorter chunks save more padded frames than
+    // they cost (DeepFilterNet3, 128 streams of 1 - 20 s on one H100 at 700 W: 2 chunks 34.6 ms, 4 chunks 30.1 ms, 8 30.3)
+    if (m->dev_chunks == 0 && (double)B * tfs[0] > 1.1 * (double)true_frames && dev_chunks < 4) dev_chunks = 4;
+    if ((rc = ragged_reserve(m, st, B, rows[0].Tf, dev_chunks, &group, &tc, &pipelined))) return rc;
+    const float lim = (atten_lim_db > 0.f) ? powf(10.f, -atten_lim_db / 20.f) : 0.f;
+    for (int64_t b0 = 0; b0 < B && !rc; b0 += group) {
+        const int64_t nb = (B - b0 < group) ? B - b0 : group, Tp = tfs[(size_t)b0] * hop;
+        m->aux_arena.reset();
+        RaggedRow *d_rows = m->aux_arena.take<RaggedRow>((size_t)nb);
+        DFB_CUDA(cudaMemcpyAsync(d_rows, rows.data() + b0, sizeof(RaggedRow) * nb, cudaMemcpyHostToDevice, s));
+        rc = enhance_group(m, st, d_audio, nb, Tp, Tp, pad, lim, d_out, out_numel, tc, pipelined, s, nullptr, d_rows, tfs.data() + b0);
+    }
+    m->arena.reset();
+    m->arena1.reset();
+    return rc;
+}
+
+// Host buffers: the streams are staged into one packed device buffer chunk by chunk, each stream's range clamped to its
+// length, the H2D copies of chunk c + 1 and the D2H copies of chunk c - 1 overlapping the compute of chunk c as in
+// dfb_enhance_host; only real samples cross PCIe.
+extern "C" int dfb_enhance_ragged_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel, const int64_t *in_offsets,
+                                       const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *h_out, int64_t out_numel,
+                                       const int64_t *out_offsets) {
+    if (!m || !st || !h_audio || !h_out) return fail(DFB_ERR_INVALID, "null argument");
+    if (int rcs = check_state(m, st)) return rcs;
+    std::vector<RaggedRow> rows;
+    int rc = ragged_plan(st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rows);
+    if (rc) return rc;
+    DFB_CUDA(cudaSetDevice(m->device));
+    if (m->cfg.model_kind == 1) return ragged_v1(m, st, std::move(rows), h_audio, h_out, pad, atten_lim_db, nullptr, true);
+    const int hop = st->hop;
+    int64_t group = 0;
+    int tc = 0;
+    bool pipelined = false;
+    if ((rc = ragged_reserve(m, st, B, rows[0].Tf, m->host_chunks, &group, &tc, &pipelined))) return rc;
+    const float lim = (atten_lim_db > 0.f) ? powf(10.f, -atten_lim_db / 20.f) : 0.f;
+    // device rows: the same streams packed back to back in the staging buffers
+    std::vector<RaggedRow> drows(rows);
+    std::vector<int64_t> tfs(rows.size());
+    int64_t n_in = 0, n_out = 0;
+    for (size_t i = 0; i < rows.size(); i++) {
+        drows[i].in_off = n_in; drows[i].out_off = n_out;
+        n_in += rows[i].len; n_out += rows[i].out_len;
+        tfs[i] = rows[i].Tf;
+    }
+    if ((rc = st->arena.reserve(sizeof(float) * (size_t)(n_in + n_out) + 4096))) return rc;
+    st->arena.reset();
+    float *d_in = st->arena.take<float>((size_t)n_in), *d_out = st->arena.take<float>((size_t)n_out);
+    cudaStream_t sc = m->stream, sh = m->h2d, sd = m->d2h;
+    std::vector<cudaEvent_t> evs;
+    auto new_event = [&]() { cudaEvent_t e = nullptr; cudaEventCreateWithFlags(&e, cudaEventDisableTiming); evs.push_back(e); return e; };
+    for (int64_t b0 = 0; b0 < B && !rc; b0 += group) {
+        const int64_t nb = (B - b0 < group) ? B - b0 : group, Tp = tfs[(size_t)b0] * hop;
+        const RaggedRow *hr = rows.data() + b0, *dr = drows.data() + b0;
+        const int64_t *tf = tfs.data() + b0;
+        ChunkHooks hooks;
+        hooks.before = [&](int64_t x0, int64_t x1, int64_t na, cudaStream_t cs) -> int {
+            for (int64_t i = 0; i < na; i++) {
+                const int64_t e = x1 < hr[i].len ? x1 : hr[i].len;
+                if (x0 < e)
+                    DFB_CUDA(cudaMemcpyAsync(d_in + dr[i].in_off + x0, h_audio + hr[i].in_off + x0, sizeof(float) * (e - x0),
+                                             cudaMemcpyHostToDevice, sh));
+            }
+            cudaEvent_t ev = new_event();
+            DFB_CUDA(cudaEventRecord(ev, sh));
+            DFB_CUDA(cudaStreamWaitEvent(cs, ev, 0));
+            return DFB_OK;
+        };
+        hooks.after = [&](int64_t y0, int64_t y1, int64_t d1, int64_t na, cudaStream_t cs) -> int {
+            cudaEvent_t ev = new_event();
+            DFB_CUDA(cudaEventRecord(ev, cs));
+            DFB_CUDA(cudaStreamWaitEvent(sd, ev, 0));
+            for (int64_t i = 0; i < na; i++) {
+                const int64_t e = tf[i] <= d1 ? hr[i].out_len : (y1 < hr[i].out_len ? y1 : hr[i].out_len);   // ended: all of it
+                if (y0 < e)
+                    DFB_CUDA(cudaMemcpyAsync(h_out + hr[i].out_off + y0, d_out + dr[i].out_off + y0, sizeof(float) * (e - y0),
+                                             cudaMemcpyDeviceToHost, sd));
+            }
+            return DFB_OK;
+        };
+        // the previous group's compute still reads the state slab and table: upload this group's table behind it
+        m->aux_arena.reset();
+        RaggedRow *d_rows = m->aux_arena.take<RaggedRow>((size_t)nb);
+        DFB_CUDA(cudaMemcpyAsync(d_rows, dr, sizeof(RaggedRow) * nb, cudaMemcpyHostToDevice, sc));
+        rc = enhance_group(m, st, d_in, nb, Tp, Tp, pad, lim, d_out, n_out, tc, pipelined, sc, &hooks, d_rows, tf);
+    }
+    cudaError_t e1 = cudaStreamSynchronize(sc), e2 = cudaStreamSynchronize(sd), e3 = cudaStreamSynchronize(sh);
+    for (cudaEvent_t e : evs) cudaEventDestroy(e);
+    m->arena.reset();
+    m->arena1.reset();
+    if (rc) return rc;
+    if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess)
+        return fail(DFB_ERR_CUDA, "enhance_ragged_host failed: %s", cudaGetErrorString(e1 != cudaSuccess ? e1 : (e2 != cudaSuccess ? e2 : e3)));
     return DFB_OK;
 }
 

@@ -7,13 +7,13 @@ from __future__ import annotations
 
 import logging
 import os
-from typing import Optional, Tuple, Union
+from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
 from torch import Tensor
 
-from . import _lib
+from . import _lib, ragged
 from ._lib import check
 from .io import load_audio, resample, save_audio
 from .libdf import DF
@@ -148,6 +148,62 @@ def enhance_device(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
     return out
 
 
+@torch.no_grad()
+def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: bool = True,
+                  atten_lim_db: Optional[float] = None) -> List[Tensor]:
+    """Several recordings of different lengths in one call: ``audios`` is a sequence of CPU [C_i, T_i] tensors as
+    :func:`enhance` takes them, every channel one stream.  Entry i of the result equals
+    ``enhance(model, df_state, audios[i], pad, atten_lim_db)``.  The batch is packed into one page-locked buffer and
+    enhanced by one ``dfb_enhance_ragged_host`` call, which copies only the streams' own samples and computes only their
+    own frames.  The results are views into one page-locked output buffer."""
+    model.eval()
+    xs = list(audios)
+    for i, a in enumerate(xs):
+        if not isinstance(a, Tensor) or a.dim() != 2:
+            raise ValueError(f"entry {i}: audio must be a tensor of shape [C, T]")
+    lens, in_off, out_off, n_in, n_out, slices = ragged.packed_layout([tuple(a.shape) for a in xs], df_state.hop_size(), pad)
+    pin = torch.cuda.is_available()
+    x = torch.empty(n_in, dtype=torch.float32, pin_memory=pin)
+    torch.cat([a.detach().to("cpu", torch.float32).reshape(-1) for a in xs], out=x)
+    y = torch.empty(n_out, dtype=torch.float32, pin_memory=pin)
+    lim = abs(float(atten_lim_db)) if atten_lim_db is not None else 0.0
+    check(_lib.lib().dfb_enhance_ragged_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
+                                             lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
+                                             out_off.ctypes.data))
+    return [y[s:s + c * n].view(c, n) for s, c, n in slices]
+
+
+@torch.no_grad()
+def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pad: bool = True,
+                          atten_lim_db: Optional[float] = None, out: Optional[Tensor] = None) -> Tensor:
+    """Device-resident ragged batch: ``audio`` is a padded CUDA tensor [B, S] whose row b holds ``lengths[b]`` real
+    samples.  Returns [B, max out_len] (asynchronous on the current stream): row b equals :func:`enhance_device` of
+    ``audio[b, :lengths[b]]`` alone, and is zero beyond its own output length.  With ``out`` given, only each row's own
+    output range is written."""
+    if not audio.is_cuda or audio.dtype != torch.float32 or not audio.is_contiguous() or audio.dim() != 2:
+        raise ValueError("enhance_device_ragged expects a contiguous float32 CUDA tensor of shape [B, S]")
+    if audio.device != model.cuda_device:
+        raise ValueError(f"audio lives on {audio.device}, the model on {model.cuda_device}")
+    b, s = audio.shape
+    lens = lengths.detach().cpu().numpy() if isinstance(lengths, Tensor) else lengths
+    lens = np.asarray(lens).reshape(-1)
+    if lens.size != b:
+        raise ValueError(f"{lens.size} lengths for {b} streams")
+    lens, in_off, out_off, ow = ragged.padded_layout(lens, s, df_state.hop_size(), pad)
+    if out is None:
+        out = torch.zeros((b, ow), dtype=torch.float32, device=audio.device)
+    elif (out.shape != (b, ow) or out.dtype != torch.float32 or not out.is_cuda or out.device != audio.device
+          or not out.is_contiguous()):
+        raise ValueError(f"out must be a contiguous float32 CUDA tensor of shape {(b, ow)} on {audio.device}")
+    lim = abs(float(atten_lim_db)) if atten_lim_db is not None else 0.0
+    with torch.cuda.device(audio.device):
+        stream = torch.cuda.current_stream(audio.device).cuda_stream
+        check(_lib.lib().dfb_enhance_ragged(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
+                                            lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow,
+                                            out_off.ctypes.data, stream))
+    return out
+
+
 # ------------------------------------------------------------------------------------------ CLI ----
 def parse_epoch_type(value: str) -> Union[int, str]:
     """enhance.py:253-261."""
@@ -196,20 +252,34 @@ def main(args) -> int:
         assert len(args.noisy_audio_files) > 0, "No audio files provided"
         input_files = args.noisy_audio_files
     n_samples = len(input_files)
-    for i, file in enumerate(input_files):
-        if not os.path.isfile(file):
-            logger.warning("File not found: %s. Skipping...", file)
+    batch_size = max(1, getattr(args, "batch_size", 1))
+    for b0 in range(0, n_samples, batch_size):
+        # --batch-size N: N files are enhanced by one enhance_batch call; each reports its share of the batch time
+        batch = []
+        for i in range(b0, min(b0 + batch_size, n_samples)):
+            file = input_files[i]
+            if not os.path.isfile(file):
+                logger.warning("File not found: %s. Skipping...", file)
+                continue
+            audio, meta = load_audio(file, df_sr, verbose=False)
+            batch.append((i, file, audio, meta))
+        if not batch:
             continue
-        audio, meta = load_audio(file, df_sr, verbose=False)
-        progress = (i + 1) / n_samples * 100
         t0 = time.time()
-        audio = enhance(model, df_state, audio, pad=args.compensate_delay, atten_lim_db=args.atten_lim)
-        t = time.time() - t0
-        t_audio = audio.shape[-1] / df_sr
-        p_str = f"{progress:2.0f}% | " if n_samples > 1 else ""
-        logger.info("%sEnhanced noisy audio file '%s' in %.2fs (RT factor: %.3f)", p_str, os.path.basename(file), t, t / t_audio)
-        audio = resample(audio.to("cpu"), df_sr, meta.sample_rate)
-        save_audio(file, audio, sr=meta.sample_rate, output_dir=args.output_dir, suffix=suffix, log=False)
+        if batch_size == 1:
+            outs = [enhance(model, df_state, batch[0][2], pad=args.compensate_delay, atten_lim_db=args.atten_lim)]
+        else:
+            outs = enhance_batch(model, df_state, [a for _, _, a, _ in batch], pad=args.compensate_delay, atten_lim_db=args.atten_lim)
+        t_batch = time.time() - t0
+        total = sum(a.numel() for _, _, a, _ in batch)
+        for (i, file, audio_in, meta), audio in zip(batch, outs):
+            progress = (i + 1) / n_samples * 100
+            t = t_batch * audio_in.numel() / total
+            t_audio = audio.shape[-1] / df_sr
+            p_str = f"{progress:2.0f}% | " if n_samples > 1 else ""
+            logger.info("%sEnhanced noisy audio file '%s' in %.2fs (RT factor: %.3f)", p_str, os.path.basename(file), t, t / t_audio)
+            audio = resample(audio.to("cpu"), df_sr, meta.sample_rate)
+            save_audio(file, audio, sr=meta.sample_rate, output_dir=args.output_dir, suffix=suffix, log=False)
     return 0
 
 
@@ -225,6 +295,8 @@ def run(argv=None) -> int:
                         help="Input directory containing noisy audio files. Use instead of `noisy_audio_files`.")
     parser.add_argument("--no-suffix", action="store_false", dest="suffix", help="Don't add the model suffix to the enhanced audio files")
     parser.add_argument("--no-df-stage", action="store_true")
+    parser.add_argument("--batch-size", type=int, default=1,
+                        help="Enhance this many files per call (streams of different lengths in one batch); 1: one file per call.")
     return main(parser.parse_args(argv))
 
 

@@ -1,0 +1,58 @@
+"""Host-side layout of a ragged batch (streams of different lengths in one ``dfb_enhance_ragged`` call): lengths, input and
+output offsets, and their validation.  Pure functions on shapes, so they are usable and testable without the library."""
+from __future__ import annotations
+
+from typing import List, Sequence, Tuple
+
+import numpy as np
+
+
+def out_len(length: int, hop: int, pad: bool) -> int:
+    """dfb_enhance_out_len: the input length with ``pad``, else the whole hops of it."""
+    return int(length) if pad else (int(length) // hop) * hop
+
+
+def check_lengths(lengths, hop: int, pad: bool, max_len: int = None) -> np.ndarray:
+    """Lengths as int64.  ValueError for a length <= 0 or beyond ``max_len``; RuntimeError when ``pad`` is off and a stream
+    is shorter than one hop (it has no frame), as ``enhance()`` does."""
+    lens = np.ascontiguousarray(np.asarray(lengths, dtype=np.int64).reshape(-1))
+    if lens.size == 0:
+        raise ValueError("empty batch")
+    if (lens <= 0).any():
+        raise ValueError(f"stream lengths must be > 0, got {int(lens.min())}")
+    if max_len is not None and (lens > max_len).any():
+        raise ValueError(f"stream length {int(lens.max())} exceeds the {max_len} samples per row")
+    if not pad and (lens < hop).any():
+        raise RuntimeError(f"stream of {int(lens.min())} samples is shorter than one hop ({hop}): no frame to enhance")
+    return lens
+
+
+def padded_layout(lengths, width: int, hop: int, pad: bool) -> Tuple[np.ndarray, np.ndarray, np.ndarray, int]:
+    """Rows of a padded [B, width] input and a [B, max out_len] output: (lengths, in_offsets, out_offsets, out_width)."""
+    lens = check_lengths(lengths, hop, pad, width)
+    ow = max(out_len(int(t), hop, pad) for t in lens)
+    rows = np.arange(lens.size, dtype=np.int64)
+    return lens, rows * width, rows * ow, ow
+
+
+def packed_layout(shapes: Sequence[Tuple[int, int]], hop: int, pad: bool):
+    """Entries [C_i, T_i] packed back to back, every channel one stream: (lengths, in_offsets, out_offsets, in_numel,
+    out_numel, slices) where slices[i] = (start, C_i, out_len_i) locates entry i in the packed output."""
+    lens: List[int] = []
+    for i, shp in enumerate(shapes):
+        if len(shp) != 2:
+            raise ValueError(f"entry {i}: audio must have shape [C, T], got {tuple(shp)}")
+        c, t = int(shp[0]), int(shp[1])
+        if c <= 0:
+            raise ValueError(f"entry {i}: no channels")
+        lens += [t] * c
+    lens = check_lengths(lens, hop, pad)
+    olens = np.array([out_len(int(t), hop, pad) for t in lens], dtype=np.int64)
+    in_off = np.concatenate(([0], np.cumsum(lens)[:-1])).astype(np.int64)
+    out_off = np.concatenate(([0], np.cumsum(olens)[:-1])).astype(np.int64)
+    slices, k = [], 0
+    for shp in shapes:
+        c = int(shp[0])
+        slices.append((int(out_off[k]), c, int(olens[k])))
+        k += c
+    return lens, in_off, out_off, int(lens.sum()), int(olens.sum()), slices

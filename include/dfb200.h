@@ -180,6 +180,24 @@ int dfb_enhance_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t 
                      float atten_lim_db, float *h_out);
 /* output length of dfb_enhance for a given input length */
 int64_t dfb_enhance_out_len(const dfb_state *st, int64_t T, int pad);
+/* A batch of B streams of different lengths: stream b is lengths[b] samples at audio + in_offsets[b]; its result,
+ * dfb_enhance_out_len(st, lengths[b], pad) samples, goes to out + out_offsets[b].  Nothing else in `out` is written.
+ * in_offsets / lengths / out_offsets are HOST arrays; in_numel / out_numel bound them (DFB_ERR_INVALID when a stream
+ * reaches outside, has a length <= 0, or has no frame: shorter than one hop with pad == 0).  Every stream's output equals
+ * dfb_enhance of that stream alone (fp32 reduction order aside) -- which zero-padding the batch to its longest stream
+ * does not give: the padded frames would change the look-ahead of every shorter stream's last frames.
+ * Offsets cover a padded [B, S] tensor (in_offsets[b] = b * S) as well as streams packed back to back.  The streams run
+ * longest first; a time chunk computes only the streams that have frames left in it, so a batch of mixed lengths costs
+ * about its true frame count, not B times the longest.  DeepFilterNet v1 (one window per signal) runs every set of
+ * equal-length streams through dfb_enhance instead: exact, without that saving.
+ * The _host variant takes host pointers (page-locked memory lets its copies overlap the compute), copies only the
+ * streams' own samples and results, and is synchronous. */
+int dfb_enhance_ragged(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
+                       const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
+                       const int64_t *out_offsets, void *stream);
+int dfb_enhance_ragged_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel, const int64_t *in_offsets,
+                            const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *h_out, int64_t out_numel,
+                            const int64_t *out_offsets);
 /* ------------------------------------------------------------------ streaming -----------------
  * Frame-incremental processing with carried per-stream state: the batched counterpart of the reference's
  * single-stream runtime `DfTract::process` (libDF/src/tract.rs:509-642) and its C ABI (libDF/src/capi.rs:83-253:
