@@ -119,9 +119,10 @@ struct DspTables {
     int fft, hop, F, E;
 };
 
-// One stream of a ragged batch (dfb_enhance_ragged), in the executor's order (longest first): its samples are
+// One stream of a batch (dfb_enhance*), in the executor's order (longest first): its samples are
 // audio[in_off, in_off + len), its result out[out_off, out_off + out_len), and it has Tf STFT frames.  Kernels that take a
-// table index their rows with it; a null table means every row has the call's common length.
+// table index their rows with it; a null table (streaming API, dfb_analysis, dfb_apply) means every row has the call's
+// common length.
 struct RaggedRow { int64_t in_off, len, out_off, out_len, Tf; };
 
 // Parameters of the fused apply + synthesis kernel (dfb_dsp.cu).

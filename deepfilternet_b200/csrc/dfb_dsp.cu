@@ -145,9 +145,9 @@ __device__ __forceinline__ void warp_fft480_twptr(LoadF load, const float2 *tw_l
 // Frame window: the grid covers frames [t_begin, t_begin + nf) of every stream (time-chunked execution); their rows
 // go to out_t0 ... of spec / erb_db buffers that hold Tbuf frames per stream.  The whole-signal call is
 // (t_begin, nf, out_t0, Tbuf) = (0, Tf, 0, Tf).
-// Ragged batch (rows != null): stream b starts at audio + rows[b].in_off and reads zeros from sample rows[b].len on, so the
+// Batch path (rows != null): stream b starts at audio + rows[b].in_off and reads zeros from sample rows[b].len on, so the
 // `pad` zeros of enhance() are implicit and no padded copy of the input is needed (RG: its own instantiation, so that the
-// equal-length kernel is compiled as without it).
+// table-free kernel of the streaming API and dfb_analysis* is compiled as without it).
 template <bool RG>
 __global__ void __launch_bounds__(32 * kAnaWarps, 4)
 k_analysis(const float *__restrict__ audio, int64_t T, int Tf, float2 *__restrict__ spec,
@@ -669,7 +669,8 @@ __global__ void __launch_bounds__(32 * kSynWarps) k_apply_synthesis_generic(Appl
 // bins lives in registers as a 5-deep shift register (one new look-ahead value per bin and frame instead of
 // five reloads), the band gains come from one register per lane via warp shuffles, and all global loads of
 // a frame are issued up front, coalesced (256-byte rows), before any use.
-// RG: ragged batch (p.rows), a separate instantiation so that the equal-length path compiles exactly as without it.
+// RG: batch path (p.rows), a separate instantiation so that the table-free kernel of the streaming API, dfb_apply and
+// dfb_model_forward_full compiles exactly as without it.
 template <int ORDER, int NDFJ, int MINB, bool RG>
 __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyParams p, DspTables tb) {
     __shared__ __align__(16) float s_win[kFft];
@@ -1098,13 +1099,11 @@ int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaS
     if (p.lsnr && !(p.mode == 1 && p.order == 5 && p.nb_df == 96 && st->tb.E == 32 && p.m && p.coefs))
         return fail(DFB_ERR_UNSUPPORTED, "LSNR stage gating is built for the DeepFilterNet3 apply kernel only");
     DFB_PROF("k_apply_synthesis", s);
-    static const int minb = getenv("DFB_APPLY_MINB") ? atoi(getenv("DFB_APPLY_MINB")) : 2;  // 2 CTAs/SM without spills measured fastest
+    // MINB 2: 2 CTAs/SM without spills measured fastest
     const bool special = p.mode != 0 && p.order == 5 && p.nb_df == 96 && st->tb.E == 32 && p.m && p.coefs;
     if (special && p.rows)
         k_apply_synthesis<5, 3, 2, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
-    else if (special && minb == 3)
-        k_apply_synthesis<5, 3, 3, false><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
-    else if (special && minb == 2)
+    else if (special)
         k_apply_synthesis<5, 3, 2, false><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
     else
         k_apply_synthesis_generic<<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);

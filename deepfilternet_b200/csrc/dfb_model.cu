@@ -840,9 +840,9 @@ struct dfb_model {
     size_t max_workspace = size_t(40) << 30;  // dfb_enhance chunks / groups the batch so that the arena stays below this
                                               // (40 GB: room for the batch itself and its output on an 80 GB H100)
     std::vector<int64_t> erb_widths;          // band table the model was built for (checked against the dfb_state)
-    Arena aux_arena;                          // carried stream state + padded input of dfb_enhance
+    Arena aux_arena;                          // carried stream state + stream table of one dfb_enhance* stream group
     cudaStream_t stream = nullptr;
-    cudaStream_t h2d = nullptr, d2h = nullptr;  // copy streams of dfb_enhance_host (both copy engines next to the compute)
+    cudaStream_t h2d = nullptr, d2h = nullptr;  // copy streams of the host batch path (both copy engines next to the compute)
     // One forward pass hops from the caller's stream onto the lane's internal streams: `hi` (ERB branch) and `aux` (DF
     // branch) for the encoder phase, `dhi` / `daux` at the greatest priority for the decoder phase (the recurrences are
     // the critical chain), `low` (least priority) for work off the critical path that only fills idle SMs.  Two lanes:
@@ -1911,7 +1911,7 @@ extern "C" int64_t dfb_enhance_out_len(const dfb_state *st, int64_t T, int pad) 
 }
 
 // enhance(): df/enhance.py:206-250.  Streams are processed in groups so that the workspace stays
-// below the model's workspace cap (64 GB by default; dfb_model_set_max_workspace / DFB_MAX_WORKSPACE_MB); streams
+// below the model's workspace cap (40 GB by default; dfb_model_set_max_workspace / DFB_MAX_WORKSPACE_MB); streams
 // are independent (per-channel state reset, pyDF/src/lib.rs:56-58).
 extern "C" int dfb_model_set_max_workspace(dfb_model *m, int64_t bytes) {
     if (!m || bytes <= 0) return fail(DFB_ERR_INVALID, "bad workspace cap");
@@ -2008,8 +2008,8 @@ struct ChunkIO {
     int64_t out_sample0;      // absolute synthesis sample (frame * hop + i) that lands at out[0]
     float atten_lim;
     const float *lsnr_th;     // {min_db_thresh, max_db_erb_thresh, max_db_df_thresh} (tract.rs:658-672) or null: no gating
-    // ragged batch (dfb_enhance_ragged): per-stream input / output rows and frame counts (device table, streams sorted
-    // longest first), and how many of them still have frames in this chunk (a prefix); null / 0: all S.B streams alike
+    // batch (dfb_enhance*): per-stream input / output rows and frame counts (device table, streams sorted longest first),
+    // and how many of them still have frames in this chunk (a prefix); null / 0 (streaming API): all S.B streams alike
     const RaggedRow *rows = nullptr;
     int nb = 0;
 };
@@ -2029,7 +2029,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     if (have_prev) DFB_CUDA(cudaStreamWaitEvent(s, P.ev_fork, 0));   // previous chunk: features + encoder phase done
     const dfb_model_config &c = m->cfg;
     const ChunkGeom g = chunk_geom(c);
-    const int B = io.nb > 0 ? io.nb : S.B, E = c.nb_erb, Fd = c.nb_df, O2 = 2 * c.df_order, F = st->tb.F, hop = st->hop, ED = E / 4 * kCh;
+    const int B = io.nb > 0 ? io.nb : S.B, E = c.nb_erb, Fd = c.nb_df, O2 = 2 * c.df_order, F = st->tb.F, hop = st->hop;
     const int64_t W0 = S.d1 > kHalo ? S.d1 - kHalo : 0;
     const int Rc = (int)(S.d1 - W0), Tw = (int)(d1n - W0), Tsb = Tw + g.Lmax;
     const int n_hist = (int)(S.a1 - W0);                 // feature frames of the window that are already known
@@ -2110,7 +2110,6 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
             S.n_mc = nm;
         }
     }
-    (void)ED;
     if (pipelined) {
         if (!run_dnn) DFB_CUDA(cudaEventRecord(L.ev_fork, s));   // no forward pass recorded it
         DFB_CUDA(cudaEventRecord(L.ev_done, s));
@@ -2120,11 +2119,12 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     return DFB_OK;
 }
 
-// Chunk length (new DNN frames per chunk) for B streams under the workspace cap; 0 when not even a short chunk fits.
-static int pick_chunk(const dfb_model *m, const dfb_state *st, int64_t B, int64_t Tf, int min_chunks) {
+// Chunk length (new DNN frames per chunk) for B streams under a workspace cap of `cap` bytes; 0 when not even a short
+// chunk fits.
+static int pick_chunk(const dfb_model *m, const dfb_state *st, int64_t B, int64_t Tf, int min_chunks, size_t cap) {
     const size_t per_frame = chunk_bytes_per_stream(m->cfg, st, 1024) / 1024 + 1;   // bytes per stream and window frame
     const ChunkGeom g = chunk_geom(m->cfg);
-    int64_t tw = (int64_t)(m->max_workspace / ((size_t)B * per_frame)) - g.Lmax - 8;
+    int64_t tw = (int64_t)(cap / ((size_t)B * per_frame)) - g.Lmax - 8;
     int64_t tc = tw - kHalo;
     if (tc > Tf) tc = Tf;
     if (min_chunks > 1 && Tf >= (int64_t)min_chunks * 64) {
@@ -2136,26 +2136,24 @@ static int pick_chunk(const dfb_model *m, const dfb_state *st, int64_t B, int64_
     if (tc < Tf && tc < 32) return 0;   // a chunk this short wastes most of its window on the halo: use stream groups
     return (int)tc;
 }
-// Runs the chunk loop over `nb` streams whose padded signal d_x [nb][Tp] is resident (or becomes resident chunk by chunk:
-// `before` / `after` are called around every chunk with the sample ranges it reads / has written).
+// Hooks around every chunk of a stream group whose buffers are staged (host batch).  `cs` is the stream the chunk's compute
+// is enqueued on (it must wait for the input / produces the output); only the first `na` streams take part in the chunk.
 struct ChunkHooks {
-    // analysis of this chunk reads input samples [x0, x1) of every stream; output samples [y0, y1) have been written
-    // `cs` is the stream the chunk's compute is enqueued on (must wait for the input / produces the output).
-    // Ragged batch: only the first `na` streams take part in the chunk, and those whose frame count is <= d1 (the chunk's
-    // last DNN frame) have ended in it: they have written all of their output, beyond y1.
+    // the chunk's analysis reads input samples [x0, x1) of every stream (as far as the stream has them)
     std::function<int(int64_t x0, int64_t x1, int64_t na, cudaStream_t cs)> before;
+    // output samples [y0, y1) of every stream have been written; a stream whose frame count is <= d1 (the chunk's last DNN
+    // frame) has ended in it and has written all of its output, beyond y1
     std::function<int(int64_t y0, int64_t y1, int64_t d1, int64_t na, cudaStream_t cs)> after;
 };
 
-// rows / tfs (ragged batch, or null): the group's device table and its streams' frame counts on the host, longest first;
-// the signal is then read through the table (d_x is the base pointer) and Tp only bounds the longest stream's frames.
-static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, int64_t nb, int64_t Tp, int64_t in_valid, int pad,
-                         float lim, float *d_out, int64_t out_len, int tc, bool pipelined, cudaStream_t s, const ChunkHooks *hooks,
-                         const RaggedRow *rows = nullptr, const int64_t *tfs = nullptr) {
+// Runs the chunk loop over one stream group: `rows` is its device table and `tfs` its streams' frame counts on the host,
+// longest first.  The analysis reads stream b from d_x + rows[b].in_off, apply + synthesis writes it to d_out + rows[b].out_off.
+static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, float *d_out, const RaggedRow *rows, const int64_t *tfs,
+                         int64_t nb, int pad, float lim, int tc, bool pipelined, cudaStream_t s, const ChunkHooks *hooks) {
     const dfb_model_config &c = m->cfg;
     const ChunkGeom g = chunk_geom(c);
     const int hop = st->hop, fft = st->fft;
-    const int64_t Tf = tfs ? tfs[0] : Tp / hop;
+    const int64_t Tf = tfs[0];
     size_t off[16];
     const size_t nstate = state_floats(c, st, (int)nb, off);
     float *slab = m->aux_arena.take<float>(nstate);
@@ -2188,22 +2186,13 @@ static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, int64_t 
         const int64_t e1n = d1n == Tf ? Tf : d1n - g.lag;
         const int lane = pipelined ? (chunk & 1) : 0;
         cudaStream_t cs = pipelined ? m->lanes[lane].main : s;
-        int64_t na = nb;   // streams with frames left: a prefix, since the ragged table is sorted longest first
-        if (tfs) while (na > 1 && tfs[na - 1] <= S.d1) na--;
-        if (hooks && hooks->before) {
-            int64_t x0 = S.a1 * hop, x1 = a1n * hop;
-            if (x1 > in_valid) x1 = in_valid;
-            if (x0 < x1 && (rc = hooks->before(x0, x1, na, cs))) break;
-        }
+        int64_t na = nb;   // streams with frames left: a prefix, since the table is sorted longest first
+        while (na > 1 && tfs[na - 1] <= S.d1) na--;
+        if (hooks && S.a1 < a1n && (rc = hooks->before(S.a1 * hop, a1n * hop, na, cs))) break;
         const int64_t e0 = S.e1;
-        ChunkIO io{d_x, Tp, Tp, 0, nullptr, d_out, out_len, out_len, delay, lim, nullptr, rows, (int)na};
+        ChunkIO io{d_x, Tf * hop, Tf * hop, 0, nullptr, d_out, 0, 0, delay, lim, nullptr, rows, (int)na};
         if ((rc = run_chunk(m, st, S, io, a1n, d1n, e1n > S.e1 ? e1n : S.e1, cs, lane, pipelined))) break;
-        if (hooks && hooks->after) {
-            int64_t y0 = e0 * hop - delay, y1 = S.e1 * hop - delay;
-            if (y0 < 0) y0 = 0;
-            if (y1 > out_len) y1 = out_len;
-            if ((y0 < y1 || rows) && (rc = hooks->after(y0, y1, d1n, na, cs))) break;
-        }
+        if (hooks && (rc = hooks->after(e0 * hop > delay ? e0 * hop - delay : 0, S.e1 * hop - delay, d1n, na, cs))) break;
         last_lane = lane;
         chunk++;
     }
@@ -2223,15 +2212,13 @@ static int enhance_plan(dfb_model *m, dfb_state *st, int64_t B, int64_t Tf, int 
     // two lanes (DFB_LANES=1 turns the chunk pipeline off): each lane's arena may take half of the workspace cap
     static const bool serial = getenv("DFB_SERIAL") && atoi(getenv("DFB_SERIAL"));
     const bool pipelined = m->n_lanes == 2 && !serial && min_chunks > 1 && Tf >= (int64_t)min_chunks * 64;
-    const size_t cap = m->max_workspace;
-    if (pipelined) m->max_workspace = cap / 2;
+    const size_t cap = pipelined ? m->max_workspace / 2 : m->max_workspace;
     int64_t group = B > 65535 ? 65535 : B;
     int tc = 0;
-    while ((tc = pick_chunk(m, st, group, Tf, min_chunks)) == 0) {
-        if (group == 1) { m->max_workspace = cap; return fail(DFB_ERR_OOM, "workspace cap of %zu bytes is too small for a single stream", cap); }
+    while ((tc = pick_chunk(m, st, group, Tf, min_chunks, cap)) == 0) {
+        if (group == 1) return fail(DFB_ERR_OOM, "workspace cap of %zu bytes is too small for a single stream", m->max_workspace);
         group = (group + 1) / 2;
     }
-    m->max_workspace = cap;
     *group_out = group; *tc_out = tc; *pipelined_out = pipelined && tc < Tf;
     const ChunkGeom g = chunk_geom(m->cfg);
     const size_t bytes = chunk_bytes_per_stream(m->cfg, st, tc + kHalo) * (size_t)group + ((size_t)g.Lmax << 10) + (2 << 20);
@@ -2240,130 +2227,19 @@ static int enhance_plan(dfb_model *m, dfb_state *st, int64_t B, int64_t Tf, int 
     return rc;
 }
 
-extern "C" int dfb_enhance(dfb_model *m, dfb_state *st, const float *d_audio, int64_t B, int64_t T, int pad,
-                           float atten_lim_db, float *d_out, void *stream) {
-    if (!m || !st || !d_audio || !d_out) return fail(DFB_ERR_INVALID, "null argument");
-    if (B <= 0 || T <= 0) return fail(DFB_ERR_INVALID, "empty input");
-    if (int rcs = check_state(m, st)) return rcs;
-    DFB_CUDA(cudaSetDevice(m->device));
-    cudaStream_t s = (cudaStream_t)stream;
-    const int hop = st->hop, fft = st->fft;
-    // pad = True appends fft zeros (enhance.py:230-233): Tf = (T + fft) / hop
-    const int64_t Tp = pad ? T + fft : T;
-    const int64_t Tf = Tp / hop;
-    if (Tf <= 0) return fail(DFB_ERR_INVALID, "input shorter than one hop");
-    const int64_t out_len = dfb_enhance_out_len(st, T, pad);
-    int64_t group = 0;
-    int tc = 0, rc;
-    bool pipelined = false;
-    // cutting a large device-resident batch into pipelined chunks can cost more (persistent kernels re-pay their prologues,
-    // short grids leave partial waves) than the overlap of encoder and decoder phases gains; for a few streams, where
-    // everything is latency bound, the overlap wins.  0 = that policy.
-    const int dev_chunks = m->dev_chunks > 0 ? m->dev_chunks : (B <= 8 ? 3 : (B <= 256 ? 2 : 1));
-    if ((rc = enhance_plan(m, st, B, Tf, dev_chunks, &group, &tc, &pipelined))) return rc;
-    const float lim = (atten_lim_db > 0.f) ? powf(10.f, -atten_lim_db / 20.f) : 0.f;
-    size_t off[16];
-    if ((rc = m->aux_arena.reserve((state_floats(m->cfg, st, (int)group, off) + (pad ? (size_t)group * Tp : 0)) * sizeof(float) + 8192))) return rc;
-    for (int64_t b0 = 0; b0 < B && !rc; b0 += group) {
-        const int64_t nb = (B - b0 < group) ? B - b0 : group;
-        const float *x = d_audio + b0 * T;
-        m->aux_arena.reset();
-        float *xp = pad ? m->aux_arena.take<float>((size_t)nb * Tp) : nullptr;
-        if (pad) {
-            rc = cudaMemsetAsync(xp, 0, sizeof(float) * nb * Tp, s) != cudaSuccess ||
-                 cudaMemcpy2DAsync(xp, sizeof(float) * Tp, x, sizeof(float) * T, sizeof(float) * T, nb, cudaMemcpyDeviceToDevice, s) != cudaSuccess
-                     ? fail(DFB_ERR_CUDA, "padding copy failed") : DFB_OK;
-            x = xp;
-        }
-        if (!rc) rc = enhance_group(m, st, x, nb, Tp, Tp, pad, lim, d_out + b0 * out_len, out_len, tc, pipelined, s, nullptr);
-    }
-    m->arena.reset();
-    m->arena1.reset();
-    return rc;
-}
-
-// Host buffers: the batch is staged chunk by chunk -- the H2D copy of chunk c + 1 and the D2H copy of chunk c - 1 run on
-// their own streams (both copy engines) while chunk c computes.
-extern "C" int dfb_enhance_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t B, int64_t T, int pad,
-                                float atten_lim_db, float *h_out) {
-    if (!m || !st || !h_audio || !h_out) return fail(DFB_ERR_INVALID, "null argument");
-    if (B <= 0 || T <= 0) return fail(DFB_ERR_INVALID, "empty input");
-    if (int rcs = check_state(m, st)) return rcs;
-    DFB_CUDA(cudaSetDevice(m->device));
-    const int hop = st->hop, fft = st->fft;
-    const int64_t Tp = pad ? T + fft : T, Tf = Tp / hop;
-    if (Tf <= 0) return fail(DFB_ERR_INVALID, "input shorter than one hop");
-    const int64_t out_len = dfb_enhance_out_len(st, T, pad);
-    int64_t group = 0;
-    int tc = 0, rc;
-    bool pipelined = false;
-    if ((rc = enhance_plan(m, st, B, Tf, m->host_chunks, &group, &tc, &pipelined))) return rc;
-    const float lim = (atten_lim_db > 0.f) ? powf(10.f, -atten_lim_db / 20.f) : 0.f;
-    size_t off[16];
-    if ((rc = m->aux_arena.reserve(state_floats(m->cfg, st, (int)group, off) * sizeof(float) + 8192))) return rc;
-    if ((rc = st->arena.reserve(sizeof(float) * (size_t)group * (Tp + out_len) + 4096))) return rc;
-    st->arena.reset();
-    float *d_in = st->arena.take<float>((size_t)group * Tp), *d_out = st->arena.take<float>((size_t)group * out_len);
-    cudaStream_t sc = m->stream, sh = m->h2d, sd = m->d2h;
-    std::vector<cudaEvent_t> evs;
-    auto new_event = [&]() { cudaEvent_t e = nullptr; cudaEventCreateWithFlags(&e, cudaEventDisableTiming); evs.push_back(e); return e; };
-    for (int64_t b0 = 0; b0 < B && !rc; b0 += group) {
-        const int64_t nb = (B - b0 < group) ? B - b0 : group;
-        const float *hx = h_audio + b0 * T;
-        float *hy = h_out + b0 * out_len;
-        // the previous group's D2H copies read d_out and its compute read d_in: order this group's first writes after them
-        cudaEvent_t e0 = new_event();
-        DFB_CUDA(cudaEventRecord(e0, sd));
-        DFB_CUDA(cudaStreamWaitEvent(sc, e0, 0));
-        cudaEvent_t e1 = new_event();
-        DFB_CUDA(cudaEventRecord(e1, sc));
-        DFB_CUDA(cudaStreamWaitEvent(sh, e1, 0));
-        if (pad)  // zero tail of the padded rows (enhance.py:233)
-            DFB_CUDA(cudaMemset2DAsync(d_in + T, sizeof(float) * Tp, 0, sizeof(float) * (Tp - T), nb, sh));
-        ChunkHooks hooks;
-        hooks.before = [&](int64_t x0, int64_t x1, int64_t, cudaStream_t cs) -> int {
-            if (x1 > T) x1 = T;
-            if (x0 < x1)
-                DFB_CUDA(cudaMemcpy2DAsync(d_in + x0, sizeof(float) * Tp, hx + x0, sizeof(float) * T, sizeof(float) * (x1 - x0), nb,
-                                           cudaMemcpyHostToDevice, sh));
-            cudaEvent_t e = new_event();
-            DFB_CUDA(cudaEventRecord(e, sh));
-            DFB_CUDA(cudaStreamWaitEvent(cs, e, 0));
-            return DFB_OK;
-        };
-        hooks.after = [&](int64_t y0, int64_t y1, int64_t, int64_t, cudaStream_t cs) -> int {
-            cudaEvent_t e = new_event();
-            DFB_CUDA(cudaEventRecord(e, cs));
-            DFB_CUDA(cudaStreamWaitEvent(sd, e, 0));
-            DFB_CUDA(cudaMemcpy2DAsync(hy + y0, sizeof(float) * out_len, d_out + y0, sizeof(float) * out_len, sizeof(float) * (y1 - y0), nb,
-                                       cudaMemcpyDeviceToHost, sd));
-            return DFB_OK;
-        };
-        m->aux_arena.reset();
-        rc = enhance_group(m, st, d_in, nb, Tp, T, pad, lim, d_out, out_len, tc, pipelined, sc, &hooks);
-    }
-    cudaError_t e1 = cudaStreamSynchronize(sc), e2 = cudaStreamSynchronize(sd), e3 = cudaStreamSynchronize(sh);
-    for (cudaEvent_t e : evs) cudaEventDestroy(e);
-    m->arena.reset();
-    m->arena1.reset();
-    if (rc) return rc;
-    if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess)
-        return fail(DFB_ERR_CUDA, "enhance_host failed: %s", cudaGetErrorString(e1 != cudaSuccess ? e1 : (e2 != cudaSuccess ? e2 : e3)));
-    return DFB_OK;
-}
-
-// ============================================================== ragged batch ====
-// B streams of different lengths in one call, each exactly as if enhanced alone.  The streams are sorted by frame count,
-// longest first, and stream groups are cut from that order.  Inside a group the chunk loop above runs only the prefix of
-// streams that still have frames (the others have ended: their padded frames are never computed), and the kernels that
-// look past the current frame -- analysis, the input convs' feature look-ahead, apply + synthesis -- read each stream's
-// own end from a small table (RaggedRow) in the aux arena.  Zero-padding the batch to its longest stream would NOT be
+// ============================================================== batch executor ====
+// Every dfb_enhance* call is a batch of streams, each an input offset, a length and an output offset (RaggedRow); an
+// equal-length [B][T] batch is the special case {b T, T, b out_len}.  The streams are sorted by frame count, longest first,
+// and stream groups are cut from that order.  Inside a group the chunk loop above runs only the prefix of streams that
+// still have frames (the others have ended: their padded frames are never computed), and the kernels that look past the
+// current frame -- analysis, the input convs' feature look-ahead, apply + synthesis -- read each stream's own end from the
+// group's table in the aux arena.  So every stream's output is exactly that of the stream enhanced alone, and the `pad`
+// zeros of enhance() need no padded copy of the input.  Zero-padding the batch to its longest stream would NOT be
 // equivalent: the padded frames would exist, with features far from zero, and change the mask and deep filter of every
 // padded stream's last look-ahead frames.  DeepFilterNet v1 runs one window per signal with the end padding applied inside
-// every layer (forward_v1): its streams go through dfb_enhance in sets of equal length instead, which is exact but not
-// compacted.
+// every layer (forward_v1), so its stream groups are also cut where the frame count changes: a group shares one window.
 
-// Validates the call and returns its streams in executor order (frame count descending; ties keep the input order).
+// Validates a ragged call and returns its streams in the caller's order.
 static int ragged_plan(const dfb_state *st, int64_t in_numel, const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad,
                        int64_t out_numel, const int64_t *out_offsets, std::vector<RaggedRow> &rows) {
     if (!in_offsets || !lengths || !out_offsets) return fail(DFB_ERR_INVALID, "null argument");
@@ -2380,48 +2256,169 @@ static int ragged_plan(const dfb_state *st, int64_t in_numel, const int64_t *in_
             return fail(DFB_ERR_INVALID, "stream %lld reaches outside the output (%lld samples)", (long long)b, (long long)out_numel);
         rows[(size_t)b] = RaggedRow{io, len, oo, ol, tf};
     }
-    std::stable_sort(rows.begin(), rows.end(), [](const RaggedRow &a, const RaggedRow &b) { return a.Tf > b.Tf; });
     return DFB_OK;
 }
 
-// DeepFilterNet v1: every set of equal-length streams is gathered into a [n][len] batch and enhanced by dfb_enhance
-// (device) / dfb_enhance_host (host).
-static int ragged_v1(dfb_model *m, dfb_state *st, std::vector<RaggedRow> rows, const float *audio, float *out, int pad,
-                     float atten_lim_db, cudaStream_t s, bool host) {
-    std::stable_sort(rows.begin(), rows.end(), [](const RaggedRow &a, const RaggedRow &b) { return a.len > b.len; });
-    int rc = DFB_OK;
-    for (size_t i = 0; i < rows.size() && !rc;) {
-        size_t j = i;
-        while (j < rows.size() && rows[j].len == rows[i].len) j++;
-        const int64_t n = (int64_t)(j - i), len = rows[i].len, ol = rows[i].out_len;
-        const size_t in_b = sizeof(float) * len, out_b = sizeof(float) * ol;
-        if (host) {
-            std::vector<float> x((size_t)(n * len)), y((size_t)(n * ol));
-            for (int64_t k = 0; k < n; k++) memcpy(x.data() + k * len, audio + rows[i + k].in_off, in_b);
-            rc = dfb_enhance_host(m, st, x.data(), n, len, pad, atten_lim_db, y.data());
-            for (int64_t k = 0; k < n && !rc; k++) memcpy(out + rows[i + k].out_off, y.data() + k * ol, out_b);
-        } else {
-            float *x = nullptr, *y = nullptr;
-            DFB_CUDA(cudaMallocAsync(&x, in_b * n, s));
-            DFB_CUDA(cudaMallocAsync(&y, out_b * n, s));
-            for (int64_t k = 0; k < n; k++) DFB_CUDA(cudaMemcpyAsync(x + k * len, audio + rows[i + k].in_off, in_b, cudaMemcpyDeviceToDevice, s));
-            rc = dfb_enhance(m, st, x, n, len, pad, atten_lim_db, y, s);
-            for (int64_t k = 0; k < n && !rc; k++)
-                DFB_CUDA(cudaMemcpyAsync(out + rows[i + k].out_off, y + k * ol, out_b, cudaMemcpyDeviceToDevice, s));
-            cudaFreeAsync(x, s);
-            cudaFreeAsync(y, s);
+// Copies samples [x0, end) of each stream i < n from src + src_off + x0 to dst + dst_off + x0 (`at(i)` describes stream i).
+// Consecutive streams with the same end and a constant pitch on both sides share one 2-D copy, so an equal-length batch
+// (or the channels of one multi-channel entry) takes one copy per chunk and direction instead of one per stream.
+struct StreamCopy { int64_t dst_off, src_off, end; };
+template <class At>
+static int copy_streams(float *dst, const float *src, int64_t x0, int64_t n, At at, cudaMemcpyKind kind, cudaStream_t s) {
+    constexpr int64_t kMaxPitch = INT32_MAX / sizeof(float);
+    for (int64_t i = 0, j; i < n; i = j) {
+        const StreamCopy a = at(i);
+        const int64_t w = a.end - x0;
+        int64_t dp = 0, sp = 0;   // pitches of the run [i, j)
+        for (j = i + 1; j < n; j++) {
+            const StreamCopy b = at(j), p = at(j - 1);
+            if (b.end != a.end) break;
+            if (j == i + 1) {
+                dp = b.dst_off - a.dst_off; sp = b.src_off - a.src_off;
+                if (dp < w || sp < w || dp > kMaxPitch || sp > kMaxPitch) break;
+            } else if (b.dst_off - p.dst_off != dp || b.src_off - p.src_off != sp) break;
         }
-        i = j;
+        if (w <= 0) continue;
+        if (j - i == 1) DFB_CUDA(cudaMemcpyAsync(dst + a.dst_off + x0, src + a.src_off + x0, sizeof(float) * w, kind, s));
+        else DFB_CUDA(cudaMemcpy2DAsync(dst + a.dst_off + x0, sizeof(float) * dp, src + a.src_off + x0, sizeof(float) * sp,
+                                        sizeof(float) * w, (size_t)(j - i), kind, s));
     }
+    return DFB_OK;
+}
+
+// The batch executor behind every dfb_enhance* entry point; `rows` (the caller's order) is sorted here.  Device buffers: the
+// work is enqueued on `s`.  Host buffers (`host`): each stream group is staged into device buffers that hold its streams
+// packed back to back, chunk by chunk and each stream's range clipped to its length -- the H2D copy of chunk c + 1 and the
+// D2H copy of chunk c - 1 run on their own streams (both copy engines) while chunk c computes -- and the call is synchronous.
+static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &rows, const float *src, float *dst, int pad,
+                        float atten_lim_db, bool host, cudaStream_t s) {
+    std::stable_sort(rows.begin(), rows.end(), [](const RaggedRow &a, const RaggedRow &b) { return a.Tf > b.Tf; });
+    const int64_t B = (int64_t)rows.size();
+    std::vector<int64_t> tfs((size_t)B);
+    int64_t true_frames = 0;
+    for (int64_t i = 0; i < B; i++) { tfs[i] = rows[i].Tf; true_frames += tfs[i]; }
+    int min_chunks = m->host_chunks;
+    if (!host) {
+        // cutting a large device-resident batch into pipelined chunks can cost more (persistent kernels re-pay their
+        // prologues, short grids leave partial waves) than the overlap of encoder and decoder phases gains; for a few
+        // streams, where everything is latency bound, the overlap wins.  dev_chunks 0 = that policy.
+        min_chunks = m->dev_chunks > 0 ? m->dev_chunks : (B <= 8 ? 3 : (B <= 256 ? 2 : 1));
+        // ended streams drop out at chunk boundaries only: with a spread of lengths, shorter chunks save more padded frames
+        // than they cost (DeepFilterNet3, 128 streams of 1 - 20 s on one H100 at 700 W: 2 chunks 34.6 ms, 4 chunks 30.1 ms, 8 30.3)
+        if (m->dev_chunks == 0 && (double)B * tfs[0] > 1.1 * (double)true_frames && min_chunks < 4) min_chunks = 4;
+    }
+    int64_t group = 0;
+    int tc = 0;
+    bool pipelined = false;
+    int rc = enhance_plan(m, st, B, tfs[0], min_chunks, &group, &tc, &pipelined);
+    if (rc) return rc;
+    size_t off[16];   // the aux arena holds one group's state slab and table
+    if ((rc = m->aux_arena.reserve(state_floats(m->cfg, st, (int)group, off) * sizeof(float) + (size_t)group * sizeof(RaggedRow) + 8192)))
+        return rc;
+    auto group_end = [&](int64_t b0) {   // stream groups: up to `group` streams; DeepFilterNet v1: of one frame count
+        int64_t b1 = B - b0 < group ? B : b0 + group;
+        if (m->cfg.model_kind == 1)
+            for (int64_t i = b0 + 1; i < b1; i++)
+                if (tfs[i] != tfs[b0]) { b1 = i; break; }
+        return b1;
+    };
+    // device rows: the streams themselves, or (host) their places in the staging buffers, sized for the largest group
+    std::vector<RaggedRow> drows(rows);
+    float *d_in = nullptr, *d_out = nullptr;
+    if (host) {
+        int64_t n_in = 0, n_out = 0;
+        for (int64_t b0 = 0, b1; b0 < B; b0 = b1) {
+            b1 = group_end(b0);
+            int64_t gi = 0, go = 0;
+            for (int64_t i = b0; i < b1; i++) {
+                drows[i].in_off = gi; drows[i].out_off = go;
+                gi += rows[i].len; go += rows[i].out_len;
+            }
+            n_in = std::max(n_in, gi); n_out = std::max(n_out, go);
+        }
+        if ((rc = st->arena.reserve(sizeof(float) * (size_t)(n_in + n_out) + 4096))) return rc;
+        st->arena.reset();
+        d_in = st->arena.take<float>((size_t)n_in); d_out = st->arena.take<float>((size_t)n_out);
+    }
+    const float lim = (atten_lim_db > 0.f) ? powf(10.f, -atten_lim_db / 20.f) : 0.f;
+    cudaStream_t sc = host ? m->stream : s, sh = m->h2d, sd = m->d2h;
+    std::vector<cudaEvent_t> evs;
+    auto order = [&](cudaStream_t from, cudaStream_t to) -> int {   // `to` waits for what has been enqueued on `from` so far
+        cudaEvent_t e = nullptr;
+        DFB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        evs.push_back(e);
+        DFB_CUDA(cudaEventRecord(e, from));
+        DFB_CUDA(cudaStreamWaitEvent(to, e, 0));
+        return DFB_OK;
+    };
+    for (int64_t b0 = 0, b1; b0 < B && !rc; b0 = b1) {
+        b1 = group_end(b0);
+        const RaggedRow *hr = rows.data() + b0, *dr = drows.data() + b0;
+        const int64_t *tf = tfs.data() + b0;
+        ChunkHooks hooks;
+        hooks.before = [&](int64_t x0, int64_t x1, int64_t na, cudaStream_t cs) -> int {
+            const int r = copy_streams(d_in, src, x0, na, [&](int64_t i) {
+                return StreamCopy{dr[i].in_off, hr[i].in_off, std::min(x1, hr[i].len)};
+            }, cudaMemcpyHostToDevice, sh);
+            return r ? r : order(sh, cs);
+        };
+        hooks.after = [&](int64_t y0, int64_t y1, int64_t d1, int64_t na, cudaStream_t cs) -> int {
+            if (const int r = order(cs, sd)) return r;
+            return copy_streams(dst, d_out, y0, na, [&](int64_t i) {   // a stream that has ended: all of its output
+                return StreamCopy{hr[i].out_off, dr[i].out_off, tf[i] <= d1 ? hr[i].out_len : std::min(y1, hr[i].out_len)};
+            }, cudaMemcpyDeviceToHost, sd);
+        };
+        // (host) the previous group's D2H copies read the staged output and its compute the staged input: order this
+        // group's first writes after them
+        if (host && ((rc = order(sd, sc)) || (rc = order(sc, sh)))) break;
+        // the previous group's compute still reads the state slab and table: upload this group's table behind it
+        m->aux_arena.reset();
+        RaggedRow *d_rows = m->aux_arena.take<RaggedRow>((size_t)(b1 - b0));
+        DFB_CUDA(cudaMemcpyAsync(d_rows, dr, sizeof(RaggedRow) * (b1 - b0), cudaMemcpyHostToDevice, sc));
+        rc = enhance_group(m, st, host ? d_in : src, host ? d_out : dst, d_rows, tf, b1 - b0, pad, lim, tc, pipelined, sc,
+                           host ? &hooks : nullptr);
+    }
+    if (host) {
+        const cudaError_t e1 = cudaStreamSynchronize(sc), e2 = cudaStreamSynchronize(sd), e3 = cudaStreamSynchronize(sh);
+        const cudaError_t e = e1 != cudaSuccess ? e1 : (e2 != cudaSuccess ? e2 : e3);
+        if (!rc && e != cudaSuccess) rc = fail(DFB_ERR_CUDA, "enhance_host failed: %s", cudaGetErrorString(e));
+    }
+    for (cudaEvent_t e : evs) cudaEventDestroy(e);
+    m->arena.reset();
+    m->arena1.reset();
     return rc;
 }
 
-// Plan shared by both entry points: chunk length, stream group size and the aux arena (state slab + table of one group).
-static int ragged_reserve(dfb_model *m, dfb_state *st, int64_t B, int64_t Tf, int min_chunks, int64_t *group, int *tc, bool *pipelined) {
-    int rc = enhance_plan(m, st, B, Tf, min_chunks, group, tc, pipelined);
-    if (rc) return rc;
-    size_t off[16];
-    return m->aux_arena.reserve(state_floats(m->cfg, st, (int)*group, off) * sizeof(float) + (size_t)*group * sizeof(RaggedRow) + 8192);
+// An equal-length batch [B][T]: stream b is {b T, T, b out_len}.  pad = True appends fft zeros (enhance.py:230-233):
+// Tf = (T + fft) / hop.
+static int equal_rows(const dfb_state *st, int64_t B, int64_t T, int pad, std::vector<RaggedRow> &rows) {
+    const int64_t Tf = (pad ? T + st->fft : T) / st->hop, out_len = dfb_enhance_out_len(st, T, pad);
+    if (Tf <= 0) return fail(DFB_ERR_INVALID, "input shorter than one hop");
+    rows.resize((size_t)B);
+    for (int64_t b = 0; b < B; b++) rows[(size_t)b] = RaggedRow{b * T, T, b * out_len, out_len, Tf};
+    return DFB_OK;
+}
+
+extern "C" int dfb_enhance(dfb_model *m, dfb_state *st, const float *d_audio, int64_t B, int64_t T, int pad,
+                           float atten_lim_db, float *d_out, void *stream) {
+    if (!m || !st || !d_audio || !d_out) return fail(DFB_ERR_INVALID, "null argument");
+    if (B <= 0 || T <= 0) return fail(DFB_ERR_INVALID, "empty input");
+    if (int rcs = check_state(m, st)) return rcs;
+    std::vector<RaggedRow> rows;
+    if (int rc = equal_rows(st, B, T, pad, rows)) return rc;
+    DFB_CUDA(cudaSetDevice(m->device));
+    return enhance_rows(m, st, rows, d_audio, d_out, pad, atten_lim_db, false, (cudaStream_t)stream);
+}
+
+extern "C" int dfb_enhance_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t B, int64_t T, int pad,
+                                float atten_lim_db, float *h_out) {
+    if (!m || !st || !h_audio || !h_out) return fail(DFB_ERR_INVALID, "null argument");
+    if (B <= 0 || T <= 0) return fail(DFB_ERR_INVALID, "empty input");
+    if (int rcs = check_state(m, st)) return rcs;
+    std::vector<RaggedRow> rows;
+    if (int rc = equal_rows(st, B, T, pad, rows)) return rc;
+    DFB_CUDA(cudaSetDevice(m->device));
+    return enhance_rows(m, st, rows, h_audio, h_out, pad, atten_lim_db, true, nullptr);
 }
 
 extern "C" int dfb_enhance_ragged(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
@@ -2430,113 +2427,20 @@ extern "C" int dfb_enhance_ragged(dfb_model *m, dfb_state *st, const float *d_au
     if (!m || !st || !d_audio || !d_out) return fail(DFB_ERR_INVALID, "null argument");
     if (int rcs = check_state(m, st)) return rcs;
     std::vector<RaggedRow> rows;
-    int rc = ragged_plan(st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rows);
-    if (rc) return rc;
+    if (int rc = ragged_plan(st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rows)) return rc;
     DFB_CUDA(cudaSetDevice(m->device));
-    cudaStream_t s = (cudaStream_t)stream;
-    if (m->cfg.model_kind == 1) return ragged_v1(m, st, std::move(rows), d_audio, d_out, pad, atten_lim_db, s, false);
-    const int hop = st->hop;
-    int64_t group = 0;
-    int tc = 0;
-    bool pipelined = false;
-    std::vector<int64_t> tfs(rows.size());
-    int64_t true_frames = 0;
-    for (size_t i = 0; i < rows.size(); i++) { tfs[i] = rows[i].Tf; true_frames += tfs[i]; }
-    int dev_chunks = m->dev_chunks > 0 ? m->dev_chunks : (B <= 8 ? 3 : (B <= 256 ? 2 : 1));   // as dfb_enhance
-    // ended streams drop out at chunk boundaries only: with a spread of lengths, shorter chunks save more padded frames than
-    // they cost (DeepFilterNet3, 128 streams of 1 - 20 s on one H100 at 700 W: 2 chunks 34.6 ms, 4 chunks 30.1 ms, 8 30.3)
-    if (m->dev_chunks == 0 && (double)B * tfs[0] > 1.1 * (double)true_frames && dev_chunks < 4) dev_chunks = 4;
-    if ((rc = ragged_reserve(m, st, B, rows[0].Tf, dev_chunks, &group, &tc, &pipelined))) return rc;
-    const float lim = (atten_lim_db > 0.f) ? powf(10.f, -atten_lim_db / 20.f) : 0.f;
-    for (int64_t b0 = 0; b0 < B && !rc; b0 += group) {
-        const int64_t nb = (B - b0 < group) ? B - b0 : group, Tp = tfs[(size_t)b0] * hop;
-        m->aux_arena.reset();
-        RaggedRow *d_rows = m->aux_arena.take<RaggedRow>((size_t)nb);
-        DFB_CUDA(cudaMemcpyAsync(d_rows, rows.data() + b0, sizeof(RaggedRow) * nb, cudaMemcpyHostToDevice, s));
-        rc = enhance_group(m, st, d_audio, nb, Tp, Tp, pad, lim, d_out, out_numel, tc, pipelined, s, nullptr, d_rows, tfs.data() + b0);
-    }
-    m->arena.reset();
-    m->arena1.reset();
-    return rc;
+    return enhance_rows(m, st, rows, d_audio, d_out, pad, atten_lim_db, false, (cudaStream_t)stream);
 }
 
-// Host buffers: the streams are staged into one packed device buffer chunk by chunk, each stream's range clamped to its
-// length, the H2D copies of chunk c + 1 and the D2H copies of chunk c - 1 overlapping the compute of chunk c as in
-// dfb_enhance_host; only real samples cross PCIe.
 extern "C" int dfb_enhance_ragged_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel, const int64_t *in_offsets,
                                        const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *h_out, int64_t out_numel,
                                        const int64_t *out_offsets) {
     if (!m || !st || !h_audio || !h_out) return fail(DFB_ERR_INVALID, "null argument");
     if (int rcs = check_state(m, st)) return rcs;
     std::vector<RaggedRow> rows;
-    int rc = ragged_plan(st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rows);
-    if (rc) return rc;
+    if (int rc = ragged_plan(st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rows)) return rc;
     DFB_CUDA(cudaSetDevice(m->device));
-    if (m->cfg.model_kind == 1) return ragged_v1(m, st, std::move(rows), h_audio, h_out, pad, atten_lim_db, nullptr, true);
-    const int hop = st->hop;
-    int64_t group = 0;
-    int tc = 0;
-    bool pipelined = false;
-    if ((rc = ragged_reserve(m, st, B, rows[0].Tf, m->host_chunks, &group, &tc, &pipelined))) return rc;
-    const float lim = (atten_lim_db > 0.f) ? powf(10.f, -atten_lim_db / 20.f) : 0.f;
-    // device rows: the same streams packed back to back in the staging buffers
-    std::vector<RaggedRow> drows(rows);
-    std::vector<int64_t> tfs(rows.size());
-    int64_t n_in = 0, n_out = 0;
-    for (size_t i = 0; i < rows.size(); i++) {
-        drows[i].in_off = n_in; drows[i].out_off = n_out;
-        n_in += rows[i].len; n_out += rows[i].out_len;
-        tfs[i] = rows[i].Tf;
-    }
-    if ((rc = st->arena.reserve(sizeof(float) * (size_t)(n_in + n_out) + 4096))) return rc;
-    st->arena.reset();
-    float *d_in = st->arena.take<float>((size_t)n_in), *d_out = st->arena.take<float>((size_t)n_out);
-    cudaStream_t sc = m->stream, sh = m->h2d, sd = m->d2h;
-    std::vector<cudaEvent_t> evs;
-    auto new_event = [&]() { cudaEvent_t e = nullptr; cudaEventCreateWithFlags(&e, cudaEventDisableTiming); evs.push_back(e); return e; };
-    for (int64_t b0 = 0; b0 < B && !rc; b0 += group) {
-        const int64_t nb = (B - b0 < group) ? B - b0 : group, Tp = tfs[(size_t)b0] * hop;
-        const RaggedRow *hr = rows.data() + b0, *dr = drows.data() + b0;
-        const int64_t *tf = tfs.data() + b0;
-        ChunkHooks hooks;
-        hooks.before = [&](int64_t x0, int64_t x1, int64_t na, cudaStream_t cs) -> int {
-            for (int64_t i = 0; i < na; i++) {
-                const int64_t e = x1 < hr[i].len ? x1 : hr[i].len;
-                if (x0 < e)
-                    DFB_CUDA(cudaMemcpyAsync(d_in + dr[i].in_off + x0, h_audio + hr[i].in_off + x0, sizeof(float) * (e - x0),
-                                             cudaMemcpyHostToDevice, sh));
-            }
-            cudaEvent_t ev = new_event();
-            DFB_CUDA(cudaEventRecord(ev, sh));
-            DFB_CUDA(cudaStreamWaitEvent(cs, ev, 0));
-            return DFB_OK;
-        };
-        hooks.after = [&](int64_t y0, int64_t y1, int64_t d1, int64_t na, cudaStream_t cs) -> int {
-            cudaEvent_t ev = new_event();
-            DFB_CUDA(cudaEventRecord(ev, cs));
-            DFB_CUDA(cudaStreamWaitEvent(sd, ev, 0));
-            for (int64_t i = 0; i < na; i++) {
-                const int64_t e = tf[i] <= d1 ? hr[i].out_len : (y1 < hr[i].out_len ? y1 : hr[i].out_len);   // ended: all of it
-                if (y0 < e)
-                    DFB_CUDA(cudaMemcpyAsync(h_out + hr[i].out_off + y0, d_out + dr[i].out_off + y0, sizeof(float) * (e - y0),
-                                             cudaMemcpyDeviceToHost, sd));
-            }
-            return DFB_OK;
-        };
-        // the previous group's compute still reads the state slab and table: upload this group's table behind it
-        m->aux_arena.reset();
-        RaggedRow *d_rows = m->aux_arena.take<RaggedRow>((size_t)nb);
-        DFB_CUDA(cudaMemcpyAsync(d_rows, dr, sizeof(RaggedRow) * nb, cudaMemcpyHostToDevice, sc));
-        rc = enhance_group(m, st, d_in, nb, Tp, Tp, pad, lim, d_out, n_out, tc, pipelined, sc, &hooks, d_rows, tf);
-    }
-    cudaError_t e1 = cudaStreamSynchronize(sc), e2 = cudaStreamSynchronize(sd), e3 = cudaStreamSynchronize(sh);
-    for (cudaEvent_t e : evs) cudaEventDestroy(e);
-    m->arena.reset();
-    m->arena1.reset();
-    if (rc) return rc;
-    if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess)
-        return fail(DFB_ERR_CUDA, "enhance_ragged_host failed: %s", cudaGetErrorString(e1 != cudaSuccess ? e1 : (e2 != cudaSuccess ? e2 : e3)));
-    return DFB_OK;
+    return enhance_rows(m, st, rows, h_audio, h_out, pad, atten_lim_db, true, nullptr);
 }
 
 // ============================================================== streaming API ====

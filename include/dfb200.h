@@ -173,7 +173,8 @@ int dfb_model_forward_full(dfb_model *m, dfb_state *st, const float *d_spec, con
  * atten_lim_db <= 0 disables the attenuation limit (enhance.py:238-240).
  * The apply + ISTFT stage is one fused kernel (gain x spectrum + deep filter + irFFT + OLA).
  * The signal is processed in time chunks with carried state (see "streaming" below), so the device workspace does
- * not grow with T; dfb_enhance_host additionally overlaps the H2D / D2H copies of neighbouring chunks with the compute. */
+ * not grow with T; dfb_enhance_host additionally overlaps the H2D / D2H copies of neighbouring chunks with the compute.
+ * An equal-length batch runs on the same executor as the ragged batch below, with stream b = {b * T, T, b * T_out}. */
 int dfb_enhance(dfb_model *m, dfb_state *st, const float *d_audio, int64_t B, int64_t T, int pad,
                 float atten_lim_db, float *d_out, void *stream);
 int dfb_enhance_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t B, int64_t T, int pad,
@@ -188,10 +189,10 @@ int64_t dfb_enhance_out_len(const dfb_state *st, int64_t T, int pad);
  * does not give: the padded frames would change the look-ahead of every shorter stream's last frames.
  * Offsets cover a padded [B, S] tensor (in_offsets[b] = b * S) as well as streams packed back to back.  The streams run
  * longest first; a time chunk computes only the streams that have frames left in it, so a batch of mixed lengths costs
- * about its true frame count, not B times the longest.  DeepFilterNet v1 (one window per signal) runs every set of
- * equal-length streams through dfb_enhance instead: exact, without that saving.
+ * about its true frame count, not B times the longest.  DeepFilterNet v1 (one window per signal) runs streams of the
+ * same frame count together, so a batch of v1 streams saves no frames.
  * The _host variant takes host pointers (page-locked memory lets its copies overlap the compute), copies only the
- * streams' own samples and results, and is synchronous. */
+ * streams' own samples and results, stages one stream group at a time on the device, and is synchronous. */
 int dfb_enhance_ragged(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
                        const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
                        const int64_t *out_offsets, void *stream);

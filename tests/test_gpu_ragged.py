@@ -215,19 +215,20 @@ def test_ragged_options(states, model_dir, opt):
 
 
 def test_ragged_v1(states):
-    """DeepFilterNet v1 runs each set of equal-length streams through the one-window path."""
+    """DeepFilterNet v1 runs one window per signal: its stream groups share one frame count.  9600 + 123 and 9600 + 300
+    samples have the same frame count (22 with pad, 20 without) but different lengths, so they run in one group."""
     st = states
     cfg = cfg_of("v1")
     model = DfNet(cfg, random_state_dict(cfg, seed=35), st)
-    lengths = [24000, 9600 + 123, 24000, 9600 + 123, 24000]
+    lengths = [24000, 9600 + 123, 24000, 9600 + 300, 9600 + 123, 24000]
     x = padded(lengths, seed=88)
     for pad in (True, False):
-        got = enhance_device_ragged(model, st, x, lengths, pad=pad)
-        assert_per_stream(got, alone(model, st, x, lengths, pad), lengths, pad, tol=1e-7)
-    dev = enhance_device_ragged(model, st, x, lengths).cpu()
-    host = enhance_batch(model, st, [x[b:b + 1, :t].cpu() for b, t in enumerate(lengths)])
-    for b, t in enumerate(lengths):
-        assert rms(host[b][0], dev[b, :t]) < 1e-7, b
+        dev = enhance_device_ragged(model, st, x, lengths, pad=pad)
+        assert_per_stream(dev, alone(model, st, x, lengths, pad), lengths, pad, tol=1e-7)
+        host = enhance_batch(model, st, [x[b:b + 1, :t].cpu() for b, t in enumerate(lengths)], pad=pad)
+        for b, t in enumerate(lengths):
+            n = out_len(t, pad)
+            assert host[b].shape == (1, n) and rms(host[b][0], dev[b, :n].cpu()) < 1e-7, (b, pad)
 
 
 def test_enhance_batch_api_and_errors(states):
