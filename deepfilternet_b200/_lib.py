@@ -96,7 +96,6 @@ SIGNATURES = {
     "dfb_stream_process": (_I, [_VP, _VP, _I64, _VP, _VP]),
     "dfb_stream_flush": (_I, [_VP, _VP, _VP]),
     "dfb_stream_process_host": (_I, [_VP, _VP, _I64, _VP]),
-    "dfb_model_set_precision": (_I, [_VP, _I]),
     "dfb_model_set_max_workspace": (_I, [_VP, _I64]),
     "dfb_model_set_options": (_I, [_VP, _I, _F, _I]),
     "dfb_model_set_chunking": (_I, [_VP, _I, _I, _I]),

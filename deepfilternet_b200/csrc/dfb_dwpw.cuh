@@ -26,11 +26,11 @@ __device__ __forceinline__ unsigned long long f2_fma(unsigned long long a, unsig
     return f2_pack(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
 }
 
-enum DwMode { DW_S1 = 0, DW_S2 = 1, DW_T2 = 2, DW_DF0 = 3 };
+enum DwMode { DW_S1 = 0, DW_S2 = 1, DW_T2 = 2 };
 constexpr int kLdA = kCh + 4;  // padded row stride of the A tile (floats)
 
 struct DwPwParams {
-    const float *in;      // [B,T,Fin,64]  (DF0: feat_spec [B,T,Fin,2])
+    const float *in;      // [B,T,Fin,64]
     const float *path;    // optional [B,T,Fin,64]
     const float *ps, *pb; // pathway scale / bias [64]
     const float *dw;      // [kt][3][64]
@@ -77,15 +77,14 @@ __device__ __forceinline__ float4 dw_prologue(const DwPwParams &p, const DwTaps 
 #pragma unroll
     for (int dt = 0; dt < 3; dt++) {
         if (dt < 3 - p.kt) continue;
-        // causal: taps at t-(kt-1) .. t; p.lookahead shifts them forward (DeepFilterNet v1 pads (kt-1-la, la), modules.py:151-154);
-        // DF0 keeps the DeepFilterNet2 / 3 meaning: the feature sequence is shifted first, then padded causally
-        const int tq = (MODE == DW_DF0) ? t - (2 - dt) : t - (2 - dt) + p.lookahead;
+        // causal: taps at t-(kt-1) .. t; p.lookahead shifts them forward (DeepFilterNet v1 pads (kt-1-la, la), modules.py:151-154)
+        const int tq = t - (2 - dt) + p.lookahead;
         if (tq < 0 || tq >= p.T) continue;
 #pragma unroll
         for (int df = 0; df < 3; df++) {
             int fi;
             float4 wv;
-            if (MODE == DW_S1 || MODE == DW_DF0) { fi = fo + df - 1; wv = tp.wd[dt * 3 + df]; }
+            if (MODE == DW_S1) { fi = fo + df - 1; wv = tp.wd[dt * 3 + df]; }
             else if (MODE == DW_S2) { fi = 2 * fo + df - 1; wv = tp.wd[dt * 3 + df]; }
             else {  // DW_T2: df enumerates the (at most two) contributing taps
                 if (df == 2) continue;
@@ -94,23 +93,14 @@ __device__ __forceinline__ float4 dw_prologue(const DwPwParams &p, const DwTaps 
                 else { fi = (fo >> 1) + 1; wv = tp.wd[dt * 3 + 0]; }
             }
             if (fi < 0 || fi >= p.Fin) continue;
-            float4 x;
-            if (MODE == DW_DF0) {
-                // channels [0,32) read re, [32,64) read im (groups = 2); look-ahead shifted
-                if (tq + p.lookahead >= p.T) continue;
-                const float *src = p.in + ((int64_t)b * p.T + tq + p.lookahead) * p.in_fs + fi * 2;
-                float v = (cq < 8) ? src[0] : src[1];
-                x = make_float4(v, v, v, v);
-            } else {
-                const int64_t o = ((int64_t)b * p.T + tq);
-                x = *reinterpret_cast<const float4 *>(p.in + o * p.in_fs + fi * kCh + cq * 4);
-                if (p.path) {
-                    float4 e = *reinterpret_cast<const float4 *>(p.path + o * p.path_fs + fi * kCh + cq * 4);
-                    x.x += fmaxf(e.x * tp.ps4.x + tp.pb4.x, 0.f);
-                    x.y += fmaxf(e.y * tp.ps4.y + tp.pb4.y, 0.f);
-                    x.z += fmaxf(e.z * tp.ps4.z + tp.pb4.z, 0.f);
-                    x.w += fmaxf(e.w * tp.ps4.w + tp.pb4.w, 0.f);
-                }
+            const int64_t o = ((int64_t)b * p.T + tq);
+            float4 x = *reinterpret_cast<const float4 *>(p.in + o * p.in_fs + fi * kCh + cq * 4);
+            if (p.path) {
+                float4 e = *reinterpret_cast<const float4 *>(p.path + o * p.path_fs + fi * kCh + cq * 4);
+                x.x += fmaxf(e.x * tp.ps4.x + tp.pb4.x, 0.f);
+                x.y += fmaxf(e.y * tp.ps4.y + tp.pb4.y, 0.f);
+                x.z += fmaxf(e.z * tp.ps4.z + tp.pb4.z, 0.f);
+                x.w += fmaxf(e.w * tp.ps4.w + tp.pb4.w, 0.f);
             }
             acc.x += x.x * wv.x; acc.y += x.y * wv.y; acc.z += x.z * wv.z; acc.w += x.w * wv.w;
         }

@@ -185,7 +185,7 @@ k_gl_bx(const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUten
 }
 
 // fp32 [M][K] (row pitch ldx) -> BF16 hi / lo planes [M][K] (pitch K): fallback producer for inputs whose own
-// producer has no plane-writing epilogue (FFMA precision modes, the H = 512 FFMA recurrence)
+// producer wrote none (ensure_planes in dfb_model.cu)
 __global__ void __launch_bounds__(256) k_to_planes(const float *__restrict__ x, int64_t ldx, int64_t M, int K,
                                                    unsigned short *__restrict__ hi, unsigned short *__restrict__ lo) {
     const int64_t n4 = M * (K / 4);

@@ -11,9 +11,10 @@
 // HBM layout: every activation is channel-last [B, T, F, C=64] (C fastest) so a 1x1 conv is a
 // row-major [rows, 64] x [64, 64] product and depthwise taps are +-64-float neighbours;
 // embeddings are [B*T, D] row-major.  BatchNorm is folded on the host (weights.py).
-// Arithmetic: IEEE fp32 (FFMA) everywhere; accumulation order differs from ATen's, which is
-// inside the 1e-4 RMS parity bound (tests/test_gpu_parity.py).
-#include <cooperative_groups.h>
+// Arithmetic: the contractions (GRU recurrence and input projections, separable blocks' 1x1 convs, grouped linears, DF
+// pathway conv) run on the BF16x3 tensor-core kernels of dfb_tc.cu / dfb_gl.cu (fp32-level accuracy, DESIGN.md section 6);
+// the kernels in this file are IEEE fp32 FFMA.  Accumulation order differs from ATen's, which is inside the 1e-4 RMS
+// parity bound (tests/test_gpu_parity.py).
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -26,8 +27,6 @@
 #include "dfb_common.cuh"
 #include "dfb_dwpw.cuh"
 #include "dfb_ptx.cuh"
-
-namespace cg = cooperative_groups;
 
 namespace dfb {
 
@@ -111,14 +110,15 @@ k_conv_in(const float *__restrict__ x, const float *__restrict__ w /*[kt][3][CIN
 }
 
 // ------------------------------------------------- depthwise (+pathway) -> 1x1 -> ReLU ----
-// One fused kernel for every "separable" block of the reference (modules.py:49-71, 104-125):
+// One fused kernel for a "separable" block of the reference (modules.py:49-71, 104-125):
 //   prologue  A[r][c] = sum_{dt,df} dw[dt][df][c] * X[t-(kt-1)+dt][fi(fo,df)][c]
 //             with X = in (+ relu(path * ps + pb) when a pathway tensor is given; that is
 //             `convNp(eN) + prev`, deepfilternet3.py:250-253)
 //   GEMM      out[r][n] = relu(sum_c A[r][c] * pw[c][n] + b[n])
+// The FFMA version of k_dwpw_bx (dfb_tc.cu) for the blocks that one does not build: DeepFilterNet v1's blocks with a
+// look-ahead and its two-time-tap transposed convs.
 // Modes: S1 stride 1, S2 stride 2 (fi = 2 fo + df - 1), T2 transposed stride 2
-// (out[2j] = w1 x[j]; out[2j+1] = w2 x[j] + w0 x[j+1]; ConvTranspose2d padding 1, output_padding 1),
-// DF0 the grouped 2 -> 64 input conv on the complex features (with look-ahead shift).
+// (out[2j] = w1 x[j]; out[2j+1] = w2 x[j] + w0 x[j+1]; ConvTranspose2d padding 1, output_padding 1).
 // Tile: NF frames x Fout rows (R = NF * Fout <= 128, multiple of 4); thread tile 4 rows x 8 cols.
 template <int MODE>
 __global__ void __launch_bounds__(256) k_dwpw(DwPwParams p) {
@@ -192,8 +192,8 @@ __global__ void __launch_bounds__(256) k_dwpw(DwPwParams p) {
 
 // ------------------------------------------------------------------ grouped linear ----
 // Y[m, g*Hg + n] = act( sum_i X[m, g*Ig + i] * W[g][i][n] + bias ) * oscale + ooffset + R[m, ...]
-// (GroupedLinearEinsum, modules.py:766-776; G = 1 with bias = GRU input projection W_ih x + b_ih
-// with W given as [I][H] i.e. already transposed on upload.)
+// (GroupedLinearEinsum, modules.py:766-776.)  The FFMA version of k_gl_bx (dfb_gl.cu) for the shapes that one does not
+// build: the N = 1 heads, DeepFilterNet v1's GroupedLinear with bias, weights without a tensor-core image.
 // CTA tile 64 rows x 64 cols (one group, or a 64-wide slice of a wide group); K chunks of 32.
 struct GlParams {
     const float *x; int64_t ldx;
@@ -335,249 +335,6 @@ __global__ void __launch_bounds__(256) k_grouped_linear(GlParams p) {
     }
 }
 
-// ------------------------------------------------------------------- GRU recurrence ----
-// torch.nn.GRU cell (gate order r, z, n; modules.py:684,723):
-//   r = s(xr + Whr h + bhr), z = s(xz + Whz h + bhz), n = tanh(xn + r (Whn h + bhn)), h' = (1-z) n + z h
-// xproj = W_ih x + b_ih comes from k_grouped_linear.  One thread-block CLUSTER owns a group of Bc
-// streams for the whole sequence: CTA `rank` keeps the W_hh rows of its U = H / C hidden units
-// (3U rows x H) in REGISTERS: 384 threads, each an 8-row x 16-k tile (128 weights), so a thread
-// reads only 16 h values per stream and step from shared memory; the H/16 lanes that share a row
-// group combine their partial sums with a shuffle reduce-scatter.  The hidden state of the group
-// lives in shared memory of every CTA (double buffered); the new slice is broadcast with st.async
-// DSMEM stores that complete bytes on the receiver's mbarrier, so a step needs neither a cluster
-// barrier nor a memory fence (ncu on the first version: membar was the top stall, the release
-// fence of cluster.sync() waited for the global h stores).  H = 256: C = 4, U = 64;  H = 512: C = 16, U = 32.
-constexpr int kGruThreads = 384, kGruRT = 8, kGruKT = 16, kGruSB = 4, kGruMaxBc = 16;
-
-// fp32 pair FMA on packed pairs (f2_fma, dfb_dwpw.cuh): two FFMAs per pair of W rows and (k, stream)
-__device__ __forceinline__ unsigned long long gru_pack2(float lo, float hi) {
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void gru_unpack2(unsigned long long v, float &lo, float &hi) {
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ unsigned long long gru_ffma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-    return f2_fma(a, b, c);
-}
-__device__ __forceinline__ uint32_t gru_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ uint32_t gru_mapa(uint32_t saddr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-    return r;
-}
-// remote (DSMEM) store that completes `4` bytes on the destination CTA's mbarrier: no fence or
-// cluster barrier is needed on the consumer side, it just waits for the expected byte count
-__device__ __forceinline__ void gru_st_async(uint32_t dst, float v, uint32_t mbar) {
-    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(dst),
-                 "r"(__float_as_uint(v)), "r"(mbar)
-                 : "memory");
-}
-__device__ __forceinline__ void gru_mbar_init(uint64_t *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(gru_smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void gru_mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(gru_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void gru_mbar_wait(uint64_t *bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE_%=;\n\t"
-        "bra WAIT_%=;\n\t"
-        "DONE_%=:\n\t"
-        "}\n" ::"r"(gru_smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
-
-struct GruParams {
-    const float *xproj;  // [B,T,3H]
-    const float *whh;    // [3H][H]
-    const float *bhh;    // [3H]
-    const float *res;    // optional [B,T,H] added to the OUTPUT only (identity skip, modules.py:696)
-    float *hout;         // [B,T,H]
-    int B, T, Bc;
-    long long *dbg;      // optional [T][8] clock64 phase stamps of CTA 0 (dfb_debug_gru_timing)
-    // time-chunked execution (see GruWindow): frames t0 + t of buffers with Ts frames per stream, carried state h0 -> hT
-    const float *h0;
-    float *hT;
-    int t0, Ts;
-};
-
-template <int H, int C>
-__global__ void __launch_bounds__(kGruThreads, 1) k_gru(GruParams p) {
-    constexpr int U = H / C;                       // hidden units per CTA
-    constexpr int LPR = H / kGruKT;                // lanes sharing one row group (16 or 32)
-    constexpr int NRG = 3 * U / kGruRT;            // row groups per CTA
-    static_assert(NRG * LPR == kGruThreads, "layout");
-    constexpr int V = kGruRT * kGruSB;             // partial sums per thread and stream chunk (32)
-    constexpr int VF = V / LPR;                    // fully reduced values a lane ends up with
-    constexpr int HP = H + 4;                      // padded h row
-    cg::cluster_group cluster = cg::this_cluster();
-    const int rank = (int)cluster.block_rank();
-    const int group = blockIdx.x / C;
-    const int b0 = group * p.Bc;
-    const int nb = min(p.Bc, p.B - b0);
-    extern __shared__ __align__(16) float gru_smem[];
-    float (*s_h)[kGruMaxBc][HP] = reinterpret_cast<float (*)[kGruMaxBc][HP]>(gru_smem);            // [2][Bc][HP]
-    float (*s_pre)[kGruMaxBc + 1] = reinterpret_cast<float (*)[kGruMaxBc + 1]>(gru_smem + 2 * kGruMaxBc * HP);  // [3U]
-    __shared__ __align__(8) uint64_t s_bar[2];     // s_bar[b]: all of h for buffer b has arrived
-    const int tid = threadIdx.x;
-    const int rg = tid / LPR, kl = tid % LPR;      // row group, k slice [16 kl, 16 kl + 16)
-    // weights -> registers as row pairs: w2[rp][k] = (Whh[row(2 rp)][16 kl + k], Whh[row(2 rp + 1)][16 kl + k])
-    unsigned long long w2[kGruRT / 2][kGruKT];
-#pragma unroll
-    for (int rp = 0; rp < kGruRT / 2; rp++) {
-        const int row0 = rg * kGruRT + 2 * rp, row1 = row0 + 1;  // row in [0, 3U): gate = row / U, unit = row % U
-        const float *s0 = p.whh + ((int64_t)(row0 / U) * H + rank * U + (row0 % U)) * H + kl * kGruKT;
-        const float *s1 = p.whh + ((int64_t)(row1 / U) * H + rank * U + (row1 % U)) * H + kl * kGruKT;
-#pragma unroll
-        for (int k = 0; k < kGruKT; k += 4) {
-            float4 a = *reinterpret_cast<const float4 *>(s0 + k), c = *reinterpret_cast<const float4 *>(s1 + k);
-            w2[rp][k] = gru_pack2(a.x, c.x); w2[rp][k + 1] = gru_pack2(a.y, c.y);
-            w2[rp][k + 2] = gru_pack2(a.z, c.z); w2[rp][k + 3] = gru_pack2(a.w, c.w);
-        }
-    }
-    // index of the first fully reduced value this lane owns after the reduce-scatter
-    int vbase = 0;
-#pragma unroll
-    for (int bit = LPR / 2, n = V / 2; bit >= 1 && n >= 1; bit >>= 1, n >>= 1)
-        if (kl & bit) vbase += n;
-    for (int i = tid; i < 2 * kGruMaxBc * HP; i += kGruThreads) gru_smem[i] = 0.f;  // h0 = 0
-    if (p.h0) {  // carried state (every CTA of the cluster keeps the whole h of its streams)
-        __syncthreads();
-        for (int i = tid; i < nb * H; i += kGruThreads) {
-            const int s = i / H, gu = i - s * H;
-            s_h[0][s][(((gu % kGruKT) / 4) * LPR + gu / kGruKT) * 4 + (gu & 3)] = p.h0[(int64_t)(b0 + s) * H + gu];
-        }
-    }
-    // gate-phase items (s, u): this thread's slots
-    constexpr int kItems = (kGruMaxBc * U + kGruThreads - 1) / kGruThreads;
-    float bh[kItems][3];
-#pragma unroll
-    for (int it = 0; it < kItems; it++) {
-        int item = tid + it * kGruThreads;
-        int u = item % U;
-        bh[it][0] = p.bhh[rank * U + u]; bh[it][1] = p.bhh[H + rank * U + u]; bh[it][2] = p.bhh[2 * H + rank * U + u];
-    }
-    if (tid == 0) {
-        gru_mbar_init(&s_bar[0], 1);
-        gru_mbar_init(&s_bar[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    cluster.sync();  // barriers initialised and h0 = 0 visible before any remote store can arrive
-    const uint32_t bar_local[2] = {gru_smem_u32(&s_bar[0]), gru_smem_u32(&s_bar[1])};
-    const uint32_t step_bytes = (uint32_t)(H * nb * 4);
-    int cur = 0;
-    for (int t = 0; t < p.T; t++) {
-        // arm the barrier of the other buffer for the h_{t+1} bytes, then wait for h_t
-        if (tid == 0 && t + 1 < p.T) gru_mbar_expect_tx(&s_bar[cur ^ 1], step_bytes);
-        const bool dbg_on = p.dbg && blockIdx.x == 0 && tid == 0;
-        if (dbg_on) p.dbg[t * 8 + 0] = clock64();
-        if (t > 0) gru_mbar_wait(&s_bar[cur], (uint32_t)(((t - 1) >> 1) & 1));
-        if (dbg_on) p.dbg[t * 8 + 1] = clock64();
-        // prefetch the input projections of this step for the gate phase (independent of h)
-        float xr[kItems][3];
-#pragma unroll
-        for (int it = 0; it < kItems; it++) {
-            int item = tid + it * kGruThreads;
-            if (item < nb * U) {
-                int s = item / U, u = item - s * U;
-                const float *xp = p.xproj + ((int64_t)(b0 + s) * p.Ts + p.t0 + t) * (3 * H) + rank * U + u;
-                xr[it][0] = xp[0]; xr[it][1] = xp[H]; xr[it][2] = xp[2 * H];
-            }
-        }
-        // matvec: pre[row][s] = sum_k W[row][k] h[s][k]
-        for (int sc = 0; sc < nb; sc += kGruSB) {
-            unsigned long long acc2[kGruRT / 2][kGruSB];
-#pragma unroll
-            for (int rp = 0; rp < kGruRT / 2; rp++)
-#pragma unroll
-                for (int s = 0; s < kGruSB; s++) acc2[rp][s] = 0ull;
-#pragma unroll
-            for (int s = 0; s < kGruSB; s++) {
-                // h is stored permuted (hpos) so that the LPR lanes read consecutive float4s
-                const float *hb = &s_h[cur][sc + s][kl * 4];
-#pragma unroll
-                for (int k = 0; k < kGruKT; k += 4) {
-                    float4 hv = *reinterpret_cast<const float4 *>(hb + (k / 4) * LPR * 4);
-                    const unsigned long long h0 = gru_pack2(hv.x, hv.x), h1 = gru_pack2(hv.y, hv.y),
-                                             h2 = gru_pack2(hv.z, hv.z), h3 = gru_pack2(hv.w, hv.w);
-#pragma unroll
-                    for (int rp = 0; rp < kGruRT / 2; rp++) {
-                        unsigned long long a = acc2[rp][s];
-                        a = gru_ffma2(w2[rp][k], h0, a); a = gru_ffma2(w2[rp][k + 1], h1, a);
-                        a = gru_ffma2(w2[rp][k + 2], h2, a); a = gru_ffma2(w2[rp][k + 3], h3, a);
-                        acc2[rp][s] = a;
-                    }
-                }
-            }
-            float acc[V];
-#pragma unroll
-            for (int rp = 0; rp < kGruRT / 2; rp++)
-#pragma unroll
-                for (int s = 0; s < kGruSB; s++)
-                    gru_unpack2(acc2[rp][s], acc[(2 * rp) * kGruSB + s], acc[(2 * rp + 1) * kGruSB + s]);
-            if (dbg_on && sc == 0) p.dbg[t * 8 + 2] = clock64();
-            // reduce-scatter over the LPR lanes of this row group
-#pragma unroll
-            for (int bit = LPR / 2, n = V / 2; bit >= 1 && n >= 1; bit >>= 1, n >>= 1) {
-                const bool up = (kl & bit) != 0;
-#pragma unroll
-                for (int i = 0; i < V / 2; i++) {
-                    if (i < n) {
-                        float send = up ? acc[i] : acc[i + n];
-                        float keep = up ? acc[i + n] : acc[i];
-                        acc[i] = keep + __shfl_xor_sync(0xffffffffu, send, bit);
-                    }
-                }
-            }
-#pragma unroll
-            for (int i = 0; i < VF; i++) {
-                int v = vbase + i;                      // v = r * kGruSB + s
-                int r = v / kGruSB, s = v % kGruSB;
-                if (sc + s < nb) s_pre[rg * kGruRT + r][sc + s] = acc[i];
-            }
-        }
-        if (dbg_on) p.dbg[t * 8 + 3] = clock64();
-        __syncthreads();
-        if (dbg_on) p.dbg[t * 8 + 4] = clock64();
-        // gates
-#pragma unroll
-        for (int it = 0; it < kItems; it++) {
-            int item = tid + it * kGruThreads;
-            if (item < nb * U) {
-                int s = item / U, u = item - s * U;
-                int gu = rank * U + u;
-                float r = sigmoidf_(xr[it][0] + s_pre[u][s] + bh[it][0]);
-                float z = sigmoidf_(xr[it][1] + s_pre[U + u][s] + bh[it][1]);
-                float n = tanhf(xr[it][2] + r * (s_pre[2 * U + u][s] + bh[it][2]));
-                const int hp = (((gu % kGruKT) / 4) * LPR + gu / kGruKT) * 4 + (gu & 3);  // hpos(gu)
-                float hprev = s_h[cur][s][hp];
-                float hn = (1.f - z) * n + z * hprev;
-                int64_t o = ((int64_t)(b0 + s) * p.Ts + p.t0 + t) * H + gu;
-                p.hout[o] = p.res ? hn + p.res[o] : hn;
-                if (p.hT && t + 1 == p.T) p.hT[(int64_t)(b0 + s) * H + gu] = hn;
-                if (t + 1 < p.T) {
-                    // broadcast the new value to every CTA of the cluster (st.async DSMEM store)
-                    const uint32_t dst_local = gru_smem_u32(&s_h[cur ^ 1][s][hp]);
-#pragma unroll
-                    for (int c = 0; c < C; c++) gru_st_async(gru_mapa(dst_local, c), hn, gru_mapa(bar_local[cur ^ 1], c));
-                }
-            }
-        }
-        if (dbg_on) p.dbg[t * 8 + 5] = clock64();
-        // no CTA barrier here: s_pre is rewritten by the next step's matvec only after the mbarrier
-        // wait at the top of the loop, which needs every gate thread's sends (issued after its reads)
-        cur ^= 1;
-    }
-    cluster.sync();  // no CTA exits while peers may still address its shared memory
-}
-
 // --------------------------------------------------------------- ERB mask output conv ----
 // m[b,t,f] = sigmoid( sum_{dt,df,c} w[dt][df][c] * X[t-(kt-1)+dt][f+df-1][c] + bias ),
 // X = relu(e0 * ps + pb) + d1   (conv0_out(conv0p(e0) + e1), deepfilternet3.py:253).
@@ -690,126 +447,7 @@ __global__ void __launch_bounds__(128) k_convp_v1(const float *__restrict__ c0, 
     for (int k = 0; k < O2; k++) o[k] = tanhf(o[k]) + fmaxf(acc[k], 0.f);
 }
 
-// ------------------------------------------------- DF pathway conv ----
-// coefs[b,t,f,:] = relu( pw( conv_t(c0) ) + b ); the df_out projection later adds tanh(df_out(c)) on top
-// (deepfilternet3.py:293-295, 328-330).  df_convp = grouped (2) temporal conv C -> 2*O with kernel (ktp,1),
-// 1x1 conv, BN, ReLU.
-// A warp owns two adjacent frequency bins and marches along t: the 512 contiguous bytes of c0 it needs per frame arrive
-// by one TMA bulk copy into a per-warp ring of kCpSlots slots (armed kCpSlots frames ahead: ~10 KB in flight per warp,
-// 120 KB per SM -- the first version prefetched five frames through registers, ~30 KB per SM, and sat at 0.30 of the HBM
-// roofline with 12 % occupancy), lane q reads channel quad q of its bin from the slot, keeps its 4 channels' taps for
-// all (dt, o) in registers for the whole kernel, and accumulates the ktp in-flight output frames in rotating registers.
-// A finished frame is reduced over the 8 lanes of its channel group with shuffles, the two groups are exchanged, and
-// lanes 0..2*O-1 apply the 1x1 conv + bias + ReLU and store 40 contiguous bytes.
-constexpr int kMaxO2 = 16, kCpWarps = 4, kCpChunk = 128, kCpSlots = 20;
-template <int ORDER, int KTP, int MINB>
-__global__ void __launch_bounds__(32 * kCpWarps, MINB)
-k_df_convp(const float *__restrict__ c0 /*[B,T,Fd,64]*/, const float *__restrict__ w1 /*[ktp][O2][32]*/,
-           const float *__restrict__ w2 /*[O2][O2]*/, const float *__restrict__ bias, float *__restrict__ coefs,
-           int T, int Fd) {
-    static_assert(kCpSlots % KTP == 0, "a group of KTP frames must not wrap around the ring");
-    constexpr int O2 = 2 * ORDER, CG = kCh / 2;
-    extern __shared__ __align__(128) unsigned char cp_smem[];   // [warp][slot][512 B] | [warp][slot] mbarriers
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int q = lane & 15, g = q >> 3, cq = q & 7;
-    const int f0 = (blockIdx.x * kCpWarps + warp) * 2;        // the warp's first bin (Fd is even: both bins exist or none)
-    const bool f_ok = f0 + 1 < Fd;
-    const int f = f0 + (lane >> 4);
-    const int b = blockIdx.z;
-    const int t_begin = blockIdx.y * kCpChunk, t_end = min(T, t_begin + kCpChunk);
-    float4 wv[KTP][ORDER];
-#pragma unroll
-    for (int dt = 0; dt < KTP; dt++)
-#pragma unroll
-        for (int o = 0; o < ORDER; o++)
-            wv[dt][o] = __ldg(reinterpret_cast<const float4 *>(w1 + (dt * O2 + g * ORDER + o) * CG + 4 * cq));
-    __shared__ float s_w2[O2 * O2 + O2];  // 1x1 conv | bias; lane q < O2 applies column q
-    for (int i = threadIdx.x; i < O2 * O2; i += blockDim.x) s_w2[i] = w2[i];
-    if (threadIdx.x < O2) s_w2[O2 * O2 + threadIdx.x] = bias[threadIdx.x];
-    const uint32_t ring = smem_u32(cp_smem) + (uint32_t)warp * kCpSlots * 512u;
-    const uint32_t bars = smem_u32(cp_smem) + (uint32_t)kCpWarps * kCpSlots * 512u + (uint32_t)warp * kCpSlots * 8u;
-    if (lane == 0) {
-        for (int i = 0; i < kCpSlots; i++) mbar_init_a(bars + 8 * i, 1);
-        fence_barrier_init();
-    }
-    __syncthreads();
-    if (!f_ok) return;
-    const float *s2c = s_w2 + (q < O2 ? q : 0);
-    float acc[KTP][ORDER];
-#pragma unroll
-    for (int u = 0; u < KTP; u++)
-#pragma unroll
-        for (int o = 0; o < ORDER; o++) acc[u][o] = 0.f;
-    const float *src0 = c0 + ((int64_t)b * T * Fd + f0) * kCh;   // frame 0 of the warp's two bins (512 contiguous bytes per frame)
-    const int64_t fs = (int64_t)Fd * kCh;
-    const int tstart = t_begin - (KTP - 1);
-    // frame tp lives in slot (tp - tstart) % kCpSlots; frames before the stream start are zeros and never loaded
-    auto arm = [&](int tp) {
-        const uint32_t slot = (uint32_t)((tp - tstart) % kCpSlots);
-        if (tp >= 0 && tp < t_end) {
-            mbar_expect_tx_a(bars + 8 * slot, 512);
-            bulk_load(ring + slot * 512u, src0 + (int64_t)tp * fs, 512, bars + 8 * slot);
-        } else if (tp < 0) {
-            mbar_arrive_a(bars + 8 * slot);   // nothing to load: still complete the phase so that the slot's parity stays in step
-        }
-    };
-    if (lane == 0)
-        for (int i = 0; i < kCpSlots; i++) arm(tstart + i);
-    __syncwarp();
-    for (int tb = tstart; tb < t_end; tb += KTP) {
-        const uint32_t slot0 = (uint32_t)((tb - tstart) % kCpSlots), parity = (uint32_t)(((tb - tstart) / kCpSlots) & 1);
-        float4 x[KTP];
-#pragma unroll
-        for (int u = 0; u < KTP; u++) {
-            const int tp = tb + u;
-            if (tp >= 0 && tp < t_end) {
-                mbar_wait_a(bars + 8 * (slot0 + u), parity);
-                x[u] = lds128(ring + (slot0 + u) * 512u + lane * 16u);
-            } else {
-                x[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-        }
-        __syncwarp();                       // every lane has its values: the slots may be refilled
-        if (lane == 0)
-#pragma unroll
-            for (int u = 0; u < KTP; u++) arm(tb + u + kCpSlots);
-#pragma unroll
-        for (int u = 0; u < KTP; u++) {
-            const int tp = tb + u;
-            // input frame tp feeds output frame tp + (KTP-1) - dt through tap dt; slot = output frame mod KTP
-#pragma unroll
-            for (int dt = 0; dt < KTP; dt++) {
-                const int slot = (u + KTP - 1 - dt) % KTP;
-#pragma unroll
-                for (int o = 0; o < ORDER; o++) {
-                    const float4 ww = wv[dt][o];
-                    float a = dt == 0 ? 0.f : acc[slot][o];
-                    a = fmaf(x[u].x, ww.x, a); a = fmaf(x[u].y, ww.y, a);
-                    a = fmaf(x[u].z, ww.z, a); a = fmaf(x[u].w, ww.w, a);
-                    acc[slot][o] = a;
-                }
-            }
-            if (tp >= t_begin && tp < t_end) {  // output frame tp (slot u) is complete; warp-uniform condition
-                float v[ORDER], w[ORDER];
-#pragma unroll
-                for (int o = 0; o < ORDER; o++) {
-                    float r = acc[u][o];
-                    r += __shfl_xor_sync(0xffffffffu, r, 1);
-                    r += __shfl_xor_sync(0xffffffffu, r, 2);
-                    r += __shfl_xor_sync(0xffffffffu, r, 4);
-                    v[o] = r;
-                    w[o] = __shfl_xor_sync(0xffffffffu, r, 8);  // the other channel group's sums
-                }
-                float out = s2c[O2 * O2];
-#pragma unroll
-                for (int k = 0; k < ORDER; k++) out = fmaf(g ? w[k] : v[k], s2c[k * O2], out);
-#pragma unroll
-                for (int k = 0; k < ORDER; k++) out = fmaf(g ? v[k] : w[k], s2c[(ORDER + k) * O2], out);
-                if (q < O2) coefs[(((int64_t)b * T + tp) * Fd + f) * O2 + q] = fmaxf(out, 0.f);
-            }
-        }
-    }
-}
+constexpr int kMaxO2 = 16;  // largest 2 * df_order dfb_model_create accepts
 
 }  // namespace dfb
 
@@ -817,7 +455,6 @@ k_df_convp(const float *__restrict__ c0 /*[B,T,Fd,64]*/, const float *__restrict
 using namespace dfb;
 
 
-struct GruLayerW { const float *w_ih_t, *w_hh, *b_ih, *b_hh; int in_dim; };
 // carried hidden states of one GRU stack between time chunks: h = [layers][Bs][H]; t0 = first frame the recurrences run.
 // Bs is the stream count the state was allocated for: a chunk may run only a prefix B <= Bs of the streams (ragged batch)
 struct GruChunk { float *h; bool have_state; int t0; int Bs; };
@@ -827,11 +464,7 @@ struct dfb_model {
     dfb_model_config cfg;
     std::map<std::string, std::pair<float *, int64_t>> t;  // device tensors
     std::map<std::string, std::pair<const float *, int64_t>> dbg;  // activations of the last forward
-    std::vector<GruLayerW> enc_gru, erb_gru, df_gru;
     float *slab = nullptr;
-    int conv_tc = 0; // 1: 1x1 convs of the separable blocks on the BF16x3 tensor-core path
-    int proj_tc = 0; // 1: GRU input projections on the BF16x3 tensor-core GEMM (needs gru_tc)
-    int gru_tc = 0;  // 1: tensor-core recurrence (BF16 hi/lo split operands) for H = 256
     long long *gru_dbg = nullptr;  // device buffer for dfb_debug_gru_timing
     Arena arena;
     int dev_chunks = 0, host_chunks = 4, n_lanes = 2;   // chunk pipeline (dfb_model_set_chunking); dev_chunks 0 = auto
@@ -899,7 +532,7 @@ extern "C" int dfb_model_create(dfb_model **out, int device, const dfb_model_con
         const long long mb = atoll(e);
         if (mb > 0) m->max_workspace = (size_t)mb << 20;
     }
-    // upload: one slab; GRU w_ih is stored transposed ([I][3H]) for the projection GEMM
+    // upload: one slab
     size_t total = 0;
     for (int i = 0; i < n_tensors; i++) total += ((size_t)tensors[i].numel * 4 + 255) & ~size_t(255);
     if (cudaMalloc(&m->slab, total + 256) != cudaSuccess) {
@@ -966,8 +599,8 @@ extern "C" void dfb_model_free(dfb_model *m) {
 }
 
 // Debug: when `steps` > 0, every following GRU launch stamps clock64() phases of CTA 0 into a device
-// buffer [steps][8] (0 step start, 1 h arrived, 2 matvec done, 3 reduce + s_pre stored, 4 CTA barrier
-// passed, 5 gates + sends issued); returns them for the LAST launch when called with h_out != NULL.
+// buffer [steps][8] (k_gru_tc: 0 step start, 1 state arrived, 2 MMAs done, 3 gates done, 4 slice sent);
+// returns them for the LAST launch when called with h_out != NULL.
 extern "C" int dfb_debug_gru_timing(dfb_model *m, int steps, long long *h_out) {
     if (!m) return fail(DFB_ERR_INVALID, "null model");
     cudaSetDevice(m->device);
@@ -980,14 +613,6 @@ extern "C" int dfb_debug_gru_timing(dfb_model *m, int steps, long long *h_out) {
         DFB_CUDA(cudaMalloc(&m->gru_dbg, sizeof(long long) * 8 * steps));
         DFB_CUDA(cudaMemset(m->gru_dbg, 0, sizeof(long long) * 8 * steps));
     }
-    return DFB_OK;
-}
-
-extern "C" int dfb_model_set_precision(dfb_model *m, int mode) {
-    if (!m || mode < 0 || mode > 15 || (mode & 1)) return fail(DFB_ERR_INVALID, "precision mode out of range (bit 0 is reserved)");
-    m->gru_tc = (mode >> 1) & 1;  // bit 1: tensor-core GRU recurrence (BF16x3 split, ~fp32 accurate)
-    m->proj_tc = (mode >> 2) & 1; // bit 2: GRU input projections on the BF16x3 tensor-core GEMM
-    m->conv_tc = (mode >> 3) & 1; // bit 3: 1x1 convs of the separable blocks and the grouped linears on the BF16x3 tensor-core kernels
     return DFB_OK;
 }
 
@@ -1027,100 +652,47 @@ int run_gl(cudaStream_t s, const float *x, int64_t ldx, const float *w, const fl
     return DFB_OK;
 }
 
-template <int H, int C>
-int launch_gru_t(cudaStream_t s, const GruParams &p, int ngroups) {
-    constexpr int smem = (2 * kGruMaxBc * (H + 4) + 3 * (H / C) * (kGruMaxBc + 1)) * 4;
-    static PerDeviceOnce attr_once;
-    if (auto once_guard = attr_once.first()) {
-        if (C > 8) DFB_CUDA(cudaFuncSetAttribute(k_gru<H, C>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-        DFB_CUDA(cudaFuncSetAttribute(k_gru<H, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(ngroups * C));
-    cfg.blockDim = dim3(kGruThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = s;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    GruParams pp = p;
-    DFB_PROF("k_gru", s);
-    DFB_CUDA(cudaLaunchKernelEx(&cfg, k_gru<H, C>, pp));
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return DFB_OK;
-}
-
-int pick_bc(int B, int max_clusters) {
-    int bc = (B + max_clusters - 1) / max_clusters;
-    bc = ((bc + kGruSB - 1) / kGruSB) * kGruSB;
-    if (bc < kGruSB) bc = kGruSB;
-    if (bc > kGruMaxBc) bc = kGruMaxBc;
-    return bc;
-}
-
 // x [M, in_dim] -> multi-layer GRU -> y [M, H]  (uses xproj scratch [M,3H] and h ping-pong buffers)
 // x_hi/x_lo: BF16 planes of x (written by the producing grouped linear), pl_hi/pl_lo: scratch planes for the
-// inter-layer hidden state; used when the projection runs on the BF16x3 tensor-core GEMM.
-int run_gru(dfb_model *m, cudaStream_t s, const char *name, int layers, int H, const float *x, int in_dim,
-            const float *res_last, float *y, float *xproj, float *tmp_h, int B, int T,
-            unsigned short *x_hi = nullptr, unsigned short *x_lo = nullptr, unsigned short *pl_hi = nullptr,
-            unsigned short *pl_lo = nullptr, int wide = 0, unsigned short *out_hi = nullptr, unsigned short *out_lo = nullptr,
-            bool *out_planes_ok = nullptr, const GruChunk *ck = nullptr) {
+// inter-layer hidden state, the input of the next layer's projection GEMM.
+int run_gru(dfb_model *m, cudaStream_t s, const char *name, int layers, int H, int in_dim, const float *res_last, float *y,
+            float *xproj, float *tmp_h, int B, int T, const unsigned short *x_hi, const unsigned short *x_lo,
+            unsigned short *pl_hi, unsigned short *pl_lo, int wide, unsigned short *out_hi, unsigned short *out_lo,
+            bool *out_planes_ok, const GruChunk *ck) {
     if (out_planes_ok) *out_planes_ok = false;
+    if (!x_hi || !x_lo || !pl_hi || !pl_lo || in_dim % 64)
+        return fail(DFB_ERR_INVALID, "GRU '%s': input planes, scratch planes and an input width that is a multiple of 64 are required", name);
     // time-chunked execution: the buffers hold T frames per stream, the recurrences run over frames [ck->t0, T) only and
     // continue from / leave behind the carried per-layer states; the projections simply cover every row
     const int t0 = ck ? ck->t0 : 0, Tn = T - t0;
     const int64_t M = (int64_t)B * T;
-    const float *cur_in = x;
     int cur_dim = in_dim;
-    const bool tc_gru = m->gru_tc && (H == 256 || H == 512);
-    const bool tc_proj = m->proj_tc && tc_gru && x_hi && pl_hi && cur_dim % 64 == 0;
     const unsigned short *cur_hi = x_hi, *cur_lo = x_lo;
     for (int l = 0; l < layers; l++) {
         std::string base = std::string(name) + ".l" + std::to_string(l);
-        const float *w_ih_t, *w_hh, *b_ih, *b_hh;
+        const float *w_hh, *b_ih, *b_hh, *w_hi, *w_lo;  // w_hi / w_lo: bf16 planes packed two per float
         int rc;
-        if ((rc = need(m, (base + ".w_ih_t").c_str(), (int64_t)3 * H * cur_dim, &w_ih_t))) return rc;
         if ((rc = need(m, (base + ".w_hh").c_str(), (int64_t)3 * H * H, &w_hh))) return rc;
         if ((rc = need(m, (base + ".b_ih").c_str(), 3 * H, &b_ih))) return rc;
         if ((rc = need(m, (base + ".b_hh").c_str(), 3 * H, &b_hh))) return rc;
-        if (tc_proj) {
-            const float *w_hi, *w_lo;  // bf16 planes packed two per float
-            if ((rc = need(m, (base + ".w_ih_hi").c_str(), (int64_t)3 * H * cur_dim / 2, &w_hi)) ||
-                (rc = need(m, (base + ".w_ih_lo").c_str(), (int64_t)3 * H * cur_dim / 2, &w_lo)))
-                return rc;
-            rc = launch_gemm_bf16x3(s, cur_hi, cur_lo, cur_dim, w_hi, w_lo, b_ih, xproj, 3 * H, M, 3 * H, cur_dim);
-        } else {
-            rc = run_gl(s, cur_in, cur_dim, w_ih_t, b_ih, nullptr, 0, xproj, 3 * H, M, 1, cur_dim, 3 * H, ACT_NONE);
-        }
-        if (rc) return rc;
-        float *dst = (l == layers - 1) ? y : tmp_h;
+        if ((rc = need(m, (base + ".w_ih_hi").c_str(), (int64_t)3 * H * cur_dim / 2, &w_hi)) ||
+            (rc = need(m, (base + ".w_ih_lo").c_str(), (int64_t)3 * H * cur_dim / 2, &w_lo)))
+            return rc;
+        if ((rc = launch_gemm_bf16x3(s, cur_hi, cur_lo, cur_dim, w_hi, w_lo, b_ih, xproj, 3 * H, M, 3 * H, cur_dim))) return rc;
+        const bool last = l == layers - 1;
+        float *dst = last ? y : tmp_h;
         float *hs = ck && ck->h ? ck->h + (int64_t)l * ck->Bs * H : nullptr;   // carried state of this layer [Bs][H], rows [0, B)
         GruWindow gw{ck && ck->have_state ? hs : nullptr, hs, t0, T};
-        GruParams p{xproj, w_hh, b_hh, (l == layers - 1) ? res_last : nullptr, dst, B, Tn, 0, m->gru_dbg, gw.h0, gw.hT, t0, T};
-        if (tc_gru) {
-            const bool last = l == layers - 1;
-            const bool planes = last ? out_hi != nullptr : tc_proj;
-            // the last layer's planes feed a grouped linear and include the residual; the others feed the next projection
-            rc = launch_gru_tc(s, xproj, w_hh, b_hh, last ? res_last : nullptr, dst, planes ? (last ? out_hi : pl_hi) : nullptr,
-                               planes ? (last ? out_lo : pl_lo) : nullptr, B, Tn, m->gru_dbg, wide, last ? 1 : 0, &gw, H);
-            if (last && planes && out_planes_ok) *out_planes_ok = true;
-            cur_hi = pl_hi; cur_lo = pl_lo;
-        } else if (H == 256) {
-            int sms = 0;
-            DFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device));
-            p.Bc = pick_bc(B, sms / 4);   // one wave of 4-CTA clusters
-            rc = launch_gru_t<256, 4>(s, p, (B + p.Bc - 1) / p.Bc);
-        } else {
-            p.Bc = pick_bc(B, 8);
-            rc = launch_gru_t<512, 16>(s, p, (B + p.Bc - 1) / p.Bc);
-        }
-        if (rc) return rc;
-        cur_in = dst;
+        // the last layer's planes feed a grouped linear and include the residual; the others feed the next projection
+        unsigned short *hi = last ? out_hi : pl_hi, *lo = last ? out_lo : pl_lo;
+        if ((rc = launch_gru_tc(s, xproj, w_hh, b_hh, last ? res_last : nullptr, dst, hi, lo, B, Tn, m->gru_dbg,
+                                wide, last ? 1 : 0, &gw, H)))
+            return rc;
+        if (last && hi && out_planes_ok) *out_planes_ok = true;
+        cur_hi = pl_hi; cur_lo = pl_lo;
         cur_dim = H;
-        // middle layers may write tmp_h in place: the recurrence only reads xproj, which the
-        // projection GEMM above has already produced from the previous contents of tmp_h.
+        // middle layers may rewrite tmp_h and the scratch planes in place: the recurrence only reads xproj, which the
+        // projection GEMM above has already produced from the previous contents of the planes.
     }
     return DFB_OK;
 }
@@ -1144,7 +716,7 @@ int run_dwpw(cudaStream_t s, DwPwParams p, int B, const float *w_sw = nullptr) {
     if (p.NF < 1) p.NF = 1;
     if (p.NF * p.Fout > 128 || (p.NF * p.Fout) % 4) return fail(DFB_ERR_UNSUPPORTED, "dwpw tile: Fout = %d", p.Fout);
     dim3 grid((unsigned)((p.T + p.NF - 1) / p.NF), (unsigned)B);
-    DFB_PROF(MODE == DW_DF0 ? "k_dwpw[df_conv0]" : "k_dwpw", s);
+    DFB_PROF("k_dwpw", s);
     k_dwpw<MODE><<<grid, 256, smem, s>>>(p);
     DFB_LAUNCH_CHECK();
     return DFB_OK;
@@ -1333,7 +905,6 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
     Pl pl_c1{f.c1_hi, f.c1_lo, (int64_t)Fd / 2 * kCh, false}, pl_embin{f.embin_hi, f.embin_lo, emb_in_dim, false},
        pl_gb{f.gb_hi, f.gb_lo, H, false}, pl_emb{f.emb_hi, f.emb_lo, emb_dim, false}, pl_dfc{f.dfc_hi, f.dfc_lo, Hd, false},
        pl_ga{f.ga_hi, f.ga_lo, H, false}, pl_ga2{f.ga2_hi, f.ga2_lo, Hd, false};
-    const bool gl_tc = m->conv_tc != 0;
     // planes of `x` for a tensor-core consumer: converts on `st` unless the producer already wrote them
     auto ensure_planes = [&](cudaStream_t st, const float *x, int64_t ldx, int K, Pl &pl) -> int {
         if (pl.ok) return DFB_OK;
@@ -1342,8 +913,8 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         if (!r) pl.ok = true;
         return r;
     };
-    // grouped linear `wname` ([G][I/G][Hh/G]): the BF16x3 tensor-core kernel when the tensor-core bit is set and the shape is
-    // built, else the FFMA kernel.  xin: planes of x (converted on demand); yout (optional): planes of y to produce,
+    // grouped linear `wname` ([G][I/G][Hh/G]): the BF16x3 tensor-core kernel when the shape is built, else the FFMA
+    // kernel.  xin: planes of x (converted on demand); yout (optional): planes of y to produce,
     // ycol: column offset of y inside its plane buffer
     auto gl = [&](cudaStream_t st, const char *wname, const float *x, int64_t ldx, Pl *xin, int G, int I, int Hh, int act,
                   const float *res, int64_t ldr, float *y, int64_t ldy, Pl *yout, int64_t ycol = 0) -> int {
@@ -1353,12 +924,12 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         unsigned short *yh = yout ? yout->hi + ycol : nullptr, *yl = yout ? yout->lo + ycol : nullptr;
         const std::string bx = std::string(wname) + "_bx";
         int gpc, hgp, stages;
-        if (gl_tc && xin && m->get(bx) && gl_bx_geometry(G, I / G, Hh / G, &gpc, &hgp, &stages)) {
+        if (xin && m->get(bx) && gl_bx_geometry(G, I / G, Hh / G, &gpc, &hgp, &stages)) {
             if ((r = ensure_planes(st, x, ldx, I, *xin))) return r;
             r = launch_gl_bx(st, xin->hi, xin->lo, xin->ld, m->get(bx), res, ldr, y, ldy, yh, yl, yout ? yout->ld : 0, M, G, I / G,
                              Hh / G, act, 1.f, 0.f);
             if (r != DFB_ERR_UNSUPPORTED) {
-                if (!r && yout && (ycol == 0 || true)) yout->ok = true;
+                if (!r && yout) yout->ok = true;
                 return r;
             }
         }
@@ -1379,15 +950,13 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         k_conv_in<1><<<grid, 256, smem, s>>>(d_feat_erb, w, bb, f.e0, T, E, c.inp_kt, c.conv_lookahead, Tsx, Tx, 0, rows, W0);
         DFB_LAUNCH_CHECK();
     }
-    const float *pw_sw = nullptr;  // set by blk(): swizzled BF16 hi | lo image of the [C_out][C_in] 1x1 weights (tensor-core path)
+    const float *pw_sw = nullptr;  // set by blk(): swizzled BF16 hi | lo image of the [C_out][C_in] 1x1 weights
     auto blk = [&](const char *name, DwPwParams &p) -> int {
         std::string n(name);
         int r;
-        if ((r = need(m, (n + ".dw").c_str(), -1, &p.dw)) || (r = need(m, (n + ".pw").c_str(), kCh * kCh, &p.pw)) ||
-            (r = need(m, (n + ".b").c_str(), kCh, &p.bias)))
+        if ((r = need(m, (n + ".dw").c_str(), -1, &p.dw)) || (r = need(m, (n + ".b").c_str(), kCh, &p.bias)) ||
+            (r = need(m, (n + ".pw_sw").c_str(), kCh * kCh, &pw_sw)))
             return r;
-        pw_sw = nullptr;
-        if (m->conv_tc && (r = need(m, (n + ".pw_sw").c_str(), kCh * kCh, &pw_sw))) return r;
         return DFB_OK;
     };
     // the DF-branch input convs run concurrently with the ERB-branch convs
@@ -1414,10 +983,9 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         }
         p = mk(f.c0, Fd, (int64_t)Fd * kCh, f.c1, Fd / 2, (int64_t)Fd / 2 * kCh, c.conv_kt);
         if ((rc = blk("enc.df_conv1", p))) return rc;
-        if (pw_sw && gl_tc) {  // c1 only feeds df_fc_emb: write its BF16 planes instead of the fp32 tensor
-            p.out = nullptr; p.out_hi = pl_c1.hi; p.out_lo = pl_c1.lo; pl_c1.ok = true;
-            m->dbg.erase("c1");
-        }
+        // c1 only feeds df_fc_emb: write its BF16 planes instead of the fp32 tensor
+        p.out = nullptr; p.out_hi = pl_c1.hi; p.out_lo = pl_c1.lo; pl_c1.ok = true;
+        m->dbg.erase("c1");
         if ((rc = run_dwpw<DW_S2>(sa, p, B, pw_sw))) return rc;
         DFB_CUDA(cudaEventRecord(L.ev_join_enc, sa));
         // DF pathway conv (needs c0 only; its result is consumed by the very last DF-decoder kernel): on the
@@ -1425,25 +993,16 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         // clusters later -- leaves idle (on the DF branch's own streams it delays df_fc_emb, which is on the critical path)
         DFB_CUDA(cudaStreamWaitEvent(sl, L.ev_c0, 0));
         const int O2 = 2 * c.df_order;
-        const float *w1, *w2, *bb;
-        if ((rc = need(m, "df_dec.df_convp.w1", (int64_t)c.df_pathway_kt * O2 * (kCh / 2), &w1)) ||
-            (rc = need(m, "df_dec.df_convp.w2", O2 * O2, &w2)) || (rc = need(m, "df_dec.df_convp.b", O2, &bb)))
-            return rc;
         if (c.df_order != 5 || c.df_pathway_kt != 5)
             return fail(DFB_ERR_UNSUPPORTED, "df_order %d / df_pathway_kernel_size_t %d (built kernels: 5, 5)", c.df_order,
                         c.df_pathway_kt);
         if (Fd % 2) return fail(DFB_ERR_UNSUPPORTED, "df pathway conv: odd nb_df");
-        dim3 grid((unsigned)((Fd + 2 * kCpWarps - 1) / (2 * kCpWarps)), (unsigned)((T + kCpChunk - 1) / kCpChunk), (unsigned)B);
-        static const bool convp_ffma = getenv("DFB_CONVP_FFMA") && atoi(getenv("DFB_CONVP_FFMA"));
-        const float *w_sw = (m->conv_tc && !convp_ffma) ? m->get("df_dec.df_convp.w_sw") : nullptr;
-        if (w_sw) {  // channel contraction on the tensor cores (BF16x3), shifted adds + 1x1 conv in the epilogue
-            if ((rc = launch_df_convp_tc(sl, f.c0, w_sw, w2, bb, d_coefs, B, T, Fd))) return rc;
-        } else {
-            DFB_PROF("k_df_convp", sl);
-            const int smem = kCpWarps * kCpSlots * (512 + 8);
-            k_df_convp<5, 5, 3><<<grid, 32 * kCpWarps, smem, sl>>>(f.c0, w1, w2, bb, d_coefs, T, Fd);
-            DFB_LAUNCH_CHECK();
-        }
+        const float *w_sw, *w2, *bb;
+        if ((rc = need(m, "df_dec.df_convp.w_sw", kCh * kCh, &w_sw)) || (rc = need(m, "df_dec.df_convp.w2", O2 * O2, &w2)) ||
+            (rc = need(m, "df_dec.df_convp.b", O2, &bb)))
+            return rc;
+        // channel contraction on the tensor cores (BF16x3), shifted adds + 1x1 conv in the epilogue
+        if ((rc = launch_df_convp_tc(sl, f.c0, w_sw, w2, bb, d_coefs, B, T, Fd))) return rc;
         DFB_CUDA(cudaEventRecord(L.ev_convp, sl));
     }
     {
@@ -1453,7 +1012,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         if ((rc = blk("enc.erb_conv2", p)) || (rc = run_dwpw<DW_S2>(s, p, B, pw_sw))) return rc;
         p = mk(f.e2, E / 4, (int64_t)E / 4 * kCh, f.e3, E / 4, e3_fs, c.conv_kt);
         if ((rc = blk("enc.erb_conv3", p))) return rc;
-        if (pw_sw && gl_tc && c.enc_concat) { p.out_hi = pl_embin.hi; p.out_lo = pl_embin.lo; }  // DFN2: e3 is the first half of emb_in
+        if (c.enc_concat) { p.out_hi = pl_embin.hi; p.out_lo = pl_embin.lo; }  // DFN2: e3 is the first half of emb_in
         if ((rc = run_dwpw<DW_S1>(s, p, B, pw_sw))) return rc;
 
     }
@@ -1461,11 +1020,9 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
     {
         // cemb = relu(df_fc_emb(c1 flat)); emb_in = e3 flat + cemb  (DFN2: concat)
         const int I = Fd / 2 * kCh;
-        const bool e3_planes = pw_sw && gl_tc && c.enc_concat;
-        if (c.enc_concat) {
+        if (c.enc_concat) {  // the first half's planes were written by erb_conv3
             rc = gl(s, "enc.df_fc_emb.gl", f.c1, I, &pl_c1, c.g_df_fc_emb, I, ED, ACT_RELU, nullptr, 0, f.emb_in + ED, emb_in_dim,
                     &pl_embin, ED);
-            pl_embin.ok = pl_embin.ok && e3_planes;  // both halves must have been written as planes
         } else {
             rc = gl(s, "enc.df_fc_emb.gl", f.c1, I, &pl_c1, c.g_df_fc_emb, I, ED, ACT_RELU, f.e3, ED, f.emb_in, emb_in_dim, &pl_embin);
         }
@@ -1477,14 +1034,14 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
                      &pl_ga))) return rc;
         float *gout = c.g_enc_out ? f.g_b : f.emb;
         Pl &pl_gout = c.g_enc_out ? pl_gb : pl_emb;
-        if ((rc = run_gru(m, s, "enc.emb_gru", c.enc_gru_layers, H, f.g_a, H, nullptr, gout, f.xproj, f.g_h, B, T, f.ga_hi, f.ga_lo,
-                          f.gh_hi, f.gh_lo, 0, gl_tc ? pl_gout.hi : nullptr, gl_tc ? pl_gout.lo : nullptr, &pl_gout.ok, cx ? &ck_enc : nullptr))) return rc;
+        if ((rc = run_gru(m, s, "enc.emb_gru", c.enc_gru_layers, H, H, nullptr, gout, f.xproj, f.g_h, B, T, f.ga_hi, f.ga_lo,
+                          f.gh_hi, f.gh_lo, 0, pl_gout.hi, pl_gout.lo, &pl_gout.ok, cx ? &ck_enc : nullptr))) return rc;
         if (c.g_enc_out) {
             if ((rc = gl(s, "enc.emb_gru.out.gl", f.g_b, H, &pl_gb, c.g_enc_out, H, ED, ACT_RELU, nullptr, 0, f.emb, emb_dim, &pl_emb)))
                 return rc;
         }
         // the decoders read emb's planes on two streams: make sure they exist before the fork
-        if (gl_tc && (rc = ensure_planes(s, f.emb, emb_dim, emb_dim, pl_emb))) return rc;
+        if ((rc = ensure_planes(s, f.emb, emb_dim, emb_dim, pl_emb))) return rc;
         if (d_lsnr) {
             const float *lw, *lb;
             if ((rc = need(m, "enc.lsnr.w", emb_dim, &lw)) || (rc = need(m, "enc.lsnr.b", 1, &lb))) return rc;
@@ -1522,8 +1079,8 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
             return rc;
         const float *res = c.model_kind == 2 ? f.g_a2 : (early_skip ? f.dfskip : nullptr);
         if (early_skip) DFB_CUDA(cudaStreamWaitEvent(s, L.ev_skip, 0));
-        if ((rc = run_gru(m, s, "df_dec.df_gru", c.df_gru_layers, Hd, f.g_a2, Hd, res, f.dfc, f.xproj2, f.g_h2, B, T, f.ga2_hi, f.ga2_lo,
-                          f.gh2_hi, f.gh2_lo, wide_df, gl_tc ? pl_dfc.hi : nullptr, gl_tc ? pl_dfc.lo : nullptr, &pl_dfc.ok, cx ? &ck_df : nullptr))) return rc;
+        if ((rc = run_gru(m, s, "df_dec.df_gru", c.df_gru_layers, Hd, Hd, res, f.dfc, f.xproj2, f.g_h2, B, T, f.ga2_hi, f.ga2_lo,
+                          f.gh2_hi, f.gh2_lo, wide_df, pl_dfc.hi, pl_dfc.lo, &pl_dfc.ok, cx ? &ck_df : nullptr))) return rc;
         if (c.g_df_skip && !early_skip) {
             if ((rc = gl(s, "df_dec.df_skip.gl", f.emb, emb_dim, &pl_emb, c.g_df_skip, emb_dim, Hd, ACT_NONE, f.dfc, Hd, f.dfc, Hd, nullptr)))
                 return rc;
@@ -1535,7 +1092,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
             if ((rc = run_gl(s, f.dfc, Hd, aw, ab, nullptr, 0, d_alpha, 1, M, 1, Hd, 1, ACT_SIGMOID))) return rc;
         }
         const int O2 = 2 * c.df_order;
-        // coefs = tanh(df_out(c)) + df_convp(c0); the pathway term was written by k_df_convp on the low-priority stream
+        // coefs = tanh(df_out(c)) + df_convp(c0); the pathway term was written by k_df_convp_tc on the low-priority stream
         DFB_CUDA(cudaStreamWaitEvent(s, L.ev_convp, 0));
         if ((rc = gl(s, "df_dec.df_out.gl", f.dfc, Hd, &pl_dfc, c.g_df_out, Hd, Fd * O2, ACT_TANH, d_coefs, (int64_t)Fd * O2, d_coefs,
                      (int64_t)Fd * O2, nullptr))) return rc;
@@ -1548,8 +1105,8 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         // DFN2 (SqueezedGRU): identity skip around the GRU, y = GRU(x) + x  (modules.py:695-697)
         const float *res = c.model_kind == 2 ? f.g_a : nullptr;
         pl_gb.ok = false;
-        if ((rc = run_gru(m, s, "erb_dec.emb_gru", c.erb_gru_layers, H, f.g_a, H, res, f.g_b, f.xproj, f.g_h, B, T, f.ga_hi, f.ga_lo,
-                          f.gh_hi, f.gh_lo, wide_erb, gl_tc ? pl_gb.hi : nullptr, gl_tc ? pl_gb.lo : nullptr, &pl_gb.ok, cx ? &ck_erb : nullptr))) return rc;
+        if ((rc = run_gru(m, s, "erb_dec.emb_gru", c.erb_gru_layers, H, H, res, f.g_b, f.xproj, f.g_h, B, T, f.ga_hi, f.ga_lo,
+                          f.gh_hi, f.gh_lo, wide_erb, pl_gb.hi, pl_gb.lo, &pl_gb.ok, cx ? &ck_erb : nullptr))) return rc;
         if ((rc = gl(s, "erb_dec.emb_gru.out.gl", f.g_b, H, &pl_gb, c.g_erb_out, H, ED, ACT_RELU, nullptr, 0, f.dec_emb, ED, nullptr)))
             return rc;
         if (cx && cx->dec_tail && c.conv_kt > 1) {
@@ -1582,8 +1139,8 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
             return rc;
         p = mk(f.d2, E / 2, (int64_t)E / 2 * kCh, f.d1, E, (int64_t)E * kCh, 1);
         if ((rc = blk("erb_dec.convt1", p)) || (rc = path(p, "erb_dec.conv1p", f.e1, (int64_t)E / 2 * kCh))) return rc;
-        // kt = 1 models on the tensor-core path: the mask head is evaluated in convt1's epilogue and d1 never leaves the SM
-        const bool fused_mask = pw_sw && c.conv_kt == 1 && 128 % E == 0;
+        // kt = 1 models: the mask head is evaluated in convt1's epilogue and d1 never leaves the SM
+        const bool fused_mask = c.conv_kt == 1 && 128 % E == 0;
         if (fused_mask) {
             p.mk_e0 = f.e0; p.mk_ps = ps; p.mk_pb = pb; p.mk_w = w; p.mk_bias = bb; p.mk_out = d_m;
             p.out = nullptr;
@@ -1644,7 +1201,6 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
     m->dbg["cemb"] = {f.cemb, M * H}; m->dbg["emb_in"] = {f.emb, M * H}; m->dbg["emb"] = {f.embo, M * H};
     m->dbg["dec_emb"] = {f.dec, M * H}; m->dbg["d3"] = {f.d3, M * (E / 4) * kCh}; m->dbg["d2"] = {f.d2, M * (E / 2) * kCh};
     m->dbg["d1"] = {f.d1, M * E * kCh}; m->dbg["dfc"] = {f.dfc, M * H}; m->dbg["y0"] = {f.y[0], M * H};
-    const bool tc = m->conv_tc != 0;
     const float *ones, *zeros;
     if ((rc = need(m, "v1.ones", kCh, &ones)) || (rc = need(m, "v1.zeros", kCh, &zeros))) return rc;
     auto table = [&](const char *name, int n, const int **out) -> int {
@@ -1681,7 +1237,7 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
         if (path) { p.path = path; p.path_fs = p.in_fs; p.ps = ones; p.pb = zeros; }   // the pathway tensor is already >= 0
         // tensor-core version where it is built: no look-ahead, transposed blocks with one time tap only
         const float *w_sw = nullptr;
-        if (tc && la == 0 && !(mode == DW_T2 && bkt != 1) && (r = need(m, (n + ".pw_sw").c_str(), kCh * kCh, &w_sw))) return r;
+        if (la == 0 && !(mode == DW_T2 && bkt != 1) && (r = need(m, (n + ".pw_sw").c_str(), kCh * kCh, &w_sw))) return r;
         if (mode == DW_S1) return run_dwpw<DW_S1>(st, p, B, w_sw);
         if (mode == DW_S2) return run_dwpw<DW_S2>(st, p, B, w_sw);
         return run_dwpw<DW_T2>(st, p, B, w_sw);
@@ -1726,26 +1282,25 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
         if ((rc = gather(s, 2, src, ld, ix, H, 0, f.emb, f.emb_hi, f.emb_lo))) return rc;
     }
     // GroupedGRU: layer l as a dense recurrence, out = sum_l shuffle(y_l) (l < last) + y_last
-    auto ggru = [&](cudaStream_t st, const char *name, int layers, const float *x, unsigned short *x_hi, unsigned short *x_lo, float **y,
+    auto ggru = [&](cudaStream_t st, const char *name, int layers, unsigned short *x_hi, unsigned short *x_lo, float **y,
                     unsigned short **y_hi, unsigned short **y_lo, float *xproj, float *hbase, float *out, unsigned short *out_hi,
                     unsigned short *out_lo) -> int {
-        const float *cur = x;
         unsigned short *ch = x_hi, *cl = x_lo;
         for (int l = 0; l < layers; l++) {
             const std::string nm = std::string(name) + ".g" + std::to_string(l);
             GruChunk ck{hbase ? hbase + (int64_t)l * B * H : nullptr, false, 0, B};
             bool ok = false;
-            int r = run_gru(m, st, nm.c_str(), 1, H, cur, H, nullptr, y[l], xproj, nullptr, B, T, ch, cl, f.scr_hi, f.scr_lo, 0, y_hi[l], y_lo[l], &ok,
+            int r = run_gru(m, st, nm.c_str(), 1, H, H, nullptr, y[l], xproj, nullptr, B, T, ch, cl, f.scr_hi, f.scr_lo, 0, y_hi[l], y_lo[l], &ok,
                             hbase ? &ck : nullptr);
             if (r) return r;
-            cur = y[l]; ch = y_hi[l]; cl = y_lo[l];
+            ch = y_hi[l]; cl = y_lo[l];
         }
         const float *src[3]; int64_t ld[3]; const int *ix[3];
         for (int l = 0; l < layers; l++) { src[l] = y[l]; ld[l] = H; ix[l] = l == layers - 1 ? idx_id : idx_gshuf; }
         return gather(st, layers, src, ld, ix, H, 0, out, out_hi, out_lo);
     };
     if (c.enc_gru_layers > 3 || c.df_gru_layers > 2) return fail(DFB_ERR_UNSUPPORTED, "DeepFilterNet v1: more GRU layers than built (3 / 2)");
-    if ((rc = ggru(s, "enc.emb_gru", c.enc_gru_layers, f.emb, f.emb_hi, f.emb_lo, f.y, f.y_hi, f.y_lo, f.xproj, cx ? cx->h_enc : nullptr, f.embo,
+    if ((rc = ggru(s, "enc.emb_gru", c.enc_gru_layers, f.emb_hi, f.emb_lo, f.y, f.y_hi, f.y_lo, f.xproj, cx ? cx->h_enc : nullptr, f.embo,
                    f.embo_hi, f.embo_lo)))
         return rc;
     if (d_lsnr) {
@@ -1758,7 +1313,7 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
     DFB_CUDA(cudaStreamWaitEvent(sa, L.ev_fork, 0));
     // ---- DF decoder, deepfilternet.py:219-229 (auxiliary stream)
     {
-        if ((rc = ggru(sa, "df_dec.df_gru", c.df_gru_layers, f.embo, f.embo_hi, f.embo_lo, f.z, f.z_hi, f.z_lo, f.xproj2, cx ? cx->h_df : nullptr, f.dfc,
+        if ((rc = ggru(sa, "df_dec.df_gru", c.df_gru_layers, f.embo_hi, f.embo_lo, f.z, f.z_hi, f.z_lo, f.xproj2, cx ? cx->h_df : nullptr, f.dfc,
                        f.dfc_hi, f.dfc_lo)))
             return rc;
         if (d_alpha) {
@@ -1770,7 +1325,7 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
         const int N = Fd * O2;
         if ((rc = need(m, "df_dec.df_fc_out.w_t", (int64_t)H * N, &w_t)) || (rc = need(m, "df_dec.df_fc_out.b", N, &bb))) return rc;
         rc = DFB_ERR_UNSUPPORTED;
-        if (m->proj_tc && m->get("df_dec.df_fc_out.w_hi")) {
+        if (m->get("df_dec.df_fc_out.w_hi")) {
             if ((rc = need(m, "df_dec.df_fc_out.w_hi", (int64_t)H * N / 2, &w_hi)) || (rc = need(m, "df_dec.df_fc_out.w_lo", (int64_t)H * N / 2, &w_lo))) return rc;
             rc = launch_gemm_bf16x3(sa, f.dfc_hi, f.dfc_lo, H, w_hi, w_lo, bb, d_coefs, N, M, N, H);
         }

@@ -369,8 +369,8 @@ template int launch_dwpw_tc<DW_T2>(cudaStream_t, DwPwParams, const float *, int)
 
 // ---------------------------------------------------------- DF pathway conv on tensor cores ----
 // coefs[b,t,f,:] = relu( pw( conv_t(c0) ) + b )  (df_convp, deepfilternet3.py:293-295: grouped (2) temporal conv 64 -> 10
-// with kernel (5,1), 1x1 conv 10 x 10, BN, ReLU).  The FFMA kernel (k_df_convp, dfb_model.cu) is instruction-issue bound
-// (~250 warp instructions per frame and bin pair).  Here the channel contraction runs on the tensor pipe:
+// with kernel (5,1), 1x1 conv 10 x 10, BN, ReLU).  On FFMA this conv is instruction-issue bound (~250 warp instructions
+// per frame and bin pair), so the channel contraction runs on the tensor pipe:
 //   Y[t, g*32 + dt*5 + o] = sum_{c in group g} w1[dt][g*5+o][c] * c0[t, f, c]        (one [128 t x 64 c] x [64 c x 64] product)
 //   z[t, g*5 + o]         = sum_dt Y[t - 4 + dt, g*32 + dt*5 + o]                     (shifted adds out of shared memory)
 //   coefs[t, f, :]        = relu(z . w2 + b)

@@ -108,22 +108,7 @@ class DfNet(nn.Module):
                                           widths.ctypes.data_as(C.POINTER(C.c_int64))))
         self._h = h
         self._derived = derived
-        self.set_precision(os.environ.get("DFB_PRECISION", "fp32+gru_tc+proj_tc+conv_tc"))
         check(_lib.lib().dfb_model_set_options(self._h, int(self.post_filter), self.post_filter_beta, int(not self.run_df)))
-
-    def set_precision(self, mode: str) -> None:
-        """Arithmetic of the contractions (everything else is always IEEE fp32):
-          'fp32'         FFMA everywhere
-          'fp32+gru_tc'  the GRU recurrence of H = 256 models on the tensor cores (mma.sync) with BF16 hi/lo split
-                         operands (3 MMAs per product, fp32 accumulate: ~2^-17 relative, 5e-8 RMS end to end)
-          'fp32+gru_tc+proj_tc'  plus the GRU input projections on the BF16x3 tensor-core GEMM
-          'fp32+gru_tc+proj_tc+conv_tc'  (default) plus the 1x1 convs of the separable conv blocks (k_dwpw_bx) and
-                         the grouped linears (k_gl_bx) on BF16x3 tensor-core kernels (1e-7 .. 4e-7 RMS end to end)."""
-        modes = {"fp32": 0, "fp32+gru_tc": 2, "fp32+gru_tc+proj_tc": 6, "fp32+gru_tc+proj_tc+conv_tc": 14}
-        if mode not in modes:
-            raise ValueError(f"unknown precision mode {mode!r}; one of {sorted(modes)}")
-        check(_lib.lib().dfb_model_set_precision(self._h, modes[mode]))
-        self.precision = mode
 
     def __del__(self):
         h = getattr(self, "_h", None)

@@ -12,18 +12,19 @@ Packed tensors (name -> layout):
   <blk>.dw          [kt][3][C]        depthwise taps of erb_conv1-3, df_conv1, convt3 (conv) and
                                       convt2, convt1 (ConvTranspose2d taps as stored, kt = 1)
   <blk>.pw          [C_in][C_out]     1x1 conv, transposed, BN folded
+  <blk>.pw_sw                         BF16 hi | lo image of the same 1x1 weight for the tensor-core kernel (umma_sw128_image)
   <blk>.b           [C]
   enc.df_conv0.w    [kt][3][2][C]     grouped 2->C conv composed with its 1x1 conv and BN (direct K = 18 conv)
-  enc.df_conv0.dw   [kt][3][C]        (unfused form, kept for reference) 2->C grouped conv taps
-  enc.df_conv0.pw/.b
+  enc.df_conv0.b    [C]
   erb_dec.conv{3,2,1,0}p.s / .b  [C]  depthwise 1x1 + BN folded: relu(x * s + b)
   erb_dec.conv0_out.w [kt][3][C]      C->1 conv, BN folded;  erb_dec.conv0_out.b [1]
-  df_dec.df_convp.w1 [kt5][10][C/2]   grouped (2) temporal conv: out o reads channels (o // 5) * C/2 + c
+  df_dec.df_convp.w_sw                BF16 hi | lo image of the grouped (2) temporal conv as one 64 x 64 product
+                                      (row g*32 + dt*5 + o, column = channel; zero outside group g)
   df_dec.df_convp.w2 [10][10]         1x1 (in, out), BN folded;  df_dec.df_convp.b [10]
   *.gl              [G][I/G][H/G]     GroupedLinearEinsum weight as stored (modules.py:752-757)
   *.gl_bx           BF16 hi | lo image of the same weight in the tensor-core kernel's operand layout (gl_bx_image)
-  <gru>.l{n}.w_ih_t [I][3H] (transposed for the projection GEMM), .w_hh [3H][H], .b_ih [3H],
-                    .b_hh [3H]        torch.nn.GRU gate order (r,z,n)
+  <gru>.l{n}.w_ih_t [I][3H] (transposed), .w_ih_hi / .w_ih_lo ([3H][I] BF16 planes for the projection GEMM),
+                    .w_hh [3H][H], .b_ih [3H], .b_hh [3H]   torch.nn.GRU gate order (r,z,n)
   enc.lsnr.w [emb_out], enc.lsnr.b [1]
 """
 from __future__ import annotations
@@ -135,8 +136,8 @@ def pack_state_dict(sd: Dict[str, torch.Tensor], cfg: ModelConfig) -> Tuple[Dict
         s, b = _bn_fold(sd, f"{prefix}.{bns[0]}")
         out[prefix + ".dw"] = f32(dw[:, 0].transpose(1, 2, 0))
         out[prefix + ".pw"] = f32((pw * s[:, None]).T)
-        out[prefix + ".pw_nk"] = f32(pw * s[:, None])  # [C_out][C_in]: B operand of the tensor-core kernel
-        out[prefix + ".pw_sw"] = umma_sw128_image(out[prefix + ".pw_nk"])  # BF16x3 tensor-core path
+        pw_nk = f32(pw * s[:, None])  # [C_out][C_in]: B operand of the tensor-core kernel
+        out[prefix + ".pw_sw"] = umma_sw128_image(pw_nk)  # BF16x3 tensor-core path
         out[prefix + ".b"] = f32(b)
         return dw.shape[2]
 
@@ -157,9 +158,6 @@ def pack_state_dict(sd: Dict[str, torch.Tensor], cfg: ModelConfig) -> Tuple[Dict
     pws = pw * s[:, None]                                 # [n][c], BN folded
     weff = np.stack([np.einsum("ctf,nc->tfn", dw[ri * g:(ri + 1) * g, 0], pws[:, ri * g:(ri + 1) * g]) for ri in range(2)], axis=2)
     out["enc.df_conv0.w"] = f32(weff)                     # [kt][3][2][C]
-    out["enc.df_conv0.dw"] = f32(dw[:, 0].transpose(1, 2, 0))
-    out["enc.df_conv0.pw"] = f32((pw * s[:, None]).T)
-    out["enc.df_conv0.pw_nk"] = f32(pw * s[:, None])
     out["enc.df_conv0.b"] = f32(b)
     # --- decoder pathway convs (depthwise 1x1 + BN + ReLU)
     for n in (3, 2, 1, 0):
@@ -182,7 +180,6 @@ def pack_state_dict(sd: Dict[str, torch.Tensor], cfg: ModelConfig) -> Tuple[Dict
     w2 = _np(sd[f"df_dec.df_convp.{convs[1]}.weight"]).astype(np.float64)[:, :, 0, 0]  # [out,in]
     s, b = _bn_fold(sd, f"df_dec.df_convp.{bns[0]}")
     assert w1.shape[0] == 2 * cfg.df_order and w1.shape[1] == C // 2
-    out["df_dec.df_convp.w1"] = f32(w1[:, :, :, 0].transpose(2, 0, 1))
     # tensor-core form (k_df_convp_tc): W2[n = g*32 + dt*O + o][k = channel] = w1[g*O + o][k - 32 g][dt] inside group g, else 0
     O, ktp = cfg.df_order, w1.shape[2]
     if C == 64 and ktp * O <= 32:
@@ -220,7 +217,6 @@ def pack_state_dict(sd: Dict[str, torch.Tensor], cfg: ModelConfig) -> Tuple[Dict
         n = gru_layers(sd, src)
         for l in range(n):
             out[f"{dst}.l{l}.w_ih_t"] = f32(_np(sd[f"{src}.weight_ih_l{l}"]).T)
-            out[f"{dst}.l{l}.w_ih"] = f32(_np(sd[f"{src}.weight_ih_l{l}"]))  # [3H][I]: B operand of the tensor-core GEMM
             hi, lo = bf16_planes(_np(sd[f"{src}.weight_ih_l{l}"]))              # [3H][I] BF16 hi / lo, two per float
             out[f"{dst}.l{l}.w_ih_hi"], out[f"{dst}.l{l}.w_ih_lo"] = hi, lo
             out[f"{dst}.l{l}.w_hh"] = f32(_np(sd[f"{src}.weight_hh_l{l}"]))
@@ -313,8 +309,7 @@ def pack_state_dict_v1(sd: Dict[str, torch.Tensor], cfg: ModelConfig) -> Tuple[D
         s, b = bn(p)
         out[p + ".dw"] = f32(taps)
         out[p + ".pw"] = f32((pw * s[:, None]).T)
-        out[p + ".pw_nk"] = f32(pw * s[:, None])
-        out[p + ".pw_sw"] = umma_sw128_image(out[p + ".pw_nk"])
+        out[p + ".pw_sw"] = umma_sw128_image(f32(pw * s[:, None]))
         out[p + ".b"] = f32(b)
         return dw.shape[2]
 
@@ -406,7 +401,6 @@ def pack_state_dict_v1(sd: Dict[str, torch.Tensor], cfg: ModelConfig) -> Tuple[D
                 w_ih = wp
             base = f"{dst}.g{l}.l0"
             out[base + ".w_ih_t"] = f32(w_ih.T)
-            out[base + ".w_ih"] = f32(w_ih)
             out[base + ".w_ih_hi"], out[base + ".w_ih_lo"] = bf16_planes(f32(w_ih))
             out[base + ".w_hh"] = f32(w_hh)
             out[base + ".b_ih"] = f32(b_ih)

@@ -229,13 +229,6 @@ int dfb_stream_flush(dfb_stream *s, float *d_out, void *stream);
 /* host pointers, synchronous; h_in == NULL flushes into h_out f32[B][latency * hop] */
 int dfb_stream_process_host(dfb_stream *s, const float *h_in, int64_t n_frames, float *h_out);
 
-/* Arithmetic of the dense contractions -- a bit mask; everything that is not a contraction is always IEEE fp32:
- *   bit 1 (2): GRU recurrence W_hh h on the tensor cores (mma.sync) with BF16 hi/lo split operands (3 MMAs per product, fp32 accumulate)
- *   bit 2 (4): GRU input projections W_ih x on the BF16x3 tensor-core GEMM
- *   bit 3 (8): 1x1 convs of the separable conv blocks and the grouped linears on the BF16x3 tensor-core kernels
- * 0 = FFMA everywhere; 14 = the default of the Python mirror (deepfilternet_b200/model.py set_precision).
- * BF16x3 is ~2^-17 relative per product: 1e-7 .. 4e-7 RMS end to end against the fp32 oracle (bound 1e-4). */
-int dfb_model_set_precision(dfb_model *m, int mode);
 /* Chunk pipeline of dfb_enhance (device_chunks) / dfb_enhance_host (host_chunks): a signal of >= 64 * chunks frames is cut
  * into at least that many time chunks; lanes = 2 overlaps the encoder phase of chunk c + 1 with the decoder phase (the
  * recurrences) of chunk c on a second set of streams and a second workspace, lanes = 1 runs them back to back.

@@ -27,19 +27,9 @@ enhance_device(model, st, audio); torch.cuda.synchronize()
 buf = np.zeros((T, 8), dtype=np.int64)
 L.dfb_debug_gru_timing(model.handle, T, buf.ctypes.data)
 d = buf[20:T - 20]
-if "gru_tc" in os.environ.get("DFB_PRECISION", "fp32+gru_tc+proj_tc+conv_tc"):
-    step = np.diff(d[:, 0])
-    print(f"TC GRU B={B}  cycles/step median {np.median(step):.0f}")
-    # k_gru_tc stamps: 0 step start, 1 state arrived, 2 MMAs + partial sums done, 3 gates + slice written, 4 slice sent
-    for a, b_, n in [(0, 1, "wait for h"), (1, 2, "W_hh h (mma.sync)"), (2, 3, "gates + own slice"), (3, 4, "barrier + send")]:
-        seg = d[:, b_] - d[:, a]
-        print(f"  {n:22s} median {np.median(seg):7.0f}  max {seg.max():7.0f}")
-    sys.exit(0)
-names = ["wait h", "matvec", "reduce+store", "cta barrier", "gates+send", "loop tail"]
 step = np.diff(d[:, 0])
-print(f"B={B}  cycles/step median {np.median(step):.0f}  mean {step.mean():.0f}")
-for i, n in enumerate(names[:5]):
-    seg = d[:, i + 1] - d[:, i]
-    print(f"  {n:14s} median {np.median(seg):7.0f}  mean {seg.mean():7.0f}  max {seg.max():7.0f}")
-seg = d[1:, 0] - d[:-1, 5]
-print(f"  {'loop tail':14s} median {np.median(seg):7.0f}")
+print(f"TC GRU B={B}  cycles/step median {np.median(step):.0f}")
+# k_gru_tc stamps: 0 step start, 1 state arrived, 2 MMAs + partial sums done, 3 gates + slice written, 4 slice sent
+for a, b_, n in [(0, 1, "wait for h"), (1, 2, "W_hh h (mma.sync)"), (2, 3, "gates + own slice"), (3, 4, "barrier + send")]:
+    seg = d[:, b_] - d[:, a]
+    print(f"  {n:22s} median {np.median(seg):7.0f}  max {seg.max():7.0f}")
