@@ -86,6 +86,8 @@ SIGNATURES = {
     "dfb_enhance_out_len": (_I64, [_VP, _I64, _I]),
     "dfb_enhance_ragged": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP]),
     "dfb_enhance_ragged_host": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP]),
+    "dfb_enhance_ragged_linked": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I, _VP]),
+    "dfb_enhance_ragged_linked_host": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I]),
     "dfb_model_workspace_bytes": (_I64, [_VP]),
     "dfb_stream_create": (_I, [C.POINTER(_VP), _VP, _VP, _I64, _F]),
     "dfb_stream_free": (None, [_VP]),
@@ -93,6 +95,7 @@ SIGNATURES = {
     "dfb_stream_frame_length": (_I64, [_VP]),
     "dfb_stream_latency_frames": (_I64, [_VP]),
     "dfb_stream_set_lsnr_thresholds": (_I, [_VP, _I, _F, _F, _F]),
+    "dfb_stream_set_mask_reduce": (_I, [_VP, _I, _I]),
     "dfb_stream_process": (_I, [_VP, _VP, _I64, _VP, _VP]),
     "dfb_stream_flush": (_I, [_VP, _VP, _VP]),
     "dfb_stream_process_host": (_I, [_VP, _VP, _I64, _VP]),

@@ -125,6 +125,12 @@ struct DspTables {
 // common length.
 struct RaggedRow { int64_t in_off, len, out_off, out_len, Tf; };
 
+// Link group of one stream (linked channels, dfb_enhance_ragged_linked / dfb_stream_set_mask_reduce): the n streams
+// first .. first + n - 1 of the kernel's batch, which include this one, are the channels of one recording and share one
+// ERB mask.  A separate table rather than more RaggedRow fields: the analysis and input-conv kernels read RaggedRow.
+struct LinkRow { int first, n; };
+enum { kReduceNone = 0, kReduceMax = 1, kReduceMean = 2 };   // dfb_reduce_mask
+
 // Parameters of the fused apply + synthesis kernel (dfb_dsp.cu).
 // mode 0: plain ISTFT; 1: DeepFilterNet3 (DF on the noisy spectrum); 2: DeepFilterNet2 (DF on the
 // masked spectrum).
@@ -167,6 +173,12 @@ struct ApplyParams {
     const RaggedRow *rows;
     int64_t w0;
     int t_emit;
+    // linked channels (or null, specialised kernel only): stream b applies the mask of its link group links[b] reduced
+    // over the group's streams (reduce: kReduceMax or kReduceMean, tract.rs:868-902) wherever it applies m, and LSNR
+    // gating reads the LSNR of the group's first stream.  Everything else -- deep filter, DeepFilterNet3's post filter,
+    // the attenuation limit, the ISTFT -- stays per stream.
+    const LinkRow *links;
+    int reduce;
 };
 
 }  // namespace dfb

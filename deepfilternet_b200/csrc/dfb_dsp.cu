@@ -671,7 +671,10 @@ __global__ void __launch_bounds__(32 * kSynWarps) k_apply_synthesis_generic(Appl
 // a frame are issued up front, coalesced (256-byte rows), before any use.
 // RG: batch path (p.rows), a separate instantiation so that the table-free kernel of the streaming API, dfb_apply and
 // dfb_model_forward_full compiles exactly as without it.
-template <int ORDER, int NDFJ, int MINB, bool RG>
+// LINK: linked channels (p.links), likewise separate.  The mask of a frame is reduced over the link group where it is
+// loaded: lane e reads row e of each member's mask and reduces in registers, so the shared mask never reaches HBM and
+// the unlinked instantiations are untouched.
+template <int ORDER, int NDFJ, int MINB, bool RG, bool LINK = false>
 __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyParams p, DspTables tb) {
     __shared__ __align__(16) float s_win[kFft];
     __shared__ __align__(16) float2 s_tw960[241];
@@ -701,6 +704,26 @@ __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyP
     const float2 *srow0 = p.spec + (int64_t)b * (p.spec_T ? p.spec_T : Tf) * kF;
     const int mcT = p.mc_T ? p.mc_T : Tf;                  // m / coefs rows per stream
     const float *mrow0 = p.m + (int64_t)b * mcT * 32;
+    int lb = b;                                            // stream whose LSNR gates this one: the link group's first
+    if constexpr (LINK) lb = p.links[b].first;
+    // ERB gain of band `lane` in frame tt: this stream's own, or (LINK) the link group's max / mean in channel order,
+    // the mean as the fp32 sum times fl32(1 / n) (tract.rs:881-898)
+    auto mask_at = [&](int tt) -> float {
+        if constexpr (!LINK) {
+            return mrow0[(int64_t)tt * 32 + lane];
+        } else {
+            const int n = p.links[b].n;
+            const int64_t stride = (int64_t)mcT * 32;
+            const float *q = p.m + (int64_t)lb * stride + (int64_t)tt * 32 + lane;
+            float v = q[0];
+            if (p.reduce == kReduceMax) {
+                for (int c = 1; c < n; c++) v = fmaxf(v, q[c * stride]);
+                return v;
+            }
+            for (int c = 1; c < n; c++) v += q[c * stride];
+            return v * __frcp_rn((float)n);
+        }
+    };
     const bool masked_df = p.mode == 2 && !p.mask_only;
     const bool pf1 = p.pf && p.mode == 1, pf2 = p.pf && p.mode == 2;
     const bool blend = p.alpha != nullptr && masked_df;   // DeepFilterNet v1: alpha blend with the masked bin
@@ -726,7 +749,7 @@ __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyP
         const bool ok = tt >= 0 && tt < Tv;
         // (DFN2) the mask of a look-ahead frame beyond the window's DNN frames does not exist yet: such rows are only
         // read for frames that are re-synthesised in the next window
-        float mrow = (ok && masked_df && tt < mcT) ? mrow0[(int64_t)tt * 32 + lane] : 1.f;
+        float mrow = (ok && masked_df && tt < mcT) ? mask_at(tt) : 1.f;
         if (pf2 && ok && masked_df && tt < mcT) mrow = pf_gain_mask(mrow, 0.02f);
 #pragma unroll
         for (int j = 0; j < NDFJ; j++) {
@@ -741,12 +764,12 @@ __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyP
     for (int o = 1; o < ORDER; o++) load_df_row(tstart + o - 1 - back, hist[o]);  // becomes taps 0..O-2 after the first shift
     for (int t = tstart; t < t1; t++) {
         // ---- loads of this frame, all issued before use
-        float mcur = mrow0[(int64_t)t * 32 + lane];
+        float mcur = mask_at(t);
         if (pf2) mcur = pf_gain_mask(mcur, 0.02f);
         const float al = blend ? p.alpha[(int64_t)b * mcT + t] : 1.f;
         int stage = 3;   // 0 zero gains, 1 unprocessed, 2 gains only, 3 gains + deep filter (tract.rs apply_stages)
         if (p.lsnr) {
-            const float l = p.lsnr[(int64_t)b * mcT + t];
+            const float l = p.lsnr[(int64_t)lb * mcT + t];
             stage = l < p.th_min ? 0 : (l > p.th_erb ? 1 : (l > p.th_df ? 2 : 3));
         }
 #pragma unroll
@@ -1098,10 +1121,16 @@ int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaS
     dim3 grid((unsigned)((p.Tf + per_cta - 1) / per_cta), (unsigned)B);
     if (p.lsnr && !(p.mode == 1 && p.order == 5 && p.nb_df == 96 && st->tb.E == 32 && p.m && p.coefs))
         return fail(DFB_ERR_UNSUPPORTED, "LSNR stage gating is built for the DeepFilterNet3 apply kernel only");
+    const bool special = p.mode != 0 && p.order == 5 && p.nb_df == 96 && st->tb.E == 32 && p.m && p.coefs;
+    if (p.links && !special) return fail(DFB_ERR_UNSUPPORTED, "linked channels are built for the specialised apply kernel only");
+    if (p.links && p.reduce != kReduceMax && p.reduce != kReduceMean) return fail(DFB_ERR_INVALID, "bad mask reduction %d", p.reduce);
     DFB_PROF("k_apply_synthesis", s);
     // MINB 2: 2 CTAs/SM without spills measured fastest
-    const bool special = p.mode != 0 && p.order == 5 && p.nb_df == 96 && st->tb.E == 32 && p.m && p.coefs;
-    if (special && p.rows)
+    if (p.links && p.rows)
+        k_apply_synthesis<5, 3, 2, true, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
+    else if (p.links)
+        k_apply_synthesis<5, 3, 2, false, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
+    else if (special && p.rows)
         k_apply_synthesis<5, 3, 2, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
     else if (special)
         k_apply_synthesis<5, 3, 2, false><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);

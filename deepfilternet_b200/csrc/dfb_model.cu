@@ -22,6 +22,7 @@
 #include <cstring>
 #include <functional>
 #include <map>
+#include <numeric>
 #include <string>
 
 #include "dfb_common.cuh"
@@ -1567,6 +1568,9 @@ struct ChunkIO {
     // and how many of them still have frames in this chunk (a prefix); null / 0 (streaming API): all S.B streams alike
     const RaggedRow *rows = nullptr;
     int nb = 0;
+    // linked channels: each stream's link group (device table in kernel batch order) and the mask reduction, or null / 0
+    const LinkRow *links = nullptr;
+    int reduce = 0;
 };
 
 // One chunk: analyse frames [S.a1, a1n), run the DNN over [S.d1, d1n), emit audio of frames [S.e1, e1n).
@@ -1654,6 +1658,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
         apply_options(m, p);
         if (ll) { p.lsnr = ll; p.th_min = io.lsnr_th[0]; p.th_erb = io.lsnr_th[1]; p.th_df = io.lsnr_th[2]; }
         if (io.rows) { p.rows = io.rows; p.w0 = W0; p.t_emit = p.Tf; p.Tf = Tw; }   // the grid covers every stream's end
+        if (io.links) { p.links = io.links; p.reduce = io.reduce; }
         if ((rc = launch_apply_synthesis(st, p, B, s))) return rc;
     }
     // ---- carry
@@ -1704,7 +1709,8 @@ struct ChunkHooks {
 // Runs the chunk loop over one stream group: `rows` is its device table and `tfs` its streams' frame counts on the host,
 // longest first.  The analysis reads stream b from d_x + rows[b].in_off, apply + synthesis writes it to d_out + rows[b].out_off.
 static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, float *d_out, const RaggedRow *rows, const int64_t *tfs,
-                         int64_t nb, int pad, float lim, int tc, bool pipelined, cudaStream_t s, const ChunkHooks *hooks) {
+                         int64_t nb, int pad, float lim, int tc, bool pipelined, cudaStream_t s, const ChunkHooks *hooks,
+                         const LinkRow *links, int reduce) {
     const dfb_model_config &c = m->cfg;
     const ChunkGeom g = chunk_geom(c);
     const int hop = st->hop, fft = st->fft;
@@ -1742,10 +1748,10 @@ static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, float *d
         const int lane = pipelined ? (chunk & 1) : 0;
         cudaStream_t cs = pipelined ? m->lanes[lane].main : s;
         int64_t na = nb;   // streams with frames left: a prefix, since the table is sorted longest first
-        while (na > 1 && tfs[na - 1] <= S.d1) na--;
+        while (na > 1 && tfs[na - 1] <= S.d1) na--;    // (the members of a link group share Tf: they leave together)
         if (hooks && S.a1 < a1n && (rc = hooks->before(S.a1 * hop, a1n * hop, na, cs))) break;
         const int64_t e0 = S.e1;
-        ChunkIO io{d_x, Tf * hop, Tf * hop, 0, nullptr, d_out, 0, 0, delay, lim, nullptr, rows, (int)na};
+        ChunkIO io{d_x, Tf * hop, Tf * hop, 0, nullptr, d_out, 0, 0, delay, lim, nullptr, rows, (int)na, links, reduce};
         if ((rc = run_chunk(m, st, S, io, a1n, d1n, e1n > S.e1 ? e1n : S.e1, cs, lane, pipelined))) break;
         if (hooks && (rc = hooks->after(e0 * hop > delay ? e0 * hop - delay : 0, S.e1 * hop - delay, d1n, na, cs))) break;
         last_lane = lane;
@@ -1762,8 +1768,9 @@ static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, float *d
 
 // enhance(): df/enhance.py:206-250.  Time chunks (above) inside stream groups: a group is as many streams as fit the
 // workspace cap with a reasonable chunk; streams are independent (per-channel state reset, pyDF/src/lib.rs:56-58).
-static int enhance_plan(dfb_model *m, dfb_state *st, int64_t B, int64_t Tf, int min_chunks, int64_t *group_out, int *tc_out,
-                        bool *pipelined_out) {
+// A stream group never splits a link group: it takes at least `min_group` streams (the largest link group), else DFB_ERR_OOM.
+static int enhance_plan(dfb_model *m, dfb_state *st, int64_t B, int64_t Tf, int min_chunks, int64_t min_group, int64_t *group_out,
+                        int *tc_out, bool *pipelined_out) {
     // two lanes (DFB_LANES=1 turns the chunk pipeline off): each lane's arena may take half of the workspace cap
     static const bool serial = getenv("DFB_SERIAL") && atoi(getenv("DFB_SERIAL"));
     const bool pipelined = m->n_lanes == 2 && !serial && min_chunks > 1 && Tf >= (int64_t)min_chunks * 64;
@@ -1772,7 +1779,10 @@ static int enhance_plan(dfb_model *m, dfb_state *st, int64_t B, int64_t Tf, int 
     int tc = 0;
     while ((tc = pick_chunk(m, st, group, Tf, min_chunks, cap)) == 0) {
         if (group == 1) return fail(DFB_ERR_OOM, "workspace cap of %zu bytes is too small for a single stream", m->max_workspace);
-        group = (group + 1) / 2;
+        if (group <= min_group)
+            return fail(DFB_ERR_OOM, "workspace cap of %zu bytes is too small for a link group of %lld channels", m->max_workspace,
+                        (long long)min_group);
+        group = std::max((group + 1) / 2, min_group);
     }
     *group_out = group; *tc_out = tc; *pipelined_out = pipelined && tc < Tf;
     const ChunkGeom g = chunk_geom(m->cfg);
@@ -1841,14 +1851,68 @@ static int copy_streams(float *dst, const float *src, int64_t x0, int64_t n, At 
     return DFB_OK;
 }
 
+// Validates the link groups of a linked call: group g is the next group_sizes[g] streams in the caller's order, all of one
+// length.  Returns each stream's group {first stream, size} in the caller's order, or an empty table when nothing is linked
+// (reduce none, or every group a single stream): such a call is the unlinked one.
+static int link_plan(const dfb_model *m, const std::vector<RaggedRow> &rows, const int64_t *group_sizes, int64_t n_groups,
+                     int reduce, std::vector<LinkRow> &links) {
+    if (reduce != kReduceNone && reduce != kReduceMax && reduce != kReduceMean)
+        return fail(DFB_ERR_INVALID, "reduce_mask %d is not 0 (none), 1 (max) or 2 (mean)", reduce);
+    if (!group_sizes || n_groups <= 0) return fail(DFB_ERR_INVALID, "no link groups");
+    const int64_t B = (int64_t)rows.size();
+    links.assign((size_t)B, LinkRow{0, 1});
+    int64_t b = 0, n_max = 0;
+    for (int64_t g = 0; g < n_groups; g++) {
+        const int64_t n = group_sizes[g];
+        if (n <= 0 || n > B - b) return fail(DFB_ERR_INVALID, "link group sizes do not sum to the %lld streams", (long long)B);
+        if (n > 65535) return fail(DFB_ERR_INVALID, "link group %lld has more than 65535 channels", (long long)g);
+        for (int64_t i = b; i < b + n; i++) {
+            if (rows[(size_t)i].len != rows[(size_t)b].len)
+                return fail(DFB_ERR_INVALID, "link group %lld has channels of different lengths", (long long)g);
+            links[(size_t)i] = LinkRow{(int)b, (int)n};
+        }
+        b += n;
+        n_max = std::max(n_max, n);
+    }
+    if (b != B) return fail(DFB_ERR_INVALID, "link group sizes do not sum to the %lld streams", (long long)B);
+    if (reduce == kReduceNone || n_max == 1) {
+        links.clear();
+        return DFB_OK;
+    }
+    if (m->cfg.model_kind == 1) return fail(DFB_ERR_UNSUPPORTED, "linked channels: DeepFilterNet v1 is not supported");
+    return DFB_OK;
+}
+
 // The batch executor behind every dfb_enhance* entry point; `rows` (the caller's order) is sorted here.  Device buffers: the
 // work is enqueued on `s`.  Host buffers (`host`): each stream group is staged into device buffers that hold its streams
 // packed back to back, chunk by chunk and each stream's range clipped to its length -- the H2D copy of chunk c + 1 and the
 // D2H copy of chunk c - 1 run on their own streams (both copy engines) while chunk c computes -- and the call is synchronous.
+// `links` (or null): each stream's link group from link_plan, sorted here along with `rows`; `reduce` the mask reduction.
 static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &rows, const float *src, float *dst, int pad,
-                        float atten_lim_db, bool host, cudaStream_t s) {
-    std::stable_sort(rows.begin(), rows.end(), [](const RaggedRow &a, const RaggedRow &b) { return a.Tf > b.Tf; });
+                        float atten_lim_db, bool host, cudaStream_t s, std::vector<LinkRow> *links = nullptr, int reduce = 0) {
     const int64_t B = (int64_t)rows.size();
+    int64_t min_group = 1;   // the largest link group: a stream group never splits one
+    if (!links) {
+        std::stable_sort(rows.begin(), rows.end(), [](const RaggedRow &a, const RaggedRow &b) { return a.Tf > b.Tf; });
+    } else {
+        // The members of a link group are consecutive and share their sort key (one length), so the stable sort keeps them
+        // one contiguous run in their own order: nothing between them has that key.  Sorting a permutation carries each
+        // stream's group along, as the new position of the group's first member.
+        std::vector<int64_t> idx((size_t)B);
+        std::iota(idx.begin(), idx.end(), (int64_t)0);
+        std::stable_sort(idx.begin(), idx.end(), [&](int64_t a, int64_t b) { return rows[(size_t)a].Tf > rows[(size_t)b].Tf; });
+        std::vector<RaggedRow> sr((size_t)B);
+        std::vector<LinkRow> sl((size_t)B);
+        for (int64_t i = 0; i < B; i++) {
+            const int64_t o = idx[(size_t)i];
+            const LinkRow g = (*links)[(size_t)o];
+            sr[(size_t)i] = rows[(size_t)o];
+            sl[(size_t)i] = LinkRow{(int)(i - (o - g.first)), g.n};
+            min_group = std::max(min_group, (int64_t)g.n);
+        }
+        rows.swap(sr);
+        links->swap(sl);
+    }
     std::vector<int64_t> tfs((size_t)B);
     int64_t true_frames = 0;
     for (int64_t i = 0; i < B; i++) { tfs[i] = rows[i].Tf; true_frames += tfs[i]; }
@@ -1865,18 +1929,31 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
     int64_t group = 0;
     int tc = 0;
     bool pipelined = false;
-    int rc = enhance_plan(m, st, B, tfs[0], min_chunks, &group, &tc, &pipelined);
+    int rc = enhance_plan(m, st, B, tfs[0], min_chunks, min_group, &group, &tc, &pipelined);
     if (rc) return rc;
-    size_t off[16];   // the aux arena holds one group's state slab and table
-    if ((rc = m->aux_arena.reserve(state_floats(m->cfg, st, (int)group, off) * sizeof(float) + (size_t)group * sizeof(RaggedRow) + 8192)))
+    size_t off[16];   // the aux arena holds one group's state slab and tables
+    if ((rc = m->aux_arena.reserve(state_floats(m->cfg, st, (int)group, off) * sizeof(float) +
+                                   (size_t)group * (sizeof(RaggedRow) + sizeof(LinkRow)) + 8192)))
         return rc;
-    auto group_end = [&](int64_t b0) {   // stream groups: up to `group` streams; DeepFilterNet v1: of one frame count
+    // stream groups: up to `group` streams, cut only between link groups (group >= every link group, so a cut inside one
+    // moves back to its first member, past b0); DeepFilterNet v1: of one frame count
+    auto group_end = [&](int64_t b0) {
         int64_t b1 = B - b0 < group ? B : b0 + group;
+        if (links && b1 < B && (*links)[(size_t)b1].first < b1) b1 = (*links)[(size_t)b1].first;
         if (m->cfg.model_kind == 1)
             for (int64_t i = b0 + 1; i < b1; i++)
                 if (tfs[i] != tfs[b0]) { b1 = i; break; }
         return b1;
     };
+    // device link tables: each stream group indexes its own streams from 0
+    std::vector<LinkRow> dlinks;
+    if (links) {
+        dlinks = *links;
+        for (int64_t b0 = 0, b1; b0 < B; b0 = b1) {
+            b1 = group_end(b0);
+            for (int64_t i = b0; i < b1; i++) dlinks[(size_t)i].first -= (int)b0;
+        }
+    }
     // device rows: the streams themselves, or (host) their places in the staging buffers, sized for the largest group
     std::vector<RaggedRow> drows(rows);
     float *d_in = nullptr, *d_out = nullptr;
@@ -1930,8 +2007,14 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
         m->aux_arena.reset();
         RaggedRow *d_rows = m->aux_arena.take<RaggedRow>((size_t)(b1 - b0));
         DFB_CUDA(cudaMemcpyAsync(d_rows, dr, sizeof(RaggedRow) * (b1 - b0), cudaMemcpyHostToDevice, sc));
+        LinkRow *d_links = nullptr;
+        if (links) {
+            d_links = m->aux_arena.take<LinkRow>((size_t)(b1 - b0));
+            if (!d_links) { rc = fail(DFB_ERR_OOM, "link table arena exhausted"); break; }
+            DFB_CUDA(cudaMemcpyAsync(d_links, dlinks.data() + b0, sizeof(LinkRow) * (b1 - b0), cudaMemcpyHostToDevice, sc));
+        }
         rc = enhance_group(m, st, host ? d_in : src, host ? d_out : dst, d_rows, tf, b1 - b0, pad, lim, tc, pipelined, sc,
-                           host ? &hooks : nullptr);
+                           host ? &hooks : nullptr, d_links, links ? reduce : 0);
     }
     if (host) {
         const cudaError_t e1 = cudaStreamSynchronize(sc), e2 = cudaStreamSynchronize(sd), e3 = cudaStreamSynchronize(sh);
@@ -1998,6 +2081,35 @@ extern "C" int dfb_enhance_ragged_host(dfb_model *m, dfb_state *st, const float 
     return enhance_rows(m, st, rows, h_audio, h_out, pad, atten_lim_db, true, nullptr);
 }
 
+extern "C" int dfb_enhance_ragged_linked(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel,
+                                         const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad, float atten_lim_db,
+                                         float *d_out, int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes,
+                                         int64_t n_groups, int reduce_mask, void *stream) {
+    if (!m || !st || !d_audio || !d_out) return fail(DFB_ERR_INVALID, "null argument");
+    if (int rcs = check_state(m, st)) return rcs;
+    std::vector<RaggedRow> rows;
+    std::vector<LinkRow> links;
+    if (int rc = ragged_plan(st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rows)) return rc;
+    if (int rc = link_plan(m, rows, group_sizes, n_groups, reduce_mask, links)) return rc;
+    DFB_CUDA(cudaSetDevice(m->device));
+    return enhance_rows(m, st, rows, d_audio, d_out, pad, atten_lim_db, false, (cudaStream_t)stream, links.empty() ? nullptr : &links,
+                        reduce_mask);
+}
+
+extern "C" int dfb_enhance_ragged_linked_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel,
+                                              const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad,
+                                              float atten_lim_db, float *h_out, int64_t out_numel, const int64_t *out_offsets,
+                                              const int64_t *group_sizes, int64_t n_groups, int reduce_mask) {
+    if (!m || !st || !h_audio || !h_out) return fail(DFB_ERR_INVALID, "null argument");
+    if (int rcs = check_state(m, st)) return rcs;
+    std::vector<RaggedRow> rows;
+    std::vector<LinkRow> links;
+    if (int rc = ragged_plan(st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rows)) return rc;
+    if (int rc = link_plan(m, rows, group_sizes, n_groups, reduce_mask, links)) return rc;
+    DFB_CUDA(cudaSetDevice(m->device));
+    return enhance_rows(m, st, rows, h_audio, h_out, pad, atten_lim_db, true, nullptr, links.empty() ? nullptr : &links, reduce_mask);
+}
+
 // ============================================================== streaming API ====
 // Frame-incremental processing with carried state: the batched counterpart of the reference's single-stream runtime
 // (libDF/src/tract.rs:509-642 `DfTract::process`, C ABI libDF/src/capi.rs:83-253 df_create / df_process_frame / df_free).
@@ -2007,6 +2119,7 @@ extern "C" int dfb_enhance_ragged_host(dfb_model *m, dfb_state *st, const float 
 struct dfb_stream {
     dfb_model *m;
     dfb_state *st;
+    int device;                                        // the model's, kept so that freeing never reads the model
     int B;
     float lim;
     StreamState S;
@@ -2015,6 +2128,9 @@ struct dfb_stream {
     float th[3] = {-10.f, 30.f, 20.f};                 // tract.rs:180-185 defaults
     float *stage_in = nullptr, *stage_out = nullptr;   // device staging of the *_host entry point
     size_t stage_cap = 0;
+    LinkRow *links = nullptr;                          // linked channels (dfb_stream_set_mask_reduce) or null
+    int reduce = 0;
+    bool fed = false;                                  // a frame has been processed since create / reset
 };
 
 extern "C" int dfb_stream_create(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B, float atten_lim_db) {
@@ -2025,7 +2141,7 @@ extern "C" int dfb_stream_create(dfb_stream **out, dfb_model *m, dfb_state *st, 
         return fail(DFB_ERR_UNSUPPORTED, "DeepFilterNet v1 runs as one window per signal (forward_v1): no frame-incremental API");
     DFB_CUDA(cudaSetDevice(m->device));
     dfb_stream *h = new dfb_stream();
-    h->m = m; h->st = st; h->B = (int)B;
+    h->m = m; h->st = st; h->device = m->device; h->B = (int)B;
     h->lim = (atten_lim_db > 0.f) ? powf(10.f, -atten_lim_db / 20.f) : 0.f;
     size_t off[16];
     const size_t n = state_floats(m->cfg, st, (int)B, off);
@@ -2038,10 +2154,11 @@ extern "C" int dfb_stream_create(dfb_stream **out, dfb_model *m, dfb_state *st, 
 
 extern "C" void dfb_stream_free(dfb_stream *h) {
     if (!h) return;
-    cudaSetDevice(h->m->device);
+    cudaSetDevice(h->device);
     if (h->slab) cudaFree(h->slab);
     if (h->stage_in) cudaFree(h->stage_in);
     if (h->stage_out) cudaFree(h->stage_out);
+    if (h->links) cudaFree(h->links);
     delete h;
 }
 
@@ -2050,6 +2167,32 @@ extern "C" int dfb_stream_reset(dfb_stream *h) {
     size_t off[16];
     state_floats(h->m->cfg, h->st, h->B, off);
     state_bind(h->S, h->slab, off, h->B);
+    h->fed = false;
+    return DFB_OK;
+}
+
+// Linked channels on a stream handle: streams g * channels + c (c < channels) are the channels of recording g and share one
+// ERB mask (reduce_mask max / mean, as dfb_enhance_ragged_linked).  Only before the first frame of a new or reset handle:
+// the frame re-synthesised for the overlap-add tail at the next call would otherwise mix the two settings.
+extern "C" int dfb_stream_set_mask_reduce(dfb_stream *h, int channels, int reduce_mask) {
+    if (!h) return fail(DFB_ERR_INVALID, "null stream");
+    if (h->fed) return fail(DFB_ERR_INVALID, "mask reduction set after the first frame: reset the stream first");
+    if (reduce_mask != kReduceNone && reduce_mask != kReduceMax && reduce_mask != kReduceMean)
+        return fail(DFB_ERR_INVALID, "reduce_mask %d is not 0 (none), 1 (max) or 2 (mean)", reduce_mask);
+    if (channels <= 0 || h->B % channels) return fail(DFB_ERR_INVALID, "%d streams are not groups of %d channels", h->B, channels);
+    DFB_CUDA(cudaSetDevice(h->m->device));
+    if (h->links) cudaFree(h->links);
+    h->links = nullptr;
+    h->reduce = 0;
+    if (reduce_mask == kReduceNone || channels == 1) return DFB_OK;
+    std::vector<LinkRow> t((size_t)h->B);
+    for (int b = 0; b < h->B; b++) t[(size_t)b] = LinkRow{b - b % channels, channels};
+    if (cudaMalloc(&h->links, sizeof(LinkRow) * t.size()) != cudaSuccess) {
+        h->links = nullptr;
+        return fail(DFB_ERR_OOM, "link table allocation failed");
+    }
+    DFB_CUDA(cudaMemcpy(h->links, t.data(), sizeof(LinkRow) * t.size(), cudaMemcpyHostToDevice));
+    h->reduce = reduce_mask;
     return DFB_OK;
 }
 
@@ -2093,6 +2236,9 @@ static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, 
     if (f0 < 0 || e1n <= S.e1) DFB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * B * n_out * hop, s));
     ChunkIO io{d_in, (flush ? 0 : n) * hop, (flush ? 0 : n) * hop, a0, S.started ? S.ana_mem : nullptr, d_out, n_out * hop, n_out * hop,
                f0 * hop, h->lim, h->gating ? h->th : nullptr};
+    io.links = h->links;
+    io.reduce = h->reduce;
+    h->fed = true;
     if (!flush && a1n > a0) {
         // zero analysis memory before the very first frame
         if (!S.started) DFB_CUDA(cudaMemsetAsync(S.ana_mem, 0, sizeof(float) * B * hop, s));

@@ -104,10 +104,13 @@ def df_features(audio: Tensor, df: DF, nb_df: int, device=None, alpha: Optional[
 
 @torch.no_grad()
 def enhance(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
-            atten_lim_db: Optional[float] = None, out: Optional[Tensor] = None) -> Tensor:
+            atten_lim_db: Optional[float] = None, out: Optional[Tensor] = None, *, reduce_mask: Optional[str] = None) -> Tensor:
     """enhance.py:206-250: audio f32 CPU [C,T] @ model sr -> enhanced f32 CPU [C,T]
     (or [C, (T // hop) * hop], delayed by n_fft - hop, when ``pad`` is False).
-    ``out`` (extension): optional preallocated (e.g. pinned) CPU tensor for the result."""
+    ``out`` (extension): optional preallocated (e.g. pinned) CPU tensor for the result.
+    ``reduce_mask`` (extension): "max" or "mean" links the C channels as the Rust runtime does (tract.rs:868-902): they
+    share one ERB mask, the max or mean of their own (include/dfb200.h, dfb_enhance_ragged_linked); None / "none": every
+    channel on its own."""
     model.eval()
     if audio.dim() != 2:
         raise ValueError("audio must have shape [C, T]")
@@ -119,8 +122,17 @@ def enhance(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
     elif out.shape != (c, out_len) or out.dtype != torch.float32 or out.is_cuda or not out.is_contiguous():
         raise ValueError(f"out must be a contiguous float32 CPU tensor of shape {(c, out_len)}")
     lim = abs(float(atten_lim_db)) if atten_lim_db is not None else 0.0
-    check(_lib.lib().dfb_enhance_host(model.handle, df_state.handle, x.data_ptr(), c, t, 1 if pad else 0,
-                                      lim, out.data_ptr()))
+    reduce = ragged.reduce_code(reduce_mask)
+    if reduce == 0:
+        check(_lib.lib().dfb_enhance_host(model.handle, df_state.handle, x.data_ptr(), c, t, 1 if pad else 0,
+                                          lim, out.data_ptr()))
+        return out
+    lens = np.full(c, t, dtype=np.int64)
+    in_off, out_off = np.arange(c, dtype=np.int64) * t, np.arange(c, dtype=np.int64) * out_len
+    groups = np.array([c], dtype=np.int64)
+    check(_lib.lib().dfb_enhance_ragged_linked_host(model.handle, df_state.handle, x.data_ptr(), c * t, in_off.ctypes.data,
+                                                    lens.ctypes.data, c, 1 if pad else 0, lim, out.data_ptr(), c * out_len,
+                                                    out_off.ctypes.data, groups.ctypes.data, 1, reduce))
     return out
 
 
@@ -150,12 +162,13 @@ def enhance_device(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
 
 @torch.no_grad()
 def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: bool = True,
-                  atten_lim_db: Optional[float] = None) -> List[Tensor]:
+                  atten_lim_db: Optional[float] = None, reduce_mask: Optional[str] = None) -> List[Tensor]:
     """Several recordings of different lengths in one call: ``audios`` is a sequence of CPU [C_i, T_i] tensors as
     :func:`enhance` takes them, every channel one stream.  Entry i of the result equals
     ``enhance(model, df_state, audios[i], pad, atten_lim_db)``.  The batch is packed into one page-locked buffer and
     enhanced by one ``dfb_enhance_ragged_host`` call, which copies only the streams' own samples and computes only their
-    own frames.  The results are views into one page-locked output buffer."""
+    own frames.  The results are views into one page-locked output buffer.  ``reduce_mask`` "max" / "mean": each entry's
+    channels are linked, as ``enhance(..., reduce_mask=reduce_mask)`` links them."""
     model.eval()
     xs = list(audios)
     for i, a in enumerate(xs):
@@ -167,19 +180,30 @@ def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: boo
     torch.cat([a.detach().to("cpu", torch.float32).reshape(-1) for a in xs], out=x)
     y = torch.empty(n_out, dtype=torch.float32, pin_memory=pin)
     lim = abs(float(atten_lim_db)) if atten_lim_db is not None else 0.0
-    check(_lib.lib().dfb_enhance_ragged_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
-                                             lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
-                                             out_off.ctypes.data))
+    reduce = ragged.reduce_code(reduce_mask)
+    if reduce == 0:
+        check(_lib.lib().dfb_enhance_ragged_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
+                                                 lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
+                                                 out_off.ctypes.data))
+    else:
+        groups = ragged.packed_groups([tuple(a.shape) for a in xs])
+        check(_lib.lib().dfb_enhance_ragged_linked_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
+                                                        lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
+                                                        out_off.ctypes.data, groups.ctypes.data, groups.size, reduce))
     return [y[s:s + c * n].view(c, n) for s, c, n in slices]
 
 
 @torch.no_grad()
 def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pad: bool = True,
-                          atten_lim_db: Optional[float] = None, out: Optional[Tensor] = None) -> Tensor:
+                          atten_lim_db: Optional[float] = None, out: Optional[Tensor] = None, group_sizes=None,
+                          reduce_mask: Optional[str] = None) -> Tensor:
     """Device-resident ragged batch: ``audio`` is a padded CUDA tensor [B, S] whose row b holds ``lengths[b]`` real
     samples.  Returns [B, max out_len] (asynchronous on the current stream): row b equals :func:`enhance_device` of
     ``audio[b, :lengths[b]]`` alone, and is zero beyond its own output length.  With ``out`` given, only each row's own
-    output range is written."""
+    output range is written.
+    ``group_sizes`` / ``reduce_mask`` "max" / "mean": linked channels -- group g is the next ``group_sizes[g]`` rows, of
+    one length, and they share one ERB mask; each group's rows equal :func:`enhance` of that recording with the same
+    ``reduce_mask``."""
     if not audio.is_cuda or audio.dtype != torch.float32 or not audio.is_contiguous() or audio.dim() != 2:
         raise ValueError("enhance_device_ragged expects a contiguous float32 CUDA tensor of shape [B, S]")
     if audio.device != model.cuda_device:
@@ -190,6 +214,10 @@ def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pa
     if lens.size != b:
         raise ValueError(f"{lens.size} lengths for {b} streams")
     lens, in_off, out_off, ow = ragged.padded_layout(lens, s, df_state.hop_size(), pad)
+    reduce = ragged.reduce_code(reduce_mask)
+    if group_sizes is None and reduce != 0:
+        raise ValueError("reduce_mask needs group_sizes: which rows are the channels of one recording")
+    groups = ragged.link_groups(group_sizes, lens) if group_sizes is not None else None
     if out is None:
         out = torch.zeros((b, ow), dtype=torch.float32, device=audio.device)
     elif (out.shape != (b, ow) or out.dtype != torch.float32 or not out.is_cuda or out.device != audio.device
@@ -198,13 +226,23 @@ def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pa
     lim = abs(float(atten_lim_db)) if atten_lim_db is not None else 0.0
     with torch.cuda.device(audio.device):
         stream = torch.cuda.current_stream(audio.device).cuda_stream
-        check(_lib.lib().dfb_enhance_ragged(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
-                                            lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow,
-                                            out_off.ctypes.data, stream))
+        if groups is None:
+            check(_lib.lib().dfb_enhance_ragged(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
+                                                lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow,
+                                                out_off.ctypes.data, stream))
+        else:
+            check(_lib.lib().dfb_enhance_ragged_linked(model.handle, df_state.handle, audio.data_ptr(), b * s,
+                                                       in_off.ctypes.data, lens.ctypes.data, b, 1 if pad else 0, lim,
+                                                       out.data_ptr(), b * ow, out_off.ctypes.data, groups.ctypes.data,
+                                                       groups.size, reduce, stream))
     return out
 
 
 # ------------------------------------------------------------------------------------------ CLI ----
+# --reduce-mask N, numbered as the deep-filter binary's flag (libDF/src/bin/enhance_wav.rs:60-62)
+REDUCE_MASK_CLI = {0: None, 1: "max", 2: "mean"}
+
+
 def parse_epoch_type(value: str) -> Union[int, str]:
     """enhance.py:253-261."""
     try:
@@ -266,10 +304,12 @@ def main(args) -> int:
         if not batch:
             continue
         t0 = time.time()
+        reduce = REDUCE_MASK_CLI[getattr(args, "reduce_mask", 0)]
         if batch_size == 1:
-            outs = [enhance(model, df_state, batch[0][2], pad=args.compensate_delay, atten_lim_db=args.atten_lim)]
+            outs = [enhance(model, df_state, batch[0][2], pad=args.compensate_delay, atten_lim_db=args.atten_lim, reduce_mask=reduce)]
         else:
-            outs = enhance_batch(model, df_state, [a for _, _, a, _ in batch], pad=args.compensate_delay, atten_lim_db=args.atten_lim)
+            outs = enhance_batch(model, df_state, [a for _, _, a, _ in batch], pad=args.compensate_delay, atten_lim_db=args.atten_lim,
+                                 reduce_mask=reduce)
         t_batch = time.time() - t0
         total = sum(a.numel() for _, _, a, _ in batch)
         for (i, file, audio_in, meta), audio in zip(batch, outs):
@@ -283,8 +323,8 @@ def main(args) -> int:
     return 0
 
 
-def run(argv=None) -> int:
-    """enhance.py:342-379."""
+def cli_parser():
+    """The `deepFilter` command's arguments (enhance.py:342-379)."""
     parser = setup_df_argument_parser()
     parser.add_argument("--no-delay-compensation", dest="compensate_delay", action="store_false",
                         help="Don't add some padding to compensate the delay introduced by the real-time STFT/ISTFT implementation.")
@@ -297,7 +337,15 @@ def run(argv=None) -> int:
     parser.add_argument("--no-df-stage", action="store_true")
     parser.add_argument("--batch-size", type=int, default=1,
                         help="Enhance this many files per call (streams of different lengths in one batch); 1: one file per call.")
-    return main(parser.parse_args(argv))
+    parser.add_argument("--reduce-mask", type=int, default=0, choices=sorted(REDUCE_MASK_CLI),
+                        help="Link the channels of a multi-channel file: they share one ERB mask, 1 = the max, 2 = the mean of "
+                             "their masks; 0 = every channel on its own (default).")
+    return parser
+
+
+def run(argv=None) -> int:
+    """enhance.py:342-379."""
+    return main(cli_parser().parse_args(argv))
 
 
 if __name__ == "__main__":

@@ -56,3 +56,42 @@ def packed_layout(shapes: Sequence[Tuple[int, int]], hop: int, pad: bool):
         slices.append((int(out_off[k]), c, int(olens[k])))
         k += c
     return lens, in_off, out_off, int(lens.sum()), int(olens.sum()), slices
+
+
+# Linked channels (dfb_enhance_ragged_linked): the channels of one recording share one ERB mask, reduced over them.
+# Numbering of dfb_reduce_mask and of the Rust runtime's ReduceMask / --reduce-mask (libDF/src/tract.rs:95-99).
+REDUCE_MASK = {"none": 0, "max": 1, "mean": 2}
+
+
+def reduce_code(reduce_mask) -> int:
+    """None, "none", "max" or "mean" -> 0, 0, 1, 2 (ValueError otherwise)."""
+    if reduce_mask is None:
+        return 0
+    if isinstance(reduce_mask, str) and reduce_mask.lower() in REDUCE_MASK:
+        return REDUCE_MASK[reduce_mask.lower()]
+    raise ValueError(f"reduce_mask must be None, 'none', 'max' or 'mean', got {reduce_mask!r}")
+
+
+def link_groups(group_sizes, lengths) -> np.ndarray:
+    """Link groups as consecutive runs of streams: group g is the next ``group_sizes[g]`` streams of ``lengths``.  Returns
+    the sizes as int64; ValueError when a size is < 1, the sizes do not sum to the number of streams, or a group's streams
+    differ in length (the channels of one recording have one length)."""
+    sizes = np.ascontiguousarray(np.asarray(group_sizes, dtype=np.int64).reshape(-1))
+    lens = np.asarray(lengths, dtype=np.int64).reshape(-1)
+    if sizes.size == 0:
+        raise ValueError("no link groups")
+    if (sizes <= 0).any():
+        raise ValueError(f"link group sizes must be >= 1, got {int(sizes.min())}")
+    if int(sizes.sum()) != lens.size:
+        raise ValueError(f"link group sizes sum to {int(sizes.sum())}, the batch has {lens.size} streams")
+    b = 0
+    for g, n in enumerate(sizes.tolist()):
+        if (lens[b:b + n] != lens[b]).any():
+            raise ValueError(f"link group {g} has channels of different lengths: {lens[b:b + n].tolist()}")
+        b += n
+    return sizes
+
+
+def packed_groups(shapes: Sequence[Tuple[int, int]]) -> np.ndarray:
+    """Link groups of a :func:`packed_layout` batch: entry i's C_i channels are one group."""
+    return np.ascontiguousarray(np.array([int(shp[0]) for shp in shapes], dtype=np.int64))

@@ -8,6 +8,9 @@
 
 The concatenation of the outputs equals ``enhance(model, df_state, audio, pad=False)`` delayed by
 ``latency_frames * hop`` samples.  Everything runs in the CUDA library (dfb_stream_* in include/dfb200.h).
+
+``channels`` / ``reduce_mask`` link the channels of each recording as the Rust runtime does: rows g * channels + c are
+the channels of recording g and share one ERB mask, the max or mean of theirs (dfb_stream_set_mask_reduce).
 """
 from __future__ import annotations
 
@@ -17,14 +20,15 @@ from typing import Optional
 import torch
 from torch import Tensor
 
-from . import _lib
+from . import _lib, ragged
 from ._lib import check
 from .libdf import DF
 from .model import DfNet
 
 
 class DfStream:
-    def __init__(self, model: DfNet, df_state: DF, batch: int = 1, atten_lim_db: Optional[float] = None):
+    def __init__(self, model: DfNet, df_state: DF, batch: int = 1, atten_lim_db: Optional[float] = None, channels: int = 1,
+                 reduce_mask: Optional[str] = None):
         self.model, self.df_state, self.batch = model, df_state, int(batch)
         h = C.c_void_p()
         lim = abs(float(atten_lim_db)) if atten_lim_db is not None else 0.0
@@ -32,6 +36,17 @@ class DfStream:
         self._h = h
         self.hop = int(_lib.lib().dfb_stream_frame_length(h))
         self.latency_frames = int(_lib.lib().dfb_stream_latency_frames(h))
+        if channels != 1 or ragged.reduce_code(reduce_mask):
+            try:
+                self.set_mask_reduce(channels, reduce_mask)
+            except Exception:
+                self.__del__()   # a constructor that fails leaves no handle behind
+                raise
+
+    def set_mask_reduce(self, channels: int, reduce_mask: Optional[str]) -> None:
+        """Linked channels: rows g * channels + c form recording g; reduce_mask None / "none", "max" or "mean".  Only on a new
+        or reset stream."""
+        check(_lib.lib().dfb_stream_set_mask_reduce(self._h, int(channels), ragged.reduce_code(reduce_mask)))
 
     def __del__(self):
         h = getattr(self, "_h", None)

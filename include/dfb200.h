@@ -199,6 +199,32 @@ int dfb_enhance_ragged(dfb_model *m, dfb_state *st, const float *d_audio, int64_
 int dfb_enhance_ragged_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel, const int64_t *in_offsets,
                             const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *h_out, int64_t out_numel,
                             const int64_t *out_offsets);
+/* Linked channels: the Rust runtime's mask reduction over the channels of one recording (libDF/src/tract.rs:95-99,
+ * 868-902; the default of its LADSPA plugin and, as --reduce-mask, of its deep-filter binary).  A link group is C >= 1
+ * streams of one length, the channels of one recording.  Everything up to the model outputs stays per channel (STFT,
+ * features and their normalisation, encoder, GRU states, m_c, coefs_c, lsnr_c).  The ERB mask is then shared:
+ *   max:  m[t][e] = max_c m_c[t][e]
+ *   mean: m[t][e] = (sum_c m_c[t][e], fp32 in channel order) * fl32(1 / C)
+ * and every channel's apply stage uses it wherever it uses its own mask: the ERB gains (bins >= nb_df, or all bins with
+ * mask_only), DeepFilterNet2's masked spectrum that feeds its deep filter, and DeepFilterNet2's post filter on the gains.
+ * The deep-filter coefficients, DeepFilterNet3's post filter, the attenuation limit and the ISTFT stay per channel.
+ * LSNR stage gating (streaming, DeepFilterNet3) makes one decision per group and frame, from the LSNR of the group's
+ * FIRST channel: this library's reading of the single scalar the Rust runtime takes from its [ch] LSNR output.
+ * With DFB_REDUCE_NONE, or groups of one stream, the result is the unlinked one.
+ * DeepFilterNet3, DeepFilterNet3_ll and DeepFilterNet2; DeepFilterNet v1 with a group of C > 1 is DFB_ERR_UNSUPPORTED. */
+typedef enum { DFB_REDUCE_NONE = 0, DFB_REDUCE_MAX = 1, DFB_REDUCE_MEAN = 2 } dfb_reduce_mask;  /* tract.rs:95-99 */
+/* dfb_enhance_ragged(_host) with link groups: group g is the next group_sizes[g] streams in the caller's order
+ * (group_sizes is a HOST array of n_groups entries summing to B; DFB_ERR_INVALID otherwise, or when a group's streams differ
+ * in length).  A group is never split across stream groups: DFB_ERR_OOM when the workspace cap (dfb_model_set_max_workspace)
+ * cannot hold the largest one. */
+int dfb_enhance_ragged_linked(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
+                              const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
+                              const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
+                              void *stream);
+int dfb_enhance_ragged_linked_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel,
+                                   const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad, float atten_lim_db,
+                                   float *h_out, int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes,
+                                   int64_t n_groups, int reduce_mask);
 /* ------------------------------------------------------------------ streaming -----------------
  * Frame-incremental processing with carried per-stream state: the batched counterpart of the reference's
  * single-stream runtime `DfTract::process` (libDF/src/tract.rs:509-642) and its C ABI (libDF/src/capi.rs:83-253:
@@ -222,6 +248,10 @@ int64_t dfb_stream_latency_frames(const dfb_stream *s);    /* hops the output tr
  * DeepFilterNet3 topologies only. */
 int dfb_stream_set_lsnr_thresholds(dfb_stream *s, int enable, float min_db_thresh, float max_db_erb_thresh,
                                    float max_db_df_thresh);
+/* Linked channels (see dfb_enhance_ragged_linked): streams g * channels + c form link group g; B % channels == 0.
+ * Only on a new or reset handle (DFB_ERR_INVALID after the first frame: the frame re-synthesised for the overlap-add
+ * tail would mix two settings).  channels = 1 or DFB_REDUCE_NONE: unlinked (the default). */
+int dfb_stream_set_mask_reduce(dfb_stream *s, int channels, int reduce_mask);
 /* capi.rs df_process_frame, batched and for n_frames hops at once: d_in / d_out f32[B][n_frames * hop] (device) */
 int dfb_stream_process(dfb_stream *s, const float *d_in, int64_t n_frames, float *d_out, void *stream);
 /* end of stream: the latency frames still in flight, d_out f32[B][latency * hop]; reset before feeding again */
