@@ -192,11 +192,12 @@ struct AnaWindow { int t_begin, nf, out_t0, Tbuf; int64_t row_stride; const Ragg
 int launch_analysis(dfb_state *st, const float *d_audio, int64_t C, int64_t T, float *d_spec, float *d_erb_db,
                     cudaStream_t s, const float *d_init_mem = nullptr, const AnaWindow *w = nullptr);
 // Ts: frames per stream in the buffers (0 = Tf; pointers pre-offset to the first frame); *_state_out: EMA states after
-// the last frame (may be null / alias the inputs)
+// the last frame (may be null / alias the inputs); ref_bits: the reference loop's bits at any length (libdf.erb_norm /
+// unit_norm): the one-thread scan, never the time-segmented one, with the reference's |x|
 int launch_feat_norm(const float *d_erb, int E, int64_t erb_stride, const float *d_spec, int Fd, int64_t spec_stride,
                      int64_t C, int64_t Tf, float alpha, const float *d_erb_state, const float *d_unit_state,
                      float *d_feat_erb, float *d_feat_spec, cudaStream_t s, int64_t Ts = 0, float *d_erb_state_out = nullptr,
-                     float *d_unit_state_out = nullptr);
+                     float *d_unit_state_out = nullptr, bool ref_bits = false);
 int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaStream_t s);
 // time window of a recurrence launch: steps 0 .. T-1 are frames t0 .. of buffers holding Ts frames per stream; h0 (null:
 // zeros) / hT (null: not stored) are the carried hidden states [B][H]

@@ -312,7 +312,13 @@ __global__ void __launch_bounds__(256) k_resample(const float *__restrict__ x, i
 // the kernel was latency bound at 0.10 of HBM), 4 for the generic libdf.erb_norm / unit_norm shapes (up to 1024 threads)
 // Ts = frames per stream in the four buffers (the pointers are pre-offset to the first frame to process, Tf = number of
 // frames processed); *_state_out (may alias the inputs) receive the EMA states after the last frame.
-template <int kPf>
+// REF_BITS (the libdf.unit_norm API): |x| as the reference computes it (Complex32::norm -> hypotf of glibc, which rounds
+// sqrt(re^2 + im^2) evaluated in double), so that the results are its bits; CUDA's hypotf is within an ulp of it but not
+// always the same float.  Separate instantiations: the enhancement path's kernels compile as without it.
+__device__ __forceinline__ float norm_ref_bits(float2 v) {
+    return __double2float_rn(__dsqrt_rn(__dadd_rn(__dmul_rn((double)v.x, (double)v.x), __dmul_rn((double)v.y, (double)v.y))));
+}
+template <int kPf, bool REF_BITS = false>
 __global__ void __launch_bounds__(kPf > 8 ? 128 : 1024) k_feat_norm(const float *erb_in, int E, int64_t erb_stride_t,
                             const float2 *__restrict__ spec_in, int Fd, int64_t spec_stride_t, int Tf,
                             float alpha, const float *erb_state, const float *unit_state,
@@ -366,7 +372,10 @@ __global__ void __launch_bounds__(kPf > 8 ? 128 : 1024) k_feat_norm(const float 
             }
             // the magnitudes and the normalisation are independent across frames; only the two-op EMA chain is serial
 #pragma unroll
-            for (int u = 0; u < kPf; u++) nrm[u] = hypotf(v[u].x, v[u].y);
+            for (int u = 0; u < kPf; u++) {
+                if constexpr (REF_BITS) nrm[u] = norm_ref_bits(v[u]);
+                else nrm[u] = hypotf(v[u].x, v[u].y);
+            }
 #pragma unroll
             for (int u = 0; u < kPf; u++) {
                 if (t + u < Tf) s = __fadd_rn(__fmul_rn(nrm[u], one_m_alpha), __fmul_rn(s, alpha));
@@ -1087,13 +1096,21 @@ int launch_analysis(dfb_state *st, const float *d_audio, int64_t C, int64_t T, f
 int launch_feat_norm(const float *d_erb, int E, int64_t erb_stride, const float *d_spec, int Fd, int64_t spec_stride,
                      int64_t C, int64_t Tf, float alpha, const float *d_erb_state, const float *d_unit_state,
                      float *d_feat_erb, float *d_feat_spec, cudaStream_t s, int64_t Ts, float *d_erb_state_out,
-                     float *d_unit_state_out) {
+                     float *d_unit_state_out, bool ref_bits) {
     if (C <= 0 || Tf <= 0 || E + Fd == 0) return DFB_OK;
     if (E + Fd > 1024) return fail(DFB_ERR_INVALID, "E + F > 1024 in norm scan");
     int threads = ((E + Fd + 31) / 32) * 32;
     DFB_PROF("k_feat_norm", s);
     static const bool no_seg = getenv("DFB_NORM_SEG") && !atoi(getenv("DFB_NORM_SEG"));
-    if (threads <= 128 && Tf >= 16 * kNormSeg && !no_seg)
+    if (ref_bits && threads <= 128)
+        k_feat_norm<24, true><<<(unsigned)C, threads, 0, s>>>(d_erb, E, erb_stride, (const float2 *)d_spec, Fd, spec_stride, (int)Tf,
+                                                             alpha, d_erb_state, d_unit_state, d_feat_erb, (float2 *)d_feat_spec,
+                                                             (int)(Ts > 0 ? Ts : Tf), d_erb_state_out, d_unit_state_out);
+    else if (ref_bits)
+        k_feat_norm<4, true><<<(unsigned)C, threads, 0, s>>>(d_erb, E, erb_stride, (const float2 *)d_spec, Fd, spec_stride, (int)Tf,
+                                                            alpha, d_erb_state, d_unit_state, d_feat_erb, (float2 *)d_feat_spec,
+                                                            (int)(Ts > 0 ? Ts : Tf), d_erb_state_out, d_unit_state_out);
+    else if (threads <= 128 && Tf >= 16 * kNormSeg && !no_seg)
         k_feat_norm_seg<<<(unsigned)C, 128 * kNormSeg, 0, s>>>(d_erb, E, erb_stride, (const float2 *)d_spec, Fd, spec_stride, (int)Tf,
                                                             alpha, d_erb_state, d_unit_state, d_feat_erb, (float2 *)d_feat_spec,
                                                             (int)(Ts > 0 ? Ts : Tf), d_erb_state_out, d_unit_state_out);
@@ -1302,7 +1319,8 @@ extern "C" int dfb_erb_norm_host(int device, const float *h_erb, int64_t C, int6
         d_st = s.alloc<float>(C * E);
         DFB_CUDA(cudaMemcpy(d_st, h_state, sizeof(float) * C * E, cudaMemcpyHostToDevice));
     }
-    rc = launch_feat_norm(d_in, (int)E, E, nullptr, 0, 0, C, T, alpha, d_st, nullptr, d_out, nullptr, 0);
+    // pyDF's bits at every length (ref_bits)
+    rc = launch_feat_norm(d_in, (int)E, E, nullptr, 0, 0, C, T, alpha, d_st, nullptr, d_out, nullptr, 0, 0, nullptr, nullptr, true);
     if (rc) return rc;
     DFB_CUDA(cudaMemcpy(h_out, d_out, sizeof(float) * C * T * E, cudaMemcpyDeviceToHost));
     return DFB_OK;
@@ -1321,7 +1339,7 @@ extern "C" int dfb_unit_norm_host(int device, const float *h_spec, int64_t C, in
         d_st = s.alloc<float>(C * F);
         DFB_CUDA(cudaMemcpy(d_st, h_state, sizeof(float) * C * F, cudaMemcpyHostToDevice));
     }
-    rc = launch_feat_norm(nullptr, 0, 0, d_in, (int)F, F, C, T, alpha, nullptr, d_st, nullptr, d_out, 0);
+    rc = launch_feat_norm(nullptr, 0, 0, d_in, (int)F, F, C, T, alpha, nullptr, d_st, nullptr, d_out, 0, 0, nullptr, nullptr, true);
     if (rc) return rc;
     DFB_CUDA(cudaMemcpy(h_out, d_out, sizeof(float) * 2 * C * T * F, cudaMemcpyDeviceToHost));
     return DFB_OK;
