@@ -1,0 +1,120 @@
+#!/usr/bin/env python3
+"""Serving simulation for streaming slots: one DfStream handle of 256 slots (seeded random weights) serves calls that
+start and end at seeded times, for DeepFilterNet3 and DeepFilterNet3_ll.
+
+Sessions last 2-30 s (uniform); arrivals (Poisson, at the rate that keeps about half of the slots open) open a free
+slot, and a session closes its slot after its last hop.  The handle is fed in calls of --hops hops (1 and 10 by
+default).  Reported per model and call size:
+  * device time per call (CUDA events around each process call, which includes the slot bookkeeping of that call),
+    p50 and p99;
+  * useful audio-s/s: audio of the open sessions per second of device time;
+  * the same traffic with all 256 slots computed on every call (no slot operations: the only option before slots).
+Prints one JSON line, with the card's name, power limit and SM clock read in the same run.
+
+    python bench_slots.py [--slots 256] [--calls 400] [--hops 1 10] [--warmup 20]
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+from bench import model_config  # noqa: E402
+from bench_ragged import card  # noqa: E402
+
+SR, HOP = 48000, 480
+
+
+def traffic(slots: int, calls: int, hops: int, seed: int):
+    """(slots open at the start, and per call: slots to close, slots to open, open slots after the operations).  Starts
+    in steady state: half of the slots open, with uniformly distributed remaining lengths."""
+    rng = np.random.default_rng(seed)
+    lo, hi = 2 * SR // HOP, 30 * SR // HOP                     # session length in hops
+    rate = (slots / 2) / ((lo + hi) / 2)                     # arrivals per hop that keep half the slots busy
+    left = np.full(slots, -1, np.int64)                      # hops a session still has; -1: free
+    start = rng.permutation(slots)[:slots // 2]
+    left[start] = rng.integers(1, hi + 1, slots // 2)
+    plan = []
+    for _ in range(calls):
+        closes = np.flatnonzero(left == 0).tolist()
+        left[closes] = -1
+        free = np.flatnonzero(left < 0)
+        k = min(int(rng.poisson(rate * hops)), free.size)
+        opens = rng.choice(free, k, replace=False).tolist() if k else []
+        left[opens] = rng.integers(lo, hi + 1, k)
+        live = int((left > 0).sum())
+        left[left > 0] = np.maximum(left[left > 0] - hops, 0)
+        plan.append((closes, opens, live))
+    return sorted(start.tolist()), plan
+
+
+def run(name: str, slots: int, calls: int, hops: int, warmup: int, seed: int):
+    import torch
+    from deepfilternet_b200 import DfNet, DfStream, libdf
+    from deepfilternet_b200.weights import random_state_dict
+    cfg = model_config(name)
+    st = libdf.DF(cfg.sr, cfg.fft_size, cfg.hop_size, cfg.nb_erb, cfg.min_nb_erb_freqs)
+    model = DfNet(cfg, random_state_dict(cfg, seed=1), st)
+    x = torch.randn(slots, hops * HOP, device="cuda") * 0.1
+    start, plan = traffic(slots, calls, hops, seed)
+    res = {}
+    for mode in ("slots", "all_computed"):
+        s = DfStream(model, st, batch=slots)
+        for _ in range(warmup):
+            s.process(x)
+        s.reset()
+        if mode == "slots":   # the steady state the plan starts from: flush frees every slot, then half of them open
+            s.flush()
+            s.open(start)
+        ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in plan]
+        torch.cuda.synchronize()
+        for (closes, opens, _), (e0, e1) in zip(plan, ev):
+            e0.record()
+            if mode == "slots":
+                if closes:
+                    s.close(closes)
+                if opens:
+                    s.open(opens)
+            s.process(x)
+            e1.record()
+        torch.cuda.synchronize()
+        ms = np.array([a.elapsed_time(b) for a, b in ev])
+        useful = sum(live for _, _, live in plan) * hops * HOP / SR
+        res[mode] = {"p50_ms": float(np.percentile(ms, 50)), "p99_ms": float(np.percentile(ms, 99)),
+                     "mean_ms": float(ms.mean()), "useful_audio_s_per_s": useful / (ms.sum() / 1e3)}
+        del s
+    res["mean_open_slots"] = float(np.mean([live for _, _, live in plan]))
+    res["speedup_useful"] = res["slots"]["useful_audio_s_per_s"] / res["all_computed"]["useful_audio_s_per_s"]
+    return res
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--slots", type=int, default=256)
+    ap.add_argument("--calls", type=int, default=400)
+    ap.add_argument("--hops", type=int, nargs="+", default=[1, 10])
+    ap.add_argument("--models", nargs="+", default=["DeepFilterNet3", "DeepFilterNet3_ll"])
+    ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--seed", type=int, default=7)
+    a = ap.parse_args()
+    import torch
+    assert torch.cuda.is_available(), "bench_slots.py measures on a GPU"
+    before = card()
+    rows = {}
+    for name in a.models:
+        for hops in a.hops:
+            calls = a.calls if hops == 1 else max(a.calls // hops, 40)
+            rows[f"{name}/{hops}hop"] = run(name, a.slots, calls, hops, a.warmup, a.seed)
+    print(json.dumps({"metric": "serving simulation, streaming slots vs every slot computed", "weights": "random (seed 1)",
+                      "card": before, "card_after": card(), "slots": a.slots, "session_s": [2, 30], "results": rows}))
+
+
+if __name__ == "__main__":
+    main()

@@ -131,6 +131,24 @@ struct RaggedRow { int64_t in_off, len, out_off, out_len, Tf; };
 struct LinkRow { int first, n; };
 enum { kReduceNone = 0, kReduceMax = 1, kReduceMean = 2 };   // dfb_reduce_mask
 
+// Streaming slots (dfb_stream_open_slots): `first` holds the absolute first frame of each stream of a launch, or is null.
+// Window frame t (absolute w0 + t) of stream b exists from the returned window frame on; the kernels that look back in
+// time read padding before it, as a fresh stream does before its frame 0.  Null: 0, every frame of the window exists.
+__device__ __forceinline__ int stream_first(const int64_t *first, int b, int64_t w0) {
+    if (!first) return 0;
+    const int64_t d = first[b] - w0;
+    return d > 0 ? (int)d : 0;
+}
+
+// Initial states of the feature normalisations (libDF/src/lib.rs: linspace(-60, -90, E) and linspace(1e-3, 1e-4, Fd)),
+// explicitly rounded so that every kernel that starts a stream produces the same fp32 bits
+__device__ __forceinline__ float erb_norm_init(int j, int E) {
+    return (E == 1) ? -60.f : __fadd_rn(-60.f, __fmul_rn((float)j, __fdiv_rn(-30.f, (float)(E - 1))));
+}
+__device__ __forceinline__ float unit_norm_init(int k, int Fd) {
+    return (Fd == 1) ? 0.001f : __fadd_rn(0.001f, __fmul_rn((float)k, __fdiv_rn(__fsub_rn(0.0001f, 0.001f), (float)(Fd - 1))));
+}
+
 // Parameters of the fused apply + synthesis kernel (dfb_dsp.cu).
 // mode 0: plain ISTFT; 1: DeepFilterNet3 (DF on the noisy spectrum); 2: DeepFilterNet2 (DF on the
 // masked spectrum).
@@ -173,6 +191,10 @@ struct ApplyParams {
     const RaggedRow *rows;
     int64_t w0;
     int t_emit;
+    // streaming slots (with rows, or null): frames before stream b's first frame (stream_first) synthesise to zero.  Their
+    // spectrum is zero, but the deep filter's look-ahead taps of the last of them reach the stream's first frames, which a
+    // fresh stream never synthesises before.
+    const int64_t *first;
     // linked channels (or null, specialised kernel only): stream b applies the mask of its link group links[b] reduced
     // over the group's streams (reduce: kReduceMax or kReduceMean, tract.rs:868-902) wherever it applies m, and LSNR
     // gating reads the LSNR of the group's first stream.  Everything else -- deep filter, DeepFilterNet3's post filter,
@@ -201,7 +223,7 @@ int launch_feat_norm(const float *d_erb, int E, int64_t erb_stride, const float 
 int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaStream_t s);
 // time window of a recurrence launch: steps 0 .. T-1 are frames t0 .. of buffers holding Ts frames per stream; h0 (null:
 // zeros) / hT (null: not stored) are the carried hidden states [B][H]
-struct GruWindow { const float *h0; float *hT; int t0, Ts; };
+struct GruWindow { const float *h0; float *hT; int t0, Ts; const int64_t *first = nullptr; int64_t w0 = 0; /* stream_first */ };
 // tensor-core GRU recurrence, H = 256 (dfb_tc.cu)
 int launch_gru_tc(cudaStream_t s, const float *xproj, const float *whh, const float *bhh, const float *res, float *hout,
                   unsigned short *hout_hi, unsigned short *hout_lo, int B, int T, long long *dbg = nullptr, int wide = 0,
@@ -217,7 +239,7 @@ int launch_gl_bx(cudaStream_t s, const unsigned short *x_hi, const unsigned shor
 bool gl_bx_geometry(int G, int Ig, int Hg, int *gpc_out, int *hgp_out, int *stages_out);
 // DF pathway conv (df_convp) on tensor cores (dfb_tc.cu)
 int launch_df_convp_tc(cudaStream_t s, const float *c0, const float *w_sw, const float *w2, const float *bias, float *coefs, int B, int T,
-                       int Fd);
+                       int Fd, const int64_t *first = nullptr, int64_t w0 = 0);
 // fp32 [M][K] -> BF16 hi / lo planes [M][K]
 int launch_to_planes(cudaStream_t s, const float *x, int64_t ldx, int64_t M, int K, unsigned short *hi, unsigned short *lo);
 }  // namespace dfb

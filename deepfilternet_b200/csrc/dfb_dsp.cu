@@ -14,6 +14,7 @@
 // HBM layout: audio f32[B,T]; spec c64[B,Tf,481] (frame-major, 3848 B rows); features
 // f32[B,Tf,32] and c64[B,Tf,96]; every kernel reads/writes whole rows with consecutive lanes on
 // consecutive addresses.
+#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -331,7 +332,7 @@ __global__ void __launch_bounds__(kPf > 8 ? 128 : 1024) k_feat_norm(const float 
         float *dst = feat_erb + (int64_t)b * Ts * E + j;
         float s;
         if (erb_state) s = erb_state[(int64_t)b * E + j];
-        else s = (E == 1) ? -60.f : __fadd_rn(-60.f, __fmul_rn((float)j, __fdiv_rn(-30.f, (float)(E - 1))));
+        else s = erb_norm_init(j, E);
         // software pipelined: the loads of batch n + 1 are in flight while batch n runs its (sequential) EMA
         float vn[kPf];
 #pragma unroll
@@ -358,7 +359,7 @@ __global__ void __launch_bounds__(kPf > 8 ? 128 : 1024) k_feat_norm(const float 
         float2 *dst = feat_spec + (int64_t)b * Ts * Fd + k;
         float s;
         if (unit_state) s = unit_state[(int64_t)b * Fd + k];
-        else s = (Fd == 1) ? 0.001f : __fadd_rn(0.001f, __fmul_rn((float)k, __fdiv_rn(__fsub_rn(0.0001f, 0.001f), (float)(Fd - 1))));
+        else s = unit_norm_init(k, Fd);
         float2 vn[kPf];
 #pragma unroll
         for (int u = 0; u < kPf; u++) vn[u] = (u < Tf) ? src[(int64_t)u * spec_stride_t] : make_float2(0.f, 0.f);
@@ -486,10 +487,10 @@ __global__ void __launch_bounds__(128 * kNormSeg) k_feat_norm_seg(const float *e
     float s0;
     if (is_erb) {
         if (erb_state) s0 = erb_state[(int64_t)b * E + j];
-        else s0 = (E == 1) ? -60.f : __fadd_rn(-60.f, __fmul_rn((float)j, __fdiv_rn(-30.f, (float)(E - 1))));
+        else s0 = erb_norm_init(j, E);
     } else {
         if (unit_state) s0 = unit_state[(int64_t)b * Fd + k];
-        else s0 = (Fd == 1) ? 0.001f : __fadd_rn(0.001f, __fmul_rn((float)k, __fdiv_rn(__fsub_rn(0.0001f, 0.001f), (float)(Fd - 1))));
+        else s0 = unit_norm_init(k, Fd);
     }
     if (seg > 0) {
         double sd = (double)s0;
@@ -600,9 +601,11 @@ __global__ void __launch_bounds__(32 * kSynWarps) k_apply_synthesis_generic(Appl
     int Te = p.Tf, Tv = p.Tv ? p.Tv : p.Tf;     // frames this stream synthesises / spectrum rows that exist
     float *orow = p.audio ? p.audio + (int64_t)b * p.out_stride : nullptr;
     int64_t out_len = p.out_len;
+    int t_zero = INT_MIN;   // frames before it synthesise to zero (streaming slots; t may be -1 for the carried tail)
     if (p.rows) {
         const RaggedRow r = p.rows[b];
         const int tfb = (int)(r.Tf - p.w0);
+        if (p.first) t_zero = stream_first(p.first, b, p.w0);
         Te = tfb <= p.Tf ? tfb : p.t_emit;
         Tv = min(Tv, tfb);
         if (orow) orow = p.audio + r.out_off;
@@ -630,6 +633,7 @@ __global__ void __launch_bounds__(32 * kSynWarps) k_apply_synthesis_generic(Appl
             if (k <= 240) {
                 float2 xk = apply_bin(p, tb, srow0, mrow0, crow, t, k, Tv);
                 float2 xnk = apply_bin(p, tb, srow0, mrow0, crow, t, kC - k, Tv);
+                if (t < t_zero) xk = xnk = make_float2(0.f, 0.f);
                 if (p.spec_out && t >= t0) {
                     float2 *orow = p.spec_out + ((int64_t)b * p.Tf + t) * kF;
                     orow[k] = xk;
@@ -700,7 +704,9 @@ __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyP
     const int Tf = p.Tf, L = p.lookahead, back = ORDER - 1 - L;
     int Te = Tf, Tv = p.Tv ? p.Tv : Tf;                    // frames synthesised; spectrum rows >= Tv do not exist (end of the stream)
     int64_t orow0 = (int64_t)b * p.out_stride, out_len = p.out_len;
+    int t_zero = 0;                                        // streaming slots: frames before it synthesise to zero
     if constexpr (RG) {                                    // ragged batch: this stream's own end and output row
+        t_zero = stream_first(p.first, b, p.w0);
         const RaggedRow r = p.rows[b];
         const int tfb = (int)(r.Tf - p.w0);
         Te = tfb <= Tf ? tfb : p.t_emit;
@@ -781,6 +787,7 @@ __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyP
             const float l = p.lsnr[(int64_t)lb * mcT + t];
             stage = l < p.th_min ? 0 : (l > p.th_erb ? 1 : (l > p.th_df ? 2 : 3));
         }
+        if (RG && t < t_zero) stage = 0;   // zero gains, no deep filter: the stream has not started
 #pragma unroll
         for (int o = 0; o < ORDER - 1; o++)
 #pragma unroll

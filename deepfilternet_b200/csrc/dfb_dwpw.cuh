@@ -47,6 +47,10 @@ struct DwPwParams {
     const float *mk_w;    // conv0_out taps [3][64]
     const float *mk_bias; // [1]
     float *mk_out;        // m [B,T,Fout]
+    // streaming slots (tensor-core kernel, kt = 2): first frame of each stream (stream_first) and the window's frame 0,
+    // or null: the previous-frame tap reads padding before it
+    const int64_t *first;
+    int64_t w0;
 };
 
 

@@ -60,11 +60,13 @@ k_conv_in(const float *__restrict__ x, const float *__restrict__ w /*[kt][3][CIN
           int Tx /* feature frames that exist; beyond = end of the stream = zero */,
           int tp_min /* 0: the features are shifted by the look-ahead, then padded causally (DeepFilterNet2 / 3, pad_feat);
                         -lookahead: the conv itself pads (kt-1-la, la) around the unshifted features (DeepFilterNet v1) */,
-          const RaggedRow *__restrict__ rg /* ragged batch: stream b's features end at its own frame count */, int64_t w0 /* absolute frame of window row 0 */) {
+          const RaggedRow *__restrict__ rg /* ragged batch: stream b's features end at its own frame count */, int64_t w0 /* absolute frame of window row 0 */,
+          const int64_t *__restrict__ first /* streaming slots: stream b's shifted features start at its own first frame */) {
     extern __shared__ float s_in[];  // [(kInFrames + kt - 1)][(F + 2) * CIN]
     const int b = blockIdx.y, t0 = blockIdx.x * kInFrames;
     const int rows = kInFrames + kt - 1, ld = (F + 2) * CIN;
     if (rg) Tx = min(Tx, (int)(rg[b].Tf - w0));
+    if (first) tp_min = max(tp_min, stream_first(first, b, w0));
     for (int i = threadIdx.x; i < rows * ld; i += blockDim.x) {
         int r = i / ld, j = i - r * ld;
         int f = j / CIN - 1, ci = j - (f + 1) * CIN;
@@ -345,11 +347,13 @@ constexpr int kMaskWarps = 4, kMaskChunk = 8, kMaskLd = kCh + 1;
 __global__ void __launch_bounds__(32 * kMaskWarps)
 k_mask_out(const float *__restrict__ e0, const float *__restrict__ d1, const float *__restrict__ ps,
            const float *__restrict__ pb, const float *__restrict__ w /*[kt][3][64]*/,
-           const float *__restrict__ bias_p, float *__restrict__ m, int T, int E, int kt) {
+           const float *__restrict__ bias_p, float *__restrict__ m, int T, int E, int kt,
+           const int64_t *__restrict__ first /* streaming slots (stream_first) or null */, int64_t w0) {
     extern __shared__ float smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int b = blockIdx.y;
     const int t0 = (blockIdx.x * kMaskWarps + warp) * kMaskChunk;
+    const int t_first = stream_first(first, b, w0);   // the previous-frame tap of frame t_first is padding
     float *buf = smem + warp * 2 * (E + 2) * kMaskLd;  // two frames
     float *ws = smem + kMaskWarps * 2 * (E + 2) * kMaskLd;  // [kt*3*64] shared by all warps
     for (int i = threadIdx.x; i < kt * 3 * kCh; i += blockDim.x) ws[i] = w[i];
@@ -377,7 +381,7 @@ k_mask_out(const float *__restrict__ e0, const float *__restrict__ d1, const flo
                 for (int dt = 0; dt < kt; dt++) {
                     // dt = kt-1 is the current frame; dt = kt-2 the previous one (kt <= 2)
                     const float *src = (dt == kt - 1) ? cur : prv;
-                    if (dt != kt - 1 && t == 0) continue;
+                    if (dt != kt - 1 && t <= t_first) continue;
                     for (int df = 0; df < 3; df++) {
                         const float *xr = src + (f + df) * kMaskLd;
                         const float *wr = ws + (dt * 3 + df) * kCh;
@@ -458,7 +462,8 @@ using namespace dfb;
 
 // carried hidden states of one GRU stack between time chunks: h = [layers][Bs][H]; t0 = first frame the recurrences run.
 // Bs is the stream count the state was allocated for: a chunk may run only a prefix B <= Bs of the streams (ragged batch)
-struct GruChunk { float *h; bool have_state; int t0; int Bs; };
+// first / w0: streaming slots, each stream's first frame (stream_first) or null
+struct GruChunk { float *h; bool have_state; int t0; int Bs; const int64_t *first; int64_t w0; };
 
 struct dfb_model {
     int device;
@@ -683,7 +688,7 @@ int run_gru(dfb_model *m, cudaStream_t s, const char *name, int layers, int H, i
         const bool last = l == layers - 1;
         float *dst = last ? y : tmp_h;
         float *hs = ck && ck->h ? ck->h + (int64_t)l * ck->Bs * H : nullptr;   // carried state of this layer [Bs][H], rows [0, B)
-        GruWindow gw{ck && ck->have_state ? hs : nullptr, hs, t0, T};
+        GruWindow gw{ck && ck->have_state ? hs : nullptr, hs, t0, T, ck ? ck->first : nullptr, ck ? ck->w0 : 0};
         // the last layer's planes feed a grouped linear and include the residual; the others feed the next projection
         unsigned short *hi = last ? out_hi : pl_hi, *lo = last ? out_lo : pl_lo;
         if ((rc = launch_gru_tc(s, xproj, w_hh, b_hh, last ? res_last : nullptr, dst, hi, lo, B, Tn, m->gru_dbg,
@@ -818,6 +823,7 @@ struct ChunkCtx {
     int Bs;                        // streams the GRU states were allocated for (layer stride); the window runs rows [0, B)
     const RaggedRow *rows;         // ragged batch: per-stream frame counts (features end at rows[b].Tf), or null
     int64_t W0;                    // absolute frame of window row 0
+    const int64_t *first;          // streaming slots: per-stream first frames (before them = padding), or null
 };
 constexpr int kHalo = 8;           // >= temporal receptive field of every feed-forward chain of the shipped models
 
@@ -861,11 +867,12 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
                         float *d_m, float *d_coefs, float *d_lsnr, float *d_alpha, cudaStream_t s_in, ChunkCtx *cx) {
     const dfb_model_config &c = m->cfg;
     const int Tsx = cx ? cx->Tsx : T, Tx = cx ? cx->Tx : T;
-    GruChunk ck_enc{cx ? cx->h_enc : nullptr, cx && cx->have_state, cx ? cx->Rc : 0, cx ? cx->Bs : B};
-    GruChunk ck_erb{cx ? cx->h_erb : nullptr, cx && cx->have_state, cx ? cx->Rc : 0, cx ? cx->Bs : B};
-    GruChunk ck_df{cx ? cx->h_df : nullptr, cx && cx->have_state, cx ? cx->Rc : 0, cx ? cx->Bs : B};
     const RaggedRow *rows = cx ? cx->rows : nullptr;
     const int64_t W0 = cx ? cx->W0 : 0;
+    const int64_t *first = cx ? cx->first : nullptr;
+    GruChunk ck_enc{cx ? cx->h_enc : nullptr, cx && cx->have_state, cx ? cx->Rc : 0, cx ? cx->Bs : B, first, W0};
+    GruChunk ck_erb{cx ? cx->h_erb : nullptr, cx && cx->have_state, cx ? cx->Rc : 0, cx ? cx->Bs : B, first, W0};
+    GruChunk ck_df{cx ? cx->h_df : nullptr, cx && cx->have_state, cx ? cx->Rc : 0, cx ? cx->Bs : B, first, W0};
     // DFB_SERIAL=1: everything on the caller's stream (profiling: per-kernel times without overlap)
     static const bool serial = getenv("DFB_SERIAL") && atoi(getenv("DFB_SERIAL"));
     dfb_model::Lane &L = m->lanes[cx ? cx->lane : 0];
@@ -948,7 +955,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         dim3 grid((unsigned)((T + kInFrames - 1) / kInFrames), (unsigned)B);
         int smem = (kInFrames + c.inp_kt - 1) * (E + 2) * 4;
         DFB_PROF("k_conv_in[erb_conv0]", s);
-        k_conv_in<1><<<grid, 256, smem, s>>>(d_feat_erb, w, bb, f.e0, T, E, c.inp_kt, c.conv_lookahead, Tsx, Tx, 0, rows, W0);
+        k_conv_in<1><<<grid, 256, smem, s>>>(d_feat_erb, w, bb, f.e0, T, E, c.inp_kt, c.conv_lookahead, Tsx, Tx, 0, rows, W0, first);
         DFB_LAUNCH_CHECK();
     }
     const float *pw_sw = nullptr;  // set by blk(): swizzled BF16 hi | lo image of the [C_out][C_in] 1x1 weights
@@ -968,6 +975,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         DwPwParams p{};
         p.in = in; p.Fin = Fin; p.in_fs = in_fs; p.out = out; p.Fout = Fout; p.out_fs = out_fs; p.kt = kt; p.T = T;
         p.lookahead = 0;
+        p.first = first; p.w0 = W0;
         return p;
     };
     {
@@ -978,7 +986,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
             dim3 grid((unsigned)((T + kInFrames - 1) / kInFrames), (unsigned)B);
             int smem = (kInFrames + c.inp_kt - 1) * (Fd + 2) * 2 * 4;
             DFB_PROF("k_conv_in[df_conv0]", sa);
-            k_conv_in<2><<<grid, 256, smem, sa>>>(d_feat_spec, w, bb, f.c0, T, Fd, c.inp_kt, c.conv_lookahead, Tsx, Tx, 0, rows, W0);
+            k_conv_in<2><<<grid, 256, smem, sa>>>(d_feat_spec, w, bb, f.c0, T, Fd, c.inp_kt, c.conv_lookahead, Tsx, Tx, 0, rows, W0, first);
             DFB_LAUNCH_CHECK();
             DFB_CUDA(cudaEventRecord(L.ev_c0, sa));
         }
@@ -1003,7 +1011,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
             (rc = need(m, "df_dec.df_convp.b", O2, &bb)))
             return rc;
         // channel contraction on the tensor cores (BF16x3), shifted adds + 1x1 conv in the epilogue
-        if ((rc = launch_df_convp_tc(sl, f.c0, w_sw, w2, bb, d_coefs, B, T, Fd))) return rc;
+        if ((rc = launch_df_convp_tc(sl, f.c0, w_sw, w2, bb, d_coefs, B, T, Fd, first, W0))) return rc;
         DFB_CUDA(cudaEventRecord(L.ev_convp, sl));
     }
     {
@@ -1158,7 +1166,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         int per_cta = kMaskWarps * kMaskChunk;
         dim3 grid((unsigned)((T + per_cta - 1) / per_cta), (unsigned)B);
         DFB_PROF("k_mask_out", s);
-        k_mask_out<<<grid, 32 * kMaskWarps, smem, s>>>(f.e0, f.d1, ps, pb, w, bb, d_m, T, E, c.conv_kt);
+        k_mask_out<<<grid, 32 * kMaskWarps, smem, s>>>(f.e0, f.d1, ps, pb, w, bb, d_m, T, E, c.conv_kt, first, W0);
         DFB_LAUNCH_CHECK();
     }
     return finish();
@@ -1254,13 +1262,13 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
         {
             DFB_PROF("k_conv_in[erb_conv0]", s);
             k_conv_in<1><<<grid, 256, (kInFrames + c.inp_kt - 1) * (E + 2) * 4, s>>>(d_feat_erb, w, bb, f.e0, T, E, c.inp_kt, la, Tsx, Tx, -la,
-                                                                                      nullptr, 0);
+                                                                                      nullptr, 0, nullptr);
             DFB_LAUNCH_CHECK();
         }
         if ((rc = need(m, "enc.df_conv0.w", c.inp_kt * 3 * 2 * kCh, &w)) || (rc = need(m, "enc.df_conv0.b", kCh, &bb))) return rc;
         DFB_PROF("k_conv_in[df_conv0]", sa);
         k_conv_in<2><<<grid, 256, (kInFrames + c.inp_kt - 1) * (Fd + 2) * 2 * 4, sa>>>(d_feat_spec, w, bb, f.c0, T, Fd, c.inp_kt, c.conv_lookahead,
-                                                                                      Tsx, Tx, -c.conv_lookahead, nullptr, 0);
+                                                                                      Tsx, Tx, -c.conv_lookahead, nullptr, 0, nullptr);
         DFB_LAUNCH_CHECK();
     }
     if ((rc = block(sa, "enc.df_conv1", DW_S2, f.c0, Fd, f.c1, Fd / 2, kt, 0, nullptr))) return rc;
@@ -1289,7 +1297,7 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
         unsigned short *ch = x_hi, *cl = x_lo;
         for (int l = 0; l < layers; l++) {
             const std::string nm = std::string(name) + ".g" + std::to_string(l);
-            GruChunk ck{hbase ? hbase + (int64_t)l * B * H : nullptr, false, 0, B};
+            GruChunk ck{hbase ? hbase + (int64_t)l * B * H : nullptr, false, 0, B, nullptr, 0};
             bool ok = false;
             int r = run_gru(m, st, nm.c_str(), 1, H, H, nullptr, y[l], xproj, nullptr, B, T, ch, cl, f.scr_hi, f.scr_lo, 0, y_hi[l], y_lo[l], &ok,
                             hbase ? &ck : nullptr);
@@ -1365,7 +1373,7 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
         const int per_cta = kMaskWarps * kMaskChunk;
         dim3 grid((unsigned)((T + per_cta - 1) / per_cta), (unsigned)B);
         DFB_PROF("k_mask_out", s);
-        k_mask_out<<<grid, 32 * kMaskWarps, smem, s>>>(f.p0, f.d1, ones, zeros, w, bb, d_m, T, E, kt);
+        k_mask_out<<<grid, 32 * kMaskWarps, smem, s>>>(f.p0, f.d1, ones, zeros, w, bb, d_m, T, E, kt, nullptr, 0);
         DFB_LAUNCH_CHECK();
     }
     DFB_CUDA(cudaStreamWaitEvent(s, L.ev_join, 0));
@@ -1510,18 +1518,25 @@ static ChunkGeom chunk_geom(const dfb_model_config &c) {
     return g;
 }
 
-static size_t state_floats(const dfb_model_config &c, const dfb_state *st, int B, size_t off[16]) {
+// Every array of the state slab is `layers` x [B][per_row] floats; only the GRU states have more than one layer.
+constexpr int kStateArrays = 13;
+struct StateLayout { int64_t off[kStateArrays]; int layers[kStateArrays], per_row[kStateArrays]; };
+
+static size_t state_floats(const dfb_model_config &c, const dfb_state *st, int B, size_t off[16], StateLayout *lay = nullptr) {
     const ChunkGeom g = chunk_geom(c);
     const int E = c.nb_erb, Fd = c.nb_df, O2 = 2 * c.df_order, F = st->tb.F, ED = E / 4 * kCh;
     size_t n = 0;
-    auto add = [&](int i, size_t k) { off[i] = n; n += (k + 63) & ~size_t(63); };
-    add(0, (size_t)B * st->hop); add(1, (size_t)B * E); add(2, (size_t)B * Fd);
-    add(3, (size_t)c.enc_gru_layers * B * c.emb_hidden); add(4, (size_t)c.erb_gru_layers * B * c.emb_hidden);
-    add(5, (size_t)c.df_gru_layers * B * c.df_hidden);
-    add(6, (size_t)B * g.Hf * 2 * F); add(7, (size_t)B * g.Hf * E); add(8, (size_t)B * g.Hf * 2 * Fd);
-    add(9, (size_t)B * kMcTail * E); add(10, (size_t)B * kMcTail * Fd * O2);
-    add(11, c.conv_kt > 1 ? (size_t)B * kHalo * ED : 0);
-    add(12, (size_t)B * kMcTail);
+    auto add = [&](int i, int layers, int per_row) {
+        off[i] = n;
+        if (lay) { lay->off[i] = (int64_t)n; lay->layers[i] = layers; lay->per_row[i] = per_row; }
+        n += ((size_t)layers * B * per_row + 63) & ~size_t(63);
+    };
+    add(0, 1, st->hop); add(1, 1, E); add(2, 1, Fd);
+    add(3, c.enc_gru_layers, c.emb_hidden); add(4, c.erb_gru_layers, c.emb_hidden); add(5, c.df_gru_layers, c.df_hidden);
+    add(6, 1, g.Hf * 2 * F); add(7, 1, g.Hf * E); add(8, 1, g.Hf * 2 * Fd);
+    add(9, 1, kMcTail * E); add(10, 1, kMcTail * Fd * O2);
+    add(11, 1, c.conv_kt > 1 ? kHalo * ED : 0);
+    add(12, 1, kMcTail);
     return n;
 }
 static void state_bind(StreamState &S, float *base, const size_t off[16], int B) {
@@ -1571,6 +1586,9 @@ struct ChunkIO {
     // linked channels: each stream's link group (device table in kernel batch order) and the mask reduction, or null / 0
     const LinkRow *links = nullptr;
     int reduce = 0;
+    // streaming slots (dfb_stream_open_slots): rows are the handle's active slots, rows[b].Tf the end of a closing one, and
+    // first[b] the absolute first frame of each; emission follows the handle's clock, clipped at each stream's end.  Or null.
+    const int64_t *first = nullptr;
 };
 
 // One chunk: analyse frames [S.a1, a1n), run the DNN over [S.d1, d1n), emit audio of frames [S.e1, e1n).
@@ -1632,7 +1650,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     // ---- DNN over the window
     if (run_dnn) {
     ChunkCtx cx{Rc, Tsb, Tv, S.h_enc, S.h_erb, S.h_df, S.dnn_started, c.conv_kt > 1 ? S.t_dec : nullptr, S.n_dec, lane,
-                have_prev ? P.ev_done : nullptr, S.B, io.rows, W0};
+                have_prev ? P.ev_done : nullptr, S.B, io.rows, W0, io.first};
     if ((rc = forward_impl(m, arena, fe, fs, B, Tw, mm, cc, ll, aa, s, &cx))) return rc;
     S.n_dec = cx.dec_tail_n;
     S.dnn_started = true;
@@ -1646,7 +1664,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     }
     }
     // ---- apply + synthesis of frames [e0, e1n) (ragged: a stream that ends in this chunk emits up to its end)
-    if (run_dnn && (e1n > S.e1 || io.rows)) {
+    if (run_dnn && (e1n > S.e1 || (io.rows && !io.first))) {
         dfb::ApplyParams p{};
         p.spec = (const float2 *)spec; p.m = mm; p.coefs = cc; p.audio = io.out; p.spec_out = nullptr;
         p.out_stride = io.out_stride; p.out_len = io.out_len;
@@ -1657,7 +1675,8 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
         p.alpha = aa;
         apply_options(m, p);
         if (ll) { p.lsnr = ll; p.th_min = io.lsnr_th[0]; p.th_erb = io.lsnr_th[1]; p.th_df = io.lsnr_th[2]; }
-        if (io.rows) { p.rows = io.rows; p.w0 = W0; p.t_emit = p.Tf; p.Tf = Tw; }   // the grid covers every stream's end
+        if (io.rows) { p.rows = io.rows; p.w0 = W0; p.t_emit = p.Tf; p.first = io.first; }
+        if (io.rows && !io.first) p.Tf = Tw;   // batch: the grid covers every stream's end; slots: Te = min(end, clock)
         if (io.links) { p.links = io.links; p.reduce = io.reduce; }
         if ((rc = launch_apply_synthesis(st, p, B, s))) return rc;
     }
@@ -2116,6 +2135,43 @@ extern "C" int dfb_enhance_ragged_linked_host(dfb_model *m, dfb_state *st, const
 // Every call feeds n >= 1 hops per stream and returns n hops; the output trails the input by `latency` frames
 // (max(conv_lookahead, df_lookahead), + df_lookahead for DeepFilterNet2) on top of the STFT's own fft - hop samples,
 // i.e. the concatenated output equals enhance(pad=False) of the concatenated input delayed by latency * hop samples.
+// Streaming slots (dfb_stream_open_slots / dfb_stream_close_slots; DESIGN.md section 5c).  Each of the handle's B slots
+// opens and closes on its own under the handle's single clock: a slot opened at analysis frame a starts a fresh stream
+// whose frame 0 is a (its state-slab row is initialised, the kernels that look back in time read padding before a), and a
+// closed slot's stream ends at the frame its input had reached (rows[b].Tf, as a ragged stream's end), then emits its
+// look-ahead tail over the next `latency` hops and becomes free.  Open and closing slots are the prefix [0, n_act) of the
+// state slab, so every kernel runs over B = n_act rows only; free slots are not computed and return zeros.
+enum { kSlotFree = 0, kSlotOpen = 1, kSlotClosing = 2 };
+constexpr int64_t kOpenEnd = 0x7fffffff;   // rows[b].Tf of an open slot: kernels take Tf - w0 as int
+
+// Row `dst` of every array of the state slab <- row `src`, or (src < 0) the initial state of a fresh stream: zeros, and the
+// normalisation EMA states at the values launch_feat_norm starts from without a state.  grid (x, kStateArrays).
+__global__ void k_slot_row(float *__restrict__ slab, StateLayout lay, int Bs, int dst, int src, int E, int Fd) {
+    const int a = blockIdx.y, per = lay.per_row[a];
+    const int64_t n = (int64_t)lay.layers[a] * per;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+        const int l = (int)(e / per), j = (int)(e - (int64_t)l * per);
+        float *base = slab + lay.off[a] + (int64_t)l * Bs * per + j;
+        float v = 0.f;
+        if (src >= 0) v = base[(int64_t)src * per];
+        else if (a == 1) v = erb_norm_init(j, E);
+        else if (a == 2) v = unit_norm_init(j, Fd);
+        base[(int64_t)dst * per] = v;
+    }
+}
+
+// carried analysis memory of the slot path: row b's last input hop, read where rows[b] says its input row is
+__global__ void k_carry_hop(float *__restrict__ ana_mem, const float *__restrict__ in, const RaggedRow *__restrict__ rows, int64_t last,
+                            int hop) {
+    const int b = blockIdx.x;
+    for (int i = threadIdx.x; i < hop; i += blockDim.x) ana_mem[(int64_t)b * hop + i] = in[rows[b].in_off + last + i];
+}
+
+// Frame-incremental processing with carried state: the batched counterpart of the reference's single-stream runtime
+// (libDF/src/tract.rs:509-642 `DfTract::process`, C ABI libDF/src/capi.rs:83-253 df_create / df_process_frame / df_free).
+// Every call feeds n >= 1 hops per stream and returns n hops; the output trails the input by `latency` frames
+// (max(conv_lookahead, df_lookahead), + df_lookahead for DeepFilterNet2) on top of the STFT's own fft - hop samples,
+// i.e. the concatenated output equals enhance(pad=False) of the concatenated input delayed by latency * hop samples.
 struct dfb_stream {
     dfb_model *m;
     dfb_state *st;
@@ -2131,6 +2187,16 @@ struct dfb_stream {
     LinkRow *links = nullptr;                          // linked channels (dfb_stream_set_mask_reduce) or null
     int reduce = 0;
     bool fed = false;                                  // a frame has been processed since create / reset
+    // streaming slots.  slots == false: every slot open since create / reset with frame 0 at clock 0 (the table-free path)
+    bool slots = false;
+    std::vector<int> slot_state, slot_row, row_slot;   // kSlot*; slot -> row of the active prefix (-1 free); row -> slot
+    std::vector<int64_t> slot_first, slot_end;         // absolute first frame; end frame of a closing slot
+    int n_act = 0;
+    std::vector<std::pair<int, int>> pend;             // state-slab rows (dst, src; src -1: initialise) for the next call
+    bool tab_dirty = true;                             // rows / first frames to re-upload
+    int64_t tab_n = -1;                                // ... for calls of this many input hops
+    RaggedRow *d_rows = nullptr;
+    int64_t *d_first = nullptr;
 };
 
 extern "C" int dfb_stream_create(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B, float atten_lim_db) {
@@ -2159,6 +2225,8 @@ extern "C" void dfb_stream_free(dfb_stream *h) {
     if (h->stage_in) cudaFree(h->stage_in);
     if (h->stage_out) cudaFree(h->stage_out);
     if (h->links) cudaFree(h->links);
+    if (h->d_rows) cudaFree(h->d_rows);
+    if (h->d_first) cudaFree(h->d_first);
     delete h;
 }
 
@@ -2168,6 +2236,8 @@ extern "C" int dfb_stream_reset(dfb_stream *h) {
     state_floats(h->m->cfg, h->st, h->B, off);
     state_bind(h->S, h->slab, off, h->B);
     h->fed = false;
+    h->slots = false;
+    h->pend.clear();
     return DFB_OK;
 }
 
@@ -2177,6 +2247,7 @@ extern "C" int dfb_stream_reset(dfb_stream *h) {
 extern "C" int dfb_stream_set_mask_reduce(dfb_stream *h, int channels, int reduce_mask) {
     if (!h) return fail(DFB_ERR_INVALID, "null stream");
     if (h->fed) return fail(DFB_ERR_INVALID, "mask reduction set after the first frame: reset the stream first");
+    if (h->slots) return fail(DFB_ERR_UNSUPPORTED, "linked channels and streaming slots do not combine: reset the stream first");
     if (reduce_mask != kReduceNone && reduce_mask != kReduceMax && reduce_mask != kReduceMean)
         return fail(DFB_ERR_INVALID, "reduce_mask %d is not 0 (none), 1 (max) or 2 (mean)", reduce_mask);
     if (channels <= 0 || h->B % channels) return fail(DFB_ERR_INVALID, "%d streams are not groups of %d channels", h->B, channels);
@@ -2214,7 +2285,181 @@ extern "C" int64_t dfb_stream_latency_frames(const dfb_stream *h) {
 }
 extern "C" int64_t dfb_stream_frame_length(const dfb_stream *h) { return h ? h->st->hop : -1; }  // capi.rs df_get_frame_length
 
+// ---- streaming slots: host bookkeeping.  Device rows follow at the next call (stream_step runs h->pend first).
+// Leaves the slot-free path: every slot is open, row b = slot b, its stream started at frame 0.
+static int slots_enable(dfb_stream *h) {
+    if (h->slots) return DFB_OK;
+    const size_t B = (size_t)h->B;
+    if (!h->d_rows) {
+        DFB_CUDA(cudaSetDevice(h->m->device));
+        if (cudaMalloc(&h->d_rows, sizeof(RaggedRow) * B) != cudaSuccess || cudaMalloc(&h->d_first, sizeof(int64_t) * B) != cudaSuccess)
+            return fail(DFB_ERR_OOM, "slot table allocation failed");
+    }
+    h->slot_state.assign(B, kSlotOpen);
+    h->slot_row.resize(B); h->row_slot.resize(B);
+    std::iota(h->slot_row.begin(), h->slot_row.end(), 0);
+    std::iota(h->row_slot.begin(), h->row_slot.end(), 0);
+    h->slot_first.assign(B, 0);
+    h->slot_end.assign(B, kOpenEnd);
+    h->n_act = h->B;
+    h->pend.clear();
+    h->tab_dirty = true;
+    h->slots = true;
+    return DFB_OK;
+}
+
+// the slot's row leaves the active prefix: the last active row moves into its place
+static void slot_release(dfb_stream *h, int slot) {
+    const int r = h->slot_row[(size_t)slot], last = h->n_act - 1;
+    if (r != last) {
+        h->pend.emplace_back(r, last);
+        const int moved = h->row_slot[(size_t)last];
+        h->row_slot[(size_t)r] = moved;
+        h->slot_row[(size_t)moved] = r;
+    }
+    h->slot_row[(size_t)slot] = -1;
+    h->slot_state[(size_t)slot] = kSlotFree;
+    h->n_act--;
+    h->tab_dirty = true;
+}
+
+// closing slots whose last frame has been output become free: `out_end` is the frame after the last output hop so far
+// (a1 - latency after a process call, a1 after a flush)
+static void slots_retire(dfb_stream *h, int64_t out_end) {
+    for (int b = 0; b < h->B; b++)
+        if (h->slot_state[(size_t)b] == kSlotClosing && h->slot_end[(size_t)b] <= out_end) slot_release(h, b);
+}
+
+static void slot_close(dfb_stream *h, int slot) {
+    if (h->slot_state[(size_t)slot] != kSlotOpen) return;
+    h->slot_state[(size_t)slot] = kSlotClosing;
+    h->slot_end[(size_t)slot] = h->S.a1;   // the stream ends after the input it has been fed
+    h->tab_dirty = true;
+}
+
+static void slots_close_all(dfb_stream *h) {
+    for (int b = 0; b < h->B; b++) slot_close(h, b);
+    slots_retire(h, h->S.a1 - dfb_stream_latency_frames(h));
+}
+
+static int slot_list(dfb_stream *h, const int64_t *slots, int64_t n) {
+    if (!h || n < 0 || (n > 0 && !slots)) return fail(DFB_ERR_INVALID, "bad argument");
+    if (h->links) return fail(DFB_ERR_UNSUPPORTED, "slot operations on a handle with linked channels");
+    std::vector<char> seen((size_t)h->B, 0);
+    for (int64_t i = 0; i < n; i++) {
+        const int64_t b = slots[i];
+        if (b < 0 || b >= h->B) return fail(DFB_ERR_INVALID, "slot %lld outside [0, %d)", (long long)b, h->B);
+        if (seen[(size_t)b]) return fail(DFB_ERR_INVALID, "slot %lld listed twice", (long long)b);
+        seen[(size_t)b] = 1;
+    }
+    return slots_enable(h);
+}
+
+extern "C" int dfb_stream_open_slots(dfb_stream *h, const int64_t *slots, int64_t n) {
+    if (int rc = slot_list(h, slots, n)) return rc;
+    for (int64_t i = 0; i < n; i++) {
+        const int b = (int)slots[i];
+        int r = h->slot_row[(size_t)b];
+        if (r < 0) {   // free: takes the row after the active prefix
+            r = h->n_act++;
+            h->slot_row[(size_t)b] = r;
+            h->row_slot[(size_t)r] = b;
+        }
+        h->pend.emplace_back(r, -1);   // a fresh stream; an open or closing one is dropped without its tail
+        h->slot_state[(size_t)b] = kSlotOpen;
+        h->slot_first[(size_t)b] = h->S.a1;
+        h->slot_end[(size_t)b] = kOpenEnd;
+    }
+    h->tab_dirty = true;
+    return DFB_OK;
+}
+
+extern "C" int dfb_stream_close_slots(dfb_stream *h, const int64_t *slots, int64_t n) {
+    if (int rc = slot_list(h, slots, n)) return rc;
+    for (int64_t i = 0; i < n; i++) slot_close(h, (int)slots[i]);
+    slots_retire(h, h->S.a1 - dfb_stream_latency_frames(h));   // without look-ahead (latency 0) a closed slot is free at once
+    return DFB_OK;
+}
+
+extern "C" int dfb_stream_slot_states(const dfb_stream *h, int32_t *h_states) {
+    if (!h || !h_states) return fail(DFB_ERR_INVALID, "null argument");
+    for (int b = 0; b < h->B; b++) h_states[b] = h->slots ? h->slot_state[(size_t)b] : kSlotOpen;
+    return DFB_OK;
+}
+
+// Slot path of one call: rows [0, n_act) of the slab, the row table for calls of n input hops, output rows zero first.
+static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, cudaStream_t s) {
+    dfb_model *m = h->m;
+    dfb_state *st = h->st;
+    StreamState &S = h->S;
+    const ChunkGeom g = chunk_geom(m->cfg);
+    const int hop = st->hop, B = h->B;
+    const int64_t Ltot = g.Lmax + g.lag, n_out = flush ? Ltot : n;
+    const int64_t a0 = S.a1, a1n = a0 + (flush ? 0 : n);
+    if (a1n >= kOpenEnd - 1) return fail(DFB_ERR_UNSUPPORTED, "stream clock beyond 2^31 - 2 frames: reset the stream");
+    int64_t d1n = flush ? a1n : a1n - g.Lmax, e1n = flush ? a1n : d1n - g.lag;
+    if (d1n < S.d1) d1n = S.d1;
+    if (e1n < S.e1) e1n = S.e1;
+    if (flush) slots_close_all(h);
+    {   // pending row operations, in order
+        size_t off[16];
+        StateLayout lay;
+        state_floats(m->cfg, st, B, off, &lay);
+        for (const auto &op : h->pend) {
+            k_slot_row<<<dim3(8, kStateArrays), 256, 0, s>>>(h->slab, lay, B, op.first, op.second, m->cfg.nb_erb, m->cfg.nb_df);
+            DFB_LAUNCH_CHECK();
+        }
+        h->pend.clear();
+    }
+    if (h->tab_dirty || h->tab_n != n) {
+        std::vector<RaggedRow> rows((size_t)h->n_act);
+        std::vector<int64_t> first((size_t)h->n_act);
+        for (int r = 0; r < h->n_act; r++) {
+            const int b = h->row_slot[(size_t)r];
+            const bool open = h->slot_state[(size_t)b] == kSlotOpen;
+            rows[(size_t)r] = RaggedRow{b * n * hop, open ? n * hop : 0, b * n_out * hop, n_out * hop, h->slot_end[(size_t)b]};
+            first[(size_t)r] = h->slot_first[(size_t)b];
+        }
+        if (h->n_act > 0) {
+            DFB_CUDA(cudaMemcpyAsync(h->d_rows, rows.data(), sizeof(RaggedRow) * rows.size(), cudaMemcpyHostToDevice, s));
+            DFB_CUDA(cudaMemcpyAsync(h->d_first, first.data(), sizeof(int64_t) * first.size(), cudaMemcpyHostToDevice, s));
+        }
+        h->tab_dirty = false;
+        h->tab_n = n;
+    }
+    if (n_out > 0) DFB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * B * n_out * hop, s));   // free slots; frames outside a stream
+    h->fed = true;
+    if (h->n_act == 0) {   // nothing to compute: the clock moves on (a slot opened later starts from zeroed tails)
+        S.a1 = a1n; S.d1 = d1n; S.e1 = e1n;
+        if (a1n > 0) S.started = true;
+        if (d1n > 0) S.dnn_started = true;
+        S.n_feat = g.Hf; S.n_mc = kMcTail; S.n_dec = kHalo;
+        slots_retire(h, flush ? a1n : a1n - Ltot);
+        return DFB_OK;
+    }
+    const int64_t f0 = a0 - Ltot;   // output hop j carries frame a0 - Ltot + j (flush: a1 = a0)
+    ChunkIO io{d_in, n * hop, n * hop, a0, nullptr, d_out, n_out * hop, n_out * hop, f0 * hop, h->lim, h->gating ? h->th : nullptr,
+               h->d_rows, h->n_act};
+    io.first = h->d_first;
+    int rc = m->arena.reserve(chunk_bytes_per_stream(m->cfg, st, (int)(d1n - (S.d1 > kHalo ? S.d1 - kHalo : 0)) + 1) * (size_t)h->n_act +
+                              (2 << 20));
+    if (rc) return rc;
+    if (!flush && a1n > a0) {
+        if (!S.started) DFB_CUDA(cudaMemsetAsync(S.ana_mem, 0, sizeof(float) * B * hop, s));
+        io.init_mem = S.ana_mem;
+    }
+    if ((rc = run_chunk(m, st, S, io, a1n, d1n, e1n, s))) return rc;
+    if (!flush) {
+        k_carry_hop<<<h->n_act, 128, 0, s>>>(S.ana_mem, d_in, h->d_rows, (n - 1) * hop, hop);
+        DFB_LAUNCH_CHECK();
+    }
+    m->arena.reset();
+    slots_retire(h, flush ? a1n : a1n - Ltot);
+    return DFB_OK;
+}
+
 static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, cudaStream_t s) {
+    if (h->slots) return slots_step(h, d_in, n, flush, d_out, s);
     dfb_model *m = h->m;
     dfb_state *st = h->st;
     StreamState &S = h->S;
@@ -2252,6 +2497,17 @@ static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, 
     return DFB_OK;
 }
 
+// After a flush every stream has ended: all slots are free (linked handles, which have no slots, stay as they were).  Without
+// look-ahead a flush computes nothing and only closes the slots.
+static void flushed_all(dfb_stream *h) {
+    if (h->links) return;
+    if (h->slots) { slots_close_all(h); return; }
+    if (slots_enable(h)) return;
+    std::fill(h->slot_state.begin(), h->slot_state.end(), (int)kSlotFree);
+    std::fill(h->slot_row.begin(), h->slot_row.end(), -1);
+    h->n_act = 0;
+}
+
 // d_in [B][n_frames * hop] -> d_out [B][n_frames * hop] (device pointers, asynchronous on `stream`)
 extern "C" int dfb_stream_process(dfb_stream *h, const float *d_in, int64_t n_frames, float *d_out, void *stream) {
     if (!h || !d_in || !d_out || n_frames <= 0) return fail(DFB_ERR_INVALID, "bad argument");
@@ -2260,21 +2516,28 @@ extern "C" int dfb_stream_process(dfb_stream *h, const float *d_in, int64_t n_fr
 }
 
 // End of the stream: the `latency` frames still in flight, computed with zero look-ahead exactly like the end of a
-// batch enhance(); d_out [B][latency * hop].  The stream must be reset before it is fed again.
+// batch enhance(); d_out [B][latency * hop].  Closes every open slot; on the slot-free path the stream must be reset before
+// it is fed again.
 extern "C" int dfb_stream_flush(dfb_stream *h, float *d_out, void *stream) {
     if (!h || !d_out) return fail(DFB_ERR_INVALID, "bad argument");
     DFB_CUDA(cudaSetDevice(h->m->device));
-    if (dfb_stream_latency_frames(h) == 0) return DFB_OK;
-    return stream_step(h, nullptr, 0, true, d_out, (cudaStream_t)stream);
+    int rc = DFB_OK;
+    if (dfb_stream_latency_frames(h) > 0) rc = stream_step(h, nullptr, 0, true, d_out, (cudaStream_t)stream);
+    if (!rc) flushed_all(h);
+    return rc;
 }
 
 // host-pointer variant (synchronous): h_in / h_out [B][n_frames * hop]; h_in == NULL flushes into h_out [B][latency * hop]
 extern "C" int dfb_stream_process_host(dfb_stream *h, const float *h_in, int64_t n_frames, float *h_out) {
-    if (!h || !h_out || (h_in && n_frames <= 0)) return fail(DFB_ERR_INVALID, "bad argument");
+    if (!h || (h_in && n_frames <= 0)) return fail(DFB_ERR_INVALID, "bad argument");
     DFB_CUDA(cudaSetDevice(h->m->device));
     const bool flush = h_in == nullptr;
     const int64_t nf = flush ? dfb_stream_latency_frames(h) : n_frames;
-    if (nf == 0) return DFB_OK;
+    if (nf == 0) {   // a flush without look-ahead has no output: it only closes the slots
+        flushed_all(h);
+        return DFB_OK;
+    }
+    if (!h_out) return fail(DFB_ERR_INVALID, "bad argument");
     const size_t bytes = sizeof(float) * (size_t)h->B * nf * h->st->hop;
     if (bytes > h->stage_cap) {
         if (h->stage_in) cudaFree(h->stage_in);
@@ -2290,5 +2553,6 @@ extern "C" int dfb_stream_process_host(dfb_stream *h, const float *h_in, int64_t
     if (rc) return rc;
     DFB_CUDA(cudaMemcpyAsync(h_out, h->stage_out, bytes, cudaMemcpyDeviceToHost, s));
     DFB_CUDA(cudaStreamSynchronize(s));
+    if (flush) flushed_all(h);
     return DFB_OK;
 }

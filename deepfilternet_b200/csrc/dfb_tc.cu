@@ -183,6 +183,7 @@ k_dwpw_bx(DwPwParams p, const float *__restrict__ w_sw /* [hi | lo] x [64 n][64 
         return x;
     };
     const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    const int t_first = KT > 1 ? stream_first(p.first, b, p.w0) : 0;
 #pragma unroll
     for (int i = 0; i < 8; i++) {
         const int r = 8 * slot + i;
@@ -191,7 +192,7 @@ k_dwpw_bx(DwPwParams p, const float *__restrict__ w_sw /* [hi | lo] x [64 n][64 
 #pragma unroll
             for (int dt = 0; dt < KT; dt++) {
                 // tap dt reads frame t - (KT-1-dt) = raw frame fr + dt; before the start of the stream it is zero padding
-                if (KT > 1 && tq0 + fr + dt < 0) continue;
+                if (KT > 1 && tq0 + fr + dt < t_first) continue;
                 const uint32_t fb = raw_in + (uint32_t)(fr + dt) * fbytes + cq * 16;
                 if (MODE == DW_S1) {
                     const uint32_t a = fb + (uint32_t)fo * 256;
@@ -389,6 +390,8 @@ struct CvParams {
     const float *bias;   // [10]
     float *coefs;        // [B,T,Fd,10]
     int T, Fd;
+    const int64_t *first;   // streaming slots: first frame of each stream (stream_first), or null
+    int64_t w0;
 };
 
 // One CTA = (stream, kCvBins consecutive bins, 124 output frames): the weight image and the barrier set-up are paid once
@@ -424,7 +427,9 @@ __global__ void __launch_bounds__(kCvThreads, 2) k_df_convp_tc(const __grid_cons
     __syncthreads();
     mbar_wait_a(bar_w, 0);
     const int r = tid & 127, half = tid >> 7;
-    const bool zero = r0 + r < 0;   // before the start of the stream (for b > 0 the box holds the previous stream's rows)
+    // before the start of the stream (for b > 0 the box holds the previous stream's rows; a slot's stream may start inside
+    // the window)
+    const bool zero = r0 + r < stream_first(p.first, b, p.w0);
     for (int f = f_begin, it = 0; f < f_end; f++, it++) {
         const uint32_t par = (uint32_t)(it & 1);
         mbar_wait_a(bar_raw, par);
@@ -570,6 +575,10 @@ struct GruTcParams {
     long long *dbg;      // optional [T][8] clock64 stamps of CTA 0, thread 0 (0 step start, 1 state arrived, 2 MMAs done,
                          // 3 gates done, 4 slice sent)
     unsigned char *xbuf; // (XG) exchange scratch in global memory [cluster][2][CTA][kPiece]
+    // streaming slots: first frame of each stream (stream_first; step t is window frame t0 + t), or null.  The state holds
+    // h = 0 through the steps before it: those frames do not exist for the stream.
+    const int64_t *first;
+    int64_t w0;
 };
 
 // XG = 1: the new state travels through L2 instead of SM to SM -- every CTA stores its slice to a global scratch piece and
@@ -641,7 +650,9 @@ __global__ void __launch_bounds__(GtCfg<NS, HH>::kThreads, 1) k_gru_tc(GruTcPara
     const int gu = rank * kGtU + 2 * up;       // first of the two global hidden units of this thread
     float hprev0 = 0.f, hprev1 = 0.f;
     float2 bhr = make_float2(0.f, 0.f), bhz = bhr, bhn = bhr;
+    int t_first = 0;   // first step of this stream (steps before it keep h = 0)
     if (active) {
+        t_first = stream_first(p.first, b0 + s, p.w0) - p.t0;
         if (p.h0) {
             const float2 hv = *reinterpret_cast<const float2 *>(p.h0 + (int64_t)(b0 + s) * H + gu);
             hprev0 = hv.x; hprev1 = hv.y;
@@ -722,6 +733,7 @@ __global__ void __launch_bounds__(GtCfg<NS, HH>::kThreads, 1) k_gru_tc(GruTcPara
             const float n0 = gt_tanh(xn.x + r0 * (a[4] + bhn.x)), n1 = gt_tanh(xn.y + r1 * (a[5] + bhn.y));
             hprev0 = (1.f - z0) * n0 + z0 * hprev0;
             hprev1 = (1.f - z1) * n1 + z1 * hprev1;
+            if (t < t_first) hprev0 = hprev1 = 0.f;
             unsigned short h0, l0, h1, l1;
             bf16_split(hprev0, h0, l0);
             bf16_split(hprev1, h1, l1);
@@ -863,6 +875,8 @@ int launch_gru_tc(cudaStream_t s, const float *xproj, const float *whh, const fl
                   const GruWindow *w, int H) {
     GruTcParams p{xproj, whh, bhh, res, hout, hout_hi, hout_lo, planes_res, w ? w->h0 : nullptr, w ? w->hT : nullptr,
                   w ? w->t0 : 0, w ? w->Ts : T, B, T, 0, dbg};
+    p.first = w ? w->first : nullptr;
+    p.w0 = w ? w->w0 : 0;
     static const int force = getenv("DFB_GRU_NS") ? atoi(getenv("DFB_GRU_NS")) : 0;
     // exchange through L2 + multicast (k_gru_tc XG): bit 0: H = 512, bit 1: H = 256 / 32 streams, bit 2: H = 256 / 16 streams.
     // Default: all.
@@ -889,7 +903,7 @@ int cached_map_f32_sw128(CUtensorMap *out, const void *base, int64_t rows, int64
 
 // c0 [B,T,Fd,64] -> coefs [B,T,Fd,10] (pathway term), tensor-core version; w_sw: host-packed operand image (weights.py)
 int launch_df_convp_tc(cudaStream_t s, const float *c0, const float *w_sw, const float *w2, const float *bias, float *coefs, int B, int T,
-                       int Fd) {
+                       int Fd, const int64_t *first, int64_t w0) {
     if ((int64_t)B * T >= (int64_t(1) << 31) - 256 || B > 65535) return fail(DFB_ERR_UNSUPPORTED, "df pathway conv: batch too large for one launch");
     CUtensorMap mc;
     int rc;
@@ -898,7 +912,7 @@ int launch_df_convp_tc(cudaStream_t s, const float *c0, const float *w_sw, const
     static PerDeviceOnce attr_once;
     if (auto once_guard = attr_once.first())
         DFB_CUDA(cudaFuncSetAttribute(k_df_convp_tc<5, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CvParams p{w_sw, w2, bias, coefs, T, Fd};
+    CvParams p{w_sw, w2, bias, coefs, T, Fd, first, w0};
     dim3 grid((unsigned)((Fd + kCvBins - 1) / kCvBins), (unsigned)((T + kCvOut - 1) / kCvOut), (unsigned)B);
     DFB_PROF("k_df_convp_tc", s);
     k_df_convp_tc<5, 5><<<grid, kCvThreads, smem, s>>>(mc, p);

@@ -11,12 +11,16 @@ The concatenation of the outputs equals ``enhance(model, df_state, audio, pad=Fa
 
 ``channels`` / ``reduce_mask`` link the channels of each recording as the Rust runtime does: rows g * channels + c are
 the channels of recording g and share one ERB mask, the max or mean of theirs (dfb_stream_set_mask_reduce).
+
+Each row is a slot that can start and end its own stream (``open`` / ``close``), so one handle serves calls that come and
+go: a call joins whenever a slot is free, and only open and closing slots are computed.
 """
 from __future__ import annotations
 
 import ctypes as C
 from typing import Optional
 
+import numpy as np
 import torch
 from torch import Tensor
 
@@ -24,6 +28,29 @@ from . import _lib, ragged
 from ._lib import check
 from .libdf import DF
 from .model import DfNet
+
+
+SLOT_FREE, SLOT_OPEN, SLOT_CLOSING = 0, 1, 2
+
+
+def slot_list(slots, batch: int) -> np.ndarray:
+    """``slots`` (an int, or a sequence / array / tensor of ints) as a contiguous int64 array of slot indices of a handle
+    with ``batch`` slots.  ValueError when an index is not an integer, lies outside [0, batch) or is listed twice."""
+    if isinstance(slots, Tensor):
+        slots = slots.detach().cpu().numpy()
+    a = np.asarray([slots] if np.isscalar(slots) else slots)
+    if a.ndim != 1 and a.size:
+        raise ValueError("slots must be a flat list of slot indices")
+    if a.size and a.dtype.kind not in "iu":
+        raise ValueError("slot indices must be integers")
+    a = np.ascontiguousarray(a.reshape(-1), dtype=np.int64)
+    bad = a[(a < 0) | (a >= batch)]
+    if bad.size:
+        raise ValueError(f"slot {int(bad[0])} outside [0, {batch})")
+    u, counts = np.unique(a, return_counts=True)
+    if (counts > 1).any():
+        raise ValueError(f"slot {int(u[counts > 1][0])} listed twice")
+    return a
 
 
 class DfStream:
@@ -64,7 +91,33 @@ class DfStream:
                                                         float(max_db_df_thresh)))
 
     def reset(self) -> None:
+        """Every slot open with a fresh stream, the clock back at 0."""
         check(_lib.lib().dfb_stream_reset(self._h))
+
+    def _slots(self, fn, slots) -> None:
+        a = slot_list(slots, self.batch)
+        check(fn(self._h, a.ctypes.data_as(C.POINTER(C.c_int64)), a.size))
+
+    def open(self, slots) -> None:
+        """Start a new stream in each listed slot, from the initial state, as a fresh handle would.  An open or closing
+        slot's old stream is dropped without its tail.  Takes effect at the next ``process`` / ``flush``; from then on row
+        b of their input and output is that stream, and its output equals ``DfStream(batch=1)`` fed the same audio in the
+        same call sizes and flushed at the end."""
+        self._slots(_lib.lib().dfb_stream_open_slots, slots)
+
+    def close(self, slots) -> None:
+        """End the stream of each listed open slot after the input it has already been fed.  From the next call on its
+        input rows are ignored; over the next ``latency_frames`` hops its output rows carry what ``flush`` would give that
+        stream alone, whatever the call sizes, then the slot is free (at once when ``latency_frames`` is 0).  Free slots
+        are not computed and return zeros.  Closing a slot that is not open does nothing."""
+        self._slots(_lib.lib().dfb_stream_close_slots, slots)
+
+    def slot_states(self) -> np.ndarray:
+        """int32 [batch]: SLOT_FREE (0), SLOT_OPEN (1) or SLOT_CLOSING (2) per slot.  A new or reset handle has every slot
+        open; ``flush`` closes them all."""
+        out = np.zeros(self.batch, np.int32)
+        check(_lib.lib().dfb_stream_slot_states(self._h, out.ctypes.data_as(C.POINTER(C.c_int32))))
+        return out
 
     @torch.no_grad()
     def process(self, audio: Tensor) -> Tensor:
@@ -88,8 +141,8 @@ class DfStream:
 
     @torch.no_grad()
     def flush(self) -> Tensor:
-        """The ``latency_frames`` hops still in flight at the end of the stream (CPU tensor)."""
+        """The ``latency_frames`` hops still in flight at the end of every stream (CPU tensor): closes every open slot,
+        and their tails come out in this call."""
         out = torch.zeros((self.batch, self.latency_frames * self.hop), dtype=torch.float32)
-        if self.latency_frames:
-            check(_lib.lib().dfb_stream_process_host(self._h, None, 0, out.data_ptr()))
+        check(_lib.lib().dfb_stream_process_host(self._h, None, 0, out.data_ptr()))
         return out

@@ -254,10 +254,31 @@ int dfb_stream_set_lsnr_thresholds(dfb_stream *s, int enable, float min_db_thres
 int dfb_stream_set_mask_reduce(dfb_stream *s, int channels, int reduce_mask);
 /* capi.rs df_process_frame, batched and for n_frames hops at once: d_in / d_out f32[B][n_frames * hop] (device) */
 int dfb_stream_process(dfb_stream *s, const float *d_in, int64_t n_frames, float *d_out, void *stream);
-/* end of stream: the latency frames still in flight, d_out f32[B][latency * hop]; reset before feeding again */
+/* end of stream: the latency frames still in flight, d_out f32[B][latency * hop]; closes every open slot (below), so
+ * afterwards every slot is free until it is opened or the handle is reset */
 int dfb_stream_flush(dfb_stream *s, float *d_out, void *stream);
-/* host pointers, synchronous; h_in == NULL flushes into h_out f32[B][latency * hop] */
+/* host pointers, synchronous; h_in == NULL flushes into h_out f32[B][latency * hop] (may be NULL when latency is 0) */
 int dfb_stream_process_host(dfb_stream *s, const float *h_in, int64_t n_frames, float *h_out);
+
+/* Streaming slots: each of a handle's B slots is one stream that starts and ends on its own (a service opens a slot when
+ * a call starts, as capi.rs df_create, and closes it when the call ends, as df_free).  At creation and after
+ * dfb_stream_reset every slot is open.  Slot operations take effect at the next process / flush call; `slots` is a HOST
+ * array of n slot indices, each in [0, B) and listed once (DFB_ERR_INVALID otherwise).
+ *   open:  each listed slot starts a new stream from the initial state, exactly as a fresh handle would; an open or
+ *          closing slot's old stream is dropped without its tail.
+ *   close: each listed open slot's stream ends after the input it has already been fed.  From the next call on its input
+ *          rows are ignored, and over the next dfb_stream_latency_frames() hops its output rows carry what
+ *          dfb_stream_flush would give that stream alone, whatever the call sizes; then the slot is free (at once when
+ *          the latency is 0).  Closing a slot that is not open does nothing.
+ *   free:  not computed; its input rows are ignored and its output rows are zeros.
+ * Row b of process / flush is slot b.  Every session's output equals a single-stream handle fed the same audio in the
+ * same call sizes and then flushed.  Only open and closing slots are computed, so the cost of a call follows the number
+ * of live streams, not B.  Linked channels (dfb_stream_set_mask_reduce) and slots do not combine: DFB_ERR_UNSUPPORTED.
+ * The handle's clock counts frames since create / reset; slot operations need it below 2^31 - 2 frames (248 days). */
+int dfb_stream_open_slots(dfb_stream *s, const int64_t *slots, int64_t n);
+int dfb_stream_close_slots(dfb_stream *s, const int64_t *slots, int64_t n);
+/* h_states i32[B] (host): 0 free, 1 open, 2 closing */
+int dfb_stream_slot_states(const dfb_stream *s, int32_t *h_states);
 
 /* Chunk pipeline of dfb_enhance (device_chunks) / dfb_enhance_host (host_chunks): a signal of >= 64 * chunks frames is cut
  * into at least that many time chunks; lanes = 2 overlaps the encoder phase of chunk c + 1 with the decoder phase (the
