@@ -8,7 +8,10 @@ default).  Reported per model and call size:
   * device time per call (CUDA events around each process call, which includes the slot bookkeeping of that call),
     p50 and p99;
   * useful audio-s/s: audio of the open sessions per second of device time;
-  * the same traffic with all 256 slots computed on every call (no slot operations: the only option before slots).
+  * the same traffic with all 256 slots computed on every call (no slot operations: the only option before slots);
+  * the same traffic with per-session settings ("controls"): every session gets its own random attenuation limit
+    (6-40 dB) and post-filter beta (0-0.05) when it opens, about 2 % of the calls change one live slot's settings, and
+    every call asks for the LSNR of its output hops.
 Prints one JSON line, with the card's name, power limit and SM clock read in the same run.
 
     python bench_slots.py [--slots 256] [--calls 400] [--hops 1 10] [--warmup 20]
@@ -64,25 +67,48 @@ def run(name: str, slots: int, calls: int, hops: int, warmup: int, seed: int):
     model = DfNet(cfg, random_state_dict(cfg, seed=1), st)
     x = torch.randn(slots, hops * HOP, device="cuda") * 0.1
     start, plan = traffic(slots, calls, hops, seed)
+    rng = np.random.default_rng(seed + 1)
+    setting = lambda: (float(rng.uniform(6, 40)), float(rng.uniform(0, 0.05)))   # (atten_lim_db, beta) of a session
+    start_set = [setting() for _ in start]
+    open_set = [[setting() for _ in opens] for _, opens, _ in plan]
+    change = [(rng.random() < 0.02, rng.random(), setting()) for _ in plan]        # (change?, which live slot, to what)
     res = {}
-    for mode in ("slots", "all_computed"):
+    for mode in ("slots", "all_computed", "controls"):
         s = DfStream(model, st, batch=slots)
         for _ in range(warmup):
             s.process(x)
         s.reset()
-        if mode == "slots":   # the steady state the plan starts from: flush frees every slot, then half of them open
+        live = set()
+        if mode != "all_computed":   # the steady state the plan starts from: flush frees every slot, then half of them open
             s.flush()
             s.open(start)
+            live = set(start)
+        if mode == "controls":
+            for b, (db, beta) in zip(start, start_set):
+                s.set_atten_lim(db, [b])
+                s.set_post_filter_beta(beta, [b])
         ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in plan]
         torch.cuda.synchronize()
-        for (closes, opens, _), (e0, e1) in zip(plan, ev):
+        for (closes, opens, _), (e0, e1), sets, (chg, which, to) in zip(plan, ev, open_set, change):
             e0.record()
-            if mode == "slots":
+            if mode != "all_computed":
                 if closes:
                     s.close(closes)
                 if opens:
                     s.open(opens)
-            s.process(x)
+                live.difference_update(closes)
+                live.update(opens)
+            if mode == "controls":
+                for b, (db, beta) in zip(opens, sets):
+                    s.set_atten_lim(db, [b])
+                    s.set_post_filter_beta(beta, [b])
+                if chg and live:
+                    b = sorted(live)[int(which * len(live))]
+                    s.set_atten_lim(to[0], [b])
+                    s.set_post_filter_beta(to[1], [b])
+                s.process(x, return_lsnr=True)
+            else:
+                s.process(x)
             e1.record()
         torch.cuda.synchronize()
         ms = np.array([a.elapsed_time(b) for a, b in ev])
@@ -92,6 +118,7 @@ def run(name: str, slots: int, calls: int, hops: int, warmup: int, seed: int):
         del s
     res["mean_open_slots"] = float(np.mean([live for _, _, live in plan]))
     res["speedup_useful"] = res["slots"]["useful_audio_s_per_s"] / res["all_computed"]["useful_audio_s_per_s"]
+    res["controls_vs_slots_useful"] = res["controls"]["useful_audio_s_per_s"] / res["slots"]["useful_audio_s_per_s"]
     return res
 
 
@@ -112,7 +139,8 @@ def main():
         for hops in a.hops:
             calls = a.calls if hops == 1 else max(a.calls // hops, 40)
             rows[f"{name}/{hops}hop"] = run(name, a.slots, calls, hops, a.warmup, a.seed)
-    print(json.dumps({"metric": "serving simulation, streaming slots vs every slot computed", "weights": "random (seed 1)",
+    print(json.dumps({"metric": "serving simulation, streaming slots vs every slot computed vs slots with per-session "
+                                "settings and LSNR output", "weights": "random (seed 1)",
                       "card": before, "card_after": card(), "slots": a.slots, "session_s": [2, 30], "results": rows}))
 
 

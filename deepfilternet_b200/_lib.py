@@ -102,6 +102,11 @@ SIGNATURES = {
     "dfb_stream_open_slots": (_I, [_VP, _I64P, _I64]),
     "dfb_stream_close_slots": (_I, [_VP, _I64P, _I64]),
     "dfb_stream_slot_states": (_I, [_VP, C.POINTER(C.c_int32)]),
+    "dfb_stream_set_atten_lim": (_I, [_VP, _I64P, _I64, _F]),
+    "dfb_stream_set_post_filter_beta": (_I, [_VP, _I64P, _I64, _F]),
+    "dfb_stream_process_lsnr": (_I, [_VP, _VP, _I64, _VP, _VP, _VP]),
+    "dfb_stream_flush_lsnr": (_I, [_VP, _VP, _VP, _VP]),
+    "dfb_stream_process_host_lsnr": (_I, [_VP, _VP, _I64, _VP, _VP]),
     "dfb_model_set_max_workspace": (_I, [_VP, _I64]),
     "dfb_model_set_options": (_I, [_VP, _I, _F, _I]),
     "dfb_model_set_chunking": (_I, [_VP, _I, _I, _I]),

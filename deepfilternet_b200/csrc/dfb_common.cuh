@@ -130,6 +130,10 @@ struct RaggedRow { int64_t in_off, len, out_off, out_len, Tf; };
 // ERB mask.  A separate table rather than more RaggedRow fields: the analysis and input-conv kernels read RaggedRow.
 struct LinkRow { int first, n; };
 enum { kReduceNone = 0, kReduceMax = 1, kReduceMean = 2 };   // dfb_reduce_mask
+// Per-slot settings of a streaming handle (dfb_stream_set_atten_lim / _post_filter_beta): limit (0 = off) and post-filter
+// beta (0 = off) from absolute frame sw on, and the previous ones before it.  Only the frame before sw, re-synthesised
+// for its overlap-add tail, still reads the previous ones.
+struct SlotCtl { float lim, beta, lim0, beta0; int64_t sw; };
 
 // Streaming slots (dfb_stream_open_slots): `first` holds the absolute first frame of each stream of a launch, or is null.
 // Window frame t (absolute w0 + t) of stream b exists from the returned window frame on; the kernels that look back in
@@ -220,7 +224,11 @@ int launch_feat_norm(const float *d_erb, int E, int64_t erb_stride, const float 
                      int64_t C, int64_t Tf, float alpha, const float *d_erb_state, const float *d_unit_state,
                      float *d_feat_erb, float *d_feat_spec, cudaStream_t s, int64_t Ts = 0, float *d_erb_state_out = nullptr,
                      float *d_unit_state_out = nullptr, bool ref_bits = false);
-int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaStream_t s);
+// ctl (or null): per-stream settings of streaming slots (SlotCtl; specialised RG kernel only).  Stream b's attenuation limit
+// and DeepFilterNet3 post-filter beta are ctl[b].lim / beta for absolute frames >= ctl[b].sw and lim0 / beta0 before it,
+// in place of p.atten_lim / pf / pf_beta.  A kernel argument of its own after ApplyParams, so that the parameter layout
+// of the other instantiations stays as it was.
+int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaStream_t s, const SlotCtl *ctl = nullptr);
 // time window of a recurrence launch: steps 0 .. T-1 are frames t0 .. of buffers holding Ts frames per stream; h0 (null:
 // zeros) / hT (null: not stored) are the carried hidden states [B][H]
 struct GruWindow { const float *h0; float *hT; int t0, Ts; const int64_t *first = nullptr; int64_t w0 = 0; /* stream_first */ };

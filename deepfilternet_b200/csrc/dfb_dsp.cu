@@ -687,8 +687,10 @@ __global__ void __launch_bounds__(32 * kSynWarps) k_apply_synthesis_generic(Appl
 // LINK: linked channels (p.links), likewise separate.  The mask of a frame is reduced over the link group where it is
 // loaded: lane e reads row e of each member's mask and reduces in registers, so the shared mask never reaches HBM and
 // the unlinked instantiations are untouched.
-template <int ORDER, int NDFJ, int MINB, bool RG, bool LINK = false>
-__global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyParams p, DspTables tb) {
+// CTL: per-stream attenuation limit and post-filter beta (p.ctl, streaming slots), likewise separate.  Each frame picks
+// the row's new or previous setting by its absolute frame against the row's switch frame.
+template <int ORDER, int NDFJ, int MINB, bool RG, bool LINK = false, bool CTL = false>
+__global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyParams p, DspTables tb, const SlotCtl *ctl_tab) {
     __shared__ __align__(16) float s_win[kFft];
     __shared__ __align__(16) float2 s_tw960[241];
     __shared__ __align__(16) float2 s_buf[kSynWarps][kTileFloat2];
@@ -740,9 +742,11 @@ __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyP
         }
     };
     const bool masked_df = p.mode == 2 && !p.mask_only;
-    const bool pf1 = p.pf && p.mode == 1, pf2 = p.pf && p.mode == 2;
+    // CTL: this row's settings (either of its two) in place of the handle's limit and DeepFilterNet3 post filter
+    const SlotCtl ctl = CTL ? ctl_tab[b] : SlotCtl{};
+    const bool pf1 = CTL ? p.mode == 1 && (ctl.beta > 0.f || ctl.beta0 > 0.f) : p.pf && p.mode == 1, pf2 = p.pf && p.mode == 2;
     const bool blend = p.alpha != nullptr && masked_df;   // DeepFilterNet v1: alpha blend with the masked bin
-    const bool need_xk = p.atten_lim > 0.f || pf1 || p.mask_only || p.lsnr || blend;   // noisy DF bins are only loaded when something reads them
+    const bool need_xk = (CTL ? ctl.lim > 0.f || ctl.lim0 > 0.f : p.atten_lim > 0.f) || pf1 || p.mask_only || p.lsnr || blend;   // noisy DF bins are only loaded when something reads them
     // bands of this lane's bins: bk[j] for k = lane + 32 j, bn[j] for 480 - k
     unsigned long long bkp = 0, bnp = 0;  // 8 band indices each, one byte per j
 #pragma unroll
@@ -788,6 +792,9 @@ __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyP
             stage = l < p.th_min ? 0 : (l > p.th_erb ? 1 : (l > p.th_df ? 2 : 3));
         }
         if (RG && t < t_zero) stage = 0;   // zero gains, no deep filter: the stream has not started
+        // CTL: the setting frame t was output with; the frame before the switch is only re-synthesised for its tail
+        const bool now = CTL && p.w0 + t >= ctl.sw;
+        const float lim = now ? ctl.lim : ctl.lim0, beta = now ? ctl.beta : ctl.beta0;
 #pragma unroll
         for (int o = 0; o < ORDER - 1; o++)
 #pragma unroll
@@ -833,12 +840,12 @@ __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyP
             float2 yn = make_float2(xn[j].x * gn, xn[j].y * gn);
             if (stage == 0) { y = make_float2(0.f, 0.f); yn = y; }
             else if (stage == 1) { y = xk[j]; yn = xn[j]; }
-            if (pf1 && stage >= 2) {
-                const float g1 = pf_gain_spec(y, xk[j], p.pf_beta), g2 = pf_gain_spec(yn, xn[j], p.pf_beta);
+            if ((CTL ? p.mode == 1 && beta > 0.f : pf1) && stage >= 2) {
+                const float g1 = pf_gain_spec(y, xk[j], CTL ? beta : p.pf_beta), g2 = pf_gain_spec(yn, xn[j], CTL ? beta : p.pf_beta);
                 y.x *= g1; y.y *= g1; yn.x *= g2; yn.y *= g2;
             }
-            if (p.atten_lim > 0.f) {
-                const float a = p.atten_lim, c = 1.f - a;
+            if (CTL ? lim > 0.f : p.atten_lim > 0.f) {
+                const float a = CTL ? lim : p.atten_lim, c = 1.f - a;
                 y.x = xk[j].x * a + y.x * c; y.y = xk[j].y * a + y.y * c;
                 yn.x = xn[j].x * a + yn.x * c; yn.y = xn[j].y * a + yn.y * c;
             }
@@ -1133,7 +1140,7 @@ int launch_feat_norm(const float *d_erb, int E, int64_t erb_stride, const float 
     return DFB_OK;
 }
 
-int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaStream_t s) {
+int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaStream_t s, const SlotCtl *ctl) {
     if (B <= 0 || p.Tf <= 0) return DFB_OK;
     if (B > 65535) return fail(DFB_ERR_INVALID, "more than 65535 channels per call");
     if (p.mode != 0 && (p.nb_df > 240 || p.order > 8)) return fail(DFB_ERR_UNSUPPORTED, "nb_df > 240 or df_order > 8");
@@ -1148,16 +1155,20 @@ int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaS
     const bool special = p.mode != 0 && p.order == 5 && p.nb_df == 96 && st->tb.E == 32 && p.m && p.coefs;
     if (p.links && !special) return fail(DFB_ERR_UNSUPPORTED, "linked channels are built for the specialised apply kernel only");
     if (p.links && p.reduce != kReduceMax && p.reduce != kReduceMean) return fail(DFB_ERR_INVALID, "bad mask reduction %d", p.reduce);
+    if (ctl && !(special && p.rows && !p.links))
+        return fail(DFB_ERR_UNSUPPORTED, "per-stream settings are built for the specialised slot apply kernel only");
     DFB_PROF("k_apply_synthesis", s);
     // MINB 2: 2 CTAs/SM without spills measured fastest
-    if (p.links && p.rows)
-        k_apply_synthesis<5, 3, 2, true, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
+    if (ctl)
+        k_apply_synthesis<5, 3, 2, true, false, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, ctl);
+    else if (p.links && p.rows)
+        k_apply_synthesis<5, 3, 2, true, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, nullptr);
     else if (p.links)
-        k_apply_synthesis<5, 3, 2, false, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
+        k_apply_synthesis<5, 3, 2, false, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, nullptr);
     else if (special && p.rows)
-        k_apply_synthesis<5, 3, 2, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
+        k_apply_synthesis<5, 3, 2, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, nullptr);
     else if (special)
-        k_apply_synthesis<5, 3, 2, false><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
+        k_apply_synthesis<5, 3, 2, false><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, nullptr);
     else
         k_apply_synthesis_generic<<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
     DFB_LAUNCH_CHECK();

@@ -1589,7 +1589,35 @@ struct ChunkIO {
     // streaming slots (dfb_stream_open_slots): rows are the handle's active slots, rows[b].Tf the end of a closing one, and
     // first[b] the absolute first frame of each; emission follows the handle's clock, clipped at each stream's end.  Or null.
     const int64_t *first = nullptr;
+    // streaming slots: per-row attenuation limit and post-filter beta (launch_apply_synthesis), or null
+    const SlotCtl *ctl = nullptr;
+    // streaming LSNR output: lsnr_from >= 0 runs the LSNR head (as gating does) and carries its tail; lsnr_out (or null)
+    // [rows][out_len / hop] receives the LSNR of every frame the apply kernel emits whose DNN step ran from lsnr_from on,
+    // at the hop that carries it.  Entries of hops that carry no frame are left as they are.
+    int64_t lsnr_from = -1;
+    float *lsnr_out = nullptr;
 };
+
+// LSNR of the frames the apply kernel emitted in this chunk, by the kernel's own emission rule: output hop j of row b
+// carries window frame t = f0 + j - w0, which was emitted when t_first <= t < Te (with rows: Te clipped at the stream's
+// end rows[b].Tf) and the stream had started (stream_first).  Frames whose DNN step ran before `from` have no LSNR.
+__global__ void k_lsnr_out(const float *__restrict__ ll, int mcT, float *__restrict__ out, int64_t n_out, int64_t f0, int64_t w0,
+                           int t_first, int Te, const RaggedRow *__restrict__ rows, const int64_t *__restrict__ first, int64_t from,
+                           int hop) {
+    const int b = blockIdx.y;
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n_out) return;
+    int64_t o = (int64_t)b * n_out;
+    int te = Te;
+    if (rows) {
+        te = min(te, (int)(rows[b].Tf - w0));
+        o = rows[b].out_off / hop;
+    }
+    int64_t t0 = max(t_first, stream_first(first, b, w0));
+    if (from - w0 > t0) t0 = from - w0;
+    const int64_t t = f0 + j - w0;
+    if (t >= t0 && t < te) out[o + j] = ll[(int64_t)b * mcT + t];
+}
 
 // One chunk: analyse frames [S.a1, a1n), run the DNN over [S.d1, d1n), emit audio of frames [S.e1, e1n).
 // Ragged batch (io.rows): only the first io.nb streams run; a stream whose frame count Tf_b is <= d1n ends in this chunk:
@@ -1621,7 +1649,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     float *fs = arena.take<float>((size_t)B * Tsb * Fd * 2);
     float *mm = arena.take<float>((size_t)B * (Tw + 1) * E);
     float *cc = arena.take<float>((size_t)B * (Tw + 1) * Fd * O2);
-    float *ll = io.lsnr_th ? arena.take<float>((size_t)B * (Tw + 1)) : nullptr;
+    float *ll = (io.lsnr_th || io.lsnr_from >= 0) ? arena.take<float>((size_t)B * (Tw + 1)) : nullptr;
     float *aa = c.model_kind == 1 ? arena.take<float>((size_t)B * (Tw + 1)) : nullptr;   // df_alpha (v1)
     if (!cc || (c.model_kind == 1 && !aa)) return fail(DFB_ERR_OOM, "chunk workspace exhausted");
     // ---- features: carried history, then the new frames
@@ -1674,11 +1702,18 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
         p.atten_lim = io.atten_lim;
         p.alpha = aa;
         apply_options(m, p);
-        if (ll) { p.lsnr = ll; p.th_min = io.lsnr_th[0]; p.th_erb = io.lsnr_th[1]; p.th_df = io.lsnr_th[2]; }
+        if (io.lsnr_th) { p.lsnr = ll; p.th_min = io.lsnr_th[0]; p.th_erb = io.lsnr_th[1]; p.th_df = io.lsnr_th[2]; }
         if (io.rows) { p.rows = io.rows; p.w0 = W0; p.t_emit = p.Tf; p.first = io.first; }
         if (io.rows && !io.first) p.Tf = Tw;   // batch: the grid covers every stream's end; slots: Te = min(end, clock)
         if (io.links) { p.links = io.links; p.reduce = io.reduce; }
-        if ((rc = launch_apply_synthesis(st, p, B, s))) return rc;
+        if ((rc = launch_apply_synthesis(st, p, B, s, io.ctl))) return rc;
+        if (io.lsnr_out && e1n > S.e1) {
+            const int64_t n_out = io.out_len / hop;
+            dim3 grid((unsigned)((n_out + 127) / 128), (unsigned)B);
+            k_lsnr_out<<<grid, 128, 0, s>>>(ll, Tw, io.lsnr_out, n_out, io.out_sample0 / hop, W0, p.t_first, (int)(e1n - W0), io.rows,
+                                            io.first, io.lsnr_from, hop);
+            DFB_LAUNCH_CHECK();
+        }
     }
     // ---- carry
     {
@@ -2197,7 +2232,24 @@ struct dfb_stream {
     int64_t tab_n = -1;                                // ... for calls of this many input hops
     RaggedRow *d_rows = nullptr;
     int64_t *d_first = nullptr;
+    // per-slot settings (dfb_stream_set_atten_lim / _post_filter_beta).  ctl_on: a setter has run since create / reset, so
+    // the slot path passes the per-row table to the apply kernel.
+    bool ctl_on = false;
+    std::vector<float> slot_lim, slot_beta;            // per slot: own limit (linear, 0 off) / beta, or NaN: the handle's
+    std::vector<char> slot_fresh;                      // per slot: opened since the last call (no previous setting)
+    std::vector<SlotCtl> slot_ctl;                     // per slot: the settings of the last call and the one before
+    std::vector<SlotCtl> ctl_up;                       // per row: the table on the device
+    SlotCtl *d_ctl = nullptr;
+    float beta_run = 0.f;                              // the handle's default beta at the last call
+    // LSNR output: computed for DNN frames >= lsnr_from, the first one after the first request since create / reset
+    int64_t lsnr_from = -1;
+    float *stage_lsnr = nullptr;                       // device staging of dfb_stream_process_host_lsnr
+    size_t stage_lsnr_cap = 0;
 };
+
+// the handle's default post-filter beta: the model's option (0 = off) for DeepFilterNet3; per-row beta is not used for
+// DeepFilterNet2, whose post filter acts on the ERB gains with a fixed beta
+static float default_beta(const dfb_model *m) { return (m->cfg.model_kind == 3 && m->post_filter) ? m->pf_beta : 0.f; }
 
 extern "C" int dfb_stream_create(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B, float atten_lim_db) {
     if (!out || !m || !st || B <= 0 || B > 65535) return fail(DFB_ERR_INVALID, "bad argument");
@@ -2214,6 +2266,7 @@ extern "C" int dfb_stream_create(dfb_stream **out, dfb_model *m, dfb_state *st, 
     if (cudaMalloc(&h->slab, n * sizeof(float)) != cudaSuccess) { delete h; return fail(DFB_ERR_OOM, "stream state allocation failed"); }
     cudaMemset(h->slab, 0, n * sizeof(float));
     state_bind(h->S, h->slab, off, (int)B);
+    h->beta_run = default_beta(m);
     *out = h;
     return DFB_OK;
 }
@@ -2227,6 +2280,8 @@ extern "C" void dfb_stream_free(dfb_stream *h) {
     if (h->links) cudaFree(h->links);
     if (h->d_rows) cudaFree(h->d_rows);
     if (h->d_first) cudaFree(h->d_first);
+    if (h->d_ctl) cudaFree(h->d_ctl);
+    if (h->stage_lsnr) cudaFree(h->stage_lsnr);
     delete h;
 }
 
@@ -2238,6 +2293,8 @@ extern "C" int dfb_stream_reset(dfb_stream *h) {
     h->fed = false;
     h->slots = false;
     h->pend.clear();
+    h->ctl_on = false;
+    h->lsnr_from = -1;
     return DFB_OK;
 }
 
@@ -2304,6 +2361,11 @@ static int slots_enable(dfb_stream *h) {
     h->n_act = h->B;
     h->pend.clear();
     h->tab_dirty = true;
+    h->slot_lim.assign(B, NAN);
+    h->slot_beta.assign(B, NAN);
+    h->slot_fresh.assign(B, 0);
+    h->slot_ctl.assign(B, SlotCtl{});
+    h->ctl_on = false;
     h->slots = true;
     return DFB_OK;
 }
@@ -2342,7 +2404,7 @@ static void slots_close_all(dfb_stream *h) {
     slots_retire(h, h->S.a1 - dfb_stream_latency_frames(h));
 }
 
-static int slot_list(dfb_stream *h, const int64_t *slots, int64_t n) {
+static int slot_list_check(const dfb_stream *h, const int64_t *slots, int64_t n) {
     if (!h || n < 0 || (n > 0 && !slots)) return fail(DFB_ERR_INVALID, "bad argument");
     if (h->links) return fail(DFB_ERR_UNSUPPORTED, "slot operations on a handle with linked channels");
     std::vector<char> seen((size_t)h->B, 0);
@@ -2352,6 +2414,11 @@ static int slot_list(dfb_stream *h, const int64_t *slots, int64_t n) {
         if (seen[(size_t)b]) return fail(DFB_ERR_INVALID, "slot %lld listed twice", (long long)b);
         seen[(size_t)b] = 1;
     }
+    return DFB_OK;
+}
+
+static int slot_list(dfb_stream *h, const int64_t *slots, int64_t n) {
+    if (int rc = slot_list_check(h, slots, n)) return rc;
     return slots_enable(h);
 }
 
@@ -2369,6 +2436,8 @@ extern "C" int dfb_stream_open_slots(dfb_stream *h, const int64_t *slots, int64_
         h->slot_state[(size_t)b] = kSlotOpen;
         h->slot_first[(size_t)b] = h->S.a1;
         h->slot_end[(size_t)b] = kOpenEnd;
+        h->slot_lim[(size_t)b] = h->slot_beta[(size_t)b] = NAN;   // back to the handle's settings
+        h->slot_fresh[(size_t)b] = 1;
     }
     h->tab_dirty = true;
     return DFB_OK;
@@ -2381,6 +2450,72 @@ extern "C" int dfb_stream_close_slots(dfb_stream *h, const int64_t *slots, int64
     return DFB_OK;
 }
 
+// ---- per-slot settings.  A setting is stored per slot; each call resolves every live slot's setting (its own, or the
+// handle's default at that call) and, when it differs from the one of the slot's last call, switches at the call's first
+// output frame f0: frame f0 - 1, which the apply kernel re-synthesises for its overlap-add tail, keeps the previous one.
+static int ctl_set(dfb_stream *h, const int64_t *slots, int64_t n, bool beta, float v) {
+    if (int rc = slot_list_check(h, slots, n)) return rc;
+    const dfb_model_config &c = h->m->cfg;
+    if (c.df_order != 5 || c.nb_df != 96 || c.nb_erb != 32)
+        return fail(DFB_ERR_UNSUPPORTED, "per-slot settings are built for df_order 5, nb_df 96 and 32 ERB bands");
+    if (beta && c.model_kind != 3)
+        return fail(DFB_ERR_UNSUPPORTED, "per-slot post-filter beta: DeepFilterNet3 topologies only (DeepFilterNet2's beta is fixed)");
+    if (std::isnan(v) || (beta && !(v >= 0.f && std::isfinite(v))))
+        return fail(DFB_ERR_INVALID, beta ? "post-filter beta must be finite and >= 0" : "attenuation limit is NaN");
+    for (int64_t i = 0; i < n; i++)
+        if (h->slots && h->slot_state[(size_t)slots[i]] == kSlotFree)
+            return fail(DFB_ERR_INVALID, "slot %lld is free", (long long)slots[i]);
+    if (n == 0) return DFB_OK;
+    if (int rc = slots_enable(h)) return rc;
+    if (!h->ctl_on) {
+        if (!h->d_ctl) {
+            DFB_CUDA(cudaSetDevice(h->m->device));
+            if (cudaMalloc(&h->d_ctl, sizeof(SlotCtl) * (size_t)h->B) != cudaSuccess) {
+                h->d_ctl = nullptr;
+                return fail(DFB_ERR_OOM, "slot settings allocation failed");
+            }
+        }
+        // every slot has run with the handle's settings so far
+        for (int b = 0; b < h->B; b++) h->slot_ctl[(size_t)b] = SlotCtl{h->lim, h->beta_run, h->lim, h->beta_run, 0};
+        std::fill(h->slot_fresh.begin(), h->slot_fresh.end(), (char)0);
+        h->ctl_up.clear();
+        h->ctl_on = true;
+    }
+    std::vector<float> &dst = beta ? h->slot_beta : h->slot_lim;
+    for (int64_t i = 0; i < n; i++) dst[(size_t)slots[i]] = v;
+    return DFB_OK;
+}
+
+extern "C" int dfb_stream_set_atten_lim(dfb_stream *h, const int64_t *slots, int64_t n, float atten_lim_db) {
+    const float lim = std::isnan(atten_lim_db) ? NAN : (atten_lim_db > 0.f ? powf(10.f, -atten_lim_db / 20.f) : 0.f);
+    return ctl_set(h, slots, n, false, lim);
+}
+
+extern "C" int dfb_stream_set_post_filter_beta(dfb_stream *h, const int64_t *slots, int64_t n, float beta) {
+    return ctl_set(h, slots, n, true, beta);
+}
+
+// the per-row settings of a call whose first output hop carries frame f0; uploaded when they differ from the last upload
+static int ctl_rows(dfb_stream *h, int64_t f0, cudaStream_t s) {
+    const float beta_def = default_beta(h->m);
+    std::vector<SlotCtl> rows((size_t)h->n_act);
+    for (int r = 0; r < h->n_act; r++) {
+        const size_t b = (size_t)h->row_slot[(size_t)r];
+        const float lim = std::isnan(h->slot_lim[b]) ? h->lim : h->slot_lim[b];
+        const float beta = std::isnan(h->slot_beta[b]) ? beta_def : h->slot_beta[b];
+        SlotCtl &c = h->slot_ctl[b];
+        if (h->slot_fresh[b]) { c = SlotCtl{lim, beta, lim, beta, f0}; h->slot_fresh[b] = 0; }
+        else if (lim != c.lim || beta != c.beta) c = SlotCtl{lim, beta, c.lim, c.beta, f0};
+        rows[(size_t)r] = c;
+    }
+    if (rows.size() != h->ctl_up.size() || memcmp(rows.data(), h->ctl_up.data(), sizeof(SlotCtl) * rows.size())) {
+        if (!rows.empty())
+            DFB_CUDA(cudaMemcpyAsync(h->d_ctl, rows.data(), sizeof(SlotCtl) * rows.size(), cudaMemcpyHostToDevice, s));
+        h->ctl_up.swap(rows);
+    }
+    return DFB_OK;
+}
+
 extern "C" int dfb_stream_slot_states(const dfb_stream *h, int32_t *h_states) {
     if (!h || !h_states) return fail(DFB_ERR_INVALID, "null argument");
     for (int b = 0; b < h->B; b++) h_states[b] = h->slots ? h->slot_state[(size_t)b] : kSlotOpen;
@@ -2388,7 +2523,7 @@ extern "C" int dfb_stream_slot_states(const dfb_stream *h, int32_t *h_states) {
 }
 
 // Slot path of one call: rows [0, n_act) of the slab, the row table for calls of n input hops, output rows zero first.
-static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, cudaStream_t s) {
+static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s) {
     dfb_model *m = h->m;
     dfb_state *st = h->st;
     StreamState &S = h->S;
@@ -2397,6 +2532,7 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
     const int64_t Ltot = g.Lmax + g.lag, n_out = flush ? Ltot : n;
     const int64_t a0 = S.a1, a1n = a0 + (flush ? 0 : n);
     if (a1n >= kOpenEnd - 1) return fail(DFB_ERR_UNSUPPORTED, "stream clock beyond 2^31 - 2 frames: reset the stream");
+    int rc = DFB_OK;
     int64_t d1n = flush ? a1n : a1n - g.Lmax, e1n = flush ? a1n : d1n - g.lag;
     if (d1n < S.d1) d1n = S.d1;
     if (e1n < S.e1) e1n = S.e1;
@@ -2428,6 +2564,10 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
         h->tab_n = n;
     }
     if (n_out > 0) DFB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * B * n_out * hop, s));   // free slots; frames outside a stream
+    if (d_lsnr && n_out > 0) DFB_CUDA(cudaMemsetAsync(d_lsnr, 0xff, sizeof(float) * B * n_out, s));   // NaN: hops without a frame
+    const int64_t f0 = a0 - Ltot;   // output hop j carries frame a0 - Ltot + j (flush: a1 = a0)
+    if (h->ctl_on && (rc = ctl_rows(h, f0, s))) return rc;
+    h->beta_run = default_beta(m);
     h->fed = true;
     if (h->n_act == 0) {   // nothing to compute: the clock moves on (a slot opened later starts from zeroed tails)
         S.a1 = a1n; S.d1 = d1n; S.e1 = e1n;
@@ -2437,11 +2577,13 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
         slots_retire(h, flush ? a1n : a1n - Ltot);
         return DFB_OK;
     }
-    const int64_t f0 = a0 - Ltot;   // output hop j carries frame a0 - Ltot + j (flush: a1 = a0)
     ChunkIO io{d_in, n * hop, n * hop, a0, nullptr, d_out, n_out * hop, n_out * hop, f0 * hop, h->lim, h->gating ? h->th : nullptr,
                h->d_rows, h->n_act};
     io.first = h->d_first;
-    int rc = m->arena.reserve(chunk_bytes_per_stream(m->cfg, st, (int)(d1n - (S.d1 > kHalo ? S.d1 - kHalo : 0)) + 1) * (size_t)h->n_act +
+    if (h->ctl_on) io.ctl = h->d_ctl;
+    io.lsnr_from = h->lsnr_from;
+    io.lsnr_out = d_lsnr;
+    rc = m->arena.reserve(chunk_bytes_per_stream(m->cfg, st, (int)(d1n - (S.d1 > kHalo ? S.d1 - kHalo : 0)) + 1) * (size_t)h->n_act +
                               (2 << 20));
     if (rc) return rc;
     if (!flush && a1n > a0) {
@@ -2458,8 +2600,9 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
     return DFB_OK;
 }
 
-static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, cudaStream_t s) {
-    if (h->slots) return slots_step(h, d_in, n, flush, d_out, s);
+static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s) {
+    if (d_lsnr && h->lsnr_from < 0) h->lsnr_from = h->S.d1;   // from now on every call runs the LSNR head
+    if (h->slots) return slots_step(h, d_in, n, flush, d_out, d_lsnr, s);
     dfb_model *m = h->m;
     dfb_state *st = h->st;
     StreamState &S = h->S;
@@ -2479,10 +2622,14 @@ static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, 
     // output slot j (hop j of d_out) carries frame a0 - Ltot + j (flush: a1 - Ltot + j); frames < 0 are silence
     const int64_t f0 = (flush ? S.a1 : a0) - Ltot;
     if (f0 < 0 || e1n <= S.e1) DFB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * B * n_out * hop, s));
+    if (d_lsnr && n_out > 0) DFB_CUDA(cudaMemsetAsync(d_lsnr, 0xff, sizeof(float) * B * n_out, s));   // NaN: hops without a frame
     ChunkIO io{d_in, (flush ? 0 : n) * hop, (flush ? 0 : n) * hop, a0, S.started ? S.ana_mem : nullptr, d_out, n_out * hop, n_out * hop,
                f0 * hop, h->lim, h->gating ? h->th : nullptr};
     io.links = h->links;
     io.reduce = h->reduce;
+    io.lsnr_from = h->lsnr_from;
+    io.lsnr_out = d_lsnr;
+    h->beta_run = default_beta(m);
     h->fed = true;
     if (!flush && a1n > a0) {
         // zero analysis memory before the very first frame
@@ -2508,27 +2655,33 @@ static void flushed_all(dfb_stream *h) {
     h->n_act = 0;
 }
 
-// d_in [B][n_frames * hop] -> d_out [B][n_frames * hop] (device pointers, asynchronous on `stream`)
-extern "C" int dfb_stream_process(dfb_stream *h, const float *d_in, int64_t n_frames, float *d_out, void *stream) {
+// d_in [B][n_frames * hop] -> d_out [B][n_frames * hop] (device pointers, asynchronous on `stream`); d_lsnr (or null)
+// [B][n_frames]: the LSNR of the frame each output hop carries, NaN where it carries none
+extern "C" int dfb_stream_process_lsnr(dfb_stream *h, const float *d_in, int64_t n_frames, float *d_out, float *d_lsnr, void *stream) {
     if (!h || !d_in || !d_out || n_frames <= 0) return fail(DFB_ERR_INVALID, "bad argument");
     DFB_CUDA(cudaSetDevice(h->m->device));
-    return stream_step(h, d_in, n_frames, false, d_out, (cudaStream_t)stream);
+    return stream_step(h, d_in, n_frames, false, d_out, d_lsnr, (cudaStream_t)stream);
+}
+extern "C" int dfb_stream_process(dfb_stream *h, const float *d_in, int64_t n_frames, float *d_out, void *stream) {
+    return dfb_stream_process_lsnr(h, d_in, n_frames, d_out, nullptr, stream);
 }
 
 // End of the stream: the `latency` frames still in flight, computed with zero look-ahead exactly like the end of a
 // batch enhance(); d_out [B][latency * hop].  Closes every open slot; on the slot-free path the stream must be reset before
-// it is fed again.
-extern "C" int dfb_stream_flush(dfb_stream *h, float *d_out, void *stream) {
+// it is fed again.  d_lsnr (or null) [B][latency]: the LSNR of the tail frames.
+extern "C" int dfb_stream_flush_lsnr(dfb_stream *h, float *d_out, float *d_lsnr, void *stream) {
     if (!h || !d_out) return fail(DFB_ERR_INVALID, "bad argument");
     DFB_CUDA(cudaSetDevice(h->m->device));
     int rc = DFB_OK;
-    if (dfb_stream_latency_frames(h) > 0) rc = stream_step(h, nullptr, 0, true, d_out, (cudaStream_t)stream);
+    if (dfb_stream_latency_frames(h) > 0) rc = stream_step(h, nullptr, 0, true, d_out, d_lsnr, (cudaStream_t)stream);
     if (!rc) flushed_all(h);
     return rc;
 }
+extern "C" int dfb_stream_flush(dfb_stream *h, float *d_out, void *stream) { return dfb_stream_flush_lsnr(h, d_out, nullptr, stream); }
 
-// host-pointer variant (synchronous): h_in / h_out [B][n_frames * hop]; h_in == NULL flushes into h_out [B][latency * hop]
-extern "C" int dfb_stream_process_host(dfb_stream *h, const float *h_in, int64_t n_frames, float *h_out) {
+// host-pointer variant (synchronous): h_in / h_out [B][n_frames * hop]; h_in == NULL flushes into h_out [B][latency * hop];
+// h_lsnr (or null) [B][n_frames] / [B][latency] as dfb_stream_process_lsnr
+extern "C" int dfb_stream_process_host_lsnr(dfb_stream *h, const float *h_in, int64_t n_frames, float *h_out, float *h_lsnr) {
     if (!h || (h_in && n_frames <= 0)) return fail(DFB_ERR_INVALID, "bad argument");
     DFB_CUDA(cudaSetDevice(h->m->device));
     const bool flush = h_in == nullptr;
@@ -2547,12 +2700,23 @@ extern "C" int dfb_stream_process_host(dfb_stream *h, const float *h_in, int64_t
             return fail(DFB_ERR_OOM, "stream staging allocation failed");
         h->stage_cap = bytes;
     }
+    const size_t lbytes = sizeof(float) * (size_t)h->B * nf;
+    if (h_lsnr && lbytes > h->stage_lsnr_cap) {
+        if (h->stage_lsnr) cudaFree(h->stage_lsnr);
+        h->stage_lsnr = nullptr; h->stage_lsnr_cap = 0;
+        if (cudaMalloc(&h->stage_lsnr, lbytes) != cudaSuccess) return fail(DFB_ERR_OOM, "stream staging allocation failed");
+        h->stage_lsnr_cap = lbytes;
+    }
     cudaStream_t s = h->m->stream;
     if (!flush) DFB_CUDA(cudaMemcpyAsync(h->stage_in, h_in, bytes, cudaMemcpyHostToDevice, s));
-    int rc = stream_step(h, h->stage_in, nf, flush, h->stage_out, s);
+    int rc = stream_step(h, h->stage_in, nf, flush, h->stage_out, h_lsnr ? h->stage_lsnr : nullptr, s);
     if (rc) return rc;
     DFB_CUDA(cudaMemcpyAsync(h_out, h->stage_out, bytes, cudaMemcpyDeviceToHost, s));
+    if (h_lsnr) DFB_CUDA(cudaMemcpyAsync(h_lsnr, h->stage_lsnr, lbytes, cudaMemcpyDeviceToHost, s));
     DFB_CUDA(cudaStreamSynchronize(s));
     if (flush) flushed_all(h);
     return DFB_OK;
+}
+extern "C" int dfb_stream_process_host(dfb_stream *h, const float *h_in, int64_t n_frames, float *h_out) {
+    return dfb_stream_process_host_lsnr(h, h_in, n_frames, h_out, nullptr);
 }

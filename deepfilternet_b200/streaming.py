@@ -13,11 +13,14 @@ The concatenation of the outputs equals ``enhance(model, df_state, audio, pad=Fa
 the channels of recording g and share one ERB mask, the max or mean of theirs (dfb_stream_set_mask_reduce).
 
 Each row is a slot that can start and end its own stream (``open`` / ``close``), so one handle serves calls that come and
-go: a call joins whenever a slot is free, and only open and closing slots are computed.
+go: a call joins whenever a slot is free, and only open and closing slots are computed.  Each slot can change its own
+attenuation limit and post-filter beta between two calls (``set_atten_lim`` / ``set_post_filter_beta``), and
+``process`` / ``flush`` return the local SNR of every output frame on request (``return_lsnr=True``).
 """
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Optional
 
 import numpy as np
@@ -51,6 +54,29 @@ def slot_list(slots, batch: int) -> np.ndarray:
     if (counts > 1).any():
         raise ValueError(f"slot {int(u[counts > 1][0])} listed twice")
     return a
+
+
+def atten_lim_arg(db: Optional[float]) -> float:
+    """``db`` of DfStream.set_atten_lim as the float the C ABI takes: None is 0 (off); NaN and non-numbers are ValueError."""
+    if db is None:
+        return 0.0
+    if isinstance(db, (bool, str)):
+        raise ValueError(f"attenuation limit must be a number of dB, got {db!r}")
+    v = float(db)
+    if math.isnan(v):
+        raise ValueError("attenuation limit is NaN")
+    return v
+
+
+def pf_beta_arg(beta: float) -> float:
+    """``beta`` of DfStream.set_post_filter_beta as a float: finite and >= 0 (0 turns the post filter off), else
+    ValueError."""
+    if isinstance(beta, (bool, str)) or beta is None:
+        raise ValueError(f"post-filter beta must be a number, got {beta!r}")
+    v = float(beta)
+    if not math.isfinite(v) or v < 0:
+        raise ValueError(f"post-filter beta must be finite and >= 0, got {beta}")
+    return v
 
 
 class DfStream:
@@ -112,6 +138,27 @@ class DfStream:
         are not computed and return zeros.  Closing a slot that is not open does nothing."""
         self._slots(_lib.lib().dfb_stream_close_slots, slots)
 
+    def _live_or(self, slots) -> np.ndarray:
+        if slots is None:
+            return np.flatnonzero(self.slot_states() != SLOT_FREE).astype(np.int64)
+        return slot_list(slots, self.batch)
+
+    def set_atten_lim(self, db: Optional[float], slots=None) -> None:
+        """Attenuation limit of the listed slots (None: every open or closing slot) from the next call on: ``db`` <= 0 or
+        None turns it off, else the enhanced spectrum is mixed with 10^(-db / 20) of the noisy one, as ``atten_lim_db`` of
+        the constructor.  The slot's first output hop of that call still carries the previous setting's overlap-add tail.
+        ``open`` returns a slot to the handle's setting; ``reset`` drops every setting (dfb_stream_set_atten_lim)."""
+        v = atten_lim_arg(db)
+        a = self._live_or(slots)
+        check(_lib.lib().dfb_stream_set_atten_lim(self._h, a.ctypes.data_as(C.POINTER(C.c_int64)), a.size, v))
+
+    def set_post_filter_beta(self, beta: float, slots=None) -> None:
+        """DeepFilterNet3 post-filter beta of the listed slots (None: every open or closing slot) from the next call on;
+        finite and >= 0, 0 turns the post filter off.  Not available for DeepFilterNet2 (dfb_stream_set_post_filter_beta)."""
+        v = pf_beta_arg(beta)
+        a = self._live_or(slots)
+        check(_lib.lib().dfb_stream_set_post_filter_beta(self._h, a.ctypes.data_as(C.POINTER(C.c_int64)), a.size, v))
+
     def slot_states(self) -> np.ndarray:
         """int32 [batch]: SLOT_FREE (0), SLOT_OPEN (1) or SLOT_CLOSING (2) per slot.  A new or reset handle has every slot
         open; ``flush`` closes them all."""
@@ -120,8 +167,11 @@ class DfStream:
         return out
 
     @torch.no_grad()
-    def process(self, audio: Tensor) -> Tensor:
-        """audio float32 [B, n * hop] (CPU or the model's CUDA device) -> enhanced [B, n * hop] on the same device."""
+    def process(self, audio: Tensor, return_lsnr: bool = False):
+        """audio float32 [B, n * hop] (CPU or the model's CUDA device) -> enhanced [B, n * hop] on the same device.
+        ``return_lsnr``: returns ``(enhanced, lsnr)``, lsnr float32 [B, n] on the same device: the local SNR in dB of the
+        frame each output hop carries, NaN where it carries none (a free slot, the first ``latency_frames`` hops of the
+        handle or of a session, a closing slot past its tail).  The handle computes the LSNR from its first request on."""
         if audio.dim() != 2 or audio.shape[0] != self.batch or audio.shape[1] == 0 or audio.shape[1] % self.hop:
             raise ValueError(f"audio must have shape [{self.batch}, n * {self.hop}]")
         n = audio.shape[1] // self.hop
@@ -130,19 +180,26 @@ class DfStream:
                 raise ValueError("audio lives on another device than the model")
             x = audio.to(torch.float32).contiguous()
             out = torch.empty_like(x)
+            lsnr = torch.empty((self.batch, n), dtype=torch.float32, device=x.device) if return_lsnr else None
             with torch.cuda.device(x.device):
-                check(_lib.lib().dfb_stream_process(self._h, x.data_ptr(), n, out.data_ptr(),
-                                                    torch.cuda.current_stream(x.device).cuda_stream))
-            return out
+                check(_lib.lib().dfb_stream_process_lsnr(self._h, x.data_ptr(), n, out.data_ptr(),
+                                                         lsnr.data_ptr() if return_lsnr else None,
+                                                         torch.cuda.current_stream(x.device).cuda_stream))
+            return (out, lsnr) if return_lsnr else out
         x = audio.detach().to("cpu", torch.float32).contiguous()
         out = torch.empty_like(x)
-        check(_lib.lib().dfb_stream_process_host(self._h, x.data_ptr(), n, out.data_ptr()))
-        return out
+        lsnr = torch.empty((self.batch, n), dtype=torch.float32) if return_lsnr else None
+        check(_lib.lib().dfb_stream_process_host_lsnr(self._h, x.data_ptr(), n, out.data_ptr(),
+                                                      lsnr.data_ptr() if return_lsnr else None))
+        return (out, lsnr) if return_lsnr else out
 
     @torch.no_grad()
-    def flush(self) -> Tensor:
+    def flush(self, return_lsnr: bool = False):
         """The ``latency_frames`` hops still in flight at the end of every stream (CPU tensor): closes every open slot,
-        and their tails come out in this call."""
+        and their tails come out in this call.  ``return_lsnr``: ``(tail, lsnr)`` with lsnr [B, latency_frames], the
+        tail frames' LSNR (CPU)."""
         out = torch.zeros((self.batch, self.latency_frames * self.hop), dtype=torch.float32)
-        check(_lib.lib().dfb_stream_process_host(self._h, None, 0, out.data_ptr()))
-        return out
+        lsnr = torch.full((self.batch, self.latency_frames), float("nan"), dtype=torch.float32) if return_lsnr else None
+        check(_lib.lib().dfb_stream_process_host_lsnr(self._h, None, 0, out.data_ptr(),
+                                                      lsnr.data_ptr() if return_lsnr and lsnr.numel() else None))
+        return (out, lsnr) if return_lsnr else out

@@ -280,6 +280,47 @@ int dfb_stream_close_slots(dfb_stream *s, const int64_t *slots, int64_t n);
 /* h_states i32[B] (host): 0 free, 1 open, 2 closing */
 int dfb_stream_slot_states(const dfb_stream *s, int32_t *h_states);
 
+/* Per-slot settings (capi.rs df_set_atten_lim / df_set_post_filter_beta, which each change one stream between two frames).
+ * `slots` is validated as for dfb_stream_open_slots; naming a free slot is DFB_ERR_INVALID, an open or closing one is fine
+ * (a closing slot's setting covers the rest of its tail).  A refused call changes nothing.  Linked handles:
+ * DFB_ERR_UNSUPPORTED, as for every slot operation.  Models whose apply step is not the specialised kernel (df_order 5,
+ * nb_df 96, 32 ERB bands, which every shipped model is): DFB_ERR_UNSUPPORTED.
+ *   atten_lim_db: the library's rule, as dfb_stream_create: <= 0 turns the limit off, else lim = 10^(-db / 20); NaN is
+ *          DFB_ERR_INVALID.  The Rust runtime instead takes |db|, treats >= 100 dB as off and < 0.01 dB as pass-through;
+ *          here 100 dB is a limit of 1e-5 and 0.001 dB one of 0.99988.  DeepFilterNet2 and DeepFilterNet3 topologies.
+ *   beta:  the DeepFilterNet3 post filter (deepfilternet3.py:448-454), finite and >= 0, 0 = off; anything else is
+ *          DFB_ERR_INVALID.  DeepFilterNet2 (whose post filter acts on the ERB gains with a fixed beta, and which the Rust
+ *          runtime does not run): DFB_ERR_UNSUPPORTED.
+ * A slot without a setting of its own follows the handle: the atten_lim_db it was created with, and the model's
+ * post_filter / pf_beta option (dfb_model_set_options) at the time of each call.  Opening a slot returns it to that; a
+ * setting made after the open and before the next call applies from the new session's first frame.  dfb_stream_reset
+ * drops every setting.  Several settings between the same two calls: the last one wins.
+ * When a change takes effect: a setting made between two calls applies to every frame whose output starts in the next
+ * process / flush call.  Output hop j of that call is the head of frame f0 + j plus the overlap-add tail of frame
+ * f0 + j - 1, so hop 0 is the new setting's head of frame f0 plus the previous setting's tail of frame f0 - 1, as in the
+ * Rust runtime, whose synthesis memory was computed in the previous call.
+ * A handle runs as before until a setter is first called; setters move it onto the slot path (every slot open, as after
+ * dfb_stream_open_slots with no slots). */
+int dfb_stream_set_atten_lim(dfb_stream *s, const int64_t *slots, int64_t n, float atten_lim_db);
+int dfb_stream_set_post_filter_beta(dfb_stream *s, const int64_t *slots, int64_t n, float beta);
+
+/* Local SNR output (capi.rs df_process_frame's return value).  d_lsnr / h_lsnr f32[B][n_frames] (flush: [B][latency]), or
+ * NULL: entry [b][j] is the LSNR, in dB, of the frame that output hop j of row b carries -- the value LSNR stage gating
+ * reads for that frame (gating itself reads the link group's first channel; linked handles return each channel's own).
+ * NaN where the hop carries no frame: a free slot, the first `latency` hops of a handle or of a new session, a closing
+ * slot past its tail.  Flush returns the tail frames' LSNR, computed with zero look-ahead like their audio.
+ * Alignment: hop j of a call that starts at input hop k carries frame k + j - latency, latency = max(conv_lookahead,
+ * df_lookahead) (+ df_lookahead for DeepFilterNet2).  df_process_frame returns, for input frame k, the LSNR of frame
+ * k - conv_lookahead (its encoder sees the features shifted by conv_lookahead, tract.rs:441-548), which is also the frame
+ * its output carries.  For DeepFilterNet3 (conv_lookahead = df_lookahead = 2) and DeepFilterNet3_ll (0 / 0) the two agree
+ * hop for hop.
+ * The LSNR head runs only on handles that ask for it: from the first call with a non-NULL buffer until dfb_stream_reset,
+ * every call computes it.  DeepFilterNet2's audio trails its DNN by df_lookahead frames, so at that first call the
+ * frames whose DNN step ran in earlier calls have no LSNR and read NaN. */
+int dfb_stream_process_lsnr(dfb_stream *s, const float *d_in, int64_t n_frames, float *d_out, float *d_lsnr, void *stream);
+int dfb_stream_flush_lsnr(dfb_stream *s, float *d_out, float *d_lsnr, void *stream);
+int dfb_stream_process_host_lsnr(dfb_stream *s, const float *h_in, int64_t n_frames, float *h_out, float *h_lsnr);
+
 /* Chunk pipeline of dfb_enhance (device_chunks) / dfb_enhance_host (host_chunks): a signal of >= 64 * chunks frames is cut
  * into at least that many time chunks; lanes = 2 overlaps the encoder phase of chunk c + 1 with the decoder phase (the
  * recurrences) of chunk c on a second set of streams and a second workspace, lanes = 1 runs them back to back.
