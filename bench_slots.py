@@ -11,10 +11,13 @@ default).  Reported per model and call size:
   * the same traffic with all 256 slots computed on every call (no slot operations: the only option before slots);
   * the same traffic with per-session settings ("controls"): every session gets its own random attenuation limit
     (6-40 dB) and post-filter beta (0-0.05) when it opens, about 2 % of the calls change one live slot's settings, and
-    every call asks for the LSNR of its output hops.
+    every call asks for the LSNR of its output hops;
+  * stereo traffic ("linked"): the same arrival process, but each arrival is a stereo call with probability 0.5 and
+    takes two free slots as one slot group (open_linked) on a handle with reduce_mask="mean", so its channels share one
+    ERB mask; "linked_as_mono" runs the identical traffic with every channel opened as its own mono slot.
 Prints one JSON line, with the card's name, power limit and SM clock read in the same run.
 
-    python bench_slots.py [--slots 256] [--calls 400] [--hops 1 10] [--warmup 20]
+    python bench_slots.py [--slots 256] [--calls 400] [--hops 1 10] [--warmup 20] [--modes ...]
 """
 from __future__ import annotations
 
@@ -33,6 +36,8 @@ from bench import model_config  # noqa: E402
 from bench_ragged import card  # noqa: E402
 
 SR, HOP = 48000, 480
+MODES = ("slots", "all_computed", "controls", "linked", "linked_as_mono")
+STEREO = ("linked", "linked_as_mono")
 
 
 def traffic(slots: int, calls: int, hops: int, seed: int):
@@ -58,7 +63,81 @@ def traffic(slots: int, calls: int, hops: int, seed: int):
     return sorted(start.tolist()), plan
 
 
-def run(name: str, slots: int, calls: int, hops: int, warmup: int, seed: int):
+def stereo_traffic(slots: int, calls: int, hops: int, seed: int):
+    """traffic() with sessions of one or two channels (probability 0.5 each): (sessions open at the start, and per call:
+    sessions to close, sessions to open, open channels after the operations); a session is its list of slots."""
+    rng = np.random.default_rng(seed)
+    lo, hi = 2 * SR // HOP, 30 * SR // HOP
+    rate = (slots / 2) / ((lo + hi) / 2) / 1.5               # 1.5 channels per session: about half the slots busy
+    left = {}                                                # session (tuple of slots) -> hops it still has
+    free = list(rng.permutation(slots))
+
+    def arrive(n_hops):
+        c = 2 if rng.random() < 0.5 else 1
+        if len(free) < c:
+            return None
+        ses = tuple(int(free.pop()) for _ in range(c))
+        left[ses] = n_hops
+        return ses
+
+    start = []
+    while sum(len(k) for k in left) < slots // 2:
+        start.append(arrive(int(rng.integers(1, hi + 1))))
+    plan, cooling = [], []                                   # a closed session's slots return once its tail is out
+    for i in range(calls):
+        closes = [k for k, v in left.items() if v == 0]
+        for k in closes:
+            del left[k]
+            cooling.append((i + 1 + -(-4 // hops), k))         # 4 hops: the longest latency (DeepFilterNet2)
+        free.extend(b for j, k in cooling if j <= i for b in k)
+        cooling = [(j, k) for j, k in cooling if j > i]
+        rng.shuffle(free)
+        opens = [o for o in (arrive(int(rng.integers(lo, hi + 1))) for _ in range(int(rng.poisson(rate * hops)))) if o]
+        live = sum(len(k) for k, v in left.items() if v > 0)
+        for k in left:
+            left[k] = max(left[k] - hops, 0)
+        plan.append(([list(k) for k in closes], [list(k) for k in opens], live))
+    return [list(k) for k in start], plan
+
+
+def run_stereo(model, st, x, slots: int, calls: int, hops: int, warmup: int, seed: int, mode: str):
+    """One pass of stereo_traffic: "linked" opens each stereo session as a slot group, "linked_as_mono" as two mono slots."""
+    import torch
+    from deepfilternet_b200 import DfStream
+    start, plan = stereo_traffic(slots, calls, hops, seed)
+    linked = mode == "linked"
+    s = DfStream(model, st, batch=slots, reduce_mask="mean" if linked else None)
+    for _ in range(warmup):
+        s.process(x)
+    s.flush()
+
+    def open_(ses):
+        if linked and len(ses) > 1:
+            s.open_linked(ses)
+        else:
+            s.open(ses)
+
+    for ses in start:
+        open_(ses)
+    ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in plan]
+    torch.cuda.synchronize()
+    for (closes, opens, _), (e0, e1) in zip(plan, ev):
+        e0.record()
+        for ses in closes:
+            s.close(ses)
+        for ses in opens:
+            open_(ses)
+        s.process(x)
+        e1.record()
+    torch.cuda.synchronize()
+    ms = np.array([a.elapsed_time(b) for a, b in ev])
+    useful = sum(live for _, _, live in plan) * hops * HOP / SR
+    return {"p50_ms": float(np.percentile(ms, 50)), "p99_ms": float(np.percentile(ms, 99)), "mean_ms": float(ms.mean()),
+            "useful_audio_s_per_s": useful / (ms.sum() / 1e3), "mean_open_channels": float(np.mean([v for _, _, v in plan])),
+            "stereo_share": float(np.mean([len(k) == 2 for _, o, _ in plan for k in o] or [0]))}
+
+
+def run(name: str, slots: int, calls: int, hops: int, warmup: int, seed: int, modes=("slots", "all_computed", "controls")):
     import torch
     from deepfilternet_b200 import DfNet, DfStream, libdf
     from deepfilternet_b200.weights import random_state_dict
@@ -73,7 +152,7 @@ def run(name: str, slots: int, calls: int, hops: int, warmup: int, seed: int):
     open_set = [[setting() for _ in opens] for _, opens, _ in plan]
     change = [(rng.random() < 0.02, rng.random(), setting()) for _ in plan]        # (change?, which live slot, to what)
     res = {}
-    for mode in ("slots", "all_computed", "controls"):
+    for mode in [m for m in modes if m not in STEREO]:
         s = DfStream(model, st, batch=slots)
         for _ in range(warmup):
             s.process(x)
@@ -116,9 +195,18 @@ def run(name: str, slots: int, calls: int, hops: int, warmup: int, seed: int):
         res[mode] = {"p50_ms": float(np.percentile(ms, 50)), "p99_ms": float(np.percentile(ms, 99)),
                      "mean_ms": float(ms.mean()), "useful_audio_s_per_s": useful / (ms.sum() / 1e3)}
         del s
+    for mode in [m for m in modes if m in STEREO]:
+        res[mode] = run_stereo(model, st, x, slots, calls, hops, warmup, seed, mode)
     res["mean_open_slots"] = float(np.mean([live for _, _, live in plan]))
-    res["speedup_useful"] = res["slots"]["useful_audio_s_per_s"] / res["all_computed"]["useful_audio_s_per_s"]
-    res["controls_vs_slots_useful"] = res["controls"]["useful_audio_s_per_s"] / res["slots"]["useful_audio_s_per_s"]
+    useful = {k: v["useful_audio_s_per_s"] for k, v in res.items() if isinstance(v, dict)}
+    if "slots" in useful and "all_computed" in useful:
+        res["speedup_useful"] = useful["slots"] / useful["all_computed"]
+    if "slots" in useful and "controls" in useful:
+        res["controls_vs_slots_useful"] = useful["controls"] / useful["slots"]
+    if "linked" in useful and "linked_as_mono" in useful:
+        res["linked_vs_mono_useful"] = useful["linked"] / useful["linked_as_mono"]
+        res["linked_vs_mono_p50"] = res["linked"]["p50_ms"] / res["linked_as_mono"]["p50_ms"]
+        res["linked_vs_mono_p99"] = res["linked"]["p99_ms"] / res["linked_as_mono"]["p99_ms"]
     return res
 
 
@@ -130,6 +218,7 @@ def main():
     ap.add_argument("--models", nargs="+", default=["DeepFilterNet3", "DeepFilterNet3_ll"])
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--seed", type=int, default=7)
+    ap.add_argument("--modes", nargs="+", default=list(MODES), choices=MODES)
     a = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "bench_slots.py measures on a GPU"
@@ -138,9 +227,9 @@ def main():
     for name in a.models:
         for hops in a.hops:
             calls = a.calls if hops == 1 else max(a.calls // hops, 40)
-            rows[f"{name}/{hops}hop"] = run(name, a.slots, calls, hops, a.warmup, a.seed)
+            rows[f"{name}/{hops}hop"] = run(name, a.slots, calls, hops, a.warmup, a.seed, a.modes)
     print(json.dumps({"metric": "serving simulation, streaming slots vs every slot computed vs slots with per-session "
-                                "settings and LSNR output", "weights": "random (seed 1)",
+                                "settings and LSNR output vs stereo slot groups", "weights": "random (seed 1)",
                       "card": before, "card_after": card(), "slots": a.slots, "session_s": [2, 30], "results": rows}))
 
 

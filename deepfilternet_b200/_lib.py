@@ -102,6 +102,8 @@ SIGNATURES = {
     "dfb_stream_open_slots": (_I, [_VP, _I64P, _I64]),
     "dfb_stream_close_slots": (_I, [_VP, _I64P, _I64]),
     "dfb_stream_slot_states": (_I, [_VP, C.POINTER(C.c_int32)]),
+    "dfb_stream_open_linked": (_I, [_VP, _I64P, _I64]),
+    "dfb_stream_slot_groups": (_I, [_VP, _I64P]),
     "dfb_stream_set_atten_lim": (_I, [_VP, _I64P, _I64, _F]),
     "dfb_stream_set_post_filter_beta": (_I, [_VP, _I64P, _I64, _F]),
     "dfb_stream_process_lsnr": (_I, [_VP, _VP, _I64, _VP, _VP, _VP]),

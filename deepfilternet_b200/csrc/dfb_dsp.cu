@@ -1155,11 +1155,13 @@ int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaS
     const bool special = p.mode != 0 && p.order == 5 && p.nb_df == 96 && st->tb.E == 32 && p.m && p.coefs;
     if (p.links && !special) return fail(DFB_ERR_UNSUPPORTED, "linked channels are built for the specialised apply kernel only");
     if (p.links && p.reduce != kReduceMax && p.reduce != kReduceMean) return fail(DFB_ERR_INVALID, "bad mask reduction %d", p.reduce);
-    if (ctl && !(special && p.rows && !p.links))
+    if (ctl && !(special && p.rows))
         return fail(DFB_ERR_UNSUPPORTED, "per-stream settings are built for the specialised slot apply kernel only");
     DFB_PROF("k_apply_synthesis", s);
     // MINB 2: 2 CTAs/SM without spills measured fastest
-    if (ctl)
+    if (ctl && p.links)   // slot groups of linked channels (dfb_stream_open_linked) with per-group settings
+        k_apply_synthesis<5, 3, 2, true, true, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, ctl);
+    else if (ctl)
         k_apply_synthesis<5, 3, 2, true, false, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, ctl);
     else if (p.links && p.rows)
         k_apply_synthesis<5, 3, 2, true, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, nullptr);

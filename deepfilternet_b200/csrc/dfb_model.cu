@@ -1520,15 +1520,21 @@ static ChunkGeom chunk_geom(const dfb_model_config &c) {
 
 // Every array of the state slab is `layers` x [B][per_row] floats; only the GRU states have more than one layer.
 constexpr int kStateArrays = 13;
-struct StateLayout { int64_t off[kStateArrays]; int layers[kStateArrays], per_row[kStateArrays]; };
+// row_off / row_floats: one stream's row of every array, packed (the scratch rows of k_slot_rows)
+struct StateLayout { int64_t off[kStateArrays], row_off[kStateArrays], row_floats; int layers[kStateArrays], per_row[kStateArrays]; };
 
 static size_t state_floats(const dfb_model_config &c, const dfb_state *st, int B, size_t off[16], StateLayout *lay = nullptr) {
     const ChunkGeom g = chunk_geom(c);
     const int E = c.nb_erb, Fd = c.nb_df, O2 = 2 * c.df_order, F = st->tb.F, ED = E / 4 * kCh;
     size_t n = 0;
+    if (lay) lay->row_floats = 0;
     auto add = [&](int i, int layers, int per_row) {
         off[i] = n;
-        if (lay) { lay->off[i] = (int64_t)n; lay->layers[i] = layers; lay->per_row[i] = per_row; }
+        if (lay) {
+            lay->off[i] = (int64_t)n; lay->layers[i] = layers; lay->per_row[i] = per_row;
+            lay->row_off[i] = lay->row_floats;
+            lay->row_floats += (int64_t)layers * per_row;
+        }
         n += ((size_t)layers * B * per_row + 63) & ~size_t(63);
     };
     add(0, 1, st->hop); add(1, 1, E); add(2, 1, Fd);
@@ -2179,19 +2185,29 @@ extern "C" int dfb_enhance_ragged_linked_host(dfb_model *m, dfb_state *st, const
 enum { kSlotFree = 0, kSlotOpen = 1, kSlotClosing = 2 };
 constexpr int64_t kOpenEnd = 0x7fffffff;   // rows[b].Tf of an open slot: kernels take Tf - w0 as int
 
-// Row `dst` of every array of the state slab <- row `src`, or (src < 0) the initial state of a fresh stream: zeros, and the
-// normalisation EMA states at the values launch_feat_norm starts from without a state.  grid (x, kStateArrays).
-__global__ void k_slot_row(float *__restrict__ slab, StateLayout lay, int Bs, int dst, int src, int E, int Fd) {
-    const int a = blockIdx.y, per = lay.per_row[a];
+// The state-slab rows of one call: ops[i] = {dst, src} sets row dst of every array to row src as the last call left it, or
+// (src < 0) to the initial state of a fresh stream: zeros, and the normalisation EMA states at the values launch_feat_norm
+// starts from without a state.  Sources and destinations overlap when rows close up behind a freed slot, so the moves come
+// first in `ops` and pass 0 copies their sources to scratch rows [i][lay.row_floats]; pass 1 writes every destination.
+// Two launches whatever the number of rows.  grid (x, ops of the pass, kStateArrays).
+__global__ void k_slot_rows(float *__restrict__ slab, StateLayout lay, int Bs, const int2 *__restrict__ ops, float *__restrict__ scratch,
+                            int pass, int E, int Fd) {
+    const int i = blockIdx.y, a = blockIdx.z, per = lay.per_row[a];
+    const int2 op = ops[i];
     const int64_t n = (int64_t)lay.layers[a] * per;
+    float *sc = scratch + (int64_t)i * lay.row_floats + lay.row_off[a];
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
         const int l = (int)(e / per), j = (int)(e - (int64_t)l * per);
         float *base = slab + lay.off[a] + (int64_t)l * Bs * per + j;
+        if (pass == 0) {
+            sc[e] = base[(int64_t)op.y * per];
+            continue;
+        }
         float v = 0.f;
-        if (src >= 0) v = base[(int64_t)src * per];
+        if (op.y >= 0) v = sc[e];
         else if (a == 1) v = erb_norm_init(j, E);
         else if (a == 2) v = unit_norm_init(j, Fd);
-        base[(int64_t)dst * per] = v;
+        base[(int64_t)op.x * per] = v;
     }
 }
 
@@ -2227,11 +2243,17 @@ struct dfb_stream {
     std::vector<int> slot_state, slot_row, row_slot;   // kSlot*; slot -> row of the active prefix (-1 free); row -> slot
     std::vector<int64_t> slot_first, slot_end;         // absolute first frame; end frame of a closing slot
     int n_act = 0;
-    std::vector<std::pair<int, int>> pend;             // state-slab rows (dst, src; src -1: initialise) for the next call
-    bool tab_dirty = true;                             // rows / first frames to re-upload
+    std::vector<int> row_src;                          // per row: its state-slab row at the last call, or -1: a fresh stream
+    // slot groups (dfb_stream_open_linked): per slot the slot of its group's channel 0 (-1 free) and the group's channel
+    // count.  A group's rows are contiguous in the active prefix, in channel order.
+    std::vector<int> slot_grp, slot_nch;
+    int group_reduce = 0;                              // mask reduction of the groups (dfb_stream_set_mask_reduce(s, 1, mode))
+    bool tab_dirty = true;                             // rows / first frames / link groups to re-upload
     int64_t tab_n = -1;                                // ... for calls of this many input hops
+    bool tab_linked = false;                           // the uploaded table has a linked group of more than one channel
     RaggedRow *d_rows = nullptr;
     int64_t *d_first = nullptr;
+    LinkRow *d_grp = nullptr;
     // per-slot settings (dfb_stream_set_atten_lim / _post_filter_beta).  ctl_on: a setter has run since create / reset, so
     // the slot path passes the per-row table to the apply kernel.
     bool ctl_on = false;
@@ -2280,6 +2302,7 @@ extern "C" void dfb_stream_free(dfb_stream *h) {
     if (h->links) cudaFree(h->links);
     if (h->d_rows) cudaFree(h->d_rows);
     if (h->d_first) cudaFree(h->d_first);
+    if (h->d_grp) cudaFree(h->d_grp);
     if (h->d_ctl) cudaFree(h->d_ctl);
     if (h->stage_lsnr) cudaFree(h->stage_lsnr);
     delete h;
@@ -2292,7 +2315,6 @@ extern "C" int dfb_stream_reset(dfb_stream *h) {
     state_bind(h->S, h->slab, off, h->B);
     h->fed = false;
     h->slots = false;
-    h->pend.clear();
     h->ctl_on = false;
     h->lsnr_from = -1;
     return DFB_OK;
@@ -2300,11 +2322,12 @@ extern "C" int dfb_stream_reset(dfb_stream *h) {
 
 // Linked channels on a stream handle: streams g * channels + c (c < channels) are the channels of recording g and share one
 // ERB mask (reduce_mask max / mean, as dfb_enhance_ragged_linked).  Only before the first frame of a new or reset handle:
-// the frame re-synthesised for the overlap-add tail at the next call would otherwise mix the two settings.
+// the frame re-synthesised for the overlap-add tail at the next call would otherwise mix the two settings.  channels = 1
+// records the reduction of the slot groups opened later (dfb_stream_open_linked).
 extern "C" int dfb_stream_set_mask_reduce(dfb_stream *h, int channels, int reduce_mask) {
     if (!h) return fail(DFB_ERR_INVALID, "null stream");
     if (h->fed) return fail(DFB_ERR_INVALID, "mask reduction set after the first frame: reset the stream first");
-    if (h->slots) return fail(DFB_ERR_UNSUPPORTED, "linked channels and streaming slots do not combine: reset the stream first");
+    if (h->slots) return fail(DFB_ERR_UNSUPPORTED, "mask reduction set after slot operations: reset the stream first");
     if (reduce_mask != kReduceNone && reduce_mask != kReduceMax && reduce_mask != kReduceMean)
         return fail(DFB_ERR_INVALID, "reduce_mask %d is not 0 (none), 1 (max) or 2 (mean)", reduce_mask);
     if (channels <= 0 || h->B % channels) return fail(DFB_ERR_INVALID, "%d streams are not groups of %d channels", h->B, channels);
@@ -2312,6 +2335,7 @@ extern "C" int dfb_stream_set_mask_reduce(dfb_stream *h, int channels, int reduc
     if (h->links) cudaFree(h->links);
     h->links = nullptr;
     h->reduce = 0;
+    h->group_reduce = channels == 1 ? reduce_mask : kReduceNone;
     if (reduce_mask == kReduceNone || channels == 1) return DFB_OK;
     std::vector<LinkRow> t((size_t)h->B);
     for (int b = 0; b < h->B; b++) t[(size_t)b] = LinkRow{b - b % channels, channels};
@@ -2342,24 +2366,30 @@ extern "C" int64_t dfb_stream_latency_frames(const dfb_stream *h) {
 }
 extern "C" int64_t dfb_stream_frame_length(const dfb_stream *h) { return h ? h->st->hop : -1; }  // capi.rs df_get_frame_length
 
-// ---- streaming slots: host bookkeeping.  Device rows follow at the next call (stream_step runs h->pend first).
+// ---- streaming slots: host bookkeeping.  Device rows follow at the next call (slots_step moves them first, by row_src).
 // Leaves the slot-free path: every slot is open, row b = slot b, its stream started at frame 0.
 static int slots_enable(dfb_stream *h) {
     if (h->slots) return DFB_OK;
     const size_t B = (size_t)h->B;
-    if (!h->d_rows) {
+    if (!h->d_grp) {
         DFB_CUDA(cudaSetDevice(h->m->device));
-        if (cudaMalloc(&h->d_rows, sizeof(RaggedRow) * B) != cudaSuccess || cudaMalloc(&h->d_first, sizeof(int64_t) * B) != cudaSuccess)
+        if ((!h->d_rows && cudaMalloc(&h->d_rows, sizeof(RaggedRow) * B) != cudaSuccess) ||
+            (!h->d_first && cudaMalloc(&h->d_first, sizeof(int64_t) * B) != cudaSuccess) ||
+            cudaMalloc(&h->d_grp, sizeof(LinkRow) * B) != cudaSuccess) {
+            h->d_grp = nullptr;
             return fail(DFB_ERR_OOM, "slot table allocation failed");
+        }
     }
     h->slot_state.assign(B, kSlotOpen);
-    h->slot_row.resize(B); h->row_slot.resize(B);
+    h->slot_row.resize(B); h->row_slot.resize(B); h->row_src.resize(B); h->slot_grp.resize(B);
     std::iota(h->slot_row.begin(), h->slot_row.end(), 0);
     std::iota(h->row_slot.begin(), h->row_slot.end(), 0);
+    std::iota(h->row_src.begin(), h->row_src.end(), 0);
+    std::iota(h->slot_grp.begin(), h->slot_grp.end(), 0);
+    h->slot_nch.assign(B, 1);
     h->slot_first.assign(B, 0);
     h->slot_end.assign(B, kOpenEnd);
     h->n_act = h->B;
-    h->pend.clear();
     h->tab_dirty = true;
     h->slot_lim.assign(B, NAN);
     h->slot_beta.assign(B, NAN);
@@ -2370,26 +2400,36 @@ static int slots_enable(dfb_stream *h) {
     return DFB_OK;
 }
 
-// the slot's row leaves the active prefix: the last active row moves into its place
+// the slot becomes free; its row stays in the active prefix until rows_compact
 static void slot_release(dfb_stream *h, int slot) {
-    const int r = h->slot_row[(size_t)slot], last = h->n_act - 1;
-    if (r != last) {
-        h->pend.emplace_back(r, last);
-        const int moved = h->row_slot[(size_t)last];
-        h->row_slot[(size_t)r] = moved;
-        h->slot_row[(size_t)moved] = r;
-    }
     h->slot_row[(size_t)slot] = -1;
+    h->slot_grp[(size_t)slot] = -1;
+    h->slot_nch[(size_t)slot] = 0;
     h->slot_state[(size_t)slot] = kSlotFree;
-    h->n_act--;
-    h->tab_dirty = true;
+}
+
+// The rows of freed slots leave the active prefix and the rows behind them close up in order, so every group stays
+// contiguous and in channel order.  A row that moves carries its source row (row_src) along: the next call moves the
+// state-slab rows in one pass (k_slot_rows), however many rows moved.
+static void rows_compact(dfb_stream *h) {
+    int n = 0;
+    for (int r = 0; r < h->n_act; r++) {
+        const int b = h->row_slot[(size_t)r];
+        if (h->slot_state[(size_t)b] == kSlotFree) continue;
+        h->row_slot[(size_t)n] = b;
+        h->row_src[(size_t)n] = h->row_src[(size_t)r];
+        h->slot_row[(size_t)b] = n++;
+    }
+    if (n != h->n_act) h->tab_dirty = true;
+    h->n_act = n;
 }
 
 // closing slots whose last frame has been output become free: `out_end` is the frame after the last output hop so far
-// (a1 - latency after a process call, a1 after a flush)
+// (a1 - latency after a process call, a1 after a flush).  The members of a group share their end frame: they leave together.
 static void slots_retire(dfb_stream *h, int64_t out_end) {
     for (int b = 0; b < h->B; b++)
         if (h->slot_state[(size_t)b] == kSlotClosing && h->slot_end[(size_t)b] <= out_end) slot_release(h, b);
+    rows_compact(h);
 }
 
 static void slot_close(dfb_stream *h, int slot) {
@@ -2404,15 +2444,27 @@ static void slots_close_all(dfb_stream *h) {
     slots_retire(h, h->S.a1 - dfb_stream_latency_frames(h));
 }
 
+// Valid slot indices, each listed once; a live group of more than one channel is listed with all of its members or not at
+// all (groups open, close and take settings as a unit).
 static int slot_list_check(const dfb_stream *h, const int64_t *slots, int64_t n) {
     if (!h || n < 0 || (n > 0 && !slots)) return fail(DFB_ERR_INVALID, "bad argument");
     if (h->links) return fail(DFB_ERR_UNSUPPORTED, "slot operations on a handle with linked channels");
-    std::vector<char> seen((size_t)h->B, 0);
+    std::vector<int> seen((size_t)h->B, 0);
     for (int64_t i = 0; i < n; i++) {
         const int64_t b = slots[i];
         if (b < 0 || b >= h->B) return fail(DFB_ERR_INVALID, "slot %lld outside [0, %d)", (long long)b, h->B);
         if (seen[(size_t)b]) return fail(DFB_ERR_INVALID, "slot %lld listed twice", (long long)b);
         seen[(size_t)b] = 1;
+    }
+    if (!h->slots) return DFB_OK;
+    std::vector<int> listed((size_t)h->B, 0);   // per group (by its channel-0 slot): members listed
+    for (int64_t i = 0; i < n; i++)
+        if (h->slot_grp[(size_t)slots[i]] >= 0) listed[(size_t)h->slot_grp[(size_t)slots[i]]]++;
+    for (int64_t i = 0; i < n; i++) {
+        const int f = h->slot_grp[(size_t)slots[i]];
+        if (f >= 0 && listed[(size_t)f] != h->slot_nch[(size_t)f])
+            return fail(DFB_ERR_INVALID, "slot %lld belongs to a group of %d channels (slot %d is channel 0): list all of them",
+                        (long long)slots[i], h->slot_nch[(size_t)f], f);
     }
     return DFB_OK;
 }
@@ -2422,17 +2474,21 @@ static int slot_list(dfb_stream *h, const int64_t *slots, int64_t n) {
     return slots_enable(h);
 }
 
-extern "C" int dfb_stream_open_slots(dfb_stream *h, const int64_t *slots, int64_t n) {
+// Opens one group per `nch` consecutive listed slots (channel c of a group in its c-th slot), each a fresh stream in rows
+// appended to the active prefix.  The listed slots' old streams (whole groups, by slot_list_check) are dropped without
+// their tails first.
+static int slots_open(dfb_stream *h, const int64_t *slots, int64_t n, int64_t nch) {
     if (int rc = slot_list(h, slots, n)) return rc;
+    for (int64_t i = 0; i < n; i++)
+        if (h->slot_state[(size_t)slots[i]] != kSlotFree) slot_release(h, (int)slots[i]);
+    rows_compact(h);
     for (int64_t i = 0; i < n; i++) {
-        const int b = (int)slots[i];
-        int r = h->slot_row[(size_t)b];
-        if (r < 0) {   // free: takes the row after the active prefix
-            r = h->n_act++;
-            h->slot_row[(size_t)b] = r;
-            h->row_slot[(size_t)r] = b;
-        }
-        h->pend.emplace_back(r, -1);   // a fresh stream; an open or closing one is dropped without its tail
+        const int b = (int)slots[i], r = h->n_act++;
+        h->slot_row[(size_t)b] = r;
+        h->row_slot[(size_t)r] = b;
+        h->row_src[(size_t)r] = -1;
+        h->slot_grp[(size_t)b] = (int)slots[i - i % nch];
+        h->slot_nch[(size_t)b] = (int)nch;
         h->slot_state[(size_t)b] = kSlotOpen;
         h->slot_first[(size_t)b] = h->S.a1;
         h->slot_end[(size_t)b] = kOpenEnd;
@@ -2441,6 +2497,13 @@ extern "C" int dfb_stream_open_slots(dfb_stream *h, const int64_t *slots, int64_
     }
     h->tab_dirty = true;
     return DFB_OK;
+}
+
+extern "C" int dfb_stream_open_slots(dfb_stream *h, const int64_t *slots, int64_t n) { return slots_open(h, slots, n, 1); }
+
+extern "C" int dfb_stream_open_linked(dfb_stream *h, const int64_t *slots, int64_t n) {
+    if (h && n == 0) return fail(DFB_ERR_INVALID, "a group of no channels");
+    return slots_open(h, slots, n, n);
 }
 
 extern "C" int dfb_stream_close_slots(dfb_stream *h, const int64_t *slots, int64_t n) {
@@ -2522,6 +2585,44 @@ extern "C" int dfb_stream_slot_states(const dfb_stream *h, int32_t *h_states) {
     return DFB_OK;
 }
 
+extern "C" int dfb_stream_slot_groups(const dfb_stream *h, int64_t *h_first) {
+    if (!h || !h_first) return fail(DFB_ERR_INVALID, "null argument");
+    for (int b = 0; b < h->B; b++) h_first[b] = h->slots ? h->slot_grp[(size_t)b] : b;
+    return DFB_OK;
+}
+
+// Row moves of a call: row r takes its state from row_src[r] as the last call left it, or starts fresh (-1).  Two
+// launches of k_slot_rows whatever the number of rows, the scratch rows in the model arena (the chunk that follows reuses
+// it in stream order).
+static int slots_move_rows(dfb_stream *h, cudaStream_t s) {
+    std::vector<int2> ops;
+    int n_mv = 0;
+    for (int pass = 0; pass < 2; pass++)   // the moves first, then the fresh rows
+        for (int r = 0; r < h->n_act; r++) {
+            const int src = h->row_src[(size_t)r];
+            if (src != r && (src >= 0) == (pass == 0)) ops.push_back(make_int2(r, src));
+        }
+    for (const int2 &op : ops) n_mv += op.y >= 0;
+    for (int r = 0; r < h->n_act; r++) h->row_src[(size_t)r] = r;
+    if (ops.empty()) return DFB_OK;
+    dfb_model *m = h->m;
+    size_t off[16];
+    StateLayout lay;
+    state_floats(m->cfg, h->st, h->B, off, &lay);
+    if (int rc = m->arena.reserve(sizeof(int2) * ops.size() + sizeof(float) * (size_t)lay.row_floats * n_mv + 1024)) return rc;
+    m->arena.reset();
+    int2 *d_ops = m->arena.take<int2>(ops.size());
+    float *scratch = m->arena.take<float>((size_t)lay.row_floats * n_mv + 1);
+    DFB_CUDA(cudaMemcpyAsync(d_ops, ops.data(), sizeof(int2) * ops.size(), cudaMemcpyHostToDevice, s));
+    for (int pass = n_mv ? 0 : 1; pass < 2; pass++) {
+        k_slot_rows<<<dim3(4, pass ? (unsigned)ops.size() : (unsigned)n_mv, kStateArrays), 256, 0, s>>>(
+            h->slab, lay, h->B, d_ops, scratch, pass, m->cfg.nb_erb, m->cfg.nb_df);
+        DFB_LAUNCH_CHECK();
+    }
+    m->arena.reset();
+    return DFB_OK;
+}
+
 // Slot path of one call: rows [0, n_act) of the slab, the row table for calls of n input hops, output rows zero first.
 static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s) {
     dfb_model *m = h->m;
@@ -2537,31 +2638,28 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
     if (d1n < S.d1) d1n = S.d1;
     if (e1n < S.e1) e1n = S.e1;
     if (flush) slots_close_all(h);
-    {   // pending row operations, in order
-        size_t off[16];
-        StateLayout lay;
-        state_floats(m->cfg, st, B, off, &lay);
-        for (const auto &op : h->pend) {
-            k_slot_row<<<dim3(8, kStateArrays), 256, 0, s>>>(h->slab, lay, B, op.first, op.second, m->cfg.nb_erb, m->cfg.nb_df);
-            DFB_LAUNCH_CHECK();
-        }
-        h->pend.clear();
-    }
+    if ((rc = slots_move_rows(h, s))) return rc;
     if (h->tab_dirty || h->tab_n != n) {
         std::vector<RaggedRow> rows((size_t)h->n_act);
         std::vector<int64_t> first((size_t)h->n_act);
+        std::vector<LinkRow> grp((size_t)h->n_act);
+        bool linked = false;   // the link table goes to the kernels only while a group of more than one channel is linked
         for (int r = 0; r < h->n_act; r++) {
             const int b = h->row_slot[(size_t)r];
             const bool open = h->slot_state[(size_t)b] == kSlotOpen;
             rows[(size_t)r] = RaggedRow{b * n * hop, open ? n * hop : 0, b * n_out * hop, n_out * hop, h->slot_end[(size_t)b]};
             first[(size_t)r] = h->slot_first[(size_t)b];
+            grp[(size_t)r] = LinkRow{h->slot_row[(size_t)h->slot_grp[(size_t)b]], h->slot_nch[(size_t)b]};
+            linked |= grp[(size_t)r].n > 1 && h->group_reduce != kReduceNone;
         }
         if (h->n_act > 0) {
             DFB_CUDA(cudaMemcpyAsync(h->d_rows, rows.data(), sizeof(RaggedRow) * rows.size(), cudaMemcpyHostToDevice, s));
             DFB_CUDA(cudaMemcpyAsync(h->d_first, first.data(), sizeof(int64_t) * first.size(), cudaMemcpyHostToDevice, s));
+            if (linked) DFB_CUDA(cudaMemcpyAsync(h->d_grp, grp.data(), sizeof(LinkRow) * grp.size(), cudaMemcpyHostToDevice, s));
         }
         h->tab_dirty = false;
         h->tab_n = n;
+        h->tab_linked = linked;
     }
     if (n_out > 0) DFB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * B * n_out * hop, s));   // free slots; frames outside a stream
     if (d_lsnr && n_out > 0) DFB_CUDA(cudaMemsetAsync(d_lsnr, 0xff, sizeof(float) * B * n_out, s));   // NaN: hops without a frame
@@ -2580,6 +2678,7 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
     ChunkIO io{d_in, n * hop, n * hop, a0, nullptr, d_out, n_out * hop, n_out * hop, f0 * hop, h->lim, h->gating ? h->th : nullptr,
                h->d_rows, h->n_act};
     io.first = h->d_first;
+    if (h->tab_linked) { io.links = h->d_grp; io.reduce = h->group_reduce; }
     if (h->ctl_on) io.ctl = h->d_ctl;
     io.lsnr_from = h->lsnr_from;
     io.lsnr_out = d_lsnr;
@@ -2650,9 +2749,8 @@ static void flushed_all(dfb_stream *h) {
     if (h->links) return;
     if (h->slots) { slots_close_all(h); return; }
     if (slots_enable(h)) return;
-    std::fill(h->slot_state.begin(), h->slot_state.end(), (int)kSlotFree);
-    std::fill(h->slot_row.begin(), h->slot_row.end(), -1);
-    h->n_act = 0;
+    for (int b = 0; b < h->B; b++) slot_release(h, b);
+    rows_compact(h);
 }
 
 // d_in [B][n_frames * hop] -> d_out [B][n_frames * hop] (device pointers, asynchronous on `stream`); d_lsnr (or null)

@@ -13,7 +13,8 @@ The concatenation of the outputs equals ``enhance(model, df_state, audio, pad=Fa
 the channels of recording g and share one ERB mask, the max or mean of theirs (dfb_stream_set_mask_reduce).
 
 Each row is a slot that can start and end its own stream (``open`` / ``close``), so one handle serves calls that come and
-go: a call joins whenever a slot is free, and only open and closing slots are computed.  Each slot can change its own
+go: a call joins whenever a slot is free, and only open and closing slots are computed.  ``open_linked`` opens a call of
+several channels in as many slots, linked by the handle's ``reduce_mask`` like a ``channels`` group.  Each slot can change its own
 attenuation limit and post-filter beta between two calls (``set_atten_lim`` / ``set_post_filter_beta``), and
 ``process`` / ``flush`` return the local SNR of every output frame on request (``return_lsnr=True``).
 """
@@ -53,6 +54,14 @@ def slot_list(slots, batch: int) -> np.ndarray:
     u, counts = np.unique(a, return_counts=True)
     if (counts > 1).any():
         raise ValueError(f"slot {int(u[counts > 1][0])} listed twice")
+    return a
+
+
+def group_list(slots, batch: int) -> np.ndarray:
+    """``slots`` of DfStream.open_linked as slot_list gives them (channel c in the c-th); ValueError also when empty."""
+    a = slot_list(slots, batch)
+    if not a.size:
+        raise ValueError("a slot group needs at least one slot")
     return a
 
 
@@ -128,14 +137,26 @@ class DfStream:
         """Start a new stream in each listed slot, from the initial state, as a fresh handle would.  An open or closing
         slot's old stream is dropped without its tail.  Takes effect at the next ``process`` / ``flush``; from then on row
         b of their input and output is that stream, and its output equals ``DfStream(batch=1)`` fed the same audio in the
-        same call sizes and flushed at the end."""
+        same call sizes and flushed at the end.  A live group (``open_linked``) must be listed with all of its members or
+        not at all (DfbError otherwise)."""
         self._slots(_lib.lib().dfb_stream_open_slots, slots)
+
+    def open_linked(self, slots) -> None:
+        """Start one session of ``len(slots)`` channels, channel c in row ``slots[c]``, whose channels share one ERB mask
+        reduced by the handle's ``reduce_mask`` (the constructor's, with ``channels=1``; None: unlinked channels that open
+        and close together).  Its output equals ``DfStream(batch=C, channels=C, reduce_mask=...)`` fed the same C rows in
+        the same call sizes and flushed at the end.  The group moves as a unit: ``open``, ``open_linked``, ``close`` and the
+        setters list all of its members or none.  Opening over a live group drops its old session without its tail
+        (dfb_stream_open_linked)."""
+        a = group_list(slots, self.batch)
+        check(_lib.lib().dfb_stream_open_linked(self._h, a.ctypes.data_as(C.POINTER(C.c_int64)), a.size))
 
     def close(self, slots) -> None:
         """End the stream of each listed open slot after the input it has already been fed.  From the next call on its
         input rows are ignored; over the next ``latency_frames`` hops its output rows carry what ``flush`` would give that
         stream alone, whatever the call sizes, then the slot is free (at once when ``latency_frames`` is 0).  Free slots
-        are not computed and return zeros.  Closing a slot that is not open does nothing."""
+        are not computed and return zeros.  Closing a slot that is not open does nothing.  A group closes as a unit: list
+        all of its members."""
         self._slots(_lib.lib().dfb_stream_close_slots, slots)
 
     def _live_or(self, slots) -> np.ndarray:
@@ -147,14 +168,16 @@ class DfStream:
         """Attenuation limit of the listed slots (None: every open or closing slot) from the next call on: ``db`` <= 0 or
         None turns it off, else the enhanced spectrum is mixed with 10^(-db / 20) of the noisy one, as ``atten_lim_db`` of
         the constructor.  The slot's first output hop of that call still carries the previous setting's overlap-add tail.
-        ``open`` returns a slot to the handle's setting; ``reset`` drops every setting (dfb_stream_set_atten_lim)."""
+        ``open`` returns a slot to the handle's setting; ``reset`` drops every setting (dfb_stream_set_atten_lim).  A group
+        takes one setting: list all of its members."""
         v = atten_lim_arg(db)
         a = self._live_or(slots)
         check(_lib.lib().dfb_stream_set_atten_lim(self._h, a.ctypes.data_as(C.POINTER(C.c_int64)), a.size, v))
 
     def set_post_filter_beta(self, beta: float, slots=None) -> None:
         """DeepFilterNet3 post-filter beta of the listed slots (None: every open or closing slot) from the next call on;
-        finite and >= 0, 0 turns the post filter off.  Not available for DeepFilterNet2 (dfb_stream_set_post_filter_beta)."""
+        finite and >= 0, 0 turns the post filter off.  Not available for DeepFilterNet2 (dfb_stream_set_post_filter_beta).
+        A group takes one setting: list all of its members."""
         v = pf_beta_arg(beta)
         a = self._live_or(slots)
         check(_lib.lib().dfb_stream_set_post_filter_beta(self._h, a.ctypes.data_as(C.POINTER(C.c_int64)), a.size, v))
@@ -164,6 +187,13 @@ class DfStream:
         open; ``flush`` closes them all."""
         out = np.zeros(self.batch, np.int32)
         check(_lib.lib().dfb_stream_slot_states(self._h, out.ctypes.data_as(C.POINTER(C.c_int32))))
+        return out
+
+    def slot_groups(self) -> np.ndarray:
+        """int64 [batch]: per slot, the slot holding channel 0 of its group (the slot itself for a one-channel session),
+        -1 for a free slot."""
+        out = np.zeros(self.batch, np.int64)
+        check(_lib.lib().dfb_stream_slot_groups(self._h, out.ctypes.data_as(C.POINTER(C.c_int64))))
         return out
 
     @torch.no_grad()

@@ -250,7 +250,9 @@ int dfb_stream_set_lsnr_thresholds(dfb_stream *s, int enable, float min_db_thres
                                    float max_db_df_thresh);
 /* Linked channels (see dfb_enhance_ragged_linked): streams g * channels + c form link group g; B % channels == 0.
  * Only on a new or reset handle (DFB_ERR_INVALID after the first frame: the frame re-synthesised for the overlap-add
- * tail would mix two settings).  channels = 1 or DFB_REDUCE_NONE: unlinked (the default). */
+ * tail would mix two settings) that has had no slot operation (DFB_ERR_UNSUPPORTED).  channels = 1 or DFB_REDUCE_NONE:
+ * unlinked (the default); channels = 1 also records reduce_mask as the reduction of the slot groups that
+ * dfb_stream_open_linked opens later (one mode per handle; it survives dfb_stream_reset, as the channel groups do). */
 int dfb_stream_set_mask_reduce(dfb_stream *s, int channels, int reduce_mask);
 /* capi.rs df_process_frame, batched and for n_frames hops at once: d_in / d_out f32[B][n_frames * hop] (device) */
 int dfb_stream_process(dfb_stream *s, const float *d_in, int64_t n_frames, float *d_out, void *stream);
@@ -273,12 +275,27 @@ int dfb_stream_process_host(dfb_stream *s, const float *h_in, int64_t n_frames, 
  *   free:  not computed; its input rows are ignored and its output rows are zeros.
  * Row b of process / flush is slot b.  Every session's output equals a single-stream handle fed the same audio in the
  * same call sizes and then flushed.  Only open and closing slots are computed, so the cost of a call follows the number
- * of live streams, not B.  Linked channels (dfb_stream_set_mask_reduce) and slots do not combine: DFB_ERR_UNSUPPORTED.
+ * of live streams, not B.  Fixed channel groups (dfb_stream_set_mask_reduce with channels > 1) and slots do not combine:
+ * every slot operation on such a handle is DFB_ERR_UNSUPPORTED; slot groups (below) are the slot path's linked channels.
  * The handle's clock counts frames since create / reset; slot operations need it below 2^31 - 2 frames (248 days). */
 int dfb_stream_open_slots(dfb_stream *s, const int64_t *slots, int64_t n);
 int dfb_stream_close_slots(dfb_stream *s, const int64_t *slots, int64_t n);
 /* h_states i32[B] (host): 0 free, 1 open, 2 closing */
 int dfb_stream_slot_states(const dfb_stream *s, int32_t *h_states);
+/* Slot groups: one session of n channels in n slots, channel c in row slots[c] (n >= 1; DFB_ERR_INVALID for n = 0, and
+ * for slots as dfb_stream_open_slots).  The channels share one ERB mask, reduced as the handle's mode says
+ * (dfb_stream_set_mask_reduce(s, 1, mode)): the session's output equals a fresh handle with B = n and
+ * dfb_stream_set_mask_reduce(s, n, mode), fed the same n rows in the same call sizes and then flushed.  With mode NONE, or
+ * n = 1, the group is n unlinked channels.  LSNR stage gating reads the group's channel 0; the LSNR output is each
+ * channel's own.  A group moves as a unit: a call that lists any member of a live group of more than one channel
+ * (open_slots, open_linked, close_slots, set_atten_lim, set_post_filter_beta) must list all of its members, else it
+ * returns DFB_ERR_INVALID and changes nothing.  dfb_stream_open_slots opens n groups of one channel.  Opening over a live
+ * group drops its old session without its tail, as a re-opened slot does.  The members share their first and end
+ * frames, so they close and become free together; settings made on all members are the group's.  Only the live rows are
+ * computed; when a session ends, the rows behind it close up in two kernel launches whatever their number. */
+int dfb_stream_open_linked(dfb_stream *s, const int64_t *slots, int64_t n);
+/* h_first i64[B] (host): per slot, the slot holding channel 0 of its group (the slot itself for one channel), -1 if free */
+int dfb_stream_slot_groups(const dfb_stream *s, int64_t *h_first);
 
 /* Per-slot settings (capi.rs df_set_atten_lim / df_set_post_filter_beta, which each change one stream between two frames).
  * `slots` is validated as for dfb_stream_open_slots; naming a free slot is DFB_ERR_INVALID, an open or closing one is fine
