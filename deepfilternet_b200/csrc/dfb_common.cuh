@@ -232,7 +232,7 @@ int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaS
 // time window of a recurrence launch: steps 0 .. T-1 are frames t0 .. of buffers holding Ts frames per stream; h0 (null:
 // zeros) / hT (null: not stored) are the carried hidden states [B][H]
 struct GruWindow { const float *h0; float *hT; int t0, Ts; const int64_t *first = nullptr; int64_t w0 = 0; /* stream_first */ };
-// tensor-core GRU recurrence, H = 256 (dfb_tc.cu)
+// tensor-core GRU recurrence, H = 256 (dfb_tc.cu); hout may be null when the planes hout_hi / hout_lo are given
 int launch_gru_tc(cudaStream_t s, const float *xproj, const float *whh, const float *bhh, const float *res, float *hout,
                   unsigned short *hout_hi, unsigned short *hout_lo, int B, int T, long long *dbg = nullptr, int wide = 0,
                   int planes_res = 0, const GruWindow *w = nullptr, int H = 256);
@@ -245,6 +245,11 @@ int launch_gl_bx(cudaStream_t s, const unsigned short *x_hi, const unsigned shor
                  const float *res, int64_t ldr, float *y, int64_t ldy, unsigned short *y_hi, unsigned short *y_lo, int64_t ldp,
                  int64_t M, int G, int Ig, int Hg, int act, float oscale, float ooffset);
 bool gl_bx_geometry(int G, int Ig, int Hg, int *gpc_out, int *hgp_out, int *stages_out);
+// df_conv1 -> df_fc_emb in one kernel, c1 kept on chip (dfb_gl.cu): emb_in planes = relu(GL(dwpw(c0))) (+ res)
+bool df_emb_geometry(int Fd, int G, int Ig, int Hg, int kt, int *s_out, int *stages_out);
+int launch_df_emb(cudaStream_t s, const float *c0, int64_t M, int T, int Fd, int kt, const float *dw, const float *bias,
+                  const float *pw_sw, const float *w_img, int G, int Ig, int Hg, const float *res, int64_t ldr,
+                  unsigned short *y_hi, unsigned short *y_lo, int64_t ldp, const int64_t *first, int64_t w0);
 // DF pathway conv (df_convp) on tensor cores (dfb_tc.cu)
 int launch_df_convp_tc(cudaStream_t s, const float *c0, const float *w_sw, const float *w2, const float *bias, float *coefs, int B, int T,
                        int Fd, const int64_t *first = nullptr, int64_t w0 = 0);

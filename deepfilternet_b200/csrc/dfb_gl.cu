@@ -23,6 +23,7 @@
 #include <tuple>
 
 #include "dfb_common.cuh"
+#include "dfb_dwpw.cuh"
 #include "dfb_ptx.cuh"
 
 namespace dfb {
@@ -184,6 +185,254 @@ k_gl_bx(const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUten
     }
 }
 
+// ------------------------------------------------------ df_conv1 -> df_fc_emb, c1 kept on chip ----
+//   emb_in[m, cols] = relu( GL( relu( pw( dw_s2(c0[m]) ) + b ) ) ) (+ e3[m])
+// (deepfilternet3.py:166-185: df_conv1, then df_fc_emb over the flattened c1).  The chain is local to a row m = b T + t
+// (kt = 2: and its previous frame), so one CTA owns a slice of S c1 bins (whole GL groups: S * 64 % Ig == 0) of every
+// row tile it visits and c1 never leaves the SM.  Per row tile and bin j of the slice, each consumer warp
+//   1. forms the depthwise result of its 16 rows right in mma.sync A-fragment layout from the three c0 bins 2j-1 .. 2j+1
+//      (fp32 TMA boxes in a ring) and splits it into BF16 hi / lo (BF16x3),
+//   2. multiplies it by the 1x1 weight (the df_conv1.pw_sw image in shared memory, ldmatrix),
+//   3. turns the accumulators into c1 = relu(acc + b) split into hi / lo -- the accumulator fragments of n-tiles 2k, 2k + 1
+//      are the A fragment of K step k of the grouped linear, so c1 stays in registers --
+//   4. multiplies that by the slice's GL weights (the df_fc_emb.gl_bx image, resident) into the GL accumulators.
+// The arithmetic and its order are those of k_dwpw_bx<DW_S2> followed by k_gl_bx, so the output bits are the same.
+//   warps 0-7: rows [16 w, +16) of the tile; warp 8: TMA producer.  A tile is 128 rows of c0 starting KT - 1 rows before
+//   its first output row (kt = 2: box row 0 is the halo frame of box row 1), so it produces RT = 128 - (KT - 1) rows.
+// Slices of one row tile are adjacent in launch order: the edge bin 2 j0 - 1 that two slices share comes from L2.
+constexpr int kDeThreads = 288, kDeMaxStages = 6, kDeMaxChunks = 4;
+constexpr uint32_t kDeBin = 32768;   // one c0 bin of a tile: 128 rows x 64 fp32 as two [128][32] swizzled boxes
+
+struct DfEmbParams {
+    const float *dw;      // df_conv1 depthwise taps [kt][3][64]
+    const float *bias;    // [64]
+    const float *pw_sw;   // df_conv1.pw_sw: [hi | lo] x [64 n][64 k] BF16, 128B-swizzled rows
+    const unsigned short *w_img;  // df_fc_emb.gl_bx: [hi | lo][G][Ig/8][Hgp/8][8][8] BF16
+    const float *res; int64_t ldr;             // e3 or null
+    unsigned short *y_hi, *y_lo; int64_t ldp;  // emb_in planes (pre-offset to the first output column)
+    int M, T, G, Ig, Hg, Hgp, S, stages;
+    float oscale, ooffset;
+    const int64_t *first;  // kt = 2, streaming slots: first frame of each stream (stream_first), or null
+    int64_t w0;
+};
+
+template <int KT>
+__global__ void __launch_bounds__(kDeThreads, 1)
+k_dwpw_gl(const __grid_constant__ CUtensorMap tmC0, const __grid_constant__ DfEmbParams p) {
+    extern __shared__ __align__(1024) unsigned char de_smem_raw[];
+    const uint32_t sb = (smem_u32(de_smem_raw) + 1023u) & ~1023u;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    constexpr int RT = 128 - (KT - 1);
+    const int ntiles = (p.M + RT - 1) / RT;
+    const int j0 = blockIdx.x * p.S;                          // c1 bins [j0, j0 + S)
+    const int f_lo = j0 > 0 ? 2 * j0 - 1 : 0, f_hi = 2 * (j0 + p.S);   // c0 bins [f_lo, f_hi) of every tile
+    const int gps = p.S * kCh / p.Ig, cpg = p.Hgp / 16, nch = gps * cpg;
+    const int g0 = j0 * kCh / p.Ig;                           // first GL group of the slice
+    const uint32_t gbytes = (uint32_t)p.Ig * p.Hgp * 2;       // one group's block in one plane
+    const uint32_t wplane = gbytes * gps;
+    const uint32_t lbo = (uint32_t)(p.Hgp / 8) * 128u;
+    // shared memory map
+    const uint32_t s_c0 = sb;                                          // [stages][32 KB]
+    const uint32_t s_pw = s_c0 + (uint32_t)p.stages * kDeBin;          // 16 KB (1024-aligned)
+    const uint32_t s_w = s_pw + 2u * kCh * 128u;                       // GL weights hi | lo
+    const uint32_t s_bias = s_w + 2 * wplane;                          // [64]
+    const uint32_t s_dw = s_bias + 256u;                               // depthwise taps [KT][3][64]
+    const uint32_t s_bar = (s_dw + KT * 3 * kCh * 4u + 127u) & ~127u;
+    const uint32_t b_full = s_bar, b_empty = s_bar + 8 * kDeMaxStages, b_w = b_empty + 8 * kDeMaxStages;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < p.stages; s++) { mbar_init_a(b_full + 8 * s, 1); mbar_init_a(b_empty + 8 * s, 8); }
+        mbar_init_a(b_w, 1);
+        fence_barrier_init();
+        mbar_expect_tx_a(b_w, 2u * kCh * 128u + 2 * wplane);
+        bulk_load(s_pw, p.pw_sw, 2u * kCh * 128u, b_w);
+        const unsigned char *src = reinterpret_cast<const unsigned char *>(p.w_img);
+        bulk_load(s_w, src + (size_t)g0 * gbytes, wplane, b_w);
+        bulk_load(s_w + wplane, src + (size_t)p.G * gbytes + (size_t)g0 * gbytes, wplane, b_w);
+    }
+    if (threadIdx.x < kCh / 4) sts128(s_bias + threadIdx.x * 16, __ldg(reinterpret_cast<const float4 *>(p.bias) + threadIdx.x));
+    for (int i = threadIdx.x; i < KT * 3 * kCh / 4; i += kDeThreads) sts128(s_dw + i * 16, __ldg(reinterpret_cast<const float4 *>(p.dw) + i));
+    __syncthreads();
+    if (warp == 8) {
+        // ===== TMA producer: c0 bins f_lo .. f_hi - 1 of every tile, in order
+        if (lane == 0) {
+            tma_prefetch_desc(&tmC0);
+            int it = 0;
+            for (int tile = blockIdx.y; tile < ntiles; tile += gridDim.y) {
+                const int row0 = tile * RT - (KT - 1);   // may be -1: out-of-bounds rows arrive as zeros
+                for (int f = f_lo; f < f_hi; f++, it++) {
+                    const int s = it % p.stages, n = it / p.stages;
+                    if (n > 0) mbar_wait_a(b_empty + 8 * s, (uint32_t)((n - 1) & 1));
+                    mbar_expect_tx_a(b_full + 8 * s, kDeBin);
+                    const uint32_t dst = s_c0 + (uint32_t)s * kDeBin;
+                    asm volatile(
+                        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                        ::"r"(dst), "l"((uint64_t)&tmC0), "r"(f * kCh), "r"(row0), "r"(b_full + 8 * s) : "memory");
+                    asm volatile(
+                        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                        ::"r"(dst + kDeBin / 2), "l"((uint64_t)&tmC0), "r"(f * kCh + 32), "r"(row0), "r"(b_full + 8 * s) : "memory");
+                }
+            }
+        }
+        return;
+    }
+    // ===== consumers.  Lane (g = lane / 4, q = lane % 4) holds A-fragment elements of rows 16 w + g + 8 rs and channels
+    //       16 ks + 8 h + 2 q + {0, 1} (register rs + 2 h of K step ks)
+    const int g = lane >> 2, q = lane & 3, mat = lane >> 3, rr = lane & 7;
+    mbar_wait_a(b_w, 0);
+    int it = 0;   // ring index of the tile's first c0 bin
+    for (int tile = blockIdx.y; tile < ntiles; tile += gridDim.y, it += f_hi - f_lo) {
+        const int row0 = tile * RT - (KT - 1);
+        // taps present per (row half rs, time tap dt): kt = 2 reads zero padding before the stream's first frame
+        bool tap_ok[2][KT];
+#pragma unroll
+        for (int rs = 0; rs < 2; rs++) {
+            const int r = warp * 16 + g + 8 * rs, m = row0 + r;
+#pragma unroll
+            for (int dt = 0; dt < KT; dt++) tap_ok[rs][dt] = true;
+            if (KT > 1) {
+                const int b = m >= 0 && m < p.M ? m / p.T : 0, t = m - b * p.T;
+                const int t_first = stream_first(p.first, b, p.w0);
+#pragma unroll
+                for (int dt = 0; dt < KT; dt++) tap_ok[rs][dt] = r - (KT - 1) + dt >= 0 && t - (KT - 1 - dt) >= t_first;
+            }
+        }
+        float gacc[kDeMaxChunks][2][4];
+#pragma unroll
+        for (int c = 0; c < kDeMaxChunks; c++)
+#pragma unroll
+            for (int e = 0; e < 8; e++) gacc[c][e >> 2][e & 3] = 0.f;
+        for (int jj = 0; jj < p.S; jj++) {
+            const int j = j0 + jj;
+            // ---- 1. depthwise (taps in the order of k_dwpw_bx: time tap, then bins 2j-1, 2j, 2j+1) -> BF16 hi / lo
+            uint32_t slot[3];
+#pragma unroll
+            for (int df = 0; df < 3; df++) {
+                const int f = 2 * j - 1 + df;
+                const int i = it + (f < f_lo ? 0 : f - f_lo);
+                slot[df] = s_c0 + (uint32_t)(i % p.stages) * kDeBin;
+                if (f >= f_lo) mbar_wait_a(b_full + 8 * (i % p.stages), (uint32_t)((i / p.stages) & 1));
+            }
+            uint32_t ah[4][4], al[4][4];
+#pragma unroll
+            for (int ks = 0; ks < 4; ks++)
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const int ch = 16 * ks + 8 * h + 2 * q;   // box (ch / 32), 16-byte chunk (ch % 32) / 4, float (ch % 4)
+                    const uint32_t cbase = (uint32_t)(ch >> 5) * (kDeBin / 2) + (uint32_t)(ch & 3) * 4u;
+                    const int chunk = (ch & 31) >> 2;
+#pragma unroll
+                    for (int rs = 0; rs < 2; rs++) {
+                        const int r = warp * 16 + g + 8 * rs;
+                        float2 acc = make_float2(0.f, 0.f);
+#pragma unroll
+                        for (int dt = 0; dt < KT; dt++) {
+                            if (!tap_ok[rs][dt]) continue;
+                            const int rb = r - (KT - 1) + dt;   // box row of this time tap
+                            const uint32_t o = cbase + (uint32_t)rb * 128u + (uint32_t)((chunk ^ (rb & 7)) << 4);
+#pragma unroll
+                            for (int df = 0; df < 3; df++) {
+                                if (df == 0 && j == 0) continue;
+                                float2 x;
+                                asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x.x), "=f"(x.y) : "r"(slot[df] + o));
+                                float2 w;
+                                asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(w.x), "=f"(w.y) : "r"(s_dw + 4u * ((dt * 3 + df) * kCh + ch)));
+                                acc.x = fmaf(x.x, w.x, acc.x);
+                                acc.y = fmaf(x.y, w.y, acc.y);
+                            }
+                        }
+                        bf16x2_split(acc.x, acc.y, ah[ks][rs + 2 * h], al[ks][rs + 2 * h]);
+                    }
+                }
+            // c0 bins this warp no longer reads: 2j-1 and 2j (2j+1 is the next bin's left tap, unless j is the slice's last)
+            __syncwarp();
+            if (lane == 0) {
+                for (int f = 2 * j - 1; f <= 2 * j + (jj + 1 == p.S ? 1 : 0); f++)
+                    if (f >= f_lo) mbar_arrive_a(b_empty + 8 * ((it + f - f_lo) % p.stages));
+            }
+            // ---- 2. 1x1 conv (order of warp_mma_sw128_k64<1>)
+            float acc[8][4];
+#pragma unroll
+            for (int nt = 0; nt < 8; nt++)
+#pragma unroll
+                for (int e = 0; e < 4; e++) acc[nt][e] = 0.f;
+#pragma unroll
+            for (int ks = 0; ks < 4; ks++)
+#pragma unroll
+                for (int np = 0; np < 4; np++) {
+                    const int n = 16 * np + rr + ((mat >> 1) << 3);
+                    const uint32_t o = sw128_off(n, 2 * ks + (mat & 1));
+                    uint32_t bh[4], bl[4];
+                    ldsm_x4(s_pw + o, bh);
+                    ldsm_x4(s_pw + 8192 + o, bl);
+                    mma_bf16x3(acc[2 * np], ah[ks], al[ks], bh[0], bh[1], bl[0], bl[1]);
+                    mma_bf16x3(acc[2 * np + 1], ah[ks], al[ks], bh[2], bh[3], bl[2], bl[3]);
+                }
+            // ---- 3. c1 = relu(acc + b) -> BF16 hi / lo A fragments of the grouped linear (K step kk = n-tiles 2 kk, 2 kk + 1)
+            uint32_t ch_[4][4], cl_[4][4];
+#pragma unroll
+            for (int nt = 0; nt < 8; nt++) {
+                const int c = 8 * nt + 2 * q;
+                float b0, b1;
+                asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(b0), "=f"(b1) : "r"(s_bias + 4 * c));
+#pragma unroll
+                for (int rs = 0; rs < 2; rs++)
+                    bf16x2_split(fmaxf(acc[nt][2 * rs] + b0, 0.f), fmaxf(acc[nt][2 * rs + 1] + b1, 0.f), ch_[nt >> 1][rs + 2 * (nt & 1)],
+                                 cl_[nt >> 1][rs + 2 * (nt & 1)]);
+            }
+            // ---- 4. grouped linear, K = this bin's 64 columns in steps of 16 (order of k_gl_bx)
+#pragma unroll
+            for (int kk = 0; kk < 4; kk++) {
+                const int col = jj * kCh + kk * 16;
+                const int gl = col / p.Ig, kq = (col - gl * p.Ig) >> 4;
+                const uint32_t wa = s_w + (uint32_t)gl * gbytes + (uint32_t)(2 * kq + (mat & 1)) * lbo + (uint32_t)rr * 16u;
+#pragma unroll
+                for (int c = 0; c < kDeMaxChunks; c++) {
+                    const int cg = c - gl * cpg;
+                    if (c >= nch || cg < 0 || cg >= cpg) continue;
+                    const uint32_t o = wa + (uint32_t)(2 * cg + (mat >> 1)) * 128u;
+                    uint32_t bh[4], bl[4];
+                    ldsm_x4(o, bh);
+                    ldsm_x4(o + wplane, bl);
+                    mma_bf16x3(gacc[c][0], ch_[kk], cl_[kk], bh[0], bh[1], bl[0], bl[1]);
+                    mma_bf16x3(gacc[c][1], ch_[kk], cl_[kk], bh[2], bh[3], bl[2], bl[3]);
+                }
+            }
+        }
+        // ---- epilogue (formula of gl_store_chunk): rows below the tile's first output row are the previous tile's
+        const int64_t mrow = (int64_t)row0 + warp * 16 + g;
+        const int64_t mmin = (int64_t)tile * RT;
+#pragma unroll
+        for (int c = 0; c < kDeMaxChunks; c++) {
+            if (c >= nch) continue;
+            const int gl = c / cpg;
+#pragma unroll
+            for (int jh = 0; jh < 2; jh++) {
+                const int n = (c - gl * cpg) * 16 + jh * 8 + 2 * q;
+                if (n >= p.Hg) continue;
+                const int64_t col = (int64_t)(g0 + gl) * p.Hg + n;
+                float2 rv[2];
+#pragma unroll
+                for (int rs = 0; rs < 2; rs++) {
+                    const int64_t m = mrow + 8 * rs;
+                    rv[rs] = (p.res && m >= mmin && m < p.M) ? *reinterpret_cast<const float2 *>(p.res + m * p.ldr + col) : make_float2(0.f, 0.f);
+                }
+#pragma unroll
+                for (int rs = 0; rs < 2; rs++) {
+                    const int64_t m = mrow + 8 * rs;
+                    if (m < mmin || m >= p.M) continue;
+                    float2 x;
+                    x.x = gx_act(gacc[c][jh][2 * rs], 1) * p.oscale + p.ooffset + rv[rs].x;
+                    x.y = gx_act(gacc[c][jh][2 * rs + 1], 1) * p.oscale + p.ooffset + rv[rs].y;
+                    uint32_t hv, lv;
+                    bf16x2_split(x.x, x.y, hv, lv);
+                    *reinterpret_cast<uint32_t *>(p.y_hi + m * p.ldp + col) = hv;
+                    *reinterpret_cast<uint32_t *>(p.y_lo + m * p.ldp + col) = lv;
+                }
+            }
+        }
+    }
+}
+
 // fp32 [M][K] (row pitch ldx) -> BF16 hi / lo planes [M][K] (pitch K): fallback producer for inputs whose own
 // producer wrote none (ensure_planes in dfb_model.cu)
 __global__ void __launch_bounds__(256) k_to_planes(const float *__restrict__ x, int64_t ldx, int64_t M, int K,
@@ -332,6 +581,59 @@ int launch_gl_bx(cudaStream_t s, const unsigned short *x_hi, const unsigned shor
     if (groups > ntiles) groups = ntiles;
     DFB_PROF("k_gl_bx", s);
     k_gl_bx<<<dim3((unsigned)slices, (unsigned)groups), kGxThreads, smem, s>>>(mh, ml, p);
+    DFB_LAUNCH_CHECK();
+    return DFB_OK;
+}
+
+// Slice width S (c1 bins per CTA: the fewest that hold whole GL groups) and ring depth of k_dwpw_gl for df_fc_emb = (G, Ig,
+// Hg) over Fd / 2 c1 bins; false when the shape is outside the kernel (the caller keeps df_conv1 and df_fc_emb apart).
+bool df_emb_geometry(int Fd, int G, int Ig, int Hg, int kt, int *s_out, int *stages_out) {
+    if ((kt != 1 && kt != 2) || Fd % 2 || Ig % 16 || Hg % 4 || G < 1 || G * Ig != Fd / 2 * kCh) return false;
+    int S = 1;
+    while ((S * kCh) % Ig) S++;
+    const int Hgp = (Hg + 15) / 16 * 16;
+    if ((Fd / 2) % S || (S * kCh / Ig) * (Hgp / 16) > kDeMaxChunks) return false;
+    const int fixed = 1024 + 2 * kCh * 128 + S * kCh * Hgp * 4 + 256 + kt * 3 * kCh * 4 + 128 + 2 * 8 * kDeMaxStages + 8;
+    int stages = (227 * 1024 - fixed) / (int)kDeBin;
+    if (stages > kDeMaxStages) stages = kDeMaxStages;
+    if (stages < 3) return false;   // bins 2j-1 .. 2j+1 are in use at once
+    *s_out = S; *stages_out = stages;
+    return true;
+}
+
+// emb_in planes (y_hi / y_lo, pitch ldp, pre-offset to the first column) = relu(df_fc_emb(df_conv1(c0))) (+ res) over
+// M = B * T rows of c0 [M][Fd][64]
+int launch_df_emb(cudaStream_t s, const float *c0, int64_t M, int T, int Fd, int kt, const float *dw, const float *bias,
+                  const float *pw_sw, const float *w_img, int G, int Ig, int Hg, const float *res, int64_t ldr,
+                  unsigned short *y_hi, unsigned short *y_lo, int64_t ldp, const int64_t *first, int64_t w0) {
+    int S = 0, stages = 0;
+    if (!df_emb_geometry(Fd, G, Ig, Hg, kt, &S, &stages) || M <= 0 || M > 0x7fffffff - 256 || T <= 0 || M % T ||
+        (res && ((ldr % 2) || ((uintptr_t)res & 7))) || (ldp % 2) || ((uintptr_t)y_hi & 3) || ((uintptr_t)y_lo & 3) ||
+        ((uintptr_t)c0 & 15) || ((uintptr_t)w_img & 15) || ((uintptr_t)pw_sw & 15))
+        return fail(DFB_ERR_UNSUPPORTED, "df_conv1 + df_fc_emb kernel: shape G %d Ig %d Hg %d kt %d", G, Ig, Hg, kt);
+    CUtensorMap mc;
+    int rc;
+    if ((rc = cached_map_f32_sw128(&mc, c0, M, (int64_t)Fd * kCh, (int64_t)Fd * kCh, 128))) return rc;
+    const int Hgp = (Hg + 15) / 16 * 16;
+    DfEmbParams p{dw, bias, pw_sw, reinterpret_cast<const unsigned short *>(w_img), res, ldr, y_hi, y_lo, ldp,
+                  (int)M, T, G, Ig, Hg, Hgp, S, stages, 1.f, 0.f, first, w0};
+    const int smem = 1024 + stages * (int)kDeBin + 2 * kCh * 128 + S * kCh * Hgp * 4 + 256 + kt * 3 * kCh * 4 + 128 + 2 * 8 * kDeMaxStages + 8;
+    static PerDeviceOnce attr_once;
+    if (auto once_guard = attr_once.first()) {
+        DFB_CUDA(cudaFuncSetAttribute(k_dwpw_gl<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        DFB_CUDA(cudaFuncSetAttribute(k_dwpw_gl<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    }
+    int dev = 0, sms = 0;
+    DFB_CUDA(cudaGetDevice(&dev));
+    DFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const int slices = Fd / 2 / S, rt = 128 - (kt - 1);
+    const int ntiles = (int)((M + rt - 1) / rt);
+    int groups = sms / slices;
+    if (groups < 1) groups = 1;
+    if (groups > ntiles) groups = ntiles;
+    DFB_PROF("k_dwpw_gl", s);
+    if (kt == 1) k_dwpw_gl<1><<<dim3((unsigned)slices, (unsigned)groups), kDeThreads, smem, s>>>(mc, p);
+    else k_dwpw_gl<2><<<dim3((unsigned)slices, (unsigned)groups), kDeThreads, smem, s>>>(mc, p);
     DFB_LAUNCH_CHECK();
     return DFB_OK;
 }

@@ -662,7 +662,7 @@ int run_gl(cudaStream_t s, const float *x, int64_t ldx, const float *w, const fl
 // x_hi/x_lo: BF16 planes of x (written by the producing grouped linear), pl_hi/pl_lo: scratch planes for the
 // inter-layer hidden state, the input of the next layer's projection GEMM.
 int run_gru(dfb_model *m, cudaStream_t s, const char *name, int layers, int H, int in_dim, const float *res_last, float *y,
-            float *xproj, float *tmp_h, int B, int T, const unsigned short *x_hi, const unsigned short *x_lo,
+            float *xproj, int B, int T, const unsigned short *x_hi, const unsigned short *x_lo,
             unsigned short *pl_hi, unsigned short *pl_lo, int wide, unsigned short *out_hi, unsigned short *out_lo,
             bool *out_planes_ok, const GruChunk *ck) {
     if (out_planes_ok) *out_planes_ok = false;
@@ -686,7 +686,7 @@ int run_gru(dfb_model *m, cudaStream_t s, const char *name, int layers, int H, i
             return rc;
         if ((rc = launch_gemm_bf16x3(s, cur_hi, cur_lo, cur_dim, w_hi, w_lo, b_ih, xproj, 3 * H, M, 3 * H, cur_dim))) return rc;
         const bool last = l == layers - 1;
-        float *dst = last ? y : tmp_h;
+        float *dst = last ? y : nullptr;   // a middle layer's output feeds only the next projection, which reads its planes
         float *hs = ck && ck->h ? ck->h + (int64_t)l * ck->Bs * H : nullptr;   // carried state of this layer [Bs][H], rows [0, B)
         GruWindow gw{ck && ck->have_state ? hs : nullptr, hs, t0, T, ck ? ck->first : nullptr, ck ? ck->w0 : 0};
         // the last layer's planes feed a grouped linear and include the residual; the others feed the next projection
@@ -697,7 +697,7 @@ int run_gru(dfb_model *m, cudaStream_t s, const char *name, int layers, int H, i
         if (last && hi && out_planes_ok) *out_planes_ok = true;
         cur_hi = pl_hi; cur_lo = pl_lo;
         cur_dim = H;
-        // middle layers may rewrite tmp_h and the scratch planes in place: the recurrence only reads xproj, which the
+        // middle layers may rewrite the scratch planes in place: the recurrence only reads xproj, which the
         // projection GEMM above has already produced from the previous contents of the planes.
     }
     return DFB_OK;
@@ -732,10 +732,10 @@ int run_dwpw(cudaStream_t s, DwPwParams p, int B, const float *w_sw = nullptr) {
 
 // Buffers of one forward pass (all from the model arena).
 struct FwdBufs {
-    float *e0, *e1, *e2, *e3, *c0, *c1, *emb_in, *emb, *g_a, *g_b, *g_h, *xproj, *dec_emb, *d3, *d2, *d1, *dfc;
+    float *e0, *e1, *e2, *e3, *c0, *c1, *emb_in, *emb, *g_a, *g_b, *xproj, *dec_emb, *d3, *d2, *d1, *dfc;
     unsigned short *ga_hi, *ga_lo, *gh_hi, *gh_lo;  // BF16 planes of g_a / inter-layer h (tensor-core projections)
     // second set of GRU scratch: the DF decoder runs concurrently with the ERB decoder on another stream
-    float *g_a2, *g_h2, *xproj2, *dfskip;
+    float *g_a2, *xproj2, *dfskip;
     unsigned short *ga2_hi, *ga2_lo, *gh2_hi, *gh2_lo;
     // BF16 hi / lo planes of the grouped linears' inputs (tensor-core path): c1, emb_in, GRU outputs, emb
     unsigned short *c1_hi, *c1_lo, *embin_hi, *embin_lo, *gb_hi, *gb_lo, *emb_hi, *emb_lo, *dfc_hi, *dfc_lo;
@@ -771,6 +771,16 @@ static size_t fwd_plan_v1(const dfb_model_config &c, size_t M, Arena *a, FwdBufs
 }
 
 // Carves the activations of `M` frames out of `a` (or only counts bytes when a == nullptr).
+// df_conv1 + df_fc_emb run as one kernel (k_dwpw_gl) for this configuration: df_fc_emb's shape is built and enc.emb_gru.in
+// runs on the tensor-core grouped linear (weights.py packs the tensor-core images of every such shape)
+static bool fused_emb_shape(const dfb_model_config &c) {
+    const int Fd = c.nb_df, ED = c.nb_erb / 4 * kCh, I = Fd / 2 * kCh, G = c.g_df_fc_emb, Ge = c.g_enc_in, H = c.emb_hidden;
+    const int emb_in_dim = c.enc_concat ? 2 * ED : ED;
+    int de_s, de_st, gpc, hgp, stg;
+    return c.model_kind != 1 && G > 0 && I % G == 0 && ED % G == 0 && df_emb_geometry(Fd, G, I / G, ED / G, c.conv_kt, &de_s, &de_st) &&
+           Ge > 0 && emb_in_dim % Ge == 0 && H % Ge == 0 && gl_bx_geometry(Ge, emb_in_dim / Ge, H / Ge, &gpc, &hgp, &stg);
+}
+
 static size_t fwd_plan(const dfb_model_config &c, size_t M, Arena *a, FwdBufs *f) {
     if (c.model_kind == 1 && !a) return fwd_plan_v1(c, M, nullptr, nullptr);
     const int E = c.nb_erb, Fd = c.nb_df, H = c.emb_hidden, Hd = c.df_hidden;
@@ -789,13 +799,17 @@ static size_t fwd_plan(const dfb_model_config &c, size_t M, Arena *a, FwdBufs *f
     t.e3 = c.enc_concat ? t.emb_in : take(M * ED);  // DFN2: e3 lives inside the concat buffer
     t.c0 = take(M * Fd * kCh); t.c1 = take(M * (Fd / 2) * kCh);
     t.emb = take(M * emb_dim);
-    t.g_a = take(M * Hmax); t.g_b = take(M * Hmax); t.g_h = take(M * Hmax);
+    t.g_a = take(M * Hmax); t.g_b = take(M * Hmax);
+    // the chunk planner sizes time windows by this plan's bytes per frame (so they decide the chunk boundaries, and with
+    // them the output bits of long signals): buffers that the path no longer uses -- the GRU middle layers' fp32 outputs
+    // here and below, c1's planes when k_dwpw_gl runs -- keep their place
+    take(M * Hmax);
     t.xproj = take(M * 3 * Hmax);
     t.dec_emb = take(M * ED); t.d3 = take(M * ED); t.d2 = take(M * (E / 2) * kCh);
     t.d1 = take(M * E * kCh); t.dfc = take(M * Hmax);
     t.ga_hi = reinterpret_cast<unsigned short *>(take(M * Hmax / 2)); t.ga_lo = reinterpret_cast<unsigned short *>(take(M * Hmax / 2));
     t.gh_hi = reinterpret_cast<unsigned short *>(take(M * Hmax / 2)); t.gh_lo = reinterpret_cast<unsigned short *>(take(M * Hmax / 2));
-    t.g_a2 = take(M * Hmax); t.g_h2 = take(M * Hmax); t.xproj2 = take(M * 3 * Hmax); t.dfskip = take(M * Hmax);
+    t.g_a2 = take(M * Hmax); take(M * Hmax); t.xproj2 = take(M * 3 * Hmax); t.dfskip = take(M * Hmax);
     t.ga2_hi = reinterpret_cast<unsigned short *>(take(M * Hmax / 2)); t.ga2_lo = reinterpret_cast<unsigned short *>(take(M * Hmax / 2));
     t.gh2_hi = reinterpret_cast<unsigned short *>(take(M * Hmax / 2)); t.gh2_lo = reinterpret_cast<unsigned short *>(take(M * Hmax / 2));
     auto take16 = [&](size_t n) { return reinterpret_cast<unsigned short *>(take((n + 1) / 2)); };
@@ -907,7 +921,34 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
     m->dbg["d2"] = {f.d2, M * (E / 2) * kCh}; m->dbg["d1"] = {f.d1, M * E * kCh}; m->dbg["dfc"] = {f.dfc, M * Hd};
     m->dbg["g_a"] = {f.g_a, M * (H > Hd ? H : Hd)}; m->dbg["g_b"] = {f.g_b, M * (H > Hd ? H : Hd)};
     m->dbg["xproj"] = {f.xproj, M * 3 * (H > Hd ? H : Hd)};
+    // BF16 planes of emb_in, fetched as pairs of BF16 per float word
+    m->dbg["emb_in_hi"] = {reinterpret_cast<const float *>(f.embin_hi), M * emb_in_dim / 2};
+    m->dbg["emb_in_lo"] = {reinterpret_cast<const float *>(f.embin_lo), M * emb_in_dim / 2};
     const int64_t e3_fs = c.enc_concat ? 2 * ED : ED;
+    // grouped linear `wname` ([G][I/G][Hh/G]) runs on the tensor-core kernel, which reads its input as BF16 planes only
+    auto gl_is_bx = [&](const char *wname, int G, int I, int Hh) -> bool {
+        int gpc, hgp, stg;
+        return G > 0 && I % G == 0 && Hh % G == 0 && m->get(std::string(wname) + "_bx") && gl_bx_geometry(G, I / G, Hh / G, &gpc, &hgp, &stg);
+    };
+    // df_conv1 + df_fc_emb run as one kernel (k_dwpw_gl, c1 stays on chip) when df_fc_emb's shape is built and enc.emb_gru.in
+    // reads emb_in as BF16 planes (the FFMA grouped linear would read the fp32 tensor, which the fused kernel does not write)
+    const float *emb_w = m->get("enc.df_fc_emb.gl_bx");
+    const bool fused_emb = fused_emb_shape(c);
+    if (fused_emb && (!emb_w || !gl_is_bx("enc.emb_gru.in.gl", c.g_enc_in, emb_in_dim, H)))
+        return fail(DFB_ERR_INVALID, "df_fc_emb / enc.emb_gru.in: tensor-core weight images missing");
+    // fp32 activations that only feed the BF16 planes of a tensor-core consumer are not written (null): the input grouped
+    // linears' g_a / g_a2 (DeepFilterNet2 adds them to the GRU output as a residual), the last-layer GRU outputs g_b (enc,
+    // erb) and dfc (DeepFilterNet2's df_fc_a and skip read it); the GRUs' middle layers never write theirs (run_gru)
+    const bool keep_ga = c.model_kind == 2;
+    float *const enc_ga = gl_is_bx("enc.emb_gru.in.gl", c.g_enc_in, emb_in_dim, H) ? nullptr : f.g_a;
+    float *const erb_ga = !keep_ga && gl_is_bx("erb_dec.emb_gru.in.gl", c.g_erb_in, emb_dim, H) ? nullptr : f.g_a;
+    float *const df_ga = !keep_ga && gl_is_bx("df_dec.df_gru.in.gl", c.g_df_in, emb_dim, Hd) ? nullptr : f.g_a2;
+    float *const enc_gb = c.g_enc_out && gl_is_bx("enc.emb_gru.out.gl", c.g_enc_out, H, ED) ? nullptr : f.g_b;
+    float *const erb_gb = gl_is_bx("erb_dec.emb_gru.out.gl", c.g_erb_out, H, ED) ? nullptr : f.g_b;
+    float *const dfc = c.model_kind != 2 && gl_is_bx("df_dec.df_out.gl", c.g_df_out, Hd, Fd * 2 * c.df_order) ? nullptr : f.dfc;
+    if (!erb_ga) m->dbg.erase("g_a");
+    if (!erb_gb) m->dbg.erase("g_b");
+    if (!dfc) m->dbg.erase("dfc");
     // BF16 hi / lo planes [M][K] (row pitch `ld` elements) of a grouped linear's input; `ok` = already written by the producer
     struct Pl { unsigned short *hi, *lo; int64_t ld; bool ok; };
     Pl pl_c1{f.c1_hi, f.c1_lo, (int64_t)Fd / 2 * kCh, false}, pl_embin{f.embin_hi, f.embin_lo, emb_in_dim, false},
@@ -917,13 +958,15 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
     auto ensure_planes = [&](cudaStream_t st, const float *x, int64_t ldx, int K, Pl &pl) -> int {
         if (pl.ok) return DFB_OK;
         if (pl.ld != K) return fail(DFB_ERR_INVALID, "plane pitch mismatch");
+        if (!x) return fail(DFB_ERR_INVALID, "planes requested of an activation whose fp32 form was not written");
         int r = launch_to_planes(st, x, ldx, M, K, pl.hi, pl.lo);
         if (!r) pl.ok = true;
         return r;
     };
     // grouped linear `wname` ([G][I/G][Hh/G]): the BF16x3 tensor-core kernel when the shape is built, else the FFMA
     // kernel.  xin: planes of x (converted on demand); yout (optional): planes of y to produce,
-    // ycol: column offset of y inside its plane buffer
+    // ycol: column offset of y inside its plane buffer.  x / y may be null (fp32 form not written / not wanted) only where
+    // gl_is_bx holds: the FFMA kernel needs both, and a launch that cannot run without them is an error.
     auto gl = [&](cudaStream_t st, const char *wname, const float *x, int64_t ldx, Pl *xin, int G, int I, int Hh, int act,
                   const float *res, int64_t ldr, float *y, int64_t ldy, Pl *yout, int64_t ycol = 0) -> int {
         const float *w;
@@ -941,6 +984,9 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
                 return r;
             }
         }
+        if (!x || !y)
+            return fail(DFB_ERR_UNSUPPORTED, "grouped linear '%s': the tensor-core kernel cannot take this launch and the fp32 %s "
+                        "the FFMA kernel needs is not written", wname, x ? "output" : "input");
         // NB: the FFMA kernel's plane output shares y's pitch, so it can only serve plane buffers with ld == ldy
         const bool ffma_planes = yout && yout->ld == ldy;
         r = run_gl(st, x, ldx, w, nullptr, res, ldr, y, ldy, M, G, I, Hh, act, 1.f, 0.f, ffma_planes ? yh : nullptr, ffma_planes ? yl : nullptr);
@@ -990,12 +1036,14 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
             DFB_LAUNCH_CHECK();
             DFB_CUDA(cudaEventRecord(L.ev_c0, sa));
         }
-        p = mk(f.c0, Fd, (int64_t)Fd * kCh, f.c1, Fd / 2, (int64_t)Fd / 2 * kCh, c.conv_kt);
-        if ((rc = blk("enc.df_conv1", p))) return rc;
-        // c1 only feeds df_fc_emb: write its BF16 planes instead of the fp32 tensor
-        p.out = nullptr; p.out_hi = pl_c1.hi; p.out_lo = pl_c1.lo; pl_c1.ok = true;
         m->dbg.erase("c1");
-        if ((rc = run_dwpw<DW_S2>(sa, p, B, pw_sw))) return rc;
+        if (!fused_emb) {
+            p = mk(f.c0, Fd, (int64_t)Fd * kCh, f.c1, Fd / 2, (int64_t)Fd / 2 * kCh, c.conv_kt);
+            if ((rc = blk("enc.df_conv1", p))) return rc;
+            // c1 only feeds df_fc_emb: write its BF16 planes instead of the fp32 tensor
+            p.out = nullptr; p.out_hi = pl_c1.hi; p.out_lo = pl_c1.lo; pl_c1.ok = true;
+            if ((rc = run_dwpw<DW_S2>(sa, p, B, pw_sw))) return rc;
+        }
         DFB_CUDA(cudaEventRecord(L.ev_join_enc, sa));
         // DF pathway conv (needs c0 only; its result is consumed by the very last DF-decoder kernel): on the
         // low-priority stream, so its CTAs only take SMs that the critical path -- the encoder convs now, the GRU
@@ -1025,11 +1073,19 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         if ((rc = run_dwpw<DW_S1>(s, p, B, pw_sw))) return rc;
 
     }
-    DFB_CUDA(cudaStreamWaitEvent(s, L.ev_join_enc, 0));  // c0 / c1 ready
+    DFB_CUDA(cudaStreamWaitEvent(s, L.ev_join_enc, 0));  // c0 (and, unfused, c1's planes) ready
     {
         // cemb = relu(df_fc_emb(c1 flat)); emb_in = e3 flat + cemb  (DFN2: concat)
         const int I = Fd / 2 * kCh;
-        if (c.enc_concat) {  // the first half's planes were written by erb_conv3
+        if (fused_emb) {  // only emb_in's planes are written: enc.emb_gru.in reads nothing else
+            DwPwParams p{};
+            if ((rc = blk("enc.df_conv1", p))) return rc;
+            const int G = c.g_df_fc_emb;
+            rc = launch_df_emb(s, f.c0, M, T, Fd, c.conv_kt, p.dw, p.bias, pw_sw, emb_w, G, I / G, ED / G, c.enc_concat ? nullptr : f.e3,
+                               ED, pl_embin.hi + (c.enc_concat ? ED : 0), pl_embin.lo + (c.enc_concat ? ED : 0), pl_embin.ld, first, W0);
+            if (!rc) pl_embin.ok = true;
+            m->dbg.erase("emb_in");
+        } else if (c.enc_concat) {  // the first half's planes were written by erb_conv3
             rc = gl(s, "enc.df_fc_emb.gl", f.c1, I, &pl_c1, c.g_df_fc_emb, I, ED, ACT_RELU, nullptr, 0, f.emb_in + ED, emb_in_dim,
                     &pl_embin, ED);
         } else {
@@ -1039,14 +1095,15 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
     }
     {
         // enc.emb_gru: linear_in + ReLU -> GRU -> [linear_out + ReLU]
-        if ((rc = gl(s, "enc.emb_gru.in.gl", f.emb_in, emb_in_dim, &pl_embin, c.g_enc_in, emb_in_dim, H, ACT_RELU, nullptr, 0, f.g_a, H,
+        if ((rc = gl(s, "enc.emb_gru.in.gl", fused_emb ? nullptr : f.emb_in, emb_in_dim, &pl_embin, c.g_enc_in, emb_in_dim, H, ACT_RELU,
+                     nullptr, 0, enc_ga, H,
                      &pl_ga))) return rc;
-        float *gout = c.g_enc_out ? f.g_b : f.emb;
+        float *gout = c.g_enc_out ? enc_gb : f.emb;
         Pl &pl_gout = c.g_enc_out ? pl_gb : pl_emb;
-        if ((rc = run_gru(m, s, "enc.emb_gru", c.enc_gru_layers, H, H, nullptr, gout, f.xproj, f.g_h, B, T, f.ga_hi, f.ga_lo,
+        if ((rc = run_gru(m, s, "enc.emb_gru", c.enc_gru_layers, H, H, nullptr, gout, f.xproj, B, T, f.ga_hi, f.ga_lo,
                           f.gh_hi, f.gh_lo, 0, pl_gout.hi, pl_gout.lo, &pl_gout.ok, cx ? &ck_enc : nullptr))) return rc;
         if (c.g_enc_out) {
-            if ((rc = gl(s, "enc.emb_gru.out.gl", f.g_b, H, &pl_gb, c.g_enc_out, H, ED, ACT_RELU, nullptr, 0, f.emb, emb_dim, &pl_emb)))
+            if ((rc = gl(s, "enc.emb_gru.out.gl", enc_gb, H, &pl_gb, c.g_enc_out, H, ED, ACT_RELU, nullptr, 0, f.emb, emb_dim, &pl_emb)))
                 return rc;
         }
         // the decoders read emb's planes on two streams: make sure they exist before the fork
@@ -1084,11 +1141,11 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
     // ---- DF decoder (deepfilternet3.py:323-331), on the auxiliary stream (forked after the encoder)
     {
         cudaStream_t s = sa;  // shadows the caller stream inside this block
-        if ((rc = gl(s, "df_dec.df_gru.in.gl", f.emb, emb_dim, &pl_emb, c.g_df_in, emb_dim, Hd, ACT_RELU, nullptr, 0, f.g_a2, Hd, &pl_ga2)))
+        if ((rc = gl(s, "df_dec.df_gru.in.gl", f.emb, emb_dim, &pl_emb, c.g_df_in, emb_dim, Hd, ACT_RELU, nullptr, 0, df_ga, Hd, &pl_ga2)))
             return rc;
         const float *res = c.model_kind == 2 ? f.g_a2 : (early_skip ? f.dfskip : nullptr);
         if (early_skip) DFB_CUDA(cudaStreamWaitEvent(s, L.ev_skip, 0));
-        if ((rc = run_gru(m, s, "df_dec.df_gru", c.df_gru_layers, Hd, Hd, res, f.dfc, f.xproj2, f.g_h2, B, T, f.ga2_hi, f.ga2_lo,
+        if ((rc = run_gru(m, s, "df_dec.df_gru", c.df_gru_layers, Hd, Hd, res, dfc, f.xproj2, B, T, f.ga2_hi, f.ga2_lo,
                           f.gh2_hi, f.gh2_lo, wide_df, pl_dfc.hi, pl_dfc.lo, &pl_dfc.ok, cx ? &ck_df : nullptr))) return rc;
         if (c.g_df_skip && !early_skip) {
             if ((rc = gl(s, "df_dec.df_skip.gl", f.emb, emb_dim, &pl_emb, c.g_df_skip, emb_dim, Hd, ACT_NONE, f.dfc, Hd, f.dfc, Hd, nullptr)))
@@ -1103,20 +1160,20 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         const int O2 = 2 * c.df_order;
         // coefs = tanh(df_out(c)) + df_convp(c0); the pathway term was written by k_df_convp_tc on the low-priority stream
         DFB_CUDA(cudaStreamWaitEvent(s, L.ev_convp, 0));
-        if ((rc = gl(s, "df_dec.df_out.gl", f.dfc, Hd, &pl_dfc, c.g_df_out, Hd, Fd * O2, ACT_TANH, d_coefs, (int64_t)Fd * O2, d_coefs,
+        if ((rc = gl(s, "df_dec.df_out.gl", dfc, Hd, &pl_dfc, c.g_df_out, Hd, Fd * O2, ACT_TANH, d_coefs, (int64_t)Fd * O2, d_coefs,
                      (int64_t)Fd * O2, nullptr))) return rc;
     }
     DFB_CUDA(cudaEventRecord(L.ev_join, sa));
     // ---- ERB decoder (deepfilternet3.py:245-254)
     {
-        if ((rc = gl(s, "erb_dec.emb_gru.in.gl", f.emb, emb_dim, &pl_emb, c.g_erb_in, emb_dim, H, ACT_RELU, nullptr, 0, f.g_a, H, &pl_ga)))
+        if ((rc = gl(s, "erb_dec.emb_gru.in.gl", f.emb, emb_dim, &pl_emb, c.g_erb_in, emb_dim, H, ACT_RELU, nullptr, 0, erb_ga, H, &pl_ga)))
             return rc;
         // DFN2 (SqueezedGRU): identity skip around the GRU, y = GRU(x) + x  (modules.py:695-697)
         const float *res = c.model_kind == 2 ? f.g_a : nullptr;
         pl_gb.ok = false;
-        if ((rc = run_gru(m, s, "erb_dec.emb_gru", c.erb_gru_layers, H, H, res, f.g_b, f.xproj, f.g_h, B, T, f.ga_hi, f.ga_lo,
+        if ((rc = run_gru(m, s, "erb_dec.emb_gru", c.erb_gru_layers, H, H, res, erb_gb, f.xproj, B, T, f.ga_hi, f.ga_lo,
                           f.gh_hi, f.gh_lo, wide_erb, pl_gb.hi, pl_gb.lo, &pl_gb.ok, cx ? &ck_erb : nullptr))) return rc;
-        if ((rc = gl(s, "erb_dec.emb_gru.out.gl", f.g_b, H, &pl_gb, c.g_erb_out, H, ED, ACT_RELU, nullptr, 0, f.dec_emb, ED, nullptr)))
+        if ((rc = gl(s, "erb_dec.emb_gru.out.gl", erb_gb, H, &pl_gb, c.g_erb_out, H, ED, ACT_RELU, nullptr, 0, f.dec_emb, ED, nullptr)))
             return rc;
         if (cx && cx->dec_tail && c.conv_kt > 1) {
             // kt = 2 decoder convs look one frame back into the halo, where this window's recurrence did not run: restore
@@ -1299,7 +1356,7 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
             const std::string nm = std::string(name) + ".g" + std::to_string(l);
             GruChunk ck{hbase ? hbase + (int64_t)l * B * H : nullptr, false, 0, B, nullptr, 0};
             bool ok = false;
-            int r = run_gru(m, st, nm.c_str(), 1, H, H, nullptr, y[l], xproj, nullptr, B, T, ch, cl, f.scr_hi, f.scr_lo, 0, y_hi[l], y_lo[l], &ok,
+            int r = run_gru(m, st, nm.c_str(), 1, H, H, nullptr, y[l], xproj, B, T, ch, cl, f.scr_hi, f.scr_lo, 0, y_hi[l], y_lo[l], &ok,
                             hbase ? &ck : nullptr);
             if (r) return r;
             ch = y_hi[l]; cl = y_lo[l];

@@ -563,7 +563,7 @@ struct GruTcParams {
     const float *whh;    // [3H][H]
     const float *bhh;    // [3H]
     const float *res;    // optional [B,T,H], added to the OUTPUT only
-    float *hout;         // [B,T,H]
+    float *hout;         // [B,T,H], or null: only the planes are wanted
     unsigned short *hout_hi, *hout_lo;  // optional BF16 hi/lo planes of hout (A operand of the next projection GEMM)
     int planes_res;      // 1: the planes hold hout + res (input of a grouped linear), 0: the residual-free h
     // time-chunked execution: steps t = 0 .. T-1 are frames t0 + t of buffers holding Ts frames per stream; the
@@ -778,7 +778,7 @@ __global__ void __launch_bounds__(GtCfg<NS, HH>::kThreads, 1) k_gru_tc(GruTcPara
             float2 ov = make_float2(hprev0, hprev1);
             if (p.hT && t + 1 == T) *reinterpret_cast<float2 *>(p.hT + (int64_t)(b0 + s) * H + gu) = ov;
             if (p.res) { const float2 rv = *reinterpret_cast<const float2 *>(p.res + o); ov.x += rv.x; ov.y += rv.y; }
-            *reinterpret_cast<float2 *>(p.hout + o) = ov;
+            if (p.hout) *reinterpret_cast<float2 *>(p.hout + o) = ov;
             if (p.hout_hi) {  // residual-free h (the next layer's projection input) or the layer output
                 if (p.planes_res && p.res) bf16x2_split(ov.x, ov.y, vhi, vlo);
                 *reinterpret_cast<uint32_t *>(p.hout_hi + o) = vhi;
@@ -873,6 +873,7 @@ static int launch_gru_tc_n(cudaStream_t s, GruTcParams p) {
 int launch_gru_tc(cudaStream_t s, const float *xproj, const float *whh, const float *bhh, const float *res, float *hout,
                   unsigned short *hout_hi, unsigned short *hout_lo, int B, int T, long long *dbg, int wide, int planes_res,
                   const GruWindow *w, int H) {
+    if (!hout && !hout_hi) return fail(DFB_ERR_INVALID, "tensor-core recurrence: neither an fp32 output nor planes");
     GruTcParams p{xproj, whh, bhh, res, hout, hout_hi, hout_lo, planes_res, w ? w->h0 : nullptr, w ? w->hT : nullptr,
                   w ? w->t0 : 0, w ? w->Ts : T, B, T, 0, dbg};
     p.first = w ? w->first : nullptr;
