@@ -15,6 +15,15 @@
 //   warps 0-7 : rows [16 w, +16) of every row tile, all gpc * Hgp <= 256 columns of the slice (ldmatrix + mma.sync,
 //               accumulators in registers), then activation / scale / residual -> fp32 and/or BF16 hi/lo plane stores
 //   warp 8    : TMA producer
+// Staged fp32 output (when y is written and shared memory holds a [128][gpc * Hg] fp32 tile next to a ring of >= 2
+// stages): each warp owns the 16 rows of the tile it computes.  The producer loads the warp's residual rows (if any) with
+// a TMA box onto the warp's own mbarrier, issued after the tile's X boxes; the warp adds them from shared memory, writes
+// the result over them (padded columns dropped, so the slice's gpc * Hg columns are contiguous) and lane 0 stores the 16
+// rows with one TMA tensor store (rows >= M are clipped).  Before the rows are overwritten again (by the next residual
+// box, or by the warp itself), lane 0 waits for the store to have read them.  The epilogue thus never waits on DRAM, and
+// its stores drain while the warp runs the next tile's MMAs.  df_out adds its residual in place (res == y): that is safe
+// because a warp's residual rows are read before the same warp's rows of y are stored, and the other CTAs own other
+// columns (slices) or other row tiles.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -38,6 +47,7 @@ struct GlBxParams {
     unsigned short *y_hi, *y_lo; int64_t ldp;
     int M, G, Ig, Hg, Hgp, gpc, act, stages;
     float oscale, ooffset;
+    int stage_y;   // fp32 output through the shared staging tile + TMA store (residual, if any, through TMA loads)
 };
 
 __device__ __forceinline__ float gx_act(float x, int act) {
@@ -46,11 +56,40 @@ __device__ __forceinline__ float gx_act(float x, int act) {
     return x;
 }
 
-// epilogue of one 16-column chunk c: fragment (n-tile j, half h) = rows mrow + 8 h, columns 2 (lane % 4) + {0, 1} of the n-tile
-__device__ __noinline__ void gl_store_chunk(const GlBxParams &p, int c, int g0, int cpg, int64_t mrow, int lane, float a00, float a01,
-                                            float a02, float a03, float a10, float a11, float a12, float a13) {
+// epilogue of one 16-column chunk c: fragment (n-tile j, half h) = rows mrow + 8 h, columns 2 (lane % 4) + {0, 1} of the n-tile.
+// st != 0: the warp's fp32 staging rows [16][gpc * Hg] (holding the residual rows when p.res): y goes there, planes to HBM
+__device__ __noinline__ void gl_store_chunk(const GlBxParams &p, int c, int g0, int cpg, int64_t mrow, int lane, uint32_t st,
+                                            float a00, float a01, float a02, float a03, float a10, float a11, float a12, float a13) {
     const float a[2][4] = {{a00, a01, a02, a03}, {a10, a11, a12, a13}};
     const int gl = c / cpg;
+    if (st) {
+        const uint32_t pitch = (uint32_t)(p.gpc * p.Hg) * 4u;
+#pragma unroll
+        for (int j = 0; j < 2; j++) {
+            const int n = (c - gl * cpg) * 16 + j * 8 + 2 * (lane & 3);
+            if (n >= p.Hg) continue;
+            const int lcol = gl * p.Hg + n;   // column inside the slice
+            const int64_t col = (int64_t)g0 * p.Hg + lcol;
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const uint32_t sa = st + (uint32_t)((lane >> 2) + 8 * h) * pitch + (uint32_t)lcol * 4u;
+                float2 rv = make_float2(0.f, 0.f);
+                if (p.res) asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(rv.x), "=f"(rv.y) : "r"(sa));
+                float2 x;
+                x.x = gx_act(a[j][2 * h], p.act) * p.oscale + p.ooffset + rv.x;
+                x.y = gx_act(a[j][2 * h + 1], p.act) * p.oscale + p.ooffset + rv.y;
+                sts64(sa, __float_as_uint(x.x), __float_as_uint(x.y));
+                const int64_t m = mrow + 8 * h;
+                if (p.y_hi && m < p.M) {
+                    uint32_t hv, lv;
+                    bf16x2_split(x.x, x.y, hv, lv);
+                    *reinterpret_cast<uint32_t *>(p.y_hi + m * p.ldp + col) = hv;
+                    *reinterpret_cast<uint32_t *>(p.y_lo + m * p.ldp + col) = lv;
+                }
+            }
+        }
+        return;
+    }
 #pragma unroll
     for (int j = 0; j < 2; j++) {
         const int n = (c - gl * cpg) * 16 + j * 8 + 2 * (lane & 3);   // column inside the group
@@ -83,7 +122,8 @@ __device__ __noinline__ void gl_store_chunk(const GlBxParams &p, int c, int g0, 
 }
 
 __global__ void __launch_bounds__(kGxThreads, 1)
-k_gl_bx(const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUtensorMap tmXlo, const __grid_constant__ GlBxParams p) {
+k_gl_bx(const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUtensorMap tmXlo, const __grid_constant__ CUtensorMap tmY,
+        const __grid_constant__ CUtensorMap tmR, const __grid_constant__ GlBxParams p) {
     extern __shared__ __align__(1024) unsigned char gx_smem_raw[];
     const uint32_t sb = (smem_u32(gx_smem_raw) + 1023u) & ~1023u;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -98,11 +138,16 @@ k_gl_bx(const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUten
     // shared memory map
     const uint32_t s_x = sb;                                             // [stages][hi | lo][16 KB]
     const uint32_t s_w = s_x + (uint32_t)p.stages * 2 * kGxBoxBytes;     // W hi | lo
-    const uint32_t s_bar = (s_w + 2 * wplane + 127u) & ~127u;            // full[6] empty[6] wbar
+    const uint32_t ybox = 16u * (uint32_t)(p.gpc * p.Hg) * 4u;           // one warp's staging rows (fp32)
+    const uint32_t s_y = s_w + 2 * wplane;                               // [8 warps][16][gpc * Hg] fp32 (stage_y)
+    const uint32_t s_bar = (s_y + (p.stage_y ? 8 * ybox : 0u) + 127u) & ~127u;   // full[6] empty[6] wbar rfull[8] rempty[8]
     const uint32_t b_full = s_bar, b_empty = s_bar + 8 * kGxMaxStages, b_w = b_empty + 8 * kGxMaxStages;
+    const uint32_t b_rfull = b_w + 8, b_rempty = b_rfull + 8 * 8;
+    const bool res_tma = p.stage_y && p.res;
     if (threadIdx.x == 0) {
         for (int s = 0; s < p.stages; s++) { mbar_init_a(b_full + 8 * s, 1); mbar_init_a(b_empty + 8 * s, 8); }
         mbar_init_a(b_w, 1);
+        for (int w = 0; w < 8; w++) { mbar_init_a(b_rfull + 8 * w, 1); mbar_init_a(b_rempty + 8 * w, 1); }
         fence_barrier_init();
         // the weight slice: two bulk copies (hi plane, lo plane)
         mbar_expect_tx_a(b_w, 2 * wplane);
@@ -115,9 +160,10 @@ k_gl_bx(const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUten
         // ===== TMA producer
         if (lane == 0) {
             tma_prefetch_desc(&tmXhi); tma_prefetch_desc(&tmXlo);
+            if (res_tma) tma_prefetch_desc(&tmR);
             const int col0 = g0 * p.Ig;
-            int it = 0;
-            for (int tile = blockIdx.y; tile < ntiles; tile += gridDim.y)
+            int it = 0, ti = 0;
+            for (int tile = blockIdx.y; tile < ntiles; tile += gridDim.y, ti++) {
                 for (int b = 0; b < nboxes; b++, it++) {
                     const int s = it % p.stages, n = it / p.stages;
                     if (n > 0) mbar_wait_a(b_empty + 8 * s, (uint32_t)((n - 1) & 1));
@@ -130,14 +176,26 @@ k_gl_bx(const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUten
                         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                         ::"r"(dst + kGxBoxBytes), "l"((uint64_t)&tmXlo), "r"(col0 + b * 64), "r"(tile * 128), "r"(b_full + 8 * s) : "memory");
                 }
+                // the tile's residual rows, one box per warp, once that warp's store of its previous tile has read them out
+                // (after the X boxes: a warp's epilogue of tile ti - 1 needs nothing issued here)
+                for (int w = 0; res_tma && w < 8; w++) {
+                    if (ti > 0) mbar_wait_a(b_rempty + 8 * w, (uint32_t)((ti - 1) & 1));
+                    mbar_expect_tx_a(b_rfull + 8 * w, ybox);
+                    asm volatile(
+                        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                        ::"r"(s_y + (uint32_t)w * ybox), "l"((uint64_t)&tmR), "r"(g0 * p.Hg), "r"(tile * 128 + 16 * w), "r"(b_rfull + 8 * w)
+                        : "memory");
+                }
+            }
         }
         return;
     }
     // ===== consumers: D[rows 16 w .. +16][chunk c] for every chunk of the slice
     const int mat = lane >> 3, rr = lane & 7;
     mbar_wait_a(b_w, 0);
-    int it = 0;
-    for (int tile = blockIdx.y; tile < ntiles; tile += gridDim.y) {
+    const uint32_t st = p.stage_y ? s_y + (uint32_t)warp * ybox : 0u;
+    int it = 0, ti = 0;
+    for (int tile = blockIdx.y; tile < ntiles; tile += gridDim.y, ti++) {
         float acc[kGxMaxChunks][2][4];
 #pragma unroll
         for (int c = 0; c < kGxMaxChunks; c++)
@@ -177,11 +235,25 @@ k_gl_bx(const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUten
         // ---- epilogue: one out-of-line call per chunk, so that this loop stays unrolled and every accumulator index constant
         //      (as one inline loop ptxas re-rolled it and moved the accumulators to local memory)
         const int64_t mrow = (int64_t)tile * 128 + warp * 16 + (lane >> 2);
+        if (res_tma) mbar_wait_a(b_rfull + 8 * warp, (uint32_t)(ti & 1));
 #pragma unroll
         for (int c = 0; c < kGxMaxChunks; c++)
             if (c < nch)
-                gl_store_chunk(p, c, g0, cpg, mrow, lane, acc[c][0][0], acc[c][0][1], acc[c][0][2], acc[c][0][3], acc[c][1][0],
+                gl_store_chunk(p, c, g0, cpg, mrow, lane, st, acc[c][0][0], acc[c][0][1], acc[c][0][2], acc[c][0][3], acc[c][1][0],
                                acc[c][1][1], acc[c][1][2], acc[c][1][3]);
+        if (st) {
+            // the staged rows -> y (one TMA store; the tensor map clips rows >= M), read out before the rows are reused
+            fence_proxy_async();
+            __syncwarp();
+            if (lane == 0) {
+                asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];"
+                             ::"l"((uint64_t)&tmY), "r"(g0 * p.Hg), "r"(tile * 128 + warp * 16), "r"(st) : "memory");
+                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+                asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+                if (res_tma) mbar_arrive_a(b_rempty + 8 * warp);
+            }
+            __syncwarp();
+        }
     }
 }
 
@@ -520,6 +592,39 @@ int cached_map_f32_sw128(CUtensorMap *out, const void *base, int64_t rows, int64
     return DFB_OK;
 }
 
+// 2-D fp32 row-major [rows][cols] (row pitch ld floats), box = [box_rows][box_cols], no swizzle: the staged epilogue of
+// k_gl_bx (residual loads, y stores)
+static int cached_map_f32_rows(CUtensorMap *out, const void *base, int64_t rows, int64_t cols, int64_t ld, int box_cols, int box_rows) {
+    static std::mutex mu;
+    static std::map<std::tuple<int, const void *, int64_t, int64_t, int64_t, int, int>, CUtensorMap> cache;
+    static PFN_encodeTiled_gl enc = nullptr;
+    int dev = 0;
+    cudaGetDevice(&dev);
+    std::lock_guard<std::mutex> g(mu);
+    auto key = std::make_tuple(dev, base, rows, cols, ld, box_cols, box_rows);
+    auto it = cache.find(key);
+    if (it != cache.end()) { *out = it->second; return DFB_OK; }
+    if (!enc) {
+        void *fp = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fp, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
+            return fail(DFB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
+        enc = (PFN_encodeTiled_gl)fp;
+    }
+    cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+    cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
+    cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
+    cuuint32_t estr[2] = {1, 1};
+    CUtensorMap m;
+    CUresult r = enc(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void *)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail(DFB_ERR_CUDA, "cuTensorMapEncodeTiled (fp32 rows) failed (%d)", (int)r);
+    if (cache.size() > 4096) cache.clear();
+    cache[key] = m;
+    *out = m;
+    return DFB_OK;
+}
+
 int launch_to_planes(cudaStream_t s, const float *x, int64_t ldx, int64_t M, int K, unsigned short *hi, unsigned short *lo) {
     if (K % 4 || ldx % 4) return fail(DFB_ERR_UNSUPPORTED, "to_planes: K = %d", K);
     int dev = 0, sms = 0;
@@ -566,9 +671,20 @@ int launch_gl_bx(cudaStream_t s, const unsigned short *x_hi, const unsigned shor
     int rc;
     if ((rc = cached_map_bf16(&mh, x_hi, M, (int64_t)G * Ig, ldx, 128)) || (rc = cached_map_bf16(&ml, x_lo, M, (int64_t)G * Ig, ldx, 128)))
         return rc;
+    // staged fp32 output: the [128][gpc * Hg] staging tile comes out of the ring, which keeps >= 2 stages
+    const int wbytes = gpc * Ig * Hgp * 4, ybytes = 128 * gpc * Hg * 4;
+    int stages_y = (227 * 1024 - 2048 - wbytes - ybytes - 256) / (2 * kGxBoxBytes);
+    if (stages_y > kGxMaxStages) stages_y = kGxMaxStages;
+    const bool stage_y = y && stages_y >= 2;
+    CUtensorMap my = mh, mr = mh;   // (unused copies when not staged / no residual)
+    if (stage_y) {
+        stages = stages_y;
+        if ((rc = cached_map_f32_rows(&my, y, M, (int64_t)G * Hg, ldy, gpc * Hg, 16))) return rc;
+        if (res && (rc = cached_map_f32_rows(&mr, res, M, (int64_t)G * Hg, ldr, gpc * Hg, 16))) return rc;
+    }
     GlBxParams p{reinterpret_cast<const unsigned short *>(w_img), res, ldr, y, ldy, y_hi, y_lo, ldp,
-                 (int)M, G, Ig, Hg, Hgp, gpc, act, stages, oscale, ooffset};
-    const int smem = 1024 + stages * 2 * kGxBoxBytes + gpc * Ig * Hgp * 4 + 128 + 256;
+                 (int)M, G, Ig, Hg, Hgp, gpc, act, stages, oscale, ooffset, stage_y ? 1 : 0};
+    const int smem = 1024 + stages * 2 * kGxBoxBytes + wbytes + (stage_y ? ybytes : 0) + 128 + 256;
     static PerDeviceOnce attr_once;
     if (auto once_guard = attr_once.first())
         DFB_CUDA(cudaFuncSetAttribute(k_gl_bx, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
@@ -580,10 +696,25 @@ int launch_gl_bx(cudaStream_t s, const unsigned short *x_hi, const unsigned shor
     if (groups < 1) groups = 1;
     if (groups > ntiles) groups = ntiles;
     DFB_PROF("k_gl_bx", s);
-    k_gl_bx<<<dim3((unsigned)slices, (unsigned)groups), kGxThreads, smem, s>>>(mh, ml, p);
+    k_gl_bx<<<dim3((unsigned)slices, (unsigned)groups), kGxThreads, smem, s>>>(mh, ml, my, mr, p);
     DFB_LAUNCH_CHECK();
     return DFB_OK;
 }
+
+}  // namespace dfb
+
+// Debug aid (bench_gl.py, tests/test_gpu_gl_bx.py): one k_gl_bx launch on caller-given device pointers
+extern "C" int dfb_debug_gl_bx(const void *x_hi, const void *x_lo, int64_t ldx, const float *w_img, const float *res, int64_t ldr,
+                               float *y, int64_t ldy, void *y_hi, void *y_lo, int64_t ldp, int64_t M, int G, int Ig, int Hg,
+                               int act, float oscale, float ooffset, void *stream) {
+    if (!x_hi || !x_lo || !w_img || (!y && !y_hi) || (!y_hi != !y_lo)) return dfb::fail(DFB_ERR_INVALID, "gl_bx: null argument");
+    const int r = dfb::launch_gl_bx((cudaStream_t)stream, (const unsigned short *)x_hi, (const unsigned short *)x_lo, ldx, w_img, res,
+                                    ldr, y, ldy, (unsigned short *)y_hi, (unsigned short *)y_lo, ldp, M, G, Ig, Hg, act, oscale, ooffset);
+    if (r == DFB_ERR_UNSUPPORTED) return dfb::fail(r, "gl_bx: shape G %d Ig %d Hg %d or pointer alignment not built", G, Ig, Hg);
+    return r;
+}
+
+namespace dfb {
 
 // Slice width S (c1 bins per CTA: the fewest that hold whole GL groups) and ring depth of k_dwpw_gl for df_fc_emb = (G, Ig,
 // Hg) over Fd / 2 c1 bins; false when the shape is outside the kernel (the caller keeps df_conv1 and df_fc_emb apart).

@@ -356,6 +356,13 @@ int dfb_model_set_max_workspace(dfb_model *m, int64_t bytes);
 /* Debug aid: steps > 0 with h_out == NULL arms clock64() phase stamps ([steps][8]) for the following
  * GRU launches; a second call with h_out != NULL copies the stamps of the last launch and disarms. */
 int dfb_debug_gru_timing(dfb_model *m, int steps, long long *h_out);
+/* Debug aid: one launch of the tensor-core grouped linear on device pointers, on `stream` (a cudaStream_t, NULL = default):
+ * y / (y_hi, y_lo) [M][G*Hg] = act(GL(x)) * oscale + ooffset + res, x given as BF16 hi / lo planes [M][G*Ig] (pitch ldx)
+ * and w_img the weight image of weights.py gl_bx_image.  y or the planes may be NULL; res may alias y.  act: 0 none,
+ * 1 ReLU, 2 tanh. */
+int dfb_debug_gl_bx(const void *x_hi, const void *x_lo, int64_t ldx, const float *w_img, const float *res, int64_t ldr,
+                    float *y, int64_t ldy, void *y_hi, void *y_lo, int64_t ldp, int64_t M, int G, int Ig, int Hg, int act,
+                    float oscale, float ooffset, void *stream);
 /* Debug aid for parity tests: copies the named activation of the LAST forward pass on this handle
  * (e0,e1,e2,e3,c0,c1,emb_in,emb,dec_emb,d3,d2,d1,dfc) to the host; returns the element count
  * (or a negative dfb_status).  Valid until the next call on the handle. */
