@@ -232,10 +232,11 @@ int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaS
 // time window of a recurrence launch: steps 0 .. T-1 are frames t0 .. of buffers holding Ts frames per stream; h0 (null:
 // zeros) / hT (null: not stored) are the carried hidden states [B][H]
 struct GruWindow { const float *h0; float *hT; int t0, Ts; const int64_t *first = nullptr; int64_t w0 = 0; /* stream_first */ };
-// tensor-core GRU recurrence, H = 256 (dfb_tc.cu); hout may be null when the planes hout_hi / hout_lo are given
+// tensor-core GRU recurrence, H = 256 or 512 (dfb_tc.cu); hout may be null when the planes hout_hi / hout_lo are given.
+// ns = 0, xg = -1: the production choice of instance; otherwise the instance <ns, H, xg> (dfb_debug_gru_tc)
 int launch_gru_tc(cudaStream_t s, const float *xproj, const float *whh, const float *bhh, const float *res, float *hout,
                   unsigned short *hout_hi, unsigned short *hout_lo, int B, int T, long long *dbg = nullptr, int wide = 0,
-                  int planes_res = 0, const GruWindow *w = nullptr, int H = 256);
+                  int planes_res = 0, const GruWindow *w = nullptr, int H = 256, int ns = 0, int xg = -1);
 // BF16x3 tensor-core GEMM on hi/lo planes (dfb_tc.cu)
 int launch_gemm_bf16x3(cudaStream_t s, const void *x_hi, const void *x_lo, int64_t ldx, const void *w_hi, const void *w_lo,
                        const float *bias, float *y, int64_t ldy, int64_t M, int N, int K);

@@ -471,7 +471,8 @@ struct dfb_model {
     std::map<std::string, std::pair<float *, int64_t>> t;  // device tensors
     std::map<std::string, std::pair<const float *, int64_t>> dbg;  // activations of the last forward
     float *slab = nullptr;
-    long long *gru_dbg = nullptr;  // device buffer for dfb_debug_gru_timing
+    long long *gru_dbg = nullptr;  // device buffer for dfb_debug_gru_timing, [gru_dbg_steps][8]
+    int gru_dbg_steps = 0;
     Arena arena;
     int dev_chunks = 0, host_chunks = 4, n_lanes = 2;   // chunk pipeline (dfb_model_set_chunking); dev_chunks 0 = auto
     int post_filter = 0, mask_only = 0;       // optional stages (dfb_model_set_options)
@@ -604,20 +605,23 @@ extern "C" void dfb_model_free(dfb_model *m) {
     delete m;
 }
 
-// Debug: when `steps` > 0, every following GRU launch stamps clock64() phases of CTA 0 into a device
-// buffer [steps][8] (k_gru_tc: 0 step start, 1 state arrived, 2 MMAs done, 3 gates done, 4 slice sent);
-// returns them for the LAST launch when called with h_out != NULL.
+// Debug: when `steps` > 0, every following GRU launch of at most `steps` steps stamps clock64() phases of CTA 0 into a
+// device buffer [steps][8] (k_gru_tc: 0 step start, 1 state arrived, 2 MMAs done, 3 gates done, 4 slice sent; the kernel
+// writes one row per step, so longer launches are not stamped); copies the rows of the armed buffer, at most `steps`
+// of them, when called with h_out != NULL.
 extern "C" int dfb_debug_gru_timing(dfb_model *m, int steps, long long *h_out) {
     if (!m) return fail(DFB_ERR_INVALID, "null model");
     cudaSetDevice(m->device);
     if (h_out && m->gru_dbg) {
+        const int n = steps < m->gru_dbg_steps ? steps : m->gru_dbg_steps;
         DFB_CUDA(cudaDeviceSynchronize());
-        DFB_CUDA(cudaMemcpy(h_out, m->gru_dbg, sizeof(long long) * 8 * steps, cudaMemcpyDeviceToHost));
+        if (n > 0) DFB_CUDA(cudaMemcpy(h_out, m->gru_dbg, sizeof(long long) * 8 * n, cudaMemcpyDeviceToHost));
     }
-    if (m->gru_dbg) { cudaFree(m->gru_dbg); m->gru_dbg = nullptr; }
+    if (m->gru_dbg) { cudaFree(m->gru_dbg); m->gru_dbg = nullptr; m->gru_dbg_steps = 0; }
     if (steps > 0 && !h_out) {
         DFB_CUDA(cudaMalloc(&m->gru_dbg, sizeof(long long) * 8 * steps));
         DFB_CUDA(cudaMemset(m->gru_dbg, 0, sizeof(long long) * 8 * steps));
+        m->gru_dbg_steps = steps;
     }
     return DFB_OK;
 }
@@ -691,8 +695,8 @@ int run_gru(dfb_model *m, cudaStream_t s, const char *name, int layers, int H, i
         GruWindow gw{ck && ck->have_state ? hs : nullptr, hs, t0, T, ck ? ck->first : nullptr, ck ? ck->w0 : 0};
         // the last layer's planes feed a grouped linear and include the residual; the others feed the next projection
         unsigned short *hi = last ? out_hi : pl_hi, *lo = last ? out_lo : pl_lo;
-        if ((rc = launch_gru_tc(s, xproj, w_hh, b_hh, last ? res_last : nullptr, dst, hi, lo, B, Tn, m->gru_dbg,
-                                wide, last ? 1 : 0, &gw, H)))
+        if ((rc = launch_gru_tc(s, xproj, w_hh, b_hh, last ? res_last : nullptr, dst, hi, lo, B, Tn,
+                                Tn <= m->gru_dbg_steps ? m->gru_dbg : nullptr, wide, last ? 1 : 0, &gw, H)))
             return rc;
         if (last && hi && out_planes_ok) *out_planes_ok = true;
         cur_hi = pl_hi; cur_lo = pl_lo;

@@ -868,21 +868,14 @@ static int launch_gru_tc_n(cudaStream_t s, GruTcParams p) {
     return DFB_OK;
 }
 
-// wide != 0: 32 streams per cluster when the batch needs more than 4 clusters of 16 (see GtCfg).  H = 512: clusters of
-// 16 CTAs with 16 streams.
-int launch_gru_tc(cudaStream_t s, const float *xproj, const float *whh, const float *bhh, const float *res, float *hout,
-                  unsigned short *hout_hi, unsigned short *hout_lo, int B, int T, long long *dbg, int wide, int planes_res,
-                  const GruWindow *w, int H) {
-    if (!hout && !hout_hi) return fail(DFB_ERR_INVALID, "tensor-core recurrence: neither an fp32 output nor planes");
-    GruTcParams p{xproj, whh, bhh, res, hout, hout_hi, hout_lo, planes_res, w ? w->h0 : nullptr, w ? w->hT : nullptr,
-                  w ? w->t0 : 0, w ? w->Ts : T, B, T, 0, dbg};
-    p.first = w ? w->first : nullptr;
-    p.w0 = w ? w->w0 : 0;
+// The instance (streams per cluster, exchange) the recurrence runs for B streams of hidden size H.  wide != 0: 32 streams
+// per cluster when the batch needs more than 4 clusters of 16 (see GtCfg).  H = 512: clusters of 16 CTAs with 16 streams.
+static int gru_tc_select(int B, int H, int wide, int *ns, int *xg_out) {
     static const int force = getenv("DFB_GRU_NS") ? atoi(getenv("DFB_GRU_NS")) : 0;
     // exchange through L2 + multicast (k_gru_tc XG): bit 0: H = 512, bit 1: H = 256 / 32 streams, bit 2: H = 256 / 16 streams.
     // Default: all.
     static const int xg = getenv("DFB_GRU_XG") ? atoi(getenv("DFB_GRU_XG")) : 7;
-    if (H == 512) return (xg & 1) ? launch_gru_tc_n<16, 512, 1>(s, p) : launch_gru_tc_n<16, 512, 0>(s, p);
+    if (H == 512) { *ns = 16; *xg_out = xg & 1; return DFB_OK; }
     if (H != 256) return fail(DFB_ERR_UNSUPPORTED, "tensor-core recurrence: hidden size %d", H);
     // 16 streams per cluster have the shortest step but more cluster time per stream: once a launch needs several waves of
     // the co-resident clusters anyway, 32 per cluster are faster
@@ -893,11 +886,33 @@ int launch_gru_tc(cudaStream_t s, const float *xproj, const float *whh, const fl
     if (use32 && !force && !no48) {
         int wave = 0, rc = gru_tc_max_clusters<32, 256, 1>(&wave);
         if (rc) return rc;
-        if (B > wave * 32) return launch_gru_tc_n<48, 256, 1>(s, p);
+        if (B > wave * 32) { *ns = 48; *xg_out = 1; return DFB_OK; }
     }
-    if (use32 && (xg & 2)) return launch_gru_tc_n<32, 256, 1>(s, p);
-    if (!use32 && (xg & 4)) return launch_gru_tc_n<16, 256, 1>(s, p);
-    return use32 ? launch_gru_tc_n<32, 256, 0>(s, p) : launch_gru_tc_n<16, 256, 0>(s, p);
+    *ns = use32 ? 32 : 16;
+    *xg_out = (xg & (use32 ? 2 : 4)) ? 1 : 0;
+    return DFB_OK;
+}
+
+// ns = 0, xg = -1: the instance gru_tc_select picks; otherwise instance <ns, H, xg>, DFB_ERR_UNSUPPORTED when it is not built
+int launch_gru_tc(cudaStream_t s, const float *xproj, const float *whh, const float *bhh, const float *res, float *hout,
+                  unsigned short *hout_hi, unsigned short *hout_lo, int B, int T, long long *dbg, int wide, int planes_res,
+                  const GruWindow *w, int H, int ns, int xg) {
+    if (!hout && !hout_hi) return fail(DFB_ERR_INVALID, "tensor-core recurrence: neither an fp32 output nor planes");
+    GruTcParams p{xproj, whh, bhh, res, hout, hout_hi, hout_lo, planes_res, w ? w->h0 : nullptr, w ? w->hT : nullptr,
+                  w ? w->t0 : 0, w ? w->Ts : T, B, T, 0, dbg};
+    p.first = w ? w->first : nullptr;
+    p.w0 = w ? w->w0 : 0;
+    if (ns == 0 && xg == -1) {
+        const int rc = gru_tc_select(B, H, wide, &ns, &xg);
+        if (rc) return rc;
+    }
+    if (xg == 0 || xg == 1) {
+        if (H == 512 && ns == 16) return xg ? launch_gru_tc_n<16, 512, 1>(s, p) : launch_gru_tc_n<16, 512, 0>(s, p);
+        if (H == 256 && ns == 16) return xg ? launch_gru_tc_n<16, 256, 1>(s, p) : launch_gru_tc_n<16, 256, 0>(s, p);
+        if (H == 256 && ns == 32) return xg ? launch_gru_tc_n<32, 256, 1>(s, p) : launch_gru_tc_n<32, 256, 0>(s, p);
+        if (H == 256 && ns == 48 && xg) return launch_gru_tc_n<48, 256, 1>(s, p);
+    }
+    return fail(DFB_ERR_UNSUPPORTED, "tensor-core recurrence: instance NS %d H %d XG %d is not built", ns, H, xg);
 }
 
 int cached_map_f32_sw128(CUtensorMap *out, const void *base, int64_t rows, int64_t cols, int64_t ld, int box_rows);
@@ -948,3 +963,23 @@ int launch_gemm_bf16x3(cudaStream_t s, const void *x_hi, const void *x_lo, int64
 }
 
 }  // namespace dfb
+
+// Debug aid (tests/test_gpu_gru_tc.py): one k_gru_tc launch on caller-given device pointers
+extern "C" int dfb_debug_gru_tc(const float *xproj, const float *whh, const float *bhh, const float *res, float *hout,
+                                void *hout_hi, void *hout_lo, int planes_res, const float *h0, float *hT, const int64_t *first,
+                                int64_t w0, int t0, int Ts, int B, int T, int H, int ns, int xg, void *stream) {
+    if (!xproj || !whh || !bhh || (!hout && !hout_hi) || (!hout_hi != !hout_lo))
+        return dfb::fail(DFB_ERR_INVALID, "gru_tc: null argument");
+    if (B <= 0 || T <= 0 || t0 < 0 || (int64_t)t0 + T > Ts)
+        return dfb::fail(DFB_ERR_INVALID, "gru_tc: B %d, window [%d, %d + %d) of %d frames", B, t0, t0, T, Ts);
+    const dfb::GruWindow w{h0, hT, t0, Ts, first, w0};
+    return dfb::launch_gru_tc((cudaStream_t)stream, xproj, whh, bhh, res, hout, (unsigned short *)hout_hi,
+                              (unsigned short *)hout_lo, B, T, nullptr, 0, planes_res, &w, H, ns, xg);
+}
+
+// Debug aid (tests/test_gpu_gru_tc.py): one k_gemm_bf16x3 launch on caller-given device pointers
+extern "C" int dfb_debug_gemm_bf16x3(const void *x_hi, const void *x_lo, int64_t ldx, const void *w_hi, const void *w_lo,
+                                     const float *bias, float *y, int64_t ldy, int64_t M, int N, int K, void *stream) {
+    if (!x_hi || !x_lo || !w_hi || !w_lo || !y) return dfb::fail(DFB_ERR_INVALID, "gemm_bf16x3: null argument");
+    return dfb::launch_gemm_bf16x3((cudaStream_t)stream, x_hi, x_lo, ldx, w_hi, w_lo, bias, y, ldy, M, N, K);
+}

@@ -354,8 +354,23 @@ int dfb_model_set_options(dfb_model *m, int post_filter, float pf_beta, int mask
  * dfb_model_create). */
 int dfb_model_set_max_workspace(dfb_model *m, int64_t bytes);
 /* Debug aid: steps > 0 with h_out == NULL arms clock64() phase stamps ([steps][8]) for the following
- * GRU launches; a second call with h_out != NULL copies the stamps of the last launch and disarms. */
+ * GRU launches of at most `steps` time steps (longer ones are not stamped); a second call with h_out != NULL copies
+ * min(steps, armed steps) rows of the stamps (of the last stamped launch) and disarms. */
 int dfb_debug_gru_timing(dfb_model *m, int steps, long long *h_out);
+/* Debug aid: one launch of the tensor-core GRU recurrence on device pointers, on `stream` (NULL = default).  For steps
+ * t = 0 .. T-1 (frame t0 + t of buffers holding Ts frames per stream): xproj [B][Ts][3H] (W_ih x + b_ih), whh [3H][H],
+ * bhh [3H]; hout [B][Ts][H] = h + res and / or the BF16 hi / lo planes of h (planes_res = 0) or of h + res (1); res may
+ * be NULL.  h0 [B][H] carried state (NULL: zeros), hT [B][H] final state (may alias h0, may be NULL).  first (NULL or
+ * [B]): stream b's first frame is first[b] - w0 of the window; h stays 0 before it.  ns = 0, xg = -1: the instance the
+ * library picks for B; otherwise the instance of ns streams per cluster and exchange xg (0: DSMEM copies, 1: L2 multicast):
+ * H = 256 with (16|32, 0|1) or (48, 1), H = 512 with (16, 0|1); others return DFB_ERR_UNSUPPORTED. */
+int dfb_debug_gru_tc(const float *xproj, const float *whh, const float *bhh, const float *res, float *hout, void *hout_hi,
+                     void *hout_lo, int planes_res, const float *h0, float *hT, const int64_t *first, int64_t w0, int t0,
+                     int Ts, int B, int T, int H, int ns, int xg, void *stream);
+/* Debug aid: one launch of the BF16x3 projection GEMM on device pointers: y [M][N] (pitch ldy) = x w^T + bias with x
+ * given as BF16 hi / lo planes [M][K] (pitch ldx) and w as BF16 hi / lo planes [N][K]; bias may be NULL. */
+int dfb_debug_gemm_bf16x3(const void *x_hi, const void *x_lo, int64_t ldx, const void *w_hi, const void *w_lo,
+                          const float *bias, float *y, int64_t ldy, int64_t M, int N, int K, void *stream);
 /* Debug aid: one launch of the tensor-core grouped linear on device pointers, on `stream` (a cudaStream_t, NULL = default):
  * y / (y_hi, y_lo) [M][G*Hg] = act(GL(x)) * oscale + ooffset + res, x given as BF16 hi / lo planes [M][G*Ig] (pitch ldx)
  * and w_img the weight image of weights.py gl_bx_image.  y or the planes may be NULL; res may alias y.  act: 0 none,
