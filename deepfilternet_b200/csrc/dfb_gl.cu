@@ -24,6 +24,9 @@
 // its stores drain while the warp runs the next tile's MMAs.  df_out adds its residual in place (res == y): that is safe
 // because a warp's residual rows are read before the same warp's rows of y are stored, and the other CTAs own other
 // columns (slices) or other row tiles.
+// Staged planes (stage_p, see launch_gl_bx for the shapes that keep register stores): each warp writes the BF16 hi / lo
+// planes of 64 output columns at a time into one of its two [16][64] staging blocks (128-byte swizzle, conflict-free for
+// the accumulator fragment) and lane 0 stores the block with one TMA tensor store per plane while the warp fills the other.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -39,6 +42,8 @@ namespace dfb {
 
 constexpr int kGxThreads = 288, kGxMaxStages = 6, kGxBoxBytes = 128 * 128 /* 128 rows x 64 bf16 */;
 constexpr int kGxMaxChunks = 16;                      // 16-column chunks of the slice (gpc * Hgp <= 256)
+constexpr uint32_t kGxPlaneBlockBytes = 4096;         // one staged 64-column plane block: hi | lo, 16 rows x 128 B each
+constexpr uint32_t kGxPlaneWarpBytes = 2 * kGxPlaneBlockBytes;   // a warp's two blocks (one filled while the other drains)
 
 struct GlBxParams {
     const unsigned short *w_img;  // [hi | lo][G][Ig/8][Hgp/8][8][8] BF16
@@ -48,12 +53,48 @@ struct GlBxParams {
     int M, G, Ig, Hg, Hgp, gpc, act, stages;
     float oscale, ooffset;
     int stage_y;   // fp32 output through the shared staging tile + TMA store (residual, if any, through TMA loads)
+    int stage_p;   // BF16 planes through per-warp staging blocks + TMA stores (Hg % 16 == 0, gpc * Hg % 64 == 0)
 };
 
 __device__ __forceinline__ float gx_act(float x, int act) {
     if (act == 1) return fmaxf(x, 0.f);
     if (act == 2) return gt_tanh(x);   // 1 - 2 / (1 + e^2x) on the MUFU units (~1e-7 absolute, as in the GRU gates); tanhf made df_out epilogue bound
     return x;
+}
+
+// BF16 pair (hi, lo) of row r, column 16 (c % 4) + cc of the warp's 64-column plane block at sp (hi [16][64] | lo [16][64],
+// 128-byte swizzle as the TMA store reads it: conflict-free for the 8 rows of a fragment)
+__device__ __forceinline__ void gl_stage_planes(uint32_t sp, int c, int r, int cc, float x0, float x1) {
+    uint32_t hv, lv;
+    bf16x2_split(x0, x1, hv, lv);
+    const uint32_t o = sw128_off(r, 2 * (c & 3) + (cc >> 3)) + (uint32_t)(cc & 7) * 2u;
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(sp + o), "r"(hv) : "memory");
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(sp + 2048u + o), "r"(lv) : "memory");
+}
+
+// gl_store_chunk with staged planes (p.stage_p): the planes of chunk c go to the warp's staging block sp of the chunk's 64
+// columns.  Hg % 16 == 0, so the chunk is slice columns [16 c, +16).  A residual is read from the staging rows st: planes are
+// staged without fp32 rows only when there is none.
+__device__ __noinline__ void gl_stage_chunk(const GlBxParams &p, int c, uint32_t st, uint32_t sp, float a00, float a01, float a02,
+                                            float a03, float a10, float a11, float a12, float a13) {
+    const float a[2][4] = {{a00, a01, a02, a03}, {a10, a11, a12, a13}};
+    const int lane = threadIdx.x & 31;
+    const uint32_t pitch = (uint32_t)(p.gpc * p.Hg) * 4u;
+#pragma unroll
+    for (int j = 0; j < 2; j++) {
+        const int cc = j * 8 + 2 * (lane & 3);
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const uint32_t sa = st + (uint32_t)((lane >> 2) + 8 * h) * pitch + (uint32_t)(16 * c + cc) * 4u;
+            float2 rv = make_float2(0.f, 0.f);
+            if (st && p.res) asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(rv.x), "=f"(rv.y) : "r"(sa));
+            float2 x;
+            x.x = gx_act(a[j][2 * h], p.act) * p.oscale + p.ooffset + rv.x;
+            x.y = gx_act(a[j][2 * h + 1], p.act) * p.oscale + p.ooffset + rv.y;
+            if (st) sts64(sa, __float_as_uint(x.x), __float_as_uint(x.y));
+            gl_stage_planes(sp, c, (lane >> 2) + 8 * h, cc, x.x, x.y);
+        }
+    }
 }
 
 // epilogue of one 16-column chunk c: fragment (n-tile j, half h) = rows mrow + 8 h, columns 2 (lane % 4) + {0, 1} of the n-tile.
@@ -123,7 +164,8 @@ __device__ __noinline__ void gl_store_chunk(const GlBxParams &p, int c, int g0, 
 
 __global__ void __launch_bounds__(kGxThreads, 1)
 k_gl_bx(const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUtensorMap tmXlo, const __grid_constant__ CUtensorMap tmY,
-        const __grid_constant__ CUtensorMap tmR, const __grid_constant__ GlBxParams p) {
+        const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmPh, const __grid_constant__ CUtensorMap tmPl,
+        const __grid_constant__ GlBxParams p) {
     extern __shared__ __align__(1024) unsigned char gx_smem_raw[];
     const uint32_t sb = (smem_u32(gx_smem_raw) + 1023u) & ~1023u;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -140,7 +182,8 @@ k_gl_bx(const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUten
     const uint32_t s_w = s_x + (uint32_t)p.stages * 2 * kGxBoxBytes;     // W hi | lo
     const uint32_t ybox = 16u * (uint32_t)(p.gpc * p.Hg) * 4u;           // one warp's staging rows (fp32)
     const uint32_t s_y = s_w + 2 * wplane;                               // [8 warps][16][gpc * Hg] fp32 (stage_y)
-    const uint32_t s_bar = (s_y + (p.stage_y ? 8 * ybox : 0u) + 127u) & ~127u;   // full[6] empty[6] wbar rfull[8] rempty[8]
+    const uint32_t s_p = s_y + (p.stage_y ? 8 * ybox : 0u);              // [8 warps][2 blocks][hi | lo][16][64] BF16 (stage_p)
+    const uint32_t s_bar = (s_p + (p.stage_p ? 8u * kGxPlaneWarpBytes : 0u) + 127u) & ~127u;   // full[6] empty[6] wbar rfull[8] rempty[8]
     const uint32_t b_full = s_bar, b_empty = s_bar + 8 * kGxMaxStages, b_w = b_empty + 8 * kGxMaxStages;
     const uint32_t b_rfull = b_w + 8, b_rempty = b_rfull + 8 * 8;
     const bool res_tma = p.stage_y && p.res;
@@ -194,6 +237,7 @@ k_gl_bx(const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUten
     const int mat = lane >> 3, rr = lane & 7;
     mbar_wait_a(b_w, 0);
     const uint32_t st = p.stage_y ? s_y + (uint32_t)warp * ybox : 0u;
+    const uint32_t spw = p.stage_p ? s_p + (uint32_t)warp * kGxPlaneWarpBytes : 0u;
     int it = 0, ti = 0;
     for (int tile = blockIdx.y; tile < ntiles; tile += gridDim.y, ti++) {
         float acc[kGxMaxChunks][2][4];
@@ -234,13 +278,41 @@ k_gl_bx(const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUten
         }
         // ---- epilogue: one out-of-line call per chunk, so that this loop stays unrolled and every accumulator index constant
         //      (as one inline loop ptxas re-rolled it and moved the accumulators to local memory)
+        //      Staged planes: chunks 4 b .. 4 b + 3 are the slice's plane columns [64 b, +64), staged in the warp's block b % 2
+        //      once the store of block b - 2 has read it (an odd block count drains at the end of the tile).
         const int64_t mrow = (int64_t)tile * 128 + warp * 16 + (lane >> 2);
         if (res_tma) mbar_wait_a(b_rfull + 8 * warp, (uint32_t)(ti & 1));
 #pragma unroll
-        for (int c = 0; c < kGxMaxChunks; c++)
-            if (c < nch)
+        for (int c = 0; c < kGxMaxChunks; c++) {
+            if (c >= nch) continue;
+            const uint32_t sp = spw ? spw + (uint32_t)((c >> 2) & 1) * kGxPlaneBlockBytes : 0u;
+            if (sp) {
+                if ((c & 3) == 0) {
+                    if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
+                    __syncwarp();
+                }
+            }
+            if (sp)
+                gl_stage_chunk(p, c, st, sp, acc[c][0][0], acc[c][0][1], acc[c][0][2], acc[c][0][3], acc[c][1][0], acc[c][1][1],
+                               acc[c][1][2], acc[c][1][3]);
+            else
                 gl_store_chunk(p, c, g0, cpg, mrow, lane, st, acc[c][0][0], acc[c][0][1], acc[c][0][2], acc[c][0][3], acc[c][1][0],
                                acc[c][1][1], acc[c][1][2], acc[c][1][3]);
+            if (sp && (c & 3) == 3) {
+                // the block's 16 rows -> both planes (two TMA stores; rows >= M are clipped)
+                fence_proxy_async();
+                __syncwarp();
+                if (lane == 0) {
+                    const int col = g0 * p.Hg + 16 * (c - 3), row = tile * 128 + warp * 16;
+                    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];"
+                                 ::"l"((uint64_t)&tmPh), "r"(col), "r"(row), "r"(sp) : "memory");
+                    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];"
+                                 ::"l"((uint64_t)&tmPl), "r"(col), "r"(row), "r"(sp + 2048u) : "memory");
+                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+                    if (c + 1 == nch && (nch & 4)) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+                }
+            }
+        }
         if (st) {
             // the staged rows -> y (one TMA store; the tensor map clips rows >= M), read out before the rows are reused
             fence_proxy_async();
@@ -255,6 +327,8 @@ k_gl_bx(const __grid_constant__ CUtensorMap tmXhi, const __grid_constant__ CUten
             __syncwarp();
         }
     }
+    // the last plane blocks are read out before the CTA's shared memory goes away
+    if (p.stage_p && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
 
 // ------------------------------------------------------ df_conv1 -> df_fc_emb, c1 kept on chip ----
@@ -671,20 +745,32 @@ int launch_gl_bx(cudaStream_t s, const unsigned short *x_hi, const unsigned shor
     int rc;
     if ((rc = cached_map_bf16(&mh, x_hi, M, (int64_t)G * Ig, ldx, 128)) || (rc = cached_map_bf16(&ml, x_lo, M, (int64_t)G * Ig, ldx, 128)))
         return rc;
-    // staged fp32 output: the [128][gpc * Hg] staging tile comes out of the ring, which keeps >= 2 stages
-    const int wbytes = gpc * Ig * Hgp * 4, ybytes = 128 * gpc * Hg * 4;
-    int stages_y = (227 * 1024 - 2048 - wbytes - ybytes - 256) / (2 * kGxBoxBytes);
-    if (stages_y > kGxMaxStages) stages_y = kGxMaxStages;
-    const bool stage_y = y && stages_y >= 2;
-    CUtensorMap my = mh, mr = mh;   // (unused copies when not staged / no residual)
+    // staged outputs come out of the ring, which keeps >= 2 stages.  fp32: the [128][gpc * Hg] staging tile.  Planes: two
+    // [16][64] hi | lo blocks per warp, stored as 64-column TMA boxes; they stay stored from registers when
+    //   - Hg % 16 or gpc * Hg % 64 (a 16-column chunk would straddle a group or the slice would end inside a block),
+    //   - ldp % 8, or a plane base not 16-byte aligned (TMA needs 16-byte global strides and addresses),
+    //   - y is written but not staged, or a residual is added without y (those rows come from registers too), or
+    //   - the ring would drop below 2 stages (e.g. DeepFilterNet3 enc.emb_gru.out: weights + fp32 tile leave room for 2).
+    const int wbytes = gpc * Ig * Hgp * 4, ybytes = 128 * gpc * Hg * 4, pbytes = 8 * (int)kGxPlaneWarpBytes;
+    auto ring = [&](int staged) {
+        const int s = (227 * 1024 - 2048 - wbytes - staged - 256) / (2 * kGxBoxBytes);
+        return s > kGxMaxStages ? kGxMaxStages : s;
+    };
+    const bool stage_y = y && ring(ybytes) >= 2;
+    const bool stage_p = y_hi && Hg % 16 == 0 && (gpc * Hg) % 64 == 0 && ldp % 8 == 0 && !((uintptr_t)y_hi & 15) &&
+                         !((uintptr_t)y_lo & 15) && (y ? stage_y : !res) && ring((stage_y ? ybytes : 0) + pbytes) >= 2;
+    CUtensorMap my = mh, mr = mh, mph = mh, mpl = mh;   // (unused copies when not staged / no residual)
     if (stage_y) {
-        stages = stages_y;
         if ((rc = cached_map_f32_rows(&my, y, M, (int64_t)G * Hg, ldy, gpc * Hg, 16))) return rc;
         if (res && (rc = cached_map_f32_rows(&mr, res, M, (int64_t)G * Hg, ldr, gpc * Hg, 16))) return rc;
     }
+    if (stage_p && ((rc = cached_map_bf16(&mph, y_hi, M, (int64_t)G * Hg, ldp, 16)) || (rc = cached_map_bf16(&mpl, y_lo, M, (int64_t)G * Hg, ldp, 16))))
+        return rc;
+    const int staged = (stage_y ? ybytes : 0) + (stage_p ? pbytes : 0);
+    if (staged) stages = ring(staged);
     GlBxParams p{reinterpret_cast<const unsigned short *>(w_img), res, ldr, y, ldy, y_hi, y_lo, ldp,
-                 (int)M, G, Ig, Hg, Hgp, gpc, act, stages, oscale, ooffset, stage_y ? 1 : 0};
-    const int smem = 1024 + stages * 2 * kGxBoxBytes + wbytes + (stage_y ? ybytes : 0) + 128 + 256;
+                 (int)M, G, Ig, Hg, Hgp, gpc, act, stages, oscale, ooffset, stage_y ? 1 : 0, stage_p ? 1 : 0};
+    const int smem = 1024 + stages * 2 * kGxBoxBytes + wbytes + staged + 128 + 256;
     static PerDeviceOnce attr_once;
     if (auto once_guard = attr_once.first())
         DFB_CUDA(cudaFuncSetAttribute(k_gl_bx, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
@@ -696,7 +782,7 @@ int launch_gl_bx(cudaStream_t s, const unsigned short *x_hi, const unsigned shor
     if (groups < 1) groups = 1;
     if (groups > ntiles) groups = ntiles;
     DFB_PROF("k_gl_bx", s);
-    k_gl_bx<<<dim3((unsigned)slices, (unsigned)groups), kGxThreads, smem, s>>>(mh, ml, my, mr, p);
+    k_gl_bx<<<dim3((unsigned)slices, (unsigned)groups), kGxThreads, smem, s>>>(mh, ml, my, mr, mph, mpl, p);
     DFB_LAUNCH_CHECK();
     return DFB_OK;
 }
