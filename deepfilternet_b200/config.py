@@ -213,12 +213,24 @@ def _load_v1(c: "ModelConfig", get) -> "ModelConfig":
         raise NotImplementedError("DeepFilterNet (v1) variants other than the shipped topology are outside the H100 hot path: " + ", ".join(bad))
     if c.hop_size * 2 > c.fft_size:
         raise ValueError("hop_size * 2 <= fft_size required (libDF/src/lib.rs:111)")
+    check_stft_size(c)
     return c
+
+
+def check_stft_size(c: "ModelConfig") -> None:
+    """The DNN and apply kernels are built for the shipped models' STFT (48 kHz, fft 960, hop 480); a model configured
+    at another rate or size fails loudly.  The DSP state itself (``libdf.DF``, ``df_features``, ``fft_features``)
+    runs at every size up to fft 8192."""
+    if (c.sr, c.fft_size, c.hop_size) != (48000, 960, 480):
+        raise NotImplementedError(
+            f"sr={c.sr}, fft_size={c.fft_size}, hop_size={c.hop_size}: the model path is built for sr=48000, "
+            "fft_size=960, hop_size=480 only")
 
 
 def check_supported(c: "ModelConfig") -> None:
     """Options the kernels do not implement must fail loudly instead of being dropped (all shipped
     configs use emb_gru_skip* = none and df_gru_skip in {none, groupedlinear})."""
+    check_stft_size(c)
     if c.model == "deepfilternet3":
         if c.emb_gru_skip != "none" or c.emb_gru_skip_enc != "none":
             raise NotImplementedError(

@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "../../include/dfb200.h"
+#include "dfb_fft_generic.cuh"
 
 namespace dfb {
 
@@ -264,6 +265,7 @@ struct dfb_state {
     std::vector<float> window;
     void *d_tables = nullptr;  // one slab holding every table
     dfb::DspTables tb{};
+    dfb::GenFftPlan plan{};    // generic real FFT of fft_size (states other than fft 960 / hop 480); tw in d_tables
     dfb::Arena arena;          // scratch of the *_host entry points
     cudaStream_t stream = nullptr;
     // STFT / ISTFT memories carried between calls (libDF analysis_mem / synthesis_mem, lib.rs:60-62)

@@ -14,6 +14,7 @@
 // HBM layout: audio f32[B,T]; spec c64[B,Tf,481] (frame-major, 3848 B rows); features
 // f32[B,Tf,32] and c64[B,Tf,96]; every kernel reads/writes whole rows with consecutive lanes on
 // consecutive addresses.
+#include <algorithm>
 #include <climits>
 #include <cmath>
 #include <cstdlib>
@@ -319,13 +320,15 @@ __global__ void __launch_bounds__(256) k_resample(const float *__restrict__ x, i
 __device__ __forceinline__ float norm_ref_bits(float2 v) {
     return __double2float_rn(__dsqrt_rn(__dadd_rn(__dmul_rn((double)v.x, (double)v.x), __dmul_rn((double)v.y, (double)v.y))));
 }
-template <int kPf, bool REF_BITS = false>
+// WIDE (E + Fd > 1024: spectra of fft_size > 2046): grid (B, blocks of the E + Fd values), value j = threadIdx.x +
+// blockIdx.y * blockDim.x; every value is its own scan, so the results are those of one block.  Separate instantiations.
+template <int kPf, bool REF_BITS = false, bool WIDE = false>
 __global__ void __launch_bounds__(kPf > 8 ? 128 : 1024) k_feat_norm(const float *erb_in, int E, int64_t erb_stride_t,
                             const float2 *__restrict__ spec_in, int Fd, int64_t spec_stride_t, int Tf,
                             float alpha, const float *erb_state, const float *unit_state,
                             float *feat_erb, float2 *__restrict__ feat_spec, int Ts, float *erb_state_out,
                             float *unit_state_out) {
-    const int b = blockIdx.x, j = threadIdx.x;
+    const int b = blockIdx.x, j = threadIdx.x + (WIDE ? blockIdx.y * blockDim.x : 0);
     const float one_m_alpha = __fsub_rn(1.f, alpha);
     if (j < E) {
         const float *src = erb_in + (int64_t)b * Ts * erb_stride_t + j;
@@ -888,6 +891,185 @@ __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyP
     }
 }
 
+// ------------------------------------------------------------- generic STFT / ISTFT ----
+// Every (fft_size N, hop H) other than 960 / 480: the real FFT of dfb_fft_generic.cuh, one CTA per group of G frames of
+// one stream, all G frames transformed together (every Stockham stage is one pass of the CTA's threads over the G M / R
+// butterflies, then a barrier).  Shared memory: two ping-pong buffers of G x M complex values (G = gen_frames(M): about
+// kGenCplx values, 32 KB), plus for the synthesis two overlap-add tails of N - H samples.
+constexpr int kGenThreads = 256;
+constexpr int kGenCplx = 2048;
+constexpr int kGenSmemMax = 200 * 1024;   // odd N = 8191: 2 x 8191 x 8 B of buffers + 2 x 8190 x 4 B of tails
+inline int gen_frames(int M) { return std::max(1, std::min(32, kGenCplx / M)); }
+
+// The stage radices go to shared memory (a dynamically indexed kernel-parameter array would be copied to local memory).
+__device__ __forceinline__ void gen_load_radices(const GenFftPlan &pl, int *s_rad) {
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int i = 0; i < kGenMaxStages; i++) s_rad[i] = pl.rad[i];
+    }
+}
+
+// M-point complex FFT of the first nf frames (frame f at a + f M), with b as the second buffer; returns the buffer that
+// holds the result.  Every thread of the CTA takes part; ends with a barrier.
+template <bool INV>
+__device__ __forceinline__ float2 *gen_block_fft(float2 *a, float2 *b, const GenFftPlan &pl, const int *s_rad, int nf) {
+    const int M = pl.M, ts = pl.N / pl.M;
+    int Ns = 1;
+    for (int s = 0; s < pl.nst; s++) {
+        const int R = s_rad[s], nb = M / R, total = nf * nb;
+#define DFB_GEN_STAGE(CALL)                                                   \
+    for (int i = threadIdx.x; i < total; i += blockDim.x) {                   \
+        const int f = i / nb, j = i - f * nb;                                 \
+        CALL;                                                                 \
+    }
+        switch (R) {
+            case 2: DFB_GEN_STAGE((gen_bfly<2, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
+            case 3: DFB_GEN_STAGE((gen_bfly<3, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
+            case 4: DFB_GEN_STAGE((gen_bfly<4, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
+            case 5: DFB_GEN_STAGE((gen_bfly<5, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
+            case 7: DFB_GEN_STAGE((gen_bfly<7, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
+            default: DFB_GEN_STAGE((gen_bfly_any<INV>(a + f * M, b + f * M, M, Ns, R, j, pl.tw, ts))) break;
+        }
+#undef DFB_GEN_STAGE
+        __syncthreads();
+        float2 *t = a; a = b; b = t;
+        Ns *= R;
+    }
+    return a;
+}
+
+// grid (ceil(Tf / G), B), kGenThreads threads.  Frame t = window x samples [t H - (N - H), t H + H) of stream b, zeros
+// (or init_mem [B][N - H], the carried analysis memory) before sample 0; spec [B][Tf][F] = wnorm * rfft; erb_db (or null)
+// [B][Tf][E] = the ERB dB of the spectrum (lib.rs:280-295, 207-210), from the band energies kept in shared memory.
+__global__ void __launch_bounds__(kGenThreads) k_analysis_gen(const float *__restrict__ audio, int64_t T, int Tf,
+                                                              float2 *__restrict__ spec, float *__restrict__ erb_db, DspTables tb,
+                                                              GenFftPlan pl, int G, const float *__restrict__ init_mem) {
+    extern __shared__ __align__(16) float2 gsm[];
+    __shared__ int s_rad[kGenMaxStages];
+    const int N = pl.N, M = pl.M, H = tb.hop, F = tb.F, mem = N - H;
+    const int b = blockIdx.y, t0 = blockIdx.x * G, nf = min(G, Tf - t0);
+    float2 *A = gsm, *Bf = gsm + G * M;
+    gen_load_radices(pl, s_rad);
+    const float *x = audio + (int64_t)b * T;
+    for (int i = threadIdx.x; i < nf * N; i += blockDim.x) {
+        const int f = i / N, n = i - f * N;
+        const int64_t s = (int64_t)(t0 + f) * H - mem + n;
+        float v = 0.f;
+        if (s >= 0) v = __ldg(x + s);
+        else if (init_mem) v = init_mem[(int64_t)b * mem + mem + s];
+        v = __fmul_rn(v, __ldg(tb.window + n));
+        if (N % 2 == 0) reinterpret_cast<float *>(A + f * M)[n] = v;   // z[n / 2] = (x[2 (n / 2)], x[2 (n / 2) + 1])
+        else A[f * M + n] = make_float2(v, 0.f);
+    }
+    __syncthreads();
+    float2 *Z = gen_block_fft<false>(A, Bf, pl, s_rad, nf);
+    float *P = reinterpret_cast<float *>(Z == A ? Bf : A);   // |X|^2 of every bin, F floats per frame
+    const float wn = tb.wnorm;
+    auto emit = [&](int f, int k, float2 v) {
+        v.x *= wn; v.y *= wn;
+        spec[((int64_t)b * Tf + t0 + f) * F + k] = v;
+        P[f * F + k] = __fadd_rn(__fmul_rn(v.x, v.x), __fmul_rn(v.y, v.y));
+    };
+    if (N % 2 == 0) {
+        const int nk = M / 2 + 1;   // k in [0, M / 2] gives X[k] and X[M - k]
+        for (int i = threadIdx.x; i < nf * nk; i += blockDim.x) {
+            const int f = i / nk, k = i - f * nk;
+            float2 xk, xnk;
+            rfft_split(Z[f * M + k], Z[f * M + (M - k) % M], __ldg(pl.tw + k), xk, xnk);
+            emit(f, k, xk);
+            if (M - k != k) emit(f, M - k, xnk);
+        }
+    } else {
+        for (int i = threadIdx.x; i < nf * F; i += blockDim.x) {
+            const int f = i / F, k = i - f * F;
+            emit(f, k, Z[f * M + k]);
+        }
+    }
+    if (erb_db == nullptr) return;
+    __syncthreads();
+    for (int i = threadIdx.x; i < nf * tb.E; i += blockDim.x) {
+        const int f = i / tb.E, band = i - f * tb.E;
+        const int o = tb.erb_off[band], n = tb.erb_off[band + 1] - o;
+        const float kinv = tb.erb_kinv[band];
+        float acc = 0.f;
+        for (int j = 0; j < n; j++) acc = __fadd_rn(acc, __fmul_rn(P[f * F + o + j], kinv));
+        erb_db[((int64_t)b * Tf + t0 + f) * tb.E + band] = __fmul_rn(log10f(__fadd_rn(acc, 1e-10f)), 10.f);
+    }
+}
+
+// grid (ceil(Tf / chunk), B), kGenThreads threads: frame_synthesis (lib.rs:396-427) of frames [c0, c0 + chunk) of stream b.
+// Output sample p of frame t is the sum of the windowed inverse transforms of every frame that covers it, oldest first
+// (the reference's order: the carried partial sum, then the new frame).  The CTA starts K = ceil((N - H) / H) frames
+// before c0 so that its overlap-add tail is complete when c0 begins (their own outputs are not written), and
+// transforms G frames at a time: the tail (N - H partial sums) plus G frames give G H output samples and the next tail.
+// Stream b starts from init_tail [N - H] when given (the carried synthesis memory) and the tail after its last frame goes
+// to final_tail when given (last stream only).
+__global__ void __launch_bounds__(kGenThreads) k_synthesis_gen(const float2 *__restrict__ spec, int Tf, float *__restrict__ audio,
+                                                               DspTables tb, GenFftPlan pl, int G, int chunk,
+                                                               const float *__restrict__ init_tail, float *__restrict__ final_tail) {
+    extern __shared__ __align__(16) float2 gsm[];
+    __shared__ int s_rad[kGenMaxStages];
+    const int N = pl.N, M = pl.M, H = tb.hop, F = tb.F, mem = N - H;
+    const int b = blockIdx.y, c0 = blockIdx.x * chunk, c1 = min(c0 + chunk, Tf);
+    float2 *A = gsm, *Bf = gsm + G * M;
+    float *tails = reinterpret_cast<float *>(gsm + 2 * G * M);   // [2][N - H]: current and next tail
+    int cur = 0;
+    gen_load_radices(pl, s_rad);
+    int tg = max(0, c0 - (mem + H - 1) / H);
+    for (int i = threadIdx.x; i < mem; i += blockDim.x) tails[i] = (tg == 0 && init_tail) ? init_tail[i] : 0.f;
+    const float2 *srow = spec + (int64_t)b * Tf * F;
+    float *orow = audio + (int64_t)b * Tf * H;
+    while (tg < c1) {
+        const int gn = min(G, c1 - tg);
+        // Hermitian half spectrum -> input of the M-point inverse transform (imaginary parts of DC and, for even N,
+        // Nyquist are ignored: lib.rs:402, realfft)
+        if (N % 2 == 0) {
+            const int nk = M / 2 + 1;
+            for (int i = threadIdx.x; i < gn * nk; i += blockDim.x) {
+                const int f = i / nk, k = i - f * nk;
+                const float2 *row = srow + (int64_t)(tg + f) * F;
+                float2 xk = row[k], xnk = row[M - k];
+                if (k == 0) { xk.y = 0.f; xnk.y = 0.f; }
+                const float2 w = __ldg(pl.tw + k);
+                float2 zk, znk;
+                irfft_merge(xk, xnk, make_float2(w.x, -w.y), zk, znk);
+                A[f * M + k] = zk;
+                if (k > 0 && k < M - k) A[f * M + M - k] = znk;
+            }
+        } else {
+            for (int i = threadIdx.x; i < gn * N; i += blockDim.x) {
+                const int f = i / N, n = i - f * N;
+                const float2 *row = srow + (int64_t)(tg + f) * F;
+                float2 v = n < F ? row[n] : cconj(row[N - n]);
+                if (n == 0) v.y = 0.f;
+                A[f * M + n] = v;
+            }
+        }
+        __syncthreads();
+        const float2 *Y = gen_block_fft<true>(A, Bf, pl, s_rad, gn);
+        // overlap-add: positions p in [0, gn H + N - H) relative to sample tg H
+        for (int p = threadIdx.x; p < gn * H + mem; p += blockDim.x) {
+            float v = p < mem ? tails[cur * mem + p] : 0.f;
+            const int f_lo = p >= N ? (p - N) / H + 1 : 0, f_hi = min(gn - 1, p / H);
+            for (int f = f_lo; f <= f_hi; f++) {
+                const int q = p - f * H;
+                const float y = (N % 2 == 0) ? reinterpret_cast<const float *>(Y + f * M)[q] : Y[f * M + q].x;
+                v = __fadd_rn(v, __fmul_rn(y, __ldg(tb.window + q)));
+            }
+            if (p < gn * H) {
+                if (tg + p / H >= c0) orow[(int64_t)tg * H + p] = v;
+            } else {
+                tails[(cur ^ 1) * mem + p - gn * H] = v;
+            }
+        }
+        __syncthreads();
+        cur ^= 1;
+        tg += gn;
+    }
+    if (final_tail && c1 == Tf && b == (int)gridDim.y - 1)
+        for (int i = threadIdx.x; i < mem; i += blockDim.x) final_tail[i] = tails[cur * mem + i];
+}
+
 }  // namespace dfb
 
 // ====================================================================== host side / C ABI ==
@@ -974,9 +1156,12 @@ extern "C" int dfb_state_create(dfb_state **out, int device, int sr, int fft_siz
     if (!out) return fail(DFB_ERR_INVALID, "null out");
     *out = nullptr;
     if (hop_size * 2 > fft_size) return fail(DFB_ERR_INVALID, "assertion failed: hop_size * 2 <= fft_size");
-    if (fft_size != kFft || hop_size != kHop)
-        return fail(DFB_ERR_UNSUPPORTED, "built kernels cover fft_size=960, hop_size=480 (got %d, %d)", fft_size,
-                    hop_size);
+    if (hop_size < 1) return fail(DFB_ERR_INVALID, "hop_size must be positive (got %d)", hop_size);
+    if (fft_size > kGenMaxN)
+        return fail(DFB_ERR_UNSUPPORTED, "fft_size %d is above the largest built transform, %d", fft_size, kGenMaxN);
+    GenFftPlan plan{};
+    std::vector<float2> gtw;
+    if (!gen_fft_plan(fft_size, plan, gtw)) return fail(DFB_ERR_INVALID, "fft_size %d outside [2, %d]", fft_size, kGenMaxN);
     if (nb_erb <= 0 || nb_erb > kMaxErb) return fail(DFB_ERR_INVALID, "nb_erb out of range");
     int rc = use_device(device);
     if (rc) return rc;
@@ -995,7 +1180,7 @@ extern "C" int dfb_state_create(dfb_state **out, int device, int sr, int fft_siz
         double s = sin(0.5 * pi * ((double)i + 0.5) / (double)(fft_size / 2));
         st->window[i] = (float)sin(0.5 * pi * s * s);
     }
-    // one slab: window | tw_a_fwd | tw_a_inv | tw960 | erb_off | erb_kinv | band_of_bin
+    // one slab: window | tw_a_fwd | tw_a_inv | tw960 | erb_off | erb_kinv | band_of_bin | generic FFT twiddles
     std::vector<float2> twf(kN2 * kN1), twi(kN2 * kN1), tw960(241);
     for (int l = 0; l < kN2; l++)
         for (int k1 = 0; k1 < kN1; k1++) {
@@ -1019,11 +1204,13 @@ extern "C" int dfb_state_create(dfb_state **out, int device, int sr, int fft_siz
         delete st;
         return fail(DFB_ERR_INVALID, "erb widths sum to %d, expected %d", off[nb_erb], F);
     }
-    size_t o_win = 0, o_twf = o_win + sizeof(float) * fft_size, o_twi = o_twf + sizeof(float2) * twf.size(),
+    // (the float2 tables start 256-byte aligned whatever fft_size is, odd included)
+    size_t o_win = 0, o_twf = o_win + ((sizeof(float) * fft_size + 255) & ~size_t(255)), o_twi = o_twf + sizeof(float2) * twf.size(),
            o_960 = o_twi + sizeof(float2) * twi.size(), o_off = o_960 + sizeof(float2) * 256,
            o_kinv = o_off + sizeof(int) * (kMaxErb + 1 + 3), o_bob = o_kinv + sizeof(float) * kMaxErb,
-           total = o_bob + ((F + 255) & ~255);
+           o_gtw = o_bob + ((F + 255) & ~255), total = o_gtw + sizeof(float2) * gtw.size();
     std::vector<char> slab(total, 0);
+    memcpy(slab.data() + o_gtw, gtw.data(), sizeof(float2) * gtw.size());
     memcpy(slab.data() + o_win, st->window.data(), sizeof(float) * fft_size);
     memcpy(slab.data() + o_twf, twf.data(), sizeof(float2) * twf.size());
     memcpy(slab.data() + o_twi, twi.data(), sizeof(float2) * twi.size());
@@ -1046,8 +1233,12 @@ extern "C" int dfb_state_create(dfb_state **out, int device, int sr, int fft_siz
     st->tb.band_of_bin = (const unsigned char *)(d + o_bob);
     st->tb.wnorm = 1.f / ((float)((int64_t)fft_size * fft_size) / (float)(2 * hop_size));  // lib.rs:133
     st->tb.fft = fft_size; st->tb.hop = hop_size; st->tb.F = F; st->tb.E = nb_erb;
+    st->plan = plan;
+    st->plan.tw = (const float2 *)(d + o_gtw);
     cudaFuncSetAttribute(k_analysis<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAnaSmem);
     cudaFuncSetAttribute(k_analysis<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAnaSmem);
+    cudaFuncSetAttribute(k_analysis_gen, cudaFuncAttributeMaxDynamicSharedMemorySize, kGenSmemMax);
+    cudaFuncSetAttribute(k_synthesis_gen, cudaFuncAttributeMaxDynamicSharedMemorySize, kGenSmemMax);
     if (cudaStreamCreateWithFlags(&st->stream, cudaStreamNonBlocking) != cudaSuccess) {
         cudaFree(d);
         delete st;
@@ -1087,11 +1278,25 @@ extern "C" int dfb_state_params(const dfb_state *st, int *sr, int *fft, int *hop
 
 namespace dfb {
 
+// fft 960 / hop 480: the specialised warp kernels; every other size runs the generic ones (outside the enhancement
+// path, so not among the kernels DFB_PROF reports)
+static bool is_960(const dfb_state *st) { return st->fft == kFft && st->hop == kHop; }
+
 int launch_analysis(dfb_state *st, const float *d_audio, int64_t C, int64_t T, float *d_spec, float *d_erb_db,
                     cudaStream_t s, const float *d_init_mem, const AnaWindow *w) {
     int64_t Tf = T / st->hop;
     if (C <= 0 || Tf <= 0) return DFB_OK;
     if (C > 65535) return fail(DFB_ERR_INVALID, "more than 65535 channels per call");
+    if (!is_960(st)) {
+        if (w) return fail(DFB_ERR_UNSUPPORTED, "time-chunked analysis is built for fft_size 960 / hop_size 480 only");
+        if (Tf > INT_MAX) return fail(DFB_ERR_INVALID, "more than 2^31 frames per channel");
+        const int G = gen_frames(st->plan.M);
+        dim3 grid((unsigned)((Tf + G - 1) / G), (unsigned)C);
+        k_analysis_gen<<<grid, kGenThreads, sizeof(float2) * 2 * G * st->plan.M, s>>>(d_audio, T, (int)Tf, (float2 *)d_spec,
+                                                                                     d_erb_db, st->tb, st->plan, G, d_init_mem);
+        DFB_LAUNCH_CHECK();
+        return DFB_OK;
+    }
     const int t_begin = w ? w->t_begin : 0, nf = w ? w->nf : (int)Tf, out_t0 = w ? w->out_t0 : 0, Tbuf = w ? w->Tbuf : (int)Tf;
     if (nf <= 0) return DFB_OK;
     dim3 grid((unsigned)((nf + kAnaWarps - 1) / kAnaWarps), (unsigned)C);
@@ -1112,9 +1317,22 @@ int launch_feat_norm(const float *d_erb, int E, int64_t erb_stride, const float 
                      float *d_feat_erb, float *d_feat_spec, cudaStream_t s, int64_t Ts, float *d_erb_state_out,
                      float *d_unit_state_out, bool ref_bits) {
     if (C <= 0 || Tf <= 0 || E + Fd == 0) return DFB_OK;
-    if (E + Fd > 1024) return fail(DFB_ERR_INVALID, "E + F > 1024 in norm scan");
     int threads = ((E + Fd + 31) / 32) * 32;
     DFB_PROF("k_feat_norm", s);
+    if (E + Fd > 1024) {
+        dim3 grid((unsigned)C, (unsigned)((E + Fd + 255) / 256));
+        const int ts = (int)(Ts > 0 ? Ts : Tf);
+        if (ref_bits)
+            k_feat_norm<4, true, true><<<grid, 256, 0, s>>>(d_erb, E, erb_stride, (const float2 *)d_spec, Fd, spec_stride, (int)Tf, alpha,
+                                                            d_erb_state, d_unit_state, d_feat_erb, (float2 *)d_feat_spec, ts,
+                                                            d_erb_state_out, d_unit_state_out);
+        else
+            k_feat_norm<4, false, true><<<grid, 256, 0, s>>>(d_erb, E, erb_stride, (const float2 *)d_spec, Fd, spec_stride, (int)Tf, alpha,
+                                                             d_erb_state, d_unit_state, d_feat_erb, (float2 *)d_feat_spec, ts,
+                                                             d_erb_state_out, d_unit_state_out);
+        DFB_LAUNCH_CHECK();
+        return DFB_OK;
+    }
     static const bool no_seg = getenv("DFB_NORM_SEG") && !atoi(getenv("DFB_NORM_SEG"));
     if (ref_bits && threads <= 128)
         k_feat_norm<24, true><<<(unsigned)C, threads, 0, s>>>(d_erb, E, erb_stride, (const float2 *)d_spec, Fd, spec_stride, (int)Tf,
@@ -1140,9 +1358,43 @@ int launch_feat_norm(const float *d_erb, int E, int64_t erb_stride, const float 
     return DFB_OK;
 }
 
+// Plain ISTFT (mode 0) of a state other than 960 / 480.  With p.carry and several channels, channel c continues from the
+// tail channel c - 1 leaves, which may still hold samples of the channels before it (a channel shorter than N - H):
+// one launch per channel, the tails chained on the device through two ping-pong buffers after final_tail.
+static int launch_synthesis_gen(dfb_state *st, const ApplyParams &p, int64_t B, cudaStream_t s) {
+    if (p.mode != 0 || p.spec_out || p.rows || p.out_offset || p.t_first || p.spec_T || p.Tv || p.out_stride != (int64_t)p.Tf * st->hop)
+        return fail(DFB_ERR_UNSUPPORTED, "the enhancement path is built for fft_size 960 / hop_size 480 only");
+    const int M = st->plan.M, G = gen_frames(M), mem = st->fft - st->hop, K = (mem + st->hop - 1) / st->hop;
+    const int chunk = G * std::max(2, (8 * K + G - 1) / G);
+    const size_t smem = sizeof(float2) * 2 * G * M + sizeof(float) * 2 * mem;
+    const int64_t F = st->tb.F, Tf = p.Tf;
+    if (!p.carry || B == 1) {
+        dim3 grid((unsigned)((Tf + chunk - 1) / chunk), (unsigned)B);
+        k_synthesis_gen<<<grid, kGenThreads, smem, s>>>(p.spec, p.Tf, p.audio, st->tb, st->plan, G, chunk,
+                                                        p.carry ? p.init_tail : nullptr, p.final_tail);
+        DFB_LAUNCH_CHECK();
+        return DFB_OK;
+    }
+    if (!p.final_tail) return fail(DFB_ERR_INVALID, "carried synthesis needs a final tail buffer of 3 (N - H) floats");
+    dim3 grid((unsigned)((Tf + chunk - 1) / chunk), 1);
+    const float *in = p.init_tail;
+    for (int64_t c = 0; c < B; c++) {
+        float *out = c == B - 1 ? p.final_tail : p.final_tail + mem * (1 + (c & 1));
+        k_synthesis_gen<<<grid, kGenThreads, smem, s>>>(p.spec + c * Tf * F, p.Tf, p.audio + c * Tf * st->hop, st->tb, st->plan,
+                                                        G, chunk, in, out);
+        DFB_LAUNCH_CHECK();
+        in = out;
+    }
+    return DFB_OK;
+}
+
 int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaStream_t s, const SlotCtl *ctl) {
     if (B <= 0 || p.Tf <= 0) return DFB_OK;
     if (B > 65535) return fail(DFB_ERR_INVALID, "more than 65535 channels per call");
+    if (!is_960(st)) {
+        if (ctl) return fail(DFB_ERR_UNSUPPORTED, "the enhancement path is built for fft_size 960 / hop_size 480 only");
+        return launch_synthesis_gen(st, p, B, s);
+    }
     if (p.mode != 0 && (p.nb_df > 240 || p.order > 8)) return fail(DFB_ERR_UNSUPPORTED, "nb_df > 240 or df_order > 8");
     // frames per warp: 16 amortises the re-synthesis of the frame before a warp's first one; short windows (time chunks)
     // take 8 so that the grid still fills the device with a few waves
@@ -1189,33 +1441,50 @@ extern "C" int dfb_state_reset(dfb_state *st);
 
 // pyDF DF.analysis(input, reset): reset != 0 starts every channel from zero memory (pyDF/src/lib.rs:56-58);
 // reset == 0 carries the STFT memory from the previous call into channel 0 and from channel c into c + 1
-// (one DFState is shared by all channels).  Either way the memory left behind is the last hop of the last channel.
+// (one DFState is shared by all channels).  The memory holds the last N - H samples a channel's frames read: the memory
+// entering channel c is the tail of (memory entering c - 1, then c - 1's first Tf hop samples), so a channel shorter than
+// N - H keeps part of the older memory.  Either way the memory left behind is the one after the last channel.
 extern "C" int dfb_analysis_host_ex(dfb_state *st, const float *h_audio, int64_t C, int64_t T, int reset, float *h_spec) {
     if (!st || !h_audio || !h_spec) return fail(DFB_ERR_INVALID, "null argument");
     if (C <= 0 || T <= 0) return fail(DFB_ERR_INVALID, "[df] Input array empty or not contiguous.");
     DFB_CUDA(cudaSetDevice(st->device));
-    const int64_t Tf = T / st->hop, hop = st->hop;
+    const int64_t Tf = T / st->hop, hop = st->hop, nm = st->fft - st->hop;
     if (reset) dfb_state_reset(st);  // DFState::reset clears BOTH memories (libDF/src/lib.rs:156-159)
     size_t nb_in = sizeof(float) * C * T, nb_out = sizeof(float) * 2 * C * Tf * st->tb.F;
-    int rc = st->arena.reserve(nb_in + nb_out + sizeof(float) * C * hop + 2048);
+    int rc = st->arena.reserve(nb_in + nb_out + sizeof(float) * C * nm + 2048);
     if (rc) return rc;
     st->arena.reset();
     float *d_in = st->arena.take<float>(C * T), *d_out = st->arena.take<float>(2 * C * Tf * st->tb.F + 2);
     float *d_mem = nullptr;
     DFB_CUDA(cudaMemcpyAsync(d_in, h_audio, nb_in, cudaMemcpyHostToDevice, st->stream));
-    std::vector<float> mem;
+    // the memory after a channel that entered with `m`: the last nm samples of m followed by its first Tf hop samples
+    auto advance = [&](std::vector<float> &m, const float *xc) {
+        const int64_t n = Tf * hop;
+        if (n >= nm) {
+            memcpy(m.data(), xc + n - nm, sizeof(float) * nm);
+        } else {
+            memmove(m.data(), m.data() + n, sizeof(float) * (nm - n));
+            memcpy(m.data() + nm - n, xc, sizeof(float) * n);
+        }
+    };
+    std::vector<float> mem, cur(st->analysis_mem);
     if (!reset && Tf > 0) {
-        mem.resize((size_t)C * hop);
-        memcpy(mem.data(), st->analysis_mem.data(), sizeof(float) * hop);
-        for (int64_t c = 1; c < C; c++) memcpy(mem.data() + c * hop, h_audio + (c - 1) * T + (Tf - 1) * hop, sizeof(float) * hop);
-        d_mem = st->arena.take<float>(C * hop);
-        DFB_CUDA(cudaMemcpyAsync(d_mem, mem.data(), sizeof(float) * C * hop, cudaMemcpyHostToDevice, st->stream));
+        mem.resize((size_t)C * nm);
+        for (int64_t c = 0; c < C; c++) {
+            memcpy(mem.data() + c * nm, cur.data(), sizeof(float) * nm);
+            if (c + 1 < C) advance(cur, h_audio + c * T);
+        }
+        d_mem = st->arena.take<float>(C * nm);
+        DFB_CUDA(cudaMemcpyAsync(d_mem, mem.data(), sizeof(float) * C * nm, cudaMemcpyHostToDevice, st->stream));
     }
     rc = launch_analysis(st, d_in, C, T, d_out, nullptr, st->stream, d_mem);
     if (rc) return rc;
     if (nb_out) DFB_CUDA(cudaMemcpyAsync(h_spec, d_out, nb_out, cudaMemcpyDeviceToHost, st->stream));
     DFB_CUDA(cudaStreamSynchronize(st->stream));
-    if (Tf > 0) memcpy(st->analysis_mem.data(), h_audio + (C - 1) * T + (Tf - 1) * hop, sizeof(float) * hop);
+    if (Tf > 0) {
+        advance(cur, h_audio + (C - 1) * T);
+        st->analysis_mem = cur;
+    }
     return DFB_OK;
 }
 extern "C" int dfb_analysis_host(dfb_state *st, const float *h_audio, int64_t C, int64_t T, float *h_spec) {
@@ -1242,16 +1511,17 @@ extern "C" int dfb_synthesis_host_ex(dfb_state *st, const float *h_spec, int64_t
     if (!st || !h_spec || !h_audio) return fail(DFB_ERR_INVALID, "null argument");
     if (C <= 0 || Tf <= 0) return fail(DFB_ERR_INVALID, "[df] Input array empty or not contiguous.");
     DFB_CUDA(cudaSetDevice(st->device));
-    const int64_t hop = st->hop;
+    const int64_t hop = st->hop, nm = st->fft - st->hop;   // the tail: N - H partial overlap-add sums
     if (reset) dfb_state_reset(st);  // clears the analysis memory as well (libDF/src/lib.rs:156-159)
     size_t nb_in = sizeof(float) * 2 * C * Tf * st->tb.F, nb_out = sizeof(float) * C * Tf * hop;
-    int rc = st->arena.reserve(nb_in + nb_out + sizeof(float) * 2 * hop + 2048);
+    int rc = st->arena.reserve(nb_in + nb_out + sizeof(float) * 4 * nm + 2048);
     if (rc) return rc;
     st->arena.reset();
     float *d_in = st->arena.take<float>(2 * C * Tf * st->tb.F), *d_out = st->arena.take<float>(C * Tf * hop);
-    float *d_init = st->arena.take<float>(hop), *d_final = st->arena.take<float>(hop);
+    // final tail + two ping-pong tails of the channel chain of the generic kernel
+    float *d_init = st->arena.take<float>(nm), *d_final = st->arena.take<float>(3 * nm);
     DFB_CUDA(cudaMemcpyAsync(d_in, h_spec, nb_in, cudaMemcpyHostToDevice, st->stream));
-    DFB_CUDA(cudaMemcpyAsync(d_init, st->synthesis_mem.data(), sizeof(float) * hop, cudaMemcpyHostToDevice, st->stream));
+    DFB_CUDA(cudaMemcpyAsync(d_init, st->synthesis_mem.data(), sizeof(float) * nm, cudaMemcpyHostToDevice, st->stream));
     ApplyParams p{};
     p.spec = (const float2 *)d_in; p.audio = d_out; p.out_stride = Tf * hop; p.out_offset = 0;
     p.out_len = Tf * hop; p.Tf = (int)Tf; p.mode = 0;
@@ -1259,7 +1529,7 @@ extern "C" int dfb_synthesis_host_ex(dfb_state *st, const float *h_spec, int64_t
     rc = launch_apply_synthesis(st, p, C, st->stream);
     if (rc) return rc;
     DFB_CUDA(cudaMemcpyAsync(h_audio, d_out, nb_out, cudaMemcpyDeviceToHost, st->stream));
-    DFB_CUDA(cudaMemcpyAsync(st->synthesis_mem.data(), d_final, sizeof(float) * hop, cudaMemcpyDeviceToHost, st->stream));
+    DFB_CUDA(cudaMemcpyAsync(st->synthesis_mem.data(), d_final, sizeof(float) * nm, cudaMemcpyDeviceToHost, st->stream));
     DFB_CUDA(cudaStreamSynchronize(st->stream));
     return DFB_OK;
 }

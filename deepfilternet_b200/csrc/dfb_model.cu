@@ -1458,6 +1458,9 @@ extern "C" int dfb_model_set_chunking(dfb_model *m, int device_chunks, int host_
 // The workspace is sized from the model's band layout but the DSP kernels index with the state's: they must agree.
 static int check_state(const dfb_model *m, const dfb_state *st) {
     if (m->device != st->device) return fail(DFB_ERR_INVALID, "model and state live on different devices");
+    if (st->fft != 960 || st->hop != 480)
+        return fail(DFB_ERR_UNSUPPORTED, "the model path is built for fft_size 960 / hop_size 480 (DSP state: %d / %d)", st->fft,
+                    st->hop);
     if (st->tb.E != m->cfg.nb_erb)
         return fail(DFB_ERR_INVALID, "DF state has %d ERB bands, the model was built for %d", st->tb.E, m->cfg.nb_erb);
     if (!m->erb_widths.empty())

@@ -8,7 +8,8 @@ Differences kept on purpose (documented in INTEGRATION.md):
     ``unsafe as_array_mut``, pyDF/src/lib.rs:87,262);
   * ``reset=False`` carries the STFT / ISTFT memories across calls and channels exactly like the
     reference's shared ``DFState`` (channel 0 continues the previous call, channel c continues c - 1);
-  * only fft_size=960 / hop_size=480 kernels are built (all shipped models).
+  * fft_size above 8192 raises ``DfbError`` (``DFB_ERR_UNSUPPORTED``); every fft_size from 2 to 8192, odd or even, and
+    every hop_size <= fft_size / 2 runs on the GPU (fft 960 / hop 480 on the shipped models' specialised kernels).
 """
 from __future__ import annotations
 

@@ -20,7 +20,7 @@ from torch import Tensor, nn
 
 from . import _lib
 from ._lib import ModelConfigC, TensorC, check
-from .config import ModelConfig, load_config
+from .config import ModelConfig, check_stft_size, load_config
 from .libdf import DF
 from .weights import pack_state_dict
 
@@ -63,6 +63,7 @@ class DfNet(nn.Module):
     def __init__(self, cfg: ModelConfig, state_dict: Dict[str, Tensor], df_state: Optional[DF] = None,
                  device: Optional[int] = None, run_df: bool = True):
         super().__init__()
+        check_stft_size(cfg)
         self.cfg = cfg
         self.nb_df = cfg.nb_df
         self.df_bins = cfg.nb_df

@@ -58,7 +58,11 @@ int64_t dfb_profile_report(char *buf, int64_t buflen);
 typedef struct dfb_state dfb_state;
 
 /* pyDF DF.__new__ (pyDF/src/lib.rs:22-39) -> DFState::new (libDF/src/lib.rs:104-154).
- * device: CUDA ordinal.  Built kernels: fft_size 960 / hop_size 480 (all shipped models). */
+ * device: CUDA ordinal.  fft_size 2 ... 8192 (odd or even) and 1 <= hop_size <= fft_size / 2; fft_size > 8192 returns
+ * DFB_ERR_UNSUPPORTED.  The STFT / ISTFT / feature entry points run at every such size (fft 960 / hop 480 on the
+ * specialised kernels of the shipped models, every other size on the generic real FFT); the model path (dfb_enhance*,
+ * dfb_apply, dfb_model_forward_full, dfb_stream_create) returns DFB_ERR_UNSUPPORTED for a state other than 960 / 480.
+ * With reset == 0, the *_host_ex entry points carry fft_size - hop_size samples of memory, as DFState does. */
 int dfb_state_create(dfb_state **out, int device, int sr, int fft_size, int hop_size, int nb_erb,
                      int min_nb_erb_freqs);
 void dfb_state_free(dfb_state *st);
