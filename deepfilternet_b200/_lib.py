@@ -109,6 +109,12 @@ SIGNATURES = {
     "dfb_stream_process_lsnr": (_I, [_VP, _VP, _I64, _VP, _VP, _VP]),
     "dfb_stream_flush_lsnr": (_I, [_VP, _VP, _VP, _VP]),
     "dfb_stream_process_host_lsnr": (_I, [_VP, _VP, _I64, _VP, _VP]),
+    "dfb_stream_create_spec": (_I, [C.POINTER(_VP), _VP, _VP, _I64]),
+    "dfb_stream_process_spec": (_I, [_VP, _VP, _I64, _VP, _VP, _VP, _VP, _VP]),
+    "dfb_stream_flush_spec": (_I, [_VP, _VP, _VP, _VP, _VP, _VP]),
+    "dfb_stream_process_spec_host": (_I, [_VP, _VP, _I64, _VP, _VP, _VP, _VP]),
+    "dfb_debug_analysis_erb": (_I, [_VP, _VP, _I64, _I64, _VP, _VP, _VP]),
+    "dfb_debug_spec_ingest": (_I, [_VP, _VP, _I64, _I64P, _I64P, _I64, _I, _VP, _VP, _VP]),
     "dfb_model_set_max_workspace": (_I, [_VP, _I64]),
     "dfb_model_set_options": (_I, [_VP, _I, _F, _I]),
     "dfb_model_set_chunking": (_I, [_VP, _I, _I, _I]),

@@ -1666,7 +1666,153 @@ struct ChunkIO {
     // at the hop that carries it.  Entries of hops that carry no frame are left as they are.
     int64_t lsnr_from = -1;
     float *lsnr_out = nullptr;
+    // spectral handle (dfb_stream_create_spec), or null: the caller's spectrum frames replace the audio (k_spec_ingest reads
+    // rows[b].in_off / len as complex values / frames, or row b of [B][spec_frames][F]) and k_spec_emit writes the network's
+    // outputs in place of apply + synthesis
+    const float *spec_in = nullptr;
+    int64_t spec_frames = 0;
+    const struct SpecOut *spec_out = nullptr;
 };
+
+// Outputs of a spectral call (k_spec_emit): caller row c, output row j of n_out carries frame f0 + j; slot_row (or null:
+// row c) maps caller rows to the kernel's live rows, -1 for a free slot.  Any output pointer but gains may be null.
+struct SpecOut {
+    float *gains, *coefs, *lsnr;
+    int8_t *stage;
+    int Bc;
+    int64_t n_out, f0;
+    const int *slot_row;
+    int gating;        // LSNR stage gating with th = {min, max_erb, max_df}
+    float th[3];
+    int mask_only;
+};
+
+// ---- spectral handle kernels (dfb_stream_create_spec)
+constexpr int kSpecF = 481, kIngWarps = 4;
+constexpr const char *kSpecIngestName = "k_spec_ingest", *kSpecEmitName = "k_spec_emit";
+// k_spec_ingest replaces k_analysis: warp w of CTA (x, b) reads frame x * kIngWarps + w of live row b once, coalesced
+// (3848 B), and writes the frame's 32 ERB band energies in dB -- |X|^2 and the in-band sums exactly as k_analysis's
+// epilogue, so the same spectrum gives the same bits -- and its first Fd bins, into rows out_t0 ... of buffers holding Tbuf
+// frames per stream, where k_feat_norm reads them.  rows (or null: row b of [B][pitch][F]): row b reads from
+// in + rows[b].in_off (complex values), and zeros from frame rows[b].len on (a closing slot).
+__global__ void __launch_bounds__(32 * kIngWarps) k_spec_ingest(const float2 *__restrict__ in, int64_t pitch, const RaggedRow *__restrict__ rows,
+                                                                int nf, float2 *__restrict__ bins, int Fd, int64_t bins_pitch,
+                                                                float *__restrict__ erb_db, int out_t0, int Tbuf, DspTables tb) {
+    __shared__ float s_p[kIngWarps][kSpecF + 3];
+    const int b = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int t = blockIdx.x * kIngWarps + warp;
+    if (t >= nf) return;
+    const bool have = !rows || t < rows[b].len;
+    const float2 *x = in + (rows ? rows[b].in_off : (int64_t)b * pitch * kSpecF) + (int64_t)t * kSpecF;
+    const int64_t orow = (int64_t)b * Tbuf + out_t0 + t;
+    float2 *brow = bins + orow * bins_pitch;
+    float *P = s_p[warp];
+    for (int k = lane; k < kSpecF; k += 32) {
+        const float2 v = have ? __ldg(x + k) : make_float2(0.f, 0.f);
+        P[k] = __fadd_rn(__fmul_rn(v.x, v.x), __fmul_rn(v.y, v.y));
+        if (k < Fd) brow[k] = v;
+    }
+    __syncwarp();
+    // band energies: sequential sum inside each band, factor 1/width inside the sum (lib.rs:288-292), as k_analysis
+    for (int band = lane; band < tb.E; band += 32) {
+        const int o = tb.erb_off[band], n = tb.erb_off[band + 1] - o;
+        const float kinv = tb.erb_kinv[band];
+        float acc = 0.f;
+        for (int j = 0; j < n; j++) acc = __fadd_rn(acc, __fmul_rn(P[o + j], kinv));
+        erb_db[orow * tb.E + band] = __fmul_rn(log10f(__fadd_rn(acc, 1e-10f)), 10.f);
+    }
+}
+
+static int launch_spec_ingest(const dfb_state *st, const float *in, int64_t pitch, const RaggedRow *rows, int B, int nf, float *bins,
+                              int Fd, int64_t bins_pitch, float *erb_db, int out_t0, int Tbuf, cudaStream_t s) {
+    if (B <= 0 || nf <= 0) return DFB_OK;
+    if (st->tb.F != kSpecF || st->tb.E > 32 * 8) return fail(DFB_ERR_UNSUPPORTED, "spectral input is built for fft_size 960");
+    // timed by dfb_profile_* like the enhancement path's kernels, but outside the DFB_PROF list whose per-kernel roofline
+    // model bench.py keeps: a spectral handle is not on the enhancement path (bench_stream_spec.py reports its share)
+    dfb::ProfScope prof_scope__(kSpecIngestName, s);
+    dim3 grid((unsigned)((nf + kIngWarps - 1) / kIngWarps), (unsigned)B);
+    k_spec_ingest<<<grid, 32 * kIngWarps, 0, s>>>((const float2 *)in, pitch, rows, nf, (float2 *)bins, Fd, bins_pitch, erb_db, out_t0,
+                                                  Tbuf, st->tb);
+    DFB_LAUNCH_CHECK();
+    return DFB_OK;
+}
+
+// k_spec_emit replaces apply + synthesis: CTA (j, c) writes output row j of caller row c in one pass -- the frame's ERB
+// gains (reduced over its link group in registers, as the LINK apply kernel does), its coefficients and LSNR, after the
+// stage rule -- or NaN / -1 where the row carries no frame.  The frame rule is k_lsnr_out's: window frame t = f0 + j - w0 is
+// emitted when t_first <= t < Te, clipped at the row's end and first frame.  m [B][mcT][E], coefs [B][mcT][FO], lsnr [B][mcT].
+__global__ void __launch_bounds__(128) k_spec_emit(SpecOut o, const float *__restrict__ m, const float *__restrict__ coefs,
+                                                   const float *__restrict__ lsnr, int mcT, int E, int FO, int64_t w0, int t_first, int Te,
+                                                   const RaggedRow *__restrict__ rows, const int64_t *__restrict__ first,
+                                                   const LinkRow *__restrict__ links, int reduce) {
+    const int c = blockIdx.y, tid = threadIdx.x;
+    const int64_t j = blockIdx.x, q = (int64_t)c * o.n_out + j;
+    const int r = o.slot_row ? o.slot_row[c] : c;
+    int64_t t = -1;
+    if (r >= 0) {
+        int te = Te;
+        if (rows) te = min(te, (int)(rows[r].Tf - w0));
+        const int t0 = max(t_first, stream_first(first, r, w0));
+        const int64_t tt = o.f0 + j - w0;
+        if (tt >= t0 && tt < te) t = tt;
+    }
+    if (t < 0) {
+        const float nan = __int_as_float(0x7fffffff);
+        for (int e = tid; e < E; e += blockDim.x) o.gains[q * E + e] = nan;
+        if (o.coefs)
+            for (int k = tid; k < FO; k += blockDim.x) o.coefs[q * FO + k] = nan;
+        if (tid == 0) {
+            if (o.lsnr) o.lsnr[q] = nan;
+            if (o.stage) o.stage[q] = -1;
+        }
+        return;
+    }
+    const float l = lsnr[(int64_t)r * mcT + t];
+    const int lb = links ? links[r].first : r;          // gating reads the link group's channel 0
+    const float lg = lsnr[(int64_t)lb * mcT + t];
+    int stage = 1;
+    if (o.gating) stage = lg < o.th[0] ? 0 : lg > o.th[1] ? 3 : lg > o.th[2] ? 2 : 1;   // tract.rs:658-672
+    if (stage == 1 && o.mask_only) stage = 2;
+    for (int e = tid; e < E; e += blockDim.x) {
+        float v = stage == 0 ? 0.f : 1.f;
+        if (stage == 1 || stage == 2) {
+            if (!links) {
+                v = m[((int64_t)r * mcT + t) * E + e];
+            } else {   // the link group's max / mean in channel order, the mean as the fp32 sum times fl32(1 / n)
+                const int n = links[r].n;
+                const int64_t stride = (int64_t)mcT * E;
+                const float *p = m + (int64_t)lb * stride + t * E + e;
+                v = p[0];
+                if (reduce == kReduceMax) {
+                    for (int k = 1; k < n; k++) v = fmaxf(v, p[k * stride]);
+                } else {
+                    for (int k = 1; k < n; k++) v += p[k * stride];
+                    v = v * __frcp_rn((float)n);
+                }
+            }
+        }
+        o.gains[q * E + e] = v;
+    }
+    if (o.coefs) {
+        const float *src = coefs + ((int64_t)r * mcT + t) * FO;
+        for (int k = tid; k < FO; k += blockDim.x) o.coefs[q * FO + k] = stage == 1 ? src[k] : 0.f;
+    }
+    if (tid == 0) {
+        if (o.lsnr) o.lsnr[q] = l;
+        if (o.stage) o.stage[q] = (int8_t)stage;
+    }
+}
+
+static int launch_spec_emit(const SpecOut &o, const float *m, const float *coefs, const float *lsnr, int mcT, int E, int FO, int64_t w0,
+                            int t_first, int Te, const RaggedRow *rows, const int64_t *first, const LinkRow *links, int reduce,
+                            cudaStream_t s) {
+    if (o.Bc <= 0 || o.n_out <= 0) return DFB_OK;
+    dfb::ProfScope prof_scope__(kSpecEmitName, s);   // (see launch_spec_ingest)
+    k_spec_emit<<<dim3((unsigned)o.n_out, (unsigned)o.Bc), 128, 0, s>>>(o, m, coefs, lsnr, mcT, E, FO, w0, t_first, Te, rows, first, links,
+                                                                        reduce);
+    DFB_LAUNCH_CHECK();
+    return DFB_OK;
+}
 
 // LSNR of the frames the apply kernel emitted in this chunk, by the kernel's own emission rule: output hop j of row b
 // carries window frame t = f0 + j - w0, which was emitted when t_first <= t < Te (with rows: Te clipped at the stream's
@@ -1719,16 +1865,22 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     float *fs = arena.take<float>((size_t)B * Tsb * Fd * 2);
     float *mm = arena.take<float>((size_t)B * (Tw + 1) * E);
     float *cc = arena.take<float>((size_t)B * (Tw + 1) * Fd * O2);
-    float *ll = (io.lsnr_th || io.lsnr_from >= 0) ? arena.take<float>((size_t)B * (Tw + 1)) : nullptr;
+    float *ll = (io.lsnr_th || io.lsnr_from >= 0 || io.spec_out) ? arena.take<float>((size_t)B * (Tw + 1)) : nullptr;
     float *aa = c.model_kind == 1 ? arena.take<float>((size_t)B * (Tw + 1)) : nullptr;   // df_alpha (v1)
     if (!cc || (c.model_kind == 1 && !aa)) return fail(DFB_ERR_OOM, "chunk workspace exhausted");
-    // ---- features: carried history, then the new frames
-    if ((rc = load_tail(s, spec, Tsb, (size_t)2 * F, n_hist, S.t_spec, g.Hf, 0, B)) || (rc = load_tail(s, fe, Tsb, E, n_hist, S.t_fe, g.Hf, 0, B)) ||
-        (rc = load_tail(s, fs, Tsb, (size_t)2 * Fd, n_hist, S.t_fs, g.Hf, 0, B)))
+    // ---- features: carried history, then the new frames (a spectral handle keeps no spectrum: nothing is applied)
+    const bool spectral = io.spec_out != nullptr;
+    if ((!spectral && (rc = load_tail(s, spec, Tsb, (size_t)2 * F, n_hist, S.t_spec, g.Hf, 0, B))) ||
+        (rc = load_tail(s, fe, Tsb, E, n_hist, S.t_fe, g.Hf, 0, B)) || (rc = load_tail(s, fs, Tsb, (size_t)2 * Fd, n_hist, S.t_fs, g.Hf, 0, B)))
         return rc;
     if (n_new > 0) {
-        AnaWindow w{(int)(S.a1 - io.audio_frame0), n_new, n_hist, Tsb, io.audio_stride, io.rows};
-        if ((rc = launch_analysis(st, io.audio, B, io.audio_T, spec, fe, s, io.init_mem, &w))) return rc;
+        if (spectral) {   // the ERB dB and the first Fd bins of the caller's frames, where k_feat_norm reads them
+            rc = launch_spec_ingest(st, io.spec_in, io.spec_frames, io.rows, B, n_new, spec, Fd, F, fe, n_hist, Tsb, s);
+        } else {
+            AnaWindow w{(int)(S.a1 - io.audio_frame0), n_new, n_hist, Tsb, io.audio_stride, io.rows};
+            rc = launch_analysis(st, io.audio, B, io.audio_T, spec, fe, s, io.init_mem, &w);
+        }
+        if (rc) return rc;
         if ((rc = launch_feat_norm(fe + (size_t)n_hist * E, E, E, spec + (size_t)n_hist * 2 * F, Fd, F, B, n_new, c.norm_alpha,
                                    S.started ? S.erb_state : nullptr, S.started ? S.unit_state : nullptr, fe + (size_t)n_hist * E,
                                    fs + (size_t)n_hist * 2 * Fd, s, Tsb, S.erb_state, S.unit_state)))
@@ -1739,7 +1891,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
         // the feature buffers hold Tsb frames per stream of which the first Tv are valid: keep the last nf valid ones
         const size_t fes[3] = {(size_t)2 * F, (size_t)E, (size_t)2 * Fd};
         float *bufs[3] = {spec, fe, fs}, *tails[3] = {S.t_spec, S.t_fe, S.t_fs};
-        for (int i = 0; i < 3; i++)
+        for (int i = spectral ? 1 : 0; i < 3; i++)
             DFB_CUDA(cudaMemcpy2DAsync(tails[i] + (size_t)(g.Hf - nf) * fes[i], sizeof(float) * fes[i] * g.Hf,
                                        bufs[i] + (size_t)(Tv - nf) * fes[i], sizeof(float) * fes[i] * Tsb, sizeof(float) * fes[i] * nf, B,
                                        cudaMemcpyDeviceToDevice, s));
@@ -1754,15 +1906,21 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     S.dnn_started = true;
     // the halo rows of m / coefs come from skipped recurrences: restore the last finished frames from the previous chunk
     // (the apply kernel re-synthesises frame e0 - 1 for its overlap-add tail; DFN2's masked taps reach 2 frames further back)
-    if (Rc > 0 && S.n_mc > 0) {
+    if (Rc > 0 && S.n_mc > 0 && !spectral) {
         const int n = S.n_mc < Rc ? S.n_mc : Rc;
         if ((rc = load_tail(s, mm, Tw, E, n, S.t_m, kMcTail, Rc - n, B)) || (rc = load_tail(s, cc, Tw, (size_t)Fd * O2, n, S.t_c, kMcTail, Rc - n, B)))
             return rc;
         if (ll && (rc = load_tail(s, ll, Tw, 1, n, S.t_l, kMcTail, Rc - n, B))) return rc;
     }
     }
+    // ---- spectral handle: the network's outputs of frames [e0, e1n) to the caller's rows (every row, NaN where none)
+    if (spectral) {
+        const int t_first = (int)(S.e1 - W0), Te = run_dnn ? (int)(e1n - W0) : t_first;
+        if ((rc = launch_spec_emit(*io.spec_out, mm, cc, ll, Tw, E, Fd * O2, W0, t_first, Te, io.rows, io.first, io.links, io.reduce, s)))
+            return rc;
+    }
     // ---- apply + synthesis of frames [e0, e1n) (ragged: a stream that ends in this chunk emits up to its end)
-    if (run_dnn && (e1n > S.e1 || (io.rows && !io.first))) {
+    else if (run_dnn && (e1n > S.e1 || (io.rows && !io.first))) {
         dfb::ApplyParams p{};
         p.spec = (const float2 *)spec; p.m = mm; p.coefs = cc; p.audio = io.out; p.spec_out = nullptr;
         p.out_stride = io.out_stride; p.out_len = io.out_len;
@@ -1787,7 +1945,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     }
     // ---- carry
     {
-        if (run_dnn) {
+        if (run_dnn && !spectral) {
             const int nm = Tw < kMcTail ? Tw : kMcTail;
             if ((rc = save_tail(s, mm, Tw, E, nm, S.t_m, kMcTail, B)) || (rc = save_tail(s, cc, Tw, (size_t)Fd * O2, nm, S.t_c, kMcTail, B))) return rc;
             if (ll && (rc = save_tail(s, ll, Tw, 1, nm, S.t_l, kMcTail, B))) return rc;
@@ -2331,13 +2489,18 @@ struct dfb_stream {
     int64_t lsnr_from = -1;
     float *stage_lsnr = nullptr;                       // device staging of dfb_stream_process_host_lsnr
     size_t stage_lsnr_cap = 0;
+    // spectral handle (dfb_stream_create_spec): spectrum frames in, the network's outputs out; runs the LSNR head always
+    bool spectral = false;
+    int *d_slotmap = nullptr;                          // slot path: per slot its row of the active prefix, -1 free
+    float *spec_stage_in = nullptr, *spec_stage_out = nullptr;   // device staging of dfb_stream_process_spec_host
+    size_t spec_in_cap = 0, spec_out_cap = 0;
 };
 
 // the handle's default post-filter beta: the model's option (0 = off) for DeepFilterNet3; per-row beta is not used for
 // DeepFilterNet2, whose post filter acts on the ERB gains with a fixed beta
 static float default_beta(const dfb_model *m) { return (m->cfg.model_kind == 3 && m->post_filter) ? m->pf_beta : 0.f; }
 
-extern "C" int dfb_stream_create(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B, float atten_lim_db) {
+static int stream_new(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B, float atten_lim_db, bool spectral) {
     if (!out || !m || !st || B <= 0 || B > 65535) return fail(DFB_ERR_INVALID, "bad argument");
     *out = nullptr;
     if (int rcs = check_state(m, st)) return rcs;
@@ -2347,6 +2510,8 @@ extern "C" int dfb_stream_create(dfb_stream **out, dfb_model *m, dfb_state *st, 
     dfb_stream *h = new dfb_stream();
     h->m = m; h->st = st; h->device = m->device; h->B = (int)B;
     h->lim = (atten_lim_db > 0.f) ? powf(10.f, -atten_lim_db / 20.f) : 0.f;
+    h->spectral = spectral;
+    if (spectral) h->lsnr_from = 0;
     size_t off[16];
     const size_t n = state_floats(m->cfg, st, (int)B, off);
     if (cudaMalloc(&h->slab, n * sizeof(float)) != cudaSuccess) { delete h; return fail(DFB_ERR_OOM, "stream state allocation failed"); }
@@ -2355,6 +2520,14 @@ extern "C" int dfb_stream_create(dfb_stream **out, dfb_model *m, dfb_state *st, 
     h->beta_run = default_beta(m);
     *out = h;
     return DFB_OK;
+}
+
+extern "C" int dfb_stream_create(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B, float atten_lim_db) {
+    return stream_new(out, m, st, B, atten_lim_db, false);
+}
+// df_process_frame_raw's handle: spectrum frames in, gains / coefs / LSNR / stage out (no STFT, nothing applied)
+extern "C" int dfb_stream_create_spec(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B) {
+    return stream_new(out, m, st, B, 0.f, true);
 }
 
 extern "C" void dfb_stream_free(dfb_stream *h) {
@@ -2369,6 +2542,9 @@ extern "C" void dfb_stream_free(dfb_stream *h) {
     if (h->d_grp) cudaFree(h->d_grp);
     if (h->d_ctl) cudaFree(h->d_ctl);
     if (h->stage_lsnr) cudaFree(h->stage_lsnr);
+    if (h->d_slotmap) cudaFree(h->d_slotmap);
+    if (h->spec_stage_in) cudaFree(h->spec_stage_in);
+    if (h->spec_stage_out) cudaFree(h->spec_stage_out);
     delete h;
 }
 
@@ -2380,7 +2556,7 @@ extern "C" int dfb_stream_reset(dfb_stream *h) {
     h->fed = false;
     h->slots = false;
     h->ctl_on = false;
-    h->lsnr_from = -1;
+    h->lsnr_from = h->spectral ? 0 : -1;
     return DFB_OK;
 }
 
@@ -2413,11 +2589,13 @@ extern "C" int dfb_stream_set_mask_reduce(dfb_stream *h, int channels, int reduc
 }
 
 // LSNR stage gating of the Rust runtime (libDF/src/tract.rs:658-672; thresholds tract.rs:180-185, DfParams of
-// deep-filter / capi.rs).  Off by default: the Python path this library mirrors does not gate.  DeepFilterNet3 only.
+// deep-filter / capi.rs).  Off by default: the Python path this library mirrors does not gate.  DeepFilterNet3 only on
+// audio handles (the apply kernel gates mode 1); a spectral handle gates in k_spec_emit, for DeepFilterNet2 too.
 extern "C" int dfb_stream_set_lsnr_thresholds(dfb_stream *h, int enable, float min_db_thresh, float max_db_erb_thresh,
                                               float max_db_df_thresh) {
     if (!h) return fail(DFB_ERR_INVALID, "null stream");
-    if (enable && h->m->cfg.model_kind != 3) return fail(DFB_ERR_UNSUPPORTED, "LSNR stage gating: DeepFilterNet3 topologies only");
+    if (enable && h->m->cfg.model_kind != 3 && !h->spectral)
+        return fail(DFB_ERR_UNSUPPORTED, "LSNR stage gating: DeepFilterNet3 topologies only");
     h->gating = enable != 0;
     h->th[0] = min_db_thresh; h->th[1] = max_db_erb_thresh; h->th[2] = max_db_df_thresh;
     return DFB_OK;
@@ -2425,6 +2603,7 @@ extern "C" int dfb_stream_set_lsnr_thresholds(dfb_stream *h, int enable, float m
 
 extern "C" int64_t dfb_stream_latency_frames(const dfb_stream *h) {
     if (!h) return -1;
+    if (h->spectral) return h->m->cfg.conv_lookahead;   // the outputs wait for the encoder's look-ahead only
     const ChunkGeom g = chunk_geom(h->m->cfg);
     return g.Lmax + g.lag;
 }
@@ -2581,6 +2760,8 @@ extern "C" int dfb_stream_close_slots(dfb_stream *h, const int64_t *slots, int64
 // handle's default at that call) and, when it differs from the one of the slot's last call, switches at the call's first
 // output frame f0: frame f0 - 1, which the apply kernel re-synthesises for its overlap-add tail, keeps the previous one.
 static int ctl_set(dfb_stream *h, const int64_t *slots, int64_t n, bool beta, float v) {
+    if (h && h->spectral)
+        return fail(DFB_ERR_UNSUPPORTED, "attenuation limit and post filter are apply-stage settings: a spectral handle applies nothing");
     if (int rc = slot_list_check(h, slots, n)) return rc;
     const dfb_model_config &c = h->m->cfg;
     if (c.df_order != 5 || c.nb_df != 96 || c.nb_erb != 32)
@@ -2687,18 +2868,39 @@ static int slots_move_rows(dfb_stream *h, cudaStream_t s) {
     return DFB_OK;
 }
 
+// The spectral side of a call's ChunkIO: input frames [B][n][F] (slot path: where the row table says), outputs to `so`
+// with n_out rows per caller row from frame f0 on, the LSNR head always on
+static void spec_io(const dfb_stream *h, ChunkIO &io, SpecOut *so, const float *d_in, int64_t n, int64_t n_out, int64_t f0,
+                    const int *slotmap) {
+    so->Bc = h->B; so->n_out = n_out; so->f0 = f0; so->slot_row = slotmap;
+    so->gating = h->gating; so->th[0] = h->th[0]; so->th[1] = h->th[1]; so->th[2] = h->th[2];
+    so->mask_only = h->m->mask_only;
+    io.spec_in = d_in; io.spec_frames = n; io.spec_out = so;
+    io.lsnr_from = 0; io.lsnr_out = nullptr;
+}
+// a spectral call with no live row: every output row carries no frame (NaN, stage -1)
+static int spec_fill_empty(const SpecOut &so, const dfb_model_config &c, int64_t rows, cudaStream_t s) {
+    DFB_CUDA(cudaMemsetAsync(so.gains, 0xff, sizeof(float) * rows * c.nb_erb, s));
+    if (so.coefs) DFB_CUDA(cudaMemsetAsync(so.coefs, 0xff, sizeof(float) * rows * c.nb_df * 2 * c.df_order, s));
+    if (so.lsnr) DFB_CUDA(cudaMemsetAsync(so.lsnr, 0xff, sizeof(float) * rows, s));
+    if (so.stage) DFB_CUDA(cudaMemsetAsync(so.stage, 0xff, rows, s));
+    return DFB_OK;
+}
+
 // Slot path of one call: rows [0, n_act) of the slab, the row table for calls of n input hops, output rows zero first.
-static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s) {
+// Spectral handle (so != null): d_in is [B][n][F] complex, the outputs go to so's buffers, d_out / d_lsnr are null.
+static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s, SpecOut *so) {
     dfb_model *m = h->m;
     dfb_state *st = h->st;
     StreamState &S = h->S;
     const ChunkGeom g = chunk_geom(m->cfg);
     const int hop = st->hop, B = h->B;
-    const int64_t Ltot = g.Lmax + g.lag, n_out = flush ? Ltot : n;
+    const int64_t Ltot = dfb_stream_latency_frames(h), n_out = flush ? Ltot : n;
+    const int64_t lag = so ? 0 : g.lag, la = Ltot - lag;   // feature look-ahead of the DNN frames; their outputs' further lag
     const int64_t a0 = S.a1, a1n = a0 + (flush ? 0 : n);
     if (a1n >= kOpenEnd - 1) return fail(DFB_ERR_UNSUPPORTED, "stream clock beyond 2^31 - 2 frames: reset the stream");
     int rc = DFB_OK;
-    int64_t d1n = flush ? a1n : a1n - g.Lmax, e1n = flush ? a1n : d1n - g.lag;
+    int64_t d1n = flush ? a1n : a1n - la, e1n = flush ? a1n : d1n - lag;
     if (d1n < S.d1) d1n = S.d1;
     if (e1n < S.e1) e1n = S.e1;
     if (flush) slots_close_all(h);
@@ -2708,10 +2910,11 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
         std::vector<int64_t> first((size_t)h->n_act);
         std::vector<LinkRow> grp((size_t)h->n_act);
         bool linked = false;   // the link table goes to the kernels only while a group of more than one channel is linked
+        const int64_t unit = so ? kSpecF : hop, per = so ? 1 : hop;   // input offsets in complex values / samples, lengths in frames / samples
         for (int r = 0; r < h->n_act; r++) {
             const int b = h->row_slot[(size_t)r];
             const bool open = h->slot_state[(size_t)b] == kSlotOpen;
-            rows[(size_t)r] = RaggedRow{b * n * hop, open ? n * hop : 0, b * n_out * hop, n_out * hop, h->slot_end[(size_t)b]};
+            rows[(size_t)r] = RaggedRow{b * n * unit, open ? n * per : 0, b * n_out * hop, n_out * hop, h->slot_end[(size_t)b]};
             first[(size_t)r] = h->slot_first[(size_t)b];
             grp[(size_t)r] = LinkRow{h->slot_row[(size_t)h->slot_grp[(size_t)b]], h->slot_nch[(size_t)b]};
             linked |= grp[(size_t)r].n > 1 && h->group_reduce != kReduceNone;
@@ -2721,17 +2924,25 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
             DFB_CUDA(cudaMemcpyAsync(h->d_first, first.data(), sizeof(int64_t) * first.size(), cudaMemcpyHostToDevice, s));
             if (linked) DFB_CUDA(cudaMemcpyAsync(h->d_grp, grp.data(), sizeof(LinkRow) * grp.size(), cudaMemcpyHostToDevice, s));
         }
+        if (so) {   // k_spec_emit covers every caller row: free slots get NaN / -1
+            if (!h->d_slotmap && cudaMalloc(&h->d_slotmap, sizeof(int) * (size_t)B) != cudaSuccess) {
+                h->d_slotmap = nullptr;
+                return fail(DFB_ERR_OOM, "slot table allocation failed");
+            }
+            DFB_CUDA(cudaMemcpyAsync(h->d_slotmap, h->slot_row.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, s));
+        }
         h->tab_dirty = false;
         h->tab_n = n;
         h->tab_linked = linked;
     }
-    if (n_out > 0) DFB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * B * n_out * hop, s));   // free slots; frames outside a stream
+    if (n_out > 0 && !so) DFB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * B * n_out * hop, s));   // free slots; frames outside a stream
     if (d_lsnr && n_out > 0) DFB_CUDA(cudaMemsetAsync(d_lsnr, 0xff, sizeof(float) * B * n_out, s));   // NaN: hops without a frame
     const int64_t f0 = a0 - Ltot;   // output hop j carries frame a0 - Ltot + j (flush: a1 = a0)
     if (h->ctl_on && (rc = ctl_rows(h, f0, s))) return rc;
     h->beta_run = default_beta(m);
     h->fed = true;
     if (h->n_act == 0) {   // nothing to compute: the clock moves on (a slot opened later starts from zeroed tails)
+        if (so && n_out > 0 && (rc = spec_fill_empty(*so, m->cfg, B * n_out, s))) return rc;
         S.a1 = a1n; S.d1 = d1n; S.e1 = e1n;
         if (a1n > 0) S.started = true;
         if (d1n > 0) S.dnn_started = true;
@@ -2739,9 +2950,10 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
         slots_retire(h, flush ? a1n : a1n - Ltot);
         return DFB_OK;
     }
-    ChunkIO io{d_in, n * hop, n * hop, a0, nullptr, d_out, n_out * hop, n_out * hop, f0 * hop, h->lim, h->gating ? h->th : nullptr,
-               h->d_rows, h->n_act};
+    ChunkIO io{so ? nullptr : d_in, n * hop, n * hop, a0, nullptr, d_out, n_out * hop, n_out * hop, f0 * hop, h->lim,
+               h->gating && !so ? h->th : nullptr, h->d_rows, h->n_act};
     io.first = h->d_first;
+    if (so) spec_io(h, io, so, d_in, n, n_out, f0, h->d_slotmap);
     if (h->tab_linked) { io.links = h->d_grp; io.reduce = h->group_reduce; }
     if (h->ctl_on) io.ctl = h->d_ctl;
     io.lsnr_from = h->lsnr_from;
@@ -2749,12 +2961,12 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
     rc = m->arena.reserve(chunk_bytes_per_stream(m->cfg, st, (int)(d1n - (S.d1 > kHalo ? S.d1 - kHalo : 0)) + 1) * (size_t)h->n_act +
                               (2 << 20));
     if (rc) return rc;
-    if (!flush && a1n > a0) {
+    if (!flush && a1n > a0 && !so) {
         if (!S.started) DFB_CUDA(cudaMemsetAsync(S.ana_mem, 0, sizeof(float) * B * hop, s));
         io.init_mem = S.ana_mem;
     }
     if ((rc = run_chunk(m, st, S, io, a1n, d1n, e1n, s))) return rc;
-    if (!flush) {
+    if (!flush && !so) {
         k_carry_hop<<<h->n_act, 128, 0, s>>>(S.ana_mem, d_in, h->d_rows, (n - 1) * hop, hop);
         DFB_LAUNCH_CHECK();
     }
@@ -2763,18 +2975,20 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
     return DFB_OK;
 }
 
-static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s) {
+static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s,
+                       SpecOut *so = nullptr) {
     if (d_lsnr && h->lsnr_from < 0) h->lsnr_from = h->S.d1;   // from now on every call runs the LSNR head
-    if (h->slots) return slots_step(h, d_in, n, flush, d_out, d_lsnr, s);
+    if (h->slots) return slots_step(h, d_in, n, flush, d_out, d_lsnr, s, so);
     dfb_model *m = h->m;
     dfb_state *st = h->st;
     StreamState &S = h->S;
     const ChunkGeom g = chunk_geom(m->cfg);
     const int hop = st->hop, B = h->B;
-    const int64_t Ltot = g.Lmax + g.lag;
+    const int64_t Ltot = dfb_stream_latency_frames(h);
+    const int64_t lag = so ? 0 : g.lag, la = Ltot - lag;
     const int64_t n_out = flush ? Ltot : n;
     const int64_t a0 = S.a1, a1n = a0 + (flush ? 0 : n);
-    int64_t d1n = flush ? a1n : a1n - g.Lmax, e1n = flush ? a1n : d1n - g.lag;
+    int64_t d1n = flush ? a1n : a1n - la, e1n = flush ? a1n : d1n - lag;
     if (d1n < S.d1) d1n = S.d1;
     if (e1n < S.e1) e1n = S.e1;
     // the window of this call: halo + new DNN frames (+ look-ahead)
@@ -2784,23 +2998,24 @@ static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, 
     if (rc) return rc;
     // output slot j (hop j of d_out) carries frame a0 - Ltot + j (flush: a1 - Ltot + j); frames < 0 are silence
     const int64_t f0 = (flush ? S.a1 : a0) - Ltot;
-    if (f0 < 0 || e1n <= S.e1) DFB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * B * n_out * hop, s));
+    if (!so && (f0 < 0 || e1n <= S.e1)) DFB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * B * n_out * hop, s));
     if (d_lsnr && n_out > 0) DFB_CUDA(cudaMemsetAsync(d_lsnr, 0xff, sizeof(float) * B * n_out, s));   // NaN: hops without a frame
-    ChunkIO io{d_in, (flush ? 0 : n) * hop, (flush ? 0 : n) * hop, a0, S.started ? S.ana_mem : nullptr, d_out, n_out * hop, n_out * hop,
-               f0 * hop, h->lim, h->gating ? h->th : nullptr};
+    ChunkIO io{so ? nullptr : d_in, (flush ? 0 : n) * hop, (flush ? 0 : n) * hop, a0, S.started ? S.ana_mem : nullptr, d_out, n_out * hop,
+               n_out * hop, f0 * hop, h->lim, h->gating && !so ? h->th : nullptr};
     io.links = h->links;
     io.reduce = h->reduce;
     io.lsnr_from = h->lsnr_from;
     io.lsnr_out = d_lsnr;
+    if (so) spec_io(h, io, so, d_in, n, n_out, f0, nullptr);
     h->beta_run = default_beta(m);
     h->fed = true;
-    if (!flush && a1n > a0) {
+    if (!flush && a1n > a0 && !so) {
         // zero analysis memory before the very first frame
         if (!S.started) DFB_CUDA(cudaMemsetAsync(S.ana_mem, 0, sizeof(float) * B * hop, s));
         io.init_mem = S.ana_mem;
     }
     if ((rc = run_chunk(m, st, S, io, a1n, d1n, e1n, s))) return rc;
-    if (!flush)  // carried analysis memory: the last hop of this call's input
+    if (!flush && !so)  // carried analysis memory: the last hop of this call's input
         DFB_CUDA(cudaMemcpy2DAsync(S.ana_mem, sizeof(float) * hop, d_in + (n - 1) * hop, sizeof(float) * n * hop, sizeof(float) * hop, B,
                                    cudaMemcpyDeviceToDevice, s));
     m->arena.reset();
@@ -2819,7 +3034,11 @@ static void flushed_all(dfb_stream *h) {
 
 // d_in [B][n_frames * hop] -> d_out [B][n_frames * hop] (device pointers, asynchronous on `stream`); d_lsnr (or null)
 // [B][n_frames]: the LSNR of the frame each output hop carries, NaN where it carries none
+static int audio_only(const dfb_stream *h) {
+    return h && h->spectral ? fail(DFB_ERR_INVALID, "a spectral handle takes spectrum frames: dfb_stream_process_spec / flush_spec") : DFB_OK;
+}
 extern "C" int dfb_stream_process_lsnr(dfb_stream *h, const float *d_in, int64_t n_frames, float *d_out, float *d_lsnr, void *stream) {
+    if (int rc = audio_only(h)) return rc;
     if (!h || !d_in || !d_out || n_frames <= 0) return fail(DFB_ERR_INVALID, "bad argument");
     DFB_CUDA(cudaSetDevice(h->m->device));
     return stream_step(h, d_in, n_frames, false, d_out, d_lsnr, (cudaStream_t)stream);
@@ -2832,6 +3051,7 @@ extern "C" int dfb_stream_process(dfb_stream *h, const float *d_in, int64_t n_fr
 // batch enhance(); d_out [B][latency * hop].  Closes every open slot; on the slot-free path the stream must be reset before
 // it is fed again.  d_lsnr (or null) [B][latency]: the LSNR of the tail frames.
 extern "C" int dfb_stream_flush_lsnr(dfb_stream *h, float *d_out, float *d_lsnr, void *stream) {
+    if (int rc = audio_only(h)) return rc;
     if (!h || !d_out) return fail(DFB_ERR_INVALID, "bad argument");
     DFB_CUDA(cudaSetDevice(h->m->device));
     int rc = DFB_OK;
@@ -2844,6 +3064,7 @@ extern "C" int dfb_stream_flush(dfb_stream *h, float *d_out, void *stream) { ret
 // host-pointer variant (synchronous): h_in / h_out [B][n_frames * hop]; h_in == NULL flushes into h_out [B][latency * hop];
 // h_lsnr (or null) [B][n_frames] / [B][latency] as dfb_stream_process_lsnr
 extern "C" int dfb_stream_process_host_lsnr(dfb_stream *h, const float *h_in, int64_t n_frames, float *h_out, float *h_lsnr) {
+    if (int rc = audio_only(h)) return rc;
     if (!h || (h_in && n_frames <= 0)) return fail(DFB_ERR_INVALID, "bad argument");
     DFB_CUDA(cudaSetDevice(h->m->device));
     const bool flush = h_in == nullptr;
@@ -2881,4 +3102,110 @@ extern "C" int dfb_stream_process_host_lsnr(dfb_stream *h, const float *h_in, in
 }
 extern "C" int dfb_stream_process_host(dfb_stream *h, const float *h_in, int64_t n_frames, float *h_out) {
     return dfb_stream_process_host_lsnr(h, h_in, n_frames, h_out, nullptr);
+}
+
+// ---- spectral handle (dfb_stream_create_spec): capi.rs df_process_frame_raw, batched and for n_frames frames at once.
+// d_spec [B][n_frames][F] complex -> [B][n_frames] rows of gains / coefs / LSNR / stage (device pointers, asynchronous).
+static int spec_only(const dfb_stream *h) {
+    if (!h) return fail(DFB_ERR_INVALID, "null stream");
+    return h->spectral ? DFB_OK : fail(DFB_ERR_INVALID, "an audio handle takes audio: dfb_stream_create_spec makes a spectral one");
+}
+extern "C" int dfb_stream_process_spec(dfb_stream *h, const float *d_spec, int64_t n_frames, float *d_gains, float *d_coefs,
+                                       float *d_lsnr, int8_t *d_stage, void *stream) {
+    if (int rc = spec_only(h)) return rc;
+    if (!d_spec || !d_gains || n_frames <= 0) return fail(DFB_ERR_INVALID, "bad argument");
+    DFB_CUDA(cudaSetDevice(h->m->device));
+    SpecOut so{d_gains, d_coefs, d_lsnr, d_stage};
+    return stream_step(h, d_spec, n_frames, false, nullptr, nullptr, (cudaStream_t)stream, &so);
+}
+// end of stream: the last `latency` frames, computed with zero look-ahead features; closes every open slot
+extern "C" int dfb_stream_flush_spec(dfb_stream *h, float *d_gains, float *d_coefs, float *d_lsnr, int8_t *d_stage, void *stream) {
+    if (int rc = spec_only(h)) return rc;
+    const int64_t L = dfb_stream_latency_frames(h);
+    if (L > 0 && !d_gains) return fail(DFB_ERR_INVALID, "bad argument");
+    DFB_CUDA(cudaSetDevice(h->m->device));
+    int rc = DFB_OK;
+    SpecOut so{d_gains, d_coefs, d_lsnr, d_stage};
+    if (L > 0) rc = stream_step(h, nullptr, 0, true, nullptr, nullptr, (cudaStream_t)stream, &so);
+    if (!rc) flushed_all(h);
+    return rc;
+}
+static int stage_grow(float **p, size_t *cap, size_t bytes) {
+    if (bytes <= *cap) return DFB_OK;
+    if (*p) cudaFree(*p);
+    *p = nullptr; *cap = 0;
+    if (cudaMalloc(p, bytes) != cudaSuccess) { *p = nullptr; return fail(DFB_ERR_OOM, "stream staging allocation failed"); }
+    *cap = bytes;
+    return DFB_OK;
+}
+// host-pointer variant (synchronous): h_spec == NULL flushes into [B][latency] rows
+extern "C" int dfb_stream_process_spec_host(dfb_stream *h, const float *h_spec, int64_t n_frames, float *h_gains, float *h_coefs,
+                                            float *h_lsnr, int8_t *h_stage) {
+    if (int rc = spec_only(h)) return rc;
+    if (h_spec && n_frames <= 0) return fail(DFB_ERR_INVALID, "bad argument");
+    DFB_CUDA(cudaSetDevice(h->m->device));
+    const bool flush = h_spec == nullptr;
+    const int64_t nf = flush ? dfb_stream_latency_frames(h) : n_frames;
+    if (nf == 0) {   // a flush without look-ahead has no output: it only closes the slots
+        flushed_all(h);
+        return DFB_OK;
+    }
+    if (!h_gains) return fail(DFB_ERR_INVALID, "bad argument");
+    const dfb_model_config &c = h->m->cfg;
+    const size_t rows = (size_t)h->B * nf, ng = rows * c.nb_erb, nc = rows * c.nb_df * 2 * c.df_order;
+    const size_t in_bytes = sizeof(float) * rows * 2 * h->st->tb.F, out_bytes = sizeof(float) * (ng + nc + rows) + rows;
+    int rc;
+    if ((!flush && (rc = stage_grow(&h->spec_stage_in, &h->spec_in_cap, in_bytes))) ||
+        (rc = stage_grow(&h->spec_stage_out, &h->spec_out_cap, out_bytes)))
+        return rc;
+    float *g = h->spec_stage_out, *cf = g + ng, *l = cf + nc;
+    int8_t *sg = (int8_t *)(l + rows);
+    cudaStream_t s = h->m->stream;
+    if (!flush) DFB_CUDA(cudaMemcpyAsync(h->spec_stage_in, h_spec, in_bytes, cudaMemcpyHostToDevice, s));
+    SpecOut so{g, h_coefs ? cf : nullptr, h_lsnr ? l : nullptr, h_stage ? sg : nullptr};
+    if ((rc = stream_step(h, h->spec_stage_in, nf, flush, nullptr, nullptr, s, &so))) return rc;
+    DFB_CUDA(cudaMemcpyAsync(h_gains, g, sizeof(float) * ng, cudaMemcpyDeviceToHost, s));
+    if (h_coefs) DFB_CUDA(cudaMemcpyAsync(h_coefs, cf, sizeof(float) * nc, cudaMemcpyDeviceToHost, s));
+    if (h_lsnr) DFB_CUDA(cudaMemcpyAsync(h_lsnr, l, sizeof(float) * rows, cudaMemcpyDeviceToHost, s));
+    if (h_stage) DFB_CUDA(cudaMemcpyAsync(h_stage, sg, rows, cudaMemcpyDeviceToHost, s));
+    DFB_CUDA(cudaStreamSynchronize(s));
+    if (flush) flushed_all(h);
+    return DFB_OK;
+}
+
+// ---- debug aids of the spectral input kernel (tests): the analysis with its ERB epilogue, and k_spec_ingest on its own
+extern "C" int dfb_debug_analysis_erb(dfb_state *st, const float *d_audio, int64_t C, int64_t T, float *d_spec, float *d_erb_db,
+                                      void *stream) {
+    if (!st || !d_audio || !d_spec || !d_erb_db || C <= 0 || T <= 0) return fail(DFB_ERR_INVALID, "bad argument");
+    if (st->fft != 960 || st->hop != 480) return fail(DFB_ERR_UNSUPPORTED, "fft_size 960 / hop_size 480 only");
+    DFB_CUDA(cudaSetDevice(st->device));
+    const int64_t Tf = T / st->hop;
+    if (Tf <= 0 || Tf > INT32_MAX) return fail(DFB_ERR_INVALID, "bad frame count");
+    AnaWindow w{0, (int)Tf, 0, (int)Tf, T, nullptr};   // the windowed kernel the streaming executor runs
+    return launch_analysis(st, d_audio, C, T, d_spec, d_erb_db, (cudaStream_t)stream, nullptr, &w);
+}
+extern "C" int dfb_debug_spec_ingest(dfb_state *st, const float *d_spec, int64_t n, const int64_t *h_src, const int64_t *h_len,
+                                     int64_t nb, int nb_df, float *d_erb_db, float *d_bins, void *stream) {
+    if (!st || !d_spec || !d_erb_db || !d_bins || n <= 0 || n > INT32_MAX || nb <= 0 || nb > 65535 || nb_df <= 0 ||
+        nb_df > st->tb.F || (!h_src) != (!h_len))
+        return fail(DFB_ERR_INVALID, "bad argument");
+    if (st->fft != 960 || st->hop != 480) return fail(DFB_ERR_UNSUPPORTED, "fft_size 960 / hop_size 480 only");
+    DFB_CUDA(cudaSetDevice(st->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    RaggedRow *d_rows = nullptr;
+    if (h_src) {
+        std::vector<RaggedRow> rows((size_t)nb);
+        for (int64_t b = 0; b < nb; b++) {
+            if (h_src[b] < 0 || h_len[b] < 0) return fail(DFB_ERR_INVALID, "bad row %lld", (long long)b);
+            rows[(size_t)b] = RaggedRow{h_src[b] * n * st->tb.F, h_len[b], 0, 0, 0};
+        }
+        DFB_CUDA(cudaMalloc(&d_rows, sizeof(RaggedRow) * rows.size()));
+        DFB_CUDA(cudaMemcpyAsync(d_rows, rows.data(), sizeof(RaggedRow) * rows.size(), cudaMemcpyHostToDevice, s));
+    }
+    const int rc = launch_spec_ingest(st, d_spec, n, d_rows, (int)nb, (int)n, d_bins, nb_df, nb_df, d_erb_db, 0, (int)n, s);
+    if (d_rows) {
+        cudaStreamSynchronize(s);
+        cudaFree(d_rows);
+    }
+    return rc;
 }

@@ -17,19 +17,30 @@ go: a call joins whenever a slot is free, and only open and closing slots are co
 several channels in as many slots, linked by the handle's ``reduce_mask`` like a ``channels`` group.  Each slot can change its own
 attenuation limit and post-filter beta between two calls (``set_atten_lim`` / ``set_post_filter_beta``), and
 ``process`` / ``flush`` return the local SNR of every output frame on request (``return_lsnr=True``).
+
+``spectral=True`` makes the handle of the Rust runtime's ``df_process_frame_raw`` (capi.rs:187-212): it takes spectrum
+frames from the caller's own filter bank and returns the network's outputs, applying nothing::
+
+    s = DfStream(model, df_state, batch=B, spectral=True)
+    out = s.process_spec(spec)           # spec: complex64 [B, n, F], e.g. DF.analysis's
+    out.gains, out.coefs, out.lsnr, out.stage
+    tail = s.flush_spec()
+
+Row j of a call that starts at input frame k carries frame k + j - ``latency_frames`` (conv_lookahead); rows that carry no
+frame are NaN with stage -1 (dfb_stream_create_spec in include/dfb200.h).
 """
 from __future__ import annotations
 
 import ctypes as C
 import math
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import numpy as np
 import torch
 from torch import Tensor
 
 from . import _lib, ragged
-from ._lib import check
+from ._lib import DFB_ERR_INVALID, DfbError, check
 from .libdf import DF
 from .model import DfNet
 
@@ -88,14 +99,57 @@ def pf_beta_arg(beta: float) -> float:
     return v
 
 
+class SpecFrames(NamedTuple):
+    """Outputs of DfStream.process_spec / flush_spec for n rows per stream, on the input's device.  gains float32 [B, n, E]
+    (the ERB mask), coefs float32 [B, n, nb_df, order, 2] (``.permute(0, 3, 1, 2, 4)`` gives DfNet.forward's layout),
+    lsnr float32 [B, n] (dB), stage int8 [B, n] (0 - 3 as tract.rs:658-672 apply_stages, -1 where the row carries no
+    frame; gains, coefs and lsnr are NaN there)."""
+    gains: Tensor
+    coefs: Tensor
+    lsnr: Tensor
+    stage: Tensor
+
+
+def spec_arg(spec, batch: int, freq_bins: int) -> Tensor:
+    """``spec`` of DfStream.process_spec, checked: a complex64 tensor (or numpy array) [batch, n >= 1, freq_bins], contiguous.
+    ValueError for a wrong rank, batch, frame count or dtype; RuntimeError with the messages of the reference's DF for
+    a wrong number of bins or a non-contiguous input."""
+    if isinstance(spec, np.ndarray):
+        spec = torch.from_numpy(spec)
+    if not isinstance(spec, Tensor):
+        raise ValueError(f"spec must be a complex64 tensor, got {type(spec).__name__}")
+    if spec.dtype != torch.complex64:
+        raise ValueError(f"spec must be complex64, got {spec.dtype}")
+    if spec.dim() != 3 or spec.shape[0] != batch or spec.shape[1] == 0:
+        raise ValueError(f"spec must have shape [{batch}, n, {freq_bins}] with n >= 1, got {list(spec.shape)}")
+    if spec.shape[2] != freq_bins:
+        raise RuntimeError(f"DF shape error: expected {freq_bins} frequency bins, got {spec.shape[2]}")
+    if not spec.is_contiguous():
+        raise RuntimeError("[df] Input array empty or not contiguous.")
+    return spec
+
+
+def need_spectral(s) -> None:
+    """DfbError (DFB_ERR_INVALID, as the C ABI) unless ``s`` is a spectral handle."""
+    if not getattr(s, "spectral", False):
+        raise DfbError(DFB_ERR_INVALID, "an audio stream takes audio: create it with spectral=True for process_spec")
+
+
 class DfStream:
     def __init__(self, model: DfNet, df_state: DF, batch: int = 1, atten_lim_db: Optional[float] = None, channels: int = 1,
-                 reduce_mask: Optional[str] = None):
+                 reduce_mask: Optional[str] = None, spectral: bool = False):
         self.model, self.df_state, self.batch = model, df_state, int(batch)
+        self.spectral = bool(spectral)
+        if self.spectral and atten_lim_db is not None:
+            raise ValueError("a spectral stream applies nothing: it takes no attenuation limit")
         h = C.c_void_p()
         lim = abs(float(atten_lim_db)) if atten_lim_db is not None else 0.0
-        check(_lib.lib().dfb_stream_create(C.byref(h), model.handle, df_state.handle, self.batch, lim))
+        if self.spectral:
+            check(_lib.lib().dfb_stream_create_spec(C.byref(h), model.handle, df_state.handle, self.batch))
+        else:
+            check(_lib.lib().dfb_stream_create(C.byref(h), model.handle, df_state.handle, self.batch, lim))
         self._h = h
+        self.freq_bins = int(df_state.fft_size()) // 2 + 1
         self.hop = int(_lib.lib().dfb_stream_frame_length(h))
         self.latency_frames = int(_lib.lib().dfb_stream_latency_frames(h))
         if channels != 1 or ragged.reduce_code(reduce_mask):
@@ -233,3 +287,42 @@ class DfStream:
         check(_lib.lib().dfb_stream_process_host_lsnr(self._h, None, 0, out.data_ptr(),
                                                       lsnr.data_ptr() if return_lsnr and lsnr.numel() else None))
         return (out, lsnr) if return_lsnr else out
+
+    # ---------------------------------------------------------------------------------------------- spectral mode ----
+    def _spec_outputs(self, n: int, device) -> SpecFrames:
+        cfg = self.model.cfg
+        B, E, Fd, O = self.batch, cfg.nb_erb, cfg.nb_df, cfg.df_order
+        return SpecFrames(torch.empty((B, n, E), dtype=torch.float32, device=device),
+                          torch.empty((B, n, Fd, O, 2), dtype=torch.float32, device=device),
+                          torch.empty((B, n), dtype=torch.float32, device=device),
+                          torch.empty((B, n), dtype=torch.int8, device=device))
+
+    @torch.no_grad()
+    def process_spec(self, spec) -> SpecFrames:
+        """spec complex64 [B, n, F] (CPU or the model's CUDA device, e.g. DF.analysis's frames) -> SpecFrames of n rows per
+        stream on the same device: row j carries frame k + j - ``latency_frames`` of a call that starts at input frame k
+        (dfb_stream_process_spec)."""
+        need_spectral(self)
+        spec = spec_arg(spec, self.batch, self.freq_bins)
+        n = spec.shape[1]
+        if spec.is_cuda:
+            if spec.device != self.model.cuda_device:
+                raise ValueError("spec lives on another device than the model")
+            out = DfStream._spec_outputs(self, n, spec.device)
+            with torch.cuda.device(spec.device):
+                check(_lib.lib().dfb_stream_process_spec(self._h, spec.data_ptr(), n, *(t.data_ptr() for t in out),
+                                                         torch.cuda.current_stream(spec.device).cuda_stream))
+            return out
+        out = DfStream._spec_outputs(self, n, "cpu")
+        check(_lib.lib().dfb_stream_process_spec_host(self._h, spec.data_ptr(), n, *(t.data_ptr() for t in out)))
+        return out
+
+    @torch.no_grad()
+    def flush_spec(self) -> SpecFrames:
+        """The last ``latency_frames`` frames of every stream (CPU), computed with zero look-ahead features; closes every
+        open slot, as ``flush``."""
+        need_spectral(self)
+        out = self._spec_outputs(self.latency_frames, "cpu")
+        ptrs = [t.data_ptr() if t.numel() else None for t in out]
+        check(_lib.lib().dfb_stream_process_spec_host(self._h, None, 0, *ptrs))
+        return out

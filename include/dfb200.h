@@ -342,6 +342,45 @@ int dfb_stream_process_lsnr(dfb_stream *s, const float *d_in, int64_t n_frames, 
 int dfb_stream_flush_lsnr(dfb_stream *s, float *d_out, float *d_lsnr, void *stream);
 int dfb_stream_process_host_lsnr(dfb_stream *s, const float *h_in, int64_t n_frames, float *h_out, float *h_lsnr);
 
+/* Spectral streaming handle (capi.rs df_process_frame_raw, DfTract::process_raw, tract.rs:441-506): the caller runs its own
+ * filter bank, passes spectrum frames in and gets the network's outputs back -- ERB gains, deep-filter coefficients, LSNR
+ * and the stage LSNR gating picks -- with the features' normalisation, the GRU, conv and norm states carried between
+ * calls.  No STFT, nothing applied: dfb_apply and the audio handle do that.  The mode is fixed at creation; a spectral
+ * handle takes only the *_spec calls below (dfb_stream_process* / flush* are DFB_ERR_INVALID, and the *_spec calls on an
+ * audio handle too), and dfb_stream_set_atten_lim / set_post_filter_beta, which are apply-stage settings, are
+ * DFB_ERR_UNSUPPORTED.  Slots, slot groups, dfb_stream_set_mask_reduce, dfb_stream_reset and the LSNR thresholds work as
+ * on audio handles (the thresholds also for DeepFilterNet2).  DeepFilterNet v1: DFB_ERR_UNSUPPORTED.
+ *   d_spec f32[B][n_frames][F][2]: complex64 rows as dfb_analysis returns them (F = fft / 2 + 1 of the state, 481).
+ *   Outputs, [B][n_frames] rows (flush: [B][latency]); every pointer except d_gains may be NULL:
+ *     d_gains f32[..][nb_erb]            the ERB mask (dfb_apply's `m` layout)
+ *     d_coefs f32[..][nb_df][2 * order]  the network's c[t][k][o * 2 + re/im] (dfb_apply's `coefs` layout; the [nb_df][order]
+ *                                        complex layout tract.rs's df() reads -- not [order][nb_df][2] as capi.rs's comment says)
+ *     d_lsnr  f32[..]                    dB
+ *     d_stage i8 [..]                    see below
+ * Alignment: row j of a call that starts at input frame k carries frame k + j - latency, latency = conv_lookahead (2 for
+ * DeepFilterNet3 and DeepFilterNet2, 0 for DeepFilterNet3_ll; dfb_stream_latency_frames returns it).  As df_process_frame
+ * (see the LSNR note above); for DeepFilterNet2 this is NOT the audio handle's latency: the outputs do not wait for the deep
+ * filter's own look-ahead.  Flush returns the last `latency` frames, computed with zero look-ahead features.
+ * Rows that carry no frame (the first `latency` rows of a handle or of a session, free slots, a closing slot past its tail):
+ * NaN gains, coefs and LSNR, stage -1.
+ * Stages (tract.rs:658-672 apply_stages on the frame's LSNR, the link group's channel 0's for a slot group; every frame is
+ * stage 1 while gating is off):
+ *   0  lsnr < min_db_thresh        gains 0, coefs 0
+ *   3  else lsnr > max_db_erb      gains 1 (unprocessed), coefs 0
+ *   2  else lsnr > max_db_df       network gains, coefs 0
+ *   1  otherwise                   network gains and coefs
+ * On a mask_only model stage 1 is stage 2.  Where the Rust runtime returns NULL for a skipped output, the values here are
+ * defined, so a caller can apply every row as it comes.  Linked channels: each member's gains are the group's reduced mask
+ * (max / mean as dfb_enhance_ragged_linked); coefs and LSNR stay per channel. */
+int dfb_stream_create_spec(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B);
+int dfb_stream_process_spec(dfb_stream *s, const float *d_spec, int64_t n_frames, float *d_gains, float *d_coefs,
+                            float *d_lsnr, int8_t *d_stage, void *stream);
+/* end of stream: closes every open slot, as dfb_stream_flush */
+int dfb_stream_flush_spec(dfb_stream *s, float *d_gains, float *d_coefs, float *d_lsnr, int8_t *d_stage, void *stream);
+/* host pointers, synchronous; h_spec == NULL flushes into [B][latency] rows (h_gains may be NULL when latency is 0) */
+int dfb_stream_process_spec_host(dfb_stream *s, const float *h_spec, int64_t n_frames, float *h_gains, float *h_coefs,
+                                 float *h_lsnr, int8_t *h_stage);
+
 /* Chunk pipeline of dfb_enhance (device_chunks) / dfb_enhance_host (host_chunks): a signal of >= 64 * chunks frames is cut
  * into at least that many time chunks; lanes = 2 overlaps the encoder phase of chunk c + 1 with the decoder phase (the
  * recurrences) of chunk c on a second set of streams and a second workspace, lanes = 1 runs them back to back.
@@ -382,6 +421,15 @@ int dfb_debug_gemm_bf16x3(const void *x_hi, const void *x_lo, int64_t ldx, const
 int dfb_debug_gl_bx(const void *x_hi, const void *x_lo, int64_t ldx, const float *w_img, const float *res, int64_t ldr,
                     float *y, int64_t ldy, void *y_hi, void *y_lo, int64_t ldp, int64_t M, int G, int Ig, int Hg, int act,
                     float oscale, float ooffset, void *stream);
+/* Debug aids for the spectral handle's input kernel.  dfb_debug_analysis_erb: the time-chunked analysis kernel on audio
+ * f32[C][T] with its ERB epilogue: spec c64[C][T / hop][F], erb_db f32[C][T / hop][E] (dB, before normalisation).
+ * dfb_debug_spec_ingest: k_spec_ingest over n frames of nb live rows, row b reading caller row h_src[b] of spec
+ * c64[..][n][F] and zeros from frame h_len[b] on (h_src / h_len HOST arrays of nb entries, or NULL: row b, n frames):
+ * erb_db f32[nb][n][E] and the first nb_df bins c64[nb][n][nb_df].  fft 960 / hop 480 states only. */
+int dfb_debug_analysis_erb(dfb_state *st, const float *d_audio, int64_t C, int64_t T, float *d_spec, float *d_erb_db,
+                           void *stream);
+int dfb_debug_spec_ingest(dfb_state *st, const float *d_spec, int64_t n, const int64_t *h_src, const int64_t *h_len, int64_t nb,
+                          int nb_df, float *d_erb_db, float *d_bins, void *stream);
 /* Debug aid for parity tests: copies the named activation of the LAST forward pass on this handle
  * (e0,e1,e2,e3,c0,c1,emb_in,emb,dec_emb,d3,d2,d1,dfc) to the host; returns the element count
  * (or a negative dfb_status).  Valid until the next call on the handle. */
