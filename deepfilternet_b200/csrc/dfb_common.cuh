@@ -200,7 +200,7 @@ struct ApplyParams {
     // spectrum is zero, but the deep filter's look-ahead taps of the last of them reach the stream's first frames, which a
     // fresh stream never synthesises before.
     const int64_t *first;
-    // linked channels (or null, specialised kernel only): stream b applies the mask of its link group links[b] reduced
+    // linked channels (or null, specialised kernel with rows only): stream b applies the mask of its link group links[b] reduced
     // over the group's streams (reduce: kReduceMax or kReduceMean, tract.rs:868-902) wherever it applies m, and LSNR
     // gating reads the LSNR of the group's first stream.  Everything else -- deep filter, DeepFilterNet3's post filter,
     // the attenuation limit, the ISTFT -- stays per stream.
@@ -212,10 +212,10 @@ struct ApplyParams {
 
 struct dfb_state;
 namespace dfb {
-// frame window of launch_analysis: frames [t_begin, t_begin + nf) of a signal of T samples per row (row pitch row_stride,
-// 0 = T) go to rows out_t0 ... of buffers holding Tbuf frames per stream.  rows (ragged batch, or null): stream b starts
-// at audio + rows[b].in_off and its samples >= rows[b].len read as zero
-struct AnaWindow { int t_begin, nf, out_t0, Tbuf; int64_t row_stride; const RaggedRow *rows = nullptr; };
+// frame window of launch_analysis: frames [t_begin, t_begin + nf) of a signal of at most T samples per row go to rows
+// out_t0 ... of buffers holding Tbuf frames per stream.  Stream b starts at audio + rows[b].in_off and its samples
+// >= rows[b].len read as zero
+struct AnaWindow { int t_begin, nf, out_t0, Tbuf; const RaggedRow *rows; };
 int launch_analysis(dfb_state *st, const float *d_audio, int64_t C, int64_t T, float *d_spec, float *d_erb_db,
                     cudaStream_t s, const float *d_init_mem = nullptr, const AnaWindow *w = nullptr);
 // Ts: frames per stream in the buffers (0 = Tf; pointers pre-offset to the first frame); *_state_out: EMA states after

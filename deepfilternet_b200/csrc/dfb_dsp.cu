@@ -147,9 +147,9 @@ __device__ __forceinline__ void warp_fft480_twptr(LoadF load, const float2 *tw_l
 // Frame window: the grid covers frames [t_begin, t_begin + nf) of every stream (time-chunked execution); their rows
 // go to out_t0 ... of spec / erb_db buffers that hold Tbuf frames per stream.  The whole-signal call is
 // (t_begin, nf, out_t0, Tbuf) = (0, Tf, 0, Tf).
-// Batch path (rows != null): stream b starts at audio + rows[b].in_off and reads zeros from sample rows[b].len on, so the
-// `pad` zeros of enhance() are implicit and no padded copy of the input is needed (RG: its own instantiation, so that the
-// table-free kernel of the streaming API and dfb_analysis* is compiled as without it).
+// Row table (RG: batch path and streaming handles): stream b starts at audio + rows[b].in_off and reads zeros from sample
+// rows[b].len on, so the `pad` zeros of enhance() are implicit and no padded copy of the input is needed (its own
+// instantiation, so that the table-free kernel of dfb_analysis* is compiled as without it).
 template <bool RG>
 __global__ void __launch_bounds__(32 * kAnaWarps, 4)
 k_analysis(const float *__restrict__ audio, int64_t T, int Tf, float2 *__restrict__ spec,
@@ -685,9 +685,9 @@ __global__ void __launch_bounds__(32 * kSynWarps) k_apply_synthesis_generic(Appl
 // bins lives in registers as a 5-deep shift register (one new look-ahead value per bin and frame instead of
 // five reloads), the band gains come from one register per lane via warp shuffles, and all global loads of
 // a frame are issued up front, coalesced (256-byte rows), before any use.
-// RG: batch path (p.rows), a separate instantiation so that the table-free kernel of the streaming API, dfb_apply and
-// dfb_model_forward_full compiles exactly as without it.
-// LINK: linked channels (p.links), likewise separate.  The mask of a frame is reduced over the link group where it is
+// RG: row table (p.rows: batch path and streaming handles), a separate instantiation so that the table-free kernel of
+// dfb_apply and dfb_model_forward_full compiles exactly as without it.
+// LINK: linked channels (p.links, with RG), likewise separate.  The mask of a frame is reduced over the link group where it is
 // loaded: lane e reads row e of each member's mask and reduces in registers, so the shared mask never reaches HBM and
 // the unlinked instantiations are untouched.
 // CTL: per-stream attenuation limit and post-filter beta (p.ctl, streaming slots), likewise separate.  Each frame picks
@@ -1301,12 +1301,11 @@ int launch_analysis(dfb_state *st, const float *d_audio, int64_t C, int64_t T, f
     if (nf <= 0) return DFB_OK;
     dim3 grid((unsigned)((nf + kAnaWarps - 1) / kAnaWarps), (unsigned)C);
     DFB_PROF("k_analysis", s);
-    const int64_t stride = w && w->row_stride ? w->row_stride : T;
-    if (w && w->rows)
-        k_analysis<true><<<grid, 32 * kAnaWarps, kAnaSmem, s>>>(d_audio, stride, (int)Tf, (float2 *)d_spec, d_erb_db, st->tb, d_init_mem,
+    if (w)
+        k_analysis<true><<<grid, 32 * kAnaWarps, kAnaSmem, s>>>(d_audio, T, (int)Tf, (float2 *)d_spec, d_erb_db, st->tb, d_init_mem,
                                                               t_begin, nf, out_t0, Tbuf, w->rows);
     else
-        k_analysis<false><<<grid, 32 * kAnaWarps, kAnaSmem, s>>>(d_audio, stride, (int)Tf, (float2 *)d_spec, d_erb_db, st->tb, d_init_mem,
+        k_analysis<false><<<grid, 32 * kAnaWarps, kAnaSmem, s>>>(d_audio, T, (int)Tf, (float2 *)d_spec, d_erb_db, st->tb, d_init_mem,
                                                                t_begin, nf, out_t0, Tbuf, nullptr);
     DFB_LAUNCH_CHECK();
     return DFB_OK;
@@ -1405,7 +1404,8 @@ int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaS
     if (p.lsnr && !(p.mode == 1 && p.order == 5 && p.nb_df == 96 && st->tb.E == 32 && p.m && p.coefs))
         return fail(DFB_ERR_UNSUPPORTED, "LSNR stage gating is built for the DeepFilterNet3 apply kernel only");
     const bool special = p.mode != 0 && p.order == 5 && p.nb_df == 96 && st->tb.E == 32 && p.m && p.coefs;
-    if (p.links && !special) return fail(DFB_ERR_UNSUPPORTED, "linked channels are built for the specialised apply kernel only");
+    if (p.links && !(special && p.rows))
+        return fail(DFB_ERR_UNSUPPORTED, "linked channels are built for the specialised row-table apply kernel only");
     if (p.links && p.reduce != kReduceMax && p.reduce != kReduceMean) return fail(DFB_ERR_INVALID, "bad mask reduction %d", p.reduce);
     if (ctl && !(special && p.rows))
         return fail(DFB_ERR_UNSUPPORTED, "per-stream settings are built for the specialised slot apply kernel only");
@@ -1415,10 +1415,8 @@ int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaS
         k_apply_synthesis<5, 3, 2, true, true, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, ctl);
     else if (ctl)
         k_apply_synthesis<5, 3, 2, true, false, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, ctl);
-    else if (p.links && p.rows)
-        k_apply_synthesis<5, 3, 2, true, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, nullptr);
     else if (p.links)
-        k_apply_synthesis<5, 3, 2, false, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, nullptr);
+        k_apply_synthesis<5, 3, 2, true, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, nullptr);
     else if (special && p.rows)
         k_apply_synthesis<5, 3, 2, true><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, nullptr);
     else if (special)

@@ -1642,15 +1642,15 @@ static size_t chunk_bytes_per_stream(const dfb_model_config &c, const dfb_state 
 
 // Where the audio of one chunk comes from and goes to.
 struct ChunkIO {
-    const float *audio; int64_t audio_T, audio_stride;  // signal the analysis reads: T samples per row (row pitch audio_stride)
+    const float *audio; int64_t audio_T;   // signal the analysis reads (rows[b].in_off / len): at most T samples per row
     int64_t audio_frame0;     // absolute frame index of the signal's first frame (0: resident whole signal; a0: streaming chunk)
     const float *init_mem;    // [B][hop] samples before audio[0] (streaming) or null (zeros)
     float *out; int64_t out_stride, out_len;
     int64_t out_sample0;      // absolute synthesis sample (frame * hop + i) that lands at out[0]
     float atten_lim;
     const float *lsnr_th;     // {min_db_thresh, max_db_erb_thresh, max_db_df_thresh} (tract.rs:658-672) or null: no gating
-    // batch (dfb_enhance*): per-stream input / output rows and frame counts (device table, streams sorted longest first),
-    // and how many of them still have frames in this chunk (a prefix); null / 0 (streaming API): all S.B streams alike
+    // per-stream input / output rows and frame counts (device table; batch: streams sorted longest first), and how many
+    // of them run in this chunk (a prefix: batch streams that still have frames, a handle's live slots)
     const RaggedRow *rows = nullptr;
     int nb = 0;
     // linked channels: each stream's link group (device table in kernel batch order) and the mask reduction, or null / 0
@@ -1667,15 +1667,15 @@ struct ChunkIO {
     int64_t lsnr_from = -1;
     float *lsnr_out = nullptr;
     // spectral handle (dfb_stream_create_spec), or null: the caller's spectrum frames replace the audio (k_spec_ingest reads
-    // rows[b].in_off / len as complex values / frames, or row b of [B][spec_frames][F]) and k_spec_emit writes the network's
-    // outputs in place of apply + synthesis
+    // rows[b].in_off / len as complex values / frames) and k_spec_emit writes the network's outputs in place of apply +
+    // synthesis
     const float *spec_in = nullptr;
     int64_t spec_frames = 0;
     const struct SpecOut *spec_out = nullptr;
 };
 
-// Outputs of a spectral call (k_spec_emit): caller row c, output row j of n_out carries frame f0 + j; slot_row (or null:
-// row c) maps caller rows to the kernel's live rows, -1 for a free slot.  Any output pointer but gains may be null.
+// Outputs of a spectral call (k_spec_emit): caller row c, output row j of n_out carries frame f0 + j; slot_row maps caller
+// rows to the kernel's live rows, -1 for a free slot.  Any output pointer but gains may be null.
 struct SpecOut {
     float *gains, *coefs, *lsnr;
     int8_t *stage;
@@ -1693,17 +1693,17 @@ constexpr const char *kSpecIngestName = "k_spec_ingest", *kSpecEmitName = "k_spe
 // k_spec_ingest replaces k_analysis: warp w of CTA (x, b) reads frame x * kIngWarps + w of live row b once, coalesced
 // (3848 B), and writes the frame's 32 ERB band energies in dB -- |X|^2 and the in-band sums exactly as k_analysis's
 // epilogue, so the same spectrum gives the same bits -- and its first Fd bins, into rows out_t0 ... of buffers holding Tbuf
-// frames per stream, where k_feat_norm reads them.  rows (or null: row b of [B][pitch][F]): row b reads from
-// in + rows[b].in_off (complex values), and zeros from frame rows[b].len on (a closing slot).
-__global__ void __launch_bounds__(32 * kIngWarps) k_spec_ingest(const float2 *__restrict__ in, int64_t pitch, const RaggedRow *__restrict__ rows,
+// frames per stream, where k_feat_norm reads them.  Row b reads from in + rows[b].in_off (complex values), and zeros from
+// frame rows[b].len on (a closing slot).
+__global__ void __launch_bounds__(32 * kIngWarps) k_spec_ingest(const float2 *__restrict__ in, const RaggedRow *__restrict__ rows,
                                                                 int nf, float2 *__restrict__ bins, int Fd, int64_t bins_pitch,
                                                                 float *__restrict__ erb_db, int out_t0, int Tbuf, DspTables tb) {
     __shared__ float s_p[kIngWarps][kSpecF + 3];
     const int b = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int t = blockIdx.x * kIngWarps + warp;
     if (t >= nf) return;
-    const bool have = !rows || t < rows[b].len;
-    const float2 *x = in + (rows ? rows[b].in_off : (int64_t)b * pitch * kSpecF) + (int64_t)t * kSpecF;
+    const bool have = t < rows[b].len;
+    const float2 *x = in + rows[b].in_off + (int64_t)t * kSpecF;
     const int64_t orow = (int64_t)b * Tbuf + out_t0 + t;
     float2 *brow = bins + orow * bins_pitch;
     float *P = s_p[warp];
@@ -1723,16 +1723,16 @@ __global__ void __launch_bounds__(32 * kIngWarps) k_spec_ingest(const float2 *__
     }
 }
 
-static int launch_spec_ingest(const dfb_state *st, const float *in, int64_t pitch, const RaggedRow *rows, int B, int nf, float *bins,
-                              int Fd, int64_t bins_pitch, float *erb_db, int out_t0, int Tbuf, cudaStream_t s) {
+static int launch_spec_ingest(const dfb_state *st, const float *in, const RaggedRow *rows, int B, int nf, float *bins, int Fd,
+                              int64_t bins_pitch, float *erb_db, int out_t0, int Tbuf, cudaStream_t s) {
     if (B <= 0 || nf <= 0) return DFB_OK;
     if (st->tb.F != kSpecF || st->tb.E > 32 * 8) return fail(DFB_ERR_UNSUPPORTED, "spectral input is built for fft_size 960");
     // timed by dfb_profile_* like the enhancement path's kernels, but outside the DFB_PROF list whose per-kernel roofline
     // model bench.py keeps: a spectral handle is not on the enhancement path (bench_stream_spec.py reports its share)
     dfb::ProfScope prof_scope__(kSpecIngestName, s);
     dim3 grid((unsigned)((nf + kIngWarps - 1) / kIngWarps), (unsigned)B);
-    k_spec_ingest<<<grid, 32 * kIngWarps, 0, s>>>((const float2 *)in, pitch, rows, nf, (float2 *)bins, Fd, bins_pitch, erb_db, out_t0,
-                                                  Tbuf, st->tb);
+    k_spec_ingest<<<grid, 32 * kIngWarps, 0, s>>>((const float2 *)in, rows, nf, (float2 *)bins, Fd, bins_pitch, erb_db, out_t0, Tbuf,
+                                                  st->tb);
     DFB_LAUNCH_CHECK();
     return DFB_OK;
 }
@@ -1747,11 +1747,10 @@ __global__ void __launch_bounds__(128) k_spec_emit(SpecOut o, const float *__res
                                                    const LinkRow *__restrict__ links, int reduce) {
     const int c = blockIdx.y, tid = threadIdx.x;
     const int64_t j = blockIdx.x, q = (int64_t)c * o.n_out + j;
-    const int r = o.slot_row ? o.slot_row[c] : c;
+    const int r = o.slot_row[c];
     int64_t t = -1;
     if (r >= 0) {
-        int te = Te;
-        if (rows) te = min(te, (int)(rows[r].Tf - w0));
+        const int te = min(Te, (int)(rows[r].Tf - w0));
         const int t0 = max(t_first, stream_first(first, r, w0));
         const int64_t tt = o.f0 + j - w0;
         if (tt >= t0 && tt < te) t = tt;
@@ -1815,20 +1814,16 @@ static int launch_spec_emit(const SpecOut &o, const float *m, const float *coefs
 }
 
 // LSNR of the frames the apply kernel emitted in this chunk, by the kernel's own emission rule: output hop j of row b
-// carries window frame t = f0 + j - w0, which was emitted when t_first <= t < Te (with rows: Te clipped at the stream's
-// end rows[b].Tf) and the stream had started (stream_first).  Frames whose DNN step ran before `from` have no LSNR.
+// carries window frame t = f0 + j - w0, which was emitted when t_first <= t < Te (Te clipped at the stream's end
+// rows[b].Tf) and the stream had started (stream_first).  Frames whose DNN step ran before `from` have no LSNR.
 __global__ void k_lsnr_out(const float *__restrict__ ll, int mcT, float *__restrict__ out, int64_t n_out, int64_t f0, int64_t w0,
                            int t_first, int Te, const RaggedRow *__restrict__ rows, const int64_t *__restrict__ first, int64_t from,
                            int hop) {
     const int b = blockIdx.y;
     const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n_out) return;
-    int64_t o = (int64_t)b * n_out;
-    int te = Te;
-    if (rows) {
-        te = min(te, (int)(rows[b].Tf - w0));
-        o = rows[b].out_off / hop;
-    }
+    const int64_t o = rows[b].out_off / hop;
+    const int te = min(Te, (int)(rows[b].Tf - w0));
     int64_t t0 = max(t_first, stream_first(first, b, w0));
     if (from - w0 > t0) t0 = from - w0;
     const int64_t t = f0 + j - w0;
@@ -1836,8 +1831,8 @@ __global__ void k_lsnr_out(const float *__restrict__ ll, int mcT, float *__restr
 }
 
 // One chunk: analyse frames [S.a1, a1n), run the DNN over [S.d1, d1n), emit audio of frames [S.e1, e1n).
-// Ragged batch (io.rows): only the first io.nb streams run; a stream whose frame count Tf_b is <= d1n ends in this chunk:
-// its features and spectrum beyond Tf_b do not exist and it emits all of its frames up to Tf_b.
+// Only the first io.nb streams run; a stream whose frame count Tf_b is <= d1n ends in this chunk: its features and
+// spectrum beyond Tf_b do not exist and it emits all of its frames up to Tf_b.
 // lane / pipelined: consecutive chunks of a batch call alternate between the model's two lanes (stream sets + arenas);
 // chunk c starts when chunk c - 1 has finished its ENCODER phase and its decoder phase waits for chunk c - 1 to finish
 // entirely, so encoder(c) overlaps decoder(c - 1).  `s` is the stream the chunk is enqueued on (the lane's main stream
@@ -1850,7 +1845,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     if (have_prev) DFB_CUDA(cudaStreamWaitEvent(s, P.ev_fork, 0));   // previous chunk: features + encoder phase done
     const dfb_model_config &c = m->cfg;
     const ChunkGeom g = chunk_geom(c);
-    const int B = io.nb > 0 ? io.nb : S.B, E = c.nb_erb, Fd = c.nb_df, O2 = 2 * c.df_order, F = st->tb.F, hop = st->hop;
+    const int B = io.nb, E = c.nb_erb, Fd = c.nb_df, O2 = 2 * c.df_order, F = st->tb.F, hop = st->hop;
     const int64_t W0 = S.d1 > kHalo ? S.d1 - kHalo : 0;
     const int Rc = (int)(S.d1 - W0), Tw = (int)(d1n - W0), Tsb = Tw + g.Lmax;
     const int n_hist = (int)(S.a1 - W0);                 // feature frames of the window that are already known
@@ -1875,9 +1870,9 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
         return rc;
     if (n_new > 0) {
         if (spectral) {   // the ERB dB and the first Fd bins of the caller's frames, where k_feat_norm reads them
-            rc = launch_spec_ingest(st, io.spec_in, io.spec_frames, io.rows, B, n_new, spec, Fd, F, fe, n_hist, Tsb, s);
+            rc = launch_spec_ingest(st, io.spec_in, io.rows, B, n_new, spec, Fd, F, fe, n_hist, Tsb, s);
         } else {
-            AnaWindow w{(int)(S.a1 - io.audio_frame0), n_new, n_hist, Tsb, io.audio_stride, io.rows};
+            AnaWindow w{(int)(S.a1 - io.audio_frame0), n_new, n_hist, Tsb, io.rows};
             rc = launch_analysis(st, io.audio, B, io.audio_T, spec, fe, s, io.init_mem, &w);
         }
         if (rc) return rc;
@@ -1920,7 +1915,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
             return rc;
     }
     // ---- apply + synthesis of frames [e0, e1n) (ragged: a stream that ends in this chunk emits up to its end)
-    else if (run_dnn && (e1n > S.e1 || (io.rows && !io.first))) {
+    else if (run_dnn && (e1n > S.e1 || !io.first)) {
         dfb::ApplyParams p{};
         p.spec = (const float2 *)spec; p.m = mm; p.coefs = cc; p.audio = io.out; p.spec_out = nullptr;
         p.out_stride = io.out_stride; p.out_len = io.out_len;
@@ -1931,8 +1926,8 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
         p.alpha = aa;
         apply_options(m, p);
         if (io.lsnr_th) { p.lsnr = ll; p.th_min = io.lsnr_th[0]; p.th_erb = io.lsnr_th[1]; p.th_df = io.lsnr_th[2]; }
-        if (io.rows) { p.rows = io.rows; p.w0 = W0; p.t_emit = p.Tf; p.first = io.first; }
-        if (io.rows && !io.first) p.Tf = Tw;   // batch: the grid covers every stream's end; slots: Te = min(end, clock)
+        p.rows = io.rows; p.w0 = W0; p.t_emit = p.Tf; p.first = io.first;
+        if (!io.first) p.Tf = Tw;   // batch: the grid covers every stream's end; slots: Te = min(end, clock)
         if (io.links) { p.links = io.links; p.reduce = io.reduce; }
         if ((rc = launch_apply_synthesis(st, p, B, s, io.ctl))) return rc;
         if (io.lsnr_out && e1n > S.e1) {
@@ -2033,7 +2028,7 @@ static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, float *d
         while (na > 1 && tfs[na - 1] <= S.d1) na--;    // (the members of a link group share Tf: they leave together)
         if (hooks && S.a1 < a1n && (rc = hooks->before(S.a1 * hop, a1n * hop, na, cs))) break;
         const int64_t e0 = S.e1;
-        ChunkIO io{d_x, Tf * hop, Tf * hop, 0, nullptr, d_out, 0, 0, delay, lim, nullptr, rows, (int)na, links, reduce};
+        ChunkIO io{d_x, Tf * hop, 0, nullptr, d_out, 0, 0, delay, lim, nullptr, rows, (int)na, links, reduce};
         if ((rc = run_chunk(m, st, S, io, a1n, d1n, e1n > S.e1 ? e1n : S.e1, cs, lane, pipelined))) break;
         if (hooks && (rc = hooks->after(e0 * hop > delay ? e0 * hop - delay : 0, S.e1 * hop - delay, d1n, na, cs))) break;
         last_lane = lane;
@@ -2433,18 +2428,13 @@ __global__ void k_slot_rows(float *__restrict__ slab, StateLayout lay, int Bs, c
     }
 }
 
-// carried analysis memory of the slot path: row b's last input hop, read where rows[b] says its input row is
+// carried analysis memory: row b's last input hop, read where rows[b] says its input row is
 __global__ void k_carry_hop(float *__restrict__ ana_mem, const float *__restrict__ in, const RaggedRow *__restrict__ rows, int64_t last,
                             int hop) {
     const int b = blockIdx.x;
     for (int i = threadIdx.x; i < hop; i += blockDim.x) ana_mem[(int64_t)b * hop + i] = in[rows[b].in_off + last + i];
 }
 
-// Frame-incremental processing with carried state: the batched counterpart of the reference's single-stream runtime
-// (libDF/src/tract.rs:509-642 `DfTract::process`, C ABI libDF/src/capi.rs:83-253 df_create / df_process_frame / df_free).
-// Every call feeds n >= 1 hops per stream and returns n hops; the output trails the input by `latency` frames
-// (max(conv_lookahead, df_lookahead), + df_lookahead for DeepFilterNet2) on top of the STFT's own fft - hop samples,
-// i.e. the concatenated output equals enhance(pad=False) of the concatenated input delayed by latency * hop samples.
 struct dfb_stream {
     dfb_model *m;
     dfb_state *st;
@@ -2456,20 +2446,20 @@ struct dfb_stream {
     bool gating = false;
     float th[3] = {-10.f, 30.f, 20.f};                 // tract.rs:180-185 defaults
     float *stage_in = nullptr, *stage_out = nullptr;   // device staging of the *_host entry point
-    size_t stage_cap = 0;
-    LinkRow *links = nullptr;                          // linked channels (dfb_stream_set_mask_reduce) or null
-    int reduce = 0;
+    size_t stage_in_cap = 0, stage_out_cap = 0;
     bool fed = false;                                  // a frame has been processed since create / reset
-    // streaming slots.  slots == false: every slot open since create / reset with frame 0 at clock 0 (the table-free path)
-    bool slots = false;
+    bool slot_ops = false;                             // a slot operation, setter or flush since create / reset
+    // streaming slots (slots_init: every slot open from frame 0 in row b = slot b)
     std::vector<int> slot_state, slot_row, row_slot;   // kSlot*; slot -> row of the active prefix (-1 free); row -> slot
     std::vector<int64_t> slot_first, slot_end;         // absolute first frame; end frame of a closing slot
     int n_act = 0;
     std::vector<int> row_src;                          // per row: its state-slab row at the last call, or -1: a fresh stream
-    // slot groups (dfb_stream_open_linked): per slot the slot of its group's channel 0 (-1 free) and the group's channel
-    // count.  A group's rows are contiguous in the active prefix, in channel order.
+    // slot groups (dfb_stream_open_linked, or the fixed channel groups of dfb_stream_set_mask_reduce): per slot the slot of
+    // its group's channel 0 (-1 free) and the group's channel count.  A group's rows are contiguous in the active prefix,
+    // in channel order.
     std::vector<int> slot_grp, slot_nch;
-    int group_reduce = 0;                              // mask reduction of the groups (dfb_stream_set_mask_reduce(s, 1, mode))
+    int group_reduce = 0;                              // mask reduction of the groups (dfb_stream_set_mask_reduce)
+    int fixed_nch = 1;                                 // channels of the fixed groups (dfb_stream_set_mask_reduce), 1: none
     bool tab_dirty = true;                             // rows / first frames / link groups to re-upload
     int64_t tab_n = -1;                                // ... for calls of this many input hops
     bool tab_linked = false;                           // the uploaded table has a linked group of more than one channel
@@ -2477,7 +2467,7 @@ struct dfb_stream {
     int64_t *d_first = nullptr;
     LinkRow *d_grp = nullptr;
     // per-slot settings (dfb_stream_set_atten_lim / _post_filter_beta).  ctl_on: a setter has run since create / reset, so
-    // the slot path passes the per-row table to the apply kernel.
+    // the per-row table goes to the apply kernel.
     bool ctl_on = false;
     std::vector<float> slot_lim, slot_beta;            // per slot: own limit (linear, 0 off) / beta, or NaN: the handle's
     std::vector<char> slot_fresh;                      // per slot: opened since the last call (no previous setting)
@@ -2491,7 +2481,7 @@ struct dfb_stream {
     size_t stage_lsnr_cap = 0;
     // spectral handle (dfb_stream_create_spec): spectrum frames in, the network's outputs out; runs the LSNR head always
     bool spectral = false;
-    int *d_slotmap = nullptr;                          // slot path: per slot its row of the active prefix, -1 free
+    int *d_slotmap = nullptr;                          // per slot its row of the active prefix, -1 free
     float *spec_stage_in = nullptr, *spec_stage_out = nullptr;   // device staging of dfb_stream_process_spec_host
     size_t spec_in_cap = 0, spec_out_cap = 0;
 };
@@ -2499,6 +2489,30 @@ struct dfb_stream {
 // the handle's default post-filter beta: the model's option (0 = off) for DeepFilterNet3; per-row beta is not used for
 // DeepFilterNet2, whose post filter acts on the ERB gains with a fixed beta
 static float default_beta(const dfb_model *m) { return (m->cfg.model_kind == 3 && m->post_filter) ? m->pf_beta : 0.f; }
+
+// The slot tables of a new or reset handle: every slot open, its stream started at frame 0 in row b = slot b, with the
+// handle's settings, and the fixed channel groups of dfb_stream_set_mask_reduce (one group per slot without them).
+// Device rows follow at the next call.
+static void slots_init(dfb_stream *h) {
+    const size_t B = (size_t)h->B;
+    h->slot_state.assign(B, kSlotOpen);
+    h->slot_row.resize(B); h->row_slot.resize(B); h->row_src.resize(B); h->slot_grp.resize(B);
+    std::iota(h->slot_row.begin(), h->slot_row.end(), 0);
+    std::iota(h->row_slot.begin(), h->row_slot.end(), 0);
+    std::iota(h->row_src.begin(), h->row_src.end(), 0);
+    for (int b = 0; b < h->B; b++) h->slot_grp[(size_t)b] = b - b % h->fixed_nch;
+    h->slot_nch.assign(B, h->fixed_nch);
+    h->slot_first.assign(B, 0);
+    h->slot_end.assign(B, kOpenEnd);
+    h->n_act = h->B;
+    h->tab_dirty = true;
+    h->slot_lim.assign(B, NAN);
+    h->slot_beta.assign(B, NAN);
+    h->slot_fresh.assign(B, 0);
+    h->slot_ctl.assign(B, SlotCtl{});
+    h->ctl_on = false;
+    h->slot_ops = false;
+}
 
 static int stream_new(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B, float atten_lim_db, bool spectral) {
     if (!out || !m || !st || B <= 0 || B > 65535) return fail(DFB_ERR_INVALID, "bad argument");
@@ -2514,9 +2528,19 @@ static int stream_new(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B, 
     if (spectral) h->lsnr_from = 0;
     size_t off[16];
     const size_t n = state_floats(m->cfg, st, (int)B, off);
-    if (cudaMalloc(&h->slab, n * sizeof(float)) != cudaSuccess) { delete h; return fail(DFB_ERR_OOM, "stream state allocation failed"); }
+    auto dev = [](auto **p, size_t bytes) {
+        if (cudaMalloc(p, bytes) == cudaSuccess) return true;
+        *p = nullptr;
+        return false;
+    };
+    if (!dev(&h->slab, n * sizeof(float)) || !dev(&h->d_rows, sizeof(RaggedRow) * B) || !dev(&h->d_first, sizeof(int64_t) * B) ||
+        !dev(&h->d_grp, sizeof(LinkRow) * B)) {
+        dfb_stream_free(h);
+        return fail(DFB_ERR_OOM, "stream state allocation failed");
+    }
     cudaMemset(h->slab, 0, n * sizeof(float));
     state_bind(h->S, h->slab, off, (int)B);
+    slots_init(h);
     h->beta_run = default_beta(m);
     *out = h;
     return DFB_OK;
@@ -2536,7 +2560,6 @@ extern "C" void dfb_stream_free(dfb_stream *h) {
     if (h->slab) cudaFree(h->slab);
     if (h->stage_in) cudaFree(h->stage_in);
     if (h->stage_out) cudaFree(h->stage_out);
-    if (h->links) cudaFree(h->links);
     if (h->d_rows) cudaFree(h->d_rows);
     if (h->d_first) cudaFree(h->d_first);
     if (h->d_grp) cudaFree(h->d_grp);
@@ -2554,37 +2577,26 @@ extern "C" int dfb_stream_reset(dfb_stream *h) {
     state_floats(h->m->cfg, h->st, h->B, off);
     state_bind(h->S, h->slab, off, h->B);
     h->fed = false;
-    h->slots = false;
-    h->ctl_on = false;
+    slots_init(h);
     h->lsnr_from = h->spectral ? 0 : -1;
     return DFB_OK;
 }
 
 // Linked channels on a stream handle: streams g * channels + c (c < channels) are the channels of recording g and share one
-// ERB mask (reduce_mask max / mean, as dfb_enhance_ragged_linked).  Only before the first frame of a new or reset handle:
-// the frame re-synthesised for the overlap-add tail at the next call would otherwise mix the two settings.  channels = 1
-// records the reduction of the slot groups opened later (dfb_stream_open_linked).
+// ERB mask (reduce_mask max / mean, as dfb_enhance_ragged_linked): fixed slot groups, which survive a reset and take no
+// slot operations.  Only before the first frame of a new or reset handle: the frame re-synthesised for the overlap-add
+// tail at the next call would otherwise mix the two settings.  channels = 1 records the reduction of the slot groups
+// opened later (dfb_stream_open_linked).
 extern "C" int dfb_stream_set_mask_reduce(dfb_stream *h, int channels, int reduce_mask) {
     if (!h) return fail(DFB_ERR_INVALID, "null stream");
     if (h->fed) return fail(DFB_ERR_INVALID, "mask reduction set after the first frame: reset the stream first");
-    if (h->slots) return fail(DFB_ERR_UNSUPPORTED, "mask reduction set after slot operations: reset the stream first");
+    if (h->slot_ops) return fail(DFB_ERR_UNSUPPORTED, "mask reduction set after slot operations: reset the stream first");
     if (reduce_mask != kReduceNone && reduce_mask != kReduceMax && reduce_mask != kReduceMean)
         return fail(DFB_ERR_INVALID, "reduce_mask %d is not 0 (none), 1 (max) or 2 (mean)", reduce_mask);
     if (channels <= 0 || h->B % channels) return fail(DFB_ERR_INVALID, "%d streams are not groups of %d channels", h->B, channels);
-    DFB_CUDA(cudaSetDevice(h->m->device));
-    if (h->links) cudaFree(h->links);
-    h->links = nullptr;
-    h->reduce = 0;
-    h->group_reduce = channels == 1 ? reduce_mask : kReduceNone;
-    if (reduce_mask == kReduceNone || channels == 1) return DFB_OK;
-    std::vector<LinkRow> t((size_t)h->B);
-    for (int b = 0; b < h->B; b++) t[(size_t)b] = LinkRow{b - b % channels, channels};
-    if (cudaMalloc(&h->links, sizeof(LinkRow) * t.size()) != cudaSuccess) {
-        h->links = nullptr;
-        return fail(DFB_ERR_OOM, "link table allocation failed");
-    }
-    DFB_CUDA(cudaMemcpy(h->links, t.data(), sizeof(LinkRow) * t.size(), cudaMemcpyHostToDevice));
-    h->reduce = reduce_mask;
+    h->group_reduce = reduce_mask;
+    h->fixed_nch = reduce_mask == kReduceNone ? 1 : channels;
+    slots_init(h);
     return DFB_OK;
 }
 
@@ -2609,40 +2621,7 @@ extern "C" int64_t dfb_stream_latency_frames(const dfb_stream *h) {
 }
 extern "C" int64_t dfb_stream_frame_length(const dfb_stream *h) { return h ? h->st->hop : -1; }  // capi.rs df_get_frame_length
 
-// ---- streaming slots: host bookkeeping.  Device rows follow at the next call (slots_step moves them first, by row_src).
-// Leaves the slot-free path: every slot is open, row b = slot b, its stream started at frame 0.
-static int slots_enable(dfb_stream *h) {
-    if (h->slots) return DFB_OK;
-    const size_t B = (size_t)h->B;
-    if (!h->d_grp) {
-        DFB_CUDA(cudaSetDevice(h->m->device));
-        if ((!h->d_rows && cudaMalloc(&h->d_rows, sizeof(RaggedRow) * B) != cudaSuccess) ||
-            (!h->d_first && cudaMalloc(&h->d_first, sizeof(int64_t) * B) != cudaSuccess) ||
-            cudaMalloc(&h->d_grp, sizeof(LinkRow) * B) != cudaSuccess) {
-            h->d_grp = nullptr;
-            return fail(DFB_ERR_OOM, "slot table allocation failed");
-        }
-    }
-    h->slot_state.assign(B, kSlotOpen);
-    h->slot_row.resize(B); h->row_slot.resize(B); h->row_src.resize(B); h->slot_grp.resize(B);
-    std::iota(h->slot_row.begin(), h->slot_row.end(), 0);
-    std::iota(h->row_slot.begin(), h->row_slot.end(), 0);
-    std::iota(h->row_src.begin(), h->row_src.end(), 0);
-    std::iota(h->slot_grp.begin(), h->slot_grp.end(), 0);
-    h->slot_nch.assign(B, 1);
-    h->slot_first.assign(B, 0);
-    h->slot_end.assign(B, kOpenEnd);
-    h->n_act = h->B;
-    h->tab_dirty = true;
-    h->slot_lim.assign(B, NAN);
-    h->slot_beta.assign(B, NAN);
-    h->slot_fresh.assign(B, 0);
-    h->slot_ctl.assign(B, SlotCtl{});
-    h->ctl_on = false;
-    h->slots = true;
-    return DFB_OK;
-}
-
+// ---- streaming slots: host bookkeeping.  Device rows follow at the next call (stream_step moves them first, by row_src).
 // the slot becomes free; its row stays in the active prefix until rows_compact
 static void slot_release(dfb_stream *h, int slot) {
     h->slot_row[(size_t)slot] = -1;
@@ -2682,16 +2661,19 @@ static void slot_close(dfb_stream *h, int slot) {
     h->tab_dirty = true;
 }
 
+// After a flush every stream has ended: all slots are free once their tails are out.  Without look-ahead a flush computes
+// nothing and only closes the slots.
 static void slots_close_all(dfb_stream *h) {
     for (int b = 0; b < h->B; b++) slot_close(h, b);
     slots_retire(h, h->S.a1 - dfb_stream_latency_frames(h));
+    h->slot_ops = true;
 }
 
 // Valid slot indices, each listed once; a live group of more than one channel is listed with all of its members or not at
 // all (groups open, close and take settings as a unit).
 static int slot_list_check(const dfb_stream *h, const int64_t *slots, int64_t n) {
     if (!h || n < 0 || (n > 0 && !slots)) return fail(DFB_ERR_INVALID, "bad argument");
-    if (h->links) return fail(DFB_ERR_UNSUPPORTED, "slot operations on a handle with linked channels");
+    if (h->fixed_nch > 1) return fail(DFB_ERR_UNSUPPORTED, "slot operations on a handle with linked channels");
     std::vector<int> seen((size_t)h->B, 0);
     for (int64_t i = 0; i < n; i++) {
         const int64_t b = slots[i];
@@ -2699,7 +2681,6 @@ static int slot_list_check(const dfb_stream *h, const int64_t *slots, int64_t n)
         if (seen[(size_t)b]) return fail(DFB_ERR_INVALID, "slot %lld listed twice", (long long)b);
         seen[(size_t)b] = 1;
     }
-    if (!h->slots) return DFB_OK;
     std::vector<int> listed((size_t)h->B, 0);   // per group (by its channel-0 slot): members listed
     for (int64_t i = 0; i < n; i++)
         if (h->slot_grp[(size_t)slots[i]] >= 0) listed[(size_t)h->slot_grp[(size_t)slots[i]]]++;
@@ -2714,7 +2695,8 @@ static int slot_list_check(const dfb_stream *h, const int64_t *slots, int64_t n)
 
 static int slot_list(dfb_stream *h, const int64_t *slots, int64_t n) {
     if (int rc = slot_list_check(h, slots, n)) return rc;
-    return slots_enable(h);
+    h->slot_ops = true;
+    return DFB_OK;
 }
 
 // Opens one group per `nch` consecutive listed slots (channel c of a group in its c-th slot), each a fresh stream in rows
@@ -2771,10 +2753,9 @@ static int ctl_set(dfb_stream *h, const int64_t *slots, int64_t n, bool beta, fl
     if (std::isnan(v) || (beta && !(v >= 0.f && std::isfinite(v))))
         return fail(DFB_ERR_INVALID, beta ? "post-filter beta must be finite and >= 0" : "attenuation limit is NaN");
     for (int64_t i = 0; i < n; i++)
-        if (h->slots && h->slot_state[(size_t)slots[i]] == kSlotFree)
-            return fail(DFB_ERR_INVALID, "slot %lld is free", (long long)slots[i]);
+        if (h->slot_state[(size_t)slots[i]] == kSlotFree) return fail(DFB_ERR_INVALID, "slot %lld is free", (long long)slots[i]);
     if (n == 0) return DFB_OK;
-    if (int rc = slots_enable(h)) return rc;
+    h->slot_ops = true;
     if (!h->ctl_on) {
         if (!h->d_ctl) {
             DFB_CUDA(cudaSetDevice(h->m->device));
@@ -2826,13 +2807,13 @@ static int ctl_rows(dfb_stream *h, int64_t f0, cudaStream_t s) {
 
 extern "C" int dfb_stream_slot_states(const dfb_stream *h, int32_t *h_states) {
     if (!h || !h_states) return fail(DFB_ERR_INVALID, "null argument");
-    for (int b = 0; b < h->B; b++) h_states[b] = h->slots ? h->slot_state[(size_t)b] : kSlotOpen;
+    for (int b = 0; b < h->B; b++) h_states[b] = h->slot_state[(size_t)b];
     return DFB_OK;
 }
 
 extern "C" int dfb_stream_slot_groups(const dfb_stream *h, int64_t *h_first) {
     if (!h || !h_first) return fail(DFB_ERR_INVALID, "null argument");
-    for (int b = 0; b < h->B; b++) h_first[b] = h->slots ? h->slot_grp[(size_t)b] : b;
+    for (int b = 0; b < h->B; b++) h_first[b] = h->slot_grp[(size_t)b];
     return DFB_OK;
 }
 
@@ -2868,11 +2849,10 @@ static int slots_move_rows(dfb_stream *h, cudaStream_t s) {
     return DFB_OK;
 }
 
-// The spectral side of a call's ChunkIO: input frames [B][n][F] (slot path: where the row table says), outputs to `so`
-// with n_out rows per caller row from frame f0 on, the LSNR head always on
-static void spec_io(const dfb_stream *h, ChunkIO &io, SpecOut *so, const float *d_in, int64_t n, int64_t n_out, int64_t f0,
-                    const int *slotmap) {
-    so->Bc = h->B; so->n_out = n_out; so->f0 = f0; so->slot_row = slotmap;
+// The spectral side of a call's ChunkIO: input frames [B][n][F] where the row table says, outputs to `so` with n_out rows
+// per caller row from frame f0 on, the LSNR head always on
+static void spec_io(const dfb_stream *h, ChunkIO &io, SpecOut *so, const float *d_in, int64_t n, int64_t n_out, int64_t f0) {
+    so->Bc = h->B; so->n_out = n_out; so->f0 = f0; so->slot_row = h->d_slotmap;
     so->gating = h->gating; so->th[0] = h->th[0]; so->th[1] = h->th[1]; so->th[2] = h->th[2];
     so->mask_only = h->m->mask_only;
     io.spec_in = d_in; io.spec_frames = n; io.spec_out = so;
@@ -2887,9 +2867,11 @@ static int spec_fill_empty(const SpecOut &so, const dfb_model_config &c, int64_t
     return DFB_OK;
 }
 
-// Slot path of one call: rows [0, n_act) of the slab, the row table for calls of n input hops, output rows zero first.
+// One call: rows [0, n_act) of the slab, the row table for calls of n input hops.
 // Spectral handle (so != null): d_in is [B][n][F] complex, the outputs go to so's buffers, d_out / d_lsnr are null.
-static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s, SpecOut *so) {
+static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s,
+                       SpecOut *so = nullptr) {
+    if (d_lsnr && h->lsnr_from < 0) h->lsnr_from = h->S.d1;   // from now on every call runs the LSNR head
     dfb_model *m = h->m;
     dfb_state *st = h->st;
     StreamState &S = h->S;
@@ -2935,9 +2917,16 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
         h->tab_n = n;
         h->tab_linked = linked;
     }
-    if (n_out > 0 && !so) DFB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * B * n_out * hop, s));   // free slots; frames outside a stream
-    if (d_lsnr && n_out > 0) DFB_CUDA(cudaMemsetAsync(d_lsnr, 0xff, sizeof(float) * B * n_out, s));   // NaN: hops without a frame
     const int64_t f0 = a0 - Ltot;   // output hop j carries frame a0 - Ltot + j (flush: a1 = a0)
+    // The apply kernel writes every hop that carries a frame of its row.  The others are zero: those of free slots, of
+    // frames before 0, before a row's first frame or from a closing row's end on, and all of them when no frame is emitted.
+    bool gaps = h->n_act < B || f0 < 0 || e1n <= S.e1;
+    for (int r = 0; r < h->n_act && !gaps; r++) {
+        const size_t b = (size_t)h->row_slot[(size_t)r];
+        gaps = h->slot_first[b] > f0 || h->slot_end[b] < f0 + n_out;
+    }
+    if (gaps && n_out > 0 && !so) DFB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * B * n_out * hop, s));
+    if (d_lsnr && n_out > 0) DFB_CUDA(cudaMemsetAsync(d_lsnr, 0xff, sizeof(float) * B * n_out, s));   // NaN: hops without a frame
     if (h->ctl_on && (rc = ctl_rows(h, f0, s))) return rc;
     h->beta_run = default_beta(m);
     h->fed = true;
@@ -2950,10 +2939,10 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
         slots_retire(h, flush ? a1n : a1n - Ltot);
         return DFB_OK;
     }
-    ChunkIO io{so ? nullptr : d_in, n * hop, n * hop, a0, nullptr, d_out, n_out * hop, n_out * hop, f0 * hop, h->lim,
+    ChunkIO io{so ? nullptr : d_in, n * hop, a0, nullptr, d_out, n_out * hop, n_out * hop, f0 * hop, h->lim,
                h->gating && !so ? h->th : nullptr, h->d_rows, h->n_act};
     io.first = h->d_first;
-    if (so) spec_io(h, io, so, d_in, n, n_out, f0, h->d_slotmap);
+    if (so) spec_io(h, io, so, d_in, n, n_out, f0);
     if (h->tab_linked) { io.links = h->d_grp; io.reduce = h->group_reduce; }
     if (h->ctl_on) io.ctl = h->d_ctl;
     io.lsnr_from = h->lsnr_from;
@@ -2975,63 +2964,6 @@ static int slots_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
     return DFB_OK;
 }
 
-static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s,
-                       SpecOut *so = nullptr) {
-    if (d_lsnr && h->lsnr_from < 0) h->lsnr_from = h->S.d1;   // from now on every call runs the LSNR head
-    if (h->slots) return slots_step(h, d_in, n, flush, d_out, d_lsnr, s, so);
-    dfb_model *m = h->m;
-    dfb_state *st = h->st;
-    StreamState &S = h->S;
-    const ChunkGeom g = chunk_geom(m->cfg);
-    const int hop = st->hop, B = h->B;
-    const int64_t Ltot = dfb_stream_latency_frames(h);
-    const int64_t lag = so ? 0 : g.lag, la = Ltot - lag;
-    const int64_t n_out = flush ? Ltot : n;
-    const int64_t a0 = S.a1, a1n = a0 + (flush ? 0 : n);
-    int64_t d1n = flush ? a1n : a1n - la, e1n = flush ? a1n : d1n - lag;
-    if (d1n < S.d1) d1n = S.d1;
-    if (e1n < S.e1) e1n = S.e1;
-    // the window of this call: halo + new DNN frames (+ look-ahead)
-    const int64_t W0 = S.d1 > kHalo ? S.d1 - kHalo : 0;
-    const int Tw = (int)(d1n - W0);
-    int rc = m->arena.reserve(chunk_bytes_per_stream(m->cfg, st, Tw + 1) * (size_t)B + (2 << 20));
-    if (rc) return rc;
-    // output slot j (hop j of d_out) carries frame a0 - Ltot + j (flush: a1 - Ltot + j); frames < 0 are silence
-    const int64_t f0 = (flush ? S.a1 : a0) - Ltot;
-    if (!so && (f0 < 0 || e1n <= S.e1)) DFB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * B * n_out * hop, s));
-    if (d_lsnr && n_out > 0) DFB_CUDA(cudaMemsetAsync(d_lsnr, 0xff, sizeof(float) * B * n_out, s));   // NaN: hops without a frame
-    ChunkIO io{so ? nullptr : d_in, (flush ? 0 : n) * hop, (flush ? 0 : n) * hop, a0, S.started ? S.ana_mem : nullptr, d_out, n_out * hop,
-               n_out * hop, f0 * hop, h->lim, h->gating && !so ? h->th : nullptr};
-    io.links = h->links;
-    io.reduce = h->reduce;
-    io.lsnr_from = h->lsnr_from;
-    io.lsnr_out = d_lsnr;
-    if (so) spec_io(h, io, so, d_in, n, n_out, f0, nullptr);
-    h->beta_run = default_beta(m);
-    h->fed = true;
-    if (!flush && a1n > a0 && !so) {
-        // zero analysis memory before the very first frame
-        if (!S.started) DFB_CUDA(cudaMemsetAsync(S.ana_mem, 0, sizeof(float) * B * hop, s));
-        io.init_mem = S.ana_mem;
-    }
-    if ((rc = run_chunk(m, st, S, io, a1n, d1n, e1n, s))) return rc;
-    if (!flush && !so)  // carried analysis memory: the last hop of this call's input
-        DFB_CUDA(cudaMemcpy2DAsync(S.ana_mem, sizeof(float) * hop, d_in + (n - 1) * hop, sizeof(float) * n * hop, sizeof(float) * hop, B,
-                                   cudaMemcpyDeviceToDevice, s));
-    m->arena.reset();
-    return DFB_OK;
-}
-
-// After a flush every stream has ended: all slots are free (linked handles, which have no slots, stay as they were).  Without
-// look-ahead a flush computes nothing and only closes the slots.
-static void flushed_all(dfb_stream *h) {
-    if (h->links) return;
-    if (h->slots) { slots_close_all(h); return; }
-    if (slots_enable(h)) return;
-    for (int b = 0; b < h->B; b++) slot_release(h, b);
-    rows_compact(h);
-}
-
 // d_in [B][n_frames * hop] -> d_out [B][n_frames * hop] (device pointers, asynchronous on `stream`); d_lsnr (or null)
 // [B][n_frames]: the LSNR of the frame each output hop carries, NaN where it carries none
 static int audio_only(const dfb_stream *h) {
@@ -3048,19 +2980,27 @@ extern "C" int dfb_stream_process(dfb_stream *h, const float *d_in, int64_t n_fr
 }
 
 // End of the stream: the `latency` frames still in flight, computed with zero look-ahead exactly like the end of a
-// batch enhance(); d_out [B][latency * hop].  Closes every open slot; on the slot-free path the stream must be reset before
-// it is fed again.  d_lsnr (or null) [B][latency]: the LSNR of the tail frames.
+// batch enhance(); d_out [B][latency * hop].  Closes every open slot.  d_lsnr (or null) [B][latency]: the LSNR of the tail
+// frames.
 extern "C" int dfb_stream_flush_lsnr(dfb_stream *h, float *d_out, float *d_lsnr, void *stream) {
     if (int rc = audio_only(h)) return rc;
     if (!h || !d_out) return fail(DFB_ERR_INVALID, "bad argument");
     DFB_CUDA(cudaSetDevice(h->m->device));
     int rc = DFB_OK;
     if (dfb_stream_latency_frames(h) > 0) rc = stream_step(h, nullptr, 0, true, d_out, d_lsnr, (cudaStream_t)stream);
-    if (!rc) flushed_all(h);
+    if (!rc) slots_close_all(h);
     return rc;
 }
 extern "C" int dfb_stream_flush(dfb_stream *h, float *d_out, void *stream) { return dfb_stream_flush_lsnr(h, d_out, nullptr, stream); }
 
+static int stage_grow(float **p, size_t *cap, size_t bytes) {
+    if (bytes <= *cap) return DFB_OK;
+    if (*p) cudaFree(*p);
+    *p = nullptr; *cap = 0;
+    if (cudaMalloc(p, bytes) != cudaSuccess) { *p = nullptr; return fail(DFB_ERR_OOM, "stream staging allocation failed"); }
+    *cap = bytes;
+    return DFB_OK;
+}
 // host-pointer variant (synchronous): h_in / h_out [B][n_frames * hop]; h_in == NULL flushes into h_out [B][latency * hop];
 // h_lsnr (or null) [B][n_frames] / [B][latency] as dfb_stream_process_lsnr
 extern "C" int dfb_stream_process_host_lsnr(dfb_stream *h, const float *h_in, int64_t n_frames, float *h_out, float *h_lsnr) {
@@ -3070,34 +3010,22 @@ extern "C" int dfb_stream_process_host_lsnr(dfb_stream *h, const float *h_in, in
     const bool flush = h_in == nullptr;
     const int64_t nf = flush ? dfb_stream_latency_frames(h) : n_frames;
     if (nf == 0) {   // a flush without look-ahead has no output: it only closes the slots
-        flushed_all(h);
+        slots_close_all(h);
         return DFB_OK;
     }
     if (!h_out) return fail(DFB_ERR_INVALID, "bad argument");
-    const size_t bytes = sizeof(float) * (size_t)h->B * nf * h->st->hop;
-    if (bytes > h->stage_cap) {
-        if (h->stage_in) cudaFree(h->stage_in);
-        if (h->stage_out) cudaFree(h->stage_out);
-        h->stage_in = h->stage_out = nullptr; h->stage_cap = 0;
-        if (cudaMalloc(&h->stage_in, bytes) != cudaSuccess || cudaMalloc(&h->stage_out, bytes) != cudaSuccess)
-            return fail(DFB_ERR_OOM, "stream staging allocation failed");
-        h->stage_cap = bytes;
-    }
-    const size_t lbytes = sizeof(float) * (size_t)h->B * nf;
-    if (h_lsnr && lbytes > h->stage_lsnr_cap) {
-        if (h->stage_lsnr) cudaFree(h->stage_lsnr);
-        h->stage_lsnr = nullptr; h->stage_lsnr_cap = 0;
-        if (cudaMalloc(&h->stage_lsnr, lbytes) != cudaSuccess) return fail(DFB_ERR_OOM, "stream staging allocation failed");
-        h->stage_lsnr_cap = lbytes;
-    }
+    const size_t bytes = sizeof(float) * (size_t)h->B * nf * h->st->hop, lbytes = sizeof(float) * (size_t)h->B * nf;
+    int rc;
+    if ((!flush && (rc = stage_grow(&h->stage_in, &h->stage_in_cap, bytes))) || (rc = stage_grow(&h->stage_out, &h->stage_out_cap, bytes)) ||
+        (h_lsnr && (rc = stage_grow(&h->stage_lsnr, &h->stage_lsnr_cap, lbytes))))
+        return rc;
     cudaStream_t s = h->m->stream;
     if (!flush) DFB_CUDA(cudaMemcpyAsync(h->stage_in, h_in, bytes, cudaMemcpyHostToDevice, s));
-    int rc = stream_step(h, h->stage_in, nf, flush, h->stage_out, h_lsnr ? h->stage_lsnr : nullptr, s);
-    if (rc) return rc;
+    if ((rc = stream_step(h, h->stage_in, nf, flush, h->stage_out, h_lsnr ? h->stage_lsnr : nullptr, s))) return rc;
     DFB_CUDA(cudaMemcpyAsync(h_out, h->stage_out, bytes, cudaMemcpyDeviceToHost, s));
     if (h_lsnr) DFB_CUDA(cudaMemcpyAsync(h_lsnr, h->stage_lsnr, lbytes, cudaMemcpyDeviceToHost, s));
     DFB_CUDA(cudaStreamSynchronize(s));
-    if (flush) flushed_all(h);
+    if (flush) slots_close_all(h);
     return DFB_OK;
 }
 extern "C" int dfb_stream_process_host(dfb_stream *h, const float *h_in, int64_t n_frames, float *h_out) {
@@ -3127,16 +3055,8 @@ extern "C" int dfb_stream_flush_spec(dfb_stream *h, float *d_gains, float *d_coe
     int rc = DFB_OK;
     SpecOut so{d_gains, d_coefs, d_lsnr, d_stage};
     if (L > 0) rc = stream_step(h, nullptr, 0, true, nullptr, nullptr, (cudaStream_t)stream, &so);
-    if (!rc) flushed_all(h);
+    if (!rc) slots_close_all(h);
     return rc;
-}
-static int stage_grow(float **p, size_t *cap, size_t bytes) {
-    if (bytes <= *cap) return DFB_OK;
-    if (*p) cudaFree(*p);
-    *p = nullptr; *cap = 0;
-    if (cudaMalloc(p, bytes) != cudaSuccess) { *p = nullptr; return fail(DFB_ERR_OOM, "stream staging allocation failed"); }
-    *cap = bytes;
-    return DFB_OK;
 }
 // host-pointer variant (synchronous): h_spec == NULL flushes into [B][latency] rows
 extern "C" int dfb_stream_process_spec_host(dfb_stream *h, const float *h_spec, int64_t n_frames, float *h_gains, float *h_coefs,
@@ -3147,7 +3067,7 @@ extern "C" int dfb_stream_process_spec_host(dfb_stream *h, const float *h_spec, 
     const bool flush = h_spec == nullptr;
     const int64_t nf = flush ? dfb_stream_latency_frames(h) : n_frames;
     if (nf == 0) {   // a flush without look-ahead has no output: it only closes the slots
-        flushed_all(h);
+        slots_close_all(h);
         return DFB_OK;
     }
     if (!h_gains) return fail(DFB_ERR_INVALID, "bad argument");
@@ -3169,20 +3089,36 @@ extern "C" int dfb_stream_process_spec_host(dfb_stream *h, const float *h_spec, 
     if (h_lsnr) DFB_CUDA(cudaMemcpyAsync(h_lsnr, l, sizeof(float) * rows, cudaMemcpyDeviceToHost, s));
     if (h_stage) DFB_CUDA(cudaMemcpyAsync(h_stage, sg, rows, cudaMemcpyDeviceToHost, s));
     DFB_CUDA(cudaStreamSynchronize(s));
-    if (flush) flushed_all(h);
+    if (flush) slots_close_all(h);
     return DFB_OK;
 }
 
-// ---- debug aids of the spectral input kernel (tests): the analysis with its ERB epilogue, and k_spec_ingest on its own
+// ---- debug aids of the spectral input kernel (tests): the analysis with its ERB epilogue, and k_spec_ingest on its own.
+// Both run the row-table kernels the streaming executor runs, the table on the device until the launch has run.
+static int with_rows(const std::vector<RaggedRow> &rows, cudaStream_t s, const std::function<int(const RaggedRow *)> &launch) {
+    RaggedRow *d_rows = nullptr;
+    DFB_CUDA(cudaMalloc(&d_rows, sizeof(RaggedRow) * rows.size()));
+    const int rc = cudaMemcpyAsync(d_rows, rows.data(), sizeof(RaggedRow) * rows.size(), cudaMemcpyHostToDevice, s) == cudaSuccess
+                       ? launch(d_rows)
+                       : fail(DFB_ERR_CUDA, "row table upload failed");
+    cudaStreamSynchronize(s);
+    cudaFree(d_rows);
+    return rc;
+}
 extern "C" int dfb_debug_analysis_erb(dfb_state *st, const float *d_audio, int64_t C, int64_t T, float *d_spec, float *d_erb_db,
                                       void *stream) {
-    if (!st || !d_audio || !d_spec || !d_erb_db || C <= 0 || T <= 0) return fail(DFB_ERR_INVALID, "bad argument");
+    if (!st || !d_audio || !d_spec || !d_erb_db || C <= 0 || C > 65535 || T <= 0) return fail(DFB_ERR_INVALID, "bad argument");
     if (st->fft != 960 || st->hop != 480) return fail(DFB_ERR_UNSUPPORTED, "fft_size 960 / hop_size 480 only");
     DFB_CUDA(cudaSetDevice(st->device));
     const int64_t Tf = T / st->hop;
     if (Tf <= 0 || Tf > INT32_MAX) return fail(DFB_ERR_INVALID, "bad frame count");
-    AnaWindow w{0, (int)Tf, 0, (int)Tf, T, nullptr};   // the windowed kernel the streaming executor runs
-    return launch_analysis(st, d_audio, C, T, d_spec, d_erb_db, (cudaStream_t)stream, nullptr, &w);
+    std::vector<RaggedRow> rows((size_t)C);
+    for (int64_t b = 0; b < C; b++) rows[(size_t)b] = RaggedRow{b * T, T, 0, 0, 0};
+    cudaStream_t s = (cudaStream_t)stream;
+    return with_rows(rows, s, [&](const RaggedRow *d_rows) {
+        AnaWindow w{0, (int)Tf, 0, (int)Tf, d_rows};
+        return launch_analysis(st, d_audio, C, T, d_spec, d_erb_db, s, nullptr, &w);
+    });
 }
 extern "C" int dfb_debug_spec_ingest(dfb_state *st, const float *d_spec, int64_t n, const int64_t *h_src, const int64_t *h_len,
                                      int64_t nb, int nb_df, float *d_erb_db, float *d_bins, void *stream) {
@@ -3191,21 +3127,14 @@ extern "C" int dfb_debug_spec_ingest(dfb_state *st, const float *d_spec, int64_t
         return fail(DFB_ERR_INVALID, "bad argument");
     if (st->fft != 960 || st->hop != 480) return fail(DFB_ERR_UNSUPPORTED, "fft_size 960 / hop_size 480 only");
     DFB_CUDA(cudaSetDevice(st->device));
+    std::vector<RaggedRow> rows((size_t)nb);
+    for (int64_t b = 0; b < nb; b++) {
+        const int64_t src = h_src ? h_src[b] : b, len = h_len ? h_len[b] : n;
+        if (src < 0 || len < 0) return fail(DFB_ERR_INVALID, "bad row %lld", (long long)b);
+        rows[(size_t)b] = RaggedRow{src * n * st->tb.F, len, 0, 0, 0};
+    }
     cudaStream_t s = (cudaStream_t)stream;
-    RaggedRow *d_rows = nullptr;
-    if (h_src) {
-        std::vector<RaggedRow> rows((size_t)nb);
-        for (int64_t b = 0; b < nb; b++) {
-            if (h_src[b] < 0 || h_len[b] < 0) return fail(DFB_ERR_INVALID, "bad row %lld", (long long)b);
-            rows[(size_t)b] = RaggedRow{h_src[b] * n * st->tb.F, h_len[b], 0, 0, 0};
-        }
-        DFB_CUDA(cudaMalloc(&d_rows, sizeof(RaggedRow) * rows.size()));
-        DFB_CUDA(cudaMemcpyAsync(d_rows, rows.data(), sizeof(RaggedRow) * rows.size(), cudaMemcpyHostToDevice, s));
-    }
-    const int rc = launch_spec_ingest(st, d_spec, n, d_rows, (int)nb, (int)n, d_bins, nb_df, nb_df, d_erb_db, 0, (int)n, s);
-    if (d_rows) {
-        cudaStreamSynchronize(s);
-        cudaFree(d_rows);
-    }
-    return rc;
+    return with_rows(rows, s, [&](const RaggedRow *d_rows) {
+        return launch_spec_ingest(st, d_spec, d_rows, (int)nb, (int)n, d_bins, nb_df, nb_df, d_erb_db, 0, (int)n, s);
+    });
 }

@@ -280,8 +280,8 @@ int dfb_stream_process_host(dfb_stream *s, const float *h_in, int64_t n_frames, 
  * Row b of process / flush is slot b.  Every session's output equals a single-stream handle fed the same audio in the
  * same call sizes and then flushed.  Only open and closing slots are computed, so the cost of a call follows the number
  * of live streams, not B.  Fixed channel groups (dfb_stream_set_mask_reduce with channels > 1) and slots do not combine:
- * every slot operation on such a handle is DFB_ERR_UNSUPPORTED; slot groups (below) are the slot path's linked channels.
- * The handle's clock counts frames since create / reset; slot operations need it below 2^31 - 2 frames (248 days). */
+ * every slot operation on such a handle is DFB_ERR_UNSUPPORTED; slot groups (below) are linked channels that take slot
+ * operations.  The handle's clock counts frames since create / reset; calls need it below 2^31 - 2 frames (248 days). */
 int dfb_stream_open_slots(dfb_stream *s, const int64_t *slots, int64_t n);
 int dfb_stream_close_slots(dfb_stream *s, const int64_t *slots, int64_t n);
 /* h_states i32[B] (host): 0 free, 1 open, 2 closing */
@@ -319,9 +319,7 @@ int dfb_stream_slot_groups(const dfb_stream *s, int64_t *h_first);
  * When a change takes effect: a setting made between two calls applies to every frame whose output starts in the next
  * process / flush call.  Output hop j of that call is the head of frame f0 + j plus the overlap-add tail of frame
  * f0 + j - 1, so hop 0 is the new setting's head of frame f0 plus the previous setting's tail of frame f0 - 1, as in the
- * Rust runtime, whose synthesis memory was computed in the previous call.
- * A handle runs as before until a setter is first called; setters move it onto the slot path (every slot open, as after
- * dfb_stream_open_slots with no slots). */
+ * Rust runtime, whose synthesis memory was computed in the previous call. */
 int dfb_stream_set_atten_lim(dfb_stream *s, const int64_t *slots, int64_t n, float atten_lim_db);
 int dfb_stream_set_post_filter_beta(dfb_stream *s, const int64_t *slots, int64_t n, float beta);
 

@@ -15,6 +15,7 @@ from tests_common import synth_audio
 
 from deepfilternet_b200 import DfNet, DfStream, _lib, enhance, enhance_batch, enhance_device_ragged, init_df, libdf
 from deepfilternet_b200.config import ModelConfig
+from deepfilternet_b200.streaming import SLOT_FREE, SLOT_OPEN
 from deepfilternet_b200.weights import random_state_dict
 
 HOP = 480
@@ -245,12 +246,14 @@ def test_streaming_linked_equals_one_shot(states, kind, reduce):
     audio = torch.cat(recs, 0)
     ref = torch.cat([enhance(model, st, r, pad=False, reduce_mask=reduce) for r in recs], 0)
     s = DfStream(model, st, batch=4, channels=2, reduce_mask=reduce)
+    assert s.slot_states().tolist() == [SLOT_OPEN] * 4 and s.slot_groups().tolist() == [0, 0, 2, 2]
     outs, pos = [], 0
     for i, k in enumerate([1, 1, 2, 1, 7, 40, 1, 3, 64, 30, 7]):
         xk = audio[:, pos * HOP:(pos + k) * HOP]
         outs.append(s.process(xk.cuda() if i % 2 else xk).cpu())
         pos += k
     outs.append(s.flush())
+    assert s.slot_states().tolist() == [SLOT_FREE] * 4 and s.slot_groups().tolist() == [-1] * 4   # every stream has ended
     lat = s.latency_frames * HOP
     got = torch.cat(outs, 1)
     assert got.shape == (4, n * HOP + lat)
@@ -261,7 +264,9 @@ def test_streaming_linked_equals_one_shot(states, kind, reduce):
         s.set_mask_reduce(2, None)
     assert e.value.code == _lib.DFB_ERR_INVALID
     s.reset()
+    assert s.slot_states().tolist() == [SLOT_OPEN] * 4 and s.slot_groups().tolist() == [0, 0, 2, 2]   # the groups survive
     s.set_mask_reduce(1, None)
+    assert s.slot_groups().tolist() == [0, 1, 2, 3]
     free = torch.cat([s.process(audio), s.flush()], 1)[:, lat:]
     assert rms(free, enhance(model, st, audio, pad=False)) <= 1e-6
     with pytest.raises(_lib.DfbError):

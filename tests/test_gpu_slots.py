@@ -257,7 +257,7 @@ def test_slot_errors(st):
         with pytest.raises(_lib.DfbError) as e:
             op([0])
         assert e.value.code == _lib.DFB_ERR_UNSUPPORTED
-    # a handle with slots cannot be linked afterwards; reset brings back the slot-free handle
+    # a handle with slot operations cannot be linked afterwards; reset brings back every slot open
     s.close([2])
     with pytest.raises(_lib.DfbError) as e:
         s.set_mask_reduce(2, "mean")
