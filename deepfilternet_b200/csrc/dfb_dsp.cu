@@ -305,6 +305,65 @@ __global__ void __launch_bounds__(256) k_resample(const float *__restrict__ x, i
     }
 }
 
+// Streaming resampler of a handle at another rate (dfb_stream_set_sample_rate; ResampleDir in dfb_common.cuh): one row's
+// call.  x: the call's nin input samples, the first nin_valid of them the session's (the rest read as zero: the session's
+// zero extension); s_in0 / s_out0: the session's sample index of x[0] / y[0].  The taps are summed as k_resample sums
+// them (fmaf over k = 0 .. K-1, taps outside the session's input skipped), so a streamed session is bit for bit
+// k_resample of the whole session, delayed by Z.  The history is updated after every thread has read it.
+__device__ __forceinline__ void resample_row(const ResampleDir &d, const float *__restrict__ x, int64_t nin, int64_t nin_valid,
+                                             float *__restrict__ hist, int64_t s_in0, int64_t s_out0, float *__restrict__ y,
+                                             int64_t nout, int64_t nout_valid) {
+    const int64_t lim = s_in0 + nin_valid;
+    for (int64_t o = threadIdx.x; o < nout; o += blockDim.x) {
+        const int64_t t = s_out0 + o;
+        float acc = 0.f;
+        if (o < nout_valid && t >= d.Z) {
+            const int64_t i = t / d.nw;
+            const int j = (int)(t - i * d.nw);
+            const int64_t p0 = i * d.og - d.S;       // session index of tap 0: >= s_in0 - S, the history's first sample
+            const float *kr = d.taps + (size_t)j * d.K;
+            for (int k = 0; k < d.K; k++) {
+                const int64_t p = p0 + k;
+                if (p >= 0 && p < lim) {
+                    const int64_t l = p - s_in0;
+                    acc = fmaf(__ldg(kr + k), l < 0 ? hist[d.S + l] : x[l], acc);
+                }
+            }
+        }
+        y[o] = acc;
+    }
+    __syncthreads();
+    for (int q = threadIdx.x; q < d.S; q += blockDim.x) {   // nin >= S: the new history lies in this call's input
+        const int64_t l = nin - d.S + q;
+        hist[q] = l < nin_valid ? x[l] : 0.f;
+    }
+}
+
+// rate r -> 48 kHz: a session's input ends one hop before its end hop (the slot path reads that hop, the zero extension)
+__global__ void __launch_bounds__(256) k_resample_up(ResampleDir d, const ResampleRow *__restrict__ rows, const float *__restrict__ in,
+                                                     int64_t in_pitch, float *__restrict__ out, int64_t out_pitch,
+                                                     float *__restrict__ hist, int64_t n, int64_t a0) {
+    const ResampleRow r = rows[blockIdx.x];
+    const int64_t s = a0 - r.first;
+    int64_t v = in ? r.end - 1 - a0 : 0;
+    v = v < 0 ? 0 : (v > n ? n : v);
+    resample_row(d, in ? in + r.slot * in_pitch : nullptr, n * d.hop_in, v * d.hop_in, hist + (int64_t)blockIdx.x * d.S,
+                 s * d.hop_in, s * d.hop_out, out + r.slot * out_pitch, n * d.hop_out, n * d.hop_out);
+}
+
+// 48 kHz -> rate r: the slot path's output rows (zeros past a session's tail); a session's output ends `tail` hops after
+// its end hop, and the hops after that are zeros
+__global__ void __launch_bounds__(256) k_resample_down(ResampleDir d, const ResampleRow *__restrict__ rows, const float *__restrict__ in,
+                                                       int64_t in_pitch, float *__restrict__ out, int64_t out_pitch,
+                                                       float *__restrict__ hist, int64_t n, int64_t a0, int64_t tail) {
+    const ResampleRow r = rows[blockIdx.x];
+    const int64_t s = a0 - r.first;
+    int64_t v = r.end + tail - a0;
+    v = v < 0 ? 0 : (v > n ? n : v);
+    resample_row(d, in + r.slot * in_pitch, n * d.hop_in, n * d.hop_in, hist + (int64_t)blockIdx.x * d.S, s * d.hop_in,
+                 s * d.hop_out, out + r.slot * out_pitch, n * d.hop_out, v * d.hop_out);
+}
+
 // ------------------------------------------------------------- feature norm scans ----
 // Exponential mean norm of the ERB dB features and exponential unit norm of the first Fd bins,
 // sequential in t per (stream, band | bin) exactly like the reference loops.
@@ -1423,6 +1482,19 @@ int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaS
         k_apply_synthesis<5, 3, 2, false><<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb, nullptr);
     else
         k_apply_synthesis_generic<<<grid, 32 * kSynWarps, 0, s>>>(q, st->tb);
+    DFB_LAUNCH_CHECK();
+    return DFB_OK;
+}
+
+int launch_resample_stream(cudaStream_t s, bool up, const ResampleDir &d, const ResampleRow *rows, int nb, const float *in,
+                           int64_t in_pitch, float *out, int64_t out_pitch, float *hist, int64_t n, int64_t a0, int64_t tail) {
+    if (nb <= 0 || n <= 0) return DFB_OK;
+    if (nb > 65535 || d.S > d.hop_in) return fail(DFB_ERR_INVALID, "bad resampler geometry");
+    // (not in the DFB_PROF timing, which covers the 48 kHz enhancement path; torch.profiler names them)
+    if (up)
+        k_resample_up<<<nb, 256, 0, s>>>(d, rows, in, in_pitch, out, out_pitch, hist, n, a0);
+    else
+        k_resample_down<<<nb, 256, 0, s>>>(d, rows, in, in_pitch, out, out_pitch, hist, n, a0, tail);
     DFB_LAUNCH_CHECK();
     return DFB_OK;
 }

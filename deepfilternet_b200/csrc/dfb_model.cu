@@ -1583,11 +1583,13 @@ static ChunkGeom chunk_geom(const dfb_model_config &c) {
 }
 
 // Every array of the state slab is `layers` x [B][per_row] floats; only the GRU states have more than one layer.
-constexpr int kStateArrays = 13;
+// Arrays 13 / 14: the histories of a resampled handle's up / down resampler (dfb_stream_set_sample_rate), 0 floats otherwise.
+constexpr int kStateArrays = 15;
 // row_off / row_floats: one stream's row of every array, packed (the scratch rows of k_slot_rows)
 struct StateLayout { int64_t off[kStateArrays], row_off[kStateArrays], row_floats; int layers[kStateArrays], per_row[kStateArrays]; };
 
-static size_t state_floats(const dfb_model_config &c, const dfb_state *st, int B, size_t off[16], StateLayout *lay = nullptr) {
+static size_t state_floats(const dfb_model_config &c, const dfb_state *st, int B, size_t off[16], StateLayout *lay = nullptr,
+                           int rs_up = 0, int rs_down = 0) {
     const ChunkGeom g = chunk_geom(c);
     const int E = c.nb_erb, Fd = c.nb_df, O2 = 2 * c.df_order, F = st->tb.F, ED = E / 4 * kCh;
     size_t n = 0;
@@ -1607,6 +1609,7 @@ static size_t state_floats(const dfb_model_config &c, const dfb_state *st, int B
     add(9, 1, kMcTail * E); add(10, 1, kMcTail * Fd * O2);
     add(11, 1, c.conv_kt > 1 ? kHalo * ED : 0);
     add(12, 1, kMcTail);
+    add(13, 1, rs_up); add(14, 1, rs_down);
     return n;
 }
 static void state_bind(StreamState &S, float *base, const size_t off[16], int B) {
@@ -2484,7 +2487,23 @@ struct dfb_stream {
     int *d_slotmap = nullptr;                          // per slot its row of the active prefix, -1 free
     float *spec_stage_in = nullptr, *spec_stage_out = nullptr;   // device staging of dfb_stream_process_spec_host
     size_t spec_in_cap = 0, spec_out_cap = 0;
+    // sample rate (dfb_stream_set_sample_rate): 0 runs at the model's 48 kHz; else the caller's rate, resampled up into the
+    // unchanged 48 kHz slot path and back down.  The histories are arrays 13 / 14 of the state slab.
+    int rate = 0;
+    ResampleDir rs_up{}, rs_down{};
+    float *d_taps = nullptr;                           // both directions' taps
+    float *rs_in = nullptr, *rs_out = nullptr;         // the slot path's 48 kHz input / output [B][n * 480]
+    size_t rs_in_cap = 0, rs_out_cap = 0;
+    float *rs_lsnr = nullptr;                          // flush: the LSNR of its two passes
+    size_t rs_lsnr_cap = 0;
+    std::vector<ResampleRow> rs_rows;                  // the live rows' table on the device
+    ResampleRow *d_rs = nullptr;
 };
+
+// rate-r handles: per_row floats of the two resampler histories in the state slab (0, 0 at 48 kHz)
+static size_t stream_state_floats(const dfb_stream *h, size_t off[16], StateLayout *lay = nullptr) {
+    return state_floats(h->m->cfg, h->st, h->B, off, lay, h->rate ? h->rs_up.S : 0, h->rate ? h->rs_down.S : 0);
+}
 
 // the handle's default post-filter beta: the model's option (0 = off) for DeepFilterNet3; per-row beta is not used for
 // DeepFilterNet2, whose post filter acts on the ERB gains with a fixed beta
@@ -2568,13 +2587,16 @@ extern "C" void dfb_stream_free(dfb_stream *h) {
     if (h->d_slotmap) cudaFree(h->d_slotmap);
     if (h->spec_stage_in) cudaFree(h->spec_stage_in);
     if (h->spec_stage_out) cudaFree(h->spec_stage_out);
+    for (float *p : {h->d_taps, h->rs_in, h->rs_out, h->rs_lsnr})
+        if (p) cudaFree(p);
+    if (h->d_rs) cudaFree(h->d_rs);
     delete h;
 }
 
 extern "C" int dfb_stream_reset(dfb_stream *h) {
     if (!h) return fail(DFB_ERR_INVALID, "null stream");
     size_t off[16];
-    state_floats(h->m->cfg, h->st, h->B, off);
+    stream_state_floats(h, off);
     state_bind(h->S, h->slab, off, h->B);
     h->fed = false;
     slots_init(h);
@@ -2613,13 +2635,22 @@ extern "C" int dfb_stream_set_lsnr_thresholds(dfb_stream *h, int enable, float m
     return DFB_OK;
 }
 
-extern "C" int64_t dfb_stream_latency_frames(const dfb_stream *h) {
-    if (!h) return -1;
+// hops the 48 kHz slot path's output trails its input by
+static int64_t path_latency(const dfb_stream *h) {
     if (h->spectral) return h->m->cfg.conv_lookahead;   // the outputs wait for the encoder's look-ahead only
     const ChunkGeom g = chunk_geom(h->m->cfg);
     return g.Lmax + g.lag;
 }
-extern "C" int64_t dfb_stream_frame_length(const dfb_stream *h) { return h ? h->st->hop : -1; }  // capi.rs df_get_frame_length
+// a resampled handle's sessions end one hop later in the slot path (its zero extension fills the resamplers' look-ahead)
+extern "C" int64_t dfb_stream_latency_frames(const dfb_stream *h) { return h ? path_latency(h) + (h->rate ? 1 : 0) : -1; }
+extern "C" int64_t dfb_stream_frame_length(const dfb_stream *h) {   // capi.rs df_get_frame_length
+    return h ? (h->rate ? h->rate / 100 : h->st->hop) : -1;
+}
+// a resampled handle's signal delay on top of the 48 kHz handle's, in samples of its rate: D r / 48000 + E
+extern "C" int64_t dfb_stream_latency_samples(const dfb_stream *h) {
+    if (!h) return -1;
+    return h->rate ? (int64_t)h->rs_up.Z / h->rs_up.nw * h->rs_up.og + h->rs_down.Z : 0;
+}
 
 // ---- streaming slots: host bookkeeping.  Device rows follow at the next call (stream_step moves them first, by row_src).
 // the slot becomes free; its row stays in the active prefix until rows_compact
@@ -2657,7 +2688,8 @@ static void slots_retire(dfb_stream *h, int64_t out_end) {
 static void slot_close(dfb_stream *h, int slot) {
     if (h->slot_state[(size_t)slot] != kSlotOpen) return;
     h->slot_state[(size_t)slot] = kSlotClosing;
-    h->slot_end[(size_t)slot] = h->S.a1;   // the stream ends after the input it has been fed
+    // the stream ends after the input it has been fed; a resampled session one hop later, the hop its zero extension fills
+    h->slot_end[(size_t)slot] = h->S.a1 + (h->rate ? 1 : 0);
     h->tab_dirty = true;
 }
 
@@ -2665,7 +2697,7 @@ static void slot_close(dfb_stream *h, int slot) {
 // nothing and only closes the slots.
 static void slots_close_all(dfb_stream *h) {
     for (int b = 0; b < h->B; b++) slot_close(h, b);
-    slots_retire(h, h->S.a1 - dfb_stream_latency_frames(h));
+    slots_retire(h, h->S.a1 - path_latency(h));
     h->slot_ops = true;
 }
 
@@ -2734,7 +2766,7 @@ extern "C" int dfb_stream_open_linked(dfb_stream *h, const int64_t *slots, int64
 extern "C" int dfb_stream_close_slots(dfb_stream *h, const int64_t *slots, int64_t n) {
     if (int rc = slot_list(h, slots, n)) return rc;
     for (int64_t i = 0; i < n; i++) slot_close(h, (int)slots[i]);
-    slots_retire(h, h->S.a1 - dfb_stream_latency_frames(h));   // without look-ahead (latency 0) a closed slot is free at once
+    slots_retire(h, h->S.a1 - path_latency(h));   // without look-ahead (latency 0) a closed slot is free at once
     return DFB_OK;
 }
 
@@ -2834,14 +2866,14 @@ static int slots_move_rows(dfb_stream *h, cudaStream_t s) {
     dfb_model *m = h->m;
     size_t off[16];
     StateLayout lay;
-    state_floats(m->cfg, h->st, h->B, off, &lay);
+    stream_state_floats(h, off, &lay);
     if (int rc = m->arena.reserve(sizeof(int2) * ops.size() + sizeof(float) * (size_t)lay.row_floats * n_mv + 1024)) return rc;
     m->arena.reset();
     int2 *d_ops = m->arena.take<int2>(ops.size());
     float *scratch = m->arena.take<float>((size_t)lay.row_floats * n_mv + 1);
     DFB_CUDA(cudaMemcpyAsync(d_ops, ops.data(), sizeof(int2) * ops.size(), cudaMemcpyHostToDevice, s));
     for (int pass = n_mv ? 0 : 1; pass < 2; pass++) {
-        k_slot_rows<<<dim3(4, pass ? (unsigned)ops.size() : (unsigned)n_mv, kStateArrays), 256, 0, s>>>(
+        k_slot_rows<<<dim3(4, pass ? (unsigned)ops.size() : (unsigned)n_mv, h->rate ? kStateArrays : kStateArrays - 2), 256, 0, s>>>(
             h->slab, lay, h->B, d_ops, scratch, pass, m->cfg.nb_erb, m->cfg.nb_df);
         DFB_LAUNCH_CHECK();
     }
@@ -2867,6 +2899,50 @@ static int spec_fill_empty(const SpecOut &so, const dfb_model_config &c, int64_t
     return DFB_OK;
 }
 
+// The slot tables of a call of n input hops: closes every open slot first on a flush, moves the state-slab rows of slots
+// that opened or closed up (slots_move_rows) and uploads the row tables when they changed.
+static int stream_tables(dfb_stream *h, int64_t n, bool flush, bool spec, cudaStream_t s) {
+    const int hop = h->st->hop, B = h->B;
+    const int64_t n_out = flush ? path_latency(h) : n, a0 = h->S.a1;
+    if (flush) slots_close_all(h);
+    if (int rc = slots_move_rows(h, s)) return rc;
+    if (h->tab_dirty || h->tab_n != n) {
+        std::vector<RaggedRow> rows((size_t)h->n_act);
+        std::vector<int64_t> first((size_t)h->n_act);
+        std::vector<LinkRow> grp((size_t)h->n_act);
+        bool linked = false;   // the link table goes to the kernels only while a group of more than one channel is linked
+        bool pending = false;  // a closing row reads input in this call
+        const int64_t unit = spec ? kSpecF : hop, per = spec ? 1 : hop;   // input offsets in complex values / samples, lengths in frames / samples
+        for (int r = 0; r < h->n_act; r++) {
+            const int b = h->row_slot[(size_t)r];
+            const bool open = h->slot_state[(size_t)b] == kSlotOpen;
+            // a closing row reads no input, but for the hops before its end frame (a resampled session's last hop)
+            const int64_t tail = std::min(n, std::max<int64_t>(0, h->slot_end[(size_t)b] - a0));
+            rows[(size_t)r] = RaggedRow{b * n * unit, (open ? n : tail) * per, b * n_out * hop, n_out * hop, h->slot_end[(size_t)b]};
+            pending |= !open && tail > 0;
+            first[(size_t)r] = h->slot_first[(size_t)b];
+            grp[(size_t)r] = LinkRow{h->slot_row[(size_t)h->slot_grp[(size_t)b]], h->slot_nch[(size_t)b]};
+            linked |= grp[(size_t)r].n > 1 && h->group_reduce != kReduceNone;
+        }
+        if (h->n_act > 0) {
+            DFB_CUDA(cudaMemcpyAsync(h->d_rows, rows.data(), sizeof(RaggedRow) * rows.size(), cudaMemcpyHostToDevice, s));
+            DFB_CUDA(cudaMemcpyAsync(h->d_first, first.data(), sizeof(int64_t) * first.size(), cudaMemcpyHostToDevice, s));
+            if (linked) DFB_CUDA(cudaMemcpyAsync(h->d_grp, grp.data(), sizeof(LinkRow) * grp.size(), cudaMemcpyHostToDevice, s));
+        }
+        if (spec) {   // k_spec_emit covers every caller row: free slots get NaN / -1
+            if (!h->d_slotmap && cudaMalloc(&h->d_slotmap, sizeof(int) * (size_t)B) != cudaSuccess) {
+                h->d_slotmap = nullptr;
+                return fail(DFB_ERR_OOM, "slot table allocation failed");
+            }
+            DFB_CUDA(cudaMemcpyAsync(h->d_slotmap, h->slot_row.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, s));
+        }
+        h->tab_dirty = pending;   // such a row reads nothing from the next call on
+        h->tab_n = n;
+        h->tab_linked = linked;
+    }
+    return DFB_OK;
+}
+
 // One call: rows [0, n_act) of the slab, the row table for calls of n input hops.
 // Spectral handle (so != null): d_in is [B][n][F] complex, the outputs go to so's buffers, d_out / d_lsnr are null.
 static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s,
@@ -2877,7 +2953,7 @@ static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, 
     StreamState &S = h->S;
     const ChunkGeom g = chunk_geom(m->cfg);
     const int hop = st->hop, B = h->B;
-    const int64_t Ltot = dfb_stream_latency_frames(h), n_out = flush ? Ltot : n;
+    const int64_t Ltot = path_latency(h), n_out = flush ? Ltot : n;
     const int64_t lag = so ? 0 : g.lag, la = Ltot - lag;   // feature look-ahead of the DNN frames; their outputs' further lag
     const int64_t a0 = S.a1, a1n = a0 + (flush ? 0 : n);
     if (a1n >= kOpenEnd - 1) return fail(DFB_ERR_UNSUPPORTED, "stream clock beyond 2^31 - 2 frames: reset the stream");
@@ -2885,38 +2961,7 @@ static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, 
     int64_t d1n = flush ? a1n : a1n - la, e1n = flush ? a1n : d1n - lag;
     if (d1n < S.d1) d1n = S.d1;
     if (e1n < S.e1) e1n = S.e1;
-    if (flush) slots_close_all(h);
-    if ((rc = slots_move_rows(h, s))) return rc;
-    if (h->tab_dirty || h->tab_n != n) {
-        std::vector<RaggedRow> rows((size_t)h->n_act);
-        std::vector<int64_t> first((size_t)h->n_act);
-        std::vector<LinkRow> grp((size_t)h->n_act);
-        bool linked = false;   // the link table goes to the kernels only while a group of more than one channel is linked
-        const int64_t unit = so ? kSpecF : hop, per = so ? 1 : hop;   // input offsets in complex values / samples, lengths in frames / samples
-        for (int r = 0; r < h->n_act; r++) {
-            const int b = h->row_slot[(size_t)r];
-            const bool open = h->slot_state[(size_t)b] == kSlotOpen;
-            rows[(size_t)r] = RaggedRow{b * n * unit, open ? n * per : 0, b * n_out * hop, n_out * hop, h->slot_end[(size_t)b]};
-            first[(size_t)r] = h->slot_first[(size_t)b];
-            grp[(size_t)r] = LinkRow{h->slot_row[(size_t)h->slot_grp[(size_t)b]], h->slot_nch[(size_t)b]};
-            linked |= grp[(size_t)r].n > 1 && h->group_reduce != kReduceNone;
-        }
-        if (h->n_act > 0) {
-            DFB_CUDA(cudaMemcpyAsync(h->d_rows, rows.data(), sizeof(RaggedRow) * rows.size(), cudaMemcpyHostToDevice, s));
-            DFB_CUDA(cudaMemcpyAsync(h->d_first, first.data(), sizeof(int64_t) * first.size(), cudaMemcpyHostToDevice, s));
-            if (linked) DFB_CUDA(cudaMemcpyAsync(h->d_grp, grp.data(), sizeof(LinkRow) * grp.size(), cudaMemcpyHostToDevice, s));
-        }
-        if (so) {   // k_spec_emit covers every caller row: free slots get NaN / -1
-            if (!h->d_slotmap && cudaMalloc(&h->d_slotmap, sizeof(int) * (size_t)B) != cudaSuccess) {
-                h->d_slotmap = nullptr;
-                return fail(DFB_ERR_OOM, "slot table allocation failed");
-            }
-            DFB_CUDA(cudaMemcpyAsync(h->d_slotmap, h->slot_row.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, s));
-        }
-        h->tab_dirty = false;
-        h->tab_n = n;
-        h->tab_linked = linked;
-    }
+    if ((rc = stream_tables(h, n, flush, so != nullptr, s))) return rc;
     const int64_t f0 = a0 - Ltot;   // output hop j carries frame a0 - Ltot + j (flush: a1 = a0)
     // The apply kernel writes every hop that carries a frame of its row.  The others are zero: those of free slots, of
     // frames before 0, before a row's first frame or from a closing row's end on, and all of them when no frame is emitted.
@@ -2964,6 +3009,186 @@ static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, 
     return DFB_OK;
 }
 
+// ---- handles at another sample rate (dfb_stream_set_sample_rate; DESIGN.md section 5g).  Each call runs the unchanged
+// 48 kHz slot path between two resamplers: k_resample_up turns the call's rate-r input into the 48 kHz hops the path reads,
+// k_resample_down turns the path's output back into rate-r hops.  Their histories are rows of the state slab, so they
+// move with the rows and start from zero with every session.
+
+constexpr int kModelRate = 48000;   // the slot path's rate: 480-sample hops of the 960 / 480 STFT
+
+// the per-direction geometry of `rate` from io.resample_kernel's (og, nw, width); DFB_ERR_UNSUPPORTED for a rate outside
+// the list, DFB_ERR_INVALID for taps of other rates or a history longer than a hop
+static int rs_geometry(int rate, bool up, const float *taps, int og, int nw, int width, ResampleDir *d) {
+    if (rate != 8000 && rate != 12000 && rate != 16000 && rate != 24000 && rate != 32000 && rate != 44100)
+        return fail(DFB_ERR_UNSUPPORTED, "sample rate %d: 8000, 12000, 16000, 24000, 32000, 44100 or 48000", rate);
+    const int g = std::gcd(rate, kModelRate), from = up ? rate : kModelRate, to = up ? kModelRate : rate;
+    if (!taps || og != from / g || nw != to / g || width <= 0 || width > 4096)
+        return fail(DFB_ERR_INVALID, "the %s taps of %d Hz are io.resample_kernel(%d, %d): og %d, nw %d", up ? "up" : "down", rate,
+                    from, to, from / g, to / g);
+    const int mz = (width + og - 1) / og;
+    *d = ResampleDir{taps, og, nw, 2 * width + og, mz * og + width, mz * nw, from / 100, to / 100};
+    if (d->S > d->hop_in) return fail(DFB_ERR_INVALID, "resampler history of %d samples is longer than a hop", d->S);
+    return DFB_OK;
+}
+
+static int stage_grow(float **p, size_t *cap, size_t bytes);
+
+// the live rows' table of the resamplers, uploaded when it changed
+static int rs_table(dfb_stream *h, cudaStream_t s) {
+    std::vector<ResampleRow> rows((size_t)h->n_act);
+    for (int r = 0; r < h->n_act; r++) {
+        const size_t b = (size_t)h->row_slot[(size_t)r];
+        rows[(size_t)r] = ResampleRow{(int64_t)b, h->slot_first[b], h->slot_end[b]};
+    }
+    if (rows.size() != h->rs_rows.size() || memcmp(rows.data(), h->rs_rows.data(), sizeof(ResampleRow) * rows.size())) {
+        if (!rows.empty())
+            DFB_CUDA(cudaMemcpyAsync(h->d_rs, rows.data(), sizeof(ResampleRow) * rows.size(), cudaMemcpyHostToDevice, s));
+        h->rs_rows.swap(rows);
+    }
+    return DFB_OK;
+}
+
+// One pass through the slot path: n hops of rate-r input (d_in null: none, the sessions' zero extension), or its flush;
+// the rate-r output hops go to d_out [B][pitch] (the caller offsets the column), their LSNR to d_lsnr [B][n_out].
+static int rate_pass(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, int64_t pitch, float *d_lsnr,
+                     cudaStream_t s) {
+    const int64_t L = path_latency(h), n_out = flush ? L : n, hop = h->st->hop, hr = h->rate / 100, B = h->B, a0 = h->S.a1;
+    int rc;
+    if ((rc = stream_tables(h, n, flush, false, s)) || (rc = rs_table(h, s))) return rc;
+    if ((!flush && (rc = stage_grow(&h->rs_in, &h->rs_in_cap, sizeof(float) * B * n * hop))) ||
+        (rc = stage_grow(&h->rs_out, &h->rs_out_cap, sizeof(float) * B * std::max<int64_t>(n_out, 1) * hop)))
+        return rc;
+    const int nb = h->n_act;
+    if (nb < B && n_out > 0)
+        DFB_CUDA(cudaMemset2DAsync(d_out, sizeof(float) * pitch, 0, sizeof(float) * n_out * hr, B, s));
+    size_t off[16];
+    stream_state_floats(h, off);
+    if (!flush && (rc = launch_resample_stream(s, true, h->rs_up, h->d_rs, nb, d_in, n * hr, h->rs_in, n * hop, h->slab + off[13], n,
+                                               a0, 0)))
+        return rc;
+    if ((rc = stream_step(h, flush ? nullptr : h->rs_in, n, flush, h->rs_out, d_lsnr, s))) return rc;
+    return launch_resample_stream(s, false, h->rs_down, h->d_rs, nb, h->rs_out, n_out * hop, d_out, pitch, h->slab + off[14], n_out,
+                                  a0, L);
+}
+
+// A call of a resampled handle.  A flush ends every open session (its input one hop before its end frame), runs that hop
+// of zero extension through the slot path and then flushes it: L + 1 output hops.
+static int rate_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s) {
+    const int64_t hr = h->rate / 100, B = h->B;
+    if (!flush) return rate_pass(h, d_in, n, false, d_out, n * hr, d_lsnr, s);
+    const int64_t L = path_latency(h), w = L + 1;
+    for (int b = 0; b < h->B; b++) slot_close(h, b);
+    h->slot_ops = true;
+    int rc;
+    float *l1 = nullptr, *l2 = nullptr;
+    if (d_lsnr) {
+        if ((rc = stage_grow(&h->rs_lsnr, &h->rs_lsnr_cap, sizeof(float) * B * w))) return rc;
+        l1 = h->rs_lsnr; l2 = l1 + B;
+    }
+    if ((rc = rate_pass(h, nullptr, 1, false, d_out, w * hr, l1, s))) return rc;
+    if (L > 0 && (rc = rate_pass(h, nullptr, 0, true, d_out + hr, w * hr, l2, s))) return rc;
+    if (d_lsnr) {
+        DFB_CUDA(cudaMemcpy2DAsync(d_lsnr, sizeof(float) * w, l1, sizeof(float), sizeof(float), B, cudaMemcpyDeviceToDevice, s));
+        if (L > 0)
+            DFB_CUDA(cudaMemcpy2DAsync(d_lsnr + 1, sizeof(float) * w, l2, sizeof(float) * L, sizeof(float) * L, B, cudaMemcpyDeviceToDevice, s));
+    }
+    return DFB_OK;
+}
+
+// the calls of an audio handle, at 48 kHz or resampled
+static int audio_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s) {
+    return h->rate ? rate_step(h, d_in, n, flush, d_out, d_lsnr, s) : stream_step(h, d_in, n, flush, d_out, d_lsnr, s);
+}
+
+// (Re)allocates the state slab of a new or reset handle for its current rate, zeroed.
+static int stream_slab(dfb_stream *h) {
+    size_t off[16];
+    const size_t n = stream_state_floats(h, off);
+    float *p = nullptr;
+    if (cudaMalloc(&p, n * sizeof(float)) != cudaSuccess) return fail(DFB_ERR_OOM, "stream state allocation failed");
+    if (h->slab) cudaFree(h->slab);
+    h->slab = p;
+    DFB_CUDA(cudaMemset(h->slab, 0, n * sizeof(float)));
+    state_bind(h->S, h->slab, off, h->B);
+    return DFB_OK;
+}
+
+extern "C" int dfb_stream_set_sample_rate(dfb_stream *h, int rate, const float *up_taps, int up_og, int up_nw, int up_width,
+                                          const float *down_taps, int down_og, int down_nw, int down_width) {
+    if (!h) return fail(DFB_ERR_INVALID, "null stream");
+    if (h->spectral) return fail(DFB_ERR_INVALID, "a spectral handle takes spectra, which have no sample rate");
+    if (h->fed || h->slot_ops)
+        return fail(DFB_ERR_INVALID, "sample rate set after the first frame or a slot operation: reset the stream first");
+    ResampleDir up{}, down{};
+    int rc;
+    if (rate != kModelRate && ((rc = rs_geometry(rate, true, up_taps, up_og, up_nw, up_width, &up)) ||
+                               (rc = rs_geometry(rate, false, down_taps, down_og, down_nw, down_width, &down))))
+        return rc;
+    DFB_CUDA(cudaSetDevice(h->m->device));
+    if (!h->d_rs && cudaMalloc(&h->d_rs, sizeof(ResampleRow) * (size_t)h->B) != cudaSuccess) {
+        h->d_rs = nullptr;
+        return fail(DFB_ERR_OOM, "resampler table allocation failed");
+    }
+    float *taps = nullptr;
+    if (rate != kModelRate) {
+        const size_t nu = (size_t)up.nw * up.K, nd = (size_t)down.nw * down.K;
+        if (cudaMalloc(&taps, sizeof(float) * (nu + nd)) != cudaSuccess) return fail(DFB_ERR_OOM, "resampler taps allocation failed");
+        if (cudaMemcpy(taps, up_taps, sizeof(float) * nu, cudaMemcpyHostToDevice) != cudaSuccess ||
+            cudaMemcpy(taps + nu, down_taps, sizeof(float) * nd, cudaMemcpyHostToDevice) != cudaSuccess) {
+            cudaFree(taps);
+            return fail(DFB_ERR_CUDA, "resampler taps upload failed");
+        }
+        up.taps = taps; down.taps = taps + nu;
+    }
+    const int old_rate = h->rate;
+    const ResampleDir old_up = h->rs_up, old_down = h->rs_down;
+    h->rate = rate == kModelRate ? 0 : rate;
+    h->rs_up = up; h->rs_down = down;
+    if ((rc = stream_slab(h))) {   // the old slab stays
+        h->rate = old_rate; h->rs_up = old_up; h->rs_down = old_down;
+        if (taps) cudaFree(taps);
+        return rc;
+    }
+    if (h->d_taps) cudaFree(h->d_taps);
+    h->d_taps = taps;
+    h->rs_rows.clear();
+    slots_init(h);
+    return DFB_OK;
+}
+
+// Debug aid: one resampler on its own over a list of call sizes, every row one session from hop 0
+extern "C" int dfb_debug_resample_stream(int up, int rate, const float *d_taps, int og, int nw, int width, const float *d_in, int64_t C,
+                                         const int64_t *h_calls, int64_t n_calls, float *d_out, void *stream) {
+    ResampleDir d{};
+    if (int rc = rs_geometry(rate, up != 0, d_taps, og, nw, width, &d)) return rc;
+    if (!d_in || !d_out || C <= 0 || C > 65535 || !h_calls || n_calls <= 0) return fail(DFB_ERR_INVALID, "bad argument");
+    int64_t H = 0;
+    for (int64_t i = 0; i < n_calls; i++) {
+        if (h_calls[i] <= 0) return fail(DFB_ERR_INVALID, "call %lld has %lld hops", (long long)i, (long long)h_calls[i]);
+        H += h_calls[i];
+    }
+    int dev = 0;
+    DFB_CUDA(cudaGetDevice(&dev));
+    if (int rc = use_device(dev)) return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    std::vector<ResampleRow> rows((size_t)C);
+    for (int64_t c = 0; c < C; c++) rows[(size_t)c] = ResampleRow{c, 0, kOpenEnd};
+    ResampleRow *d_rows = nullptr;
+    float *hist = nullptr;
+    int rc = DFB_OK;
+    if (cudaMalloc(&d_rows, sizeof(ResampleRow) * C) != cudaSuccess || cudaMalloc(&hist, sizeof(float) * C * d.S) != cudaSuccess ||
+        cudaMemcpyAsync(d_rows, rows.data(), sizeof(ResampleRow) * C, cudaMemcpyHostToDevice, s) != cudaSuccess ||
+        cudaMemsetAsync(hist, 0, sizeof(float) * C * d.S, s) != cudaSuccess)
+        rc = fail(DFB_ERR_OOM, "debug buffers");
+    for (int64_t i = 0, a0 = 0; i < n_calls && !rc; a0 += h_calls[i++])
+        rc = launch_resample_stream(s, up != 0, d, d_rows, (int)C, d_in + a0 * d.hop_in, H * d.hop_in, d_out + a0 * d.hop_out,
+                                    H * d.hop_out, hist, h_calls[i], a0, kOpenEnd);
+    cudaStreamSynchronize(s);
+    if (d_rows) cudaFree(d_rows);
+    if (hist) cudaFree(hist);
+    return rc;
+}
+
 // d_in [B][n_frames * hop] -> d_out [B][n_frames * hop] (device pointers, asynchronous on `stream`); d_lsnr (or null)
 // [B][n_frames]: the LSNR of the frame each output hop carries, NaN where it carries none
 static int audio_only(const dfb_stream *h) {
@@ -2973,7 +3198,7 @@ extern "C" int dfb_stream_process_lsnr(dfb_stream *h, const float *d_in, int64_t
     if (int rc = audio_only(h)) return rc;
     if (!h || !d_in || !d_out || n_frames <= 0) return fail(DFB_ERR_INVALID, "bad argument");
     DFB_CUDA(cudaSetDevice(h->m->device));
-    return stream_step(h, d_in, n_frames, false, d_out, d_lsnr, (cudaStream_t)stream);
+    return audio_step(h, d_in, n_frames, false, d_out, d_lsnr, (cudaStream_t)stream);
 }
 extern "C" int dfb_stream_process(dfb_stream *h, const float *d_in, int64_t n_frames, float *d_out, void *stream) {
     return dfb_stream_process_lsnr(h, d_in, n_frames, d_out, nullptr, stream);
@@ -2987,7 +3212,7 @@ extern "C" int dfb_stream_flush_lsnr(dfb_stream *h, float *d_out, float *d_lsnr,
     if (!h || !d_out) return fail(DFB_ERR_INVALID, "bad argument");
     DFB_CUDA(cudaSetDevice(h->m->device));
     int rc = DFB_OK;
-    if (dfb_stream_latency_frames(h) > 0) rc = stream_step(h, nullptr, 0, true, d_out, d_lsnr, (cudaStream_t)stream);
+    if (dfb_stream_latency_frames(h) > 0) rc = audio_step(h, nullptr, 0, true, d_out, d_lsnr, (cudaStream_t)stream);
     if (!rc) slots_close_all(h);
     return rc;
 }
@@ -3014,14 +3239,14 @@ extern "C" int dfb_stream_process_host_lsnr(dfb_stream *h, const float *h_in, in
         return DFB_OK;
     }
     if (!h_out) return fail(DFB_ERR_INVALID, "bad argument");
-    const size_t bytes = sizeof(float) * (size_t)h->B * nf * h->st->hop, lbytes = sizeof(float) * (size_t)h->B * nf;
+    const size_t bytes = sizeof(float) * (size_t)h->B * nf * dfb_stream_frame_length(h), lbytes = sizeof(float) * (size_t)h->B * nf;
     int rc;
     if ((!flush && (rc = stage_grow(&h->stage_in, &h->stage_in_cap, bytes))) || (rc = stage_grow(&h->stage_out, &h->stage_out_cap, bytes)) ||
         (h_lsnr && (rc = stage_grow(&h->stage_lsnr, &h->stage_lsnr_cap, lbytes))))
         return rc;
     cudaStream_t s = h->m->stream;
     if (!flush) DFB_CUDA(cudaMemcpyAsync(h->stage_in, h_in, bytes, cudaMemcpyHostToDevice, s));
-    if ((rc = stream_step(h, h->stage_in, nf, flush, h->stage_out, h_lsnr ? h->stage_lsnr : nullptr, s))) return rc;
+    if ((rc = audio_step(h, h->stage_in, nf, flush, h->stage_out, h_lsnr ? h->stage_lsnr : nullptr, s))) return rc;
     DFB_CUDA(cudaMemcpyAsync(h_out, h->stage_out, bytes, cudaMemcpyDeviceToHost, s));
     if (h_lsnr) DFB_CUDA(cudaMemcpyAsync(h_lsnr, h->stage_lsnr, lbytes, cudaMemcpyDeviceToHost, s));
     DFB_CUDA(cudaStreamSynchronize(s));

@@ -28,6 +28,14 @@ frames from the caller's own filter bank and returns the network's outputs, appl
 
 Row j of a call that starts at input frame k carries frame k + j - ``latency_frames`` (conv_lookahead); rows that carry no
 frame are NaN with stage -1 (dfb_stream_create_spec in include/dfb200.h).
+
+``sr`` runs an audio handle at 8, 12, 16, 24, 32 or 44.1 kHz: its hops are ``sr // 100`` samples, and each call is resampled
+to 48 kHz on the device (``io.resample``'s sinc_fast taps, with per-slot filter history), enhanced by the unchanged 48 kHz
+slot path and resampled back.  ``latency_frames`` grows by one hop and ``latency_samples`` is the resamplers' own delay
+(dfb_stream_set_sample_rate in include/dfb200.h)::
+
+    s = DfStream(model, df_state, batch=B, sr=16000)
+    out = s.process(chunk)               # chunk: float32 [B, n * 160]
 """
 from __future__ import annotations
 
@@ -39,13 +47,34 @@ import numpy as np
 import torch
 from torch import Tensor
 
-from . import _lib, ragged
-from ._lib import DFB_ERR_INVALID, DfbError, check
+from . import _lib, io, ragged
+from ._lib import DFB_ERR_INVALID, DFB_ERR_UNSUPPORTED, DfbError, check
 from .libdf import DF
 from .model import DfNet
 
 
 SLOT_FREE, SLOT_OPEN, SLOT_CLOSING = 0, 1, 2
+MODEL_SR = 48000
+# rates with a whole number of samples per 10 ms hop that a streaming handle resamples to and from MODEL_SR
+STREAM_RATES = (8000, 12000, 16000, 24000, 32000, 44100)
+
+
+def rate_taps(sr: int):
+    """The resamplers of a handle at ``sr``: ((taps, og, nw, width) of sr -> 48 kHz, the same of 48 kHz -> sr), the
+    sinc_fast taps of io.resample.  DfbError (DFB_ERR_UNSUPPORTED, as the C ABI) for a rate outside STREAM_RATES."""
+    if isinstance(sr, bool) or not isinstance(sr, (int, np.integer)) or int(sr) not in STREAM_RATES:
+        raise DfbError(DFB_ERR_UNSUPPORTED, f"sample rate {sr!r}: one of {STREAM_RATES} or {MODEL_SR}")
+    p = io.get_resample_params("sinc_fast")
+    return io.resample_kernel(int(sr), MODEL_SR, **p), io.resample_kernel(MODEL_SR, int(sr), **p)
+
+
+def rate_delays(og_up: int, nw_up: int, width_up: int, og_down: int, nw_down: int, width_down: int):
+    """(D, E, delay) of a handle whose resamplers have these geometries: the zeros in front of the upsampled session (48 kHz
+    samples) and of the downsampled output (rate-r samples), the smallest whole numbers of polyphase groups after which
+    every hop's outputs need only input received with that hop, and the delay they add in rate-r samples."""
+    D = -(-width_up // og_up) * nw_up
+    E = -(-width_down // og_down) * nw_down
+    return D, E, D // nw_up * og_up + E
 
 
 def slot_list(slots, batch: int) -> np.ndarray:
@@ -137,7 +166,7 @@ def need_spectral(s) -> None:
 
 class DfStream:
     def __init__(self, model: DfNet, df_state: DF, batch: int = 1, atten_lim_db: Optional[float] = None, channels: int = 1,
-                 reduce_mask: Optional[str] = None, spectral: bool = False):
+                 reduce_mask: Optional[str] = None, spectral: bool = False, sr: Optional[int] = None):
         self.model, self.df_state, self.batch = model, df_state, int(batch)
         self.spectral = bool(spectral)
         if self.spectral and atten_lim_db is not None:
@@ -150,14 +179,35 @@ class DfStream:
             check(_lib.lib().dfb_stream_create(C.byref(h), model.handle, df_state.handle, self.batch, lim))
         self._h = h
         self.freq_bins = int(df_state.fft_size()) // 2 + 1
-        self.hop = int(_lib.lib().dfb_stream_frame_length(h))
-        self.latency_frames = int(_lib.lib().dfb_stream_latency_frames(h))
-        if channels != 1 or ragged.reduce_code(reduce_mask):
-            try:
+        self._read_rate()
+        try:
+            if sr is not None:
+                self.set_sample_rate(sr)
+            if channels != 1 or ragged.reduce_code(reduce_mask):
                 self.set_mask_reduce(channels, reduce_mask)
-            except Exception:
-                self.__del__()   # a constructor that fails leaves no handle behind
-                raise
+        except Exception:
+            self.__del__()   # a constructor that fails leaves no handle behind
+            raise
+
+    def _read_rate(self) -> None:
+        L = _lib.lib()
+        self.hop = int(L.dfb_stream_frame_length(self._h))
+        self.latency_frames = int(L.dfb_stream_latency_frames(self._h))
+        self.latency_samples = int(L.dfb_stream_latency_samples(self._h))
+        self.sr = self.hop * 100
+
+    def set_sample_rate(self, sr: int) -> None:
+        """Run every slot at ``sr`` (STREAM_RATES, or 48000: the model's own rate), resampled on the device; afterwards
+        ``hop``, ``latency_frames`` and ``latency_samples`` are the rate's.  Only on a new or reset audio handle before its
+        first frame and any slot operation (DfbError otherwise); survives ``reset`` (dfb_stream_set_sample_rate)."""
+        if getattr(self, "spectral", False):
+            raise DfbError(DFB_ERR_INVALID, "a spectral handle takes spectra, which have no sample rate")
+        if isinstance(sr, (int, np.integer)) and not isinstance(sr, bool) and int(sr) == MODEL_SR:
+            check(_lib.lib().dfb_stream_set_sample_rate(self._h, MODEL_SR, None, 0, 0, 0, None, 0, 0, 0))
+        else:
+            (ku, wu, ou, nu), (kd, wd, od, nd) = rate_taps(sr)
+            check(_lib.lib().dfb_stream_set_sample_rate(self._h, int(sr), ku.data_ptr(), ou, nu, wu, kd.data_ptr(), od, nd, wd))
+        self._read_rate()
 
     def set_mask_reduce(self, channels: int, reduce_mask: Optional[str]) -> None:
         """Linked channels: rows g * channels + c form recording g; reduce_mask None / "none", "max" or "mean".  Only on a new

@@ -340,6 +340,47 @@ int dfb_stream_process_lsnr(dfb_stream *s, const float *d_in, int64_t n_frames, 
 int dfb_stream_flush_lsnr(dfb_stream *s, float *d_out, float *d_lsnr, void *stream);
 int dfb_stream_process_host_lsnr(dfb_stream *s, const float *h_in, int64_t n_frames, float *h_out, float *h_lsnr);
 
+/* Sample rate of an audio handle: its slots, slot groups and fixed channel groups run at rate r in {8000, 12000, 16000,
+ * 24000, 32000, 44100} -- the rates with a whole number of samples per 10 ms hop, h_r = r / 100 -- while inside them the
+ * 48 kHz slot path runs unchanged between two resamplers with the taps of df.io.resample's default method, sinc_fast:
+ *   R_up = io.resample(., r, 48000), R_down = io.resample(., 48000, r)   (torchaudio's resample; dfb_resample_host)
+ * both over a session's audio zero-extended past its end.  up_* / down_* are io.resample_kernel's (kernel [nw][2 width +
+ * og], width, og, nw) for (r, 48000) and (48000, r), passed as dfb_resample_host takes them.  Every slot carries its own
+ * filter histories, and a new session starts from zero ones.
+ * Frames are h_r samples: dfb_stream_process takes and returns [B][n * h_r]; flush, close and the _host variants keep
+ * their meaning in units of h_r.  A session of calls n_1 .. n_c (a_1 = sum n_i hops) ended by flush, or by close and its
+ * drain, outputs exactly:
+ *   1. u' = D_r zeros followed by R_up(x)                                 (48 kHz)
+ *   2. y48 = a 48 kHz handle fed u' in the calls n_1 .. n_c, one more call of 1 hop, then flushed
+ *   3. E_r zeros followed by R_down(y48), cropped to (a_1 + L + 1) h_r samples   (L: the 48 kHz handle's latency)
+ * D_r (48 kHz samples, a multiple of 48000 / gcd(r, 48000)) and E_r (rate-r samples) are the smallest delays with which every
+ * call can form its n model hops from the input received so far and return its n h_r samples:
+ *   D_r = ceil(width_up / og_up) nw_up,   E_r = ceil(width_down / og_down) nw_down.
+ * So dfb_stream_latency_frames is L + 1 (the hops a flush returns and a closing slot drains for), and
+ * dfb_stream_latency_samples the signal delay beyond the 48 kHz handle's, D_r r / 48000 + E_r, always below one hop:
+ *      r    h_r  og/nw/width up  D_r   og/nw/width down  E_r   delay (samples / ms)
+ *    8000    80     1/6/17       102       6/1/97         17     34 / 4.25
+ *   12000   120     1/4/17        68       4/1/65         17     34 / 2.833
+ *   16000   160     1/3/17        51       3/1/49         17     34 / 2.125
+ *   24000   240     1/2/17        34       2/1/33         17     34 / 1.417
+ *   32000   320     2/3/17        27       3/2/25         18     36 / 1.125
+ *   44100   441   147/160/17     160     160/147/18      147    294 / 6.667
+ * LSNR rows (NaN rows and stage gating included), per-slot settings, slot groups and re-opened slots behave as at 48 kHz
+ * on the model frames of this composition.  Only on a new or reset handle before its first frame and any slot operation
+ * (else DFB_ERR_INVALID); it survives dfb_stream_reset.  A spectral handle: DFB_ERR_INVALID (spectra have no rate).  Other
+ * rates: DFB_ERR_UNSUPPORTED; 48000 is the plain 48 kHz handle (the taps are ignored and may be NULL).  Taps of other rates
+ * or geometry: DFB_ERR_INVALID. */
+int dfb_stream_set_sample_rate(dfb_stream *s, int rate, const float *up_taps, int up_og, int up_nw, int up_width,
+                               const float *down_taps, int down_og, int down_nw, int down_width);
+int64_t dfb_stream_latency_samples(const dfb_stream *s);   /* D_r r / 48000 + E_r; 0 at 48 kHz */
+/* Debug aid: one of the two resamplers of a resampled handle on its own (up != 0: k_resample_up, r -> 48 kHz; else
+ * k_resample_down, 48 kHz -> r), taps d_taps [nw][2 width + og] (device) as dfb_stream_set_sample_rate takes them.  C rows,
+ * each one session from hop 0, run through the calls h_calls[0 .. n_calls) (HOST array of hop counts >= 1) with their
+ * histories carried: d_in f32[C][H * hop_in] -> d_out f32[C][H * hop_out], H = sum of the calls, hop = 480 at 48 kHz and
+ * h_r at r.  Row c of d_out is the resampled row delayed by D_r (up) or E_r (down) output samples, bit for bit. */
+int dfb_debug_resample_stream(int up, int rate, const float *d_taps, int og, int nw, int width, const float *d_in, int64_t C,
+                              const int64_t *h_calls, int64_t n_calls, float *d_out, void *stream);
+
 /* Spectral streaming handle (capi.rs df_process_frame_raw, DfTract::process_raw, tract.rs:441-506): the caller runs its own
  * filter bank, passes spectrum frames in and gets the network's outputs back -- ERB gains, deep-filter coefficients, LSNR
  * and the stage LSNR gating picks -- with the features' normalisation, the GRU, conv and norm states carried between
