@@ -465,10 +465,40 @@ using namespace dfb;
 // first / w0: streaming slots, each stream's first frame (stream_first) or null
 struct GruChunk { float *h; bool have_state; int t0; int Bs; const int64_t *first; int64_t w0; };
 
+// Weight tables: device pointers into the weight slab, bound once by dfb_model_create for the layers the configured
+// forward pass runs.  A tensor that pass does not read stays null.
+struct Wb { const float *w = nullptr, *b = nullptr; };  // input conv, head, DeepFilterNet v1 grouped linear with bias
+struct Blk { const float *dw = nullptr, *pw = nullptr, *b = nullptr, *pw_sw = nullptr; };  // separable block (pw: v1)
+struct PathW { const float *s = nullptr, *b = nullptr; };  // decoder pathway: relu(x * s + b)
+// grouped linear [G][I/G][H/G]; bx: its tensor-core image `img` was uploaded and the shape is built, so it runs on the
+// tensor-core kernel, which reads its input as BF16 planes only
+struct Gl { const float *w = nullptr, *img = nullptr; int G = 0, I = 0, H = 0; bool bx = false; };
+struct GruLayer { const float *w_hh, *b_ih, *b_hh, *w_ih_hi, *w_ih_lo; };  // w_ih_hi / lo: BF16 planes, two per float
+
+struct NetW {  // DeepFilterNet2 / 3 (forward_body)
+    Wb erb_conv0, df_conv0, lsnr, df_fc_a /* DeepFilterNet2 */, conv0_out;
+    Blk erb_conv1, erb_conv2, erb_conv3, df_conv1, convt3, convt2, convt1;
+    PathW conv3p, conv2p, conv1p, conv0p;
+    Gl df_fc_emb, enc_in, enc_out, df_skip, df_in, df_out, erb_in, erb_out;
+    std::vector<GruLayer> enc_gru, df_gru, erb_gru;
+    struct { const float *w_sw, *w2, *b; } df_convp{};  // bound for the built df_order / df_pathway_kt (5, 5) only
+    bool fused_emb = false;  // df_conv1 + df_fc_emb run as one kernel (k_dwpw_gl); df_fc_emb's fp32 weight is not read then
+};
+
+struct NetWV1 {  // DeepFilterNet v1 (forward_v1)
+    Wb erb_conv0, df_conv0, df_fc_emb, erb_fc_emb, lsnr, df_fc_a, df_convp, conv0_out;
+    Blk erb_conv1, erb_conv2, erb_conv3, df_conv1, conv3p, conv2p, conv1p, conv0p, convt3, convt2, convt1;
+    std::vector<GruLayer> enc_gru, df_gru;  // one GroupedGRULayer each
+    struct { const float *w_t, *b, *w_hi, *w_lo; } df_fc_out{};  // w_hi / w_lo (BF16x3 GEMM) optional
+    const float *ones = nullptr, *zeros = nullptr;
+    const int *idx_c1 = nullptr, *idx_e3 = nullptr, *idx_shuf = nullptr, *idx_id = nullptr, *idx_dec = nullptr, *idx_gshuf = nullptr;
+};
+
 struct dfb_model {
     int device;
     dfb_model_config cfg;
-    std::map<std::string, std::pair<float *, int64_t>> t;  // device tensors
+    NetW net;      // model_kind 2 / 3
+    NetWV1 net1;   // model_kind 1
     std::map<std::string, std::pair<const float *, int64_t>> dbg;  // activations of the last forward
     float *slab = nullptr;
     long long *gru_dbg = nullptr;  // device buffer for dfb_debug_gru_timing, [gru_dbg_steps][8]
@@ -494,20 +524,101 @@ struct dfb_model {
                     ev_out = nullptr, ev_c0 = nullptr, ev_convp = nullptr, ev_skip = nullptr, ev_done = nullptr;
     } lanes[2];
     Arena arena1;                           // lane 1's activations (lane 0 uses `arena`)
-    const float *get(const std::string &n) const {
+};
+
+// Looks the uploaded tensors up by name.  The first missing or wrong-sized one (numel < 0: any size) becomes the bind's
+// error; lookups after it return null.
+struct Binder {
+    const std::map<std::string, std::pair<const float *, int64_t>> &t;
+    int rc = DFB_OK;
+    const float *opt(const std::string &n) const { auto it = t.find(n); return it == t.end() ? nullptr : it->second.first; }
+    const float *need(const std::string &n, int64_t numel) {
         auto it = t.find(n);
-        return it == t.end() ? nullptr : it->second.first;
+        if (!rc && it == t.end()) rc = fail(DFB_ERR_INVALID, "missing weight tensor '%s'", n.c_str());
+        if (!rc && numel >= 0 && it->second.second != numel)
+            rc = fail(DFB_ERR_INVALID, "weight tensor '%s' has %lld elements, expected %lld", n.c_str(), (long long)it->second.second, (long long)numel);
+        return rc ? nullptr : it->second.first;
+    }
+    Wb wb(const std::string &n, int64_t nw, int64_t nb) { return {need(n + ".w", nw), need(n + ".b", nb)}; }
+    PathW path(const std::string &n) { return {need(n + ".s", kCh), need(n + ".b", kCh)}; }
+    Blk blk(const std::string &n, int64_t n_dw, bool pw, bool pw_sw) {
+        return {need(n + ".dw", n_dw), pw ? need(n + ".pw", kCh * kCh) : nullptr, need(n + ".b", kCh), pw_sw ? need(n + ".pw_sw", kCh * kCh) : nullptr};
+    }
+    Gl gl(const std::string &n, int G, int I, int H, bool fp32 = true) {  // fp32 = false: only the tensor-core image is read
+        const float *img = opt(n + "_bx");
+        int gpc, hgp, stg;
+        return {fp32 ? need(n, (int64_t)I * H / G) : nullptr, img, G, I, H,
+                img && I % G == 0 && H % G == 0 && gl_bx_geometry(G, I / G, H / G, &gpc, &hgp, &stg)};
+    }
+    std::vector<GruLayer> gru(const std::string &n, int layers, int H) {  // every recurrence the forward passes run is H -> H
+        std::vector<GruLayer> v;
+        for (int l = 0; l < layers; l++) {
+            const std::string p = n + ".l" + std::to_string(l);
+            v.push_back({need(p + ".w_hh", (int64_t)3 * H * H), need(p + ".b_ih", 3 * H), need(p + ".b_hh", 3 * H),
+                         need(p + ".w_ih_hi", (int64_t)3 * H * H / 2), need(p + ".w_ih_lo", (int64_t)3 * H * H / 2)});
+        }
+        return v;
     }
 };
 
-static int need(const dfb_model *m, const char *name, int64_t numel, const float **out) {
-    auto it = m->t.find(name);
-    if (it == m->t.end()) return fail(DFB_ERR_INVALID, "missing weight tensor '%s'", name);
-    if (numel >= 0 && it->second.second != numel)
-        return fail(DFB_ERR_INVALID, "weight tensor '%s' has %lld elements, expected %lld", name,
-                    (long long)it->second.second, (long long)numel);
-    *out = it->second.first;
-    return DFB_OK;
+static int bind_net(const dfb_model_config &c, Binder &b, NetW &w) {
+    const int E = c.nb_erb, Fd = c.nb_df, H = c.emb_hidden, Hd = c.df_hidden, O2 = 2 * c.df_order;
+    const int ED = E / 4 * kCh, emb_in_dim = c.enc_concat ? 2 * ED : ED, emb_dim = c.model_kind == 2 ? H : ED;
+    w.erb_conv0 = b.wb("enc.erb_conv0", c.inp_kt * 3 * kCh, kCh); w.df_conv0 = b.wb("enc.df_conv0", c.inp_kt * 3 * 2 * kCh, kCh);
+    auto blk = [&](const char *n) { return b.blk(n, -1, false, true); };
+    w.erb_conv1 = blk("enc.erb_conv1"); w.erb_conv2 = blk("enc.erb_conv2"); w.erb_conv3 = blk("enc.erb_conv3"); w.df_conv1 = blk("enc.df_conv1");
+    w.convt3 = blk("erb_dec.convt3"); w.convt2 = blk("erb_dec.convt2"); w.convt1 = blk("erb_dec.convt1");
+    w.conv3p = b.path("erb_dec.conv3p"); w.conv2p = b.path("erb_dec.conv2p"); w.conv1p = b.path("erb_dec.conv1p"); w.conv0p = b.path("erb_dec.conv0p");
+    w.enc_in = b.gl("enc.emb_gru.in.gl", c.g_enc_in, emb_in_dim, H);
+    // df_conv1 + df_fc_emb run fused when df_fc_emb's shape is built and enc.emb_gru.in reads emb_in as BF16 planes (the
+    // FFMA grouped linear would read the fp32 tensor, which the fused kernel does not write); weights.py packs the
+    // tensor-core images of every such shape
+    const int I = Fd / 2 * kCh, G = c.g_df_fc_emb, Ge = c.g_enc_in;
+    int de_s, de_st, gpc, hgp, stg;
+    w.fused_emb = G > 0 && I % G == 0 && ED % G == 0 && df_emb_geometry(Fd, G, I / G, ED / G, c.conv_kt, &de_s, &de_st) &&
+                  Ge > 0 && emb_in_dim % Ge == 0 && H % Ge == 0 && gl_bx_geometry(Ge, emb_in_dim / Ge, H / Ge, &gpc, &hgp, &stg);
+    w.df_fc_emb = b.gl("enc.df_fc_emb.gl", G, I, ED, !w.fused_emb);
+    if (w.fused_emb && (!w.df_fc_emb.img || !w.enc_in.bx) && !b.rc)
+        b.rc = fail(DFB_ERR_INVALID, "df_fc_emb / enc.emb_gru.in: tensor-core weight images missing");
+    if (c.g_enc_out) w.enc_out = b.gl("enc.emb_gru.out.gl", c.g_enc_out, H, ED);
+    if (c.g_df_skip) w.df_skip = b.gl("df_dec.df_skip.gl", c.g_df_skip, emb_dim, Hd);
+    w.df_in = b.gl("df_dec.df_gru.in.gl", c.g_df_in, emb_dim, Hd);
+    w.df_out = b.gl("df_dec.df_out.gl", c.g_df_out, Hd, Fd * O2);
+    w.erb_in = b.gl("erb_dec.emb_gru.in.gl", c.g_erb_in, emb_dim, H);
+    w.erb_out = b.gl("erb_dec.emb_gru.out.gl", c.g_erb_out, H, ED);
+    w.enc_gru = b.gru("enc.emb_gru", c.enc_gru_layers, H); w.df_gru = b.gru("df_dec.df_gru", c.df_gru_layers, Hd);
+    w.erb_gru = b.gru("erb_dec.emb_gru", c.erb_gru_layers, H);
+    w.lsnr = b.wb("enc.lsnr", emb_dim, 1); w.conv0_out = b.wb("erb_dec.conv0_out", c.conv_kt * 3 * kCh, 1);
+    if (c.model_kind == 2) w.df_fc_a = b.wb("df_dec.df_fc_a", Hd, 1);
+    if (c.df_order == 5 && c.df_pathway_kt == 5)
+        w.df_convp = {b.need("df_dec.df_convp.w_sw", kCh * kCh), b.need("df_dec.df_convp.w2", O2 * O2), b.need("df_dec.df_convp.b", O2)};
+    return b.rc;
+}
+
+static int bind_v1(const dfb_model_config &c, Binder &b, NetWV1 &w) {
+    const int Fd = c.nb_df, H = c.emb_hidden, O2 = 2 * c.df_order, N = Fd * O2, kt = c.conv_kt;
+    w.ones = b.need("v1.ones", kCh); w.zeros = b.need("v1.zeros", kCh);
+    auto idx = [&](const char *n, int numel) { return reinterpret_cast<const int *>(b.need(n, numel)); };
+    w.idx_c1 = idx("v1.idx_c1", Fd / 2 * kCh); w.idx_e3 = idx("v1.idx_e3", H); w.idx_shuf = idx("v1.idx_shuf", H);
+    w.idx_id = idx("v1.idx_id", H); w.idx_dec = idx("v1.idx_dec", H); w.idx_gshuf = idx("v1.idx_gshuf", H);
+    // the tensor-core version of a block (pw_sw) is built for blocks without look-ahead whose transposed convs have one time tap
+    auto blk = [&](const char *n, int mode, int bkt, int la) { return b.blk(n, bkt * 3 * kCh, true, la == 0 && !(mode == DW_T2 && bkt != 1)); };
+    w.erb_conv1 = blk("enc.erb_conv1", DW_S2, kt, c.conv_lookahead > 1 ? 1 : 0); w.erb_conv2 = blk("enc.erb_conv2", DW_S2, kt, c.conv_lookahead > 2 ? 1 : 0);
+    w.erb_conv3 = blk("enc.erb_conv3", DW_S1, kt, 0); w.df_conv1 = blk("enc.df_conv1", DW_S2, kt, 0);
+    w.conv3p = blk("erb_dec.conv3p", DW_S1, 1, 0); w.conv2p = blk("erb_dec.conv2p", DW_S1, 1, 0);
+    w.conv1p = blk("erb_dec.conv1p", DW_S1, 1, 0); w.conv0p = blk("erb_dec.conv0p", DW_S1, 1, 0);
+    w.convt3 = blk("erb_dec.convt3", DW_S1, kt, 0); w.convt2 = blk("erb_dec.convt2", DW_T2, kt, 0); w.convt1 = blk("erb_dec.convt1", DW_T2, kt, 0);
+    w.erb_conv0 = b.wb("enc.erb_conv0", c.inp_kt * 3 * kCh, kCh); w.df_conv0 = b.wb("enc.df_conv0", c.inp_kt * 3 * 2 * kCh, kCh);
+    w.df_fc_emb = {b.need("enc.df_fc_emb.gl", (int64_t)Fd / 2 * kCh * H / c.g_df_fc_emb), b.need("enc.df_fc_emb.bias", H)};
+    w.erb_fc_emb = {b.need("erb_dec.fc_emb.gl", (int64_t)H * H / c.g_erb_in), b.need("erb_dec.fc_emb.bias", H)};
+    for (int l = 0; l < c.enc_gru_layers; l++) w.enc_gru.push_back(b.gru("enc.emb_gru.g" + std::to_string(l), 1, H)[0]);
+    for (int l = 0; l < c.df_gru_layers; l++) w.df_gru.push_back(b.gru("df_dec.df_gru.g" + std::to_string(l), 1, H)[0]);
+    w.lsnr = b.wb("enc.lsnr", H, 1); w.df_fc_a = b.wb("df_dec.df_fc_a", H, 1);
+    const bool planes = b.opt("df_dec.df_fc_out.w_hi");  // BF16x3 GEMM operand, else the FFMA grouped linear reads w_t
+    w.df_fc_out = {b.need("df_dec.df_fc_out.w_t", (int64_t)H * N), b.need("df_dec.df_fc_out.b", N),
+                   planes ? b.need("df_dec.df_fc_out.w_hi", (int64_t)H * N / 2) : nullptr, planes ? b.need("df_dec.df_fc_out.w_lo", (int64_t)H * N / 2) : nullptr};
+    w.df_convp = b.wb("df_dec.df_convp", kCh * O2, O2); w.conv0_out = b.wb("erb_dec.conv0_out", kt * 3 * kCh, 1);
+    return b.rc;
 }
 
 extern "C" int dfb_model_create(dfb_model **out, int device, const dfb_model_config *cfg, const dfb_tensor *tensors,
@@ -547,7 +658,7 @@ extern "C" int dfb_model_create(dfb_model **out, int device, const dfb_model_con
         return fail(DFB_ERR_OOM, "cudaMalloc(%zu) for weights failed", total);
     }
     size_t off = 0;
-    std::vector<float> tmp;
+    std::map<std::string, std::pair<const float *, int64_t>> t;
     for (int i = 0; i < n_tensors; i++) {
         const dfb_tensor &tt = tensors[i];
         if (!tt.name || !tt.data || tt.numel <= 0) { dfb_model_free(m); return fail(DFB_ERR_INVALID, "bad tensor %d", i); }
@@ -556,8 +667,13 @@ extern "C" int dfb_model_create(dfb_model **out, int device, const dfb_model_con
             dfb_model_free(m);
             return fail(DFB_ERR_CUDA, "weight upload failed");
         }
-        m->t[tt.name] = {dst, tt.numel};
+        t[tt.name] = {dst, tt.numel};
         off += ((size_t)tt.numel * 4 + 255) & ~size_t(255);
+    }
+    Binder b{t};
+    if ((rc = cfg->model_kind == 1 ? bind_v1(*cfg, b, m->net1) : bind_net(*cfg, b, m->net))) {
+        dfb_model_free(m);
+        return rc;
     }
     int prio_least = 0, prio_greatest = 0;
     cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest);
@@ -662,45 +778,35 @@ int run_gl(cudaStream_t s, const float *x, int64_t ldx, const float *w, const fl
     return DFB_OK;
 }
 
-// x [M, in_dim] -> multi-layer GRU -> y [M, H]  (uses xproj scratch [M,3H] and h ping-pong buffers)
+// x [M, H] -> multi-layer GRU -> y [M, H]  (uses xproj scratch [M,3H] and h ping-pong buffers)
 // x_hi/x_lo: BF16 planes of x (written by the producing grouped linear), pl_hi/pl_lo: scratch planes for the
 // inter-layer hidden state, the input of the next layer's projection GEMM.
-int run_gru(dfb_model *m, cudaStream_t s, const char *name, int layers, int H, int in_dim, const float *res_last, float *y,
+int run_gru(dfb_model *m, cudaStream_t s, const GruLayer *lw, int layers, int H, const float *res_last, float *y,
             float *xproj, int B, int T, const unsigned short *x_hi, const unsigned short *x_lo,
             unsigned short *pl_hi, unsigned short *pl_lo, int wide, unsigned short *out_hi, unsigned short *out_lo,
             bool *out_planes_ok, const GruChunk *ck) {
     if (out_planes_ok) *out_planes_ok = false;
-    if (!x_hi || !x_lo || !pl_hi || !pl_lo || in_dim % 64)
-        return fail(DFB_ERR_INVALID, "GRU '%s': input planes, scratch planes and an input width that is a multiple of 64 are required", name);
+    if (!x_hi || !x_lo || !pl_hi || !pl_lo) return fail(DFB_ERR_INVALID, "GRU: input planes and scratch planes are required");
     // time-chunked execution: the buffers hold T frames per stream, the recurrences run over frames [ck->t0, T) only and
     // continue from / leave behind the carried per-layer states; the projections simply cover every row
     const int t0 = ck ? ck->t0 : 0, Tn = T - t0;
     const int64_t M = (int64_t)B * T;
-    int cur_dim = in_dim;
     const unsigned short *cur_hi = x_hi, *cur_lo = x_lo;
     for (int l = 0; l < layers; l++) {
-        std::string base = std::string(name) + ".l" + std::to_string(l);
-        const float *w_hh, *b_ih, *b_hh, *w_hi, *w_lo;  // w_hi / w_lo: bf16 planes packed two per float
+        const GruLayer &g = lw[l];
         int rc;
-        if ((rc = need(m, (base + ".w_hh").c_str(), (int64_t)3 * H * H, &w_hh))) return rc;
-        if ((rc = need(m, (base + ".b_ih").c_str(), 3 * H, &b_ih))) return rc;
-        if ((rc = need(m, (base + ".b_hh").c_str(), 3 * H, &b_hh))) return rc;
-        if ((rc = need(m, (base + ".w_ih_hi").c_str(), (int64_t)3 * H * cur_dim / 2, &w_hi)) ||
-            (rc = need(m, (base + ".w_ih_lo").c_str(), (int64_t)3 * H * cur_dim / 2, &w_lo)))
-            return rc;
-        if ((rc = launch_gemm_bf16x3(s, cur_hi, cur_lo, cur_dim, w_hi, w_lo, b_ih, xproj, 3 * H, M, 3 * H, cur_dim))) return rc;
+        if ((rc = launch_gemm_bf16x3(s, cur_hi, cur_lo, H, g.w_ih_hi, g.w_ih_lo, g.b_ih, xproj, 3 * H, M, 3 * H, H))) return rc;
         const bool last = l == layers - 1;
         float *dst = last ? y : nullptr;   // a middle layer's output feeds only the next projection, which reads its planes
         float *hs = ck && ck->h ? ck->h + (int64_t)l * ck->Bs * H : nullptr;   // carried state of this layer [Bs][H], rows [0, B)
         GruWindow gw{ck && ck->have_state ? hs : nullptr, hs, t0, T, ck ? ck->first : nullptr, ck ? ck->w0 : 0};
         // the last layer's planes feed a grouped linear and include the residual; the others feed the next projection
         unsigned short *hi = last ? out_hi : pl_hi, *lo = last ? out_lo : pl_lo;
-        if ((rc = launch_gru_tc(s, xproj, w_hh, b_hh, last ? res_last : nullptr, dst, hi, lo, B, Tn,
+        if ((rc = launch_gru_tc(s, xproj, g.w_hh, g.b_hh, last ? res_last : nullptr, dst, hi, lo, B, Tn,
                                 Tn <= m->gru_dbg_steps ? m->gru_dbg : nullptr, wide, last ? 1 : 0, &gw, H)))
             return rc;
         if (last && hi && out_planes_ok) *out_planes_ok = true;
         cur_hi = pl_hi; cur_lo = pl_lo;
-        cur_dim = H;
         // middle layers may rewrite the scratch planes in place: the recurrence only reads xproj, which the
         // projection GEMM above has already produced from the previous contents of the planes.
     }
@@ -775,16 +881,6 @@ static size_t fwd_plan_v1(const dfb_model_config &c, size_t M, Arena *a, FwdBufs
 }
 
 // Carves the activations of `M` frames out of `a` (or only counts bytes when a == nullptr).
-// df_conv1 + df_fc_emb run as one kernel (k_dwpw_gl) for this configuration: df_fc_emb's shape is built and enc.emb_gru.in
-// runs on the tensor-core grouped linear (weights.py packs the tensor-core images of every such shape)
-static bool fused_emb_shape(const dfb_model_config &c) {
-    const int Fd = c.nb_df, ED = c.nb_erb / 4 * kCh, I = Fd / 2 * kCh, G = c.g_df_fc_emb, Ge = c.g_enc_in, H = c.emb_hidden;
-    const int emb_in_dim = c.enc_concat ? 2 * ED : ED;
-    int de_s, de_st, gpc, hgp, stg;
-    return c.model_kind != 1 && G > 0 && I % G == 0 && ED % G == 0 && df_emb_geometry(Fd, G, I / G, ED / G, c.conv_kt, &de_s, &de_st) &&
-           Ge > 0 && emb_in_dim % Ge == 0 && H % Ge == 0 && gl_bx_geometry(Ge, emb_in_dim / Ge, H / Ge, &gpc, &hgp, &stg);
-}
-
 static size_t fwd_plan(const dfb_model_config &c, size_t M, Arena *a, FwdBufs *f) {
     if (c.model_kind == 1 && !a) return fwd_plan_v1(c, M, nullptr, nullptr);
     const int E = c.nb_erb, Fd = c.nb_df, H = c.emb_hidden, Hd = c.df_hidden;
@@ -875,8 +971,9 @@ static int forward_impl(dfb_model *m, Arena &arena, const float *d_feat_erb, con
     const int rc = m->cfg.model_kind == 1
         ? forward_v1(m, arena, d_feat_erb, d_feat_spec, B, T, d_m, d_coefs, d_lsnr, d_alpha, s_in, cx)
         : forward_body(m, arena, d_feat_erb, d_feat_spec, B, T, d_m, d_coefs, d_lsnr, d_alpha, s_in, cx);
-    // an early return may leave work on the forked internal streams un-joined while the caller goes on to reuse
-    // the arena: drain the device before handing the error back (error path only)
+    // a failed launch or CUDA call, or a shape the built kernels do not cover, returns early and may leave work on the
+    // forked internal streams un-joined while the caller goes on to reuse the arena: drain the device before handing
+    // the error back (error path only)
     if (rc) cudaDeviceSynchronize();
     return rc;
 }
@@ -884,6 +981,7 @@ static int forward_impl(dfb_model *m, Arena &arena, const float *d_feat_erb, con
 static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, const float *d_feat_spec, int B, int T,
                         float *d_m, float *d_coefs, float *d_lsnr, float *d_alpha, cudaStream_t s_in, ChunkCtx *cx) {
     const dfb_model_config &c = m->cfg;
+    const NetW &w = m->net;
     const int Tsx = cx ? cx->Tsx : T, Tx = cx ? cx->Tx : T;
     const RaggedRow *rows = cx ? cx->rows : nullptr;
     const int64_t W0 = cx ? cx->W0 : 0;
@@ -929,27 +1027,16 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
     m->dbg["emb_in_hi"] = {reinterpret_cast<const float *>(f.embin_hi), M * emb_in_dim / 2};
     m->dbg["emb_in_lo"] = {reinterpret_cast<const float *>(f.embin_lo), M * emb_in_dim / 2};
     const int64_t e3_fs = c.enc_concat ? 2 * ED : ED;
-    // grouped linear `wname` ([G][I/G][Hh/G]) runs on the tensor-core kernel, which reads its input as BF16 planes only
-    auto gl_is_bx = [&](const char *wname, int G, int I, int Hh) -> bool {
-        int gpc, hgp, stg;
-        return G > 0 && I % G == 0 && Hh % G == 0 && m->get(std::string(wname) + "_bx") && gl_bx_geometry(G, I / G, Hh / G, &gpc, &hgp, &stg);
-    };
-    // df_conv1 + df_fc_emb run as one kernel (k_dwpw_gl, c1 stays on chip) when df_fc_emb's shape is built and enc.emb_gru.in
-    // reads emb_in as BF16 planes (the FFMA grouped linear would read the fp32 tensor, which the fused kernel does not write)
-    const float *emb_w = m->get("enc.df_fc_emb.gl_bx");
-    const bool fused_emb = fused_emb_shape(c);
-    if (fused_emb && (!emb_w || !gl_is_bx("enc.emb_gru.in.gl", c.g_enc_in, emb_in_dim, H)))
-        return fail(DFB_ERR_INVALID, "df_fc_emb / enc.emb_gru.in: tensor-core weight images missing");
     // fp32 activations that only feed the BF16 planes of a tensor-core consumer are not written (null): the input grouped
     // linears' g_a / g_a2 (DeepFilterNet2 adds them to the GRU output as a residual), the last-layer GRU outputs g_b (enc,
     // erb) and dfc (DeepFilterNet2's df_fc_a and skip read it); the GRUs' middle layers never write theirs (run_gru)
     const bool keep_ga = c.model_kind == 2;
-    float *const enc_ga = gl_is_bx("enc.emb_gru.in.gl", c.g_enc_in, emb_in_dim, H) ? nullptr : f.g_a;
-    float *const erb_ga = !keep_ga && gl_is_bx("erb_dec.emb_gru.in.gl", c.g_erb_in, emb_dim, H) ? nullptr : f.g_a;
-    float *const df_ga = !keep_ga && gl_is_bx("df_dec.df_gru.in.gl", c.g_df_in, emb_dim, Hd) ? nullptr : f.g_a2;
-    float *const enc_gb = c.g_enc_out && gl_is_bx("enc.emb_gru.out.gl", c.g_enc_out, H, ED) ? nullptr : f.g_b;
-    float *const erb_gb = gl_is_bx("erb_dec.emb_gru.out.gl", c.g_erb_out, H, ED) ? nullptr : f.g_b;
-    float *const dfc = c.model_kind != 2 && gl_is_bx("df_dec.df_out.gl", c.g_df_out, Hd, Fd * 2 * c.df_order) ? nullptr : f.dfc;
+    float *const enc_ga = w.enc_in.bx ? nullptr : f.g_a;
+    float *const erb_ga = !keep_ga && w.erb_in.bx ? nullptr : f.g_a;
+    float *const df_ga = !keep_ga && w.df_in.bx ? nullptr : f.g_a2;
+    float *const enc_gb = w.enc_out.bx ? nullptr : f.g_b;
+    float *const erb_gb = w.erb_out.bx ? nullptr : f.g_b;
+    float *const dfc = c.model_kind != 2 && w.df_out.bx ? nullptr : f.dfc;
     if (!erb_ga) m->dbg.erase("g_a");
     if (!erb_gb) m->dbg.erase("g_b");
     if (!dfc) m->dbg.erase("dfc");
@@ -967,156 +1054,126 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         if (!r) pl.ok = true;
         return r;
     };
-    // grouped linear `wname` ([G][I/G][Hh/G]): the BF16x3 tensor-core kernel when the shape is built, else the FFMA
-    // kernel.  xin: planes of x (converted on demand); yout (optional): planes of y to produce,
+    // grouped linear `g`: the BF16x3 tensor-core kernel when g.bx, else (or when that kernel cannot take the launch) the
+    // FFMA kernel.  xin: planes of x (converted on demand); yout (optional): planes of y to produce,
     // ycol: column offset of y inside its plane buffer.  x / y may be null (fp32 form not written / not wanted) only where
-    // gl_is_bx holds: the FFMA kernel needs both, and a launch that cannot run without them is an error.
-    auto gl = [&](cudaStream_t st, const char *wname, const float *x, int64_t ldx, Pl *xin, int G, int I, int Hh, int act,
+    // g.bx holds: the FFMA kernel needs both, and a launch that cannot run without them is an error.
+    auto gl = [&](cudaStream_t st, const Gl &g, const float *x, int64_t ldx, Pl *xin, int act,
                   const float *res, int64_t ldr, float *y, int64_t ldy, Pl *yout, int64_t ycol = 0) -> int {
-        const float *w;
         int r;
-        if ((r = need(m, wname, (int64_t)I * Hh / G, &w))) return r;
         unsigned short *yh = yout ? yout->hi + ycol : nullptr, *yl = yout ? yout->lo + ycol : nullptr;
-        const std::string bx = std::string(wname) + "_bx";
-        int gpc, hgp, stages;
-        if (xin && m->get(bx) && gl_bx_geometry(G, I / G, Hh / G, &gpc, &hgp, &stages)) {
-            if ((r = ensure_planes(st, x, ldx, I, *xin))) return r;
-            r = launch_gl_bx(st, xin->hi, xin->lo, xin->ld, m->get(bx), res, ldr, y, ldy, yh, yl, yout ? yout->ld : 0, M, G, I / G,
-                             Hh / G, act, 1.f, 0.f);
+        if (xin && g.bx) {
+            if ((r = ensure_planes(st, x, ldx, g.I, *xin))) return r;
+            r = launch_gl_bx(st, xin->hi, xin->lo, xin->ld, g.img, res, ldr, y, ldy, yh, yl, yout ? yout->ld : 0, M, g.G, g.I / g.G,
+                             g.H / g.G, act, 1.f, 0.f);
             if (r != DFB_ERR_UNSUPPORTED) {
                 if (!r && yout) yout->ok = true;
                 return r;
             }
         }
         if (!x || !y)
-            return fail(DFB_ERR_UNSUPPORTED, "grouped linear '%s': the tensor-core kernel cannot take this launch and the fp32 %s "
-                        "the FFMA kernel needs is not written", wname, x ? "output" : "input");
+            return fail(DFB_ERR_UNSUPPORTED, "grouped linear %dx%d/%d: the tensor-core kernel cannot take this launch and the fp32 %s "
+                        "the FFMA kernel needs is not written", g.I, g.H, g.G, x ? "output" : "input");
         // NB: the FFMA kernel's plane output shares y's pitch, so it can only serve plane buffers with ld == ldy
         const bool ffma_planes = yout && yout->ld == ldy;
-        r = run_gl(st, x, ldx, w, nullptr, res, ldr, y, ldy, M, G, I, Hh, act, 1.f, 0.f, ffma_planes ? yh : nullptr, ffma_planes ? yl : nullptr);
+        r = run_gl(st, x, ldx, g.w, nullptr, res, ldr, y, ldy, M, g.G, g.I, g.H, act, 1.f, 0.f, ffma_planes ? yh : nullptr, ffma_planes ? yl : nullptr);
         if (!r && yout) yout->ok = ffma_planes;
         return r;
     };
 
     // ---- encoder (deepfilternet3.py:166-185)
     {
-        const float *w, *bb;
-        if ((rc = need(m, "enc.erb_conv0.w", c.inp_kt * 3 * kCh, &w)) || (rc = need(m, "enc.erb_conv0.b", kCh, &bb))) return rc;
         dim3 grid((unsigned)((T + kInFrames - 1) / kInFrames), (unsigned)B);
         int smem = (kInFrames + c.inp_kt - 1) * (E + 2) * 4;
         DFB_PROF("k_conv_in[erb_conv0]", s);
-        k_conv_in<1><<<grid, 256, smem, s>>>(d_feat_erb, w, bb, f.e0, T, E, c.inp_kt, c.conv_lookahead, Tsx, Tx, 0, rows, W0, first);
+        k_conv_in<1><<<grid, 256, smem, s>>>(d_feat_erb, w.erb_conv0.w, w.erb_conv0.b, f.e0, T, E, c.inp_kt, c.conv_lookahead, Tsx, Tx, 0, rows, W0, first);
         DFB_LAUNCH_CHECK();
     }
-    const float *pw_sw = nullptr;  // set by blk(): swizzled BF16 hi | lo image of the [C_out][C_in] 1x1 weights
-    auto blk = [&](const char *name, DwPwParams &p) -> int {
-        std::string n(name);
-        int r;
-        if ((r = need(m, (n + ".dw").c_str(), -1, &p.dw)) || (r = need(m, (n + ".b").c_str(), kCh, &p.bias)) ||
-            (r = need(m, (n + ".pw_sw").c_str(), kCh * kCh, &pw_sw)))
-            return r;
-        return DFB_OK;
-    };
     // the DF-branch input convs run concurrently with the ERB-branch convs
     cudaStream_t sa = serial ? s : L.aux;
     DFB_CUDA(cudaEventRecord(L.ev_fork_enc, s));
     DFB_CUDA(cudaStreamWaitEvent(sa, L.ev_fork_enc, 0));
-    auto mk = [&](const float *in, int Fin, int64_t in_fs, float *out, int Fout, int64_t out_fs, int kt) {
+    // separable block k; its tensor-core kernel reads k.pw_sw, the swizzled BF16 hi | lo image of the [C_out][C_in] 1x1 weights
+    auto mk = [&](const Blk &k, const float *in, int Fin, int64_t in_fs, float *out, int Fout, int64_t out_fs, int kt) {
         DwPwParams p{};
         p.in = in; p.Fin = Fin; p.in_fs = in_fs; p.out = out; p.Fout = Fout; p.out_fs = out_fs; p.kt = kt; p.T = T;
         p.lookahead = 0;
-        p.first = first; p.w0 = W0;
+        p.first = first; p.w0 = W0; p.dw = k.dw; p.bias = k.b;
         return p;
     };
     {
-        DwPwParams p{};
         {
-            const float *w, *bb;
-            if ((rc = need(m, "enc.df_conv0.w", c.inp_kt * 3 * 2 * kCh, &w)) || (rc = need(m, "enc.df_conv0.b", kCh, &bb))) return rc;
             dim3 grid((unsigned)((T + kInFrames - 1) / kInFrames), (unsigned)B);
             int smem = (kInFrames + c.inp_kt - 1) * (Fd + 2) * 2 * 4;
             DFB_PROF("k_conv_in[df_conv0]", sa);
-            k_conv_in<2><<<grid, 256, smem, sa>>>(d_feat_spec, w, bb, f.c0, T, Fd, c.inp_kt, c.conv_lookahead, Tsx, Tx, 0, rows, W0, first);
+            k_conv_in<2><<<grid, 256, smem, sa>>>(d_feat_spec, w.df_conv0.w, w.df_conv0.b, f.c0, T, Fd, c.inp_kt, c.conv_lookahead, Tsx, Tx, 0, rows, W0, first);
             DFB_LAUNCH_CHECK();
             DFB_CUDA(cudaEventRecord(L.ev_c0, sa));
         }
         m->dbg.erase("c1");
-        if (!fused_emb) {
-            p = mk(f.c0, Fd, (int64_t)Fd * kCh, f.c1, Fd / 2, (int64_t)Fd / 2 * kCh, c.conv_kt);
-            if ((rc = blk("enc.df_conv1", p))) return rc;
+        if (!w.fused_emb) {
+            DwPwParams p = mk(w.df_conv1, f.c0, Fd, (int64_t)Fd * kCh, f.c1, Fd / 2, (int64_t)Fd / 2 * kCh, c.conv_kt);
             // c1 only feeds df_fc_emb: write its BF16 planes instead of the fp32 tensor
             p.out = nullptr; p.out_hi = pl_c1.hi; p.out_lo = pl_c1.lo; pl_c1.ok = true;
-            if ((rc = run_dwpw<DW_S2>(sa, p, B, pw_sw))) return rc;
+            if ((rc = run_dwpw<DW_S2>(sa, p, B, w.df_conv1.pw_sw))) return rc;
         }
         DFB_CUDA(cudaEventRecord(L.ev_join_enc, sa));
         // DF pathway conv (needs c0 only; its result is consumed by the very last DF-decoder kernel): on the
         // low-priority stream, so its CTAs only take SMs that the critical path -- the encoder convs now, the GRU
         // clusters later -- leaves idle (on the DF branch's own streams it delays df_fc_emb, which is on the critical path)
         DFB_CUDA(cudaStreamWaitEvent(sl, L.ev_c0, 0));
-        const int O2 = 2 * c.df_order;
         if (c.df_order != 5 || c.df_pathway_kt != 5)
             return fail(DFB_ERR_UNSUPPORTED, "df_order %d / df_pathway_kernel_size_t %d (built kernels: 5, 5)", c.df_order,
                         c.df_pathway_kt);
         if (Fd % 2) return fail(DFB_ERR_UNSUPPORTED, "df pathway conv: odd nb_df");
-        const float *w_sw, *w2, *bb;
-        if ((rc = need(m, "df_dec.df_convp.w_sw", kCh * kCh, &w_sw)) || (rc = need(m, "df_dec.df_convp.w2", O2 * O2, &w2)) ||
-            (rc = need(m, "df_dec.df_convp.b", O2, &bb)))
-            return rc;
         // channel contraction on the tensor cores (BF16x3), shifted adds + 1x1 conv in the epilogue
-        if ((rc = launch_df_convp_tc(sl, f.c0, w_sw, w2, bb, d_coefs, B, T, Fd, first, W0))) return rc;
+        if ((rc = launch_df_convp_tc(sl, f.c0, w.df_convp.w_sw, w.df_convp.w2, w.df_convp.b, d_coefs, B, T, Fd, first, W0))) return rc;
         DFB_CUDA(cudaEventRecord(L.ev_convp, sl));
     }
     {
-        DwPwParams p = mk(f.e0, E, (int64_t)E * kCh, f.e1, E / 2, (int64_t)E / 2 * kCh, c.conv_kt);
-        if ((rc = blk("enc.erb_conv1", p)) || (rc = run_dwpw<DW_S2>(s, p, B, pw_sw))) return rc;
-        p = mk(f.e1, E / 2, (int64_t)E / 2 * kCh, f.e2, E / 4, (int64_t)E / 4 * kCh, c.conv_kt);
-        if ((rc = blk("enc.erb_conv2", p)) || (rc = run_dwpw<DW_S2>(s, p, B, pw_sw))) return rc;
-        p = mk(f.e2, E / 4, (int64_t)E / 4 * kCh, f.e3, E / 4, e3_fs, c.conv_kt);
-        if ((rc = blk("enc.erb_conv3", p))) return rc;
+        DwPwParams p = mk(w.erb_conv1, f.e0, E, (int64_t)E * kCh, f.e1, E / 2, (int64_t)E / 2 * kCh, c.conv_kt);
+        if ((rc = run_dwpw<DW_S2>(s, p, B, w.erb_conv1.pw_sw))) return rc;
+        p = mk(w.erb_conv2, f.e1, E / 2, (int64_t)E / 2 * kCh, f.e2, E / 4, (int64_t)E / 4 * kCh, c.conv_kt);
+        if ((rc = run_dwpw<DW_S2>(s, p, B, w.erb_conv2.pw_sw))) return rc;
+        p = mk(w.erb_conv3, f.e2, E / 4, (int64_t)E / 4 * kCh, f.e3, E / 4, e3_fs, c.conv_kt);
         if (c.enc_concat) { p.out_hi = pl_embin.hi; p.out_lo = pl_embin.lo; }  // DFN2: e3 is the first half of emb_in
-        if ((rc = run_dwpw<DW_S1>(s, p, B, pw_sw))) return rc;
+        if ((rc = run_dwpw<DW_S1>(s, p, B, w.erb_conv3.pw_sw))) return rc;
 
     }
     DFB_CUDA(cudaStreamWaitEvent(s, L.ev_join_enc, 0));  // c0 (and, unfused, c1's planes) ready
     {
         // cemb = relu(df_fc_emb(c1 flat)); emb_in = e3 flat + cemb  (DFN2: concat)
         const int I = Fd / 2 * kCh;
-        if (fused_emb) {  // only emb_in's planes are written: enc.emb_gru.in reads nothing else
-            DwPwParams p{};
-            if ((rc = blk("enc.df_conv1", p))) return rc;
+        if (w.fused_emb) {  // only emb_in's planes are written: enc.emb_gru.in reads nothing else
             const int G = c.g_df_fc_emb;
-            rc = launch_df_emb(s, f.c0, M, T, Fd, c.conv_kt, p.dw, p.bias, pw_sw, emb_w, G, I / G, ED / G, c.enc_concat ? nullptr : f.e3,
-                               ED, pl_embin.hi + (c.enc_concat ? ED : 0), pl_embin.lo + (c.enc_concat ? ED : 0), pl_embin.ld, first, W0);
+            rc = launch_df_emb(s, f.c0, M, T, Fd, c.conv_kt, w.df_conv1.dw, w.df_conv1.b, w.df_conv1.pw_sw, w.df_fc_emb.img, G, I / G, ED / G,
+                               c.enc_concat ? nullptr : f.e3, ED, pl_embin.hi + (c.enc_concat ? ED : 0), pl_embin.lo + (c.enc_concat ? ED : 0),
+                               pl_embin.ld, first, W0);
             if (!rc) pl_embin.ok = true;
             m->dbg.erase("emb_in");
         } else if (c.enc_concat) {  // the first half's planes were written by erb_conv3
-            rc = gl(s, "enc.df_fc_emb.gl", f.c1, I, &pl_c1, c.g_df_fc_emb, I, ED, ACT_RELU, nullptr, 0, f.emb_in + ED, emb_in_dim,
-                    &pl_embin, ED);
+            rc = gl(s, w.df_fc_emb, f.c1, I, &pl_c1, ACT_RELU, nullptr, 0, f.emb_in + ED, emb_in_dim, &pl_embin, ED);
         } else {
-            rc = gl(s, "enc.df_fc_emb.gl", f.c1, I, &pl_c1, c.g_df_fc_emb, I, ED, ACT_RELU, f.e3, ED, f.emb_in, emb_in_dim, &pl_embin);
+            rc = gl(s, w.df_fc_emb, f.c1, I, &pl_c1, ACT_RELU, f.e3, ED, f.emb_in, emb_in_dim, &pl_embin);
         }
         if (rc) return rc;
     }
     {
         // enc.emb_gru: linear_in + ReLU -> GRU -> [linear_out + ReLU]
-        if ((rc = gl(s, "enc.emb_gru.in.gl", fused_emb ? nullptr : f.emb_in, emb_in_dim, &pl_embin, c.g_enc_in, emb_in_dim, H, ACT_RELU,
-                     nullptr, 0, enc_ga, H,
-                     &pl_ga))) return rc;
+        if ((rc = gl(s, w.enc_in, w.fused_emb ? nullptr : f.emb_in, emb_in_dim, &pl_embin, ACT_RELU, nullptr, 0, enc_ga, H, &pl_ga)))
+            return rc;
         float *gout = c.g_enc_out ? enc_gb : f.emb;
         Pl &pl_gout = c.g_enc_out ? pl_gb : pl_emb;
-        if ((rc = run_gru(m, s, "enc.emb_gru", c.enc_gru_layers, H, H, nullptr, gout, f.xproj, B, T, f.ga_hi, f.ga_lo,
+        if ((rc = run_gru(m, s, w.enc_gru.data(), c.enc_gru_layers, H, nullptr, gout, f.xproj, B, T, f.ga_hi, f.ga_lo,
                           f.gh_hi, f.gh_lo, 0, pl_gout.hi, pl_gout.lo, &pl_gout.ok, cx ? &ck_enc : nullptr))) return rc;
         if (c.g_enc_out) {
-            if ((rc = gl(s, "enc.emb_gru.out.gl", enc_gb, H, &pl_gb, c.g_enc_out, H, ED, ACT_RELU, nullptr, 0, f.emb, emb_dim, &pl_emb)))
-                return rc;
+            if ((rc = gl(s, w.enc_out, enc_gb, H, &pl_gb, ACT_RELU, nullptr, 0, f.emb, emb_dim, &pl_emb))) return rc;
         }
         // the decoders read emb's planes on two streams: make sure they exist before the fork
         if ((rc = ensure_planes(s, f.emb, emb_dim, emb_dim, pl_emb))) return rc;
-        if (d_lsnr) {
-            const float *lw, *lb;
-            if ((rc = need(m, "enc.lsnr.w", emb_dim, &lw)) || (rc = need(m, "enc.lsnr.b", 1, &lb))) return rc;
-            if ((rc = run_gl(s, f.emb, emb_dim, lw, lb, nullptr, 0, d_lsnr, 1, M, 1, emb_dim, 1, ACT_SIGMOID, c.lsnr_scale, c.lsnr_offset))) return rc;
-        }
+        if (d_lsnr && (rc = run_gl(s, f.emb, emb_dim, w.lsnr.w, w.lsnr.b, nullptr, 0, d_lsnr, 1, M, 1, emb_dim, 1, ACT_SIGMOID, c.lsnr_scale,
+                                   c.lsnr_offset)))
+            return rc;
     }
     // fork: the two decoders only share read-only encoder outputs
     // the encoder phase is done (ev_fork also tells the next time chunk that it may start); the decoder phase runs on the
@@ -1138,47 +1195,38 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
     const int wide_erb = wide_env && (!strcmp(wide_env, "erb") || !strcmp(wide_env, "both"));
     const bool early_skip = c.g_df_skip && c.model_kind != 2;
     if (early_skip) {
-        if ((rc = gl(s, "df_dec.df_skip.gl", f.emb, emb_dim, &pl_emb, c.g_df_skip, emb_dim, Hd, ACT_NONE, nullptr, 0, f.dfskip, Hd, nullptr)))
-            return rc;
+        if ((rc = gl(s, w.df_skip, f.emb, emb_dim, &pl_emb, ACT_NONE, nullptr, 0, f.dfskip, Hd, nullptr))) return rc;
         DFB_CUDA(cudaEventRecord(L.ev_skip, s));
     }
     // ---- DF decoder (deepfilternet3.py:323-331), on the auxiliary stream (forked after the encoder)
     {
         cudaStream_t s = sa;  // shadows the caller stream inside this block
-        if ((rc = gl(s, "df_dec.df_gru.in.gl", f.emb, emb_dim, &pl_emb, c.g_df_in, emb_dim, Hd, ACT_RELU, nullptr, 0, df_ga, Hd, &pl_ga2)))
-            return rc;
+        if ((rc = gl(s, w.df_in, f.emb, emb_dim, &pl_emb, ACT_RELU, nullptr, 0, df_ga, Hd, &pl_ga2))) return rc;
         const float *res = c.model_kind == 2 ? f.g_a2 : (early_skip ? f.dfskip : nullptr);
         if (early_skip) DFB_CUDA(cudaStreamWaitEvent(s, L.ev_skip, 0));
-        if ((rc = run_gru(m, s, "df_dec.df_gru", c.df_gru_layers, Hd, Hd, res, dfc, f.xproj2, B, T, f.ga2_hi, f.ga2_lo,
+        if ((rc = run_gru(m, s, w.df_gru.data(), c.df_gru_layers, Hd, res, dfc, f.xproj2, B, T, f.ga2_hi, f.ga2_lo,
                           f.gh2_hi, f.gh2_lo, wide_df, pl_dfc.hi, pl_dfc.lo, &pl_dfc.ok, cx ? &ck_df : nullptr))) return rc;
         if (c.g_df_skip && !early_skip) {
-            if ((rc = gl(s, "df_dec.df_skip.gl", f.emb, emb_dim, &pl_emb, c.g_df_skip, emb_dim, Hd, ACT_NONE, f.dfc, Hd, f.dfc, Hd, nullptr)))
-                return rc;
+            if ((rc = gl(s, w.df_skip, f.emb, emb_dim, &pl_emb, ACT_NONE, f.dfc, Hd, f.dfc, Hd, nullptr))) return rc;
             pl_dfc.ok = false;
         }
-        if (d_alpha && c.model_kind == 2) {  // alpha = sigmoid(df_fc_a(c)), deepfilternet2.py:368
-            const float *aw, *ab;
-            if ((rc = need(m, "df_dec.df_fc_a.w", Hd, &aw)) || (rc = need(m, "df_dec.df_fc_a.b", 1, &ab))) return rc;
-            if ((rc = run_gl(s, f.dfc, Hd, aw, ab, nullptr, 0, d_alpha, 1, M, 1, Hd, 1, ACT_SIGMOID))) return rc;
-        }
+        if (d_alpha && c.model_kind == 2 &&  // alpha = sigmoid(df_fc_a(c)), deepfilternet2.py:368
+            (rc = run_gl(s, f.dfc, Hd, w.df_fc_a.w, w.df_fc_a.b, nullptr, 0, d_alpha, 1, M, 1, Hd, 1, ACT_SIGMOID))) return rc;
         const int O2 = 2 * c.df_order;
         // coefs = tanh(df_out(c)) + df_convp(c0); the pathway term was written by k_df_convp_tc on the low-priority stream
         DFB_CUDA(cudaStreamWaitEvent(s, L.ev_convp, 0));
-        if ((rc = gl(s, "df_dec.df_out.gl", dfc, Hd, &pl_dfc, c.g_df_out, Hd, Fd * O2, ACT_TANH, d_coefs, (int64_t)Fd * O2, d_coefs,
-                     (int64_t)Fd * O2, nullptr))) return rc;
+        if ((rc = gl(s, w.df_out, dfc, Hd, &pl_dfc, ACT_TANH, d_coefs, (int64_t)Fd * O2, d_coefs, (int64_t)Fd * O2, nullptr))) return rc;
     }
     DFB_CUDA(cudaEventRecord(L.ev_join, sa));
     // ---- ERB decoder (deepfilternet3.py:245-254)
     {
-        if ((rc = gl(s, "erb_dec.emb_gru.in.gl", f.emb, emb_dim, &pl_emb, c.g_erb_in, emb_dim, H, ACT_RELU, nullptr, 0, erb_ga, H, &pl_ga)))
-            return rc;
+        if ((rc = gl(s, w.erb_in, f.emb, emb_dim, &pl_emb, ACT_RELU, nullptr, 0, erb_ga, H, &pl_ga))) return rc;
         // DFN2 (SqueezedGRU): identity skip around the GRU, y = GRU(x) + x  (modules.py:695-697)
         const float *res = c.model_kind == 2 ? f.g_a : nullptr;
         pl_gb.ok = false;
-        if ((rc = run_gru(m, s, "erb_dec.emb_gru", c.erb_gru_layers, H, H, res, erb_gb, f.xproj, B, T, f.ga_hi, f.ga_lo,
+        if ((rc = run_gru(m, s, w.erb_gru.data(), c.erb_gru_layers, H, res, erb_gb, f.xproj, B, T, f.ga_hi, f.ga_lo,
                           f.gh_hi, f.gh_lo, wide_erb, pl_gb.hi, pl_gb.lo, &pl_gb.ok, cx ? &ck_erb : nullptr))) return rc;
-        if ((rc = gl(s, "erb_dec.emb_gru.out.gl", erb_gb, H, &pl_gb, c.g_erb_out, H, ED, ACT_RELU, nullptr, 0, f.dec_emb, ED, nullptr)))
-            return rc;
+        if ((rc = gl(s, w.erb_out, erb_gb, H, &pl_gb, ACT_RELU, nullptr, 0, f.dec_emb, ED, nullptr))) return rc;
         if (cx && cx->dec_tail && c.conv_kt > 1) {
             // kt = 2 decoder convs look one frame back into the halo, where this window's recurrence did not run: restore
             // dec_emb there from the previous chunk, then keep this window's last frames for the next one
@@ -1192,31 +1240,22 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
                                        fb * ns, B, cudaMemcpyDeviceToDevice, s));
             cx->dec_tail_n = ns;
         }
-        auto path = [&](DwPwParams &p, const char *pn, const float *pt, int64_t pfs) -> int {
-            std::string n(pn);
-            p.path = pt; p.path_fs = pfs;
-            int r;
-            if ((r = need(m, (n + ".s").c_str(), kCh, &p.ps)) || (r = need(m, (n + ".b").c_str(), kCh, &p.pb))) return r;
-            return DFB_OK;
-        };
-        DwPwParams p = mk(f.dec_emb, E / 4, ED, f.d3, E / 4, ED, c.conv_kt);
-        if ((rc = blk("erb_dec.convt3", p)) || (rc = path(p, "erb_dec.conv3p", f.e3, e3_fs)) || (rc = run_dwpw<DW_S1>(s, p, B, pw_sw))) return rc;
-        p = mk(f.d3, E / 4, ED, f.d2, E / 2, (int64_t)E / 2 * kCh, 1);
-        if ((rc = blk("erb_dec.convt2", p)) || (rc = path(p, "erb_dec.conv2p", f.e2, (int64_t)E / 4 * kCh)) || (rc = run_dwpw<DW_T2>(s, p, B, pw_sw))) return rc;
-        const float *ps, *pb, *w, *bb;
-        if ((rc = need(m, "erb_dec.conv0p.s", kCh, &ps)) || (rc = need(m, "erb_dec.conv0p.b", kCh, &pb)) ||
-            (rc = need(m, "erb_dec.conv0_out.w", c.conv_kt * 3 * kCh, &w)) || (rc = need(m, "erb_dec.conv0_out.b", 1, &bb)))
-            return rc;
-        p = mk(f.d2, E / 2, (int64_t)E / 2 * kCh, f.d1, E, (int64_t)E * kCh, 1);
-        if ((rc = blk("erb_dec.convt1", p)) || (rc = path(p, "erb_dec.conv1p", f.e1, (int64_t)E / 2 * kCh))) return rc;
+        DwPwParams p = mk(w.convt3, f.dec_emb, E / 4, ED, f.d3, E / 4, ED, c.conv_kt);
+        p.path = f.e3; p.path_fs = e3_fs; p.ps = w.conv3p.s; p.pb = w.conv3p.b;
+        if ((rc = run_dwpw<DW_S1>(s, p, B, w.convt3.pw_sw))) return rc;
+        p = mk(w.convt2, f.d3, E / 4, ED, f.d2, E / 2, (int64_t)E / 2 * kCh, 1);
+        p.path = f.e2; p.path_fs = (int64_t)E / 4 * kCh; p.ps = w.conv2p.s; p.pb = w.conv2p.b;
+        if ((rc = run_dwpw<DW_T2>(s, p, B, w.convt2.pw_sw))) return rc;
+        p = mk(w.convt1, f.d2, E / 2, (int64_t)E / 2 * kCh, f.d1, E, (int64_t)E * kCh, 1);
+        p.path = f.e1; p.path_fs = (int64_t)E / 2 * kCh; p.ps = w.conv1p.s; p.pb = w.conv1p.b;
         // kt = 1 models: the mask head is evaluated in convt1's epilogue and d1 never leaves the SM
         const bool fused_mask = c.conv_kt == 1 && 128 % E == 0;
         if (fused_mask) {
-            p.mk_e0 = f.e0; p.mk_ps = ps; p.mk_pb = pb; p.mk_w = w; p.mk_bias = bb; p.mk_out = d_m;
+            p.mk_e0 = f.e0; p.mk_ps = w.conv0p.s; p.mk_pb = w.conv0p.b; p.mk_w = w.conv0_out.w; p.mk_bias = w.conv0_out.b; p.mk_out = d_m;
             p.out = nullptr;
             m->dbg.erase("d1");
         }
-        if ((rc = run_dwpw<DW_T2>(s, p, B, pw_sw))) return rc;
+        if ((rc = run_dwpw<DW_T2>(s, p, B, w.convt1.pw_sw))) return rc;
         if (fused_mask) return finish();
         static PerDeviceOnce attr_once;
         int smem = (kMaskWarps * 2 * (E + 2) * kMaskLd + c.conv_kt * 3 * kCh) * 4;
@@ -1227,7 +1266,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         int per_cta = kMaskWarps * kMaskChunk;
         dim3 grid((unsigned)((T + per_cta - 1) / per_cta), (unsigned)B);
         DFB_PROF("k_mask_out", s);
-        k_mask_out<<<grid, 32 * kMaskWarps, smem, s>>>(f.e0, f.d1, ps, pb, w, bb, d_m, T, E, c.conv_kt, first, W0);
+        k_mask_out<<<grid, 32 * kMaskWarps, smem, s>>>(f.e0, f.d1, w.conv0p.s, w.conv0p.b, w.conv0_out.w, w.conv0_out.b, d_m, T, E, c.conv_kt, first, W0);
         DFB_LAUNCH_CHECK();
     }
     return finish();
@@ -1250,6 +1289,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
 static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const float *d_feat_spec, int B, int T,
                       float *d_m, float *d_coefs, float *d_lsnr, float *d_alpha, cudaStream_t s_in, ChunkCtx *cx) {
     const dfb_model_config &c = m->cfg;
+    const NetWV1 &w = m->net1;
     if (cx && (cx->Rc != 0 || cx->have_state)) return fail(DFB_ERR_UNSUPPORTED, "DeepFilterNet v1 runs as one window per signal");
     const int Tsx = cx ? cx->Tsx : T, Tx = cx ? cx->Tx : T;
     static const bool serial = getenv("DFB_SERIAL") && atoi(getenv("DFB_SERIAL"));
@@ -1271,18 +1311,6 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
     m->dbg["cemb"] = {f.cemb, M * H}; m->dbg["emb_in"] = {f.emb, M * H}; m->dbg["emb"] = {f.embo, M * H};
     m->dbg["dec_emb"] = {f.dec, M * H}; m->dbg["d3"] = {f.d3, M * (E / 4) * kCh}; m->dbg["d2"] = {f.d2, M * (E / 2) * kCh};
     m->dbg["d1"] = {f.d1, M * E * kCh}; m->dbg["dfc"] = {f.dfc, M * H}; m->dbg["y0"] = {f.y[0], M * H};
-    const float *ones, *zeros;
-    if ((rc = need(m, "v1.ones", kCh, &ones)) || (rc = need(m, "v1.zeros", kCh, &zeros))) return rc;
-    auto table = [&](const char *name, int n, const int **out) -> int {
-        const float *t;
-        int r = need(m, name, n, &t);
-        *out = reinterpret_cast<const int *>(t);
-        return r;
-    };
-    const int *idx_c1, *idx_e3, *idx_shuf, *idx_id, *idx_dec, *idx_gshuf;
-    if ((rc = table("v1.idx_c1", Fd / 2 * kCh, &idx_c1)) || (rc = table("v1.idx_e3", H, &idx_e3)) || (rc = table("v1.idx_shuf", H, &idx_shuf)) ||
-        (rc = table("v1.idx_id", H, &idx_id)) || (rc = table("v1.idx_dec", H, &idx_dec)) || (rc = table("v1.idx_gshuf", H, &idx_gshuf)))
-        return rc;
     auto gather = [&](cudaStream_t st, int n, const float *const *src, const int64_t *ld, const int *const *idx, int K, int relu,
                       float *out, unsigned short *hi, unsigned short *lo) -> int {
         GatherParams g{};
@@ -1293,139 +1321,109 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
         DFB_LAUNCH_CHECK();
         return DFB_OK;
     };
-    // separable block `name`: depthwise (kt x 3, look-ahead la) -> 1x1 -> BN -> ReLU, input = in (+ path)
-    auto block = [&](cudaStream_t st, const char *name, int mode, const float *in, int Fin, float *out, int Fout, int bkt, int la,
+    // separable block k: depthwise (kt x 3, look-ahead la) -> 1x1 -> BN -> ReLU, input = in (+ path); on the tensor-core
+    // kernel where k.pw_sw is bound
+    auto block = [&](cudaStream_t st, const Blk &k, int mode, const float *in, int Fin, float *out, int Fout, int bkt, int la,
                      const float *path) -> int {
         DwPwParams p{};
-        std::string n(name);
-        int r;
-        if ((r = need(m, (n + ".dw").c_str(), bkt * 3 * kCh, &p.dw)) || (r = need(m, (n + ".pw").c_str(), kCh * kCh, &p.pw)) ||
-            (r = need(m, (n + ".b").c_str(), kCh, &p.bias)))
-            return r;
-        p.in = in; p.Fin = Fin; p.in_fs = (int64_t)Fin * kCh; p.out = out; p.Fout = Fout; p.out_fs = (int64_t)Fout * kCh; p.kt = bkt; p.T = T;
+        p.dw = k.dw; p.pw = k.pw; p.bias = k.b; p.in = in; p.Fin = Fin; p.in_fs = (int64_t)Fin * kCh; p.out = out; p.Fout = Fout; p.out_fs = (int64_t)Fout * kCh; p.kt = bkt; p.T = T;
         p.lookahead = la;
-        if (path) { p.path = path; p.path_fs = p.in_fs; p.ps = ones; p.pb = zeros; }   // the pathway tensor is already >= 0
-        // tensor-core version where it is built: no look-ahead, transposed blocks with one time tap only
-        const float *w_sw = nullptr;
-        if (la == 0 && !(mode == DW_T2 && bkt != 1) && (r = need(m, (n + ".pw_sw").c_str(), kCh * kCh, &w_sw))) return r;
-        if (mode == DW_S1) return run_dwpw<DW_S1>(st, p, B, w_sw);
-        if (mode == DW_S2) return run_dwpw<DW_S2>(st, p, B, w_sw);
-        return run_dwpw<DW_T2>(st, p, B, w_sw);
+        if (path) { p.path = path; p.path_fs = p.in_fs; p.ps = w.ones; p.pb = w.zeros; }   // the pathway tensor is already >= 0
+        if (mode == DW_S1) return run_dwpw<DW_S1>(st, p, B, k.pw_sw);
+        if (mode == DW_S2) return run_dwpw<DW_S2>(st, p, B, k.pw_sw);
+        return run_dwpw<DW_T2>(st, p, B, k.pw_sw);
     };
     // ---- encoder, deepfilternet.py:122-141
     DFB_CUDA(cudaEventRecord(L.ev_fork_enc, s));
     DFB_CUDA(cudaStreamWaitEvent(sa, L.ev_fork_enc, 0));
     {
-        const float *w, *bb;
-        if ((rc = need(m, "enc.erb_conv0.w", c.inp_kt * 3 * kCh, &w)) || (rc = need(m, "enc.erb_conv0.b", kCh, &bb))) return rc;
         dim3 grid((unsigned)((T + kInFrames - 1) / kInFrames), (unsigned)B);
         const int la = c.conv_lookahead > 0 ? 1 : 0;
         {
             DFB_PROF("k_conv_in[erb_conv0]", s);
-            k_conv_in<1><<<grid, 256, (kInFrames + c.inp_kt - 1) * (E + 2) * 4, s>>>(d_feat_erb, w, bb, f.e0, T, E, c.inp_kt, la, Tsx, Tx, -la,
-                                                                                      nullptr, 0, nullptr);
+            k_conv_in<1><<<grid, 256, (kInFrames + c.inp_kt - 1) * (E + 2) * 4, s>>>(d_feat_erb, w.erb_conv0.w, w.erb_conv0.b, f.e0, T, E, c.inp_kt, la,
+                                                                                      Tsx, Tx, -la, nullptr, 0, nullptr);
             DFB_LAUNCH_CHECK();
         }
-        if ((rc = need(m, "enc.df_conv0.w", c.inp_kt * 3 * 2 * kCh, &w)) || (rc = need(m, "enc.df_conv0.b", kCh, &bb))) return rc;
         DFB_PROF("k_conv_in[df_conv0]", sa);
-        k_conv_in<2><<<grid, 256, (kInFrames + c.inp_kt - 1) * (Fd + 2) * 2 * 4, sa>>>(d_feat_spec, w, bb, f.c0, T, Fd, c.inp_kt, c.conv_lookahead,
-                                                                                      Tsx, Tx, -c.conv_lookahead, nullptr, 0, nullptr);
+        k_conv_in<2><<<grid, 256, (kInFrames + c.inp_kt - 1) * (Fd + 2) * 2 * 4, sa>>>(d_feat_spec, w.df_conv0.w, w.df_conv0.b, f.c0, T, Fd, c.inp_kt,
+                                                                                      c.conv_lookahead, Tsx, Tx, -c.conv_lookahead, nullptr, 0, nullptr);
         DFB_LAUNCH_CHECK();
     }
-    if ((rc = block(sa, "enc.df_conv1", DW_S2, f.c0, Fd, f.c1, Fd / 2, kt, 0, nullptr))) return rc;
+    if ((rc = block(sa, w.df_conv1, DW_S2, f.c0, Fd, f.c1, Fd / 2, kt, 0, nullptr))) return rc;
     {   // cemb = df_fc_emb(c1 channel-major), pre-shuffle order
-        const float *src[1] = {f.c1}; const int64_t ld[1] = {(int64_t)Fd / 2 * kCh}; const int *ix[1] = {idx_c1};
+        const float *src[1] = {f.c1}; const int64_t ld[1] = {(int64_t)Fd / 2 * kCh}; const int *ix[1] = {w.idx_c1};
         if ((rc = gather(sa, 1, src, ld, ix, Fd / 2 * kCh, 0, f.c1g, nullptr, nullptr))) return rc;
-        const float *w, *bb;
         const int I = Fd / 2 * kCh;
-        if ((rc = need(m, "enc.df_fc_emb.gl", (int64_t)I * H / c.g_df_fc_emb, &w)) || (rc = need(m, "enc.df_fc_emb.bias", H, &bb))) return rc;
-        if ((rc = run_gl(sa, f.c1g, I, w, bb, nullptr, 0, f.cemb, H, M, c.g_df_fc_emb, I, H, ACT_NONE))) return rc;
+        if ((rc = run_gl(sa, f.c1g, I, w.df_fc_emb.w, w.df_fc_emb.b, nullptr, 0, f.cemb, H, M, c.g_df_fc_emb, I, H, ACT_NONE))) return rc;
     }
     DFB_CUDA(cudaEventRecord(L.ev_join_enc, sa));
-    if ((rc = block(s, "enc.erb_conv1", DW_S2, f.e0, E, f.e1, E / 2, kt, c.conv_lookahead > 1 ? 1 : 0, nullptr)) ||
-        (rc = block(s, "enc.erb_conv2", DW_S2, f.e1, E / 2, f.e2, E / 4, kt, c.conv_lookahead > 2 ? 1 : 0, nullptr)) ||
-        (rc = block(s, "enc.erb_conv3", DW_S1, f.e2, E / 4, f.e3, E / 4, kt, 0, nullptr)))
+    if ((rc = block(s, w.erb_conv1, DW_S2, f.e0, E, f.e1, E / 2, kt, c.conv_lookahead > 1 ? 1 : 0, nullptr)) ||
+        (rc = block(s, w.erb_conv2, DW_S2, f.e1, E / 2, f.e2, E / 4, kt, c.conv_lookahead > 2 ? 1 : 0, nullptr)) ||
+        (rc = block(s, w.erb_conv3, DW_S1, f.e2, E / 4, f.e3, E / 4, kt, 0, nullptr)))
         return rc;
     DFB_CUDA(cudaStreamWaitEvent(s, L.ev_join_enc, 0));
     {   // emb = e3 (channel-major flatten) + shuffle(cemb)
-        const float *src[2] = {f.e3, f.cemb}; const int64_t ld[2] = {H, H}; const int *ix[2] = {idx_e3, idx_shuf};
+        const float *src[2] = {f.e3, f.cemb}; const int64_t ld[2] = {H, H}; const int *ix[2] = {w.idx_e3, w.idx_shuf};
         if ((rc = gather(s, 2, src, ld, ix, H, 0, f.emb, f.emb_hi, f.emb_lo))) return rc;
     }
     // GroupedGRU: layer l as a dense recurrence, out = sum_l shuffle(y_l) (l < last) + y_last
-    auto ggru = [&](cudaStream_t st, const char *name, int layers, unsigned short *x_hi, unsigned short *x_lo, float **y,
+    auto ggru = [&](cudaStream_t st, const GruLayer *g, int layers, unsigned short *x_hi, unsigned short *x_lo, float **y,
                     unsigned short **y_hi, unsigned short **y_lo, float *xproj, float *hbase, float *out, unsigned short *out_hi,
                     unsigned short *out_lo) -> int {
         unsigned short *ch = x_hi, *cl = x_lo;
         for (int l = 0; l < layers; l++) {
-            const std::string nm = std::string(name) + ".g" + std::to_string(l);
             GruChunk ck{hbase ? hbase + (int64_t)l * B * H : nullptr, false, 0, B, nullptr, 0};
             bool ok = false;
-            int r = run_gru(m, st, nm.c_str(), 1, H, H, nullptr, y[l], xproj, B, T, ch, cl, f.scr_hi, f.scr_lo, 0, y_hi[l], y_lo[l], &ok,
+            int r = run_gru(m, st, &g[l], 1, H, nullptr, y[l], xproj, B, T, ch, cl, f.scr_hi, f.scr_lo, 0, y_hi[l], y_lo[l], &ok,
                             hbase ? &ck : nullptr);
             if (r) return r;
             ch = y_hi[l]; cl = y_lo[l];
         }
         const float *src[3]; int64_t ld[3]; const int *ix[3];
-        for (int l = 0; l < layers; l++) { src[l] = y[l]; ld[l] = H; ix[l] = l == layers - 1 ? idx_id : idx_gshuf; }
+        for (int l = 0; l < layers; l++) { src[l] = y[l]; ld[l] = H; ix[l] = l == layers - 1 ? w.idx_id : w.idx_gshuf; }
         return gather(st, layers, src, ld, ix, H, 0, out, out_hi, out_lo);
     };
     if (c.enc_gru_layers > 3 || c.df_gru_layers > 2) return fail(DFB_ERR_UNSUPPORTED, "DeepFilterNet v1: more GRU layers than built (3 / 2)");
-    if ((rc = ggru(s, "enc.emb_gru", c.enc_gru_layers, f.emb_hi, f.emb_lo, f.y, f.y_hi, f.y_lo, f.xproj, cx ? cx->h_enc : nullptr, f.embo,
+    if ((rc = ggru(s, w.enc_gru.data(), c.enc_gru_layers, f.emb_hi, f.emb_lo, f.y, f.y_hi, f.y_lo, f.xproj, cx ? cx->h_enc : nullptr, f.embo,
                    f.embo_hi, f.embo_lo)))
         return rc;
-    if (d_lsnr) {
-        const float *lw, *lb;
-        if ((rc = need(m, "enc.lsnr.w", H, &lw)) || (rc = need(m, "enc.lsnr.b", 1, &lb))) return rc;
-        if ((rc = run_gl(s, f.embo, H, lw, lb, nullptr, 0, d_lsnr, 1, M, 1, H, 1, ACT_SIGMOID, c.lsnr_scale, c.lsnr_offset))) return rc;
-    }
+    if (d_lsnr && (rc = run_gl(s, f.embo, H, w.lsnr.w, w.lsnr.b, nullptr, 0, d_lsnr, 1, M, 1, H, 1, ACT_SIGMOID, c.lsnr_scale, c.lsnr_offset)))
+        return rc;
     DFB_CUDA(cudaEventRecord(L.ev_fork, s));
     if (!serial) { s = L.dhi; sa = L.daux; DFB_CUDA(cudaStreamWaitEvent(s, L.ev_fork, 0)); }
     DFB_CUDA(cudaStreamWaitEvent(sa, L.ev_fork, 0));
     // ---- DF decoder, deepfilternet.py:219-229 (auxiliary stream)
     {
-        if ((rc = ggru(sa, "df_dec.df_gru", c.df_gru_layers, f.embo_hi, f.embo_lo, f.z, f.z_hi, f.z_lo, f.xproj2, cx ? cx->h_df : nullptr, f.dfc,
+        if ((rc = ggru(sa, w.df_gru.data(), c.df_gru_layers, f.embo_hi, f.embo_lo, f.z, f.z_hi, f.z_lo, f.xproj2, cx ? cx->h_df : nullptr, f.dfc,
                        f.dfc_hi, f.dfc_lo)))
             return rc;
-        if (d_alpha) {
-            const float *aw, *ab;
-            if ((rc = need(m, "df_dec.df_fc_a.w", H, &aw)) || (rc = need(m, "df_dec.df_fc_a.b", 1, &ab))) return rc;
-            if ((rc = run_gl(sa, f.dfc, H, aw, ab, nullptr, 0, d_alpha, 1, M, 1, H, 1, ACT_SIGMOID))) return rc;
-        }
-        const float *w_t, *bb, *w_hi, *w_lo;
+        if (d_alpha && (rc = run_gl(sa, f.dfc, H, w.df_fc_a.w, w.df_fc_a.b, nullptr, 0, d_alpha, 1, M, 1, H, 1, ACT_SIGMOID))) return rc;
         const int N = Fd * O2;
-        if ((rc = need(m, "df_dec.df_fc_out.w_t", (int64_t)H * N, &w_t)) || (rc = need(m, "df_dec.df_fc_out.b", N, &bb))) return rc;
         rc = DFB_ERR_UNSUPPORTED;
-        if (m->get("df_dec.df_fc_out.w_hi")) {
-            if ((rc = need(m, "df_dec.df_fc_out.w_hi", (int64_t)H * N / 2, &w_hi)) || (rc = need(m, "df_dec.df_fc_out.w_lo", (int64_t)H * N / 2, &w_lo))) return rc;
-            rc = launch_gemm_bf16x3(sa, f.dfc_hi, f.dfc_lo, H, w_hi, w_lo, bb, d_coefs, N, M, N, H);
-        }
-        if (rc == DFB_ERR_UNSUPPORTED) rc = run_gl(sa, f.dfc, H, w_t, bb, nullptr, 0, d_coefs, N, M, 1, H, N, ACT_NONE);
+        if (w.df_fc_out.w_hi) rc = launch_gemm_bf16x3(sa, f.dfc_hi, f.dfc_lo, H, w.df_fc_out.w_hi, w.df_fc_out.w_lo, w.df_fc_out.b, d_coefs, N, M, N, H);
+        if (rc == DFB_ERR_UNSUPPORTED) rc = run_gl(sa, f.dfc, H, w.df_fc_out.w_t, w.df_fc_out.b, nullptr, 0, d_coefs, N, M, 1, H, N, ACT_NONE);
         if (rc) return rc;
-        const float *pw, *pb;
-        if ((rc = need(m, "df_dec.df_convp.w", kCh * O2, &pw)) || (rc = need(m, "df_dec.df_convp.b", O2, &pb))) return rc;
         const long long rows = (long long)M * Fd;
         DFB_PROF("k_convp_v1", sa);
-        k_convp_v1<10><<<(unsigned)((rows + 127) / 128), 128, 0, sa>>>(f.c0, pw, pb, d_coefs, rows);
+        k_convp_v1<10><<<(unsigned)((rows + 127) / 128), 128, 0, sa>>>(f.c0, w.df_convp.w, w.df_convp.b, d_coefs, rows);
         DFB_LAUNCH_CHECK();
     }
     DFB_CUDA(cudaEventRecord(L.ev_join, sa));
     // ---- ERB decoder, deepfilternet.py:179-189
     {
-        const float *w, *bb;
-        if ((rc = need(m, "erb_dec.fc_emb.gl", (int64_t)H * H / c.g_erb_in, &w)) || (rc = need(m, "erb_dec.fc_emb.bias", H, &bb))) return rc;
-        if ((rc = run_gl(s, f.embo, H, w, bb, nullptr, 0, f.dec_old, H, M, c.g_erb_in, H, H, ACT_RELU))) return rc;
-        const float *src[1] = {f.dec_old}; const int64_t ld[1] = {H}; const int *ix[1] = {idx_dec};
+        if ((rc = run_gl(s, f.embo, H, w.erb_fc_emb.w, w.erb_fc_emb.b, nullptr, 0, f.dec_old, H, M, c.g_erb_in, H, H, ACT_RELU))) return rc;
+        const float *src[1] = {f.dec_old}; const int64_t ld[1] = {H}; const int *ix[1] = {w.idx_dec};
         if ((rc = gather(s, 1, src, ld, ix, H, 0, f.dec, nullptr, nullptr))) return rc;
-        if ((rc = block(s, "erb_dec.conv3p", DW_S1, f.e3, E / 4, f.p3, E / 4, 1, 0, nullptr)) ||
-            (rc = block(s, "erb_dec.conv2p", DW_S1, f.e2, E / 4, f.p2, E / 4, 1, 0, nullptr)) ||
-            (rc = block(s, "erb_dec.conv1p", DW_S1, f.e1, E / 2, f.p1, E / 2, 1, 0, nullptr)) ||
-            (rc = block(s, "erb_dec.conv0p", DW_S1, f.e0, E, f.p0, E, 1, 0, nullptr)))
+        if ((rc = block(s, w.conv3p, DW_S1, f.e3, E / 4, f.p3, E / 4, 1, 0, nullptr)) ||
+            (rc = block(s, w.conv2p, DW_S1, f.e2, E / 4, f.p2, E / 4, 1, 0, nullptr)) ||
+            (rc = block(s, w.conv1p, DW_S1, f.e1, E / 2, f.p1, E / 2, 1, 0, nullptr)) ||
+            (rc = block(s, w.conv0p, DW_S1, f.e0, E, f.p0, E, 1, 0, nullptr)))
             return rc;
-        if ((rc = block(s, "erb_dec.convt3", DW_S1, f.dec, E / 4, f.d3, E / 4, kt, 0, f.p3)) ||
-            (rc = block(s, "erb_dec.convt2", DW_T2, f.d3, E / 4, f.d2, E / 2, kt, 0, f.p2)) ||
-            (rc = block(s, "erb_dec.convt1", DW_T2, f.d2, E / 2, f.d1, E, kt, 0, f.p1)))
+        if ((rc = block(s, w.convt3, DW_S1, f.dec, E / 4, f.d3, E / 4, kt, 0, f.p3)) ||
+            (rc = block(s, w.convt2, DW_T2, f.d3, E / 4, f.d2, E / 2, kt, 0, f.p2)) ||
+            (rc = block(s, w.convt1, DW_T2, f.d2, E / 2, f.d1, E, kt, 0, f.p1)))
             return rc;
-        if ((rc = need(m, "erb_dec.conv0_out.w", kt * 3 * kCh, &w)) || (rc = need(m, "erb_dec.conv0_out.b", 1, &bb))) return rc;
         static PerDeviceOnce attr_once;
         const int smem = (kMaskWarps * 2 * (E + 2) * kMaskLd + kt * 3 * kCh) * 4;
         if (auto once_guard = attr_once.first()) {
@@ -1434,7 +1432,7 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
         const int per_cta = kMaskWarps * kMaskChunk;
         dim3 grid((unsigned)((T + per_cta - 1) / per_cta), (unsigned)B);
         DFB_PROF("k_mask_out", s);
-        k_mask_out<<<grid, 32 * kMaskWarps, smem, s>>>(f.p0, f.d1, ones, zeros, w, bb, d_m, T, E, kt, nullptr, 0);
+        k_mask_out<<<grid, 32 * kMaskWarps, smem, s>>>(f.p0, f.d1, w.ones, w.zeros, w.conv0_out.w, w.conv0_out.b, d_m, T, E, kt, nullptr, 0);
         DFB_LAUNCH_CHECK();
     }
     DFB_CUDA(cudaStreamWaitEvent(s, L.ev_join, 0));

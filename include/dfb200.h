@@ -148,7 +148,8 @@ typedef struct {
     int64_t numel;
 } dfb_tensor;
 
-/* Replaces init_model + load_state_dict (deepfilternet3.py:80-87, checkpoint.py:46-104). */
+/* Replaces init_model + load_state_dict (deepfilternet3.py:80-87, checkpoint.py:46-104).  Rejects a weight set that
+ * lacks a tensor, or has a tensor of the wrong size, for the layers the config runs (DFB_ERR_INVALID, naming the tensor). */
 int dfb_model_create(dfb_model **out, int device, const dfb_model_config *cfg, const dfb_tensor *tensors,
                      int n_tensors, const int64_t *erb_widths);
 void dfb_model_free(dfb_model *m);
