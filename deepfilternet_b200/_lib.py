@@ -112,6 +112,11 @@ SIGNATURES = {
     "dfb_stream_set_sample_rate": (_I, [_VP, _I, _VP, _I, _I, _I, _VP, _I, _I, _I]),
     "dfb_stream_latency_samples": (_I64, [_VP]),
     "dfb_debug_resample_stream": (_I, [_I, _I, _VP, _I, _I, _I, _VP, _I64, _I64P, _I64, _VP, _VP]),
+    "dfb_stream_add_slot_rate": (_I, [_VP, _I, _VP, _I, _I, _I, _VP, _I, _I, _I]),
+    "dfb_stream_open_slots_at": (_I, [_VP, _I64P, _I64, _I]),
+    "dfb_stream_open_linked_at": (_I, [_VP, _I64P, _I64, _I]),
+    "dfb_stream_slot_rates": (_I, [_VP, C.POINTER(C.c_int32)]),
+    "dfb_debug_resample_slots": (_I, [_I, _VP, C.POINTER(C.c_int32), _VP, _I64, _I64P, _I64, _VP, _VP]),
     "dfb_stream_create_spec": (_I, [C.POINTER(_VP), _VP, _VP, _I64]),
     "dfb_stream_process_spec": (_I, [_VP, _VP, _I64, _VP, _VP, _VP, _VP, _VP]),
     "dfb_stream_flush_spec": (_I, [_VP, _VP, _VP, _VP, _VP, _VP]),

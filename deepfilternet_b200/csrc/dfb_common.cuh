@@ -136,11 +136,26 @@ enum { kReduceNone = 0, kReduceMax = 1, kReduceMean = 2 };   // dfb_reduce_mask
 // t < Z and otherwise sum_k taps[t % nw][k] * x[(t / nw) og - S + k] over the session's input x, taps outside the input
 // received so far skipped: the resampled session delayed by Z = m nw output samples, m = ceil(width / og), so that every
 // tap a hop's outputs need has arrived with that hop.  A row carries the last S = m og + width input samples between
-// calls (S <= hop_in).  hop_in / hop_out: samples per 10 ms hop on either side.
-struct ResampleDir { const float *taps; int og, nw, K, S, Z, hop_in, hop_out; };
-// A live row of a resampled call: its slot (row of the caller's buffers), the handle's hop its session started at, and
-// the end hop of a closed session (as the slot path's rows[].Tf; open: far in the future).
-struct ResampleRow { int64_t slot, first, end; };
+// calls (S <= hop_in).  hop_in / hop_out: samples per 10 ms hop on either side.  ext: the hops of zero extension a
+// session's input ends before its end hop (1; 0 for the identity direction of a 48 kHz slot on a mixed-rate handle:
+// og = nw = K = 1, one tap of 1.0, S = Z = 0, which copies its row exactly: fmaf(1, x, +0) is x, but for -0, which
+// comes out as +0).
+struct ResampleDir { const float *taps; int og, nw, K, S, Z, hop_in, hop_out, ext; };
+// The directions of one resampler of a handle, indexed by ResampleRow::dir: one on a handle at one rate, the identity and
+// one per registered rate on a mixed-rate handle (dfb_stream_add_slot_rate).
+constexpr int kMaxRateDirs = 7;
+struct ResampleDirs { ResampleDir d[kMaxRateDirs]; };
+// A live row of a resampled call: its slot (row of the caller's buffers), the handle's hop its session started at, the
+// end hop of a closed session (as the slot path's rows[].Tf; open: far in the future) and its direction.
+struct ResampleRow { int64_t slot, first, end, dir; };
+// The buffers of one resampler call of n hops from the handle's hop a0: row r reads in + slot * in_pitch + in_col * hop_in
+// and writes n * hop_out samples to out + slot * out_pitch + out_col * hop_out, then zeros up to sample out_w of its row
+// (none when out_w ends before them); hist [rows][hist_pitch] are the rows' carried histories; tail: the hops a session's output runs past its end hop.
+struct ResampleIO {
+    const float *in;
+    float *out, *hist;
+    int64_t in_pitch, out_pitch, out_w, hist_pitch, in_col, out_col, n, a0, tail;
+};
 // Per-slot settings of a streaming handle (dfb_stream_set_atten_lim / _post_filter_beta): limit (0 = off) and post-filter
 // beta (0 = off) from absolute frame sw on, and the previous ones before it.  Only the frame before sw, re-synthesised
 // for its overlap-add tail, still reads the previous ones.
@@ -240,12 +255,11 @@ int launch_feat_norm(const float *d_erb, int E, int64_t erb_stride, const float 
 // in place of p.atten_lim / pf / pf_beta.  A kernel argument of its own after ApplyParams, so that the parameter layout
 // of the other instantiations stays as it was.
 int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaStream_t s, const SlotCtl *ctl = nullptr);
-// One call of n hops through a streaming resampler (k_resample_up / k_resample_down), one CTA per row of rows[0, nb):
-// slot b reads in + b * in_pitch (up: its session's input ends at hop end - 1; in null: no input) and writes n * hop_out
-// samples to out + b * out_pitch (down: zeros from hop end + tail on); hist [nb][S] are the rows' carried histories; a0 is
-// the handle's hop at the call's start.
-int launch_resample_stream(cudaStream_t s, bool up, const ResampleDir &d, const ResampleRow *rows, int nb, const float *in,
-                           int64_t in_pitch, float *out, int64_t out_pitch, float *hist, int64_t n, int64_t a0, int64_t tail);
+// One call of n hops through a streaming resampler (k_resample_up / k_resample_down), one CTA per row of rows[0, nb),
+// each with the direction dirs.d[row.dir] and the buffers of io (up: a session's input ends at hop end - ext; io.in null:
+// no input; down: zeros from hop end + tail on).
+int launch_resample_stream(cudaStream_t s, bool up, const ResampleDirs &dirs, int n_dirs, const ResampleRow *rows, int nb,
+                           const ResampleIO &io);
 // time window of a recurrence launch: steps 0 .. T-1 are frames t0 .. of buffers holding Ts frames per stream; h0 (null:
 // zeros) / hT (null: not stored) are the carried hidden states [B][H]
 struct GruWindow { const float *h0; float *hT; int t0, Ts; const int64_t *first = nullptr; int64_t w0 = 0; /* stream_first */ };

@@ -305,16 +305,17 @@ __global__ void __launch_bounds__(256) k_resample(const float *__restrict__ x, i
     }
 }
 
-// Streaming resampler of a handle at another rate (dfb_stream_set_sample_rate; ResampleDir in dfb_common.cuh): one row's
-// call.  x: the call's nin input samples, the first nin_valid of them the session's (the rest read as zero: the session's
-// zero extension); s_in0 / s_out0: the session's sample index of x[0] / y[0].  The taps are summed as k_resample sums
-// them (fmaf over k = 0 .. K-1, taps outside the session's input skipped), so a streamed session is bit for bit
-// k_resample of the whole session, delayed by Z.  The history is updated after every thread has read it.
+// Streaming resampler of a handle at another rate (dfb_stream_set_sample_rate / dfb_stream_add_slot_rate; ResampleDir in
+// dfb_common.cuh): one row's call.  x: the call's nin input samples, the first nin_valid of them the session's (the rest
+// read as zero: the session's zero extension); s_in0 / s_out0: the session's sample index of x[0] / y[0].  The taps are
+// summed as k_resample sums them (fmaf over k = 0 .. K-1, taps outside the session's input skipped), so a streamed session
+// is bit for bit k_resample of the whole session, delayed by Z.  y[0, nout_valid) are outputs, y[nout_valid, yw) zeros.
+// The history is updated after every thread has read it.
 __device__ __forceinline__ void resample_row(const ResampleDir &d, const float *__restrict__ x, int64_t nin, int64_t nin_valid,
                                              float *__restrict__ hist, int64_t s_in0, int64_t s_out0, float *__restrict__ y,
-                                             int64_t nout, int64_t nout_valid) {
+                                             int64_t nout_valid, int64_t yw) {
     const int64_t lim = s_in0 + nin_valid;
-    for (int64_t o = threadIdx.x; o < nout; o += blockDim.x) {
+    for (int64_t o = threadIdx.x; o < yw; o += blockDim.x) {
         const int64_t t = s_out0 + o;
         float acc = 0.f;
         if (o < nout_valid && t >= d.Z) {
@@ -339,29 +340,36 @@ __device__ __forceinline__ void resample_row(const ResampleDir &d, const float *
     }
 }
 
-// rate r -> 48 kHz: a session's input ends one hop before its end hop (the slot path reads that hop, the zero extension)
-__global__ void __launch_bounds__(256) k_resample_up(ResampleDir d, const ResampleRow *__restrict__ rows, const float *__restrict__ in,
-                                                     int64_t in_pitch, float *__restrict__ out, int64_t out_pitch,
-                                                     float *__restrict__ hist, int64_t n, int64_t a0) {
-    const ResampleRow r = rows[blockIdx.x];
-    const int64_t s = a0 - r.first;
-    int64_t v = in ? r.end - 1 - a0 : 0;
-    v = v < 0 ? 0 : (v > n ? n : v);
-    resample_row(d, in ? in + r.slot * in_pitch : nullptr, n * d.hop_in, v * d.hop_in, hist + (int64_t)blockIdx.x * d.S,
-                 s * d.hop_in, s * d.hop_out, out + r.slot * out_pitch, n * d.hop_out, n * d.hop_out);
+// the samples of a row's output from its call's first one on that the call writes: its n hops, then zeros up to out_w
+__device__ __forceinline__ int64_t fill_to(const ResampleIO &io, const ResampleDir &d) {
+    const int64_t w = io.out_w - io.out_col * d.hop_out, own = io.n * d.hop_out;
+    return w > own ? w : own;
 }
 
-// 48 kHz -> rate r: the slot path's output rows (zeros past a session's tail); a session's output ends `tail` hops after
-// its end hop, and the hops after that are zeros
-__global__ void __launch_bounds__(256) k_resample_down(ResampleDir d, const ResampleRow *__restrict__ rows, const float *__restrict__ in,
-                                                       int64_t in_pitch, float *__restrict__ out, int64_t out_pitch,
-                                                       float *__restrict__ hist, int64_t n, int64_t a0, int64_t tail) {
+// rate r -> 48 kHz, each row in its own direction: a session's input ends ext hops before its end hop (a resampled
+// session's slot path reads that hop, the zero extension; a 48 kHz row's input ends at its end hop)
+__global__ void __launch_bounds__(256) k_resample_up(ResampleDirs dirs, const ResampleRow *__restrict__ rows, ResampleIO io) {
     const ResampleRow r = rows[blockIdx.x];
-    const int64_t s = a0 - r.first;
-    int64_t v = r.end + tail - a0;
+    const ResampleDir d = dirs.d[r.dir];   // in registers: the tap loops read it every iteration
+    const int64_t s = io.a0 - r.first, n = io.n;
+    int64_t v = io.in ? r.end - d.ext - io.a0 : 0;
     v = v < 0 ? 0 : (v > n ? n : v);
-    resample_row(d, in + r.slot * in_pitch, n * d.hop_in, n * d.hop_in, hist + (int64_t)blockIdx.x * d.S, s * d.hop_in,
-                 s * d.hop_out, out + r.slot * out_pitch, n * d.hop_out, v * d.hop_out);
+    resample_row(d, io.in ? io.in + r.slot * io.in_pitch + io.in_col * d.hop_in : nullptr, n * d.hop_in, v * d.hop_in,
+                 io.hist + (int64_t)blockIdx.x * io.hist_pitch, s * d.hop_in, s * d.hop_out,
+                 io.out + r.slot * io.out_pitch + io.out_col * d.hop_out, n * d.hop_out, fill_to(io, d));
+}
+
+// 48 kHz -> rate r, each row in its own direction: the slot path's output rows (zeros past a session's tail); a session's
+// output ends `tail` hops after its end hop, and the hops after that are zeros
+__global__ void __launch_bounds__(256) k_resample_down(ResampleDirs dirs, const ResampleRow *__restrict__ rows, ResampleIO io) {
+    const ResampleRow r = rows[blockIdx.x];
+    const ResampleDir d = dirs.d[r.dir];   // in registers: the tap loops read it every iteration
+    const int64_t s = io.a0 - r.first, n = io.n;
+    int64_t v = r.end + io.tail - io.a0;
+    v = v < 0 ? 0 : (v > n ? n : v);
+    resample_row(d, io.in + r.slot * io.in_pitch + io.in_col * d.hop_in, n * d.hop_in, n * d.hop_in,
+                 io.hist + (int64_t)blockIdx.x * io.hist_pitch, s * d.hop_in, s * d.hop_out,
+                 io.out + r.slot * io.out_pitch + io.out_col * d.hop_out, v * d.hop_out, fill_to(io, d));
 }
 
 // ------------------------------------------------------------- feature norm scans ----
@@ -1486,15 +1494,20 @@ int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaS
     return DFB_OK;
 }
 
-int launch_resample_stream(cudaStream_t s, bool up, const ResampleDir &d, const ResampleRow *rows, int nb, const float *in,
-                           int64_t in_pitch, float *out, int64_t out_pitch, float *hist, int64_t n, int64_t a0, int64_t tail) {
-    if (nb <= 0 || n <= 0) return DFB_OK;
-    if (nb > 65535 || d.S > d.hop_in) return fail(DFB_ERR_INVALID, "bad resampler geometry");
+int launch_resample_stream(cudaStream_t s, bool up, const ResampleDirs &dirs, int n_dirs, const ResampleRow *rows, int nb,
+                           const ResampleIO &io) {
+    if (nb <= 0 || io.n <= 0) return DFB_OK;
+    if (nb > 65535 || n_dirs <= 0 || n_dirs > kMaxRateDirs) return fail(DFB_ERR_INVALID, "bad resampler geometry");
+    for (int i = 0; i < n_dirs; i++) {
+        const ResampleDir &d = dirs.d[i];
+        if (d.S > d.hop_in || d.S > io.hist_pitch)
+            return fail(DFB_ERR_INVALID, "bad resampler geometry");
+    }
     // (not in the DFB_PROF timing, which covers the 48 kHz enhancement path; torch.profiler names them)
     if (up)
-        k_resample_up<<<nb, 256, 0, s>>>(d, rows, in, in_pitch, out, out_pitch, hist, n, a0);
+        k_resample_up<<<nb, 256, 0, s>>>(dirs, rows, io);
     else
-        k_resample_down<<<nb, 256, 0, s>>>(d, rows, in, in_pitch, out, out_pitch, hist, n, a0, tail);
+        k_resample_down<<<nb, 256, 0, s>>>(dirs, rows, io);
     DFB_LAUNCH_CHECK();
     return DFB_OK;
 }

@@ -2486,10 +2486,14 @@ struct dfb_stream {
     float *spec_stage_in = nullptr, *spec_stage_out = nullptr;   // device staging of dfb_stream_process_spec_host
     size_t spec_in_cap = 0, spec_out_cap = 0;
     // sample rate (dfb_stream_set_sample_rate): 0 runs at the model's 48 kHz; else the caller's rate, resampled up into the
-    // unchanged 48 kHz slot path and back down.  The histories are arrays 13 / 14 of the state slab.
+    // unchanged 48 kHz slot path and back down.  A mixed-rate handle (dfb_stream_add_slot_rate) stays at 48 kHz and runs
+    // each slot in its own direction of the resamplers: the identity at 48 kHz, or one of its registered rates.  The
+    // histories are arrays 13 / 14 of the state slab, as wide as the directions' largest S.
     int rate = 0;
-    ResampleDir rs_up{}, rs_down{};
-    float *d_taps = nullptr;                           // both directions' taps
+    std::vector<int> rs_rates;                         // per direction its rate: {rate}, {48000, registered ...} or none
+    ResampleDirs rs_up{}, rs_down{};
+    std::vector<float *> rs_taps;                      // the directions' taps on the device
+    std::vector<int> slot_dir;                         // per slot: its session's direction
     float *rs_in = nullptr, *rs_out = nullptr;         // the slot path's 48 kHz input / output [B][n * 480]
     size_t rs_in_cap = 0, rs_out_cap = 0;
     float *rs_lsnr = nullptr;                          // flush: the LSNR of its two passes
@@ -2498,9 +2502,17 @@ struct dfb_stream {
     ResampleRow *d_rs = nullptr;
 };
 
-// rate-r handles: per_row floats of the two resampler histories in the state slab (0, 0 at 48 kHz)
+// a handle that runs the resamplers: at another rate than 48 kHz, or mixed-rate
+static bool resampled(const dfb_stream *h) { return !h->rs_rates.empty(); }
+static bool mixed_rate(const dfb_stream *h) { return !h->rate && resampled(h); }
+// per-row floats of one resampler's histories: its directions' largest S (0 without resamplers)
+static int rs_hist(const dfb_stream *h, const ResampleDirs &d) {
+    int S = 0;
+    for (size_t i = 0; i < h->rs_rates.size(); i++) S = std::max(S, d.d[i].S);
+    return S;
+}
 static size_t stream_state_floats(const dfb_stream *h, size_t off[16], StateLayout *lay = nullptr) {
-    return state_floats(h->m->cfg, h->st, h->B, off, lay, h->rate ? h->rs_up.S : 0, h->rate ? h->rs_down.S : 0);
+    return state_floats(h->m->cfg, h->st, h->B, off, lay, rs_hist(h, h->rs_up), rs_hist(h, h->rs_down));
 }
 
 // the handle's default post-filter beta: the model's option (0 = off) for DeepFilterNet3; per-row beta is not used for
@@ -2521,6 +2533,7 @@ static void slots_init(dfb_stream *h) {
     h->slot_nch.assign(B, h->fixed_nch);
     h->slot_first.assign(B, 0);
     h->slot_end.assign(B, kOpenEnd);
+    h->slot_dir.assign(B, 0);
     h->n_act = h->B;
     h->tab_dirty = true;
     h->slot_lim.assign(B, NAN);
@@ -2585,8 +2598,9 @@ extern "C" void dfb_stream_free(dfb_stream *h) {
     if (h->d_slotmap) cudaFree(h->d_slotmap);
     if (h->spec_stage_in) cudaFree(h->spec_stage_in);
     if (h->spec_stage_out) cudaFree(h->spec_stage_out);
-    for (float *p : {h->d_taps, h->rs_in, h->rs_out, h->rs_lsnr})
+    for (float *p : {h->rs_in, h->rs_out, h->rs_lsnr})
         if (p) cudaFree(p);
+    for (float *p : h->rs_taps) cudaFree(p);
     if (h->d_rs) cudaFree(h->d_rs);
     delete h;
 }
@@ -2639,15 +2653,17 @@ static int64_t path_latency(const dfb_stream *h) {
     const ChunkGeom g = chunk_geom(h->m->cfg);
     return g.Lmax + g.lag;
 }
-// a resampled handle's sessions end one hop later in the slot path (its zero extension fills the resamplers' look-ahead)
-extern "C" int64_t dfb_stream_latency_frames(const dfb_stream *h) { return h ? path_latency(h) + (h->rate ? 1 : 0) : -1; }
+// a resampled session ends one hop later in the slot path (its zero extension fills the resamplers' look-ahead); a
+// mixed-rate handle's flush returns its longest drain
+extern "C" int64_t dfb_stream_latency_frames(const dfb_stream *h) { return h ? path_latency(h) + (resampled(h) ? 1 : 0) : -1; }
 extern "C" int64_t dfb_stream_frame_length(const dfb_stream *h) {   // capi.rs df_get_frame_length
     return h ? (h->rate ? h->rate / 100 : h->st->hop) : -1;
 }
 // a resampled handle's signal delay on top of the 48 kHz handle's, in samples of its rate: D r / 48000 + E
 extern "C" int64_t dfb_stream_latency_samples(const dfb_stream *h) {
     if (!h) return -1;
-    return h->rate ? (int64_t)h->rs_up.Z / h->rs_up.nw * h->rs_up.og + h->rs_down.Z : 0;
+    const ResampleDir &u = h->rs_up.d[0];
+    return h->rate ? (int64_t)u.Z / u.nw * u.og + h->rs_down.d[0].Z : 0;
 }
 
 // ---- streaming slots: host bookkeeping.  Device rows follow at the next call (stream_step moves them first, by row_src).
@@ -2687,7 +2703,7 @@ static void slot_close(dfb_stream *h, int slot) {
     if (h->slot_state[(size_t)slot] != kSlotOpen) return;
     h->slot_state[(size_t)slot] = kSlotClosing;
     // the stream ends after the input it has been fed; a resampled session one hop later, the hop its zero extension fills
-    h->slot_end[(size_t)slot] = h->S.a1 + (h->rate ? 1 : 0);
+    h->slot_end[(size_t)slot] = h->S.a1 + (resampled(h) ? h->rs_up.d[h->slot_dir[(size_t)slot]].ext : 0);
     h->tab_dirty = true;
 }
 
@@ -2731,8 +2747,8 @@ static int slot_list(dfb_stream *h, const int64_t *slots, int64_t n) {
 
 // Opens one group per `nch` consecutive listed slots (channel c of a group in its c-th slot), each a fresh stream in rows
 // appended to the active prefix.  The listed slots' old streams (whole groups, by slot_list_check) are dropped without
-// their tails first.
-static int slots_open(dfb_stream *h, const int64_t *slots, int64_t n, int64_t nch) {
+// their tails first.  dir: the sessions' direction of the resamplers (0: the handle's rate, 48 kHz on a mixed-rate handle).
+static int slots_open(dfb_stream *h, const int64_t *slots, int64_t n, int64_t nch, int dir = 0) {
     if (int rc = slot_list(h, slots, n)) return rc;
     for (int64_t i = 0; i < n; i++)
         if (h->slot_state[(size_t)slots[i]] != kSlotFree) slot_release(h, (int)slots[i]);
@@ -2747,6 +2763,7 @@ static int slots_open(dfb_stream *h, const int64_t *slots, int64_t n, int64_t nc
         h->slot_state[(size_t)b] = kSlotOpen;
         h->slot_first[(size_t)b] = h->S.a1;
         h->slot_end[(size_t)b] = kOpenEnd;
+        h->slot_dir[(size_t)b] = dir;
         h->slot_lim[(size_t)b] = h->slot_beta[(size_t)b] = NAN;   // back to the handle's settings
         h->slot_fresh[(size_t)b] = 1;
     }
@@ -2759,6 +2776,40 @@ extern "C" int dfb_stream_open_slots(dfb_stream *h, const int64_t *slots, int64_
 extern "C" int dfb_stream_open_linked(dfb_stream *h, const int64_t *slots, int64_t n) {
     if (h && n == 0) return fail(DFB_ERR_INVALID, "a group of no channels");
     return slots_open(h, slots, n, n);
+}
+
+// the rates a streaming handle resamples to and from 48 kHz (dfb_stream_set_sample_rate / dfb_stream_add_slot_rate)
+constexpr int kModelRate = 48000;   // the slot path's rate: 480-sample hops of the 960 / 480 STFT
+static bool stream_rate(int rate) {
+    return rate == 8000 || rate == 12000 || rate == 16000 || rate == 24000 || rate == 32000 || rate == 44100;
+}
+
+// the direction of a mixed-rate handle's sessions at `rate`
+static int rate_dir(const dfb_stream *h, int rate, int *dir) {
+    if (rate != kModelRate && !stream_rate(rate))
+        return fail(DFB_ERR_UNSUPPORTED, "sample rate %d: 8000, 12000, 16000, 24000, 32000, 44100 or 48000", rate);
+    if (!mixed_rate(h)) return fail(DFB_ERR_INVALID, "slots open at their own rates on a handle with slot rates only (dfb_stream_add_slot_rate)");
+    for (size_t i = 0; i < h->rs_rates.size(); i++)
+        if (h->rs_rates[i] == rate) {
+            *dir = (int)i;
+            return DFB_OK;
+        }
+    return fail(DFB_ERR_INVALID, "sample rate %d is not registered on this handle (dfb_stream_add_slot_rate)", rate);
+}
+
+extern "C" int dfb_stream_open_slots_at(dfb_stream *h, const int64_t *slots, int64_t n, int rate) {
+    int dir = 0;
+    if (!h) return fail(DFB_ERR_INVALID, "null stream");
+    if (int rc = rate_dir(h, rate, &dir)) return rc;
+    return slots_open(h, slots, n, 1, dir);
+}
+
+extern "C" int dfb_stream_open_linked_at(dfb_stream *h, const int64_t *slots, int64_t n, int rate) {
+    int dir = 0;
+    if (!h) return fail(DFB_ERR_INVALID, "null stream");
+    if (n == 0) return fail(DFB_ERR_INVALID, "a group of no channels");
+    if (int rc = rate_dir(h, rate, &dir)) return rc;
+    return slots_open(h, slots, n, n, dir);
 }
 
 extern "C" int dfb_stream_close_slots(dfb_stream *h, const int64_t *slots, int64_t n) {
@@ -2841,6 +2892,16 @@ extern "C" int dfb_stream_slot_states(const dfb_stream *h, int32_t *h_states) {
     return DFB_OK;
 }
 
+extern "C" int dfb_stream_slot_rates(const dfb_stream *h, int32_t *h_rates) {
+    if (!h || !h_rates) return fail(DFB_ERR_INVALID, "null argument");
+    if (h->spectral) return fail(DFB_ERR_INVALID, "a spectral handle takes spectra, which have no sample rate");
+    for (int b = 0; b < h->B; b++)
+        h_rates[b] = h->slot_state[(size_t)b] == kSlotFree ? 0
+                     : resampled(h)                         ? h->rs_rates[(size_t)h->slot_dir[(size_t)b]]
+                                                            : kModelRate;
+    return DFB_OK;
+}
+
 extern "C" int dfb_stream_slot_groups(const dfb_stream *h, int64_t *h_first) {
     if (!h || !h_first) return fail(DFB_ERR_INVALID, "null argument");
     for (int b = 0; b < h->B; b++) h_first[b] = h->slot_grp[(size_t)b];
@@ -2871,7 +2932,7 @@ static int slots_move_rows(dfb_stream *h, cudaStream_t s) {
     float *scratch = m->arena.take<float>((size_t)lay.row_floats * n_mv + 1);
     DFB_CUDA(cudaMemcpyAsync(d_ops, ops.data(), sizeof(int2) * ops.size(), cudaMemcpyHostToDevice, s));
     for (int pass = n_mv ? 0 : 1; pass < 2; pass++) {
-        k_slot_rows<<<dim3(4, pass ? (unsigned)ops.size() : (unsigned)n_mv, h->rate ? kStateArrays : kStateArrays - 2), 256, 0, s>>>(
+        k_slot_rows<<<dim3(4, pass ? (unsigned)ops.size() : (unsigned)n_mv, resampled(h) ? kStateArrays : kStateArrays - 2), 256, 0, s>>>(
             h->slab, lay, h->B, d_ops, scratch, pass, m->cfg.nb_erb, m->cfg.nb_df);
         DFB_LAUNCH_CHECK();
     }
@@ -3007,25 +3068,44 @@ static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, 
     return DFB_OK;
 }
 
-// ---- handles at another sample rate (dfb_stream_set_sample_rate; DESIGN.md section 5g).  Each call runs the unchanged
-// 48 kHz slot path between two resamplers: k_resample_up turns the call's rate-r input into the 48 kHz hops the path reads,
-// k_resample_down turns the path's output back into rate-r hops.  Their histories are rows of the state slab, so they
-// move with the rows and start from zero with every session.
-
-constexpr int kModelRate = 48000;   // the slot path's rate: 480-sample hops of the 960 / 480 STFT
+// ---- handles at another sample rate (dfb_stream_set_sample_rate; DESIGN.md section 5g) and mixed-rate handles
+// (dfb_stream_add_slot_rate; section 5h).  Each call runs the unchanged 48 kHz slot path between two resamplers:
+// k_resample_up turns the call's input into the 48 kHz hops the path reads, k_resample_down turns the path's output back
+// into the caller's hops, each row in its session's direction.  Their histories are rows of the state slab, so they move
+// with the rows and start from zero with every session.
 
 // the per-direction geometry of `rate` from io.resample_kernel's (og, nw, width); DFB_ERR_UNSUPPORTED for a rate outside
 // the list, DFB_ERR_INVALID for taps of other rates or a history longer than a hop
 static int rs_geometry(int rate, bool up, const float *taps, int og, int nw, int width, ResampleDir *d) {
-    if (rate != 8000 && rate != 12000 && rate != 16000 && rate != 24000 && rate != 32000 && rate != 44100)
+    if (!stream_rate(rate))
         return fail(DFB_ERR_UNSUPPORTED, "sample rate %d: 8000, 12000, 16000, 24000, 32000, 44100 or 48000", rate);
     const int g = std::gcd(rate, kModelRate), from = up ? rate : kModelRate, to = up ? kModelRate : rate;
     if (!taps || og != from / g || nw != to / g || width <= 0 || width > 4096)
         return fail(DFB_ERR_INVALID, "the %s taps of %d Hz are io.resample_kernel(%d, %d): og %d, nw %d", up ? "up" : "down", rate,
                     from, to, from / g, to / g);
     const int mz = (width + og - 1) / og;
-    *d = ResampleDir{taps, og, nw, 2 * width + og, mz * og + width, mz * nw, from / 100, to / 100};
+    *d = ResampleDir{taps, og, nw, 2 * width + og, mz * og + width, mz * nw, from / 100, to / 100, 1};
     if (d->S > d->hop_in) return fail(DFB_ERR_INVALID, "resampler history of %d samples is longer than a hop", d->S);
+    return DFB_OK;
+}
+
+// Both directions of `rate` from the caller's taps, uploaded: *buf holds them on the device (the caller owns it).
+static int rs_directions(int rate, const float *up_taps, int up_og, int up_nw, int up_width, const float *down_taps, int down_og,
+                         int down_nw, int down_width, ResampleDir *up, ResampleDir *down, float **buf) {
+    int rc;
+    if ((rc = rs_geometry(rate, true, up_taps, up_og, up_nw, up_width, up)) ||
+        (rc = rs_geometry(rate, false, down_taps, down_og, down_nw, down_width, down)))
+        return rc;
+    const size_t nu = (size_t)up->nw * up->K, nd = (size_t)down->nw * down->K;
+    float *taps = nullptr;
+    if (cudaMalloc(&taps, sizeof(float) * (nu + nd)) != cudaSuccess) return fail(DFB_ERR_OOM, "resampler taps allocation failed");
+    if (cudaMemcpy(taps, up_taps, sizeof(float) * nu, cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaMemcpy(taps + nu, down_taps, sizeof(float) * nd, cudaMemcpyHostToDevice) != cudaSuccess) {
+        cudaFree(taps);
+        return fail(DFB_ERR_CUDA, "resampler taps upload failed");
+    }
+    up->taps = taps; down->taps = taps + nu;
+    *buf = taps;
     return DFB_OK;
 }
 
@@ -3036,7 +3116,7 @@ static int rs_table(dfb_stream *h, cudaStream_t s) {
     std::vector<ResampleRow> rows((size_t)h->n_act);
     for (int r = 0; r < h->n_act; r++) {
         const size_t b = (size_t)h->row_slot[(size_t)r];
-        rows[(size_t)r] = ResampleRow{(int64_t)b, h->slot_first[b], h->slot_end[b]};
+        rows[(size_t)r] = ResampleRow{(int64_t)b, h->slot_first[b], h->slot_end[b], h->slot_dir[b]};
     }
     if (rows.size() != h->rs_rows.size() || memcmp(rows.data(), h->rs_rows.data(), sizeof(ResampleRow) * rows.size())) {
         if (!rows.empty())
@@ -3046,34 +3126,36 @@ static int rs_table(dfb_stream *h, cudaStream_t s) {
     return DFB_OK;
 }
 
-// One pass through the slot path: n hops of rate-r input (d_in null: none, the sessions' zero extension), or its flush;
-// the rate-r output hops go to d_out [B][pitch] (the caller offsets the column), their LSNR to d_lsnr [B][n_out].
-static int rate_pass(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, int64_t pitch, float *d_lsnr,
-                     cudaStream_t s) {
-    const int64_t L = path_latency(h), n_out = flush ? L : n, hop = h->st->hop, hr = h->rate / 100, B = h->B, a0 = h->S.a1;
+// One pass through the slot path: n hops of input (d_in null: none, the sessions' zero extension), or its flush; the
+// output hops go to d_out [B][pitch] from hop `col` of each row on, in the row's own samples, and its LSNR to d_lsnr
+// [B][n_out].  Input rows are [B][n * frame_length]: a row reads the first n hops at its own rate.
+static int rate_pass(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, int64_t pitch, int64_t col,
+                     float *d_lsnr, cudaStream_t s) {
+    const int64_t L = path_latency(h), n_out = flush ? L : n, hop = h->st->hop, wide = dfb_stream_frame_length(h), B = h->B,
+                  a0 = h->S.a1;
     int rc;
     if ((rc = stream_tables(h, n, flush, false, s)) || (rc = rs_table(h, s))) return rc;
     if ((!flush && (rc = stage_grow(&h->rs_in, &h->rs_in_cap, sizeof(float) * B * n * hop))) ||
         (rc = stage_grow(&h->rs_out, &h->rs_out_cap, sizeof(float) * B * std::max<int64_t>(n_out, 1) * hop)))
         return rc;
-    const int nb = h->n_act;
-    if (nb < B && n_out > 0)
-        DFB_CUDA(cudaMemset2DAsync(d_out, sizeof(float) * pitch, 0, sizeof(float) * n_out * hr, B, s));
+    const int nb = h->n_act, nd = (int)h->rs_rates.size();
+    // Free rows are zeroed over their whole width by a call's first pass.  A row live in it fills its own row past its
+    // samples with zeros, and only such rows turn free before the call's next pass.
+    if (nb < B && n_out > 0 && col == 0) DFB_CUDA(cudaMemset2DAsync(d_out, sizeof(float) * pitch, 0, sizeof(float) * pitch, B, s));
     size_t off[16];
     stream_state_floats(h, off);
-    if (!flush && (rc = launch_resample_stream(s, true, h->rs_up, h->d_rs, nb, d_in, n * hr, h->rs_in, n * hop, h->slab + off[13], n,
-                                               a0, 0)))
-        return rc;
+    const ResampleIO up{d_in, h->rs_in, h->slab + off[13], n * wide, n * hop, n * hop, rs_hist(h, h->rs_up), 0, 0, n, a0, 0};
+    if (!flush && (rc = launch_resample_stream(s, true, h->rs_up, nd, h->d_rs, nb, up))) return rc;
     if ((rc = stream_step(h, flush ? nullptr : h->rs_in, n, flush, h->rs_out, d_lsnr, s))) return rc;
-    return launch_resample_stream(s, false, h->rs_down, h->d_rs, nb, h->rs_out, n_out * hop, d_out, pitch, h->slab + off[14], n_out,
-                                  a0, L);
+    const ResampleIO down{h->rs_out, d_out, h->slab + off[14], n_out * hop, pitch, pitch, rs_hist(h, h->rs_down), 0, col, n_out, a0, L};
+    return launch_resample_stream(s, false, h->rs_down, nd, h->d_rs, nb, down);
 }
 
-// A call of a resampled handle.  A flush ends every open session (its input one hop before its end frame), runs that hop
-// of zero extension through the slot path and then flushes it: L + 1 output hops.
+// A call of a resampled or mixed-rate handle.  A flush ends every open session (a resampled session's input one hop
+// before its end frame), runs that hop of zero extension through the slot path and then flushes it: L + 1 output hops.
 static int rate_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s) {
-    const int64_t hr = h->rate / 100, B = h->B;
-    if (!flush) return rate_pass(h, d_in, n, false, d_out, n * hr, d_lsnr, s);
+    const int64_t wide = dfb_stream_frame_length(h), B = h->B;
+    if (!flush) return rate_pass(h, d_in, n, false, d_out, n * wide, 0, d_lsnr, s);
     const int64_t L = path_latency(h), w = L + 1;
     for (int b = 0; b < h->B; b++) slot_close(h, b);
     h->slot_ops = true;
@@ -3083,8 +3165,8 @@ static int rate_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, fl
         if ((rc = stage_grow(&h->rs_lsnr, &h->rs_lsnr_cap, sizeof(float) * B * w))) return rc;
         l1 = h->rs_lsnr; l2 = l1 + B;
     }
-    if ((rc = rate_pass(h, nullptr, 1, false, d_out, w * hr, l1, s))) return rc;
-    if (L > 0 && (rc = rate_pass(h, nullptr, 0, true, d_out + hr, w * hr, l2, s))) return rc;
+    if ((rc = rate_pass(h, nullptr, 1, false, d_out, w * wide, 0, l1, s))) return rc;
+    if (L > 0 && (rc = rate_pass(h, nullptr, 0, true, d_out, w * wide, 1, l2, s))) return rc;
     if (d_lsnr) {
         DFB_CUDA(cudaMemcpy2DAsync(d_lsnr, sizeof(float) * w, l1, sizeof(float), sizeof(float), B, cudaMemcpyDeviceToDevice, s));
         if (L > 0)
@@ -3095,10 +3177,10 @@ static int rate_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, fl
 
 // the calls of an audio handle, at 48 kHz or resampled
 static int audio_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s) {
-    return h->rate ? rate_step(h, d_in, n, flush, d_out, d_lsnr, s) : stream_step(h, d_in, n, flush, d_out, d_lsnr, s);
+    return resampled(h) ? rate_step(h, d_in, n, flush, d_out, d_lsnr, s) : stream_step(h, d_in, n, flush, d_out, d_lsnr, s);
 }
 
-// (Re)allocates the state slab of a new or reset handle for its current rate, zeroed.
+// (Re)allocates the state slab of a new or reset handle for its current directions, zeroed.
 static int stream_slab(dfb_stream *h) {
     size_t off[16];
     const size_t n = stream_state_floats(h, off);
@@ -3111,53 +3193,143 @@ static int stream_slab(dfb_stream *h) {
     return DFB_OK;
 }
 
-extern "C" int dfb_stream_set_sample_rate(dfb_stream *h, int rate, const float *up_taps, int up_og, int up_nw, int up_width,
-                                          const float *down_taps, int down_og, int down_nw, int down_width) {
+// The rules both rate setters share: an audio handle, new or reset, before its first frame and any slot operation.
+static int rate_setter(dfb_stream *h) {
     if (!h) return fail(DFB_ERR_INVALID, "null stream");
     if (h->spectral) return fail(DFB_ERR_INVALID, "a spectral handle takes spectra, which have no sample rate");
     if (h->fed || h->slot_ops)
         return fail(DFB_ERR_INVALID, "sample rate set after the first frame or a slot operation: reset the stream first");
-    ResampleDir up{}, down{};
-    int rc;
-    if (rate != kModelRate && ((rc = rs_geometry(rate, true, up_taps, up_og, up_nw, up_width, &up)) ||
-                               (rc = rs_geometry(rate, false, down_taps, down_og, down_nw, down_width, &down))))
-        return rc;
     DFB_CUDA(cudaSetDevice(h->m->device));
     if (!h->d_rs && cudaMalloc(&h->d_rs, sizeof(ResampleRow) * (size_t)h->B) != cudaSuccess) {
         h->d_rs = nullptr;
         return fail(DFB_ERR_OOM, "resampler table allocation failed");
     }
-    float *taps = nullptr;
-    if (rate != kModelRate) {
-        const size_t nu = (size_t)up.nw * up.K, nd = (size_t)down.nw * down.K;
-        if (cudaMalloc(&taps, sizeof(float) * (nu + nd)) != cudaSuccess) return fail(DFB_ERR_OOM, "resampler taps allocation failed");
-        if (cudaMemcpy(taps, up_taps, sizeof(float) * nu, cudaMemcpyHostToDevice) != cudaSuccess ||
-            cudaMemcpy(taps + nu, down_taps, sizeof(float) * nd, cudaMemcpyHostToDevice) != cudaSuccess) {
-            cudaFree(taps);
-            return fail(DFB_ERR_CUDA, "resampler taps upload failed");
-        }
-        up.taps = taps; down.taps = taps + nu;
-    }
+    return DFB_OK;
+}
+
+// Installs the directions `rates` / up / down with the new tap buffers `added` (owned from here on, freed on failure):
+// the slab is reallocated for their histories and every slot starts afresh.
+static int rs_install(dfb_stream *h, int rate, std::vector<int> rates, const ResampleDirs &up, const ResampleDirs &down,
+                      const std::vector<float *> &added, bool replace) {
     const int old_rate = h->rate;
-    const ResampleDir old_up = h->rs_up, old_down = h->rs_down;
-    h->rate = rate == kModelRate ? 0 : rate;
-    h->rs_up = up; h->rs_down = down;
-    if ((rc = stream_slab(h))) {   // the old slab stays
-        h->rate = old_rate; h->rs_up = old_up; h->rs_down = old_down;
-        if (taps) cudaFree(taps);
+    std::vector<int> old_rates = h->rs_rates;
+    const ResampleDirs old_up = h->rs_up, old_down = h->rs_down;
+    h->rate = rate; h->rs_rates = std::move(rates); h->rs_up = up; h->rs_down = down;
+    if (int rc = stream_slab(h)) {   // the old slab stays
+        h->rate = old_rate; h->rs_rates = std::move(old_rates); h->rs_up = old_up; h->rs_down = old_down;
+        for (float *p : added) cudaFree(p);
         return rc;
     }
-    if (h->d_taps) cudaFree(h->d_taps);
-    h->d_taps = taps;
+    if (replace) {
+        for (float *p : h->rs_taps) cudaFree(p);
+        h->rs_taps.clear();
+    }
+    h->rs_taps.insert(h->rs_taps.end(), added.begin(), added.end());
     h->rs_rows.clear();
     slots_init(h);
     return DFB_OK;
 }
 
+extern "C" int dfb_stream_set_sample_rate(dfb_stream *h, int rate, const float *up_taps, int up_og, int up_nw, int up_width,
+                                          const float *down_taps, int down_og, int down_nw, int down_width) {
+    if (int rc = rate_setter(h)) return rc;
+    if (mixed_rate(h))   // already at 48 kHz, with its registered slot rates
+        return rate == kModelRate ? DFB_OK : fail(DFB_ERR_INVALID, "a handle with slot rates runs at 48000 Hz: its slots open at their rates");
+    ResampleDirs up{}, down{};
+    float *taps = nullptr;
+    if (rate != kModelRate) {
+        if (int rc = rs_directions(rate, up_taps, up_og, up_nw, up_width, down_taps, down_og, down_nw, down_width, &up.d[0],
+                                   &down.d[0], &taps))
+            return rc;
+        return rs_install(h, rate, {rate}, up, down, {taps}, true);
+    }
+    return rs_install(h, 0, {}, up, down, {}, true);
+}
+
+// A rate of a mixed-rate handle's slots: one more direction of both resamplers, the first registration also adds the
+// identity (48 kHz) direction 0.
+extern "C" int dfb_stream_add_slot_rate(dfb_stream *h, int rate, const float *up_taps, int up_og, int up_nw, int up_width,
+                                        const float *down_taps, int down_og, int down_nw, int down_width) {
+    if (h && !h->spectral && h->rate)
+        return fail(DFB_ERR_INVALID, "slot rates are registered on a 48 kHz handle: this one runs at %d Hz", h->rate);
+    if (int rc = rate_setter(h)) return rc;
+    ResampleDir up{}, down{};
+    for (int i = 0; i < 2; i++)   // the arguments' checks first, the upload once the rate is known to be new
+        if (int rc = rs_geometry(rate, i == 0, i ? down_taps : up_taps, i ? down_og : up_og, i ? down_nw : up_nw,
+                                 i ? down_width : up_width, i ? &down : &up))
+            return rc;
+    if (std::find(h->rs_rates.begin(), h->rs_rates.end(), rate) != h->rs_rates.end()) return DFB_OK;
+    std::vector<int> rates = h->rs_rates;
+    ResampleDirs ups = h->rs_up, downs = h->rs_down;
+    std::vector<float *> added;
+    if (rates.empty()) {
+        static const float one = 1.f;
+        float *d_one = nullptr;
+        if (cudaMalloc(&d_one, sizeof(float)) != cudaSuccess) return fail(DFB_ERR_OOM, "resampler taps allocation failed");
+        if (cudaMemcpy(d_one, &one, sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
+            cudaFree(d_one);
+            return fail(DFB_ERR_CUDA, "resampler taps upload failed");
+        }
+        added.push_back(d_one);
+        const int hop = h->st->hop;
+        ups.d[0] = downs.d[0] = ResampleDir{d_one, 1, 1, 1, 0, 0, hop, hop, 0};
+        rates.push_back(kModelRate);
+    }
+    float *taps = nullptr;
+    const size_t k = rates.size();
+    if (int rc = rs_directions(rate, up_taps, up_og, up_nw, up_width, down_taps, down_og, down_nw, down_width, &ups.d[k],
+                               &downs.d[k], &taps)) {
+        for (float *p : added) cudaFree(p);
+        return rc;
+    }
+    added.push_back(taps);
+    rates.push_back(rate);
+    return rs_install(h, 0, std::move(rates), ups, downs, added, false);
+}
+
+// Debug aid: the resamplers of a handle on their own over a list of call sizes, every row one session from hop 0 in the
+// direction of its rate
+extern "C" int dfb_debug_resample_slots(int up, const dfb_stream *h, const int32_t *h_rates, const float *d_in, int64_t C,
+                                        const int64_t *h_calls, int64_t n_calls, float *d_out, void *stream) {
+    if (!h || !h_rates || !d_in || !d_out || C <= 0 || C > 65535 || !h_calls || n_calls <= 0)
+        return fail(DFB_ERR_INVALID, "bad argument");
+    std::vector<ResampleRow> rows((size_t)C);
+    for (int64_t c = 0; c < C; c++) {
+        const auto it = std::find(h->rs_rates.begin(), h->rs_rates.end(), (int)h_rates[c]);
+        if (it == h->rs_rates.end()) return fail(DFB_ERR_INVALID, "row %lld: the handle has no direction at %d Hz", (long long)c, h_rates[c]);
+        rows[(size_t)c] = ResampleRow{c, 0, kOpenEnd, it - h->rs_rates.begin()};
+    }
+    int64_t H = 0;
+    for (int64_t i = 0; i < n_calls; i++) {
+        if (h_calls[i] <= 0) return fail(DFB_ERR_INVALID, "call %lld has %lld hops", (long long)i, (long long)h_calls[i]);
+        H += h_calls[i];
+    }
+    if (int rc = use_device(h->m->device)) return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    const ResampleDirs &dirs = up ? h->rs_up : h->rs_down;
+    const int64_t hp = rs_hist(h, dirs), W = H * h->st->hop;
+    ResampleRow *d_rows = nullptr;
+    float *hist = nullptr;
+    int rc = DFB_OK;
+    if (cudaMalloc(&d_rows, sizeof(ResampleRow) * C) != cudaSuccess || cudaMalloc(&hist, sizeof(float) * (C * hp + 1)) != cudaSuccess ||
+        cudaMemcpyAsync(d_rows, rows.data(), sizeof(ResampleRow) * C, cudaMemcpyHostToDevice, s) != cudaSuccess ||
+        cudaMemsetAsync(hist, 0, sizeof(float) * (C * hp + 1), s) != cudaSuccess)
+        rc = fail(DFB_ERR_OOM, "debug buffers");
+    for (int64_t i = 0, a0 = 0; i < n_calls && !rc; a0 += h_calls[i++])
+        rc = launch_resample_stream(s, up != 0, dirs, (int)h->rs_rates.size(), d_rows, (int)C,
+                                    ResampleIO{d_in, d_out, hist, W, W, i == n_calls - 1 ? W : 0, hp, a0, a0, h_calls[i], a0,
+                                               kOpenEnd});   // the last call fills each row's end with zeros
+    cudaStreamSynchronize(s);
+    if (d_rows) cudaFree(d_rows);
+    if (hist) cudaFree(hist);
+    return rc;
+}
+
 // Debug aid: one resampler on its own over a list of call sizes, every row one session from hop 0
 extern "C" int dfb_debug_resample_stream(int up, int rate, const float *d_taps, int og, int nw, int width, const float *d_in, int64_t C,
                                          const int64_t *h_calls, int64_t n_calls, float *d_out, void *stream) {
-    ResampleDir d{};
+    ResampleDirs dirs{};
+    ResampleDir &d = dirs.d[0];
     if (int rc = rs_geometry(rate, up != 0, d_taps, og, nw, width, &d)) return rc;
     if (!d_in || !d_out || C <= 0 || C > 65535 || !h_calls || n_calls <= 0) return fail(DFB_ERR_INVALID, "bad argument");
     int64_t H = 0;
@@ -3170,7 +3342,7 @@ extern "C" int dfb_debug_resample_stream(int up, int rate, const float *d_taps, 
     if (int rc = use_device(dev)) return rc;
     cudaStream_t s = (cudaStream_t)stream;
     std::vector<ResampleRow> rows((size_t)C);
-    for (int64_t c = 0; c < C; c++) rows[(size_t)c] = ResampleRow{c, 0, kOpenEnd};
+    for (int64_t c = 0; c < C; c++) rows[(size_t)c] = ResampleRow{c, 0, kOpenEnd, 0};
     ResampleRow *d_rows = nullptr;
     float *hist = nullptr;
     int rc = DFB_OK;
@@ -3179,8 +3351,9 @@ extern "C" int dfb_debug_resample_stream(int up, int rate, const float *d_taps, 
         cudaMemsetAsync(hist, 0, sizeof(float) * C * d.S, s) != cudaSuccess)
         rc = fail(DFB_ERR_OOM, "debug buffers");
     for (int64_t i = 0, a0 = 0; i < n_calls && !rc; a0 += h_calls[i++])
-        rc = launch_resample_stream(s, up != 0, d, d_rows, (int)C, d_in + a0 * d.hop_in, H * d.hop_in, d_out + a0 * d.hop_out,
-                                    H * d.hop_out, hist, h_calls[i], a0, kOpenEnd);
+        rc = launch_resample_stream(s, up != 0, dirs, 1, d_rows, (int)C,
+                                    ResampleIO{d_in, d_out, hist, H * d.hop_in, H * d.hop_out, 0, d.S, a0, a0, h_calls[i], a0,
+                                               kOpenEnd});
     cudaStreamSynchronize(s);
     if (d_rows) cudaFree(d_rows);
     if (hist) cudaFree(hist);

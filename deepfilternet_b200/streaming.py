@@ -36,6 +36,16 @@ slot path and resampled back.  ``latency_frames`` grows by one hop and ``latency
 
     s = DfStream(model, df_state, batch=B, sr=16000)
     out = s.process(chunk)               # chunk: float32 [B, n * 160]
+
+``slot_rates`` makes a mixed-rate handle: a 48 kHz handle whose slots each open at their own rate, so that calls at
+different rates share one pass through the slot path.  Rows stay 480 samples per hop; a slot at rate r reads the first
+``n * r // 100`` samples of its row and returns as many, followed by zeros.  Each session equals a handle at its own rate
+(dfb_stream_add_slot_rate in include/dfb200.h)::
+
+    s = DfStream(model, df_state, batch=256, slot_rates=(8000, 16000))
+    s.open([3, 9], sr=16000)
+    s.open([7])                          # 48 kHz
+    out = s.process(chunk)               # chunk: float32 [256, n * 480]
 """
 from __future__ import annotations
 
@@ -75,6 +85,24 @@ def rate_delays(og_up: int, nw_up: int, width_up: int, og_down: int, nw_down: in
     D = -(-width_up // og_up) * nw_up
     E = -(-width_down // og_down) * nw_down
     return D, E, D // nw_up * og_up + E
+
+
+def slot_rate_arg(s, sr, opening: bool = True) -> int:
+    """``sr`` of DfStream.open / open_linked (``opening``) or rate_latency as an int, checked against handle ``s`` as the C
+    ABI checks it: DfbError DFB_ERR_UNSUPPORTED outside STREAM_RATES and MODEL_SR, DFB_ERR_INVALID for a rate the handle
+    does not run.  A mixed-rate handle runs MODEL_SR and its registered rates; any other audio handle runs its own rate,
+    but opens no slot at an explicit rate."""
+    if isinstance(sr, bool) or not isinstance(sr, (int, np.integer)) or (int(sr) not in STREAM_RATES and int(sr) != MODEL_SR):
+        raise DfbError(DFB_ERR_UNSUPPORTED, f"sample rate {sr!r}: one of {STREAM_RATES} or {MODEL_SR}")
+    if getattr(s, "spectral", False):
+        raise DfbError(DFB_ERR_INVALID, "a spectral handle takes spectra, which have no sample rate")
+    reg = tuple(getattr(s, "registered_rates", ()))
+    if not reg and opening:
+        raise DfbError(DFB_ERR_INVALID, "slots open at their own rates on a handle with slot rates only (slot_rates=...)")
+    runs = (MODEL_SR,) + reg if reg else (s.sr,)
+    if int(sr) not in runs:
+        raise DfbError(DFB_ERR_INVALID, f"sample rate {int(sr)}: this handle runs {runs}")
+    return int(sr)
 
 
 def slot_list(slots, batch: int) -> np.ndarray:
@@ -166,8 +194,10 @@ def need_spectral(s) -> None:
 
 class DfStream:
     def __init__(self, model: DfNet, df_state: DF, batch: int = 1, atten_lim_db: Optional[float] = None, channels: int = 1,
-                 reduce_mask: Optional[str] = None, spectral: bool = False, sr: Optional[int] = None):
+                 reduce_mask: Optional[str] = None, spectral: bool = False, sr: Optional[int] = None,
+                 slot_rates=None):
         self.model, self.df_state, self.batch = model, df_state, int(batch)
+        self.registered_rates = ()
         self.spectral = bool(spectral)
         if self.spectral and atten_lim_db is not None:
             raise ValueError("a spectral stream applies nothing: it takes no attenuation limit")
@@ -183,6 +213,8 @@ class DfStream:
         try:
             if sr is not None:
                 self.set_sample_rate(sr)
+            for r in slot_rates or ():
+                self.add_slot_rate(r)
             if channels != 1 or ragged.reduce_code(reduce_mask):
                 self.set_mask_reduce(channels, reduce_mask)
         except Exception:
@@ -202,12 +234,45 @@ class DfStream:
         first frame and any slot operation (DfbError otherwise); survives ``reset`` (dfb_stream_set_sample_rate)."""
         if getattr(self, "spectral", False):
             raise DfbError(DFB_ERR_INVALID, "a spectral handle takes spectra, which have no sample rate")
-        if isinstance(sr, (int, np.integer)) and not isinstance(sr, bool) and int(sr) == MODEL_SR:
+        is_model_sr = isinstance(sr, (int, np.integer)) and not isinstance(sr, bool) and int(sr) == MODEL_SR
+        if getattr(self, "registered_rates", ()) and not is_model_sr:
+            raise DfbError(DFB_ERR_INVALID, "a handle with slot rates runs at 48000 Hz: its slots open at their rates")
+        if is_model_sr:
             check(_lib.lib().dfb_stream_set_sample_rate(self._h, MODEL_SR, None, 0, 0, 0, None, 0, 0, 0))
         else:
             (ku, wu, ou, nu), (kd, wd, od, nd) = rate_taps(sr)
             check(_lib.lib().dfb_stream_set_sample_rate(self._h, int(sr), ku.data_ptr(), ou, nu, wu, kd.data_ptr(), od, nd, wd))
         self._read_rate()
+
+    def add_slot_rate(self, sr: int) -> None:
+        """Let slots of this 48 kHz audio handle open at ``sr`` (STREAM_RATES): ``open(..., sr=sr)``.  Only on a new or reset
+        handle before its first frame and any slot operation (DfbError otherwise); survives ``reset``.  ``latency_frames``
+        becomes L + 1, the longest drain of any slot (dfb_stream_add_slot_rate)."""
+        if getattr(self, "spectral", False):
+            raise DfbError(DFB_ERR_INVALID, "a spectral handle takes spectra, which have no sample rate")
+        if getattr(self, "sr", MODEL_SR) != MODEL_SR:
+            raise DfbError(DFB_ERR_INVALID, f"slot rates are registered on a 48 kHz handle: this one runs at {self.sr} Hz")
+        (ku, wu, ou, nu), (kd, wd, od, nd) = rate_taps(sr)
+        check(_lib.lib().dfb_stream_add_slot_rate(self._h, int(sr), ku.data_ptr(), ou, nu, wu, kd.data_ptr(), od, nd, wd))
+        if int(sr) not in self.registered_rates:
+            self.registered_rates += (int(sr),)
+        self._read_rate()
+
+    def rate_latency(self, sr: int):
+        """(frames, samples): the latency of a session at ``sr`` on this handle, as ``latency_frames`` / ``latency_samples``
+        of a handle at ``sr``: the hops a closing slot drains for, and the resamplers' delay in samples of ``sr``."""
+        sr = slot_rate_arg(self, sr, opening=False)
+        L = self.latency_frames - (1 if self.registered_rates or self.sr != MODEL_SR else 0)   # the 48 kHz path's
+        if sr == MODEL_SR:
+            return L, 0
+        (_, wu, ou, nu), (_, wd, od, nd) = rate_taps(sr)
+        return L + 1, rate_delays(ou, nu, wu, od, nd, wd)[2]
+
+    def slot_rates(self) -> np.ndarray:
+        """int32 [batch]: the rate of each live slot's session, 0 for a free slot (dfb_stream_slot_rates)."""
+        out = np.zeros(self.batch, np.int32)
+        check(_lib.lib().dfb_stream_slot_rates(self._h, out.ctypes.data_as(C.POINTER(C.c_int32))))
+        return out
 
     def set_mask_reduce(self, channels: int, reduce_mask: Optional[str]) -> None:
         """Linked channels: rows g * channels + c form recording g; reduce_mask None / "none", "max" or "mean".  Only on a new
@@ -237,23 +302,34 @@ class DfStream:
         a = slot_list(slots, self.batch)
         check(fn(self._h, a.ctypes.data_as(C.POINTER(C.c_int64)), a.size))
 
-    def open(self, slots) -> None:
+    def open(self, slots, sr: Optional[int] = None) -> None:
         """Start a new stream in each listed slot, from the initial state, as a fresh handle would.  An open or closing
         slot's old stream is dropped without its tail.  Takes effect at the next ``process`` / ``flush``; from then on row
         b of their input and output is that stream, and its output equals ``DfStream(batch=1)`` fed the same audio in the
         same call sizes and flushed at the end.  A live group (``open_linked``) must be listed with all of its members or
-        not at all (DfbError otherwise)."""
-        self._slots(_lib.lib().dfb_stream_open_slots, slots)
+        not at all (DfbError otherwise).  ``sr`` on a mixed-rate handle: the sessions run at ``sr`` (48000 or a registered
+        rate), each equal to ``DfStream(batch=1, sr=sr)``; None opens at the handle's rate."""
+        if sr is None:
+            self._slots(_lib.lib().dfb_stream_open_slots, slots)
+            return
+        sr = slot_rate_arg(self, sr)
+        a = slot_list(slots, self.batch)
+        check(_lib.lib().dfb_stream_open_slots_at(self._h, a.ctypes.data_as(C.POINTER(C.c_int64)), a.size, sr))
 
-    def open_linked(self, slots) -> None:
+    def open_linked(self, slots, sr: Optional[int] = None) -> None:
         """Start one session of ``len(slots)`` channels, channel c in row ``slots[c]``, whose channels share one ERB mask
         reduced by the handle's ``reduce_mask`` (the constructor's, with ``channels=1``; None: unlinked channels that open
         and close together).  Its output equals ``DfStream(batch=C, channels=C, reduce_mask=...)`` fed the same C rows in
         the same call sizes and flushed at the end.  The group moves as a unit: ``open``, ``open_linked``, ``close`` and the
         setters list all of its members or none.  Opening over a live group drops its old session without its tail
-        (dfb_stream_open_linked)."""
+        (dfb_stream_open_linked).  ``sr``: the session's rate on a mixed-rate handle, as for ``open``."""
+        if sr is not None:
+            sr = slot_rate_arg(self, sr)
         a = group_list(slots, self.batch)
-        check(_lib.lib().dfb_stream_open_linked(self._h, a.ctypes.data_as(C.POINTER(C.c_int64)), a.size))
+        if sr is None:
+            check(_lib.lib().dfb_stream_open_linked(self._h, a.ctypes.data_as(C.POINTER(C.c_int64)), a.size))
+        else:
+            check(_lib.lib().dfb_stream_open_linked_at(self._h, a.ctypes.data_as(C.POINTER(C.c_int64)), a.size, sr))
 
     def close(self, slots) -> None:
         """End the stream of each listed open slot after the input it has already been fed.  From the next call on its

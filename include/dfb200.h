@@ -358,7 +358,9 @@ int dfb_stream_process_host_lsnr(dfb_stream *s, const float *h_in, int64_t n_fra
  * call can form its n model hops from the input received so far and return its n h_r samples:
  *   D_r = ceil(width_up / og_up) nw_up,   E_r = ceil(width_down / og_down) nw_down.
  * So dfb_stream_latency_frames is L + 1 (the hops a flush returns and a closing slot drains for), and
- * dfb_stream_latency_samples the signal delay beyond the 48 kHz handle's, D_r r / 48000 + E_r, always below one hop:
+ * dfb_stream_latency_samples the signal delay beyond the 48 kHz handle's, D_r r / 48000 + E_r, always below one hop.  The
+ * same holds for every session at rate r: on a handle at r, and in a slot opened at r on a mixed-rate handle
+ * (dfb_stream_add_slot_rate below):
  *      r    h_r  og/nw/width up  D_r   og/nw/width down  E_r   delay (samples / ms)
  *    8000    80     1/6/17       102       6/1/97         17     34 / 4.25
  *   12000   120     1/4/17        68       4/1/65         17     34 / 2.833
@@ -381,6 +383,47 @@ int64_t dfb_stream_latency_samples(const dfb_stream *s);   /* D_r r / 48000 + E_
  * h_r at r.  Row c of d_out is the resampled row delayed by D_r (up) or E_r (down) output samples, bit for bit. */
 int dfb_debug_resample_stream(int up, int rate, const float *d_taps, int og, int nw, int width, const float *d_in, int64_t C,
                               const int64_t *h_calls, int64_t n_calls, float *d_out, void *stream);
+
+/* Mixed-rate handle: a 48 kHz audio handle whose slots each run at their own rate, so that calls at different rates share
+ * one pass through the slot path.  dfb_stream_add_slot_rate registers rate r (one of the rates above, with the arguments
+ * of dfb_stream_set_sample_rate); a handle may register several.  Sessions then open at r with dfb_stream_open_slots_at /
+ * dfb_stream_open_linked_at (a group at one rate, under the rules of dfb_stream_open_linked), and at 48 kHz with those
+ * and rate 48000, or with dfb_stream_open_slots / dfb_stream_open_linked; dfb_stream_reset reopens every slot at 48 kHz.
+ *   Row layout: rows stay 480 samples per hop.  dfb_stream_process takes and returns [B][n * 480], and
+ *   dfb_stream_frame_length is 480.  A slot at rate r reads the first n h_r samples of its input row and ignores the
+ *   rest; its output row carries n h_r samples followed by exact zeros.  The _host and _lsnr variants keep these
+ *   meanings, and LSNR rows are one value per hop as on every handle.
+ *   Composition: a slot at r outputs, over the first n h_r samples of each call, exactly what a handle at r
+ *   (dfb_stream_set_sample_rate) with one slot outputs for that session: the composition above, ended by its close and
+ *   L + 1 drain hops or by flush.  A 48 kHz slot outputs what a 48 kHz handle with one slot does (its resamplers copy
+ *   its rows value for value: a -0 comes out as +0), and drains for L hops after its close.  Linked groups, per-slot settings, LSNR rows and stage
+ *   gating behave as on a handle at the session's rate.
+ *   Drain: dfb_stream_latency_frames is L + 1, the longest drain of any slot, and dfb_stream_latency_samples is 0 (a
+ *   48 kHz slot's); a session at r has the latency of a handle at r, from the table above.  dfb_stream_flush returns
+ *   [B][(L + 1) * 480]: a 48 kHz slot's L tail hops, then one hop of zeros; a slot at r its L + 1 tail hops of h_r
+ *   samples each, each row followed by zeros to its end.
+ * Errors (DFB_ERR_INVALID unless said otherwise): registering after the handle's first frame or a slot operation (the
+ * registrations themselves survive dfb_stream_reset), on a spectral handle, or on a handle set to another rate than
+ * 48000; taps of another rate or geometry; a rate outside the list (DFB_ERR_UNSUPPORTED).  Opening at a rate the handle has
+ * not registered, or on a handle without slot rates; opening at a rate outside the list and 48000 (DFB_ERR_UNSUPPORTED).
+ * dfb_stream_set_sample_rate of a mixed-rate handle to another rate than 48000 (48000 changes nothing).  Registering a
+ * rate twice registers it once. */
+int dfb_stream_add_slot_rate(dfb_stream *s, int rate, const float *up_taps, int up_og, int up_nw, int up_width,
+                             const float *down_taps, int down_og, int down_nw, int down_width);
+int dfb_stream_open_slots_at(dfb_stream *s, const int64_t *slots, int64_t n, int rate);
+int dfb_stream_open_linked_at(dfb_stream *s, const int64_t *slots, int64_t n, int rate);
+/* h_rates [B]: the rate of each live slot's session (the handle's rate on a handle at one rate, 48000 on a 48 kHz one),
+ * 0 for a free slot.  A spectral handle: DFB_ERR_INVALID. */
+int dfb_stream_slot_rates(const dfb_stream *s, int32_t *h_rates);
+/* Debug aid: both resamplers of a handle on their own, with its own taps (up != 0: k_resample_up, else k_resample_down),
+ * row c in the direction of rate h_rates[c] (HOST array; a rate the handle runs: its registered rates and 48000 on a
+ * mixed-rate handle, its rate on a handle at one rate; else DFB_ERR_INVALID).  Every row is one session from hop 0, run
+ * through the calls h_calls[0 .. n_calls) (HOST array of hop counts >= 1) with its histories carried: d_in f32[C][H * 480]
+ * -> d_out f32[C][H * 480], H = sum of the calls.  Row c reads its first H hop_in samples and writes H hop_out samples
+ * (hop = 480 at 48 kHz and h_r at r) followed by zeros: its row resampled and delayed by D_r (up) or E_r (down) output
+ * samples, bit for bit, and a 48 kHz row copied (a -0 as +0). */
+int dfb_debug_resample_slots(int up, const dfb_stream *s, const int32_t *h_rates, const float *d_in, int64_t C,
+                             const int64_t *h_calls, int64_t n_calls, float *d_out, void *stream);
 
 /* Spectral streaming handle (capi.rs df_process_frame_raw, DfTract::process_raw, tract.rs:441-506): the caller runs its own
  * filter bank, passes spectrum frames in and gets the network's outputs back -- ERB gains, deep-filter coefficients, LSNR
