@@ -156,6 +156,48 @@ struct ResampleIO {
     float *out, *hist;
     int64_t in_pitch, out_pitch, out_w, hist_pitch, in_col, out_col, n, a0, tail;
 };
+// One direction of a model's offline resampler (dfb_model_add_rate; DESIGN.md section 5i): torchaudio's sinc taps
+// [nw][K = 2 width + og] for the gcd-reduced rates og -> nw.  Output t of a stream is sum_k taps[t % nw][k] x[(t / nw) og -
+// width + k] over k = 0 .. K-1 in that order, taps outside the stream's input skipped: k_resample's sum, bit for bit.
+struct RateDir { const float *taps; int og, nw, K, width; };
+// A stream of a rated batch (dfb_enhance_ragged_rates) as a resampler launch sees it: in_len input samples at in + in_off,
+// out_len outputs at out + out_off, its direction (-1: a 48 kHz stream, which no resampler touches) and its 48 kHz frame
+// count tf (it has ended, every 48 kHz output written, once the chunk loop's DNN frames reach tf).
+struct RateRow { int64_t in_off, in_len, out_off, out_len, tf; int dir; };
+// The buffers and range of one launch.  Up (rate r -> 48 kHz): every row writes its outputs [lo, hi), clipped to its length.
+// Down (48 kHz -> r): a row's input is written up to sample w, or entirely once it has ended; it writes the outputs whose
+// taps all lie below w, from those complete at (w, d) = (lo, d_lo), which an earlier launch wrote, to those at (hi, d_hi).
+struct RateIO { const float *in; float *out; int64_t lo, hi, d_lo, d_hi; };
+
+// Down direction: the outputs of row r complete once its input is written up to w (all of them when it has ended).  Output
+// block i's last tap is input i og + width + og - 1.
+__host__ __device__ __forceinline__ int64_t rate_down_ready(const RateDir &d, const RateRow &r, int64_t w, bool ended) {
+    if (ended || w >= r.in_len) return r.out_len;
+    const int64_t span = (int64_t)d.width + d.og;
+    if (w < span) return 0;
+    const int64_t n = ((w - span) / d.og + 1) * d.nw;
+    return n < r.out_len ? n : r.out_len;
+}
+// Up direction: the input samples the outputs below x read (their taps past the stream's end are skipped).
+__host__ __device__ __forceinline__ int64_t rate_up_need(const RateDir &d, const RateRow &r, int64_t x) {
+    if (x > r.out_len) x = r.out_len;
+    if (x <= 0) return 0;
+    const int64_t n = ((x - 1) / d.nw) * d.og + d.width + d.og;
+    return n < r.in_len ? n : r.in_len;
+}
+// The outputs [*o0, *o1) row r writes in launch io.
+__host__ __device__ __forceinline__ void rate_range(bool up, const RateDir &d, const RateRow &r, const RateIO &io, int64_t *o0,
+                                                    int64_t *o1) {
+    if (up) {
+        *o0 = io.lo < r.out_len ? io.lo : r.out_len;
+        *o1 = io.hi < r.out_len ? io.hi : r.out_len;
+    } else {
+        *o0 = rate_down_ready(d, r, io.lo, r.tf <= io.d_lo);
+        *o1 = rate_down_ready(d, r, io.hi, r.tf <= io.d_hi);
+    }
+    if (*o1 < *o0) *o1 = *o0;
+}
+
 // Per-slot settings of a streaming handle (dfb_stream_set_atten_lim / _post_filter_beta): limit (0 = off) and post-filter
 // beta (0 = off) from absolute frame sw on, and the previous ones before it.  Only the frame before sw, re-synthesised
 // for its overlap-add tail, still reads the previous ones.
@@ -260,6 +302,12 @@ int launch_apply_synthesis(dfb_state *st, const ApplyParams &p, int64_t B, cudaS
 // no input; down: zeros from hop end + tail on).
 int launch_resample_stream(cudaStream_t s, bool up, const ResampleDirs &dirs, int n_dirs, const ResampleRow *rows, int nb,
                            const ResampleIO &io);
+// One launch of the offline resampler (k_resample_rows) over the rows [0, nb) of a rated batch: d_dirs / d_rows on the
+// device, max_out the most outputs any row writes in it.  A direction of at most smem_floats taps (<= kRateSmemFloats) is
+// read from shared memory.
+constexpr int kRateSmemFloats = 12288;   // 48 KB: no opt-in, and at least four CTAs per SM
+int launch_resample_rows(cudaStream_t s, bool up, const RateDir *d_dirs, const RateRow *d_rows, int nb, const RateIO &io,
+                         int64_t max_out, int smem_floats);
 // time window of a recurrence launch: steps 0 .. T-1 are frames t0 .. of buffers holding Ts frames per stream; h0 (null:
 // zeros) / hT (null: not stored) are the carried hidden states [B][H]
 struct GruWindow { const float *h0; float *hT; int t0, Ts; const int64_t *first = nullptr; int64_t w0 = 0; /* stream_first */ };

@@ -372,6 +372,53 @@ __global__ void __launch_bounds__(256) k_resample_down(ResampleDirs dirs, const 
                  io.out + r.slot * io.out_pitch + io.out_col * d.hop_out, v * d.hop_out, fill_to(io, d));
 }
 
+// Offline resampler of a rated batch (dfb_enhance_ragged_rates; RateDir / RateRow / RateIO in dfb_common.cuh; DESIGN.md
+// section 5i).  The whole input of a stream is on the device, so no history is carried: an output reads its taps straight
+// from the input, and an output is computed once, by the launch in whose range it falls.  Grid (tiles, rows): CTA (x, b)
+// writes row b's outputs [o0 + x kRateTile, o0 + (x + 1) kRateTile) of its range [o0, o1), so a row's outputs spread over
+// as many CTAs as they fill, and a CTA holds its row's taps in shared memory when they fit.  The sum runs over the taps
+// inside the input in k order from +0, which is k_resample's sum with the taps outside skipped.
+constexpr int kRateTile = 1024;
+template <bool kSmemTaps>
+__device__ __forceinline__ void resample_tile(const float *__restrict__ taps, const RateDir &d, const float *__restrict__ x,
+                                              int64_t n_in, float *__restrict__ y, int64_t t0, int64_t t1) {
+    for (int64_t t = t0 + threadIdx.x; t < t1; t += blockDim.x) {
+        const int64_t i = t / d.nw;
+        const int j = (int)(t - i * d.nw);
+        const int64_t p0 = i * d.og - d.width;
+        const int k0 = p0 < 0 ? (int)-p0 : 0;
+        const int64_t e = n_in - p0;
+        const int k1 = e < d.K ? (int)e : d.K;
+        const float *kr = taps + (size_t)j * d.K;
+        float acc = 0.f;
+        for (int k = k0; k < k1; k++) acc = fmaf(kSmemTaps ? kr[k] : __ldg(kr + k), __ldg(x + p0 + k), acc);
+        y[t] = acc;
+    }
+}
+
+__global__ void __launch_bounds__(256) k_resample_rows(const RateDir *__restrict__ dirs, const RateRow *__restrict__ rows, RateIO io,
+                                                       bool up, int smem_floats) {
+    const RateRow r = rows[blockIdx.y];
+    if (r.dir < 0) return;
+    const RateDir d = dirs[r.dir];
+    int64_t o0, o1;
+    rate_range(up, d, r, io, &o0, &o1);
+    const int64_t t0 = o0 + (int64_t)blockIdx.x * kRateTile;
+    if (t0 >= o1) return;   // (uniform over the CTA)
+    const int64_t t1 = o1 - t0 < kRateTile ? o1 : t0 + kRateTile;
+    const float *x = io.in + r.in_off;
+    float *y = io.out + r.out_off;
+    const int nk = d.nw * d.K;
+    if (nk <= smem_floats) {
+        extern __shared__ float s_taps[];
+        for (int i = threadIdx.x; i < nk; i += blockDim.x) s_taps[i] = __ldg(d.taps + i);
+        __syncthreads();
+        resample_tile<true>(s_taps, d, x, r.in_len, y, t0, t1);
+    } else {
+        resample_tile<false>(d.taps, d, x, r.in_len, y, t0, t1);
+    }
+}
+
 // ------------------------------------------------------------- feature norm scans ----
 // Exponential mean norm of the ERB dB features and exponential unit norm of the first Fd bins,
 // sequential in t per (stream, band | bin) exactly like the reference loops.
@@ -1508,6 +1555,18 @@ int launch_resample_stream(cudaStream_t s, bool up, const ResampleDirs &dirs, in
         k_resample_up<<<nb, 256, 0, s>>>(dirs, rows, io);
     else
         k_resample_down<<<nb, 256, 0, s>>>(dirs, rows, io);
+    DFB_LAUNCH_CHECK();
+    return DFB_OK;
+}
+
+int launch_resample_rows(cudaStream_t s, bool up, const RateDir *d_dirs, const RateRow *d_rows, int nb, const RateIO &io,
+                         int64_t max_out, int smem_floats) {
+    if (nb <= 0 || max_out <= 0) return DFB_OK;
+    if (nb > 65535 || smem_floats < 0 || smem_floats > kRateSmemFloats) return fail(DFB_ERR_INVALID, "bad resampler geometry");
+    const int64_t tiles = (max_out + kRateTile - 1) / kRateTile;
+    // (not in the DFB_PROF timing, which covers the 48 kHz enhancement path; torch.profiler names it)
+    k_resample_rows<<<dim3((unsigned)tiles, (unsigned)nb), 256, sizeof(float) * (size_t)smem_floats, s>>>(d_dirs, d_rows, io, up,
+                                                                                                          smem_floats);
     DFB_LAUNCH_CHECK();
     return DFB_OK;
 }

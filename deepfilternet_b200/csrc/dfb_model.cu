@@ -524,6 +524,12 @@ struct dfb_model {
                     ev_out = nullptr, ev_c0 = nullptr, ev_convp = nullptr, ev_skip = nullptr, ev_done = nullptr;
     } lanes[2];
     Arena arena1;                           // lane 1's activations (lane 0 uses `arena`)
+    // offline resamplers of rated batches (dfb_model_add_rate): the registered rates, their directions (rate_up[i] /
+    // rate_down[i] for rates[i]; on the device as [up directions | down directions]) and their tap buffers
+    std::vector<int> rates;
+    std::vector<RateDir> rate_up, rate_down;
+    std::vector<float *> rate_taps;
+    RateDir *d_rate_dirs = nullptr;
 };
 
 // Looks the uploaded tensors up by name.  The first missing or wrong-sized one (numel < 0: any size) becomes the bind's
@@ -711,6 +717,8 @@ extern "C" void dfb_model_free(dfb_model *m) {
     if (m->h2d) cudaStreamDestroy(m->h2d);
     if (m->d2h) cudaStreamDestroy(m->d2h);
     if (m->slab) cudaFree(m->slab);
+    for (float *p : m->rate_taps) cudaFree(p);
+    if (m->d_rate_dirs) cudaFree(m->d_rate_dirs);
     if (m->stream) cudaStreamDestroy(m->stream);
     for (auto &L : m->lanes) {
         for (cudaStream_t st : {L.main, L.hi, L.aux, L.dhi, L.daux, L.low})
@@ -1536,6 +1544,75 @@ extern "C" int64_t dfb_enhance_out_len(const dfb_state *st, int64_t T, int pad) 
     return pad ? T : (T / st->hop) * st->hop;
 }
 
+constexpr int kModelRate = 48000;   // the model's rate: 480-sample hops of the 960 / 480 STFT
+
+// A stream of T samples at `rate` resampled to 48 kHz: ceil(T * 48000 / rate) samples (io.resample's length)
+static int64_t len_at_48k(int64_t T, int rate) {
+    const int64_t g = std::gcd(rate, kModelRate), og = rate / g, nw = kModelRate / g;
+    return (T * nw + og - 1) / og;
+}
+static int64_t len_from_48k(int64_t T48, int rate) {
+    const int64_t g = std::gcd(rate, kModelRate), og = kModelRate / g, nw = rate / g;
+    return (T48 * nw + og - 1) / og;
+}
+
+extern "C" int64_t dfb_enhance_out_len_at(const dfb_state *st, int64_t T, int pad, int rate) {
+    if (!st || T <= 0 || rate <= 0) return -1;
+    if (rate == kModelRate) return dfb_enhance_out_len(st, T, pad);
+    return len_from_48k(dfb_enhance_out_len(st, len_at_48k(T, rate), pad), rate);
+}
+
+// The taps of rated batches at `rate` (DESIGN.md section 5i): both directions of io.resample_kernel's sinc_fast taps,
+// at most kMaxRateTaps floats together.  48000 registers nothing (a 48 kHz stream is never resampled).
+constexpr int64_t kMaxRateTaps = int64_t(1) << 18;
+extern "C" int dfb_model_add_rate(dfb_model *m, int rate, const float *up_taps, int up_og, int up_nw, int up_width,
+                                  const float *down_taps, int down_og, int down_nw, int down_width) {
+    if (!m) return fail(DFB_ERR_INVALID, "null model");
+    if (rate == kModelRate) return DFB_OK;
+    if (rate <= 0) return fail(DFB_ERR_UNSUPPORTED, "sample rate %d Hz", rate);
+    const int g = std::gcd(rate, kModelRate);
+    if (up_og != rate / g || up_nw != kModelRate / g || down_og != kModelRate / g || down_nw != rate / g)
+        return fail(DFB_ERR_INVALID, "the taps of %d Hz are io.resample_kernel(%d, 48000) (og %d, nw %d) and (48000, %d) (og %d, nw %d)",
+                    rate, rate, rate / g, kModelRate / g, rate, kModelRate / g, rate / g);
+    if (up_width <= 0 || down_width <= 0 || up_width > (1 << 20) || down_width > (1 << 20))
+        return fail(DFB_ERR_INVALID, "the taps of %d Hz have widths %d / %d", rate, up_width, down_width);
+    const int64_t nu = (int64_t)up_nw * (2 * up_width + up_og), nd = (int64_t)down_nw * (2 * down_width + down_og);
+    if (nu + nd > kMaxRateTaps)
+        return fail(DFB_ERR_UNSUPPORTED, "sample rate %d Hz: its resampler taps hold %lld floats, more than 2^18", rate,
+                    (long long)(nu + nd));
+    if (!up_taps || !down_taps) return fail(DFB_ERR_INVALID, "null taps");
+    if (std::find(m->rates.begin(), m->rates.end(), rate) != m->rates.end()) return DFB_OK;
+    DFB_CUDA(cudaSetDevice(m->device));
+    float *taps = nullptr;
+    RateDir *dirs = nullptr;
+    const size_t n = m->rates.size() + 1;
+    if (cudaMalloc(&taps, sizeof(float) * (size_t)(nu + nd)) != cudaSuccess || cudaMalloc(&dirs, sizeof(RateDir) * 2 * n) != cudaSuccess) {
+        if (taps) cudaFree(taps);
+        return fail(DFB_ERR_OOM, "resampler taps allocation failed");
+    }
+    std::vector<RateDir> up = m->rate_up, down = m->rate_down, all;
+    up.push_back(RateDir{taps, up_og, up_nw, 2 * up_width + up_og, up_width});
+    down.push_back(RateDir{taps + nu, down_og, down_nw, 2 * down_width + down_og, down_width});
+    all = up;
+    all.insert(all.end(), down.begin(), down.end());
+    // (synchronous: a call still running reads the old table, which is freed below)
+    if (cudaMemcpy(taps, up_taps, sizeof(float) * (size_t)nu, cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaMemcpy(taps + nu, down_taps, sizeof(float) * (size_t)nd, cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaMemcpy(dirs, all.data(), sizeof(RateDir) * all.size(), cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaDeviceSynchronize() != cudaSuccess) {
+        cudaFree(taps);
+        cudaFree(dirs);
+        return fail(DFB_ERR_CUDA, "resampler taps upload failed");
+    }
+    if (m->d_rate_dirs) cudaFree(m->d_rate_dirs);
+    m->d_rate_dirs = dirs;
+    m->rates.push_back(rate);
+    m->rate_up.swap(up);
+    m->rate_down.swap(down);
+    m->rate_taps.push_back(taps);
+    return DFB_OK;
+}
+
 // enhance(): df/enhance.py:206-250.  Streams are processed in groups so that the workspace stays
 // below the model's workspace cap (40 GB by default; dfb_model_set_max_workspace / DFB_MAX_WORKSPACE_MB); streams
 // are independent (per-channel state reset, pyDF/src/lib.rs:56-58).
@@ -1974,9 +2051,11 @@ static int pick_chunk(const dfb_model *m, const dfb_state *st, int64_t B, int64_
     if (tc < Tf && tc < 32) return 0;   // a chunk this short wastes most of its window on the halo: use stream groups
     return (int)tc;
 }
-// Hooks around every chunk of a stream group whose buffers are staged (host batch).  `cs` is the stream the chunk's compute
-// is enqueued on (it must wait for the input / produces the output); only the first `na` streams take part in the chunk.
+// Hooks around every chunk of a stream group whose buffers are staged (host batch, rated batch).  `cs` is the stream the
+// chunk's compute is enqueued on (it must wait for the input / produces the output); only the first `na` streams take part
+// in the chunk.  `pcie`: the hooks copy over PCIe, and the end chunks are tapered so that their copies overlap more.
 struct ChunkHooks {
+    bool pcie = false;
     // the chunk's analysis reads input samples [x0, x1) of every stream (as far as the stream has them)
     std::function<int(int64_t x0, int64_t x1, int64_t na, cudaStream_t cs)> before;
     // output samples [y0, y1) of every stream have been written; a stream whose frame count is <= d1 (the chunk's last DNN
@@ -2012,7 +2091,7 @@ static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, float *d
     int chunk = 0, last_lane = 0;
     // Host path: the first chunk's H2D copy and the last chunk's D2H copy are the only ones nothing overlaps, so both end
     // chunks are half as long as the others (128 x 10 s in 4 chunks: 250 / 250 / 250 / 252 frames -> 125 / 250 / 250 / 250 / 127).
-    const bool taper = hooks && pipelined && tc < Tf && tc >= 64;
+    const bool taper = hooks && hooks->pcie && pipelined && tc < Tf && tc >= 64;
     while (S.d1 < Tf) {
         int64_t step = tc;
         if (taper) {
@@ -2032,6 +2111,11 @@ static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, float *d
         ChunkIO io{d_x, Tf * hop, 0, nullptr, d_out, 0, 0, delay, lim, nullptr, rows, (int)na, links, reduce};
         if ((rc = run_chunk(m, st, S, io, a1n, d1n, e1n > S.e1 ? e1n : S.e1, cs, lane, pipelined))) break;
         if (hooks && (rc = hooks->after(e0 * hop > delay ? e0 * hop - delay : 0, S.e1 * hop - delay, d1n, na, cs))) break;
+        // what the hook enqueued on the lane is part of the chunk: the caller's stream and the next chunk's decoder wait for it
+        if (hooks && pipelined && cudaEventRecord(m->lanes[lane].ev_done, cs) != cudaSuccess) {
+            rc = fail(DFB_ERR_CUDA, "chunk event record failed");
+            break;
+        }
         last_lane = lane;
         chunk++;
     }
@@ -2166,30 +2250,39 @@ static int link_plan(const dfb_model *m, const std::vector<RaggedRow> &rows, con
 // packed back to back, chunk by chunk and each stream's range clipped to its length -- the H2D copy of chunk c + 1 and the
 // D2H copy of chunk c - 1 run on their own streams (both copy engines) while chunk c computes -- and the call is synchronous.
 // `links` (or null): each stream's link group from link_plan, sorted here along with `rows`; `reduce` the mask reduction.
+// `rates` (or null): a rated batch (rates_plan; DESIGN.md section 5i).  `rows` are then the streams at 48 kHz, which is what
+// the chunk loop runs, and rates[b] is stream b at its own rate: the caller's buffers hold that.  Every stream group is
+// staged in 48 kHz device buffers (a host batch also in staging buffers at the streams' rates); per chunk, before the
+// analysis, the up-resampler writes the 48 kHz samples it reads, and after apply + synthesis the down-resampler writes the
+// outputs that became complete.  48 kHz streams are copied, never resampled.
 static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &rows, const float *src, float *dst, int pad,
-                        float atten_lim_db, bool host, cudaStream_t s, std::vector<LinkRow> *links = nullptr, int reduce = 0) {
+                        float atten_lim_db, bool host, cudaStream_t s, std::vector<LinkRow> *links = nullptr, int reduce = 0,
+                        std::vector<RateRow> *rates = nullptr) {
     const int64_t B = (int64_t)rows.size();
     int64_t min_group = 1;   // the largest link group: a stream group never splits one
-    if (!links) {
-        std::stable_sort(rows.begin(), rows.end(), [](const RaggedRow &a, const RaggedRow &b) { return a.Tf > b.Tf; });
-    } else {
+    {
         // The members of a link group are consecutive and share their sort key (one length), so the stable sort keeps them
         // one contiguous run in their own order: nothing between them has that key.  Sorting a permutation carries each
-        // stream's group along, as the new position of the group's first member.
+        // stream's group along, as the new position of the group's first member, and its rate.
         std::vector<int64_t> idx((size_t)B);
         std::iota(idx.begin(), idx.end(), (int64_t)0);
         std::stable_sort(idx.begin(), idx.end(), [&](int64_t a, int64_t b) { return rows[(size_t)a].Tf > rows[(size_t)b].Tf; });
         std::vector<RaggedRow> sr((size_t)B);
-        std::vector<LinkRow> sl((size_t)B);
+        std::vector<LinkRow> sl(links ? (size_t)B : 0);
+        std::vector<RateRow> sq(rates ? (size_t)B : 0);
         for (int64_t i = 0; i < B; i++) {
             const int64_t o = idx[(size_t)i];
-            const LinkRow g = (*links)[(size_t)o];
             sr[(size_t)i] = rows[(size_t)o];
-            sl[(size_t)i] = LinkRow{(int)(i - (o - g.first)), g.n};
-            min_group = std::max(min_group, (int64_t)g.n);
+            if (rates) sq[(size_t)i] = (*rates)[(size_t)o];
+            if (links) {
+                const LinkRow g = (*links)[(size_t)o];
+                sl[(size_t)i] = LinkRow{(int)(i - (o - g.first)), g.n};
+                min_group = std::max(min_group, (int64_t)g.n);
+            }
         }
         rows.swap(sr);
-        links->swap(sl);
+        if (links) links->swap(sl);
+        if (rates) rates->swap(sq);
     }
     std::vector<int64_t> tfs((size_t)B);
     int64_t true_frames = 0;
@@ -2211,7 +2304,7 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
     if (rc) return rc;
     size_t off[16];   // the aux arena holds one group's state slab and tables
     if ((rc = m->aux_arena.reserve(state_floats(m->cfg, st, (int)group, off) * sizeof(float) +
-                                   (size_t)group * (sizeof(RaggedRow) + sizeof(LinkRow)) + 8192)))
+                                   (size_t)group * (sizeof(RaggedRow) + sizeof(LinkRow) + (rates ? 2 * sizeof(RateRow) : 0)) + 8192)))
         return rc;
     // stream groups: up to `group` streams, cut only between link groups (group >= every link group, so a cut inside one
     // moves back to its first member, past b0); DeepFilterNet v1: of one frame count
@@ -2232,24 +2325,54 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
             for (int64_t i = b0; i < b1; i++) dlinks[(size_t)i].first -= (int)b0;
         }
     }
-    // device rows: the streams themselves, or (host) their places in the staging buffers, sized for the largest group
+    // device rows: the streams themselves, or (host, rated) their places in the staging buffers, sized for the largest group.
+    // A rated host batch also stages its streams at their own rates: ur / dr_ are the up / down resamplers' rows.
+    const bool staged = host || rates;
     std::vector<RaggedRow> drows(rows);
-    float *d_in = nullptr, *d_out = nullptr;
-    if (host) {
-        int64_t n_in = 0, n_out = 0;
+    std::vector<RateRow> ur, dr_;
+    float *d_in = nullptr, *d_out = nullptr, *d_rin = nullptr, *d_rout = nullptr;
+    int smem_up = 0, smem_down = 0;
+    if (staged) {
+        int64_t n_in = 0, n_out = 0, n_rin = 0, n_rout = 0;
+        if (rates) { ur = *rates; dr_ = *rates; }
         for (int64_t b0 = 0, b1; b0 < B; b0 = b1) {
             b1 = group_end(b0);
-            int64_t gi = 0, go = 0;
+            int64_t gi = 0, go = 0, gri = 0, gro = 0;
             for (int64_t i = b0; i < b1; i++) {
                 drows[i].in_off = gi; drows[i].out_off = go;
                 gi += rows[i].len; go += rows[i].out_len;
+                if (!rates) continue;
+                const RateRow &q = (*rates)[(size_t)i];
+                ur[i] = RateRow{q.in_off, q.in_len, drows[i].in_off, rows[i].len, q.tf, q.dir};
+                dr_[i] = RateRow{drows[i].out_off, rows[i].out_len, q.out_off, q.out_len, q.tf, q.dir};
+                if (q.dir < 0) continue;
+                if (host) {
+                    ur[i].in_off = gri; dr_[i].out_off = gro;
+                    gri += q.in_len; gro += q.out_len;
+                }
+                const RateDir &u = m->rate_up[(size_t)q.dir], &d = m->rate_down[(size_t)q.dir];
+                if (u.nw * u.K <= kRateSmemFloats) smem_up = std::max(smem_up, u.nw * u.K);
+                if (d.nw * d.K <= kRateSmemFloats) smem_down = std::max(smem_down, d.nw * d.K);
             }
             n_in = std::max(n_in, gi); n_out = std::max(n_out, go);
+            n_rin = std::max(n_rin, gri); n_rout = std::max(n_rout, gro);
         }
-        if ((rc = st->arena.reserve(sizeof(float) * (size_t)(n_in + n_out) + 4096))) return rc;
+        if ((rc = st->arena.reserve(sizeof(float) * (size_t)(n_in + n_out + n_rin + n_rout) + 4096))) return rc;
         st->arena.reset();
         d_in = st->arena.take<float>((size_t)n_in); d_out = st->arena.take<float>((size_t)n_out);
+        if (n_rin) d_rin = st->arena.take<float>((size_t)n_rin);
+        if (n_rout) d_rout = st->arena.take<float>((size_t)n_rout);
     }
+    // the most outputs a row of rr[0, na) writes in a resampler launch
+    auto max_range = [&](bool up, const RateRow *rr, int64_t na, const RateIO &io) {
+        int64_t mx = 0, o0, o1;
+        for (int64_t i = 0; i < na; i++) {
+            if (rr[i].dir < 0) continue;
+            rate_range(up, (up ? m->rate_up : m->rate_down)[(size_t)rr[i].dir], rr[i], io, &o0, &o1);
+            mx = std::max(mx, o1 - o0);
+        }
+        return mx;
+    };
     const float lim = (atten_lim_db > 0.f) ? powf(10.f, -atten_lim_db / 20.f) : 0.f;
     cudaStream_t sc = host ? m->stream : s, sh = m->h2d, sd = m->d2h;
     std::vector<cudaEvent_t> evs;
@@ -2266,18 +2389,66 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
         const RaggedRow *hr = rows.data() + b0, *dr = drows.data() + b0;
         const int64_t *tf = tfs.data() + b0;
         ChunkHooks hooks;
-        hooks.before = [&](int64_t x0, int64_t x1, int64_t na, cudaStream_t cs) -> int {
-            const int r = copy_streams(d_in, src, x0, na, [&](int64_t i) {
-                return StreamCopy{dr[i].in_off, hr[i].in_off, std::min(x1, hr[i].len)};
-            }, cudaMemcpyHostToDevice, sh);
-            return r ? r : order(sh, cs);
-        };
-        hooks.after = [&](int64_t y0, int64_t y1, int64_t d1, int64_t na, cudaStream_t cs) -> int {
-            if (const int r = order(cs, sd)) return r;
-            return copy_streams(dst, d_out, y0, na, [&](int64_t i) {   // a stream that has ended: all of its output
-                return StreamCopy{hr[i].out_off, dr[i].out_off, tf[i] <= d1 ? hr[i].out_len : std::min(y1, hr[i].out_len)};
-            }, cudaMemcpyDeviceToHost, sd);
-        };
+        hooks.pcie = host;
+        if (!rates) {
+            hooks.before = [&](int64_t x0, int64_t x1, int64_t na, cudaStream_t cs) -> int {
+                const int r = copy_streams(d_in, src, x0, na, [&](int64_t i) {
+                    return StreamCopy{dr[i].in_off, hr[i].in_off, std::min(x1, hr[i].len)};
+                }, cudaMemcpyHostToDevice, sh);
+                return r ? r : order(sh, cs);
+            };
+            hooks.after = [&](int64_t y0, int64_t y1, int64_t d1, int64_t na, cudaStream_t cs) -> int {
+                if (const int r = order(cs, sd)) return r;
+                return copy_streams(dst, d_out, y0, na, [&](int64_t i) {   // a stream that has ended: all of its output
+                    return StreamCopy{hr[i].out_off, dr[i].out_off, tf[i] <= d1 ? hr[i].out_len : std::min(y1, hr[i].out_len)};
+                }, cudaMemcpyDeviceToHost, sd);
+            };
+        }
+        // rated batch: uh / dh the group's resampler rows, rh its streams in the caller's buffers; d_prev the DNN frames of
+        // the previous chunk (which streams had ended at its down-resampler launch)
+        const RateRow *uh = rates ? ur.data() + b0 : nullptr, *dh = rates ? dr_.data() + b0 : nullptr,
+                      *rh = rates ? rates->data() + b0 : nullptr;
+        RateRow *d_ur = nullptr, *d_dr = nullptr;
+        int64_t d_prev = 0;
+        const RateDir *d_up = m->d_rate_dirs, *d_down = m->d_rate_dirs + m->rates.size();
+        if (rates) {
+            hooks.before = [&](int64_t x0, int64_t x1, int64_t na, cudaStream_t cs) -> int {
+                // a 48 kHz stream is copied as in an unrated batch; a stream at another rate reads what its resampler needs for
+                // the 48 kHz samples below x1, its tap look-ahead included, of which earlier chunks copied those below x0's need
+                const cudaMemcpyKind kind = host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+                int r = copy_streams(d_in, src, x0, na, [&](int64_t i) {
+                    return StreamCopy{dr[i].in_off, hr[i].in_off, uh[i].dir < 0 ? std::min(x1, hr[i].len) : x0};
+                }, kind, host ? sh : cs);
+                if (!r && host)
+                    r = copy_streams(d_rin, src, 0, na, [&](int64_t i) {
+                        if (uh[i].dir < 0) return StreamCopy{0, 0, 0};
+                        const RateDir &d = m->rate_up[(size_t)uh[i].dir];
+                        const int64_t a = rate_up_need(d, uh[i], x0), b = rate_up_need(d, uh[i], x1);
+                        return StreamCopy{uh[i].in_off + a, rh[i].in_off + a, b - a};
+                    }, cudaMemcpyHostToDevice, sh);
+                if (!r && host) r = order(sh, cs);
+                if (r) return r;
+                const RateIO io{host ? d_rin : src, d_in, x0, x1, 0, 0};
+                return launch_resample_rows(cs, true, d_up, d_ur, (int)na, io, max_range(true, uh, na, io), smem_up);
+            };
+            hooks.after = [&](int64_t y0, int64_t y1, int64_t d1, int64_t na, cudaStream_t cs) -> int {
+                const RateIO io{d_out, host ? d_rout : dst, y0, y1, d_prev, d1};
+                d_prev = d1;
+                int r = launch_resample_rows(cs, false, d_down, d_dr, (int)na, io, max_range(false, dh, na, io), smem_down);
+                if (r || (host && (r = order(cs, sd)))) return r;
+                r = copy_streams(dst, d_out, y0, na, [&](int64_t i) {   // a 48 kHz stream that has ended: all of its output
+                    return StreamCopy{hr[i].out_off, dr[i].out_off,
+                                      dh[i].dir >= 0 ? y0 : tf[i] <= d1 ? hr[i].out_len : std::min(y1, hr[i].out_len)};
+                }, host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, host ? sd : cs);
+                if (r || !host) return r;
+                return copy_streams(dst, d_rout, 0, na, [&](int64_t i) {
+                    if (dh[i].dir < 0) return StreamCopy{0, 0, 0};
+                    int64_t a, b;
+                    rate_range(false, m->rate_down[(size_t)dh[i].dir], dh[i], io, &a, &b);
+                    return StreamCopy{rh[i].out_off + a, dh[i].out_off + a, b - a};
+                }, cudaMemcpyDeviceToHost, sd);
+            };
+        }
         // (host) the previous group's D2H copies read the staged output and its compute the staged input: order this
         // group's first writes after them
         if (host && ((rc = order(sd, sc)) || (rc = order(sc, sh)))) break;
@@ -2291,8 +2462,15 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
             if (!d_links) { rc = fail(DFB_ERR_OOM, "link table arena exhausted"); break; }
             DFB_CUDA(cudaMemcpyAsync(d_links, dlinks.data() + b0, sizeof(LinkRow) * (b1 - b0), cudaMemcpyHostToDevice, sc));
         }
-        rc = enhance_group(m, st, host ? d_in : src, host ? d_out : dst, d_rows, tf, b1 - b0, pad, lim, tc, pipelined, sc,
-                           host ? &hooks : nullptr, d_links, links ? reduce : 0);
+        if (rates) {
+            d_ur = m->aux_arena.take<RateRow>((size_t)(b1 - b0));
+            d_dr = m->aux_arena.take<RateRow>((size_t)(b1 - b0));
+            if (!d_ur || !d_dr) { rc = fail(DFB_ERR_OOM, "resampler table arena exhausted"); break; }
+            DFB_CUDA(cudaMemcpyAsync(d_ur, uh, sizeof(RateRow) * (b1 - b0), cudaMemcpyHostToDevice, sc));
+            DFB_CUDA(cudaMemcpyAsync(d_dr, dh, sizeof(RateRow) * (b1 - b0), cudaMemcpyHostToDevice, sc));
+        }
+        rc = enhance_group(m, st, staged ? d_in : src, staged ? d_out : dst, d_rows, tf, b1 - b0, pad, lim, tc, pipelined, sc,
+                           staged ? &hooks : nullptr, d_links, links ? reduce : 0);
     }
     if (host) {
         const cudaError_t e1 = cudaStreamSynchronize(sc), e2 = cudaStreamSynchronize(sd), e3 = cudaStreamSynchronize(sh);
@@ -2386,6 +2564,133 @@ extern "C" int dfb_enhance_ragged_linked_host(dfb_model *m, dfb_state *st, const
     if (int rc = link_plan(m, rows, group_sizes, n_groups, reduce_mask, links)) return rc;
     DFB_CUDA(cudaSetDevice(m->device));
     return enhance_rows(m, st, rows, h_audio, h_out, pad, atten_lim_db, true, nullptr, links.empty() ? nullptr : &links, reduce_mask);
+}
+
+// ============================================================== rated batches ====
+// dfb_enhance_ragged_rates (DESIGN.md section 5i): stream b is lengths[b] samples at rates[b].  The chunk loop runs its
+// 48 kHz signal, ceil(lengths[b] 48000 / rate) samples (io.resample's length), so rows are planned from the 48 kHz lengths
+// and sorting, stream groups, the active prefix and link groups work unchanged; its output is the 48 kHz output resampled
+// back, ceil(out48 rate / 48000) samples.  Validates the call: `rows` at 48 kHz (offsets the caller's, used for 48 kHz
+// streams only), `rr` the streams at their rates with their directions of the model's resamplers (-1: 48 kHz), `links`
+// as link_plan (a group of one rate and one length), and *rated whether any stream is at another rate than 48 kHz.
+static int rates_plan(const dfb_model *m, const dfb_state *st, int64_t in_numel, const int64_t *in_offsets, const int64_t *lengths,
+                      int64_t B, int pad, int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes,
+                      int64_t n_groups, int reduce, const int32_t *rates, std::vector<RaggedRow> &rows, std::vector<RateRow> &rr,
+                      std::vector<LinkRow> &links, bool *rated) {
+    if (!in_offsets || !lengths || !out_offsets || !rates) return fail(DFB_ERR_INVALID, "null argument");
+    if (B <= 0) return fail(DFB_ERR_INVALID, "empty batch");
+    rows.resize((size_t)B);
+    rr.resize((size_t)B);
+    *rated = false;
+    for (int64_t b = 0; b < B; b++) {
+        const int64_t len = lengths[b], io = in_offsets[b], oo = out_offsets[b];
+        const int rate = rates[b];
+        int dir = -1;
+        if (rate != kModelRate) {
+            const auto it = std::find(m->rates.begin(), m->rates.end(), rate);
+            if (it == m->rates.end())
+                return fail(DFB_ERR_INVALID, "stream %lld: sample rate %d Hz is not registered (dfb_model_add_rate)", (long long)b, rate);
+            dir = (int)(it - m->rates.begin());
+            *rated = true;
+        }
+        if (len <= 0) return fail(DFB_ERR_INVALID, "stream %lld has length %lld", (long long)b, (long long)len);
+        const int64_t len48 = dir < 0 ? len : len_at_48k(len, rate), tf = (pad ? len48 + st->fft : len48) / st->hop,
+                      ol48 = dfb_enhance_out_len(st, len48, pad), ol = dir < 0 ? ol48 : len_from_48k(ol48, rate);
+        if (tf <= 0) return fail(DFB_ERR_INVALID, "stream %lld is shorter than one hop at 48 kHz", (long long)b);
+        if (io < 0 || io > in_numel - len)
+            return fail(DFB_ERR_INVALID, "stream %lld reaches outside the input (%lld samples)", (long long)b, (long long)in_numel);
+        if (oo < 0 || oo > out_numel - ol)
+            return fail(DFB_ERR_INVALID, "stream %lld reaches outside the output (%lld samples)", (long long)b, (long long)out_numel);
+        rows[(size_t)b] = RaggedRow{io, len48, oo, ol48, tf};
+        rr[(size_t)b] = RateRow{io, len, oo, ol, tf, dir};
+    }
+    links.clear();
+    if (!group_sizes) return DFB_OK;
+    if (int rc = link_plan(m, rows, group_sizes, n_groups, reduce, links)) return rc;
+    for (int64_t b = 0, g = 0; b < B; b += group_sizes[g++])
+        for (int64_t i = b + 1; i < b + group_sizes[g]; i++)
+            if (rates[i] != rates[b] || lengths[i] != lengths[b])
+                return fail(DFB_ERR_INVALID, "link group %lld mixes sample rates or lengths", (long long)g);
+    return DFB_OK;
+}
+
+static int enhance_rates(dfb_model *m, dfb_state *st, const float *src, int64_t in_numel, const int64_t *in_offsets,
+                         const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *dst, int64_t out_numel,
+                         const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
+                         const int32_t *rates, bool host, cudaStream_t s) {
+    if (!m || !st || !src || !dst) return fail(DFB_ERR_INVALID, "null argument");
+    if (int rcs = check_state(m, st)) return rcs;
+    std::vector<RaggedRow> rows;
+    std::vector<RateRow> rr;
+    std::vector<LinkRow> links;
+    bool rated = false;
+    if (int rc = rates_plan(m, st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, group_sizes, n_groups, reduce_mask,
+                            rates, rows, rr, links, &rated))
+        return rc;
+    DFB_CUDA(cudaSetDevice(m->device));
+    return enhance_rows(m, st, rows, src, dst, pad, atten_lim_db, host, s, links.empty() ? nullptr : &links, reduce_mask,
+                        rated ? &rr : nullptr);
+}
+
+extern "C" int dfb_enhance_ragged_rates(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
+                                        const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out,
+                                        int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups,
+                                        int reduce_mask, const int32_t *rates, void *stream) {
+    return enhance_rates(m, st, d_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, d_out, out_numel, out_offsets,
+                         group_sizes, n_groups, reduce_mask, rates, false, (cudaStream_t)stream);
+}
+
+extern "C" int dfb_enhance_ragged_rates_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel,
+                                             const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad, float atten_lim_db,
+                                             float *h_out, int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes,
+                                             int64_t n_groups, int reduce_mask, const int32_t *rates) {
+    return enhance_rates(m, st, h_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, h_out, out_numel, out_offsets,
+                         group_sizes, n_groups, reduce_mask, rates, true, nullptr);
+}
+
+// Debug aid: one of the model's offline resamplers alone over a ragged batch, in the launches the chunk loop would make
+extern "C" int dfb_debug_resample_rows(int up, const dfb_model *m, const float *d_in, const int64_t *in_offsets,
+                                       const int64_t *in_lengths, const int32_t *rates, int64_t B, float *d_out,
+                                       const int64_t *out_offsets, const int64_t *h_bounds, int64_t n_bounds, void *stream) {
+    if (!m || !d_in || !in_offsets || !in_lengths || !rates || !d_out || !out_offsets || !h_bounds || n_bounds <= 0 || B <= 0 ||
+        B > 65535)
+        return fail(DFB_ERR_INVALID, "bad argument");
+    std::vector<RateRow> rows((size_t)B);
+    int smem = 0;
+    for (int64_t b = 0; b < B; b++) {
+        const auto it = std::find(m->rates.begin(), m->rates.end(), (int)rates[b]);
+        if (it == m->rates.end()) return fail(DFB_ERR_INVALID, "row %lld: sample rate %d Hz is not registered", (long long)b, rates[b]);
+        if (in_lengths[b] <= 0) return fail(DFB_ERR_INVALID, "row %lld has length %lld", (long long)b, (long long)in_lengths[b]);
+        const int dir = (int)(it - m->rates.begin());
+        const RateDir &d = (up ? m->rate_up : m->rate_down)[(size_t)dir];
+        const int64_t n = up ? len_at_48k(in_lengths[b], rates[b]) : len_from_48k(in_lengths[b], rates[b]);
+        rows[(size_t)b] = RateRow{in_offsets[b], in_lengths[b], out_offsets[b], n, INT64_MAX, dir};
+        if (d.nw * d.K <= kRateSmemFloats) smem = std::max(smem, d.nw * d.K);
+    }
+    for (int64_t i = 0; i < n_bounds; i++)
+        if (h_bounds[i] <= (i ? h_bounds[i - 1] : 0)) return fail(DFB_ERR_INVALID, "chunk bounds must increase from > 0");
+    if (int rc = use_device(m->device)) return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    const RateDir *dirs = m->d_rate_dirs + (up ? 0 : m->rates.size());
+    RateRow *d_rows = nullptr;
+    int rc = DFB_OK;
+    if (cudaMalloc(&d_rows, sizeof(RateRow) * B) != cudaSuccess ||
+        cudaMemcpyAsync(d_rows, rows.data(), sizeof(RateRow) * B, cudaMemcpyHostToDevice, s) != cudaSuccess)
+        rc = fail(DFB_ERR_OOM, "debug buffers");
+    // up: launch c writes the 48 kHz outputs [bounds[c - 1], bounds[c]); down: the outputs complete once the 48 kHz input is
+    // known up to bounds[c]
+    for (int64_t i = 0; i < n_bounds && !rc; i++) {
+        const RateIO io{d_in, d_out, i ? h_bounds[i - 1] : 0, h_bounds[i], 0, 0};
+        int64_t mx = 0, o0, o1;
+        for (const RateRow &r : rows) {
+            rate_range(up != 0, (up ? m->rate_up : m->rate_down)[(size_t)r.dir], r, io, &o0, &o1);
+            mx = std::max(mx, o1 - o0);
+        }
+        rc = launch_resample_rows(s, up != 0, dirs, d_rows, (int)B, io, mx, smem);
+    }
+    cudaStreamSynchronize(s);
+    if (d_rows) cudaFree(d_rows);
+    return rc;
 }
 
 // ============================================================== streaming API ====
@@ -2779,7 +3084,6 @@ extern "C" int dfb_stream_open_linked(dfb_stream *h, const int64_t *slots, int64
 }
 
 // the rates a streaming handle resamples to and from 48 kHz (dfb_stream_set_sample_rate / dfb_stream_add_slot_rate)
-constexpr int kModelRate = 48000;   // the slot path's rate: 480-sample hops of the 960 / 480 STFT
 static bool stream_rate(int rate) {
     return rate == 8000 || rate == 12000 || rate == 16000 || rate == 24000 || rate == 32000 || rate == 44100;
 }

@@ -102,18 +102,36 @@ def df_features(audio: Tensor, df: DF, nb_df: int, device=None, alpha: Optional[
     return out
 
 
+def _rated(model: DfNet, sr, n: int):
+    """The batch calls' ``sr``: None when every entry is at 48 kHz, else the rates as int32, each registered on the model."""
+    rates = ragged.rates_arg(sr, n)
+    if rates is not None:
+        for r in sorted(set(rates.tolist())):
+            model.add_rate(r)
+    return rates
+
+
 @torch.no_grad()
 def enhance(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
-            atten_lim_db: Optional[float] = None, out: Optional[Tensor] = None, *, reduce_mask: Optional[str] = None) -> Tensor:
+            atten_lim_db: Optional[float] = None, out: Optional[Tensor] = None, *, reduce_mask: Optional[str] = None,
+            sr: Optional[int] = None) -> Tensor:
     """enhance.py:206-250: audio f32 CPU [C,T] @ model sr -> enhanced f32 CPU [C,T]
     (or [C, (T // hop) * hop], delayed by n_fft - hop, when ``pad`` is False).
     ``out`` (extension): optional preallocated (e.g. pinned) CPU tensor for the result.
     ``reduce_mask`` (extension): "max" or "mean" links the C channels as the Rust runtime does (tract.rs:868-902): they
     share one ERB mask, the max or mean of their own (include/dfb200.h, dfb_enhance_ragged_linked); None / "none": every
-    channel on its own."""
+    channel on its own.
+    ``sr`` (extension): the rate of ``audio`` when it is not the model's 48 kHz, as :func:`enhance_batch` takes it."""
     model.eval()
     if audio.dim() != 2:
         raise ValueError("audio must have shape [C, T]")
+    if _rated(model, sr, 1) is not None:
+        y = enhance_batch(model, df_state, [audio], pad, atten_lim_db, reduce_mask, sr=[sr])[0]
+        if out is None:
+            return y
+        if out.shape != y.shape or out.dtype != torch.float32 or out.is_cuda or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous float32 CPU tensor of shape {tuple(y.shape)}")
+        return out.copy_(y)
     x = audio.detach().to("cpu", torch.float32).contiguous()
     c, t = x.shape
     out_len = int(_lib.lib().dfb_enhance_out_len(df_state.handle, t, 1 if pad else 0))
@@ -162,26 +180,41 @@ def enhance_device(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
 
 @torch.no_grad()
 def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: bool = True,
-                  atten_lim_db: Optional[float] = None, reduce_mask: Optional[str] = None) -> List[Tensor]:
+                  atten_lim_db: Optional[float] = None, reduce_mask: Optional[str] = None, *, sr=None) -> List[Tensor]:
     """Several recordings of different lengths in one call: ``audios`` is a sequence of CPU [C_i, T_i] tensors as
     :func:`enhance` takes them, every channel one stream.  Entry i of the result equals
     ``enhance(model, df_state, audios[i], pad, atten_lim_db)``.  The batch is packed into one page-locked buffer and
     enhanced by one ``dfb_enhance_ragged_host`` call, which copies only the streams' own samples and computes only their
     own frames.  The results are views into one page-locked output buffer.  ``reduce_mask`` "max" / "mean": each entry's
-    channels are linked, as ``enhance(..., reduce_mask=reduce_mask)`` links them."""
+    channels are linked, as ``enhance(..., reduce_mask=reduce_mask)`` links them.
+    ``sr``: the entries' sample rate, one for all or one per entry (None: 48 kHz).  Entry i at rate r is then
+    ``io.resample(enhance(model, df_state, io.resample(audios[i], r, 48000), ...), 48000, r)``, with both resamplers run
+    on the device per time chunk so that only rate-r samples cross PCIe (dfb_enhance_ragged_rates_host; any rate whose
+    sinc_fast taps hold at most 2^18 floats, e.g. 8, 11.025, 16, 22.05, 44.1, 96 kHz)."""
     model.eval()
     xs = list(audios)
     for i, a in enumerate(xs):
         if not isinstance(a, Tensor) or a.dim() != 2:
             raise ValueError(f"entry {i}: audio must be a tensor of shape [C, T]")
-    lens, in_off, out_off, n_in, n_out, slices = ragged.packed_layout([tuple(a.shape) for a in xs], df_state.hop_size(), pad)
+    rates = _rated(model, sr, len(xs))
+    shapes = [tuple(a.shape) for a in xs]
+    if rates is None:
+        lens, in_off, out_off, n_in, n_out, slices = ragged.packed_layout(shapes, df_state.hop_size(), pad)
+    else:
+        lens, in_off, out_off, n_in, n_out, slices, srates = ragged.packed_layout_at(shapes, rates, df_state.hop_size(), pad)
     pin = torch.cuda.is_available()
     x = torch.empty(n_in, dtype=torch.float32, pin_memory=pin)
     torch.cat([a.detach().to("cpu", torch.float32).reshape(-1) for a in xs], out=x)
     y = torch.empty(n_out, dtype=torch.float32, pin_memory=pin)
     lim = abs(float(atten_lim_db)) if atten_lim_db is not None else 0.0
     reduce = ragged.reduce_code(reduce_mask)
-    if reduce == 0:
+    if rates is not None:
+        groups = ragged.packed_groups(shapes) if reduce != 0 else None
+        check(_lib.lib().dfb_enhance_ragged_rates_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
+                                                       lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
+                                                       out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
+                                                       groups.size if groups is not None else 0, reduce, srates.ctypes.data))
+    elif reduce == 0:
         check(_lib.lib().dfb_enhance_ragged_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
                                                  lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
                                                  out_off.ctypes.data))
@@ -196,14 +229,16 @@ def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: boo
 @torch.no_grad()
 def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pad: bool = True,
                           atten_lim_db: Optional[float] = None, out: Optional[Tensor] = None, group_sizes=None,
-                          reduce_mask: Optional[str] = None) -> Tensor:
+                          reduce_mask: Optional[str] = None, *, sr=None) -> Tensor:
     """Device-resident ragged batch: ``audio`` is a padded CUDA tensor [B, S] whose row b holds ``lengths[b]`` real
     samples.  Returns [B, max out_len] (asynchronous on the current stream): row b equals :func:`enhance_device` of
     ``audio[b, :lengths[b]]`` alone, and is zero beyond its own output length.  With ``out`` given, only each row's own
     output range is written.
     ``group_sizes`` / ``reduce_mask`` "max" / "mean": linked channels -- group g is the next ``group_sizes[g]`` rows, of
     one length, and they share one ERB mask; each group's rows equal :func:`enhance` of that recording with the same
-    ``reduce_mask``."""
+    ``reduce_mask``.
+    ``sr``: the rows' sample rate, one for all or one per row (a link group's rows at one rate), as :func:`enhance_batch`
+    takes it; lengths and the result are in each row's own samples (dfb_enhance_ragged_rates)."""
     if not audio.is_cuda or audio.dtype != torch.float32 or not audio.is_contiguous() or audio.dim() != 2:
         raise ValueError("enhance_device_ragged expects a contiguous float32 CUDA tensor of shape [B, S]")
     if audio.device != model.cuda_device:
@@ -213,11 +248,17 @@ def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pa
     lens = np.asarray(lens).reshape(-1)
     if lens.size != b:
         raise ValueError(f"{lens.size} lengths for {b} streams")
-    lens, in_off, out_off, ow = ragged.padded_layout(lens, s, df_state.hop_size(), pad)
+    rates = _rated(model, sr, b)
+    if rates is None:
+        lens, in_off, out_off, ow = ragged.padded_layout(lens, s, df_state.hop_size(), pad)
+    else:
+        lens, in_off, out_off, ow = ragged.padded_layout_at(lens, rates, s, df_state.hop_size(), pad)
     reduce = ragged.reduce_code(reduce_mask)
     if group_sizes is None and reduce != 0:
         raise ValueError("reduce_mask needs group_sizes: which rows are the channels of one recording")
     groups = ragged.link_groups(group_sizes, lens) if group_sizes is not None else None
+    if groups is not None and rates is not None:
+        ragged.check_group_rates(groups, rates)
     if out is None:
         out = torch.zeros((b, ow), dtype=torch.float32, device=audio.device)
     elif (out.shape != (b, ow) or out.dtype != torch.float32 or not out.is_cuda or out.device != audio.device
@@ -226,7 +267,13 @@ def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pa
     lim = abs(float(atten_lim_db)) if atten_lim_db is not None else 0.0
     with torch.cuda.device(audio.device):
         stream = torch.cuda.current_stream(audio.device).cuda_stream
-        if groups is None:
+        if rates is not None:
+            check(_lib.lib().dfb_enhance_ragged_rates(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
+                                                      lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow,
+                                                      out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
+                                                      groups.size if groups is not None else 0, reduce, rates.ctypes.data,
+                                                      stream))
+        elif groups is None:
             check(_lib.lib().dfb_enhance_ragged(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
                                                 lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow,
                                                 out_off.ctypes.data, stream))

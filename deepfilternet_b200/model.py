@@ -147,6 +147,19 @@ class DfNet(nn.Module):
     def workspace_bytes(self) -> int:
         return int(_lib.lib().dfb_model_workspace_bytes(self._h))
 
+    def add_rate(self, sr: int) -> None:
+        """Registers the resamplers of rated batches at ``sr`` (io.resample's sinc_fast taps to and from 48 kHz;
+        dfb_model_add_rate).  The batch calls' ``sr=`` registers each rate when first used; 48000 needs none."""
+        from . import io, ragged
+        sr = ragged.check_rate(sr)
+        if sr == ragged.MODEL_SR or sr in self.__dict__.setdefault("_rates", set()):
+            return
+        p = io.get_resample_params("sinc_fast")
+        ku, wu, ou, nu = io.resample_kernel(sr, ragged.MODEL_SR, **p)
+        kd, wd, od, nd = io.resample_kernel(ragged.MODEL_SR, sr, **p)
+        check(_lib.lib().dfb_model_add_rate(self._h, sr, ku.data_ptr(), ou, nu, wu, kd.data_ptr(), od, nd, wd))
+        self._rates.add(sr)
+
     # -- forward ---------------------------------------------------------------------------
     @torch.no_grad()
     def forward(self, spec: Tensor, feat_erb: Tensor, feat_spec: Tensor):

@@ -2,6 +2,7 @@
 output offsets, and their validation.  Pure functions on shapes, so they are usable and testable without the library."""
 from __future__ import annotations
 
+import math
 from typing import List, Sequence, Tuple
 
 import numpy as np
@@ -95,3 +96,109 @@ def link_groups(group_sizes, lengths) -> np.ndarray:
 def packed_groups(shapes: Sequence[Tuple[int, int]]) -> np.ndarray:
     """Link groups of a :func:`packed_layout` batch: entry i's C_i channels are one group."""
     return np.ascontiguousarray(np.array([int(shp[0]) for shp in shapes], dtype=np.int64))
+
+
+# Rated batches (dfb_enhance_ragged_rates): every stream at its own sample rate, resampled to and from the model's 48 kHz
+# with io.resample's sinc_fast taps.  A rate is supported when its two gcd-reduced tap tables hold at most MAX_RATE_TAPS
+# floats together.
+MODEL_SR = 48000
+MAX_RATE_TAPS = 1 << 18
+SINC_FAST_WIDTH, SINC_FAST_ROLLOFF = 16, 0.99   # io.get_resample_params("sinc_fast"), with resample_kernel's rolloff
+
+
+def rate_tap_floats(rate: int) -> int:
+    """Floats of the sinc_fast tap tables rate -> 48 kHz and 48 kHz -> rate together (io.resample_kernel's shapes)."""
+    n = 0
+    for orig, new in ((rate, MODEL_SR), (MODEL_SR, rate)):
+        g = math.gcd(orig, new)
+        og, nw = orig // g, new // g
+        width = math.ceil(SINC_FAST_WIDTH * og / (min(og, nw) * SINC_FAST_ROLLOFF))
+        n += nw * (2 * width + og)
+    return n
+
+
+def check_rate(rate) -> int:
+    """A sample rate as int; ValueError, naming it, for anything but a positive integer whose taps fit MAX_RATE_TAPS."""
+    if isinstance(rate, bool) or not isinstance(rate, (int, np.integer)) or int(rate) <= 0:
+        raise ValueError(f"sample rate {rate!r}: a positive integer number of Hz")
+    rate = int(rate)
+    if rate != MODEL_SR and rate_tap_floats(rate) > MAX_RATE_TAPS:
+        raise ValueError(f"sample rate {rate} Hz is not supported: its resampler taps would hold {rate_tap_floats(rate)} floats, "
+                         f"more than 2^18")
+    return rate
+
+
+def rates_arg(sr, n: int):
+    """``sr`` of the batch calls for n entries: None, one rate for all, or one per entry.  Returns the rates as int32, or
+    None when every one is 48 kHz (the unrated call).  ValueError for a list of another length or an unsupported rate."""
+    if sr is None:
+        return None
+    if isinstance(sr, (int, np.integer)) and not isinstance(sr, bool):
+        rates = [sr] * n
+    else:
+        rates = list(np.asarray(sr).reshape(-1).tolist()) if not isinstance(sr, (list, tuple)) else list(sr)
+        if len(rates) != n:
+            raise ValueError(f"{len(rates)} sample rates for {n} entries")
+    rates = np.ascontiguousarray(np.array([check_rate(r) for r in rates], dtype=np.int32))
+    return None if (rates == MODEL_SR).all() else rates
+
+
+def len_48k(length: int, rate: int) -> int:
+    """io.resample's length of ``length`` samples at ``rate`` resampled to 48 kHz: ceil(length * 48000 / rate)."""
+    return -(-int(length) * MODEL_SR // int(rate))
+
+
+def out_len_at(length: int, rate: int, hop: int, pad: bool) -> int:
+    """dfb_enhance_out_len_at: the 48 kHz output length of the resampled stream, resampled back to ``rate``."""
+    if int(rate) == MODEL_SR:
+        return out_len(length, hop, pad)
+    return -(-out_len(len_48k(length, rate), hop, pad) * int(rate) // MODEL_SR)
+
+
+def check_lengths_at(lengths, rates, hop: int, pad: bool, max_len: int = None) -> np.ndarray:
+    """:func:`check_lengths` of a rated batch: lengths in each stream's own samples, the frame check at 48 kHz."""
+    lens = check_lengths(lengths, 1, True, max_len)
+    check_lengths([len_48k(t, r) for t, r in zip(lens.tolist(), np.asarray(rates).tolist())], hop, pad)
+    return lens
+
+
+def packed_layout_at(shapes: Sequence[Tuple[int, int]], rates: np.ndarray, hop: int, pad: bool):
+    """:func:`packed_layout` of a rated batch (entry i at rates[i]): (lengths, in_offsets, out_offsets, in_numel, out_numel,
+    slices, stream_rates), every count in each stream's own samples; stream_rates int32, one per stream."""
+    lens: List[int] = []
+    srates: List[int] = []
+    for i, shp in enumerate(shapes):
+        if len(shp) != 2:
+            raise ValueError(f"entry {i}: audio must have shape [C, T], got {tuple(shp)}")
+        c, t = int(shp[0]), int(shp[1])
+        if c <= 0:
+            raise ValueError(f"entry {i}: no channels")
+        lens += [t] * c
+        srates += [int(rates[i])] * c
+    lens = check_lengths_at(lens, srates, hop, pad)
+    olens = np.array([out_len_at(int(t), r, hop, pad) for t, r in zip(lens, srates)], dtype=np.int64)
+    in_off = np.concatenate(([0], np.cumsum(lens)[:-1])).astype(np.int64)
+    out_off = np.concatenate(([0], np.cumsum(olens)[:-1])).astype(np.int64)
+    slices, k = [], 0
+    for shp in shapes:
+        c = int(shp[0])
+        slices.append((int(out_off[k]), c, int(olens[k])))
+        k += c
+    return lens, in_off, out_off, int(lens.sum()), int(olens.sum()), slices, np.ascontiguousarray(np.array(srates, dtype=np.int32))
+
+
+def padded_layout_at(lengths, rates: np.ndarray, width: int, hop: int, pad: bool):
+    """:func:`padded_layout` of a rated batch (row b at rates[b]): (lengths, in_offsets, out_offsets, out_width)."""
+    lens = check_lengths_at(lengths, rates, hop, pad, width)
+    ow = max(out_len_at(int(t), int(r), hop, pad) for t, r in zip(lens, rates))
+    rows = np.arange(lens.size, dtype=np.int64)
+    return lens, rows * width, rows * ow, ow
+
+
+def check_group_rates(group_sizes, rates) -> None:
+    """ValueError when a link group's streams are at different rates (the channels of one recording have one rate)."""
+    b = 0
+    for g, n in enumerate(np.asarray(group_sizes, dtype=np.int64).reshape(-1).tolist()):
+        if (np.asarray(rates[b:b + n]) != rates[b]).any():
+            raise ValueError(f"link group {g} has channels at different sample rates: {np.asarray(rates[b:b + n]).tolist()}")
+        b += n

@@ -230,6 +230,46 @@ int dfb_enhance_ragged_linked_host(dfb_model *m, dfb_state *st, const float *h_a
                                    const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad, float atten_lim_db,
                                    float *h_out, int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes,
                                    int64_t n_groups, int reduce_mask);
+/* Rated batches: streams at their own sample rates, resampled to and from 48 kHz on the device (DESIGN.md section 5i).
+ * dfb_model_add_rate registers rate r on the model, with the arguments of dfb_stream_add_slot_rate: up_taps / down_taps
+ * [nw][2 width + og] (HOST arrays) are io.resample_kernel(r, 48000) / (48000, r) with the sinc_fast parameters, og / nw the
+ * gcd-reduced rates (DFB_ERR_INVALID otherwise).  Every integer rate whose two tables hold at most 2^18 floats together is
+ * supported (8000, 11025, 12000, 16000, 22050, 24000, 32000, 44100, 88200, 96000 among them; 11025 is the largest, 230,794);
+ * any other is DFB_ERR_UNSUPPORTED.  48000 is the identity and registers nothing; registering a rate twice registers it once.
+ * Synchronises the model's device. */
+int dfb_model_add_rate(dfb_model *m, int rate, const float *up_taps, int up_og, int up_nw, int up_width,
+                       const float *down_taps, int down_og, int down_nw, int down_width);
+/* dfb_enhance_ragged_linked(_host) with a HOST array rates[B]: stream b is lengths[b] samples at rates[b] Hz (48000 or a
+ * registered rate), and lengths, offsets and in_numel / out_numel count each stream's own samples.  group_sizes may be null
+ * (no links); a link group has one rate and one length.  Stream b's result, dfb_enhance_out_len_at(st, lengths[b], pad,
+ * rates[b]) samples at out + out_offsets[b], is
+ *     io.resample(enhance(io.resample(x_b, r_b, 48000), pad, atten_lim_db), 48000, r_b)
+ * with io.resample's sinc_fast taps: the 48 kHz signal the analysis reads and the rate-r output are those of io.resample
+ * (k_resample's sums) bit for bit, and the enhancement between them is that of the ragged batch (fp32 reduction order
+ * aside).  A 48 kHz stream is enhanced as in dfb_enhance_ragged, untouched by any resampler.  Only rate-r samples cross
+ * PCIe in the _host variant, whose copies overlap the compute as dfb_enhance_ragged_host's do.  DFB_ERR_INVALID for an
+ * unregistered rate, mixed rates or lengths in a link group, a stream with no frame at 48 kHz when pad == 0, or a stream
+ * that reaches outside in_numel / out_numel. */
+int dfb_enhance_ragged_rates(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
+                             const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
+                             const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
+                             const int32_t *rates, void *stream);
+int dfb_enhance_ragged_rates_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel, const int64_t *in_offsets,
+                                  const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *h_out, int64_t out_numel,
+                                  const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
+                                  const int32_t *rates);
+/* output length of a stream of T samples at `rate` in a rated batch: ceil(out48 rate / 48000), out48 =
+ * dfb_enhance_out_len(st, ceil(T 48000 / rate), pad); -1 for a null state, T <= 0 or rate <= 0 */
+int64_t dfb_enhance_out_len_at(const dfb_state *st, int64_t T, int pad, int rate);
+/* Debug aid: one of a model's offline resamplers (up != 0: rate -> 48 kHz, else 48 kHz -> rate) alone over B rows (B <= 65535):
+ * row b is in_lengths[b] samples at d_in + in_offsets[b] (at rates[b] going up, at 48 kHz going down; registered rates
+ * only), and its resampled signal, io.resample's length, goes to d_out + out_offsets[b].  The launches are those of a chunk
+ * loop with the bounds h_bounds[0 .. n_bounds) (HOST, increasing, > 0): going up, launch c writes the 48 kHz outputs
+ * [h_bounds[c - 1], h_bounds[c]); going down, the outputs whose taps lie below input sample h_bounds[c], or all of them
+ * once h_bounds[c] reaches the row's end.  Each output is written once, and nothing outside the rows' outputs. */
+int dfb_debug_resample_rows(int up, const dfb_model *m, const float *d_in, const int64_t *in_offsets, const int64_t *in_lengths,
+                            const int32_t *rates, int64_t B, float *d_out, const int64_t *out_offsets, const int64_t *h_bounds,
+                            int64_t n_bounds, void *stream);
 /* ------------------------------------------------------------------ streaming -----------------
  * Frame-incremental processing with carried per-stream state: the batched counterpart of the reference's
  * single-stream runtime `DfTract::process` (libDF/src/tract.rs:509-642) and its C ABI (libDF/src/capi.rs:83-253:
