@@ -2166,22 +2166,39 @@ static int enhance_plan(dfb_model *m, dfb_state *st, int64_t B, int64_t Tf, int 
 // padded stream's last look-ahead frames.  DeepFilterNet v1 runs one window per signal with the end padding applied inside
 // every layer (forward_v1), so its stream groups are also cut where the frame count changes: a group shares one window.
 
-// Validates a ragged call and returns its streams in the caller's order.
-static int ragged_plan(const dfb_state *st, int64_t in_numel, const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad,
-                       int64_t out_numel, const int64_t *out_offsets, std::vector<RaggedRow> &rows) {
+// Validates a ragged call and returns its streams in the caller's order.  Stream b is lengths[b] samples at rates[b] (rates
+// null: every stream at 48 kHz; DESIGN.md section 5i).  The chunk loop runs its 48 kHz signal, ceil(lengths[b] 48000 / rate)
+// samples (io.resample's length), so rows are planned from the 48 kHz lengths and sorting, stream groups, the active prefix
+// and link groups work unchanged; its output is the 48 kHz output resampled back, ceil(out48 rate / 48000) samples.
+// `rows` are the streams at 48 kHz (offsets the caller's, used for 48 kHz streams only), `rr` the streams at their rates
+// with their directions of the model's resamplers (-1: 48 kHz).
+static int batch_plan(const dfb_model *m, const dfb_state *st, int64_t in_numel, const int64_t *in_offsets, const int64_t *lengths,
+                      int64_t B, int pad, int64_t out_numel, const int64_t *out_offsets, const int32_t *rates,
+                      std::vector<RaggedRow> &rows, std::vector<RateRow> &rr) {
     if (!in_offsets || !lengths || !out_offsets) return fail(DFB_ERR_INVALID, "null argument");
     if (B <= 0) return fail(DFB_ERR_INVALID, "empty batch");
     rows.resize((size_t)B);
+    rr.resize((size_t)B);
     for (int64_t b = 0; b < B; b++) {
         const int64_t len = lengths[b], io = in_offsets[b], oo = out_offsets[b];
+        const int rate = rates ? rates[b] : kModelRate;
+        int dir = -1;
+        if (rate != kModelRate) {
+            const auto it = std::find(m->rates.begin(), m->rates.end(), rate);
+            if (it == m->rates.end())
+                return fail(DFB_ERR_INVALID, "stream %lld: sample rate %d Hz is not registered (dfb_model_add_rate)", (long long)b, rate);
+            dir = (int)(it - m->rates.begin());
+        }
         if (len <= 0) return fail(DFB_ERR_INVALID, "stream %lld has length %lld", (long long)b, (long long)len);
-        const int64_t tf = (pad ? len + st->fft : len) / st->hop, ol = dfb_enhance_out_len(st, len, pad);
-        if (tf <= 0) return fail(DFB_ERR_INVALID, "stream %lld is shorter than one hop", (long long)b);
+        const int64_t len48 = dir < 0 ? len : len_at_48k(len, rate), tf = (pad ? len48 + st->fft : len48) / st->hop,
+                      ol48 = dfb_enhance_out_len(st, len48, pad), ol = dir < 0 ? ol48 : len_from_48k(ol48, rate);
+        if (tf <= 0) return fail(DFB_ERR_INVALID, "stream %lld is shorter than one hop%s", (long long)b, rates ? " at 48 kHz" : "");
         if (io < 0 || io > in_numel - len)
             return fail(DFB_ERR_INVALID, "stream %lld reaches outside the input (%lld samples)", (long long)b, (long long)in_numel);
         if (oo < 0 || oo > out_numel - ol)
             return fail(DFB_ERR_INVALID, "stream %lld reaches outside the output (%lld samples)", (long long)b, (long long)out_numel);
-        rows[(size_t)b] = RaggedRow{io, len, oo, ol, tf};
+        rows[(size_t)b] = RaggedRow{io, len48, oo, ol48, tf};
+        rr[(size_t)b] = RateRow{io, len, oo, ol, tf, dir};
     }
     return DFB_OK;
 }
@@ -2213,11 +2230,12 @@ static int copy_streams(float *dst, const float *src, int64_t x0, int64_t n, At 
     return DFB_OK;
 }
 
-// Validates the link groups of a linked call: group g is the next group_sizes[g] streams in the caller's order, all of one
-// length.  Returns each stream's group {first stream, size} in the caller's order, or an empty table when nothing is linked
-// (reduce none, or every group a single stream): such a call is the unlinked one.
-static int link_plan(const dfb_model *m, const std::vector<RaggedRow> &rows, const int64_t *group_sizes, int64_t n_groups,
-                     int reduce, std::vector<LinkRow> &links) {
+// Validates the link groups of a linked call: group g is the next group_sizes[g] streams in the caller's order (`rows` and
+// `rr` from batch_plan), all of one rate and one length.  Returns each stream's group {first stream, size} in the caller's
+// order, or an empty table when nothing is linked (reduce none, or every group a single stream): such a call is the unlinked
+// one.
+static int link_plan(const dfb_model *m, const std::vector<RaggedRow> &rows, const std::vector<RateRow> &rr,
+                     const int64_t *group_sizes, int64_t n_groups, int reduce, std::vector<LinkRow> &links) {
     if (reduce != kReduceNone && reduce != kReduceMax && reduce != kReduceMean)
         return fail(DFB_ERR_INVALID, "reduce_mask %d is not 0 (none), 1 (max) or 2 (mean)", reduce);
     if (!group_sizes || n_groups <= 0) return fail(DFB_ERR_INVALID, "no link groups");
@@ -2231,6 +2249,8 @@ static int link_plan(const dfb_model *m, const std::vector<RaggedRow> &rows, con
         for (int64_t i = b; i < b + n; i++) {
             if (rows[(size_t)i].len != rows[(size_t)b].len)
                 return fail(DFB_ERR_INVALID, "link group %lld has channels of different lengths", (long long)g);
+            if (rr[(size_t)i].dir != rr[(size_t)b].dir || rr[(size_t)i].in_len != rr[(size_t)b].in_len)
+                return fail(DFB_ERR_INVALID, "link group %lld mixes sample rates or lengths", (long long)g);
             links[(size_t)i] = LinkRow{(int)b, (int)n};
         }
         b += n;
@@ -2245,20 +2265,22 @@ static int link_plan(const dfb_model *m, const std::vector<RaggedRow> &rows, con
     return DFB_OK;
 }
 
-// The batch executor behind every dfb_enhance* entry point; `rows` (the caller's order) is sorted here.  Device buffers: the
-// work is enqueued on `s`.  Host buffers (`host`): each stream group is staged into device buffers that hold its streams
-// packed back to back, chunk by chunk and each stream's range clipped to its length -- the H2D copy of chunk c + 1 and the
-// D2H copy of chunk c - 1 run on their own streams (both copy engines) while chunk c computes -- and the call is synchronous.
+// The batch executor behind every dfb_enhance* entry point; `rows` and `rates` (the caller's order, from batch_plan) are
+// sorted here.  `rows` are the streams at 48 kHz, which is what the chunk loop runs, and rates[b] is stream b at its own
+// rate (DESIGN.md section 5i): the caller's buffers hold that.  Device buffers: the work is enqueued on `s`, on the caller's
+// buffers when every stream is at 48 kHz.  Host buffers (`host`) or a rated batch (a stream at another rate than 48 kHz):
+// each stream group is staged into 48 kHz device buffers that hold its streams packed back to back (a rated host batch also
+// in staging buffers at the streams' rates), chunk by chunk and each stream's range clipped to its length.  Per chunk,
+// before the analysis, the up-resampler writes the 48 kHz samples it reads, and after apply + synthesis the down-resampler
+// writes the outputs that became complete; 48 kHz streams are copied, never resampled.  On the host path the H2D copy of
+// chunk c + 1 and the D2H copy of chunk c - 1 run on their own streams (both copy engines) while chunk c computes, and the
+// call is synchronous.
 // `links` (or null): each stream's link group from link_plan, sorted here along with `rows`; `reduce` the mask reduction.
-// `rates` (or null): a rated batch (rates_plan; DESIGN.md section 5i).  `rows` are then the streams at 48 kHz, which is what
-// the chunk loop runs, and rates[b] is stream b at its own rate: the caller's buffers hold that.  Every stream group is
-// staged in 48 kHz device buffers (a host batch also in staging buffers at the streams' rates); per chunk, before the
-// analysis, the up-resampler writes the 48 kHz samples it reads, and after apply + synthesis the down-resampler writes the
-// outputs that became complete.  48 kHz streams are copied, never resampled.
-static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &rows, const float *src, float *dst, int pad,
-                        float atten_lim_db, bool host, cudaStream_t s, std::vector<LinkRow> *links = nullptr, int reduce = 0,
-                        std::vector<RateRow> *rates = nullptr) {
+static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &rows, std::vector<RateRow> &rates, const float *src,
+                        float *dst, int pad, float atten_lim_db, bool host, cudaStream_t s, std::vector<LinkRow> *links = nullptr,
+                        int reduce = 0) {
     const int64_t B = (int64_t)rows.size();
+    const bool rated = std::any_of(rates.begin(), rates.end(), [](const RateRow &q) { return q.dir >= 0; });
     int64_t min_group = 1;   // the largest link group: a stream group never splits one
     {
         // The members of a link group are consecutive and share their sort key (one length), so the stable sort keeps them
@@ -2269,11 +2291,11 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
         std::stable_sort(idx.begin(), idx.end(), [&](int64_t a, int64_t b) { return rows[(size_t)a].Tf > rows[(size_t)b].Tf; });
         std::vector<RaggedRow> sr((size_t)B);
         std::vector<LinkRow> sl(links ? (size_t)B : 0);
-        std::vector<RateRow> sq(rates ? (size_t)B : 0);
+        std::vector<RateRow> sq((size_t)B);
         for (int64_t i = 0; i < B; i++) {
             const int64_t o = idx[(size_t)i];
             sr[(size_t)i] = rows[(size_t)o];
-            if (rates) sq[(size_t)i] = (*rates)[(size_t)o];
+            sq[(size_t)i] = rates[(size_t)o];
             if (links) {
                 const LinkRow g = (*links)[(size_t)o];
                 sl[(size_t)i] = LinkRow{(int)(i - (o - g.first)), g.n};
@@ -2282,7 +2304,7 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
         }
         rows.swap(sr);
         if (links) links->swap(sl);
-        if (rates) rates->swap(sq);
+        rates.swap(sq);
     }
     std::vector<int64_t> tfs((size_t)B);
     int64_t true_frames = 0;
@@ -2304,7 +2326,7 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
     if (rc) return rc;
     size_t off[16];   // the aux arena holds one group's state slab and tables
     if ((rc = m->aux_arena.reserve(state_floats(m->cfg, st, (int)group, off) * sizeof(float) +
-                                   (size_t)group * (sizeof(RaggedRow) + sizeof(LinkRow) + (rates ? 2 * sizeof(RateRow) : 0)) + 8192)))
+                                   (size_t)group * (sizeof(RaggedRow) + sizeof(LinkRow) + (rated ? 2 * sizeof(RateRow) : 0)) + 8192)))
         return rc;
     // stream groups: up to `group` streams, cut only between link groups (group >= every link group, so a cut inside one
     // moves back to its first member, past b0); DeepFilterNet v1: of one frame count
@@ -2327,22 +2349,20 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
     }
     // device rows: the streams themselves, or (host, rated) their places in the staging buffers, sized for the largest group.
     // A rated host batch also stages its streams at their own rates: ur / dr_ are the up / down resamplers' rows.
-    const bool staged = host || rates;
+    const bool staged = host || rated;
     std::vector<RaggedRow> drows(rows);
-    std::vector<RateRow> ur, dr_;
+    std::vector<RateRow> ur(rates), dr_(rates);
     float *d_in = nullptr, *d_out = nullptr, *d_rin = nullptr, *d_rout = nullptr;
     int smem_up = 0, smem_down = 0;
     if (staged) {
         int64_t n_in = 0, n_out = 0, n_rin = 0, n_rout = 0;
-        if (rates) { ur = *rates; dr_ = *rates; }
         for (int64_t b0 = 0, b1; b0 < B; b0 = b1) {
             b1 = group_end(b0);
             int64_t gi = 0, go = 0, gri = 0, gro = 0;
             for (int64_t i = b0; i < b1; i++) {
                 drows[i].in_off = gi; drows[i].out_off = go;
                 gi += rows[i].len; go += rows[i].out_len;
-                if (!rates) continue;
-                const RateRow &q = (*rates)[(size_t)i];
+                const RateRow &q = rates[(size_t)i];
                 ur[i] = RateRow{q.in_off, q.in_len, drows[i].in_off, rows[i].len, q.tf, q.dir};
                 dr_[i] = RateRow{drows[i].out_off, rows[i].out_len, q.out_off, q.out_len, q.tf, q.dir};
                 if (q.dir < 0) continue;
@@ -2390,65 +2410,49 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
         const int64_t *tf = tfs.data() + b0;
         ChunkHooks hooks;
         hooks.pcie = host;
-        if (!rates) {
-            hooks.before = [&](int64_t x0, int64_t x1, int64_t na, cudaStream_t cs) -> int {
-                const int r = copy_streams(d_in, src, x0, na, [&](int64_t i) {
-                    return StreamCopy{dr[i].in_off, hr[i].in_off, std::min(x1, hr[i].len)};
-                }, cudaMemcpyHostToDevice, sh);
-                return r ? r : order(sh, cs);
-            };
-            hooks.after = [&](int64_t y0, int64_t y1, int64_t d1, int64_t na, cudaStream_t cs) -> int {
-                if (const int r = order(cs, sd)) return r;
-                return copy_streams(dst, d_out, y0, na, [&](int64_t i) {   // a stream that has ended: all of its output
-                    return StreamCopy{hr[i].out_off, dr[i].out_off, tf[i] <= d1 ? hr[i].out_len : std::min(y1, hr[i].out_len)};
-                }, cudaMemcpyDeviceToHost, sd);
-            };
-        }
-        // rated batch: uh / dh the group's resampler rows, rh its streams in the caller's buffers; d_prev the DNN frames of
-        // the previous chunk (which streams had ended at its down-resampler launch)
-        const RateRow *uh = rates ? ur.data() + b0 : nullptr, *dh = rates ? dr_.data() + b0 : nullptr,
-                      *rh = rates ? rates->data() + b0 : nullptr;
+        // uh / dh the group's resampler rows, rh its streams in the caller's buffers; d_prev the DNN frames of the previous
+        // chunk (which streams had ended at its down-resampler launch).  In a batch at 48 kHz only, both resampler launches
+        // have no outputs and return before launching, and the copies of the staging buffers at the streams' rates are empty.
+        const RateRow *uh = ur.data() + b0, *dh = dr_.data() + b0, *rh = rates.data() + b0;
         RateRow *d_ur = nullptr, *d_dr = nullptr;
         int64_t d_prev = 0;
         const RateDir *d_up = m->d_rate_dirs, *d_down = m->d_rate_dirs + m->rates.size();
-        if (rates) {
-            hooks.before = [&](int64_t x0, int64_t x1, int64_t na, cudaStream_t cs) -> int {
-                // a 48 kHz stream is copied as in an unrated batch; a stream at another rate reads what its resampler needs for
-                // the 48 kHz samples below x1, its tap look-ahead included, of which earlier chunks copied those below x0's need
-                const cudaMemcpyKind kind = host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
-                int r = copy_streams(d_in, src, x0, na, [&](int64_t i) {
-                    return StreamCopy{dr[i].in_off, hr[i].in_off, uh[i].dir < 0 ? std::min(x1, hr[i].len) : x0};
-                }, kind, host ? sh : cs);
-                if (!r && host)
-                    r = copy_streams(d_rin, src, 0, na, [&](int64_t i) {
-                        if (uh[i].dir < 0) return StreamCopy{0, 0, 0};
-                        const RateDir &d = m->rate_up[(size_t)uh[i].dir];
-                        const int64_t a = rate_up_need(d, uh[i], x0), b = rate_up_need(d, uh[i], x1);
-                        return StreamCopy{uh[i].in_off + a, rh[i].in_off + a, b - a};
-                    }, cudaMemcpyHostToDevice, sh);
-                if (!r && host) r = order(sh, cs);
-                if (r) return r;
-                const RateIO io{host ? d_rin : src, d_in, x0, x1, 0, 0};
-                return launch_resample_rows(cs, true, d_up, d_ur, (int)na, io, max_range(true, uh, na, io), smem_up);
-            };
-            hooks.after = [&](int64_t y0, int64_t y1, int64_t d1, int64_t na, cudaStream_t cs) -> int {
-                const RateIO io{d_out, host ? d_rout : dst, y0, y1, d_prev, d1};
-                d_prev = d1;
-                int r = launch_resample_rows(cs, false, d_down, d_dr, (int)na, io, max_range(false, dh, na, io), smem_down);
-                if (r || (host && (r = order(cs, sd)))) return r;
-                r = copy_streams(dst, d_out, y0, na, [&](int64_t i) {   // a 48 kHz stream that has ended: all of its output
-                    return StreamCopy{hr[i].out_off, dr[i].out_off,
-                                      dh[i].dir >= 0 ? y0 : tf[i] <= d1 ? hr[i].out_len : std::min(y1, hr[i].out_len)};
-                }, host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, host ? sd : cs);
-                if (r || !host) return r;
-                return copy_streams(dst, d_rout, 0, na, [&](int64_t i) {
-                    if (dh[i].dir < 0) return StreamCopy{0, 0, 0};
-                    int64_t a, b;
-                    rate_range(false, m->rate_down[(size_t)dh[i].dir], dh[i], io, &a, &b);
-                    return StreamCopy{rh[i].out_off + a, dh[i].out_off + a, b - a};
-                }, cudaMemcpyDeviceToHost, sd);
-            };
-        }
+        hooks.before = [&](int64_t x0, int64_t x1, int64_t na, cudaStream_t cs) -> int {
+            // a 48 kHz stream is copied; a stream at another rate reads what its resampler needs for the 48 kHz samples below
+            // x1, its tap look-ahead included, of which earlier chunks copied those below x0's need
+            const cudaMemcpyKind kind = host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+            int r = copy_streams(d_in, src, x0, na, [&](int64_t i) {
+                return StreamCopy{dr[i].in_off, hr[i].in_off, uh[i].dir < 0 ? std::min(x1, hr[i].len) : x0};
+            }, kind, host ? sh : cs);
+            if (!r && host)
+                r = copy_streams(d_rin, src, 0, na, [&](int64_t i) {
+                    if (uh[i].dir < 0) return StreamCopy{0, 0, 0};
+                    const RateDir &d = m->rate_up[(size_t)uh[i].dir];
+                    const int64_t a = rate_up_need(d, uh[i], x0), b = rate_up_need(d, uh[i], x1);
+                    return StreamCopy{uh[i].in_off + a, rh[i].in_off + a, b - a};
+                }, cudaMemcpyHostToDevice, sh);
+            if (!r && host) r = order(sh, cs);
+            if (r) return r;
+            const RateIO io{host ? d_rin : src, d_in, x0, x1, 0, 0};
+            return launch_resample_rows(cs, true, d_up, d_ur, (int)na, io, max_range(true, uh, na, io), smem_up);
+        };
+        hooks.after = [&](int64_t y0, int64_t y1, int64_t d1, int64_t na, cudaStream_t cs) -> int {
+            const RateIO io{d_out, host ? d_rout : dst, y0, y1, d_prev, d1};
+            d_prev = d1;
+            int r = launch_resample_rows(cs, false, d_down, d_dr, (int)na, io, max_range(false, dh, na, io), smem_down);
+            if (r || (host && (r = order(cs, sd)))) return r;
+            r = copy_streams(dst, d_out, y0, na, [&](int64_t i) {   // a 48 kHz stream that has ended: all of its output
+                return StreamCopy{hr[i].out_off, dr[i].out_off,
+                                  dh[i].dir >= 0 ? y0 : tf[i] <= d1 ? hr[i].out_len : std::min(y1, hr[i].out_len)};
+            }, host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, host ? sd : cs);
+            if (r || !host) return r;
+            return copy_streams(dst, d_rout, 0, na, [&](int64_t i) {
+                if (dh[i].dir < 0) return StreamCopy{0, 0, 0};
+                int64_t a, b;
+                rate_range(false, m->rate_down[(size_t)dh[i].dir], dh[i], io, &a, &b);
+                return StreamCopy{rh[i].out_off + a, dh[i].out_off + a, b - a};
+            }, cudaMemcpyDeviceToHost, sd);
+        };
         // (host) the previous group's D2H copies read the staged output and its compute the staged input: order this
         // group's first writes after them
         if (host && ((rc = order(sd, sc)) || (rc = order(sc, sh)))) break;
@@ -2462,7 +2466,7 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
             if (!d_links) { rc = fail(DFB_ERR_OOM, "link table arena exhausted"); break; }
             DFB_CUDA(cudaMemcpyAsync(d_links, dlinks.data() + b0, sizeof(LinkRow) * (b1 - b0), cudaMemcpyHostToDevice, sc));
         }
-        if (rates) {
+        if (rated) {
             d_ur = m->aux_arena.take<RateRow>((size_t)(b1 - b0));
             d_dr = m->aux_arena.take<RateRow>((size_t)(b1 - b0));
             if (!d_ur || !d_dr) { rc = fail(DFB_ERR_OOM, "resampler table arena exhausted"); break; }
@@ -2483,13 +2487,17 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
     return rc;
 }
 
-// An equal-length batch [B][T]: stream b is {b T, T, b out_len}.  pad = True appends fft zeros (enhance.py:230-233):
-// Tf = (T + fft) / hop.
-static int equal_rows(const dfb_state *st, int64_t B, int64_t T, int pad, std::vector<RaggedRow> &rows) {
+// An equal-length batch [B][T] at 48 kHz: stream b is {b T, T, b out_len}.  pad = True appends fft zeros
+// (enhance.py:230-233): Tf = (T + fft) / hop.
+static int equal_rows(const dfb_state *st, int64_t B, int64_t T, int pad, std::vector<RaggedRow> &rows, std::vector<RateRow> &rr) {
     const int64_t Tf = (pad ? T + st->fft : T) / st->hop, out_len = dfb_enhance_out_len(st, T, pad);
     if (Tf <= 0) return fail(DFB_ERR_INVALID, "input shorter than one hop");
     rows.resize((size_t)B);
-    for (int64_t b = 0; b < B; b++) rows[(size_t)b] = RaggedRow{b * T, T, b * out_len, out_len, Tf};
+    rr.resize((size_t)B);
+    for (int64_t b = 0; b < B; b++) {
+        rows[(size_t)b] = RaggedRow{b * T, T, b * out_len, out_len, Tf};
+        rr[(size_t)b] = RateRow{b * T, T, b * out_len, out_len, Tf, -1};
+    }
     return DFB_OK;
 }
 
@@ -2499,9 +2507,10 @@ extern "C" int dfb_enhance(dfb_model *m, dfb_state *st, const float *d_audio, in
     if (B <= 0 || T <= 0) return fail(DFB_ERR_INVALID, "empty input");
     if (int rcs = check_state(m, st)) return rcs;
     std::vector<RaggedRow> rows;
-    if (int rc = equal_rows(st, B, T, pad, rows)) return rc;
+    std::vector<RateRow> rr;
+    if (int rc = equal_rows(st, B, T, pad, rows, rr)) return rc;
     DFB_CUDA(cudaSetDevice(m->device));
-    return enhance_rows(m, st, rows, d_audio, d_out, pad, atten_lim_db, false, (cudaStream_t)stream);
+    return enhance_rows(m, st, rows, rr, d_audio, d_out, pad, atten_lim_db, false, (cudaStream_t)stream);
 }
 
 extern "C" int dfb_enhance_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t B, int64_t T, int pad,
@@ -2510,142 +2519,78 @@ extern "C" int dfb_enhance_host(dfb_model *m, dfb_state *st, const float *h_audi
     if (B <= 0 || T <= 0) return fail(DFB_ERR_INVALID, "empty input");
     if (int rcs = check_state(m, st)) return rcs;
     std::vector<RaggedRow> rows;
-    if (int rc = equal_rows(st, B, T, pad, rows)) return rc;
+    std::vector<RateRow> rr;
+    if (int rc = equal_rows(st, B, T, pad, rows, rr)) return rc;
     DFB_CUDA(cudaSetDevice(m->device));
-    return enhance_rows(m, st, rows, h_audio, h_out, pad, atten_lim_db, true, nullptr);
+    return enhance_rows(m, st, rows, rr, h_audio, h_out, pad, atten_lim_db, true, nullptr);
+}
+
+// The body of every dfb_enhance_ragged* entry point: `group_sizes` null for a call without link groups, `rates` null for
+// one whose streams are all at 48 kHz.
+static int enhance_ragged(dfb_model *m, dfb_state *st, const float *src, int64_t in_numel, const int64_t *in_offsets,
+                          const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *dst, int64_t out_numel,
+                          const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
+                          const int32_t *rates, bool host, cudaStream_t s) {
+    if (!m || !st || !src || !dst) return fail(DFB_ERR_INVALID, "null argument");
+    if (int rcs = check_state(m, st)) return rcs;
+    std::vector<RaggedRow> rows;
+    std::vector<RateRow> rr;
+    std::vector<LinkRow> links;
+    if (int rc = batch_plan(m, st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rates, rows, rr)) return rc;
+    if (group_sizes)
+        if (int rc = link_plan(m, rows, rr, group_sizes, n_groups, reduce_mask, links)) return rc;
+    DFB_CUDA(cudaSetDevice(m->device));
+    return enhance_rows(m, st, rows, rr, src, dst, pad, atten_lim_db, host, s, links.empty() ? nullptr : &links, reduce_mask);
 }
 
 extern "C" int dfb_enhance_ragged(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
                                   const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
                                   const int64_t *out_offsets, void *stream) {
-    if (!m || !st || !d_audio || !d_out) return fail(DFB_ERR_INVALID, "null argument");
-    if (int rcs = check_state(m, st)) return rcs;
-    std::vector<RaggedRow> rows;
-    if (int rc = ragged_plan(st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rows)) return rc;
-    DFB_CUDA(cudaSetDevice(m->device));
-    return enhance_rows(m, st, rows, d_audio, d_out, pad, atten_lim_db, false, (cudaStream_t)stream);
+    return enhance_ragged(m, st, d_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, d_out, out_numel, out_offsets,
+                          nullptr, 0, kReduceNone, nullptr, false, (cudaStream_t)stream);
 }
 
 extern "C" int dfb_enhance_ragged_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel, const int64_t *in_offsets,
                                        const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *h_out, int64_t out_numel,
                                        const int64_t *out_offsets) {
-    if (!m || !st || !h_audio || !h_out) return fail(DFB_ERR_INVALID, "null argument");
-    if (int rcs = check_state(m, st)) return rcs;
-    std::vector<RaggedRow> rows;
-    if (int rc = ragged_plan(st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rows)) return rc;
-    DFB_CUDA(cudaSetDevice(m->device));
-    return enhance_rows(m, st, rows, h_audio, h_out, pad, atten_lim_db, true, nullptr);
+    return enhance_ragged(m, st, h_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, h_out, out_numel, out_offsets,
+                          nullptr, 0, kReduceNone, nullptr, true, nullptr);
 }
 
 extern "C" int dfb_enhance_ragged_linked(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel,
                                          const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad, float atten_lim_db,
                                          float *d_out, int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes,
                                          int64_t n_groups, int reduce_mask, void *stream) {
-    if (!m || !st || !d_audio || !d_out) return fail(DFB_ERR_INVALID, "null argument");
-    if (int rcs = check_state(m, st)) return rcs;
-    std::vector<RaggedRow> rows;
-    std::vector<LinkRow> links;
-    if (int rc = ragged_plan(st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rows)) return rc;
-    if (int rc = link_plan(m, rows, group_sizes, n_groups, reduce_mask, links)) return rc;
-    DFB_CUDA(cudaSetDevice(m->device));
-    return enhance_rows(m, st, rows, d_audio, d_out, pad, atten_lim_db, false, (cudaStream_t)stream, links.empty() ? nullptr : &links,
-                        reduce_mask);
+    return !group_sizes ? fail(DFB_ERR_INVALID, "no link groups")
+                        : enhance_ragged(m, st, d_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, d_out, out_numel,
+                                         out_offsets, group_sizes, n_groups, reduce_mask, nullptr, false, (cudaStream_t)stream);
 }
 
 extern "C" int dfb_enhance_ragged_linked_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel,
                                               const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad,
                                               float atten_lim_db, float *h_out, int64_t out_numel, const int64_t *out_offsets,
                                               const int64_t *group_sizes, int64_t n_groups, int reduce_mask) {
-    if (!m || !st || !h_audio || !h_out) return fail(DFB_ERR_INVALID, "null argument");
-    if (int rcs = check_state(m, st)) return rcs;
-    std::vector<RaggedRow> rows;
-    std::vector<LinkRow> links;
-    if (int rc = ragged_plan(st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rows)) return rc;
-    if (int rc = link_plan(m, rows, group_sizes, n_groups, reduce_mask, links)) return rc;
-    DFB_CUDA(cudaSetDevice(m->device));
-    return enhance_rows(m, st, rows, h_audio, h_out, pad, atten_lim_db, true, nullptr, links.empty() ? nullptr : &links, reduce_mask);
-}
-
-// ============================================================== rated batches ====
-// dfb_enhance_ragged_rates (DESIGN.md section 5i): stream b is lengths[b] samples at rates[b].  The chunk loop runs its
-// 48 kHz signal, ceil(lengths[b] 48000 / rate) samples (io.resample's length), so rows are planned from the 48 kHz lengths
-// and sorting, stream groups, the active prefix and link groups work unchanged; its output is the 48 kHz output resampled
-// back, ceil(out48 rate / 48000) samples.  Validates the call: `rows` at 48 kHz (offsets the caller's, used for 48 kHz
-// streams only), `rr` the streams at their rates with their directions of the model's resamplers (-1: 48 kHz), `links`
-// as link_plan (a group of one rate and one length), and *rated whether any stream is at another rate than 48 kHz.
-static int rates_plan(const dfb_model *m, const dfb_state *st, int64_t in_numel, const int64_t *in_offsets, const int64_t *lengths,
-                      int64_t B, int pad, int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes,
-                      int64_t n_groups, int reduce, const int32_t *rates, std::vector<RaggedRow> &rows, std::vector<RateRow> &rr,
-                      std::vector<LinkRow> &links, bool *rated) {
-    if (!in_offsets || !lengths || !out_offsets || !rates) return fail(DFB_ERR_INVALID, "null argument");
-    if (B <= 0) return fail(DFB_ERR_INVALID, "empty batch");
-    rows.resize((size_t)B);
-    rr.resize((size_t)B);
-    *rated = false;
-    for (int64_t b = 0; b < B; b++) {
-        const int64_t len = lengths[b], io = in_offsets[b], oo = out_offsets[b];
-        const int rate = rates[b];
-        int dir = -1;
-        if (rate != kModelRate) {
-            const auto it = std::find(m->rates.begin(), m->rates.end(), rate);
-            if (it == m->rates.end())
-                return fail(DFB_ERR_INVALID, "stream %lld: sample rate %d Hz is not registered (dfb_model_add_rate)", (long long)b, rate);
-            dir = (int)(it - m->rates.begin());
-            *rated = true;
-        }
-        if (len <= 0) return fail(DFB_ERR_INVALID, "stream %lld has length %lld", (long long)b, (long long)len);
-        const int64_t len48 = dir < 0 ? len : len_at_48k(len, rate), tf = (pad ? len48 + st->fft : len48) / st->hop,
-                      ol48 = dfb_enhance_out_len(st, len48, pad), ol = dir < 0 ? ol48 : len_from_48k(ol48, rate);
-        if (tf <= 0) return fail(DFB_ERR_INVALID, "stream %lld is shorter than one hop at 48 kHz", (long long)b);
-        if (io < 0 || io > in_numel - len)
-            return fail(DFB_ERR_INVALID, "stream %lld reaches outside the input (%lld samples)", (long long)b, (long long)in_numel);
-        if (oo < 0 || oo > out_numel - ol)
-            return fail(DFB_ERR_INVALID, "stream %lld reaches outside the output (%lld samples)", (long long)b, (long long)out_numel);
-        rows[(size_t)b] = RaggedRow{io, len48, oo, ol48, tf};
-        rr[(size_t)b] = RateRow{io, len, oo, ol, tf, dir};
-    }
-    links.clear();
-    if (!group_sizes) return DFB_OK;
-    if (int rc = link_plan(m, rows, group_sizes, n_groups, reduce, links)) return rc;
-    for (int64_t b = 0, g = 0; b < B; b += group_sizes[g++])
-        for (int64_t i = b + 1; i < b + group_sizes[g]; i++)
-            if (rates[i] != rates[b] || lengths[i] != lengths[b])
-                return fail(DFB_ERR_INVALID, "link group %lld mixes sample rates or lengths", (long long)g);
-    return DFB_OK;
-}
-
-static int enhance_rates(dfb_model *m, dfb_state *st, const float *src, int64_t in_numel, const int64_t *in_offsets,
-                         const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *dst, int64_t out_numel,
-                         const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
-                         const int32_t *rates, bool host, cudaStream_t s) {
-    if (!m || !st || !src || !dst) return fail(DFB_ERR_INVALID, "null argument");
-    if (int rcs = check_state(m, st)) return rcs;
-    std::vector<RaggedRow> rows;
-    std::vector<RateRow> rr;
-    std::vector<LinkRow> links;
-    bool rated = false;
-    if (int rc = rates_plan(m, st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, group_sizes, n_groups, reduce_mask,
-                            rates, rows, rr, links, &rated))
-        return rc;
-    DFB_CUDA(cudaSetDevice(m->device));
-    return enhance_rows(m, st, rows, src, dst, pad, atten_lim_db, host, s, links.empty() ? nullptr : &links, reduce_mask,
-                        rated ? &rr : nullptr);
+    return !group_sizes ? fail(DFB_ERR_INVALID, "no link groups")
+                        : enhance_ragged(m, st, h_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, h_out, out_numel,
+                                         out_offsets, group_sizes, n_groups, reduce_mask, nullptr, true, nullptr);
 }
 
 extern "C" int dfb_enhance_ragged_rates(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
                                         const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out,
                                         int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups,
                                         int reduce_mask, const int32_t *rates, void *stream) {
-    return enhance_rates(m, st, d_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, d_out, out_numel, out_offsets,
-                         group_sizes, n_groups, reduce_mask, rates, false, (cudaStream_t)stream);
+    return !rates ? fail(DFB_ERR_INVALID, "null argument")
+                  : enhance_ragged(m, st, d_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, d_out, out_numel, out_offsets,
+                                   group_sizes, n_groups, reduce_mask, rates, false, (cudaStream_t)stream);
 }
 
 extern "C" int dfb_enhance_ragged_rates_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel,
                                              const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad, float atten_lim_db,
                                              float *h_out, int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes,
                                              int64_t n_groups, int reduce_mask, const int32_t *rates) {
-    return enhance_rates(m, st, h_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, h_out, out_numel, out_offsets,
-                         group_sizes, n_groups, reduce_mask, rates, true, nullptr);
+    return !rates ? fail(DFB_ERR_INVALID, "null argument")
+                  : enhance_ragged(m, st, h_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, h_out, out_numel, out_offsets,
+                                   group_sizes, n_groups, reduce_mask, rates, true, nullptr);
 }
 
 // Debug aid: one of the model's offline resamplers alone over a ragged batch, in the launches the chunk loop would make

@@ -184,7 +184,7 @@ def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: boo
     """Several recordings of different lengths in one call: ``audios`` is a sequence of CPU [C_i, T_i] tensors as
     :func:`enhance` takes them, every channel one stream.  Entry i of the result equals
     ``enhance(model, df_state, audios[i], pad, atten_lim_db)``.  The batch is packed into one page-locked buffer and
-    enhanced by one ``dfb_enhance_ragged_host`` call, which copies only the streams' own samples and computes only their
+    enhanced by one ``dfb_enhance_ragged_rates_host`` call, which copies only the streams' own samples and computes only their
     own frames.  The results are views into one page-locked output buffer.  ``reduce_mask`` "max" / "mean": each entry's
     channels are linked, as ``enhance(..., reduce_mask=reduce_mask)`` links them.
     ``sr``: the entries' sample rate, one for all or one per entry (None: 48 kHz).  Entry i at rate r is then
@@ -198,31 +198,18 @@ def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: boo
             raise ValueError(f"entry {i}: audio must be a tensor of shape [C, T]")
     rates = _rated(model, sr, len(xs))
     shapes = [tuple(a.shape) for a in xs]
-    if rates is None:
-        lens, in_off, out_off, n_in, n_out, slices = ragged.packed_layout(shapes, df_state.hop_size(), pad)
-    else:
-        lens, in_off, out_off, n_in, n_out, slices, srates = ragged.packed_layout_at(shapes, rates, df_state.hop_size(), pad)
+    lens, in_off, out_off, n_in, n_out, slices, srates = ragged.packed_layout(shapes, df_state.hop_size(), pad, rates)
     pin = torch.cuda.is_available()
     x = torch.empty(n_in, dtype=torch.float32, pin_memory=pin)
     torch.cat([a.detach().to("cpu", torch.float32).reshape(-1) for a in xs], out=x)
     y = torch.empty(n_out, dtype=torch.float32, pin_memory=pin)
     lim = abs(float(atten_lim_db)) if atten_lim_db is not None else 0.0
     reduce = ragged.reduce_code(reduce_mask)
-    if rates is not None:
-        groups = ragged.packed_groups(shapes) if reduce != 0 else None
-        check(_lib.lib().dfb_enhance_ragged_rates_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
-                                                       lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
-                                                       out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
-                                                       groups.size if groups is not None else 0, reduce, srates.ctypes.data))
-    elif reduce == 0:
-        check(_lib.lib().dfb_enhance_ragged_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
-                                                 lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
-                                                 out_off.ctypes.data))
-    else:
-        groups = ragged.packed_groups([tuple(a.shape) for a in xs])
-        check(_lib.lib().dfb_enhance_ragged_linked_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
-                                                        lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
-                                                        out_off.ctypes.data, groups.ctypes.data, groups.size, reduce))
+    groups = ragged.packed_groups(shapes) if reduce != 0 else None
+    check(_lib.lib().dfb_enhance_ragged_rates_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
+                                                   lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
+                                                   out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
+                                                   groups.size if groups is not None else 0, reduce, srates.ctypes.data))
     return [y[s:s + c * n].view(c, n) for s, c, n in slices]
 
 
@@ -250,14 +237,13 @@ def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pa
         raise ValueError(f"{lens.size} lengths for {b} streams")
     rates = _rated(model, sr, b)
     if rates is None:
-        lens, in_off, out_off, ow = ragged.padded_layout(lens, s, df_state.hop_size(), pad)
-    else:
-        lens, in_off, out_off, ow = ragged.padded_layout_at(lens, rates, s, df_state.hop_size(), pad)
+        rates = np.full(b, ragged.MODEL_SR, dtype=np.int32)
+    lens, in_off, out_off, ow = ragged.padded_layout(lens, s, df_state.hop_size(), pad, rates)
     reduce = ragged.reduce_code(reduce_mask)
     if group_sizes is None and reduce != 0:
         raise ValueError("reduce_mask needs group_sizes: which rows are the channels of one recording")
     groups = ragged.link_groups(group_sizes, lens) if group_sizes is not None else None
-    if groups is not None and rates is not None:
+    if groups is not None:
         ragged.check_group_rates(groups, rates)
     if out is None:
         out = torch.zeros((b, ow), dtype=torch.float32, device=audio.device)
@@ -267,21 +253,10 @@ def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pa
     lim = abs(float(atten_lim_db)) if atten_lim_db is not None else 0.0
     with torch.cuda.device(audio.device):
         stream = torch.cuda.current_stream(audio.device).cuda_stream
-        if rates is not None:
-            check(_lib.lib().dfb_enhance_ragged_rates(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
-                                                      lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow,
-                                                      out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
-                                                      groups.size if groups is not None else 0, reduce, rates.ctypes.data,
-                                                      stream))
-        elif groups is None:
-            check(_lib.lib().dfb_enhance_ragged(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
-                                                lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow,
-                                                out_off.ctypes.data, stream))
-        else:
-            check(_lib.lib().dfb_enhance_ragged_linked(model.handle, df_state.handle, audio.data_ptr(), b * s,
-                                                       in_off.ctypes.data, lens.ctypes.data, b, 1 if pad else 0, lim,
-                                                       out.data_ptr(), b * ow, out_off.ctypes.data, groups.ctypes.data,
-                                                       groups.size, reduce, stream))
+        check(_lib.lib().dfb_enhance_ragged_rates(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
+                                                  lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow,
+                                                  out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
+                                                  groups.size if groups is not None else 0, reduce, rates.ctypes.data, stream))
     return out
 
 

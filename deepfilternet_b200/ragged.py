@@ -13,9 +13,10 @@ def out_len(length: int, hop: int, pad: bool) -> int:
     return int(length) if pad else (int(length) // hop) * hop
 
 
-def check_lengths(lengths, hop: int, pad: bool, max_len: int = None) -> np.ndarray:
-    """Lengths as int64.  ValueError for a length <= 0 or beyond ``max_len``; RuntimeError when ``pad`` is off and a stream
-    is shorter than one hop (it has no frame), as ``enhance()`` does."""
+def check_lengths(lengths, hop: int, pad: bool, max_len: int = None, rates=None) -> np.ndarray:
+    """Lengths as int64, each in its stream's own samples at rates[b] (None: every stream at 48 kHz).  ValueError for a
+    length <= 0 or beyond ``max_len``; RuntimeError when ``pad`` is off and a stream is shorter than one hop at 48 kHz (it
+    has no frame), as ``enhance()`` does."""
     lens = np.ascontiguousarray(np.asarray(lengths, dtype=np.int64).reshape(-1))
     if lens.size == 0:
         raise ValueError("empty batch")
@@ -23,23 +24,28 @@ def check_lengths(lengths, hop: int, pad: bool, max_len: int = None) -> np.ndarr
         raise ValueError(f"stream lengths must be > 0, got {int(lens.min())}")
     if max_len is not None and (lens > max_len).any():
         raise ValueError(f"stream length {int(lens.max())} exceeds the {max_len} samples per row")
-    if not pad and (lens < hop).any():
-        raise RuntimeError(f"stream of {int(lens.min())} samples is shorter than one hop ({hop}): no frame to enhance")
+    lens48 = lens if rates is None else -(-lens * MODEL_SR // np.asarray(rates, dtype=np.int64))   # len_48k of every stream
+    if not pad and (lens48 < hop).any():
+        raise RuntimeError(f"stream of {int(lens48.min())} samples is shorter than one hop ({hop}): no frame to enhance")
     return lens
 
 
-def padded_layout(lengths, width: int, hop: int, pad: bool) -> Tuple[np.ndarray, np.ndarray, np.ndarray, int]:
-    """Rows of a padded [B, width] input and a [B, max out_len] output: (lengths, in_offsets, out_offsets, out_width)."""
-    lens = check_lengths(lengths, hop, pad, width)
-    ow = max(out_len(int(t), hop, pad) for t in lens)
+def padded_layout(lengths, width: int, hop: int, pad: bool, rates=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray, int]:
+    """Rows of a padded [B, width] input and a [B, max out_len] output, row b at rates[b] (None: every row at 48 kHz):
+    (lengths, in_offsets, out_offsets, out_width), every count in each row's own samples."""
+    lens = check_lengths(lengths, hop, pad, width, rates)
+    ow = int(_out_lens(lens, MODEL_SR if rates is None else rates, hop, pad).max())
     rows = np.arange(lens.size, dtype=np.int64)
     return lens, rows * width, rows * ow, ow
 
 
-def packed_layout(shapes: Sequence[Tuple[int, int]], hop: int, pad: bool):
-    """Entries [C_i, T_i] packed back to back, every channel one stream: (lengths, in_offsets, out_offsets, in_numel,
-    out_numel, slices) where slices[i] = (start, C_i, out_len_i) locates entry i in the packed output."""
+def packed_layout(shapes: Sequence[Tuple[int, int]], hop: int, pad: bool, rates=None):
+    """Entries [C_i, T_i] packed back to back, every channel one stream, entry i at rates[i] (None: every entry at 48 kHz):
+    (lengths, in_offsets, out_offsets, in_numel, out_numel, slices, stream_rates), every count in each stream's own
+    samples, where slices[i] = (start, C_i, out_len_i) locates entry i in the packed output and stream_rates are int32, one
+    per stream."""
     lens: List[int] = []
+    srates: List[int] = []
     for i, shp in enumerate(shapes):
         if len(shp) != 2:
             raise ValueError(f"entry {i}: audio must have shape [C, T], got {tuple(shp)}")
@@ -47,8 +53,9 @@ def packed_layout(shapes: Sequence[Tuple[int, int]], hop: int, pad: bool):
         if c <= 0:
             raise ValueError(f"entry {i}: no channels")
         lens += [t] * c
-    lens = check_lengths(lens, hop, pad)
-    olens = np.array([out_len(int(t), hop, pad) for t in lens], dtype=np.int64)
+        srates += [MODEL_SR if rates is None else int(rates[i])] * c
+    lens = check_lengths(lens, hop, pad, rates=srates)
+    olens = _out_lens(lens, srates, hop, pad)
     in_off = np.concatenate(([0], np.cumsum(lens)[:-1])).astype(np.int64)
     out_off = np.concatenate(([0], np.cumsum(olens)[:-1])).astype(np.int64)
     slices, k = [], 0
@@ -56,7 +63,7 @@ def packed_layout(shapes: Sequence[Tuple[int, int]], hop: int, pad: bool):
         c = int(shp[0])
         slices.append((int(out_off[k]), c, int(olens[k])))
         k += c
-    return lens, in_off, out_off, int(lens.sum()), int(olens.sum()), slices
+    return lens, in_off, out_off, int(lens.sum()), int(olens.sum()), slices, np.ascontiguousarray(np.array(srates, dtype=np.int32))
 
 
 # Linked channels (dfb_enhance_ragged_linked): the channels of one recording share one ERB mask, reduced over them.
@@ -155,44 +162,14 @@ def out_len_at(length: int, rate: int, hop: int, pad: bool) -> int:
     return -(-out_len(len_48k(length, rate), hop, pad) * int(rate) // MODEL_SR)
 
 
-def check_lengths_at(lengths, rates, hop: int, pad: bool, max_len: int = None) -> np.ndarray:
-    """:func:`check_lengths` of a rated batch: lengths in each stream's own samples, the frame check at 48 kHz."""
-    lens = check_lengths(lengths, 1, True, max_len)
-    check_lengths([len_48k(t, r) for t, r in zip(lens.tolist(), np.asarray(rates).tolist())], hop, pad)
-    return lens
-
-
-def packed_layout_at(shapes: Sequence[Tuple[int, int]], rates: np.ndarray, hop: int, pad: bool):
-    """:func:`packed_layout` of a rated batch (entry i at rates[i]): (lengths, in_offsets, out_offsets, in_numel, out_numel,
-    slices, stream_rates), every count in each stream's own samples; stream_rates int32, one per stream."""
-    lens: List[int] = []
-    srates: List[int] = []
-    for i, shp in enumerate(shapes):
-        if len(shp) != 2:
-            raise ValueError(f"entry {i}: audio must have shape [C, T], got {tuple(shp)}")
-        c, t = int(shp[0]), int(shp[1])
-        if c <= 0:
-            raise ValueError(f"entry {i}: no channels")
-        lens += [t] * c
-        srates += [int(rates[i])] * c
-    lens = check_lengths_at(lens, srates, hop, pad)
-    olens = np.array([out_len_at(int(t), r, hop, pad) for t, r in zip(lens, srates)], dtype=np.int64)
-    in_off = np.concatenate(([0], np.cumsum(lens)[:-1])).astype(np.int64)
-    out_off = np.concatenate(([0], np.cumsum(olens)[:-1])).astype(np.int64)
-    slices, k = [], 0
-    for shp in shapes:
-        c = int(shp[0])
-        slices.append((int(out_off[k]), c, int(olens[k])))
-        k += c
-    return lens, in_off, out_off, int(lens.sum()), int(olens.sum()), slices, np.ascontiguousarray(np.array(srates, dtype=np.int32))
-
-
-def padded_layout_at(lengths, rates: np.ndarray, width: int, hop: int, pad: bool):
-    """:func:`padded_layout` of a rated batch (row b at rates[b]): (lengths, in_offsets, out_offsets, out_width)."""
-    lens = check_lengths_at(lengths, rates, hop, pad, width)
-    ow = max(out_len_at(int(t), int(r), hop, pad) for t, r in zip(lens, rates))
-    rows = np.arange(lens.size, dtype=np.int64)
-    return lens, rows * width, rows * ow, ow
+def _out_lens(lens: np.ndarray, rates, hop: int, pad: bool) -> np.ndarray:
+    """:func:`out_len_at` of every stream (int64 lengths, rates one or one per stream) as one int64 array: array arithmetic,
+    so that laying out a batch costs no Python call per stream."""
+    r = np.asarray(rates, dtype=np.int64)
+    o48 = -(-lens * MODEL_SR // r)
+    if not pad:
+        o48 = o48 // hop * hop
+    return -(-o48 * r // MODEL_SR)
 
 
 def check_group_rates(group_sizes, rates) -> None:

@@ -227,6 +227,32 @@ def test_48k_calls_are_unchanged(st, dfn3):
     d0 = enhance_device_ragged(model, st, x, lens)
     assert torch.equal(enhance_device_ragged(model, st, x, lens, sr=48000), d0)
     assert torch.equal(enhance(model, st, a[0], sr=48000), enhance(model, st, a[0]))
+    # every ragged entry point on one packed batch: a rated call at 48 kHz is the plain or linked call, and a linked call
+    # with groups of one the plain call, bit for bit and in as many launches
+    L = _lib.lib()
+    i64 = lambda v: np.ascontiguousarray(np.asarray(v, np.int64))   # noqa: E731
+    lens = i64([30000, 30000, 4801, 12345, 12345, 12345])
+    off, n = i64(np.concatenate(([0], np.cumsum(lens)[:-1]))), int(lens.sum())
+    ones, groups, r48 = i64([1] * 6), i64([2, 1, 3]), np.full(6, 48000, np.int32)
+    x = synth_audio(1, n, seed=642)[0].contiguous()
+    stream = torch.cuda.current_stream().cuda_stream
+
+    def run(dev, name, *tail):
+        src, out = (x.cuda(), torch.zeros(n, device="cuda")) if dev else (x, torch.zeros(n))
+        n0 = L.dfb_kernel_launches()
+        _lib.check(getattr(L, name if dev else name + "_host")(model.handle, st.handle, src.data_ptr(), n, off.ctypes.data,
+                                                             lens.ctypes.data, 6, 1, 0.0, out.data_ptr(), n, off.ctypes.data,
+                                                             *tail, *((stream,) if dev else ())))
+        return out.cpu(), L.dfb_kernel_launches() - n0
+
+    for dev in (True, False):
+        plain = run(dev, "dfb_enhance_ragged")
+        linked = run(dev, "dfb_enhance_ragged_linked", groups.ctypes.data, 3, 2)
+        assert not torch.equal(linked[0], plain[0]), dev
+        for got, ref in ((run(dev, "dfb_enhance_ragged_rates", None, 0, 0, r48.ctypes.data), plain),
+                         (run(dev, "dfb_enhance_ragged_linked", ones.ctypes.data, 6, 2), plain),
+                         (run(dev, "dfb_enhance_ragged_rates", groups.ctypes.data, 3, 2, r48.ctypes.data), linked)):
+            assert torch.equal(got[0], ref[0]) and got[1] == ref[1], (dev, got[1], ref[1])
 
 
 def test_workspace_of_a_rated_call(st):

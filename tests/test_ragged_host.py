@@ -39,13 +39,14 @@ def test_padded_layout():
     assert ow == 960 and out_off.tolist() == [0, 960, 1920]
 
 
-def test_packed_layout():
-    lens, in_off, out_off, n_in, n_out, sl = ragged.packed_layout([(2, 1000), (1, 481), (3, 50)], HOP, True)
+def test_packed_layout_at_48k():
+    lens, in_off, out_off, n_in, n_out, sl, sr = ragged.packed_layout([(2, 1000), (1, 481), (3, 50)], HOP, True)
     assert lens.tolist() == [1000, 1000, 481, 50, 50, 50]
+    assert sr.dtype == np.int32 and sr.tolist() == [48000] * 6
     assert in_off.tolist() == [0, 1000, 2000, 2481, 2531, 2581] and n_in == 2631
     assert out_off.tolist() == in_off.tolist() and n_out == n_in
     assert sl == [(0, 2, 1000), (2000, 1, 481), (2481, 3, 50)]
-    lens, in_off, out_off, n_in, n_out, sl = ragged.packed_layout([(2, 1000), (1, 481)], HOP, False)
+    lens, in_off, out_off, n_in, n_out, sl, _ = ragged.packed_layout([(2, 1000), (1, 481)], HOP, False)
     assert out_off.tolist() == [0, 960, 1920] and n_out == 2400 and n_in == 2481
     assert sl == [(0, 2, 960), (1920, 1, 480)]
     with pytest.raises(ValueError):

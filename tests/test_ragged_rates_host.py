@@ -70,10 +70,10 @@ def test_rates_arg():
         ragged.rates_arg([8000, 47999], 2)
 
 
-def test_packed_layout_at():
+def test_packed_layout_with_rates():
     shapes = [(2, 16000), (1, 4801), (1, 30)]
     rates = np.array([16000, 48000, 8000], np.int32)
-    lens, in_off, out_off, n_in, n_out, slices, sr = ragged.packed_layout_at(shapes, rates, HOP, True)
+    lens, in_off, out_off, n_in, n_out, slices, sr = ragged.packed_layout(shapes, HOP, True, rates)
     assert lens.tolist() == [16000, 16000, 4801, 30]
     assert sr.tolist() == [16000, 16000, 48000, 8000]
     olens = [ragged.out_len_at(t, r, HOP, True) for t, r in zip(lens, sr)]
@@ -82,15 +82,15 @@ def test_packed_layout_at():
     assert slices == [(0, 2, olens[0]), (2 * olens[0], 1, olens[2]), (2 * olens[0] + olens[2], 1, olens[3])]
     # 100 samples at 16 kHz are 300 at 48 kHz: no frame without pad, as enhance() refuses a stream shorter than a hop
     with pytest.raises(RuntimeError, match="shorter than one hop"):
-        ragged.packed_layout_at([(1, 100)], np.array([16000], np.int32), HOP, False)
-    ragged.packed_layout_at([(1, 160)], np.array([16000], np.int32), HOP, False)
+        ragged.packed_layout([(1, 100)], HOP, False, np.array([16000], np.int32))
+    ragged.packed_layout([(1, 160)], HOP, False, np.array([16000], np.int32))
 
 
-def test_padded_layout_at_and_group_rates():
-    lens, in_off, out_off, ow = ragged.padded_layout_at([16000, 8000, 300], np.array([16000, 8000, 48000]), 16000, HOP, True)
+def test_padded_layout_with_rates_and_group_rates():
+    lens, in_off, out_off, ow = ragged.padded_layout([16000, 8000, 300], 16000, HOP, True, np.array([16000, 8000, 48000]))
     assert ow == 16000 and in_off.tolist() == [0, 16000, 32000] and out_off.tolist() == [0, ow, 2 * ow]
     with pytest.raises(ValueError, match="exceeds"):
-        ragged.padded_layout_at([16001], np.array([16000]), 16000, HOP, True)
+        ragged.padded_layout([16001], 16000, HOP, True, np.array([16000]))
     ragged.check_group_rates([2, 1], np.array([16000, 16000, 8000]))
     with pytest.raises(ValueError, match="different sample rates"):
         ragged.check_group_rates([2, 1], np.array([16000, 8000, 8000]))
