@@ -134,6 +134,7 @@ SIGNATURES = {
     "dfb_debug_gru_timing": (_I, [_VP, _I, _VP]),
     "dfb_debug_gru_tc": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _VP, _VP, _VP, _I64, _I, _I, _I, _I, _I, _I, _I, _VP]),
     "dfb_debug_gemm_bf16x3": (_I, [_VP, _VP, _I64, _VP, _VP, _VP, _VP, _I64, _I64, _I, _I, _VP]),
+    "dfb_debug_df_convp_tc": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP, _I64, _VP]),
     "dfb_debug_gl_bx": (_I, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _I64, _VP, _VP, _I64, _I64, _I, _I, _I, _I, _F, _F, _VP]),
     "dfb_model_debug_fetch": (_I64, [_VP, C.c_char_p, _VP, _I64]),
 }

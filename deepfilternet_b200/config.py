@@ -122,7 +122,7 @@ def load_config(path: str, env: Optional[dict] = None) -> ModelConfig:
     model = get("model", "deepfilternet3", str, "train").lower()
     if model not in ("deepfilternet", "deepfilternet2", "deepfilternet3"):
         raise NotImplementedError(
-            f"model '{model}' is outside the H100 hot path (DeepFilterNet/2/3/3_ll supported)")
+            f"model '{model}' is outside the H100 hot path (DeepFilterNet/2/3/3_ll/2_ll supported)")
     c = ModelConfig(model=model, path=path)
     S = "df"
     c.sr = get("sr", 48000, int, S)

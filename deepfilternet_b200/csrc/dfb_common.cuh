@@ -330,9 +330,11 @@ bool df_emb_geometry(int Fd, int G, int Ig, int Hg, int kt, int *s_out, int *sta
 int launch_df_emb(cudaStream_t s, const float *c0, int64_t M, int T, int Fd, int kt, const float *dw, const float *bias,
                   const float *pw_sw, const float *w_img, int G, int Ig, int Hg, const float *res, int64_t ldr,
                   unsigned short *y_hi, unsigned short *y_lo, int64_t ldp, const int64_t *first, int64_t w0);
-// DF pathway conv (df_convp) on tensor cores (dfb_tc.cu)
+// DF pathway conv (df_convp) on tensor cores (dfb_tc.cu): df_convp_built says which (df_order, df_pathway_kt) have a
+// kernel instance (df_order 5, kt 1 to 5); launch_df_convp_tc refuses the others with DFB_ERR_UNSUPPORTED
+bool df_convp_built(int order, int kt);
 int launch_df_convp_tc(cudaStream_t s, const float *c0, const float *w_sw, const float *w2, const float *bias, float *coefs, int B, int T,
-                       int Fd, const int64_t *first = nullptr, int64_t w0 = 0);
+                       int Fd, int order, int kt, const int64_t *first = nullptr, int64_t w0 = 0);
 // fp32 [M][K] -> BF16 hi / lo planes [M][K]
 int launch_to_planes(cudaStream_t s, const float *x, int64_t ldx, int64_t M, int K, unsigned short *hi, unsigned short *lo);
 }  // namespace dfb

@@ -481,7 +481,7 @@ struct NetW {  // DeepFilterNet2 / 3 (forward_body)
     PathW conv3p, conv2p, conv1p, conv0p;
     Gl df_fc_emb, enc_in, enc_out, df_skip, df_in, df_out, erb_in, erb_out;
     std::vector<GruLayer> enc_gru, df_gru, erb_gru;
-    struct { const float *w_sw, *w2, *b; } df_convp{};  // bound for the built df_order / df_pathway_kt (5, 5) only
+    struct { const float *w_sw, *w2, *b; } df_convp{};  // bound for a built df_order / df_pathway_kt (df_convp_built)
     bool fused_emb = false;  // df_conv1 + df_fc_emb run as one kernel (k_dwpw_gl); df_fc_emb's fp32 weight is not read then
 };
 
@@ -596,7 +596,7 @@ static int bind_net(const dfb_model_config &c, Binder &b, NetW &w) {
     w.erb_gru = b.gru("erb_dec.emb_gru", c.erb_gru_layers, H);
     w.lsnr = b.wb("enc.lsnr", emb_dim, 1); w.conv0_out = b.wb("erb_dec.conv0_out", c.conv_kt * 3 * kCh, 1);
     if (c.model_kind == 2) w.df_fc_a = b.wb("df_dec.df_fc_a", Hd, 1);
-    if (c.df_order == 5 && c.df_pathway_kt == 5)
+    if (df_convp_built(c.df_order, c.df_pathway_kt))
         w.df_convp = {b.need("df_dec.df_convp.w_sw", kCh * kCh), b.need("df_dec.df_convp.w2", O2 * O2), b.need("df_dec.df_convp.b", O2)};
     return b.rc;
 }
@@ -1130,12 +1130,14 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         // low-priority stream, so its CTAs only take SMs that the critical path -- the encoder convs now, the GRU
         // clusters later -- leaves idle (on the DF branch's own streams it delays df_fc_emb, which is on the critical path)
         DFB_CUDA(cudaStreamWaitEvent(sl, L.ev_c0, 0));
-        if (c.df_order != 5 || c.df_pathway_kt != 5)
-            return fail(DFB_ERR_UNSUPPORTED, "df_order %d / df_pathway_kernel_size_t %d (built kernels: 5, 5)", c.df_order,
-                        c.df_pathway_kt);
+        if (!df_convp_built(c.df_order, c.df_pathway_kt))
+            return fail(DFB_ERR_UNSUPPORTED, "df_order %d / df_pathway_kernel_size_t %d (built kernels: df_order 5, kt 1-5)",
+                        c.df_order, c.df_pathway_kt);
         if (Fd % 2) return fail(DFB_ERR_UNSUPPORTED, "df pathway conv: odd nb_df");
         // channel contraction on the tensor cores (BF16x3), shifted adds + 1x1 conv in the epilogue
-        if ((rc = launch_df_convp_tc(sl, f.c0, w.df_convp.w_sw, w.df_convp.w2, w.df_convp.b, d_coefs, B, T, Fd, first, W0))) return rc;
+        if ((rc = launch_df_convp_tc(sl, f.c0, w.df_convp.w_sw, w.df_convp.w2, w.df_convp.b, d_coefs, B, T, Fd, c.df_order,
+                                     c.df_pathway_kt, first, W0)))
+            return rc;
         DFB_CUDA(cudaEventRecord(L.ev_convp, sl));
     }
     {
@@ -1644,7 +1646,7 @@ struct StreamState {
     float *t_dec = nullptr;                                      // (conv_kt == 2) last kHalo frames of dec_emb
     int n_feat = 0, n_mc = 0, n_dec = 0;                         // valid frames in the tails
 };
-constexpr int kMcTail = 6;   // >= lag + 3 (see run_chunk)
+constexpr int kMcTail = 6;   // >= df_order (DeepFilterNet2, see run_chunk)
 
 struct ChunkGeom { int Lmax, lag, Hf; };
 static ChunkGeom chunk_geom(const dfb_model_config &c) {
@@ -1978,7 +1980,9 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     S.n_dec = cx.dec_tail_n;
     S.dnn_started = true;
     // the halo rows of m / coefs come from skipped recurrences: restore the last finished frames from the previous chunk
-    // (the apply kernel re-synthesises frame e0 - 1 for its overlap-add tail; DFN2's masked taps reach 2 frames further back)
+    // (the apply kernel re-synthesises frame e0 - 1 for its overlap-add tail.  DFN2's masked taps of that frame reach
+    // df_order - 1 - df_lookahead frames further back, and e0 = d1 - lag with lag = df_lookahead, so they read the masks
+    // of frames [d1 - df_order, d1) at any look-ahead: 5 frames at df_lookahead 2 and at 0, within kMcTail and kHalo)
     if (Rc > 0 && S.n_mc > 0 && !spectral) {
         const int n = S.n_mc < Rc ? S.n_mc : Rc;
         if ((rc = load_tail(s, mm, Tw, E, n, S.t_m, kMcTail, Rc - n, B)) || (rc = load_tail(s, cc, Tw, (size_t)Fd * O2, n, S.t_c, kMcTail, Rc - n, B)))

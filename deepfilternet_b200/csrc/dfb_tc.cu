@@ -370,12 +370,14 @@ template int launch_dwpw_tc<DW_T2>(cudaStream_t, DwPwParams, const float *, int)
 
 // ---------------------------------------------------------- DF pathway conv on tensor cores ----
 // coefs[b,t,f,:] = relu( pw( conv_t(c0) ) + b )  (df_convp, deepfilternet3.py:293-295: grouped (2) temporal conv 64 -> 10
-// with kernel (5,1), 1x1 conv 10 x 10, BN, ReLU).  On FFMA this conv is instruction-issue bound (~250 warp instructions
-// per frame and bin pair), so the channel contraction runs on the tensor pipe:
+// with kernel (KTP,1), 1x1 conv 10 x 10, BN, ReLU; KTP = 5 for DeepFilterNet2 / 3, 3 for DeepFilterNet2_ll, and
+// instances for every KTP from 1 to 5).  On FFMA this conv is instruction-issue bound (~250 warp instructions
+// per frame and bin pair at KTP = 5), so the channel contraction runs on the tensor pipe:
 //   Y[t, g*32 + dt*5 + o] = sum_{c in group g} w1[dt][g*5+o][c] * c0[t, f, c]        (one [128 t x 64 c] x [64 c x 64] product)
-//   z[t, g*5 + o]         = sum_dt Y[t - 4 + dt, g*32 + dt*5 + o]                     (shifted adds out of shared memory)
+//   z[t, g*5 + o]         = sum_dt Y[t - (KTP - 1) + dt, g*32 + dt*5 + o]             (shifted adds out of shared memory)
 //   coefs[t, f, :]        = relu(z . w2 + b)
-// One CTA = (stream, bin f, 124 output frames): its 128 time rows of c0[., f, :] (4 frames of history) arrive as two TMA
+// One CTA = (stream, bin f, 124 output frames): its 128 time rows of c0[., f, :] (KTP - 1 <= 4 frames of history; every
+// KTP keeps the 124-frame tile, so the launch geometry does not depend on it) arrive as two TMA
 // tensor boxes (rows 24.5 KB apart in HBM, 2 x 128 B per row, 128-byte swizzle), are split into BF16 hi / lo operand planes
 // (BF16x3: fp32-level accuracy), each warp multiplies 16 of the rows by the 64 x 64 weight with mma.sync and stages its part
 // of Y in shared memory (row stride 51 floats) and 128 threads (one per time row) do the shifted sums, the 1x1 conv and the 40-byte store.
@@ -917,23 +919,39 @@ int launch_gru_tc(cudaStream_t s, const float *xproj, const float *whh, const fl
 
 int cached_map_f32_sw128(CUtensorMap *out, const void *base, int64_t rows, int64_t cols, int64_t ld, int box_rows);
 
+bool df_convp_built(int order, int kt) { return order == 5 && kt >= 1 && kt <= 5; }
+
+template <int ORDER, int KTP>
+static int launch_df_convp_kt(cudaStream_t s, const CUtensorMap &mc, const CvParams &p, int B) {
+    const int smem = 1024 + (int)kCvTail + 512 + 64;
+    static PerDeviceOnce attr_once;
+    if (auto once_guard = attr_once.first())
+        DFB_CUDA(cudaFuncSetAttribute(k_df_convp_tc<ORDER, KTP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    // every KTP keeps the 124-frame output tile: the 128 staged rows hold at least KTP - 1 <= 4 rows of history
+    dim3 grid((unsigned)((p.Fd + kCvBins - 1) / kCvBins), (unsigned)((p.T + kCvOut - 1) / kCvOut), (unsigned)B);
+    DFB_PROF("k_df_convp_tc", s);
+    k_df_convp_tc<ORDER, KTP><<<grid, kCvThreads, smem, s>>>(mc, p);
+    DFB_LAUNCH_CHECK();
+    return DFB_OK;
+}
+
 // c0 [B,T,Fd,64] -> coefs [B,T,Fd,10] (pathway term), tensor-core version; w_sw: host-packed operand image (weights.py)
 int launch_df_convp_tc(cudaStream_t s, const float *c0, const float *w_sw, const float *w2, const float *bias, float *coefs, int B, int T,
-                       int Fd, const int64_t *first, int64_t w0) {
+                       int Fd, int order, int kt, const int64_t *first, int64_t w0) {
+    if (!df_convp_built(order, kt))
+        return fail(DFB_ERR_UNSUPPORTED, "df_order %d / df_pathway_kernel_size_t %d (built kernels: df_order 5, kt 1-5)", order, kt);
     if ((int64_t)B * T >= (int64_t(1) << 31) - 256 || B > 65535) return fail(DFB_ERR_UNSUPPORTED, "df pathway conv: batch too large for one launch");
     CUtensorMap mc;
     int rc;
     if ((rc = cached_map_f32_sw128(&mc, c0, (int64_t)B * T, (int64_t)Fd * kCh, (int64_t)Fd * kCh, 128))) return rc;
-    const int smem = 1024 + (int)kCvTail + 512 + 64;
-    static PerDeviceOnce attr_once;
-    if (auto once_guard = attr_once.first())
-        DFB_CUDA(cudaFuncSetAttribute(k_df_convp_tc<5, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CvParams p{w_sw, w2, bias, coefs, T, Fd, first, w0};
-    dim3 grid((unsigned)((Fd + kCvBins - 1) / kCvBins), (unsigned)((T + kCvOut - 1) / kCvOut), (unsigned)B);
-    DFB_PROF("k_df_convp_tc", s);
-    k_df_convp_tc<5, 5><<<grid, kCvThreads, smem, s>>>(mc, p);
-    DFB_LAUNCH_CHECK();
-    return DFB_OK;
+    const CvParams p{w_sw, w2, bias, coefs, T, Fd, first, w0};
+    switch (kt) {
+        case 1: return launch_df_convp_kt<5, 1>(s, mc, p, B);
+        case 2: return launch_df_convp_kt<5, 2>(s, mc, p, B);
+        case 3: return launch_df_convp_kt<5, 3>(s, mc, p, B);
+        case 4: return launch_df_convp_kt<5, 4>(s, mc, p, B);
+        default: return launch_df_convp_kt<5, 5>(s, mc, p, B);
+    }
 }
 
 // ------------------------------------------------------------------------------- host side ----
@@ -982,4 +1000,12 @@ extern "C" int dfb_debug_gemm_bf16x3(const void *x_hi, const void *x_lo, int64_t
                                      const float *bias, float *y, int64_t ldy, int64_t M, int N, int K, void *stream) {
     if (!x_hi || !x_lo || !w_hi || !w_lo || !y) return dfb::fail(DFB_ERR_INVALID, "gemm_bf16x3: null argument");
     return dfb::launch_gemm_bf16x3((cudaStream_t)stream, x_hi, x_lo, ldx, w_hi, w_lo, bias, y, ldy, M, N, K);
+}
+
+// Debug aid (tests/test_gpu_dfn2_ll.py): one k_df_convp_tc launch on caller-given device pointers
+extern "C" int dfb_debug_df_convp_tc(const float *c0, const float *w_sw, const float *w2, const float *bias, float *coefs, int B,
+                                     int T, int Fd, int order, int kt, const int64_t *first, int64_t w0, void *stream) {
+    if (!c0 || !w_sw || !w2 || !bias || !coefs) return dfb::fail(DFB_ERR_INVALID, "df_convp_tc: null argument");
+    if (B <= 0 || T <= 0 || Fd <= 0) return dfb::fail(DFB_ERR_INVALID, "df_convp_tc: B %d, T %d, Fd %d", B, T, Fd);
+    return dfb::launch_df_convp_tc((cudaStream_t)stream, c0, w_sw, w2, bias, coefs, B, T, Fd, order, kt, first, w0);
 }

@@ -1,11 +1,16 @@
-"""Weights of DeepFilterNet3_ll ship only as ONNX (``enc.onnx`` / ``erb_dec.onnx`` / ``df_dec.onnx`` inside
-``models/DeepFilterNet3_ll_onnx.tar.gz``; export code: DeepFilterNet/df/scripts/export.py:133-285).  This
+"""Weights of DeepFilterNet3_ll and DeepFilterNet2_ll ship only as ONNX (``enc.onnx`` / ``erb_dec.onnx`` / ``df_dec.onnx``
+inside ``models/DeepFilterNet3_ll_onnx.tar.gz`` and ``models/DeepFilterNet2_onnx_ll.tar.gz``; export code:
+DeepFilterNet/df/scripts/export.py:133-285).  This
 module transplants them into a reference-style ``state_dict`` (SURVEY.md Appendix B) so that the same weight
 packer / kernels serve the ONNX-only model.  The ``onnx`` package is not available, so the files are read with
 a ~60-line protobuf wire-format reader (only the fields needed: graph.node, graph.initializer, Constant
 node tensors).
 
-Mapping (verified against the DeepFilterNet3 checkpoint, whose ONNX export ships next to it):
+Mapping (verified against the DeepFilterNet3 checkpoint, whose ONNX export ships next to it; DeepFilterNet2's three
+graphs map the same way: the transplant of ``DeepFilterNet2_onnx`` has every tensor name and shape of the
+``DeepFilterNet2`` checkpoint except the buffers computed from the config (``erb_fb``, ``erb_comp.*``,
+``mask.erb_inv_fb``), and the reference's deepfilternet2 module computes the same outputs from both weight sets to
+1e-5, tests/test_dfn2_ll_host.py):
   * Einsum / depthwise-conv / ConvTranspose initialisers keep their torch names (``erb_conv1.1.weight`` ...);
   * a conv that had a BatchNorm behind it appears as an anonymous ``onnx::Conv_<n>`` (weight, bias) pair with
     the BN folded in -> stored as that conv + an identity BatchNorm carrying the bias;

@@ -133,7 +133,7 @@ typedef struct {
     int32_t inp_kt;          /* time taps of conv_kernel_inp (3)                             */
     int32_t emb_hidden, df_hidden;
     int32_t enc_gru_layers, erb_gru_layers, df_gru_layers;
-    int32_t df_pathway_kt;   /* 5 */
+    int32_t df_pathway_kt;   /* 5; 3 for DeepFilterNet2_ll; kernel instances for 1 to 5 at df_order 5 */
     int32_t enc_concat;      /* DFN2: 1 */
     int32_t g_df_fc_emb, g_enc_in, g_enc_out, g_erb_in, g_erb_out, g_df_in, g_df_skip, g_df_out;
     float lsnr_scale, lsnr_offset;
@@ -370,10 +370,11 @@ int dfb_stream_set_post_filter_beta(dfb_stream *s, const int64_t *slots, int64_t
  * NaN where the hop carries no frame: a free slot, the first `latency` hops of a handle or of a new session, a closing
  * slot past its tail.  Flush returns the tail frames' LSNR, computed with zero look-ahead like their audio.
  * Alignment: hop j of a call that starts at input hop k carries frame k + j - latency, latency = max(conv_lookahead,
- * df_lookahead) (+ df_lookahead for DeepFilterNet2).  df_process_frame returns, for input frame k, the LSNR of frame
+ * df_lookahead) (+ df_lookahead for DeepFilterNet2): 2 for DeepFilterNet3, 4 for DeepFilterNet2, 0 for DeepFilterNet3_ll
+ * and DeepFilterNet2_ll.  df_process_frame returns, for input frame k, the LSNR of frame
  * k - conv_lookahead (its encoder sees the features shifted by conv_lookahead, tract.rs:441-548), which is also the frame
- * its output carries.  For DeepFilterNet3 (conv_lookahead = df_lookahead = 2) and DeepFilterNet3_ll (0 / 0) the two agree
- * hop for hop.
+ * its output carries.  For DeepFilterNet3 (conv_lookahead = df_lookahead = 2), DeepFilterNet3_ll and DeepFilterNet2_ll
+ * (0 / 0) the two agree hop for hop.
  * The LSNR head runs only on handles that ask for it: from the first call with a non-NULL buffer until dfb_stream_reset,
  * every call computes it.  DeepFilterNet2's audio trails its DNN by df_lookahead frames, so at that first call the
  * frames whose DNN step ran in earlier calls have no LSNR and read NaN. */
@@ -544,6 +545,13 @@ int dfb_debug_gemm_bf16x3(const void *x_hi, const void *x_lo, int64_t ldx, const
 int dfb_debug_gl_bx(const void *x_hi, const void *x_lo, int64_t ldx, const float *w_img, const float *res, int64_t ldr,
                     float *y, int64_t ldy, void *y_hi, void *y_lo, int64_t ldp, int64_t M, int G, int Ig, int Hg, int act,
                     float oscale, float ooffset, void *stream);
+/* Debug aid: one launch of the tensor-core DF pathway conv on device pointers, on `stream` (NULL = default):
+ * coefs [B][T][Fd][2 order] = relu(w2^T (grouped (2) temporal conv of c0 [B][T][Fd][64] with kt taps) + bias), w_sw the
+ * operand image of weights.py (df_dec.df_convp.w_sw), w2 [2 order][2 order] (in, out), bias [2 order].  Frames before
+ * frame 0 of a stream, and (first != NULL, [B]) before frame first[b] - w0, read as zeros.  order 5 with kt 1 to 5 are
+ * built; others return DFB_ERR_UNSUPPORTED. */
+int dfb_debug_df_convp_tc(const float *c0, const float *w_sw, const float *w2, const float *bias, float *coefs, int B, int T,
+                          int Fd, int order, int kt, const int64_t *first, int64_t w0, void *stream);
 /* Debug aids for the spectral handle's input kernel.  dfb_debug_analysis_erb: the time-chunked analysis kernel on audio
  * f32[C][T] with its ERB epilogue: spec c64[C][T / hop][F], erb_db f32[C][T / hop][E] (dB, before normalisation).
  * dfb_debug_spec_ingest: k_spec_ingest over n frames of nb live rows, row b reading caller row h_src[b] of spec
