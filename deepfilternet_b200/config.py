@@ -227,6 +227,30 @@ def check_stft_size(c: "ModelConfig") -> None:
             "fft_size=960, hop_size=480 only")
 
 
+MAX_LOOKAHEAD = 3   # kMaxLookahead in csrc/dfb_model.cu
+_GROUPED_LINEARS = ("enc.df_fc_emb.0.weight", "enc.emb_gru.linear_in.0.weight", "enc.emb_gru.linear_out.0.weight",
+                    "erb_dec.emb_gru.linear_in.0.weight", "erb_dec.emb_gru.linear_out.0.weight",
+                    "df_dec.df_gru.linear_in.0.weight", "df_dec.df_skip.weight", "df_dec.df_out.0.weight")
+
+
+def check_model_shape(c: "ModelConfig", state_dict) -> None:
+    """The shapes dfb_model_create refuses (DFB_ERR_UNSUPPORTED), refused before the library is called: a look-ahead
+    outside 0..3 (DeepFilterNet v1: a conv look-ahead other than 2), and (DeepFilterNet2 / 3) a grouped linear whose group
+    width is not a multiple of 4.  DeepFilterNet v1's grouped linears are packed for the shipped topology only, which the
+    library checks on its own (dfb_model_create)."""
+    if not (0 <= c.conv_lookahead <= MAX_LOOKAHEAD and 0 <= c.df_lookahead <= MAX_LOOKAHEAD) or (
+            c.model == "deepfilternet" and c.conv_lookahead != 2):
+        raise NotImplementedError(f"look-ahead (conv {c.conv_lookahead}, df {c.df_lookahead}): the kernels take look-aheads "
+                                  f"0..{MAX_LOOKAHEAD} (DeepFilterNet v1: conv 2)")
+    if c.model == "deepfilternet":
+        return
+    for name in _GROUPED_LINEARS:
+        if name in state_dict:
+            g, ig, hg = state_dict[name].shape
+            if ig % 4 or (g > 1 and hg % 4):
+                raise NotImplementedError(f"{name}: {g} groups of {ig} x {hg}: the kernels build group widths that are multiples of 4")
+
+
 def check_supported(c: "ModelConfig") -> None:
     """Options the kernels do not implement must fail loudly instead of being dropped (all shipped
     configs use emb_gru_skip* = none and df_gru_skip in {none, groupedlinear})."""

@@ -453,6 +453,7 @@ __global__ void __launch_bounds__(128) k_convp_v1(const float *__restrict__ c0, 
 }
 
 constexpr int kMaxO2 = 16;  // largest 2 * df_order dfb_model_create accepts
+constexpr int kMaxLookahead = 3;  // largest conv_lookahead / df_lookahead dfb_model_create accepts
 
 }  // namespace dfb
 
@@ -598,6 +599,15 @@ static int bind_net(const dfb_model_config &c, Binder &b, NetW &w) {
     if (c.model_kind == 2) w.df_fc_a = b.wb("df_dec.df_fc_a", Hd, 1);
     if (df_convp_built(c.df_order, c.df_pathway_kt))
         w.df_convp = {b.need("df_dec.df_convp.w_sw", kCh * kCh), b.need("df_dec.df_convp.w2", O2 * O2), b.need("df_dec.df_convp.b", O2)};
+    // a group width that is not a multiple of 4 has no tensor-core image and the FFMA kernel refuses it (run_gl): refuse
+    // the model here instead of at its first forward pass
+    const std::pair<const char *, const Gl *> gls[] = {{"df_fc_emb", &w.df_fc_emb}, {"enc.emb_gru.in", &w.enc_in}, {"enc.emb_gru.out", &w.enc_out},
+                                                       {"df_dec.df_skip", &w.df_skip}, {"df_dec.df_gru.in", &w.df_in}, {"df_dec.df_out", &w.df_out},
+                                                       {"erb_dec.emb_gru.in", &w.erb_in}, {"erb_dec.emb_gru.out", &w.erb_out}};
+    for (const auto &g : gls)
+        if (!b.rc && g.second->G > 0 && ((g.second->I / g.second->G) % 4 || (g.second->G > 1 && (g.second->H / g.second->G) % 4)))
+            b.rc = fail(DFB_ERR_UNSUPPORTED, "grouped linear %s: %d x %d in %d groups (built kernels: group widths that are multiples of 4)",
+                        g.first, g.second->I, g.second->H, g.second->G);
     return b.rc;
 }
 
@@ -643,6 +653,14 @@ extern "C" int dfb_model_create(dfb_model **out, int device, const dfb_model_con
                     cfg->df_hidden);
     if (cfg->nb_erb % 8 || cfg->nb_erb > 64 || cfg->nb_df % 8 || cfg->nb_df > 128 || 2 * cfg->df_order > kMaxO2)
         return fail(DFB_ERR_UNSUPPORTED, "nb_erb / nb_df / df_order outside the built kernels");
+    // the input convs read feature frame t + conv_lookahead for every t >= 0 (k_conv_in), the deep filter frames
+    // t - (df_order - 1 - df_lookahead) ... t + df_lookahead: a negative look-ahead would read before the buffers.  The
+    // chunked and streaming paths are tested up to look-ahead 3 (tests/test_gpu_parity.py); DeepFilterNet v1 spreads its
+    // conv look-ahead over erb_conv0-2 and is built for the shipped 2 only
+    if (cfg->conv_lookahead < 0 || cfg->df_lookahead < 0 || cfg->conv_lookahead > kMaxLookahead || cfg->df_lookahead > kMaxLookahead ||
+        (cfg->model_kind == 1 && cfg->conv_lookahead != 2))
+        return fail(DFB_ERR_UNSUPPORTED, "look-ahead (conv %d, df %d): built kernels take look-aheads 0..%d (DeepFilterNet v1: conv 2)",
+                    cfg->conv_lookahead, cfg->df_lookahead, kMaxLookahead);
     int rc = use_device(device);
     if (rc) return rc;
     dfb_model *m = new dfb_model();
@@ -1034,6 +1052,9 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
     // BF16 planes of emb_in, fetched as pairs of BF16 per float word
     m->dbg["emb_in_hi"] = {reinterpret_cast<const float *>(f.embin_hi), M * emb_in_dim / 2};
     m->dbg["emb_in_lo"] = {reinterpret_cast<const float *>(f.embin_lo), M * emb_in_dim / 2};
+    // BF16 planes of the DF GRU's output (with its skip), the input df_out reads
+    m->dbg["dfc_hi"] = {reinterpret_cast<const float *>(f.dfc_hi), M * Hd / 2};
+    m->dbg["dfc_lo"] = {reinterpret_cast<const float *>(f.dfc_lo), M * Hd / 2};
     const int64_t e3_fs = c.enc_concat ? 2 * ED : ED;
     // fp32 activations that only feed the BF16 planes of a tensor-core consumer are not written (null): the input grouped
     // linears' g_a / g_a2 (DeepFilterNet2 adds them to the GRU output as a residual), the last-layer GRU outputs g_b (enc,
@@ -1118,11 +1139,12 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
             DFB_LAUNCH_CHECK();
             DFB_CUDA(cudaEventRecord(L.ev_c0, sa));
         }
-        m->dbg.erase("c1");
+        if (w.fused_emb) m->dbg.erase("c1");
         if (!w.fused_emb) {
             DwPwParams p = mk(w.df_conv1, f.c0, Fd, (int64_t)Fd * kCh, f.c1, Fd / 2, (int64_t)Fd / 2 * kCh, c.conv_kt);
-            // c1 only feeds df_fc_emb: write its BF16 planes instead of the fp32 tensor
-            p.out = nullptr; p.out_hi = pl_c1.hi; p.out_lo = pl_c1.lo; pl_c1.ok = true;
+            // c1 only feeds df_fc_emb: its BF16 planes for the tensor-core kernel, and the fp32 tensor for the FFMA kernel,
+            // which runs where df_fc_emb's shape has no tensor-core geometry (the planes alone left it reading unwritten c1)
+            p.out_hi = pl_c1.hi; p.out_lo = pl_c1.lo; pl_c1.ok = true;
             if ((rc = run_dwpw<DW_S2>(sa, p, B, w.df_conv1.pw_sw))) return rc;
         }
         DFB_CUDA(cudaEventRecord(L.ev_join_enc, sa));

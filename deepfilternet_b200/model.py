@@ -20,7 +20,7 @@ from torch import Tensor, nn
 
 from . import _lib
 from ._lib import ModelConfigC, TensorC, check
-from .config import ModelConfig, check_stft_size, load_config
+from .config import ModelConfig, check_model_shape, check_stft_size, load_config
 from .libdf import DF
 from .weights import pack_state_dict
 
@@ -64,6 +64,7 @@ class DfNet(nn.Module):
                  device: Optional[int] = None, run_df: bool = True):
         super().__init__()
         check_stft_size(cfg)
+        check_model_shape(cfg, state_dict)
         self.cfg = cfg
         self.nb_df = cfg.nb_df
         self.df_bins = cfg.nb_df

@@ -149,7 +149,12 @@ typedef struct {
 } dfb_tensor;
 
 /* Replaces init_model + load_state_dict (deepfilternet3.py:80-87, checkpoint.py:46-104).  Rejects a weight set that
- * lacks a tensor, or has a tensor of the wrong size, for the layers the config runs (DFB_ERR_INVALID, naming the tensor). */
+ * lacks a tensor, or has a tensor of the wrong size, for the layers the config runs (DFB_ERR_INVALID, naming the tensor).
+ * Refuses with DFB_ERR_UNSUPPORTED, naming what is built, the shapes the kernels do not build: conv_ch != 64, nb_erb or
+ * nb_df not a multiple of 8 or above 64 / 128, 2 * df_order > 16, conv_kt outside 1..2 or inp_kt outside 1..3, GRU
+ * hidden sizes other than 256 / 512, a conv_lookahead or df_lookahead outside 0..3 (DeepFilterNet v1: conv_lookahead other
+ * than 2), and (DeepFilterNet2 / 3) a grouped linear whose group width (inputs or outputs per group) is not a multiple of 4.  df_order != 5 and df_pathway_kt outside 1..5
+ * are accepted here and refused by the first forward pass. */
 int dfb_model_create(dfb_model **out, int device, const dfb_model_config *cfg, const dfb_tensor *tensors,
                      int n_tensors, const int64_t *erb_widths);
 void dfb_model_free(dfb_model *m);

@@ -93,6 +93,8 @@ KINDS = {   # name: (test_gpu_parity config, nb_df, apply mode, df look-ahead)
     "dfn3": ("dfn3", 96, 1, 2), "ll": ("ll", 96, 1, 0), "dfn2": ("dfn2", 96, 2, 2),
     # nb_df != 96: the generic apply kernel
     "dfn3_df64": ("dfn3", 64, 1, 2), "dfn2_df64": ("dfn2", 64, 2, 2),
+    # 24 ERB bands: the generic apply kernel at another band count
+    "dfn3_e24": ("e24", 96, 1, 2),
 }
 OPTS = {"plain": (False, False), "pf": (True, False), "mask_only": (False, True)}
 
@@ -102,16 +104,16 @@ def models(st):
     out = {}
     for name, (kind, nb_df, _, _) in KINDS.items():
         cfg = dataclasses.replace(cfg_of(kind), nb_df=nb_df)
-        out[name] = DfNet(cfg, random_state_dict(cfg, seed=3), st)
+        out[name] = DfNet(cfg, random_state_dict(cfg, seed=3), st if cfg.nb_erb == 32 else libdf.DF(48000, 960, HOP, cfg.nb_erb, 2))
     return out
 
 
-def apply_inputs(B, T, nb_df, seed):
+def apply_inputs(B, T, nb_df, seed, E=32):
     """Random spectra with exact-zero bins, masks with exact 0 and 1 entries, random deep-filter coefficients."""
     rng = np.random.default_rng(seed)
     spec = ((rng.standard_normal((B, T, 481)) + 1j * rng.standard_normal((B, T, 481))) * 0.1).astype(np.complex64)
     spec[rng.random(spec.shape) < 0.1] = 0
-    m = rng.random((B, T, 32)).astype(np.float32)
+    m = rng.random((B, T, E)).astype(np.float32)
     m[rng.random(m.shape) < 0.1] = 0
     m[rng.random(m.shape) < 0.1] = 1
     c = ((rng.standard_normal((B, T, nb_df, 5)) + 1j * rng.standard_normal((B, T, nb_df, 5))) * 0.5).astype(np.complex64)
@@ -137,7 +139,8 @@ def dfb_apply(model, st, spec, m, c, pf, mask_only):
 def run_apply_case(st, models, kind, opt, B, Tf, seed, rows=None):
     _, nb_df, mode, la = KINDS[kind]
     pf, mask_only = OPTS[opt]
-    spec, m, c = apply_inputs(B, Tf, nb_df, seed)
+    st = models[kind].df_state
+    spec, m, c = apply_inputs(B, Tf, nb_df, seed, st.nb_erb())
     got = dfb_apply(models[kind], st, spec, m, c, pf, mask_only)
     rows = list(range(B)) if rows is None else rows
     ref, b = R.apply(spec[rows], m[rows], c[rows], st.erb_widths(), mode=mode, nb_df=nb_df, order=5, lookahead=la,
@@ -168,10 +171,10 @@ def test_apply_16_frame_warps(st, models, kind, opt):
 
 @pytest.mark.parametrize("Tf", [1, 8, 9, 17, 33, 64, 65])
 @pytest.mark.parametrize("opt", list(OPTS))
-@pytest.mark.parametrize("kind", ["dfn3_df64", "dfn2_df64"])
+@pytest.mark.parametrize("kind", ["dfn3_df64", "dfn2_df64", "dfn3_e24"])
 def test_generic_apply_against_ref64(st, models, kind, opt, Tf):
-    """nb_df = 64: dfb_apply runs k_apply_synthesis_generic.  K = 1 (worst err / bound on an H100 80GB HBM3: 0.996; 0.60
-    with the post filter)."""
+    """nb_df = 64, or 24 ERB bands: dfb_apply runs k_apply_synthesis_generic.  K = 1 (worst err / bound on an H100 80GB HBM3:
+    0.996, 0.60 with the post filter at nb_df = 64; 0.991, 0.56 with the post filter at 24 bands)."""
     run_apply_case(st, models, kind, opt, 2, Tf, seed=50 + Tf)
 
 

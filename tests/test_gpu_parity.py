@@ -2,6 +2,7 @@
 seeded inputs, against the committed golden fixtures, and through size-independent properties at
 larger sizes.  Tolerances: integer indexing (ERB widths, frame counts, crop offsets) bit exact;
 floating point RMS(out - oracle) <= 1e-4 as BASELINE.json states (measured: ~2e-8)."""
+import dataclasses
 import json
 import os
 
@@ -34,6 +35,12 @@ def rms(a, b):
 
 def cfg_of(kind):
     base = dict(conv_ch=64, df_pathway_kernel_size_t=5)
+    if kind == "e24":           # 24 ERB bands: k_mask_out at kt = 1, block tiles of 120 / 120 / 126 rows
+        return dataclasses.replace(cfg_of("dfn3"), nb_erb=24)
+    if kind == "dfn2_e56_la1":  # 56 ERB bands, 48 DF bins (df_conv1 and df_fc_emb not fused), look-ahead 1
+        return dataclasses.replace(cfg_of("dfn2"), nb_erb=56, nb_df=48, conv_lookahead=1, df_lookahead=1)
+    if kind == "dfn2_la3":      # the largest look-ahead dfb_model_create accepts
+        return dataclasses.replace(cfg_of("dfn2"), conv_lookahead=3, df_lookahead=3)
     if kind == "dfn3":
         return ModelConfig(model="deepfilternet3", conv_lookahead=2, df_lookahead=2, emb_num_layers=3, df_num_layers=2,
                            lin_groups=16, enc_lin_groups=32, df_gru_skip="groupedlinear", **base)
@@ -406,14 +413,19 @@ def test_mismatched_df_state_is_rejected(states):
 
 
 # ------------------------------------------------------------------ time chunks / streaming ----
-@pytest.mark.parametrize("kind", ["dfn3", "dfn2", "ll"])
+def state_of(states, cfg):
+    return states[0] if cfg.nb_erb == 32 else libdf.DF(48000, 960, 480, cfg.nb_erb, 2)
+
+
+@pytest.mark.parametrize("kind", ["dfn3", "dfn2", "ll", "e24", "dfn2_e56_la1", "dfn2_la3"])
 def test_time_chunked_enhance_equals_one_shot(states, kind):
     """dfb_enhance runs in time chunks with carried state (STFT / ISTFT memories, norm EMAs, GRU states, conv and deep
     filter history -- SURVEY Appendix D).  One chunk, six chunks back to back, six chunks pipelined over the two lanes
     (encoder of chunk c + 1 overlapping the decoder of chunk c) and a workspace cap that forces many short chunks must all
-    give the same audio, on the device and the host path, and match the oracle."""
-    st, _ = states
+    give the same audio, on the device and the host path, and match the oracle.  Also at 24 and 56 ERB bands (the conv
+    kernels' halo at other tile geometries, look-ahead 1) and at look-ahead 3, the largest accepted."""
     cfg = cfg_of(kind)
+    st = state_of(states, cfg)
     sd = random_state_dict(cfg, seed=13)
     model = DfNet(cfg, sd, st)
     audio = synth_audio(3, 48000 * 5 + 123, seed=61, device="cuda")    # 501 frames + a partial hop
@@ -441,20 +453,20 @@ def test_time_chunked_enhance_equals_one_shot(states, kind):
     assert rms(nopad.cpu(), O.enhance(sd, cfg.as_dict(), audio.cpu(), pad=False)) < RMS_TOL
 
 
-@pytest.mark.parametrize("kind", ["dfn3", "dfn2", "ll"])
+@pytest.mark.parametrize("kind", ["dfn3", "dfn2", "ll", "e24", "dfn2_e56_la1", "dfn2_la3"])
 def test_streaming_equals_one_shot(states, kind):
     """SURVEY 8(f)-1: frame-incremental processing (DfTract::process, tract.rs:509-642) == one-shot enhance(pad=False)
     delayed by the model's look-ahead, for ragged call sizes down to a single hop, device and host tensors."""
     from deepfilternet_b200 import DfStream
-    st, _ = states
     cfg = cfg_of(kind)
+    st = state_of(states, cfg)
     sd = random_state_dict(cfg, seed=14)
     model = DfNet(cfg, sd, st)
     hop, n = 480, 157
     audio = synth_audio(2, hop * n, seed=71)
     ref = enhance(model, st, audio, pad=False)            # [2, n * hop], delayed by fft - hop
     s = DfStream(model, st, batch=2)
-    assert s.hop == hop and s.latency_frames == max(cfg.conv_lookahead, cfg.df_lookahead) + (cfg.df_lookahead if kind == "dfn2" else 0)
+    assert s.hop == hop and s.latency_frames == max(cfg.conv_lookahead, cfg.df_lookahead) + (cfg.df_lookahead if cfg.model == "deepfilternet2" else 0)
     outs, pos = [], 0
     for i, k in enumerate([1, 1, 2, 1, 7, 40, 1, 3, 64, 30, 7]):
         x = audio[:, pos * hop:(pos + k) * hop]
