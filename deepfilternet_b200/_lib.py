@@ -137,6 +137,12 @@ SIGNATURES = {
     "dfb_debug_df_convp_tc": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP, _I64, _VP]),
     "dfb_debug_gl_bx": (_I, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _I64, _VP, _VP, _I64, _I64, _I, _I, _I, _I, _F, _F, _VP]),
     "dfb_model_debug_fetch": (_I64, [_VP, C.c_char_p, _VP, _I64]),
+    "dfb_metrics_create": (_I, [C.POINTER(_VP), _I, _I, _VP, _I, _I, _I, _VP, _I, _I, _I]),
+    "dfb_metrics_free": (None, [_VP]),
+    "dfb_metrics_compute": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _VP, _I64, _I, _VP, _VP]),
+    "dfb_metrics_compute_host": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _VP, _I64, _I, _VP]),
+    "dfb_metrics_workspace_bytes": (_I64, [_VP]),
+    "dfb_debug_metrics_counts": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _VP]),
 }
 
 

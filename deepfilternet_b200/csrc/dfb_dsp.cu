@@ -1015,43 +1015,6 @@ constexpr int kGenCplx = 2048;
 constexpr int kGenSmemMax = 200 * 1024;   // odd N = 8191: 2 x 8191 x 8 B of buffers + 2 x 8190 x 4 B of tails
 inline int gen_frames(int M) { return std::max(1, std::min(32, kGenCplx / M)); }
 
-// The stage radices go to shared memory (a dynamically indexed kernel-parameter array would be copied to local memory).
-__device__ __forceinline__ void gen_load_radices(const GenFftPlan &pl, int *s_rad) {
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int i = 0; i < kGenMaxStages; i++) s_rad[i] = pl.rad[i];
-    }
-}
-
-// M-point complex FFT of the first nf frames (frame f at a + f M), with b as the second buffer; returns the buffer that
-// holds the result.  Every thread of the CTA takes part; ends with a barrier.
-template <bool INV>
-__device__ __forceinline__ float2 *gen_block_fft(float2 *a, float2 *b, const GenFftPlan &pl, const int *s_rad, int nf) {
-    const int M = pl.M, ts = pl.N / pl.M;
-    int Ns = 1;
-    for (int s = 0; s < pl.nst; s++) {
-        const int R = s_rad[s], nb = M / R, total = nf * nb;
-#define DFB_GEN_STAGE(CALL)                                                   \
-    for (int i = threadIdx.x; i < total; i += blockDim.x) {                   \
-        const int f = i / nb, j = i - f * nb;                                 \
-        CALL;                                                                 \
-    }
-        switch (R) {
-            case 2: DFB_GEN_STAGE((gen_bfly<2, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
-            case 3: DFB_GEN_STAGE((gen_bfly<3, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
-            case 4: DFB_GEN_STAGE((gen_bfly<4, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
-            case 5: DFB_GEN_STAGE((gen_bfly<5, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
-            case 7: DFB_GEN_STAGE((gen_bfly<7, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
-            default: DFB_GEN_STAGE((gen_bfly_any<INV>(a + f * M, b + f * M, M, Ns, R, j, pl.tw, ts))) break;
-        }
-#undef DFB_GEN_STAGE
-        __syncthreads();
-        float2 *t = a; a = b; b = t;
-        Ns *= R;
-    }
-    return a;
-}
-
 // grid (ceil(Tf / G), B), kGenThreads threads.  Frame t = window x samples [t H - (N - H), t H + H) of stream b, zeros
 // (or init_mem [B][N - H], the carried analysis memory) before sample 0; spec [B][Tf][F] = wnorm * rfft; erb_db (or null)
 // [B][Tf][E] = the ERB dB of the spectrum (lib.rs:280-295, 207-210), from the band energies kept in shared memory.

@@ -141,4 +141,45 @@ DFB_HD void gen_stage_bfly(const float2 *src, float2 *dst, int M, int Ns, int R,
     }
 }
 
+#ifdef __CUDACC__
+// Block-wide transforms of several frames at once (the generic STFT / ISTFT kernels of dfb_dsp.cu, the STOI STFT of
+// dfb_metrics.cu).
+// The stage radices go to shared memory (a dynamically indexed kernel-parameter array would be copied to local memory).
+__device__ __forceinline__ void gen_load_radices(const GenFftPlan &pl, int *s_rad) {
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int i = 0; i < kGenMaxStages; i++) s_rad[i] = pl.rad[i];
+    }
+}
+
+// M-point complex FFT of the first nf frames (frame f at a + f M), with b as the second buffer; returns the buffer that
+// holds the result.  Every thread of the CTA takes part; ends with a barrier.
+template <bool INV>
+__device__ __forceinline__ float2 *gen_block_fft(float2 *a, float2 *b, const GenFftPlan &pl, const int *s_rad, int nf) {
+    const int M = pl.M, ts = pl.N / pl.M;
+    int Ns = 1;
+    for (int s = 0; s < pl.nst; s++) {
+        const int R = s_rad[s], nb = M / R, total = nf * nb;
+#define DFB_GEN_STAGE(CALL)                                                   \
+    for (int i = threadIdx.x; i < total; i += blockDim.x) {                   \
+        const int f = i / nb, j = i - f * nb;                                 \
+        CALL;                                                                 \
+    }
+        switch (R) {
+            case 2: DFB_GEN_STAGE((gen_bfly<2, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
+            case 3: DFB_GEN_STAGE((gen_bfly<3, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
+            case 4: DFB_GEN_STAGE((gen_bfly<4, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
+            case 5: DFB_GEN_STAGE((gen_bfly<5, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
+            case 7: DFB_GEN_STAGE((gen_bfly<7, INV>(a + f * M, b + f * M, M, Ns, j, pl.tw, ts))) break;
+            default: DFB_GEN_STAGE((gen_bfly_any<INV>(a + f * M, b + f * M, M, Ns, R, j, pl.tw, ts))) break;
+        }
+#undef DFB_GEN_STAGE
+        __syncthreads();
+        float2 *t = a; a = b; b = t;
+        Ns *= R;
+    }
+    return a;
+}
+#endif
+
 }  // namespace dfb

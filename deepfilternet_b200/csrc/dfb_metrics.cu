@@ -1,0 +1,656 @@
+// dfb_metrics.cu -- batched speech-quality metrics of a ragged batch (dfb_metrics* in include/dfb200.h; DESIGN.md section 5j):
+// SI-SDR (DeepFilterNet/df/evaluation_utils.py si_sdr_speechmetrics), STOI (df/stoi.py stoi, after io.resample to 10 kHz)
+// and segmental SNR (df/sepm.py SNRseg, after io.resample to 16 kHz).
+//
+// One call is a fixed sequence of launches, with no host round trip between them:
+//   k_resample_rows (dfb_dsp.cu)  clean and degraded rows -> 10 kHz / 16 kHz, one launch per signal
+//   k_stoi_energy                 one warp per 256-sample frame: the frame's energy in dB
+//   k_stoi_mask                   one CTA per entry: the entry's loudest frame, the 40 dB mask, the prefix count of kept
+//                                 frames (their index list), the compacted and STFT lengths
+//   k_stoi_stft                   four STFT frames of both signals per CTA, their samples computed from the kept-frame list
+//                                 (never materialised): the 15 third-octave band magnitudes
+//   k_stoi_seg                    one warp per 30-frame segment: the sum over bands of the clipped, normalised correlations
+//   k_ssnr                        one warp per 480-sample frame at 16 kHz: the clipped segmental SNR (fp64)
+//   k_sisdr                       one CTA per 4096-sample chunk: fp64 sums r.r, r.e, e.e
+//   k_metrics_final               one CTA per entry: the per-entry means / SI-SDR from the frame, segment and chunk values
+// Every per-entry sum runs in an order fixed relative to the entry's start (per-thread strided sums, then a fixed shuffle
+// and shared-memory tree), with no atomics, so an entry's results are the same bits wherever and with whatever it is batched.
+#include <algorithm>
+#include <cmath>
+#include <cstring>
+#include <numeric>
+#include <vector>
+
+#include "dfb_common.cuh"
+
+namespace dfb {
+namespace {
+
+constexpr int kStoiFs = 10000, kSsnrFs = 16000;
+constexpr int kStoiFrame = 256, kStoiHop = 128, kStoiFft = 512, kStoiBands = 15, kStoiSeg = 30;
+constexpr int kSsnrWin = 480, kSsnrHop = 120;            // round(0.03 fs), floor(0.25 * 0.03 fs) at 16 kHz
+constexpr int kSisdrChunk = 4096;
+constexpr int kStftFrames = 4;                           // STFT frames per CTA of k_stoi_stft (two signals each)
+constexpr float kEps64f = 2.220446049250313e-16f;        // np.finfo(float).eps, as df/stoi.py adds it to float32 tensors
+constexpr double kEps64 = 2.220446049250313e-16;         // np.finfo(np.float64).eps (sepm.SNRseg)
+constexpr double kEps32 = 1.1920928955078125e-07;        // np.finfo(np.float32).eps (si_sdr_speechmetrics on float32)
+
+__constant__ float c_w256[kStoiFrame];   // torch.hann_window(258, periodic=False)[1:-1]
+__constant__ double c_wss[kSsnrWin];     // SNRseg's hannWin: 0.5 (1 - cos(2 pi n / 481)), n = 1 .. 480
+
+// One entry of a call, planned on the host.
+struct MetEntry {
+    int64_t in_off, len;    // clean / degraded samples at the call's rate
+    int64_t o10, t10;       // its 10 kHz rows at x10 / y10 + o10
+    int64_t o16, t16;       // its 16 kHz rows at x16 / y16 + o16
+    int64_t fo;             // first STOI frame: energies en[fo ..], kept list kidx[fo ..], segments seg[fo ..], bands at 15 fo
+    int64_t so;             // first SSNR frame value
+    int64_t co;             // first SI-SDR chunk
+    int nfr, pad_front, pad_end, nfs, nch;
+};
+// What the device finds out about an entry's STOI (dfb_debug_metrics_counts reads it back).
+struct MetState { int nk, s0, lc, nf; };
+struct StoiBands { int lo[kStoiBands], hi[kStoiBands]; float inv_wsum; };
+
+struct MetBufs {
+    const float *x10, *y10, *x16, *y16, *clean, *degraded;
+    float *en, *bx, *by, *seg;
+    int *kidx;
+    double *ss;
+    double *ch;   // [3][chunks]
+    MetState *st;
+    int64_t n_fr, n_ch;
+};
+
+// ---- deterministic reductions ----
+template <typename T>
+__device__ __forceinline__ T warp_sum(T v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+// Sum over the CTA (blockDim.x a multiple of 32, <= 1024); every thread gets the result.  A fixed tree.
+template <typename T>
+__device__ T block_sum(T v, T *sm) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    v = warp_sum(v);
+    __syncthreads();
+    if (lane == 0) sm[w] = v;
+    __syncthreads();
+    T r = lane < nw ? sm[lane] : T(0);
+    r = warp_sum(r);
+    return r;
+}
+
+__device__ __forceinline__ float xat(const float *x, int64_t n, int64_t p) { return p >= 0 && p < n ? __ldg(x + p) : 0.f; }
+
+// grid (ceil(max nfr / 8), B), 256 threads: warp w of CTA x is frame 8 x + w of entry blockIdx.y.  Frame i is samples
+// [128 i, 128 i + 256) of the clean 10 kHz row padded by pad_front zeros in front, times the window:
+// en = 20 log10(|frame| / sqrt(256) + eps).
+__global__ void __launch_bounds__(256) k_stoi_energy(const MetEntry *__restrict__ ents, MetBufs b) {
+    const MetEntry e = ents[blockIdx.y];
+    const int i = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (i >= e.nfr) return;
+    const float *x = b.x10 + e.o10;
+    const int64_t p0 = (int64_t)i * kStoiHop - e.pad_front;
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < kStoiFrame / 32; k++) {
+        const int n = lane + 32 * k;
+        const float v = xat(x, e.t10, p0 + n) * c_w256[n];
+        s = fmaf(v, v, s);
+    }
+    s = warp_sum(s);
+    if (lane == 0) b.en[e.fo + i] = 20.f * log10f(sqrtf(s) / 16.f + kEps64f);
+}
+
+// grid B, 1024 threads: frame i is kept when (max_j en_j - 40) - en_i < 0 (df/stoi.py remove_silent_frames, in float32);
+// kidx[fo + j] is the j-th kept frame.  The overlap-added kept frames have (nk - 1) 128 + 256 samples; the first pad_front
+// are dropped when frame 0 is kept, the last pad_end when the last frame is kept.  STOI needs at least 512 samples.
+__global__ void __launch_bounds__(1024) k_stoi_mask(const MetEntry *__restrict__ ents, MetBufs b) {
+    __shared__ float s_red[32];
+    __shared__ int s_cnt[33];
+    const MetEntry e = ents[blockIdx.x];
+    const float *en = b.en + e.fo;
+    float mx = -INFINITY;
+    for (int i = threadIdx.x; i < e.nfr; i += blockDim.x) mx = fmaxf(mx, en[i]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    if (lane == 0) s_red[w] = mx;
+    __syncthreads();
+    mx = s_red[0];
+    for (int k = 1; k < nw; k++) mx = fmaxf(mx, s_red[k]);
+    const float thr = mx - 40.f;
+    int base = 0;
+    for (int c0 = 0; c0 < e.nfr; c0 += blockDim.x) {
+        const int i = c0 + threadIdx.x;
+        const bool keep = i < e.nfr && (thr - en[i]) < 0.f;
+        const unsigned bal = __ballot_sync(0xffffffffu, keep);
+        __syncthreads();   // s_cnt of the previous chunk is consumed
+        if (lane == 0) s_cnt[w] = __popc(bal);
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            int a = 0;
+            for (int k = 0; k < nw; k++) { const int c = s_cnt[k]; s_cnt[k] = a; a += c; }
+            s_cnt[32] = a;
+        }
+        __syncthreads();
+        if (keep) b.kidx[e.fo + base + s_cnt[w] + __popc(bal & ((1u << lane) - 1u))] = i;
+        base += s_cnt[32];
+    }
+    if (threadIdx.x == 0) {
+        const int nk = base;
+        const bool first = (thr - en[0]) < 0.f, last = (thr - en[e.nfr - 1]) < 0.f;
+        MetState s;
+        s.nk = nk;
+        s.s0 = first ? e.pad_front : 0;
+        s.lc = (nk - 1) * kStoiHop + kStoiFrame - s.s0 - (last ? e.pad_end : 0);
+        s.nf = s.lc >= kStoiFft ? 1 + (s.lc - kStoiFrame) / kStoiHop : 0;
+        b.st[blockIdx.x] = s;
+    }
+}
+
+// Sample s of the compacted signal (after the front trim s0): overlap-add of the kept frames that cover it, at most two at
+// 50 % overlap, divided by the overlap-added window.
+__device__ __forceinline__ void compact_at(const MetEntry &e, const MetState &st, const int *__restrict__ kidx, const float *x,
+                                           const float *y, int64_t s, float &xv, float &yv) {
+    const int64_t r = s + st.s0;
+    const int64_t j1 = r >> 7;
+    const int q = (int)(r & 127);
+    float nx = 0.f, ny = 0.f, den = 0.f;
+    if (j1 >= 1) {
+        const int64_t p = (int64_t)__ldg(kidx + j1 - 1) * kStoiHop + q + kStoiHop - e.pad_front;
+        const float w = c_w256[q + kStoiHop];
+        nx = xat(x, e.t10, p) * w; ny = xat(y, e.t10, p) * w; den = w;
+    }
+    if (j1 < st.nk) {
+        const int64_t p = (int64_t)__ldg(kidx + j1) * kStoiHop + q - e.pad_front;
+        const float w = c_w256[q];
+        nx += xat(x, e.t10, p) * w; ny += xat(y, e.t10, p) * w; den += w;
+    }
+    xv = nx / den;
+    yv = ny / den;
+}
+
+// grid (ceil(max nfr / 4), B), 256 threads: STFT frames [4 x, 4 x + 4) of entry blockIdx.y (df/stoi.py _stft: the windowed
+// 256 samples [128 f, 128 f + 256) of the compacted signal in a 512-point real FFT, / sum(window)), both signals: 8 real
+// transforms as 256-point complex ones (dfb_fft_generic.cuh), then the band magnitudes sqrt(sum_band |X_k|^2) to
+// bx / by [15 fo + band nfr + f].
+__global__ void __launch_bounds__(256) k_stoi_stft(const MetEntry *__restrict__ ents, MetBufs b, GenFftPlan pl, StoiBands bands) {
+    constexpr int M = kStoiFft / 2, NS = 2 * kStftFrames;
+    __shared__ __align__(16) float2 A[NS * M], Bf[NS * M];
+    __shared__ int s_rad[kGenMaxStages];
+    const MetEntry e = ents[blockIdx.y];
+    const MetState st = b.st[blockIdx.y];
+    const int f0 = blockIdx.x * kStftFrames;
+    if (f0 >= st.nf) return;
+    const int nf = min(kStftFrames, st.nf - f0);
+    gen_load_radices(pl, s_rad);
+    const int *kidx = b.kidx + e.fo;
+    const float *x = b.x10 + e.o10, *y = b.y10 + e.o10;
+    for (int i = threadIdx.x; i < kStftFrames * kStoiFft; i += blockDim.x) {
+        const int f = i / kStoiFft, n = i - f * kStoiFft;
+        float xv = 0.f, yv = 0.f;
+        if (f < nf && n < kStoiFrame) {
+            compact_at(e, st, kidx, x, y, (int64_t)(f0 + f) * kStoiHop + n, xv, yv);
+            xv *= c_w256[n];
+            yv *= c_w256[n];
+        }
+        reinterpret_cast<float *>(A + (2 * f) * M)[n] = xv;
+        reinterpret_cast<float *>(A + (2 * f + 1) * M)[n] = yv;
+    }
+    __syncthreads();
+    float2 *Z = gen_block_fft<false>(A, Bf, pl, s_rad, NS);
+    float *P = reinterpret_cast<float *>(Z == A ? Bf : A);   // |X_k|^2, bins [klo, khi) of each transform
+    const int klo = bands.lo[0], khi = bands.hi[kStoiBands - 1], nk = khi - klo;
+    for (int i = threadIdx.x; i < NS * nk; i += blockDim.x) {
+        const int t = i / nk, k = klo + (i - t * nk);
+        float2 xk, xnk;
+        rfft_split(Z[t * M + k % M], Z[t * M + (M - k) % M], __ldg(pl.tw + k), xk, xnk);
+        xk.x *= bands.inv_wsum; xk.y *= bands.inv_wsum;
+        P[t * nk + (k - klo)] = xk.x * xk.x + xk.y * xk.y;
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < NS * kStoiBands; i += blockDim.x) {
+        const int t = i / kStoiBands, band = i - t * kStoiBands, f = t >> 1;
+        if (f >= nf) continue;
+        float acc = 0.f;
+        for (int k = bands.lo[band]; k < bands.hi[band]; k++) acc += P[t * nk + (k - klo)];
+        float *dst = (t & 1) ? b.by : b.bx;
+        dst[kStoiBands * e.fo + (int64_t)band * e.nfr + f0 + f] = sqrtf(acc);
+    }
+}
+
+// grid (ceil(max nfr / 8), B), 256 threads: warp w of CTA x is segment m = 8 x + w of entry blockIdx.y: frames [m, m + 30)
+// (one segment of all L frames when L <= 30).  seg[fo + m] = sum over the bands of the correlation of the normalised,
+// clipped, mean-free band envelopes (df/stoi.py stoi), lane l holding frame m + l.
+__global__ void __launch_bounds__(256) k_stoi_seg(const MetEntry *__restrict__ ents, MetBufs b) {
+    const MetEntry e = ents[blockIdx.y];
+    const int L = b.st[blockIdx.y].nf;
+    const int J = L > kStoiSeg ? L - kStoiSeg + 1 : 1, N = L > kStoiSeg ? kStoiSeg : L;
+    const int m = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (L == 0 || m >= J) return;
+    const float c1 = 1.f + 5.62341325190349f;   // 1 + 10^(15 / 20), Beta = -15 dB
+    const bool in = lane < N;
+    float corr = 0.f;
+    for (int band = 0; band < kStoiBands; band++) {
+        const int64_t o = kStoiBands * e.fo + (int64_t)band * e.nfr + m + lane;
+        const float xv = in ? b.bx[o] : 0.f, yv0 = in ? b.by[o] : 0.f;
+        const float nrm = sqrtf(warp_sum(xv * xv)) / (sqrtf(warp_sum(yv0 * yv0)) + kEps64f);
+        const float yv = in ? fminf(yv0 * nrm, xv * c1) : 0.f;
+        const float xm = warp_sum(xv) / (float)N, ym = warp_sum(yv) / (float)N;
+        const float xd = in ? xv - xm : 0.f, yd = in ? yv - ym : 0.f;
+        const float xn = xd / (sqrtf(warp_sum(xd * xd)) + kEps64f), yn = yd / (sqrtf(warp_sum(yd * yd)) + kEps64f);
+        corr += warp_sum(xn * yn);
+    }
+    if (lane == 0) b.seg[e.fo + m] = corr;
+}
+
+// grid (ceil(max nfs / 8), B), 256 threads: warp w of CTA x is SSNR frame i = 8 x + w (samples [120 i, 120 i + 480) at 16 kHz)
+// of entry blockIdx.y; the last frame is not computed (SNRseg drops it).  fp64, as SNRseg computes.
+__global__ void __launch_bounds__(256) k_ssnr(const MetEntry *__restrict__ ents, MetBufs b) {
+    const MetEntry e = ents[blockIdx.y];
+    const int i = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (i >= e.nfs - 1) return;
+    const float *c = b.x16 + e.o16 + (int64_t)i * kSsnrHop, *d = b.y16 + e.o16 + (int64_t)i * kSsnrHop;
+    double sig = 0.0, noi = 0.0;
+    for (int n = lane; n < kSsnrWin; n += 32) {
+        const double w = c_wss[n], cw = w * (double)__ldg(c + n), dw = w * (double)__ldg(d + n);
+        sig = fma(cw, cw, sig);
+        noi = fma(cw - dw, cw - dw, noi);
+    }
+    sig = warp_sum(sig);
+    noi = warp_sum(noi);
+    if (lane == 0) {
+        double v = 10.0 * log10(sig / (noi + kEps64) + kEps64);
+        b.ss[e.so + i] = v < -10.0 ? -10.0 : (v > 35.0 ? 35.0 : v);
+    }
+}
+
+// grid (ceil(max chunks), B), 256 threads: chunk k of entry blockIdx.y, samples [4096 k, 4096 k + 4096): fp64 sums of
+// r r, r e and e e (each product of two floats is exact in fp64).
+__global__ void __launch_bounds__(256) k_sisdr(const MetEntry *__restrict__ ents, MetBufs b) {
+    __shared__ double sm[32];
+    const MetEntry e = ents[blockIdx.y];
+    if ((int)blockIdx.x >= e.nch) return;
+    const int64_t p0 = e.in_off + (int64_t)blockIdx.x * kSisdrChunk;
+    const int64_t n = min((int64_t)kSisdrChunk, e.len - (int64_t)blockIdx.x * kSisdrChunk);
+    double rr = 0.0, re = 0.0, ee = 0.0;
+    for (int64_t k = threadIdx.x; k < n; k += blockDim.x) {
+        const double r = __ldg(b.clean + p0 + k), s = __ldg(b.degraded + p0 + k);
+        rr = fma(r, r, rr); re = fma(r, s, re); ee = fma(s, s, ee);
+    }
+    rr = block_sum(rr, sm);
+    re = block_sum(re, sm);
+    ee = block_sum(ee, sm);
+    if (threadIdx.x == 0) {
+        const int64_t o = e.co + blockIdx.x;
+        b.ch[o] = rr; b.ch[b.n_ch + o] = re; b.ch[2 * b.n_ch + o] = ee;
+    }
+}
+
+// grid B, 256 threads: out[row][b] for the metrics of `bits`, rows in the order SI-SDR, STOI, SSNR.
+__global__ void __launch_bounds__(256) k_metrics_final(const MetEntry *__restrict__ ents, MetBufs b, int bits, float *out, int64_t B) {
+    __shared__ double sm[32];
+    const MetEntry e = ents[blockIdx.x];
+    int row = 0;
+    if (bits & DFB_METRIC_SISDR) {
+        double rr = 0.0, re = 0.0, ee = 0.0;
+        for (int k = threadIdx.x; k < e.nch; k += blockDim.x) {
+            rr += b.ch[e.co + k]; re += b.ch[b.n_ch + e.co + k]; ee += b.ch[2 * b.n_ch + e.co + k];
+        }
+        rr = block_sum(rr, sm);
+        re = block_sum(re, sm);
+        ee = block_sum(ee, sm);
+        if (threadIdx.x == 0) {
+            const double a = (kEps32 + re) / (rr + kEps32);
+            const double sss = a * a * rr;
+            double snn = ee - 2.0 * a * re + a * a * rr;   // |e - a r|^2; the sums are exact to ~1e-16 of ee
+            if (snn < 0.0) snn = 0.0;
+            out[row * B + blockIdx.x] = (float)(10.0 * log10((kEps32 + sss) / (kEps32 + snn)));
+        }
+        row++;
+    }
+    if (bits & DFB_METRIC_STOI) {
+        const int L = b.st[blockIdx.x].nf, J = L > kStoiSeg ? L - kStoiSeg + 1 : 1;
+        float s = 0.f;
+        for (int k = threadIdx.x; k < J && L > 0; k += blockDim.x) s += b.seg[e.fo + k];
+        s = block_sum(s, reinterpret_cast<float *>(sm));
+        if (threadIdx.x == 0) out[row * B + blockIdx.x] = L > 0 ? s / (float)(kStoiBands * J) : __int_as_float(0x7fc00000);
+        row++;
+    }
+    if (bits & DFB_METRIC_SSNR) {
+        const int n = e.nfs - 1;
+        double s = 0.0;
+        for (int k = threadIdx.x; k < n; k += blockDim.x) s += b.ss[e.so + k];
+        s = block_sum(s, sm);
+        if (threadIdx.x == 0) out[row * B + blockIdx.x] = n > 0 ? (float)(s / n) : __int_as_float(0x7fc00000);
+    }
+}
+
+// thirdoct (df/stoi.py): band i covers the FFT bins [lo, hi) nearest to 150 Hz 2^((2 i -+ 1) / 6) at 10 kHz, 512 points
+StoiBands stoi_bands() {
+    StoiBands b{};
+    const int nb = kStoiFft / 2 + 1;
+    auto nearest = [&](double fq) {
+        int best = 0;
+        double bd = INFINITY;
+        for (int k = 0; k < nb; k++) {
+            const double d = (k * ((double)kStoiFs / kStoiFft) - fq) * (k * ((double)kStoiFs / kStoiFft) - fq);
+            if (d < bd) { bd = d; best = k; }
+        }
+        return best;
+    };
+    for (int i = 0; i < kStoiBands; i++) {
+        b.lo[i] = nearest(150.0 * std::pow(2.0, (2.0 * i - 1) / 6));
+        b.hi[i] = nearest(150.0 * std::pow(2.0, (2.0 * i + 1) / 6));
+    }
+    double ws = 0.0;
+    for (int n = 0; n < kStoiFrame; n++) ws += (double)(float)(0.5 - 0.5 * std::cos(2.0 * M_PI * (n + 1) / (kStoiFrame + 1)));
+    b.inv_wsum = (float)(1.0 / ws);
+    return b;
+}
+
+}  // namespace
+}  // namespace dfb
+
+using namespace dfb;
+
+struct dfb_metrics {
+    int device, sr;
+    cudaStream_t stream = nullptr;
+    float *d_taps = nullptr;      // the sr -> 10 kHz and sr -> 16 kHz tap tables
+    RateDir dirs[2]{};            // 0: -> 10 kHz, 1: -> 16 kHz (taps null: sr is that rate)
+    RateDir *d_dirs = nullptr;
+    float2 *d_tw = nullptr;       // twiddles of the 512-point real FFT
+    GenFftPlan plan{};
+    StoiBands bands{};
+    Arena arena;                  // per-call workspace, grown when a call needs more
+    int64_t last_b = 0;           // entries of the last call (dfb_debug_metrics_counts)
+    MetState *last_st = nullptr;  // their STOI states, inside the arena
+};
+
+namespace {
+
+int64_t resampled_len(int64_t T, int og, int nw) { return (nw * T + og - 1) / og; }
+
+int check_taps(int sr, int to, const float *taps, int og, int nw, int width, int64_t *floats) {
+    *floats = 0;
+    if (sr == to) return DFB_OK;
+    int64_t g = std::gcd((int64_t)sr, (int64_t)to);
+    if (!taps || og != sr / g || nw != to / g || width <= 0)
+        return fail(DFB_ERR_INVALID, "the taps of %d Hz -> %d Hz are io.resample_kernel(%d, %d) (og %lld, nw %lld)", sr, to, sr, to,
+                    (long long)(sr / g), (long long)(to / g));
+    *floats = (int64_t)nw * (2 * width + og);
+    return DFB_OK;
+}
+
+// The buffers of a call of B entries, planned on the host: (entries, workspace bytes).
+struct MetPlan {
+    std::vector<MetEntry> ents;
+    std::vector<RateRow> rows;
+    int64_t n10 = 0, n16 = 0, n_fr = 0, n_ss = 0, n_ch = 0, max_fr = 0, max_ss = 0, max_ch = 0, max_out = 0;
+};
+
+int plan_call(const dfb_metrics *h, int64_t in_numel, const int64_t *offsets, const int64_t *lengths, const int64_t *deg_lengths,
+              int64_t B, int bits, MetPlan &p) {
+    if (B <= 0 || B > 32767) return fail(DFB_ERR_INVALID, "batch of %lld entries: 1 .. 32767 per call", (long long)B);
+    if (bits <= 0 || (bits & ~(DFB_METRIC_SISDR | DFB_METRIC_STOI | DFB_METRIC_SSNR)))
+        return fail(DFB_ERR_INVALID, "unknown metric bits 0x%x (SI-SDR 1, STOI 2, SSNR 4)", bits);
+    if (!offsets || !lengths || !deg_lengths) return fail(DFB_ERR_INVALID, "null layout");
+    const bool stoi = bits & DFB_METRIC_STOI, ssnr = bits & DFB_METRIC_SSNR;
+    const bool rs10 = stoi && h->dirs[0].taps, rs16 = ssnr && h->dirs[1].taps;
+    p.ents.resize(B);
+    for (int64_t b = 0; b < B; b++) {
+        const int64_t T = lengths[b];
+        if (T <= 0) return fail(DFB_ERR_INVALID, "entry %lld: length %lld, must be > 0", (long long)b, (long long)T);
+        if (deg_lengths[b] != T)
+            return fail(DFB_ERR_INVALID, "entry %lld: clean has %lld samples, degraded %lld", (long long)b, (long long)T,
+                        (long long)deg_lengths[b]);
+        if (offsets[b] < 0 || offsets[b] > in_numel - T)
+            return fail(DFB_ERR_INVALID, "entry %lld reaches outside the %lld input samples", (long long)b, (long long)in_numel);
+        MetEntry &e = p.ents[b];
+        std::memset(&e, 0, sizeof e);
+        e.in_off = offsets[b];
+        e.len = T;
+        if (stoi) {
+            e.t10 = rs10 ? resampled_len(T, h->dirs[0].og, h->dirs[0].nw) : T;
+            e.o10 = rs10 ? p.n10 : e.in_off;
+            if (rs10) {
+                p.rows.push_back(RateRow{e.in_off, T, e.o10, e.t10, 0, 0});
+                p.n10 += e.t10;
+                p.max_out = std::max(p.max_out, e.t10);
+            }
+            const int64_t pad = kStoiFrame - e.t10 % kStoiFrame;
+            e.pad_front = (int)(pad / 2);
+            e.pad_end = (int)(pad - pad / 2);
+            const int64_t nfr = (e.t10 + pad) / kStoiHop - 1;
+            if (nfr > (1 << 30)) return fail(DFB_ERR_INVALID, "entry %lld is too long", (long long)b);
+            e.nfr = (int)nfr;
+            e.fo = p.n_fr;
+            p.n_fr += nfr;
+            p.max_fr = std::max(p.max_fr, nfr);
+        }
+        if (ssnr) {
+            e.t16 = rs16 ? resampled_len(T, h->dirs[1].og, h->dirs[1].nw) : T;
+            e.o16 = rs16 ? 0 : e.in_off;   // (16 kHz rows follow the 10 kHz ones: offset set below)
+            if (rs16) {
+                p.rows.push_back(RateRow{e.in_off, T, p.n16, e.t16, 0, 1});
+                e.o16 = p.n16;
+                p.n16 += e.t16;
+                p.max_out = std::max(p.max_out, e.t16);
+            }
+            const int64_t nfs = e.t16 >= kSsnrWin - kSsnrHop ? (e.t16 - kSsnrWin + kSsnrHop) / kSsnrHop : 0;
+            e.nfs = (int)nfs;
+            e.so = p.n_ss;
+            p.n_ss += std::max<int64_t>(nfs - 1, 0);
+            p.max_ss = std::max(p.max_ss, nfs);
+        }
+        if (bits & DFB_METRIC_SISDR) {
+            e.nch = (int)((T + kSisdrChunk - 1) / kSisdrChunk);
+            e.co = p.n_ch;
+            p.n_ch += e.nch;
+            p.max_ch = std::max<int64_t>(p.max_ch, e.nch);
+        }
+    }
+    // the 16 kHz rows live after the 10 kHz ones in the same resampled buffer
+    for (auto &r : p.rows)
+        if (r.dir == 1) r.out_off += p.n10;
+    for (auto &e : p.ents)
+        if (rs16) e.o16 += p.n10;
+    return DFB_OK;
+}
+
+size_t a256(size_t n) { return (n + 255) & ~size_t(255); }
+
+size_t call_bytes(const MetPlan &p, int64_t B, bool host, int64_t in_numel, int n_rows) {
+    size_t s = a256(sizeof(MetEntry) * B) + a256(sizeof(RateRow) * (p.rows.size() + 1)) + a256(sizeof(MetState) * B);
+    s += 2 * a256(sizeof(float) * (p.n10 + p.n16 + 1));                  // resampled clean / degraded
+    s += a256(sizeof(float) * (p.n_fr + 1)) * 2 + a256(sizeof(int) * (p.n_fr + 1));   // energies, segments, kept list
+    s += 2 * a256(sizeof(float) * (kStoiBands * p.n_fr + 1));            // band magnitudes
+    s += a256(sizeof(double) * (p.n_ss + 1)) + a256(sizeof(double) * (3 * p.n_ch + 1));
+    if (host) s += 2 * a256(sizeof(float) * in_numel) + a256(sizeof(float) * n_rows * B);
+    return s;
+}
+
+int run_call(dfb_metrics *h, const float *d_clean, const float *d_deg, const MetPlan &p, int64_t B, int bits, float *d_out,
+             cudaStream_t s, const float *h_clean, const float *h_deg, int64_t in_numel, float *h_out) {
+    const bool host = h_clean != nullptr;
+    const int n_rows = __builtin_popcount(bits);
+    int rc = h->arena.reserve(call_bytes(p, B, host, in_numel, n_rows));
+    if (rc) return rc;
+    Arena &a = h->arena;
+    a.reset();
+    MetEntry *d_ents = a.take<MetEntry>(B);
+    RateRow *d_rows = a.take<RateRow>(p.rows.size() + 1);
+    MetBufs mb{};
+    mb.st = a.take<MetState>(B);
+    float *rx = a.take<float>(p.n10 + p.n16 + 1), *ry = a.take<float>(p.n10 + p.n16 + 1);
+    mb.en = a.take<float>(p.n_fr + 1);
+    mb.seg = a.take<float>(p.n_fr + 1);
+    mb.kidx = a.take<int>(p.n_fr + 1);
+    mb.bx = a.take<float>(kStoiBands * p.n_fr + 1);
+    mb.by = a.take<float>(kStoiBands * p.n_fr + 1);
+    mb.ss = a.take<double>(p.n_ss + 1);
+    mb.ch = a.take<double>(3 * p.n_ch + 1);
+    mb.n_fr = p.n_fr;
+    mb.n_ch = p.n_ch;
+    if (host) {
+        float *c = a.take<float>(in_numel), *d = a.take<float>(in_numel);
+        d_out = a.take<float>((size_t)n_rows * B);
+        DFB_CUDA(cudaMemcpyAsync(c, h_clean, sizeof(float) * in_numel, cudaMemcpyHostToDevice, s));
+        DFB_CUDA(cudaMemcpyAsync(d, h_deg, sizeof(float) * in_numel, cudaMemcpyHostToDevice, s));
+        d_clean = c;
+        d_deg = d;
+    }
+    mb.clean = d_clean;
+    mb.degraded = d_deg;
+    mb.x10 = h->dirs[0].taps ? rx : d_clean;
+    mb.y10 = h->dirs[0].taps ? ry : d_deg;
+    mb.x16 = h->dirs[1].taps ? rx : d_clean;
+    mb.y16 = h->dirs[1].taps ? ry : d_deg;
+    DFB_CUDA(cudaMemcpyAsync(d_ents, p.ents.data(), sizeof(MetEntry) * B, cudaMemcpyHostToDevice, s));
+    if (!p.rows.empty()) {
+        DFB_CUDA(cudaMemcpyAsync(d_rows, p.rows.data(), sizeof(RateRow) * p.rows.size(), cudaMemcpyHostToDevice, s));
+        int smem = 0;
+        for (const RateDir &d : h->dirs)
+            if (d.taps && d.nw * d.K <= kRateSmemFloats) smem = std::max(smem, d.nw * d.K);
+        for (int sig = 0; sig < 2; sig++) {
+            const RateIO io{sig ? d_deg : d_clean, sig ? ry : rx, 0, p.max_out, 0, 0};
+            rc = launch_resample_rows(s, true, h->d_dirs, d_rows, (int)p.rows.size(), io, p.max_out, smem);
+            if (rc) return rc;
+        }
+    }
+    const unsigned ub = (unsigned)B;
+    if (bits & DFB_METRIC_STOI) {
+        k_stoi_energy<<<dim3((unsigned)((p.max_fr + 7) / 8), ub), 256, 0, s>>>(d_ents, mb);
+        DFB_LAUNCH_CHECK();
+        k_stoi_mask<<<ub, 1024, 0, s>>>(d_ents, mb);
+        DFB_LAUNCH_CHECK();
+        k_stoi_stft<<<dim3((unsigned)((p.max_fr + kStftFrames - 1) / kStftFrames), ub), 256, 0, s>>>(d_ents, mb, h->plan, h->bands);
+        DFB_LAUNCH_CHECK();
+        k_stoi_seg<<<dim3((unsigned)((p.max_fr + 7) / 8), ub), 256, 0, s>>>(d_ents, mb);
+        DFB_LAUNCH_CHECK();
+    }
+    if ((bits & DFB_METRIC_SSNR) && p.max_ss > 1) {
+        k_ssnr<<<dim3((unsigned)((p.max_ss + 7) / 8), ub), 256, 0, s>>>(d_ents, mb);
+        DFB_LAUNCH_CHECK();
+    }
+    if (bits & DFB_METRIC_SISDR) {
+        k_sisdr<<<dim3((unsigned)p.max_ch, ub), 256, 0, s>>>(d_ents, mb);
+        DFB_LAUNCH_CHECK();
+    }
+    k_metrics_final<<<ub, 256, 0, s>>>(d_ents, mb, bits, d_out, B);
+    DFB_LAUNCH_CHECK();
+    h->last_b = (bits & DFB_METRIC_STOI) ? B : 0;
+    h->last_st = mb.st;
+    if (host) {
+        DFB_CUDA(cudaMemcpyAsync(h_out, d_out, sizeof(float) * n_rows * B, cudaMemcpyDeviceToHost, s));
+        DFB_CUDA(cudaStreamSynchronize(s));
+    }
+    return DFB_OK;
+}
+
+}  // namespace
+
+extern "C" int dfb_metrics_create(dfb_metrics **out, int device, int sr, const float *taps10, int og10, int nw10, int width10,
+                                  const float *taps16, int og16, int nw16, int width16) {
+    if (!out) return fail(DFB_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (sr <= 0) return fail(DFB_ERR_UNSUPPORTED, "sample rate %d Hz", sr);
+    int64_t f10 = 0, f16 = 0;
+    int rc = check_taps(sr, kStoiFs, taps10, og10, nw10, width10, &f10);
+    if (!rc) rc = check_taps(sr, kSsnrFs, taps16, og16, nw16, width16, &f16);
+    if (rc) return rc;
+    if (f10 + f16 > (1 << 18))
+        return fail(DFB_ERR_UNSUPPORTED, "sample rate %d Hz: its resampler taps hold %lld floats, more than 2^18", sr,
+                    (long long)(f10 + f16));
+    rc = use_device(device);
+    if (rc) return rc;
+    auto *h = new dfb_metrics();
+    h->device = device;
+    h->sr = sr;
+    auto bail = [&](int code) { dfb_metrics_free(h); return code; };
+    std::vector<float2> tw;
+    gen_fft_plan(kStoiFft, h->plan, tw);
+    h->bands = stoi_bands();
+    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaMalloc(&h->d_tw, sizeof(float2) * tw.size()) != cudaSuccess ||
+        cudaMalloc(&h->d_dirs, sizeof(RateDir) * 2) != cudaSuccess ||
+        cudaMalloc(&h->d_taps, sizeof(float) * (size_t)(f10 + f16 + 1)) != cudaSuccess)
+        return bail(fail(DFB_ERR_OOM, "metrics handle allocation failed"));
+    if (f10) {
+        if (cudaMemcpy(h->d_taps, taps10, sizeof(float) * f10, cudaMemcpyHostToDevice) != cudaSuccess)
+            return bail(fail(DFB_ERR_CUDA, "tap upload failed"));
+        h->dirs[0] = RateDir{h->d_taps, og10, nw10, 2 * width10 + og10, width10};
+    }
+    if (f16) {
+        if (cudaMemcpy(h->d_taps + f10, taps16, sizeof(float) * f16, cudaMemcpyHostToDevice) != cudaSuccess)
+            return bail(fail(DFB_ERR_CUDA, "tap upload failed"));
+        h->dirs[1] = RateDir{h->d_taps + f10, og16, nw16, 2 * width16 + og16, width16};
+    }
+    float w256[kStoiFrame];
+    for (int n = 0; n < kStoiFrame; n++) w256[n] = (float)(0.5 - 0.5 * std::cos(2.0 * M_PI * (n + 1) / (kStoiFrame + 1)));
+    double wss[kSsnrWin];
+    for (int n = 0; n < kSsnrWin; n++) wss[n] = 0.5 * (1.0 - std::cos(2.0 * M_PI * (n + 1) / (kSsnrWin + 1)));
+    if (cudaMemcpy(h->d_tw, tw.data(), sizeof(float2) * tw.size(), cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaMemcpy(h->d_dirs, h->dirs, sizeof(RateDir) * 2, cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaMemcpyToSymbol(c_w256, w256, sizeof w256) != cudaSuccess || cudaMemcpyToSymbol(c_wss, wss, sizeof wss) != cudaSuccess)
+        return bail(fail(DFB_ERR_CUDA, "metrics table upload failed"));
+    h->plan.tw = h->d_tw;
+    *out = h;
+    return DFB_OK;
+}
+
+extern "C" void dfb_metrics_free(dfb_metrics *h) {
+    if (!h) return;
+    cudaSetDevice(h->device);
+    if (h->stream) cudaStreamSynchronize(h->stream);
+    h->arena.release();
+    cudaFree(h->d_taps);
+    cudaFree(h->d_dirs);
+    cudaFree(h->d_tw);
+    if (h->stream) cudaStreamDestroy(h->stream);
+    delete h;
+}
+
+extern "C" int64_t dfb_metrics_workspace_bytes(const dfb_metrics *h) { return h ? (int64_t)h->arena.cap : -1; }
+
+extern "C" int dfb_metrics_compute(dfb_metrics *h, const float *d_clean, const float *d_degraded, int64_t in_numel, const int64_t *offsets,
+                           const int64_t *clean_lengths, const int64_t *degraded_lengths, int64_t B, int metrics, float *d_out,
+                           void *stream) {
+    if (!h || !d_clean || !d_degraded || !d_out) return fail(DFB_ERR_INVALID, "null argument");
+    MetPlan p;
+    int rc = plan_call(h, in_numel, offsets, clean_lengths, degraded_lengths, B, metrics, p);
+    if (rc) return rc;
+    DFB_CUDA(cudaSetDevice(h->device));
+    return run_call(h, d_clean, d_degraded, p, B, metrics, d_out, (cudaStream_t)stream, nullptr, nullptr, in_numel, nullptr);
+}
+
+extern "C" int dfb_metrics_compute_host(dfb_metrics *h, const float *h_clean, const float *h_degraded, int64_t in_numel,
+                                const int64_t *offsets, const int64_t *clean_lengths, const int64_t *degraded_lengths, int64_t B,
+                                int metrics, float *h_out) {
+    if (!h || !h_clean || !h_degraded || !h_out) return fail(DFB_ERR_INVALID, "null argument");
+    MetPlan p;
+    int rc = plan_call(h, in_numel, offsets, clean_lengths, degraded_lengths, B, metrics, p);
+    if (rc) return rc;
+    DFB_CUDA(cudaSetDevice(h->device));
+    return run_call(h, nullptr, nullptr, p, B, metrics, nullptr, h->stream, h_clean, h_degraded, in_numel, h_out);
+}
+
+extern "C" int dfb_debug_metrics_counts(dfb_metrics *h, const float *h_clean, const float *h_degraded, int64_t in_numel,
+                                        const int64_t *offsets, const int64_t *lengths, int64_t B, int64_t *h_counts) {
+    if (!h || !h_counts) return fail(DFB_ERR_INVALID, "null argument");
+    std::vector<float> stoi((size_t)(B > 0 ? B : 1));
+    int rc = dfb_metrics_compute_host(h, h_clean, h_degraded, in_numel, offsets, lengths, lengths, B, DFB_METRIC_STOI, stoi.data());
+    if (rc) return rc;
+    std::vector<MetState> st(B);
+    DFB_CUDA(cudaMemcpy(st.data(), h->last_st, sizeof(MetState) * B, cudaMemcpyDeviceToHost));
+    for (int64_t b = 0; b < B; b++) {
+        h_counts[3 * b] = st[b].nk;
+        h_counts[3 * b + 1] = st[b].lc;
+        h_counts[3 * b + 2] = st[b].nf;
+    }
+    return DFB_OK;
+}

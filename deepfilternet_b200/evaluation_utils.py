@@ -1,0 +1,383 @@
+"""Speech-quality scoring on the device, after ``df.evaluation_utils`` (DeepFilterNet/df/evaluation_utils.py).
+
+Three metrics, each equal to the reference function applied to one entry alone (include/dfb200.h, DESIGN.md section 5j):
+
+* ``"sisdr"``: ``si_sdr_speechmetrics(clean, degraded)`` at the input rate.
+* ``"stoi"``: ``df.stoi.stoi(clean[None], degraded[None], sr)[0]`` (:func:`deepfilternet_b200.stoi.stoi`), NaN for an
+  entry with fewer than 512 samples left at 10 kHz after silence removal (the reference leaves garbage there).  This is
+  df/stoi.py's STOI, not pystoi's, which the reference's ``StoiMetric`` reports: pystoi removes silence and frames the
+  signal differently.  How far the two differ is not measured.
+* ``"ssnr"``: ``df.sepm.SNRseg(c16, d16, 16000)`` after ``io.resample(x, sr, 16000)``, the fifth value of the reference's
+  ``CompositeMetric``; NaN for an entry with no frame left.
+
+A batch is scored by one library call (``dfb_metrics_compute(_host)``): resampling, silence removal, STFT, band
+envelopes, segment correlations and every per-entry mean run on the GPU.  PESQ (and with it CSIG / CBAK / COVL) and
+DNSMOS are not provided.
+
+``python -m deepfilternet_b200.evaluation_utils DATASET_DIR -m MODEL`` scores a VoiceBank-DEMAND style test set as the
+reference's ``scripts/test_voicebank_demand.py`` does.
+"""
+from __future__ import annotations
+
+import csv
+import ctypes as C
+import logging
+import math
+import os
+from collections import defaultdict
+from typing import Callable, Dict, List, Optional, Sequence, Tuple
+
+import numpy as np
+import torch
+from torch import Tensor
+
+from . import _lib
+from ._lib import check
+
+logger = logging.getLogger("deepfilternet_b200")
+
+# metric name -> (bit of dfb_metrics_compute, name in results and CSV files); the output rows follow the bit order
+METRICS = {"sisdr": (1, "SISDR"), "stoi": (2, "STOI"), "ssnr": (4, "SSNR")}
+UNSUPPORTED = {
+    "composite": "needs PESQ (an external C package)",
+    "composite-octave": "needs PESQ and Octave",
+    "pesq": "needs PESQ (an external C package)",
+    "pesq-nb": "needs PESQ (an external C package)",
+    "dnsmos5": "needs DNSMOS's downloaded ONNX models",
+}
+MAX_TAP_FLOATS = 1 << 18
+MAX_ENTRIES = 32767
+SINC_FAST_WIDTH, SINC_FAST_ROLLOFF = 16, 0.99
+
+
+def metric_bits(metrics: Sequence[str]) -> int:
+    """The bit mask of ``metrics`` (names as :data:`METRICS`, any case).  ValueError for an empty list, a metric the library
+    does not provide (saying what it needs) or an unknown name."""
+    if isinstance(metrics, str):
+        metrics = [metrics]
+    bits = 0
+    for m in metrics:
+        k = str(m).lower()
+        if k in UNSUPPORTED:
+            raise ValueError(f"metric {m!r} {UNSUPPORTED[k]}, which deepfilternet_b200 does not provide; "
+                             f"available: {sorted(METRICS)}")
+        if k not in METRICS:
+            raise ValueError(f"unknown metric {m!r}; available: {sorted(METRICS)}")
+        bits |= METRICS[k][0]
+    if bits == 0:
+        raise ValueError("no metric requested")
+    return bits
+
+
+def bit_names(bits: int) -> List[str]:
+    """The metric names of the rows of a call with ``bits``, in row order."""
+    return [k for k, (b, _) in METRICS.items() if bits & b]
+
+
+def tap_floats(sr: int, to: int) -> int:
+    """Floats of io.resample_kernel(sr, to)'s sinc_fast table (0 when sr == to)."""
+    if sr == to:
+        return 0
+    g = math.gcd(sr, to)
+    og, nw = sr // g, to // g
+    width = math.ceil(SINC_FAST_WIDTH * og / (min(og, nw) * SINC_FAST_ROLLOFF))
+    return nw * (2 * width + og)
+
+
+def check_sr(sr) -> int:
+    """A metrics rate as int: ValueError for anything but a positive integer whose sr -> 10 kHz and sr -> 16 kHz tables
+    hold at most 2^18 floats together."""
+    if isinstance(sr, bool) or not isinstance(sr, (int, np.integer)) or int(sr) <= 0:
+        raise ValueError(f"sample rate {sr!r}: a positive integer number of Hz")
+    sr = int(sr)
+    n = tap_floats(sr, 10000) + tap_floats(sr, 16000)
+    if n > MAX_TAP_FLOATS:
+        raise ValueError(f"sample rate {sr} Hz is not supported for scoring: its resampler taps would hold {n} floats, more than 2^18")
+    return sr
+
+
+def check_pair_lengths(clean_lengths, degraded_lengths) -> np.ndarray:
+    """Entry lengths as contiguous int64: ValueError for an empty batch, more than 32767 entries, a length <= 0 or clean
+    and degraded lengths that differ."""
+    c = np.ascontiguousarray(np.asarray(clean_lengths, dtype=np.int64).reshape(-1))
+    d = np.asarray(degraded_lengths, dtype=np.int64).reshape(-1)
+    if c.size == 0:
+        raise ValueError("empty batch")
+    if c.size > MAX_ENTRIES:
+        raise ValueError(f"{c.size} entries: at most {MAX_ENTRIES} per call")
+    if d.size != c.size:
+        raise ValueError(f"{c.size} clean entries, {d.size} degraded")
+    bad = np.nonzero(c != d)[0]
+    if bad.size:
+        i = int(bad[0])
+        raise ValueError(f"entry {i}: clean has {int(c[i])} samples, degraded {int(d[i])}")
+    if (c <= 0).any():
+        raise ValueError(f"entry lengths must be > 0, got {int(c.min())}")
+    return c
+
+
+def packed_offsets(lengths: np.ndarray) -> Tuple[np.ndarray, int]:
+    """Entries back to back: (offsets, total samples)."""
+    off = np.concatenate(([0], np.cumsum(lengths)[:-1])).astype(np.int64)
+    return np.ascontiguousarray(off), int(lengths.sum())
+
+
+class _Metrics:
+    """A dfb_metrics handle: one device, one input rate."""
+
+    def __init__(self, device: int, sr: int):
+        from .io import get_resample_params, resample_kernel
+
+        self.sr = check_sr(sr)
+        self.device = int(device)
+        taps = []
+        for to in (10000, 16000):
+            if self.sr == to:
+                taps.append((None, 0, 0, 0))
+            else:
+                k, width, og, nw = resample_kernel(self.sr, to, **get_resample_params("sinc_fast"))
+                taps.append((k.contiguous(), og, nw, width))
+        self._keep = [t[0] for t in taps]
+        h = C.c_void_p()
+        (k10, og10, nw10, w10), (k16, og16, nw16, w16) = taps
+        check(_lib.lib().dfb_metrics_create(C.byref(h), self.device, self.sr,
+                                            k10.data_ptr() if k10 is not None else None, og10, nw10, w10,
+                                            k16.data_ptr() if k16 is not None else None, og16, nw16, w16))
+        self.handle = h
+
+    def __del__(self):
+        h = getattr(self, "handle", None)
+        if h is not None and h.value and _lib is not None:
+            try:
+                _lib.lib().dfb_metrics_free(h)
+            except Exception:  # interpreter shutdown
+                pass
+
+    def workspace_bytes(self) -> int:
+        return int(_lib.lib().dfb_metrics_workspace_bytes(self.handle))
+
+
+_HANDLES: Dict[Tuple[int, int], _Metrics] = {}
+
+
+def metrics_handle(sr: int, device: int = 0) -> _Metrics:
+    """The process's metrics handle for (device, sr), created on first use."""
+    key = (int(device), check_sr(sr))
+    if key not in _HANDLES:
+        _HANDLES[key] = _Metrics(*key)
+    return _HANDLES[key]
+
+
+def _rows_to_dict(out: Tensor, bits: int, metrics: Sequence[str]) -> Dict[str, Tensor]:
+    rows = {k: out[i] for i, k in enumerate(bit_names(bits))}
+    return {str(m).lower(): rows[str(m).lower()] for m in metrics}
+
+
+@torch.no_grad()
+def evaluate_batch(clean: Sequence[Tensor], degraded: Sequence[Tensor], sr: int,
+                   metrics: Sequence[str] = ("sisdr", "stoi", "ssnr"), device: int = 0) -> Dict[str, Tensor]:
+    """Scores entries of different lengths in one call: ``clean[i]`` and ``degraded[i]`` are 1-D CPU tensors of one length
+    at ``sr`` Hz.  Returns {metric: float32 CPU tensor [B]}, in the order of ``metrics``; entry i equals the reference
+    function on entry i alone.  The batch is packed into page-locked buffers and scored by one ``dfb_metrics_compute_host``
+    call, which copies only the entries' samples."""
+    bits = metric_bits(metrics)
+    cs, ds = list(clean), list(degraded)
+    for i, t in enumerate(cs + ds):
+        if not isinstance(t, Tensor) or t.dim() != 1:
+            raise ValueError(f"entry {i % max(len(cs), 1)}: audio must be a 1-D tensor")
+    lens = check_pair_lengths([t.numel() for t in cs], [t.numel() for t in ds])
+    off, n = packed_offsets(lens)
+    h = metrics_handle(sr, device)
+    pin = torch.cuda.is_available()
+    xc = torch.empty(n, dtype=torch.float32, pin_memory=pin)
+    xd = torch.empty(n, dtype=torch.float32, pin_memory=pin)
+    torch.cat([t.detach().to("cpu", torch.float32) for t in cs], out=xc)
+    torch.cat([t.detach().to("cpu", torch.float32) for t in ds], out=xd)
+    out = torch.empty((bin(bits).count("1"), lens.size), dtype=torch.float32)
+    check(_lib.lib().dfb_metrics_compute_host(h.handle, xc.data_ptr(), xd.data_ptr(), n, off.ctypes.data, lens.ctypes.data,
+                                              lens.ctypes.data, lens.size, bits, out.data_ptr()))
+    return _rows_to_dict(out, bits, metrics)
+
+
+@torch.no_grad()
+def evaluate_device_ragged(clean: Tensor, degraded: Tensor, lengths, sr: int,
+                           metrics: Sequence[str] = ("sisdr", "stoi", "ssnr")) -> Dict[str, Tensor]:
+    """Device-resident scoring: ``clean`` and ``degraded`` are padded float32 CUDA tensors [B, S] whose row b holds
+    ``lengths[b]`` samples at ``sr`` Hz.  Returns {metric: CUDA tensor [B]} (asynchronous on the current stream), entry b
+    equal to :func:`evaluate_batch` of the rows' first ``lengths[b]`` samples."""
+    for name, t in (("clean", clean), ("degraded", degraded)):
+        if not isinstance(t, Tensor) or not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous() or t.dim() != 2:
+            raise ValueError(f"evaluate_device_ragged expects {name} as a contiguous float32 CUDA tensor of shape [B, S]")
+    if clean.shape != degraded.shape or clean.device != degraded.device:
+        raise ValueError(f"clean {tuple(clean.shape)} on {clean.device} and degraded {tuple(degraded.shape)} on "
+                         f"{degraded.device} differ")
+    bits = metric_bits(metrics)
+    b, s = clean.shape
+    lens = lengths.detach().cpu().numpy() if isinstance(lengths, Tensor) else lengths
+    lens = np.asarray(lens).reshape(-1)
+    if lens.size != b:
+        raise ValueError(f"{lens.size} lengths for {b} rows")
+    lens = check_pair_lengths(lens, lens)
+    if (lens > s).any():
+        raise ValueError(f"entry length {int(lens.max())} exceeds the {s} samples per row")
+    off = np.ascontiguousarray(np.arange(b, dtype=np.int64) * s)
+    h = metrics_handle(sr, clean.device.index or 0)
+    out = torch.empty((bin(bits).count("1"), b), dtype=torch.float32, device=clean.device)
+    with torch.cuda.device(clean.device):
+        stream = torch.cuda.current_stream(clean.device).cuda_stream
+        check(_lib.lib().dfb_metrics_compute(h.handle, clean.data_ptr(), degraded.data_ptr(), b * s, off.ctypes.data,
+                                             lens.ctypes.data, lens.ctypes.data, b, bits, out.data_ptr(), stream))
+    return _rows_to_dict(out, bits, metrics)
+
+
+def si_sdr_speechmetrics(reference, estimate) -> float:
+    """evaluation_utils.si_sdr_speechmetrics of one pair of equal-length 1-D signals at any rate, on the device."""
+    r = torch.as_tensor(np.asarray(reference, dtype=np.float32).reshape(-1))
+    e = torch.as_tensor(np.asarray(estimate, dtype=np.float32).reshape(-1))
+    # SI-SDR does not resample, so any supported rate serves
+    return float(evaluate_batch([r], [e], 48000, ("sisdr",))["sisdr"][0])
+
+
+# ----------------------------------------------------------------------------------- evaluation loop ----
+def write_csv(path: str, flat_metrics: Dict[str, Dict[str, float]]):
+    """evaluation_utils.write_csv: ``filename,metric_a,metric_b,...`` then one row per file."""
+    metric_names = list(iter(flat_metrics.values()).__next__().keys())
+    with open(path, mode="w", newline="") as csvfile:
+        w = csv.writer(csvfile, delimiter=",", quoting=csv.QUOTE_MINIMAL)
+        w.writerow(["filename"] + metric_names)
+        for fn, m in flat_metrics.items():
+            w.writerow([fn] + [str(m[n]) for n in metric_names])
+
+
+@torch.no_grad()
+def evaluation_loop(df_state, model, clean_files: List[str], noisy_files: List[str],
+                    metrics: List[str] = ["stoi", "sisdr", "ssnr"],  # noqa: B006 (the reference's signature)
+                    save_audio_callback: Optional[Callable[[str, Tensor], None]] = None, batch_size: int = 32,
+                    log_percent: int = 25, csv_path_enh: Optional[str] = None, csv_path_noisy: Optional[str] = None,
+                    noisy_metric: bool = False) -> Dict[str, float]:
+    """evaluation_utils.evaluation_loop: enhance each noisy file and score it against its clean file.
+
+    Per file, as the reference: ``enh = enhance(model, df_state, noisy, pad=False)[0]`` and
+    ``clean = df_state.synthesis(df_state.analysis(clean))[0]`` (the same for noisy with ``noisy_metric``), files loaded
+    at the model's rate with sinc_fast resampling.  ``batch_size`` files are enhanced by one :func:`enhance_batch` call and
+    scored by one metrics call (noisy entries included).  Returns the reference's means, ``"Noisy    STOI"`` (with
+    ``noisy_metric``) and ``"Enhanced STOI"`` for each metric in ``metrics`` order; ``csv_path_enh`` / ``csv_path_noisy``
+    get the reference's per-file CSV layout.  Metrics other than "stoi", "sisdr" and "ssnr" raise ValueError."""
+    from .enhance import enhance_batch
+    from .io import load_audio
+
+    names = [str(m).lower() for m in metrics]
+    metric_bits(names)
+    if len(clean_files) != len(noisy_files):
+        raise ValueError(f"{len(clean_files)} clean files, {len(noisy_files)} noisy")
+    sr = df_state.sr()
+    check_sr(sr)
+    enh_vals: Dict[str, List[Tuple[str, float]]] = {m: [] for m in names}
+    noisy_vals: Dict[str, List[Tuple[str, float]]] = {m: [] for m in names}
+    pairs = list(zip(noisy_files, clean_files))
+    batch_size = max(1, int(batch_size))
+    batches = [pairs[i:i + batch_size] for i in range(0, len(pairs), batch_size)]
+    done = 0
+    for batch in batches:
+        noisy = [load_audio(nf, sr, method="sinc_fast")[0] for nf, _ in batch]
+        clean = [load_audio(cf, sr, method="sinc_fast")[0] for _, cf in batch]
+        enh = [e[0] for e in enhance_batch(model, df_state, noisy, pad=False)]
+        clean = [torch.from_numpy(df_state.synthesis(df_state.analysis(c.numpy()))[0]) for c in clean]
+        for (nf, _), c, e in zip(batch, clean, enh):
+            if c.shape != e.shape:
+                raise RuntimeError(f"{c.shape}, {e.shape}, {os.path.basename(nf)}")
+        degraded = list(enh)
+        refs = list(clean)
+        if noisy_metric:
+            degraded += [torch.from_numpy(df_state.synthesis(df_state.analysis(n.numpy()))[0]) for n in noisy]
+            refs += clean
+        scores = evaluate_batch(refs, degraded, sr, names, device=model.cuda_device.index or 0)
+        for j, (nf, cf) in enumerate(batch):
+            fn = os.path.basename(nf)
+            for m in names:
+                enh_vals[m].append((fn, float(scores[m][j])))
+                if noisy_metric:
+                    noisy_vals[m].append((fn, float(scores[m][len(batch) + j])))
+            if save_audio_callback is not None:
+                save_audio_callback(cf, enh[j].to(torch.float32).view(1, -1))
+        prev, done = done, done + len(batch)
+        if 0 < log_percent < 100:   # evaluation_utils.log_progress's messages
+            for p in range(int(100 * prev / len(pairs)) + 1, int(100 * done / len(pairs)) + 1):
+                if p % log_percent == 0:
+                    logger.info("Progress: %2d%%", p)
+    label = {m: METRICS[m][1] for m in names}
+
+    def flat(vals) -> Dict[str, Dict[str, float]]:
+        out: Dict[str, Dict[str, float]] = defaultdict(dict)
+        for m in names:
+            for fn, v in vals[m]:
+                out[fn][label[m]] = v
+        return out
+
+    if csv_path_enh is not None:
+        write_csv(csv_path_enh, flat(enh_vals))
+    if csv_path_noisy is not None and noisy_metric:
+        write_csv(csv_path_noisy, flat(noisy_vals))
+    out_dict: Dict[str, float] = {}
+    for m in names:
+        if noisy_metric:
+            out_dict[f"Noisy    {label[m]}"] = float(np.mean([v for _, v in noisy_vals[m]]))
+        out_dict[f"Enhanced {label[m]}"] = float(np.mean([v for _, v in enh_vals[m]]))
+    return out_dict
+
+
+# ---------------------------------------------------------------------------------------------- CLI ----
+def cli_parser():
+    """scripts/test_voicebank_demand.py's arguments, without --metric-workers and --sleep-ms (no worker pool here)."""
+    from .enhance import setup_df_argument_parser
+
+    parser = setup_df_argument_parser()
+    parser.add_argument("dataset_dir", type=str,
+                        help="Voicebank Demand Test set directory. Must contain 'noisy_testset_wav' and 'clean_testset_wav'.")
+    parser.add_argument("--csv-path-enh", type=str, default=None, help="Path to csv score file containing metrics of enhanced audios.")
+    parser.add_argument("--csv-path-noisy", type=str, default=None, help="Path to csv score file containing metrics of noisy audios.")
+    parser.add_argument("--compute-noisy-metric", action="store_true")
+    parser.add_argument("--batch-size", type=int, default=32, help="Files enhanced and scored per call.")
+    parser.add_argument("--metrics", type=str, nargs="+", default=["stoi", "sisdr", "ssnr"],
+                        help=f"Metrics to compute, of {sorted(METRICS)}.")
+    return parser
+
+
+def main(args) -> Dict[str, float]:
+    """scripts/test_voicebank_demand.py main: score the test set, log every mean and print them comma-separated (without
+    SSNR, as the reference prints)."""
+    import glob
+
+    from .enhance import init_df
+    from .io import save_audio
+
+    metric_bits(args.metrics)
+    model, df_state, suffix, _ = init_df(args.model_base_dir, post_filter=args.pf, log_level=args.log_level,
+                                         config_allow_defaults=True, epoch=args.epoch)
+    if not os.path.isdir(args.dataset_dir):
+        raise FileNotFoundError(f"{args.dataset_dir} is not a directory")
+    sr = df_state.sr()
+    noisy_dir = os.path.join(args.dataset_dir, "noisy_testset_wav")
+    clean_dir = os.path.join(args.dataset_dir, "clean_testset_wav")
+    if not (os.path.isdir(noisy_dir) and os.path.isdir(clean_dir)):
+        raise FileNotFoundError(f"{args.dataset_dir} must contain 'noisy_testset_wav' and 'clean_testset_wav'")
+    clean_files = sorted(glob.glob(clean_dir + "/*.wav"))
+    noisy_files = sorted(glob.glob(noisy_dir + "/*.wav"))
+    if args.output_dir is not None:
+        os.makedirs(args.output_dir, exist_ok=True)
+
+    def save_audio_callback(cleanfn: str, enh: Tensor):
+        save_audio(os.path.basename(cleanfn), enh, sr, output_dir=args.output_dir, suffix=suffix)
+
+    metrics = evaluation_loop(df_state, model, clean_files, noisy_files, metrics=args.metrics,
+                              save_audio_callback=save_audio_callback if args.output_dir is not None else None,
+                              batch_size=args.batch_size, csv_path_enh=args.csv_path_enh, csv_path_noisy=args.csv_path_noisy,
+                              noisy_metric=args.compute_noisy_metric)
+    for k, v in metrics.items():
+        logger.info("%s: %s", k, v)
+    print("".join(f"{m}," for k, m in metrics.items() if "SSNR" not in k)[:-1])
+    return metrics
+
+
+if __name__ == "__main__":
+    main(cli_parser().parse_args())

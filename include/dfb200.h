@@ -573,6 +573,42 @@ int64_t dfb_model_debug_fetch(dfb_model *m, const char *name, float *h_out, int6
 /* bytes of device workspace the model handle currently owns (grow-only arena) */
 int64_t dfb_model_workspace_bytes(const dfb_model *m);
 
+/* ------------------------------------------------------------------ metrics -------------------
+ * Speech-quality metrics of a ragged batch on the device (DESIGN.md section 5j), each equal to the reference function
+ * applied to one entry alone:
+ *   DFB_METRIC_SISDR  DeepFilterNet/df/evaluation_utils.py si_sdr_speechmetrics(clean, degraded) at the input rate
+ *                     (fp64 sums, float32 eps);
+ *   DFB_METRIC_STOI   df/stoi.py stoi(clean[None], degraded[None], sr)[0]: io.resample to 10 kHz (sinc_fast), silent
+ *                     frames removed, 15 third-octave bands, 30-frame segments; NaN when fewer than 512 samples remain;
+ *   DFB_METRIC_SSNR   df/sepm.py SNRseg(c16, d16, 16000) after io.resample to 16 kHz (sinc_fast); NaN when no frame is left.
+ * This STOI is df/stoi.py's, not pystoi's, which removes silence and frames differently. */
+enum { DFB_METRIC_SISDR = 1, DFB_METRIC_STOI = 2, DFB_METRIC_SSNR = 4 };
+typedef struct dfb_metrics dfb_metrics;
+/* A metrics handle on `device` for inputs at `sr` Hz: taps10 / taps16 [nw][2 width + og] (HOST arrays) are
+ * io.resample_kernel(sr, 10000) / (sr, 16000) with the sinc_fast parameters, og / nw the gcd-reduced rates (DFB_ERR_INVALID
+ * otherwise); NULL when sr is that rate.  DFB_ERR_UNSUPPORTED when the two tables hold more than 2^18 floats together (as
+ * dfb_model_add_rate).  The handle owns the tables, a stream and a workspace that grows when a call needs more. */
+int dfb_metrics_create(dfb_metrics **out, int device, int sr, const float *taps10, int og10, int nw10, int width10,
+                       const float *taps16, int og16, int nw16, int width16);
+void dfb_metrics_free(dfb_metrics *h);
+/* One call scores B <= 32767 entries: entry b is clean_lengths[b] samples of clean at d_clean + offsets[b] and as many of
+ * degraded at d_degraded + offsets[b] (offsets / lengths HOST arrays, in_numel bounding both buffers).  d_out [n][B] fp32
+ * gets one row per bit of `metrics`, in the order SI-SDR, STOI, SSNR.  DFB_ERR_INVALID for a length <= 0, different clean
+ * and degraded lengths, an entry outside in_numel, no metric or an unknown metric bit.  Asynchronous on `stream`; the
+ * handle's workspace serves one call at a time. */
+int dfb_metrics_compute(dfb_metrics *h, const float *d_clean, const float *d_degraded, int64_t in_numel, const int64_t *offsets,
+                        const int64_t *clean_lengths, const int64_t *degraded_lengths, int64_t B, int metrics, float *d_out,
+                        void *stream);
+int dfb_metrics_compute_host(dfb_metrics *h, const float *h_clean, const float *h_degraded, int64_t in_numel,
+                             const int64_t *offsets, const int64_t *clean_lengths, const int64_t *degraded_lengths, int64_t B,
+                             int metrics, float *h_out);
+/* bytes of device workspace the metrics handle owns */
+int64_t dfb_metrics_workspace_bytes(const dfb_metrics *h);
+/* Debug aid: the STOI of a dfb_metrics_host call, then h_counts [B][3] = each entry's kept frames, its length after silence
+ * removal and its STFT frames (0 when that length is below 512). */
+int dfb_debug_metrics_counts(dfb_metrics *h, const float *h_clean, const float *h_degraded, int64_t in_numel,
+                             const int64_t *offsets, const int64_t *lengths, int64_t B, int64_t *h_counts);
+
 #ifdef __cplusplus
 }
 #endif
