@@ -92,6 +92,11 @@ SIGNATURES = {
     "dfb_enhance_ragged_rates": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I, _VP, _VP]),
     "dfb_enhance_ragged_rates_host": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I, _VP]),
     "dfb_enhance_out_len_at": (_I64, [_VP, _I64, _I, _I]),
+    "dfb_enhance_ragged_ex": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I, _VP, _VP, _I64, _VP,
+                                   _I64, _VP, _VP]),
+    "dfb_enhance_ragged_ex_host": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I, _VP, _VP, _I64,
+                                        _VP, _I64, _VP]),
+    "dfb_enhance_lsnr_len": (_I64, [_VP, _I64, _I, _I]),
     "dfb_debug_resample_rows": (_I, [_I, _VP, _VP, _VP, _VP, _VP, _I64, _VP, _VP, _VP, _I64, _VP]),
     "dfb_model_workspace_bytes": (_I64, [_VP]),
     "dfb_stream_create": (_I, [C.POINTER(_VP), _VP, _VP, _I64, _F]),
@@ -100,6 +105,7 @@ SIGNATURES = {
     "dfb_stream_frame_length": (_I64, [_VP]),
     "dfb_stream_latency_frames": (_I64, [_VP]),
     "dfb_stream_set_lsnr_thresholds": (_I, [_VP, _I, _F, _F, _F]),
+    "dfb_stream_set_lsnr_thresholds_slots": (_I, [_VP, _I64P, _I64, _I, _F, _F, _F]),
     "dfb_stream_set_mask_reduce": (_I, [_VP, _I, _I]),
     "dfb_stream_process": (_I, [_VP, _VP, _I64, _VP, _VP]),
     "dfb_stream_flush": (_I, [_VP, _VP, _VP]),

@@ -200,8 +200,10 @@ __host__ __device__ __forceinline__ void rate_range(bool up, const RateDir &d, c
 
 // Per-slot settings of a streaming handle (dfb_stream_set_atten_lim / _post_filter_beta): limit (0 = off) and post-filter
 // beta (0 = off) from absolute frame sw on, and the previous ones before it.  Only the frame before sw, re-synthesised
-// for its overlap-add tail, still reads the previous ones.
-struct SlotCtl { float lim, beta, lim0, beta0; int64_t sw; };
+// for its overlap-add tail, still reads the previous ones.  gate != 0: LSNR stage gating with the thresholds th_min /
+// th_erb / th_df (tract.rs:658-672), which apply to every frame of the row; it takes effect only in launches that run the
+// LSNR head (ApplyParams::lsnr).  Batch rows (dfb_enhance_ragged_ex) have sw = 0: one setting for the whole stream.
+struct SlotCtl { float lim, beta, lim0, beta0; int64_t sw; float th_min, th_erb, th_df; int gate; };
 
 // Streaming slots (dfb_stream_open_slots): `first` holds the absolute first frame of each stream of a launch, or is null.
 // Window frame t (absolute w0 + t) of stream b exists from the returned window frame on; the kernels that look back in

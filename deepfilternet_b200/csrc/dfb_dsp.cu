@@ -804,8 +804,9 @@ __global__ void __launch_bounds__(32 * kSynWarps) k_apply_synthesis_generic(Appl
 // LINK: linked channels (p.links, with RG), likewise separate.  The mask of a frame is reduced over the link group where it is
 // loaded: lane e reads row e of each member's mask and reduces in registers, so the shared mask never reaches HBM and
 // the unlinked instantiations are untouched.
-// CTL: per-stream attenuation limit and post-filter beta (p.ctl, streaming slots), likewise separate.  Each frame picks
-// the row's new or previous setting by its absolute frame against the row's switch frame.
+// CTL: per-stream attenuation limit, post-filter beta and LSNR gating thresholds (ctl_tab: streaming slots, and batches
+// with a settings table), likewise separate.  Each frame picks the row's new or previous limit and beta by its absolute
+// frame against the row's switch frame; with the LSNR head on (p.lsnr), a row gates when its entry says so.
 template <int ORDER, int NDFJ, int MINB, bool RG, bool LINK = false, bool CTL = false>
 __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyParams p, DspTables tb, const SlotCtl *ctl_tab) {
     __shared__ __align__(16) float s_win[kFft];
@@ -904,9 +905,10 @@ __global__ void __launch_bounds__(32 * kSynWarps, MINB) k_apply_synthesis(ApplyP
         if (pf2) mcur = pf_gain_mask(mcur, 0.02f);
         const float al = blend ? p.alpha[(int64_t)b * mcT + t] : 1.f;
         int stage = 3;   // 0 zero gains, 1 unprocessed, 2 gains only, 3 gains + deep filter (tract.rs apply_stages)
-        if (p.lsnr) {
+        if (p.lsnr && (!CTL || ctl.gate)) {   // CTL: the row's own thresholds
             const float l = p.lsnr[(int64_t)lb * mcT + t];
-            stage = l < p.th_min ? 0 : (l > p.th_erb ? 1 : (l > p.th_df ? 2 : 3));
+            const float th_min = CTL ? ctl.th_min : p.th_min, th_erb = CTL ? ctl.th_erb : p.th_erb, th_df = CTL ? ctl.th_df : p.th_df;
+            stage = l < th_min ? 0 : (l > th_erb ? 1 : (l > th_df ? 2 : 3));
         }
         if (RG && t < t_zero) stage = 0;   // zero gains, no deep filter: the stream has not started
         // CTL: the setting frame t was output with; the frame before the switch is only re-synthesised for its tail

@@ -1586,6 +1586,13 @@ extern "C" int64_t dfb_enhance_out_len_at(const dfb_state *st, int64_t T, int pa
     return len_from_48k(dfb_enhance_out_len(st, len_at_48k(T, rate), pad), rate);
 }
 
+// LSNR values of a stream in dfb_enhance_ragged_ex: one per 10 ms hop of its 48 kHz output, ceil(out48 / hop)
+extern "C" int64_t dfb_enhance_lsnr_len(const dfb_state *st, int64_t T, int pad, int rate) {
+    if (!st || T <= 0 || rate <= 0) return -1;
+    const int64_t o48 = dfb_enhance_out_len(st, rate == kModelRate ? T : len_at_48k(T, rate), pad);
+    return (o48 + st->hop - 1) / st->hop;
+}
+
 // The taps of rated batches at `rate` (DESIGN.md section 5i): both directions of io.resample_kernel's sinc_fast taps,
 // at most kMaxRateTaps floats together.  48000 registers nothing (a 48 kHz stream is never resampled).
 constexpr int64_t kMaxRateTaps = int64_t(1) << 18;
@@ -1761,8 +1768,14 @@ struct ChunkIO {
     // streaming slots (dfb_stream_open_slots): rows are the handle's active slots, rows[b].Tf the end of a closing one, and
     // first[b] the absolute first frame of each; emission follows the handle's clock, clipped at each stream's end.  Or null.
     const int64_t *first = nullptr;
-    // streaming slots: per-row attenuation limit and post-filter beta (launch_apply_synthesis), or null
+    // per-row attenuation limit, post-filter beta and gating thresholds (launch_apply_synthesis; streaming slots and
+    // batches with a settings table), or null.  ctl_gate: some row gates, so the LSNR head runs.
     const SlotCtl *ctl = nullptr;
+    bool ctl_gate = false;
+    // ragged batch LSNR rows (dfb_enhance_ragged_ex), or null: row b's value j, at lsnr_rows + lsnr_offs[b] (device table),
+    // is the LSNR of the frame output hop j carries, frame j + out_sample0 / hop (k_lsnr_rows)
+    float *lsnr_rows = nullptr;
+    const int64_t *lsnr_offs = nullptr;
     // streaming LSNR output: lsnr_from >= 0 runs the LSNR head (as gating does) and carries its tail; lsnr_out (or null)
     // [rows][out_len / hop] receives the LSNR of every frame the apply kernel emits whose DNN step ran from lsnr_from on,
     // at the hop that carries it.  Entries of hops that carry no frame are left as they are.
@@ -1932,6 +1945,20 @@ __global__ void k_lsnr_out(const float *__restrict__ ll, int mcT, float *__restr
     if (t >= t0 && t < te) out[o + j] = ll[(int64_t)b * mcT + t];
 }
 
+// LSNR rows of a ragged batch: every window frame t that the apply kernel emitted for row b in this chunk (t_first <= t
+// < te, te the stream's own end when it ends in this window, else t_emit) goes to value (w0 + t) - f0 of the row, the
+// output hop that carries it, when that hop exists: ceil(out_len / hop) values per row.
+__global__ void k_lsnr_rows(const float *__restrict__ ll, int mcT, float *__restrict__ out, const int64_t *__restrict__ offs,
+                            int64_t f0, int64_t w0, int t_first, int t_emit, const RaggedRow *__restrict__ rows, int hop) {
+    const int b = blockIdx.y;
+    const int t = t_first + blockIdx.x * blockDim.x + threadIdx.x;
+    const RaggedRow r = rows[b];
+    const int64_t tfb = r.Tf - w0;
+    const int64_t te = tfb <= mcT ? tfb : t_emit;
+    const int64_t j = w0 + t - f0, n = (r.out_len + hop - 1) / hop;
+    if (t < te && j >= 0 && j < n) out[offs[b] + j] = ll[(int64_t)b * mcT + t];
+}
+
 // One chunk: analyse frames [S.a1, a1n), run the DNN over [S.d1, d1n), emit audio of frames [S.e1, e1n).
 // Only the first io.nb streams run; a stream whose frame count Tf_b is <= d1n ends in this chunk: its features and
 // spectrum beyond Tf_b do not exist and it emits all of its frames up to Tf_b.
@@ -1962,7 +1989,8 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     float *fs = arena.take<float>((size_t)B * Tsb * Fd * 2);
     float *mm = arena.take<float>((size_t)B * (Tw + 1) * E);
     float *cc = arena.take<float>((size_t)B * (Tw + 1) * Fd * O2);
-    float *ll = (io.lsnr_th || io.lsnr_from >= 0 || io.spec_out) ? arena.take<float>((size_t)B * (Tw + 1)) : nullptr;
+    float *ll = (io.lsnr_th || io.ctl_gate || io.lsnr_rows || io.lsnr_from >= 0 || io.spec_out) ? arena.take<float>((size_t)B * (Tw + 1))
+                                                                                                   : nullptr;
     float *aa = c.model_kind == 1 ? arena.take<float>((size_t)B * (Tw + 1)) : nullptr;   // df_alpha (v1)
     if (!cc || (c.model_kind == 1 && !aa)) return fail(DFB_ERR_OOM, "chunk workspace exhausted");
     // ---- features: carried history, then the new frames (a spectral handle keeps no spectrum: nothing is applied)
@@ -2030,6 +2058,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
         p.alpha = aa;
         apply_options(m, p);
         if (io.lsnr_th) { p.lsnr = ll; p.th_min = io.lsnr_th[0]; p.th_erb = io.lsnr_th[1]; p.th_df = io.lsnr_th[2]; }
+        if (io.ctl_gate) p.lsnr = ll;   // each row's thresholds from io.ctl
         p.rows = io.rows; p.w0 = W0; p.t_emit = p.Tf; p.first = io.first;
         if (!io.first) p.Tf = Tw;   // batch: the grid covers every stream's end; slots: Te = min(end, clock)
         if (io.links) { p.links = io.links; p.reduce = io.reduce; }
@@ -2039,6 +2068,11 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
             dim3 grid((unsigned)((n_out + 127) / 128), (unsigned)B);
             k_lsnr_out<<<grid, 128, 0, s>>>(ll, Tw, io.lsnr_out, n_out, io.out_sample0 / hop, W0, p.t_first, (int)(e1n - W0), io.rows,
                                             io.first, io.lsnr_from, hop);
+            DFB_LAUNCH_CHECK();
+        }
+        if (io.lsnr_rows && Tw > p.t_first) {
+            dim3 grid((unsigned)((Tw - p.t_first + 127) / 128), (unsigned)B);
+            k_lsnr_rows<<<grid, 128, 0, s>>>(ll, Tw, io.lsnr_rows, io.lsnr_offs, io.out_sample0 / hop, W0, p.t_first, p.t_emit, io.rows, hop);
             DFB_LAUNCH_CHECK();
         }
     }
@@ -2089,11 +2123,20 @@ struct ChunkHooks {
     std::function<int(int64_t y0, int64_t y1, int64_t d1, int64_t na, cudaStream_t cs)> after;
 };
 
+// Per-row settings and LSNR rows of one stream group (dfb_enhance_ragged_ex), as device tables in the group's order, or
+// nulls: ctl the settings (sw = 0), gate whether any row gates, lsnr / lsnr_offs the LSNR rows (ChunkIO::lsnr_rows).
+struct BatchOut {
+    const SlotCtl *ctl = nullptr;
+    bool gate = false;
+    float *lsnr = nullptr;
+    const int64_t *lsnr_offs = nullptr;
+};
+
 // Runs the chunk loop over one stream group: `rows` is its device table and `tfs` its streams' frame counts on the host,
 // longest first.  The analysis reads stream b from d_x + rows[b].in_off, apply + synthesis writes it to d_out + rows[b].out_off.
 static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, float *d_out, const RaggedRow *rows, const int64_t *tfs,
                          int64_t nb, int pad, float lim, int tc, bool pipelined, cudaStream_t s, const ChunkHooks *hooks,
-                         const LinkRow *links, int reduce) {
+                         const LinkRow *links, int reduce, const BatchOut &bo) {
     const dfb_model_config &c = m->cfg;
     const ChunkGeom g = chunk_geom(c);
     const int hop = st->hop, fft = st->fft;
@@ -2135,6 +2178,8 @@ static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, float *d
         if (hooks && S.a1 < a1n && (rc = hooks->before(S.a1 * hop, a1n * hop, na, cs))) break;
         const int64_t e0 = S.e1;
         ChunkIO io{d_x, Tf * hop, 0, nullptr, d_out, 0, 0, delay, lim, nullptr, rows, (int)na, links, reduce};
+        io.ctl = bo.ctl; io.ctl_gate = bo.gate;
+        io.lsnr_rows = bo.lsnr; io.lsnr_offs = bo.lsnr_offs;
         if ((rc = run_chunk(m, st, S, io, a1n, d1n, e1n > S.e1 ? e1n : S.e1, cs, lane, pipelined))) break;
         if (hooks && (rc = hooks->after(e0 * hop > delay ? e0 * hop - delay : 0, S.e1 * hop - delay, d1n, na, cs))) break;
         // what the hook enqueued on the lane is part of the chunk: the caller's stream and the next chunk's decoder wait for it
@@ -2302,12 +2347,17 @@ static int link_plan(const dfb_model *m, const std::vector<RaggedRow> &rows, con
 // chunk c + 1 and the D2H copy of chunk c - 1 run on their own streams (both copy engines) while chunk c computes, and the
 // call is synchronous.
 // `links` (or null): each stream's link group from link_plan, sorted here along with `rows`; `reduce` the mask reduction.
+// `ctl` (or null): each stream's settings (sw = 0), sorted likewise; they replace atten_lim_db and the model's DeepFilterNet3
+// post filter, and `gate` says whether any of them gates.  `lsnr` (or null): each stream's LSNR row goes to
+// lsnr + lsnr_offsets[b] (caller's buffer, host or device as `host` says; k_lsnr_rows).
 static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &rows, std::vector<RateRow> &rates, const float *src,
                         float *dst, int pad, float atten_lim_db, bool host, cudaStream_t s, std::vector<LinkRow> *links = nullptr,
-                        int reduce = 0) {
+                        int reduce = 0, std::vector<SlotCtl> *ctl = nullptr, bool gate = false, float *lsnr = nullptr,
+                        const int64_t *lsnr_offsets = nullptr) {
     const int64_t B = (int64_t)rows.size();
     const bool rated = std::any_of(rates.begin(), rates.end(), [](const RateRow &q) { return q.dir >= 0; });
     int64_t min_group = 1;   // the largest link group: a stream group never splits one
+    std::vector<int64_t> lsnr_off;   // the streams' LSNR offsets in the caller's buffer, sorted
     {
         // The members of a link group are consecutive and share their sort key (one length), so the stable sort keeps them
         // one contiguous run in their own order: nothing between them has that key.  Sorting a permutation carries each
@@ -2318,10 +2368,14 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
         std::vector<RaggedRow> sr((size_t)B);
         std::vector<LinkRow> sl(links ? (size_t)B : 0);
         std::vector<RateRow> sq((size_t)B);
+        std::vector<SlotCtl> sc(ctl ? (size_t)B : 0);
+        std::vector<int64_t> so(lsnr ? (size_t)B : 0);
         for (int64_t i = 0; i < B; i++) {
             const int64_t o = idx[(size_t)i];
             sr[(size_t)i] = rows[(size_t)o];
             sq[(size_t)i] = rates[(size_t)o];
+            if (ctl) sc[(size_t)i] = (*ctl)[(size_t)o];
+            if (lsnr) so[(size_t)i] = lsnr_offsets[o];
             if (links) {
                 const LinkRow g = (*links)[(size_t)o];
                 sl[(size_t)i] = LinkRow{(int)(i - (o - g.first)), g.n};
@@ -2331,6 +2385,8 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
         rows.swap(sr);
         if (links) links->swap(sl);
         rates.swap(sq);
+        if (ctl) ctl->swap(sc);
+        lsnr_off.swap(so);
     }
     std::vector<int64_t> tfs((size_t)B);
     int64_t true_frames = 0;
@@ -2352,7 +2408,8 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
     if (rc) return rc;
     size_t off[16];   // the aux arena holds one group's state slab and tables
     if ((rc = m->aux_arena.reserve(state_floats(m->cfg, st, (int)group, off) * sizeof(float) +
-                                   (size_t)group * (sizeof(RaggedRow) + sizeof(LinkRow) + (rated ? 2 * sizeof(RateRow) : 0)) + 8192)))
+                                   (size_t)group * (sizeof(RaggedRow) + sizeof(LinkRow) + (rated ? 2 * sizeof(RateRow) : 0) +
+                                                    sizeof(SlotCtl) + sizeof(int64_t)) + 8192)))
         return rc;
     // stream groups: up to `group` streams, cut only between link groups (group >= every link group, so a cut inside one
     // moves back to its first member, past b0); DeepFilterNet v1: of one frame count
@@ -2378,8 +2435,20 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
     const bool staged = host || rated;
     std::vector<RaggedRow> drows(rows);
     std::vector<RateRow> ur(rates), dr_(rates);
-    float *d_in = nullptr, *d_out = nullptr, *d_rin = nullptr, *d_rout = nullptr;
+    // LSNR rows: written to the caller's device buffer, or (host) staged per stream group, packed, at dlo
+    const int hop = st->hop;
+    auto lsnr_n = [&](int64_t i) { return (rows[(size_t)i].out_len + hop - 1) / hop; };
+    std::vector<int64_t> dlo(lsnr_off);
+    float *d_in = nullptr, *d_out = nullptr, *d_rin = nullptr, *d_rout = nullptr, *d_lsnr = nullptr;
     int smem_up = 0, smem_down = 0;
+    int64_t n_lsnr = 0;
+    if (lsnr && host)
+        for (int64_t b0 = 0, b1; b0 < B; b0 = b1) {
+            b1 = group_end(b0);
+            int64_t gl = 0;
+            for (int64_t i = b0; i < b1; i++) { dlo[(size_t)i] = gl; gl += lsnr_n(i); }
+            n_lsnr = std::max(n_lsnr, gl);
+        }
     if (staged) {
         int64_t n_in = 0, n_out = 0, n_rin = 0, n_rout = 0;
         for (int64_t b0 = 0, b1; b0 < B; b0 = b1) {
@@ -2403,12 +2472,14 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
             n_in = std::max(n_in, gi); n_out = std::max(n_out, go);
             n_rin = std::max(n_rin, gri); n_rout = std::max(n_rout, gro);
         }
-        if ((rc = st->arena.reserve(sizeof(float) * (size_t)(n_in + n_out + n_rin + n_rout) + 4096))) return rc;
+        if ((rc = st->arena.reserve(sizeof(float) * (size_t)(n_in + n_out + n_rin + n_rout + n_lsnr) + 5120))) return rc;
         st->arena.reset();
         d_in = st->arena.take<float>((size_t)n_in); d_out = st->arena.take<float>((size_t)n_out);
         if (n_rin) d_rin = st->arena.take<float>((size_t)n_rin);
         if (n_rout) d_rout = st->arena.take<float>((size_t)n_rout);
+        if (n_lsnr) d_lsnr = st->arena.take<float>((size_t)n_lsnr);
     }
+    if (lsnr && !host) d_lsnr = lsnr;
     // the most outputs a row of rr[0, na) writes in a resampler launch
     auto max_range = [&](bool up, const RateRow *rr, int64_t na, const RateIO &io) {
         int64_t mx = 0, o0, o1;
@@ -2472,11 +2543,18 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
                                   dh[i].dir >= 0 ? y0 : tf[i] <= d1 ? hr[i].out_len : std::min(y1, hr[i].out_len)};
             }, host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, host ? sd : cs);
             if (r || !host) return r;
-            return copy_streams(dst, d_rout, 0, na, [&](int64_t i) {
+            r = copy_streams(dst, d_rout, 0, na, [&](int64_t i) {
                 if (dh[i].dir < 0) return StreamCopy{0, 0, 0};
                 int64_t a, b;
                 rate_range(false, m->rate_down[(size_t)dh[i].dir], dh[i], io, &a, &b);
                 return StreamCopy{rh[i].out_off + a, dh[i].out_off + a, b - a};
+            }, cudaMemcpyDeviceToHost, sd);
+            if (r || !lsnr) return r;
+            // LSNR values [y0 / hop, y1 / hop) carry the frames emitted in this chunk (y = e hop - delay), all of them once
+            // the stream has ended
+            return copy_streams(lsnr, d_lsnr, y0 / hop, na, [&](int64_t i) {
+                const int64_t n = lsnr_n(b0 + i);
+                return StreamCopy{lsnr_off[(size_t)(b0 + i)], dlo[(size_t)(b0 + i)], tf[i] <= d1 ? n : std::min(y1 / hop, n)};
             }, cudaMemcpyDeviceToHost, sd);
         };
         // (host) the previous group's D2H copies read the staged output and its compute the staged input: order this
@@ -2499,8 +2577,23 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
             DFB_CUDA(cudaMemcpyAsync(d_ur, uh, sizeof(RateRow) * (b1 - b0), cudaMemcpyHostToDevice, sc));
             DFB_CUDA(cudaMemcpyAsync(d_dr, dh, sizeof(RateRow) * (b1 - b0), cudaMemcpyHostToDevice, sc));
         }
+        BatchOut bo;
+        if (ctl) {
+            SlotCtl *d_ctl = m->aux_arena.take<SlotCtl>((size_t)(b1 - b0));
+            if (!d_ctl) { rc = fail(DFB_ERR_OOM, "settings table arena exhausted"); break; }
+            DFB_CUDA(cudaMemcpyAsync(d_ctl, ctl->data() + b0, sizeof(SlotCtl) * (b1 - b0), cudaMemcpyHostToDevice, sc));
+            bo.ctl = d_ctl;
+            bo.gate = gate;
+        }
+        if (lsnr) {
+            int64_t *d_lo = m->aux_arena.take<int64_t>((size_t)(b1 - b0));
+            if (!d_lo) { rc = fail(DFB_ERR_OOM, "LSNR table arena exhausted"); break; }
+            DFB_CUDA(cudaMemcpyAsync(d_lo, dlo.data() + b0, sizeof(int64_t) * (b1 - b0), cudaMemcpyHostToDevice, sc));
+            bo.lsnr = d_lsnr;
+            bo.lsnr_offs = d_lo;
+        }
         rc = enhance_group(m, st, staged ? d_in : src, staged ? d_out : dst, d_rows, tf, b1 - b0, pad, lim, tc, pipelined, sc,
-                           staged ? &hooks : nullptr, d_links, links ? reduce : 0);
+                           staged ? &hooks : nullptr, d_links, links ? reduce : 0, bo);
     }
     if (host) {
         const cudaError_t e1 = cudaStreamSynchronize(sc), e2 = cudaStreamSynchronize(sd), e3 = cudaStreamSynchronize(sh);
@@ -2551,22 +2644,94 @@ extern "C" int dfb_enhance_host(dfb_model *m, dfb_state *st, const float *h_audi
     return enhance_rows(m, st, rows, rr, h_audio, h_out, pad, atten_lim_db, true, nullptr);
 }
 
+// Validates the per-stream settings of dfb_enhance_ragged_ex (n of them, one per stream in the caller's order) and returns
+// them as apply-kernel rows with sw = 0 (*gate: some stream gates).  Linked streams (`links` non-empty) must agree within
+// their group.  The table runs the specialised CTL apply kernel, so it follows the slot path's model rules.
+static int settings_plan(const dfb_model *m, const dfb_enhance_settings *set, int64_t n, int64_t B, const std::vector<LinkRow> &links,
+                         std::vector<SlotCtl> &ctl, bool *gate) {
+    if (n != B) return fail(DFB_ERR_INVALID, "%lld settings for %lld streams", (long long)n, (long long)B);
+    const dfb_model_config &c = m->cfg;
+    if (c.model_kind == 1) return fail(DFB_ERR_UNSUPPORTED, "per-stream settings: DeepFilterNet v1 is not supported");
+    if (c.df_order != 5 || c.nb_df != 96 || c.nb_erb != 32)
+        return fail(DFB_ERR_UNSUPPORTED, "per-stream settings are built for df_order 5, nb_df 96 and 32 ERB bands");
+    ctl.resize((size_t)B);
+    *gate = false;
+    for (int64_t b = 0; b < B; b++) {
+        const dfb_enhance_settings &e = set[b];
+        if (std::isnan(e.atten_lim_db)) return fail(DFB_ERR_INVALID, "stream %lld: attenuation limit is NaN", (long long)b);
+        if (!(std::isfinite(e.post_filter_beta) && e.post_filter_beta >= 0.f))
+            return fail(DFB_ERR_INVALID, "stream %lld: post-filter beta must be finite and >= 0", (long long)b);
+        if (e.lsnr_gating && (std::isnan(e.min_db_thresh) || std::isnan(e.max_db_erb_thresh) || std::isnan(e.max_db_df_thresh)))
+            return fail(DFB_ERR_INVALID, "stream %lld: an LSNR threshold is NaN", (long long)b);
+        if (e.post_filter_beta > 0.f && c.model_kind != 3)
+            return fail(DFB_ERR_UNSUPPORTED, "per-stream post-filter beta: DeepFilterNet3 topologies only (DeepFilterNet2's beta is fixed)");
+        if (e.lsnr_gating && c.model_kind != 3) return fail(DFB_ERR_UNSUPPORTED, "LSNR stage gating: DeepFilterNet3 topologies only");
+        const float lim = e.atten_lim_db > 0.f ? powf(10.f, -e.atten_lim_db / 20.f) : 0.f;
+        SlotCtl r{lim, e.post_filter_beta, lim, e.post_filter_beta, 0};
+        if (e.lsnr_gating) { r.th_min = e.min_db_thresh; r.th_erb = e.max_db_erb_thresh; r.th_df = e.max_db_df_thresh; r.gate = 1; }
+        ctl[(size_t)b] = r;
+        *gate |= r.gate != 0;
+    }
+    for (int64_t b = 0; b < (int64_t)links.size(); b++)
+        if (memcmp(&ctl[(size_t)b], &ctl[(size_t)links[(size_t)b].first], sizeof(SlotCtl)))
+            return fail(DFB_ERR_INVALID, "stream %lld: the streams of a link group take one setting", (long long)b);
+    return DFB_OK;
+}
+
 // The body of every dfb_enhance_ragged* entry point: `group_sizes` null for a call without link groups, `rates` null for
-// one whose streams are all at 48 kHz.
+// one whose streams are all at 48 kHz, `settings` null for one setting (atten_lim_db, the model's post filter, no gating)
+// for every stream, `lsnr` null for no LSNR rows.
 static int enhance_ragged(dfb_model *m, dfb_state *st, const float *src, int64_t in_numel, const int64_t *in_offsets,
                           const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *dst, int64_t out_numel,
                           const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
-                          const int32_t *rates, bool host, cudaStream_t s) {
+                          const int32_t *rates, bool host, cudaStream_t s, const dfb_enhance_settings *settings = nullptr,
+                          int64_t n_settings = 0, float *lsnr = nullptr, int64_t lsnr_numel = 0, const int64_t *lsnr_offsets = nullptr) {
     if (!m || !st || !src || !dst) return fail(DFB_ERR_INVALID, "null argument");
     if (int rcs = check_state(m, st)) return rcs;
     std::vector<RaggedRow> rows;
     std::vector<RateRow> rr;
     std::vector<LinkRow> links;
+    std::vector<SlotCtl> ctl;
+    bool gate = false;
     if (int rc = batch_plan(m, st, in_numel, in_offsets, lengths, B, pad, out_numel, out_offsets, rates, rows, rr)) return rc;
     if (group_sizes)
         if (int rc = link_plan(m, rows, rr, group_sizes, n_groups, reduce_mask, links)) return rc;
+    if (settings)
+        if (int rc = settings_plan(m, settings, n_settings, B, links, ctl, &gate)) return rc;
+    if (lsnr) {
+        if (!lsnr_offsets) return fail(DFB_ERR_INVALID, "LSNR output without offsets");
+        if (m->cfg.model_kind == 1) return fail(DFB_ERR_UNSUPPORTED, "LSNR rows: DeepFilterNet v1 is not supported");
+        for (int64_t b = 0; b < B; b++) {
+            const int64_t o = lsnr_offsets[b], n = (rows[(size_t)b].out_len + st->hop - 1) / st->hop;
+            if (o < 0 || o > lsnr_numel - n)
+                return fail(DFB_ERR_INVALID, "stream %lld's LSNR row reaches outside the LSNR output (%lld values)", (long long)b,
+                            (long long)lsnr_numel);
+        }
+    }
     DFB_CUDA(cudaSetDevice(m->device));
-    return enhance_rows(m, st, rows, rr, src, dst, pad, atten_lim_db, host, s, links.empty() ? nullptr : &links, reduce_mask);
+    return enhance_rows(m, st, rows, rr, src, dst, pad, atten_lim_db, host, s, links.empty() ? nullptr : &links, reduce_mask,
+                        settings ? &ctl : nullptr, gate, lsnr, lsnr_offsets);
+}
+
+extern "C" int dfb_enhance_ragged_ex(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
+                                     const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
+                                     const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
+                                     const int32_t *rates, const dfb_enhance_settings *settings, int64_t n_settings, float *d_lsnr,
+                                     int64_t lsnr_numel, const int64_t *lsnr_offsets, void *stream) {
+    return enhance_ragged(m, st, d_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, d_out, out_numel, out_offsets,
+                          group_sizes, n_groups, reduce_mask, rates, false, (cudaStream_t)stream, settings, n_settings, d_lsnr,
+                          lsnr_numel, lsnr_offsets);
+}
+
+extern "C" int dfb_enhance_ragged_ex_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel,
+                                          const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad, float atten_lim_db,
+                                          float *h_out, int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes,
+                                          int64_t n_groups, int reduce_mask, const int32_t *rates,
+                                          const dfb_enhance_settings *settings, int64_t n_settings, float *h_lsnr, int64_t lsnr_numel,
+                                          const int64_t *lsnr_offsets) {
+    return enhance_ragged(m, st, h_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, h_out, out_numel, out_offsets,
+                          group_sizes, n_groups, reduce_mask, rates, true, nullptr, settings, n_settings, h_lsnr, lsnr_numel,
+                          lsnr_offsets);
 }
 
 extern "C" int dfb_enhance_ragged(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
@@ -2747,6 +2912,9 @@ struct dfb_stream {
     // the per-row table goes to the apply kernel.
     bool ctl_on = false;
     std::vector<float> slot_lim, slot_beta;            // per slot: own limit (linear, 0 off) / beta, or NaN: the handle's
+    std::vector<signed char> slot_gate;                // per slot: own LSNR gating (0 off, 1 on with slot_th), or -1: the handle's
+    std::vector<float> slot_th;                        // per slot: own thresholds [3]
+    bool ctl_gate = false;                             // a row of the uploaded table gates
     std::vector<char> slot_fresh;                      // per slot: opened since the last call (no previous setting)
     std::vector<SlotCtl> slot_ctl;                     // per slot: the settings of the last call and the one before
     std::vector<SlotCtl> ctl_up;                       // per row: the table on the device
@@ -2814,6 +2982,8 @@ static void slots_init(dfb_stream *h) {
     h->tab_dirty = true;
     h->slot_lim.assign(B, NAN);
     h->slot_beta.assign(B, NAN);
+    h->slot_gate.assign(B, -1);
+    h->slot_th.assign(3 * B, 0.f);
     h->slot_fresh.assign(B, 0);
     h->slot_ctl.assign(B, SlotCtl{});
     h->ctl_on = false;
@@ -3041,6 +3211,7 @@ static int slots_open(dfb_stream *h, const int64_t *slots, int64_t n, int64_t nc
         h->slot_end[(size_t)b] = kOpenEnd;
         h->slot_dir[(size_t)b] = dir;
         h->slot_lim[(size_t)b] = h->slot_beta[(size_t)b] = NAN;   // back to the handle's settings
+        h->slot_gate[(size_t)b] = -1;
         h->slot_fresh[(size_t)b] = 1;
     }
     h->tab_dirty = true;
@@ -3097,17 +3268,19 @@ extern "C" int dfb_stream_close_slots(dfb_stream *h, const int64_t *slots, int64
 // ---- per-slot settings.  A setting is stored per slot; each call resolves every live slot's setting (its own, or the
 // handle's default at that call) and, when it differs from the one of the slot's last call, switches at the call's first
 // output frame f0: frame f0 - 1, which the apply kernel re-synthesises for its overlap-add tail, keeps the previous one.
-static int ctl_set(dfb_stream *h, const int64_t *slots, int64_t n, bool beta, float v) {
+// The checks every per-slot setter makes before the value's own: a spectral handle, the slot list, the model shape.
+static int ctl_check(const dfb_stream *h, const int64_t *slots, int64_t n) {
     if (h && h->spectral)
-        return fail(DFB_ERR_UNSUPPORTED, "attenuation limit and post filter are apply-stage settings: a spectral handle applies nothing");
+        return fail(DFB_ERR_UNSUPPORTED, "per-slot settings are apply-stage settings: a spectral handle applies nothing");
     if (int rc = slot_list_check(h, slots, n)) return rc;
     const dfb_model_config &c = h->m->cfg;
     if (c.df_order != 5 || c.nb_df != 96 || c.nb_erb != 32)
         return fail(DFB_ERR_UNSUPPORTED, "per-slot settings are built for df_order 5, nb_df 96 and 32 ERB bands");
-    if (beta && c.model_kind != 3)
-        return fail(DFB_ERR_UNSUPPORTED, "per-slot post-filter beta: DeepFilterNet3 topologies only (DeepFilterNet2's beta is fixed)");
-    if (std::isnan(v) || (beta && !(v >= 0.f && std::isfinite(v))))
-        return fail(DFB_ERR_INVALID, beta ? "post-filter beta must be finite and >= 0" : "attenuation limit is NaN");
+    return DFB_OK;
+}
+
+// After the value's checks: naming a free slot is refused; otherwise the per-row table is on from now on.
+static int ctl_begin(dfb_stream *h, const int64_t *slots, int64_t n) {
     for (int64_t i = 0; i < n; i++)
         if (h->slot_state[(size_t)slots[i]] == kSlotFree) return fail(DFB_ERR_INVALID, "slot %lld is free", (long long)slots[i]);
     if (n == 0) return DFB_OK;
@@ -3126,8 +3299,35 @@ static int ctl_set(dfb_stream *h, const int64_t *slots, int64_t n, bool beta, fl
         h->ctl_up.clear();
         h->ctl_on = true;
     }
+    return DFB_OK;
+}
+
+static int ctl_set(dfb_stream *h, const int64_t *slots, int64_t n, bool beta, float v) {
+    if (int rc = ctl_check(h, slots, n)) return rc;
+    if (beta && h->m->cfg.model_kind != 3)
+        return fail(DFB_ERR_UNSUPPORTED, "per-slot post-filter beta: DeepFilterNet3 topologies only (DeepFilterNet2's beta is fixed)");
+    if (std::isnan(v) || (beta && !(v >= 0.f && std::isfinite(v))))
+        return fail(DFB_ERR_INVALID, beta ? "post-filter beta must be finite and >= 0" : "attenuation limit is NaN");
+    if (int rc = ctl_begin(h, slots, n)) return rc;
     std::vector<float> &dst = beta ? h->slot_beta : h->slot_lim;
     for (int64_t i = 0; i < n; i++) dst[(size_t)slots[i]] = v;
+    return DFB_OK;
+}
+
+// Per-slot LSNR stage gating (the LADSPA plugin's per-instance thresholds): the listed slots gate with their own thresholds,
+// or not at all (enable == 0), from the next call on, every frame of that call included.
+extern "C" int dfb_stream_set_lsnr_thresholds_slots(dfb_stream *h, const int64_t *slots, int64_t n, int enable, float min_db_thresh,
+                                                    float max_db_erb_thresh, float max_db_df_thresh) {
+    if (int rc = ctl_check(h, slots, n)) return rc;
+    if (enable && h->m->cfg.model_kind != 3) return fail(DFB_ERR_UNSUPPORTED, "LSNR stage gating: DeepFilterNet3 topologies only");
+    if (enable && (std::isnan(min_db_thresh) || std::isnan(max_db_erb_thresh) || std::isnan(max_db_df_thresh)))
+        return fail(DFB_ERR_INVALID, "an LSNR threshold is NaN");
+    if (int rc = ctl_begin(h, slots, n)) return rc;
+    for (int64_t i = 0; i < n; i++) {
+        const size_t b = (size_t)slots[i];
+        h->slot_gate[b] = enable ? 1 : 0;
+        h->slot_th[3 * b] = min_db_thresh; h->slot_th[3 * b + 1] = max_db_erb_thresh; h->slot_th[3 * b + 2] = max_db_df_thresh;
+    }
     return DFB_OK;
 }
 
@@ -3144,6 +3344,7 @@ extern "C" int dfb_stream_set_post_filter_beta(dfb_stream *h, const int64_t *slo
 static int ctl_rows(dfb_stream *h, int64_t f0, cudaStream_t s) {
     const float beta_def = default_beta(h->m);
     std::vector<SlotCtl> rows((size_t)h->n_act);
+    h->ctl_gate = false;
     for (int r = 0; r < h->n_act; r++) {
         const size_t b = (size_t)h->row_slot[(size_t)r];
         const float lim = std::isnan(h->slot_lim[b]) ? h->lim : h->slot_lim[b];
@@ -3151,6 +3352,12 @@ static int ctl_rows(dfb_stream *h, int64_t f0, cudaStream_t s) {
         SlotCtl &c = h->slot_ctl[b];
         if (h->slot_fresh[b]) { c = SlotCtl{lim, beta, lim, beta, f0}; h->slot_fresh[b] = 0; }
         else if (lim != c.lim || beta != c.beta) c = SlotCtl{lim, beta, c.lim, c.beta, f0};
+        // gating: the slot's own, or the handle's (dfb_stream_set_lsnr_thresholds)
+        const bool own = h->slot_gate[b] >= 0;
+        const float *th = own ? &h->slot_th[3 * b] : h->th;
+        c.gate = own ? h->slot_gate[b] : (h->gating ? 1 : 0);
+        c.th_min = th[0]; c.th_erb = th[1]; c.th_df = th[2];
+        h->ctl_gate |= c.gate != 0;
         rows[(size_t)r] = c;
     }
     if (rows.size() != h->ctl_up.size() || memcmp(rows.data(), h->ctl_up.data(), sizeof(SlotCtl) * rows.size())) {
@@ -3323,7 +3530,7 @@ static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, 
     io.first = h->d_first;
     if (so) spec_io(h, io, so, d_in, n, n_out, f0);
     if (h->tab_linked) { io.links = h->d_grp; io.reduce = h->group_reduce; }
-    if (h->ctl_on) io.ctl = h->d_ctl;
+    if (h->ctl_on) { io.ctl = h->d_ctl; io.ctl_gate = h->ctl_gate; }
     io.lsnr_from = h->lsnr_from;
     io.lsnr_out = d_lsnr;
     rc = m->arena.reserve(chunk_bytes_per_stream(m->cfg, st, (int)(d1n - (S.d1 > kHalo ? S.d1 - kHalo : 0)) + 1) * (size_t)h->n_act +

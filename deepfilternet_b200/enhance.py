@@ -111,27 +111,48 @@ def _rated(model: DfNet, sr, n: int):
     return rates
 
 
+def _settings(model: DfNet, n: int, atten_lim_db, post_filter_beta, lsnr_thresholds, return_lsnr: bool):
+    """The batch calls' per-entry settings as a dfb_enhance_settings table (ragged.settings_table), or None when the call
+    needs none; the combinations the library refuses are refused here first (DfbError, DFB_ERR_UNSUPPORTED)."""
+    c = model.cfg
+    default_beta = model.post_filter_beta if (c.model == "deepfilternet3" and model.post_filter) else 0.0
+    tab = ragged.settings_table(n, atten_lim_db, post_filter_beta, lsnr_thresholds, default_beta)
+    ragged.check_settings_model(c.model, c.nb_erb, c.nb_df, c.df_order, tab, return_lsnr)
+    return tab
+
+
 @torch.no_grad()
 def enhance(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
             atten_lim_db: Optional[float] = None, out: Optional[Tensor] = None, *, reduce_mask: Optional[str] = None,
-            sr: Optional[int] = None) -> Tensor:
+            sr: Optional[int] = None, post_filter_beta: Optional[float] = None, lsnr_thresholds=None,
+            return_lsnr: bool = False):
     """enhance.py:206-250: audio f32 CPU [C,T] @ model sr -> enhanced f32 CPU [C,T]
     (or [C, (T // hop) * hop], delayed by n_fft - hop, when ``pad`` is False).
     ``out`` (extension): optional preallocated (e.g. pinned) CPU tensor for the result.
     ``reduce_mask`` (extension): "max" or "mean" links the C channels as the Rust runtime does (tract.rs:868-902): they
     share one ERB mask, the max or mean of their own (include/dfb200.h, dfb_enhance_ragged_linked); None / "none": every
     channel on its own.
-    ``sr`` (extension): the rate of ``audio`` when it is not the model's 48 kHz, as :func:`enhance_batch` takes it."""
+    ``sr`` (extension): the rate of ``audio`` when it is not the model's 48 kHz, as :func:`enhance_batch` takes it.
+    ``post_filter_beta`` / ``lsnr_thresholds`` / ``return_lsnr`` (extensions): one value each, as :func:`enhance_batch`
+    takes them; with ``return_lsnr`` the result is ``(enhanced, lsnr)``."""
     model.eval()
     if audio.dim() != 2:
         raise ValueError("audio must have shape [C, T]")
-    if _rated(model, sr, 1) is not None:
-        y = enhance_batch(model, df_state, [audio], pad, atten_lim_db, reduce_mask, sr=[sr])[0]
-        if out is None:
-            return y
-        if out.shape != y.shape or out.dtype != torch.float32 or out.is_cuda or not out.is_contiguous():
-            raise ValueError(f"out must be a contiguous float32 CPU tensor of shape {tuple(y.shape)}")
-        return out.copy_(y)
+    if isinstance(atten_lim_db, (list, tuple, np.ndarray, Tensor)):
+        raise ValueError("enhance() takes one attenuation limit: use enhance_batch for one per entry")
+    if (_rated(model, sr, 1) is not None or post_filter_beta is not None or lsnr_thresholds is not None or return_lsnr):
+        if post_filter_beta is not None and not ragged._is_number(post_filter_beta):
+            raise ValueError("enhance() takes one post-filter beta: use enhance_batch for one per entry")
+        if lsnr_thresholds is not None:
+            lsnr_thresholds = ragged._thresholds(lsnr_thresholds, "lsnr_thresholds")
+        r = enhance_batch(model, df_state, [audio], pad, atten_lim_db, reduce_mask, sr=None if sr is None else [sr],
+                          post_filter_beta=post_filter_beta, lsnr_thresholds=lsnr_thresholds, return_lsnr=return_lsnr)
+        y = (r[0] if return_lsnr else r)[0]
+        if out is not None:
+            if out.shape != y.shape or out.dtype != torch.float32 or out.is_cuda or not out.is_contiguous():
+                raise ValueError(f"out must be a contiguous float32 CPU tensor of shape {tuple(y.shape)}")
+            y = out.copy_(y)
+        return (y, r[1][0]) if return_lsnr else y
     x = audio.detach().to("cpu", torch.float32).contiguous()
     c, t = x.shape
     out_len = int(_lib.lib().dfb_enhance_out_len(df_state.handle, t, 1 if pad else 0))
@@ -180,7 +201,8 @@ def enhance_device(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
 
 @torch.no_grad()
 def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: bool = True,
-                  atten_lim_db: Optional[float] = None, reduce_mask: Optional[str] = None, *, sr=None) -> List[Tensor]:
+                  atten_lim_db=None, reduce_mask: Optional[str] = None, *, sr=None, post_filter_beta=None,
+                  lsnr_thresholds=None, return_lsnr: bool = False):
     """Several recordings of different lengths in one call: ``audios`` is a sequence of CPU [C_i, T_i] tensors as
     :func:`enhance` takes them, every channel one stream.  Entry i of the result equals
     ``enhance(model, df_state, audios[i], pad, atten_lim_db)``.  The batch is packed into one page-locked buffer and
@@ -190,33 +212,64 @@ def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: boo
     ``sr``: the entries' sample rate, one for all or one per entry (None: 48 kHz).  Entry i at rate r is then
     ``io.resample(enhance(model, df_state, io.resample(audios[i], r, 48000), ...), 48000, r)``, with both resamplers run
     on the device per time chunk so that only rate-r samples cross PCIe (dfb_enhance_ragged_rates_host; any rate whose
-    sinc_fast taps hold at most 2^18 floats, e.g. 8, 11.025, 16, 22.05, 44.1, 96 kHz)."""
+    sinc_fast taps hold at most 2^18 floats, e.g. 8, 11.025, 16, 22.05, 44.1, 96 kHz).
+    Per-entry settings (dfb_enhance_ragged_ex_host): ``atten_lim_db`` one value or one per entry; ``post_filter_beta`` None
+    (the model's DeepFilterNet3 post filter), one value or one per entry, 0 = off (DeepFilterNet3 topologies); and
+    ``lsnr_thresholds`` None (no gating), one (min_db_thresh, max_db_erb_thresh, max_db_df_thresh) or one per entry (None:
+    that entry does not gate) -- the Rust runtime's LSNR stage gating (DeepFilterNet3 topologies).  Entry i then equals
+    the batch with entry i's settings given to every entry.  ``return_lsnr``: the result is ``(outputs, lsnrs)``, lsnrs[i]
+    float32 [n_i] (a multi-channel entry [C_i, n_i]) with value j the LSNR in dB of the frame 10 ms output hop j carries
+    (include/dfb200.h, dfb_enhance_ragged_ex)."""
     model.eval()
     xs = list(audios)
     for i, a in enumerate(xs):
         if not isinstance(a, Tensor) or a.dim() != 2:
             raise ValueError(f"entry {i}: audio must be a tensor of shape [C, T]")
     rates = _rated(model, sr, len(xs))
+    tab = _settings(model, len(xs), atten_lim_db, post_filter_beta, lsnr_thresholds, return_lsnr)
     shapes = [tuple(a.shape) for a in xs]
     lens, in_off, out_off, n_in, n_out, slices, srates = ragged.packed_layout(shapes, df_state.hop_size(), pad, rates)
     pin = torch.cuda.is_available()
     x = torch.empty(n_in, dtype=torch.float32, pin_memory=pin)
     torch.cat([a.detach().to("cpu", torch.float32).reshape(-1) for a in xs], out=x)
     y = torch.empty(n_out, dtype=torch.float32, pin_memory=pin)
-    lim = abs(float(atten_lim_db)) if atten_lim_db is not None else 0.0
+    lim = abs(float(atten_lim_db)) if atten_lim_db is not None and tab is None else 0.0
     reduce = ragged.reduce_code(reduce_mask)
     groups = ragged.packed_groups(shapes) if reduce != 0 else None
-    check(_lib.lib().dfb_enhance_ragged_rates_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
-                                                   lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
-                                                   out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
-                                                   groups.size if groups is not None else 0, reduce, srates.ctypes.data))
-    return [y[s:s + c * n].view(c, n) for s, c, n in slices]
+    outs = [y[s:s + c * n].view(c, n) for s, c, n in slices]
+    if tab is None and not return_lsnr:
+        check(_lib.lib().dfb_enhance_ragged_rates_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
+                                                       lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
+                                                       out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
+                                                       groups.size if groups is not None else 0, reduce, srates.ctypes.data))
+        return outs
+    chans = np.array([c for c, _ in shapes], dtype=np.int64)
+    stab = np.ascontiguousarray(np.repeat(tab, chans)) if tab is not None else None   # every channel takes its entry's
+    ln = ragged.lsnr_lens(lens, srates, df_state.hop_size(), pad) if return_lsnr else None
+    l_off = np.concatenate(([0], np.cumsum(ln)[:-1])).astype(np.int64) if return_lsnr else None
+    lz = torch.empty(int(ln.sum()) if return_lsnr else 0, dtype=torch.float32, pin_memory=pin)
+    check(_lib.lib().dfb_enhance_ragged_ex_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
+                                                lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
+                                                out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
+                                                groups.size if groups is not None else 0, reduce, srates.ctypes.data,
+                                                stab.ctypes.data if stab is not None else None, lens.size,
+                                                lz.data_ptr() if return_lsnr else None, lz.numel(),
+                                                l_off.ctypes.data if return_lsnr else None))
+    if not return_lsnr:
+        return outs
+    lsnrs, k = [], 0
+    for c, _ in shapes:
+        v = lz[int(l_off[k]):int(l_off[k]) + c * int(ln[k])].view(c, int(ln[k]))   # an entry's channels are consecutive
+        lsnrs.append(v[0] if c == 1 else v)
+        k += c
+    return outs, lsnrs
 
 
 @torch.no_grad()
 def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pad: bool = True,
-                          atten_lim_db: Optional[float] = None, out: Optional[Tensor] = None, group_sizes=None,
-                          reduce_mask: Optional[str] = None, *, sr=None) -> Tensor:
+                          atten_lim_db=None, out: Optional[Tensor] = None, group_sizes=None,
+                          reduce_mask: Optional[str] = None, *, sr=None, post_filter_beta=None, lsnr_thresholds=None,
+                          return_lsnr: bool = False):
     """Device-resident ragged batch: ``audio`` is a padded CUDA tensor [B, S] whose row b holds ``lengths[b]`` real
     samples.  Returns [B, max out_len] (asynchronous on the current stream): row b equals :func:`enhance_device` of
     ``audio[b, :lengths[b]]`` alone, and is zero beyond its own output length.  With ``out`` given, only each row's own
@@ -225,7 +278,10 @@ def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pa
     one length, and they share one ERB mask; each group's rows equal :func:`enhance` of that recording with the same
     ``reduce_mask``.
     ``sr``: the rows' sample rate, one for all or one per row (a link group's rows at one rate), as :func:`enhance_batch`
-    takes it; lengths and the result are in each row's own samples (dfb_enhance_ragged_rates)."""
+    takes it; lengths and the result are in each row's own samples (dfb_enhance_ragged_rates).
+    ``atten_lim_db`` / ``post_filter_beta`` / ``lsnr_thresholds``: as :func:`enhance_batch` takes them, one per row where
+    per entry (a link group's rows take one setting).  ``return_lsnr``: the result is ``(out, lsnr, lsnr_lengths)``, lsnr a
+    [B, max n] float32 CUDA tensor whose row b holds lsnr_lengths[b] values (NaN after them), as enhance_batch's."""
     if not audio.is_cuda or audio.dtype != torch.float32 or not audio.is_contiguous() or audio.dim() != 2:
         raise ValueError("enhance_device_ragged expects a contiguous float32 CUDA tensor of shape [B, S]")
     if audio.device != model.cuda_device:
@@ -238,6 +294,7 @@ def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pa
     rates = _rated(model, sr, b)
     if rates is None:
         rates = np.full(b, ragged.MODEL_SR, dtype=np.int32)
+    tab = _settings(model, b, atten_lim_db, post_filter_beta, lsnr_thresholds, return_lsnr)
     lens, in_off, out_off, ow = ragged.padded_layout(lens, s, df_state.hop_size(), pad, rates)
     reduce = ragged.reduce_code(reduce_mask)
     if group_sizes is None and reduce != 0:
@@ -250,14 +307,29 @@ def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pa
     elif (out.shape != (b, ow) or out.dtype != torch.float32 or not out.is_cuda or out.device != audio.device
           or not out.is_contiguous()):
         raise ValueError(f"out must be a contiguous float32 CUDA tensor of shape {(b, ow)} on {audio.device}")
-    lim = abs(float(atten_lim_db)) if atten_lim_db is not None else 0.0
+    lim = abs(float(atten_lim_db)) if atten_lim_db is not None and tab is None else 0.0
+    if tab is None and not return_lsnr:
+        with torch.cuda.device(audio.device):
+            stream = torch.cuda.current_stream(audio.device).cuda_stream
+            check(_lib.lib().dfb_enhance_ragged_rates(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
+                                                      lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow,
+                                                      out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
+                                                      groups.size if groups is not None else 0, reduce, rates.ctypes.data, stream))
+        return out
+    ln = ragged.lsnr_lens(lens, rates, df_state.hop_size(), pad)
+    nl = int(ln.max())
+    lz = torch.full((b, nl), float("nan"), dtype=torch.float32, device=audio.device) if return_lsnr else None
+    l_off = np.arange(b, dtype=np.int64) * nl
     with torch.cuda.device(audio.device):
         stream = torch.cuda.current_stream(audio.device).cuda_stream
-        check(_lib.lib().dfb_enhance_ragged_rates(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
-                                                  lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow,
-                                                  out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
-                                                  groups.size if groups is not None else 0, reduce, rates.ctypes.data, stream))
-    return out
+        check(_lib.lib().dfb_enhance_ragged_ex(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
+                                               lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow,
+                                               out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
+                                               groups.size if groups is not None else 0, reduce, rates.ctypes.data,
+                                               tab.ctypes.data if tab is not None else None, b,
+                                               lz.data_ptr() if return_lsnr else None, b * nl,
+                                               l_off.ctypes.data if return_lsnr else None, stream))
+    return (out, lz, torch.from_numpy(ln)) if return_lsnr else out
 
 
 # ------------------------------------------------------------------------------------------ CLI ----
@@ -327,11 +399,13 @@ def main(args) -> int:
             continue
         t0 = time.time()
         reduce = REDUCE_MASK_CLI[getattr(args, "reduce_mask", 0)]
+        extra = cli_settings(args, model)
         if batch_size == 1:
-            outs = [enhance(model, df_state, batch[0][2], pad=args.compensate_delay, atten_lim_db=args.atten_lim, reduce_mask=reduce)]
+            outs = [enhance(model, df_state, batch[0][2], pad=args.compensate_delay, atten_lim_db=args.atten_lim, reduce_mask=reduce,
+                            **extra)]
         else:
             outs = enhance_batch(model, df_state, [a for _, _, a, _ in batch], pad=args.compensate_delay, atten_lim_db=args.atten_lim,
-                                 reduce_mask=reduce)
+                                 reduce_mask=reduce, **extra)
         t_batch = time.time() - t0
         total = sum(a.numel() for _, _, a, _ in batch)
         for (i, file, audio_in, meta), audio in zip(batch, outs):
@@ -343,6 +417,24 @@ def main(args) -> int:
             audio = resample(audio.to("cpu"), df_sr, meta.sample_rate)
             save_audio(file, audio, sr=meta.sample_rate, output_dir=args.output_dir, suffix=suffix, log=False)
     return 0
+
+
+# LSNR stage gating thresholds of the deep-filter binary: its flags and defaults (libDF/src/bin/enhance_wav.rs:41-59)
+LSNR_THRESH_CLI = (("min_db_thresh", -15.0), ("max_db_erb_thresh", 35.0), ("max_db_df_thresh", 35.0))
+
+
+def cli_settings(args, model: DfNet) -> dict:
+    """The keyword arguments of enhance / enhance_batch that --pf-beta and the threshold flags ask for: with --pf, a
+    DeepFilterNet3 model's post filter takes --pf-beta (where it differs from the model's pf_beta, the plain call runs);
+    any threshold flag turns LSNR stage gating on, the flags not given taking the deep-filter binary's defaults."""
+    kw = {}
+    beta = getattr(args, "pf_beta", None)
+    if getattr(args, "pf", False) and model.cfg.model == "deepfilternet3" and beta is not None and beta != model.post_filter_beta:
+        kw["post_filter_beta"] = args.pf_beta
+    th = [getattr(args, name, None) for name, _ in LSNR_THRESH_CLI]
+    if any(v is not None for v in th):
+        kw["lsnr_thresholds"] = tuple(d if v is None else v for v, (_, d) in zip(th, LSNR_THRESH_CLI))
+    return kw
 
 
 def cli_parser():
@@ -362,6 +454,13 @@ def cli_parser():
     parser.add_argument("--reduce-mask", type=int, default=0, choices=sorted(REDUCE_MASK_CLI),
                         help="Link the channels of a multi-channel file: they share one ERB mask, 1 = the max, 2 = the mean of "
                              "their masks; 0 = every channel on its own (default).")
+    # the deep-filter binary's flags (enhance_wav.rs:30-59)
+    parser.add_argument("--pf-beta", type=float, default=0.02,
+                        help="Post-filter beta (with --pf, DeepFilterNet3). Higher beta results in stronger attenuation.")
+    for name, default in LSNR_THRESH_CLI:
+        parser.add_argument("--" + name.replace("_", "-"), type=float, default=None,
+                            help=f"LSNR stage gating threshold in dB (DeepFilterNet3; default {default:g} when any threshold "
+                                 "flag is given). Without any of these flags every frame is processed (no gating).")
     return parser
 
 

@@ -172,6 +172,100 @@ def _out_lens(lens: np.ndarray, rates, hop: int, pad: bool) -> np.ndarray:
     return -(-o48 * r // MODEL_SR)
 
 
+def lsnr_lens(lens: np.ndarray, rates, hop: int, pad: bool) -> np.ndarray:
+    """dfb_enhance_lsnr_len of every stream (int64 lengths in their own samples, rates one or one per stream): one value per
+    10 ms hop of the 48 kHz output, ceil(out48 / hop)."""
+    r = np.asarray(rates, dtype=np.int64)
+    o48 = -(-np.asarray(lens, dtype=np.int64) * MODEL_SR // r)
+    if not pad:
+        o48 = o48 // hop * hop
+    return -(-o48 // hop)
+
+
+# Per-entry settings of the batch calls (dfb_enhance_ragged_ex): the layout of dfb_enhance_settings
+SETTINGS_DTYPE = np.dtype([("atten_lim_db", "<f4"), ("post_filter_beta", "<f4"), ("lsnr_gating", "<i4"),
+                           ("min_db_thresh", "<f4"), ("max_db_erb_thresh", "<f4"), ("max_db_df_thresh", "<f4")])
+
+
+def _is_number(v) -> bool:
+    return isinstance(v, (int, float, np.integer, np.floating)) and not isinstance(v, bool)
+
+
+def _per_entry(v, n: int, what: str) -> list:
+    """A scalar for every entry or one value per entry (list, tuple, array or tensor of n)."""
+    if v is None or _is_number(v):
+        return [v] * n
+    vals = list(np.asarray(v.detach().cpu() if hasattr(v, "detach") else v, dtype=object).reshape(-1))
+    if len(vals) != n:
+        raise ValueError(f"{len(vals)} values of {what} for {n} entries")
+    return vals
+
+
+def _thresholds(v, what: str):
+    if v is None:
+        return None
+    t = list(v) if isinstance(v, (list, tuple, np.ndarray)) else None
+    if t is None or len(t) != 3 or not all(_is_number(x) for x in t):
+        raise ValueError(f"{what}: (min_db_thresh, max_db_erb_thresh, max_db_df_thresh), got {v!r}")
+    if any(math.isnan(float(x)) for x in t):
+        raise ValueError(f"{what}: a threshold is NaN")
+    return tuple(float(x) for x in t)
+
+
+def settings_table(n: int, atten_lim_db, post_filter_beta, lsnr_thresholds, default_beta: float):
+    """The dfb_enhance_settings table of n entries for the batch calls' arguments, or None when they need none: a scalar (or
+    None) atten_lim_db with post_filter_beta and lsnr_thresholds None runs the call without a table, as before.
+    atten_lim_db: None, a scalar or one per entry (None: off; |db| as enhance() takes it).  post_filter_beta: None (the
+    model's, ``default_beta``), a scalar or one per entry, finite and >= 0.  lsnr_thresholds: None (no gating), one
+    (min_db_thresh, max_db_erb_thresh, max_db_df_thresh) for all, or one per entry (None: that entry does not gate).
+    ValueError for a wrong count, a NaN limit or threshold, or a negative / non-finite beta."""
+    if (atten_lim_db is None or _is_number(atten_lim_db)) and post_filter_beta is None and lsnr_thresholds is None:
+        return None
+    tab = np.zeros(n, dtype=SETTINGS_DTYPE)
+    for i, v in enumerate(_per_entry(atten_lim_db, n, "atten_lim_db")):
+        if v is not None and not _is_number(v):
+            raise ValueError(f"entry {i}: attenuation limit must be a number of dB, got {v!r}")
+        if v is not None and math.isnan(float(v)):
+            raise ValueError(f"entry {i}: attenuation limit is NaN")
+        tab["atten_lim_db"][i] = abs(float(v)) if v is not None else 0.0
+    for i, v in enumerate(_per_entry(post_filter_beta, n, "post_filter_beta")):
+        if v is None:
+            v = default_beta
+        if not _is_number(v) or not math.isfinite(float(v)) or float(v) < 0:
+            raise ValueError(f"entry {i}: post-filter beta must be finite and >= 0, got {v!r}")
+        tab["post_filter_beta"][i] = float(v)
+    if lsnr_thresholds is not None:
+        if isinstance(lsnr_thresholds, np.ndarray) and lsnr_thresholds.ndim == 1:
+            lsnr_thresholds = tuple(lsnr_thresholds.tolist())
+        one = isinstance(lsnr_thresholds, (list, tuple)) and len(lsnr_thresholds) == 3 and all(_is_number(x) for x in lsnr_thresholds)
+        ths = [lsnr_thresholds] * n if one else list(lsnr_thresholds)
+        if len(ths) != n:
+            raise ValueError(f"{len(ths)} threshold triples for {n} entries")
+        for i, t in enumerate(ths):
+            t = _thresholds(t, f"entry {i}: lsnr_thresholds")
+            if t is not None:
+                tab["lsnr_gating"][i] = 1
+                tab["min_db_thresh"][i], tab["max_db_erb_thresh"][i], tab["max_db_df_thresh"][i] = t
+    return tab
+
+
+def check_settings_model(model: str, nb_erb: int, nb_df: int, df_order: int, tab, return_lsnr: bool) -> None:
+    """The combinations dfb_enhance_ragged_ex refuses with DFB_ERR_UNSUPPORTED, refused before the library is called
+    (DfbError): a settings table needs the specialised apply kernel (df_order 5, nb_df 96, 32 ERB bands) and not DeepFilterNet
+    v1; a beta > 0 or gating needs a DeepFilterNet3 topology; DeepFilterNet v1 returns no LSNR rows."""
+    from ._lib import DFB_ERR_UNSUPPORTED, DfbError
+    if model == "deepfilternet" and (tab is not None or return_lsnr):
+        raise DfbError(DFB_ERR_UNSUPPORTED, "per-entry settings and LSNR rows: DeepFilterNet v1 is not supported")
+    if tab is None:
+        return
+    if df_order != 5 or nb_df != 96 or nb_erb != 32:
+        raise DfbError(DFB_ERR_UNSUPPORTED, "per-entry settings are built for df_order 5, nb_df 96 and 32 ERB bands")
+    if model != "deepfilternet3" and (tab["post_filter_beta"] > 0).any():
+        raise DfbError(DFB_ERR_UNSUPPORTED, "per-entry post-filter beta: DeepFilterNet3 topologies only (DeepFilterNet2's beta is fixed)")
+    if model != "deepfilternet3" and tab["lsnr_gating"].any():
+        raise DfbError(DFB_ERR_UNSUPPORTED, "LSNR stage gating: DeepFilterNet3 topologies only")
+
+
 def check_group_rates(group_sizes, rates) -> None:
     """ValueError when a link group's streams are at different rates (the channels of one recording have one rate)."""
     b = 0

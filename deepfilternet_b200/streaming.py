@@ -289,10 +289,21 @@ class DfStream:
             self._h = None
 
     def set_lsnr_thresholds(self, min_db_thresh: float = -10.0, max_db_erb_thresh: float = 30.0,
-                            max_db_df_thresh: float = 20.0, enable: bool = True) -> None:
-        """Stage gating of the Rust runtime (tract.rs:658-672, defaults tract.rs:180-185); off unless called."""
-        check(_lib.lib().dfb_stream_set_lsnr_thresholds(self._h, int(enable), float(min_db_thresh), float(max_db_erb_thresh),
-                                                        float(max_db_df_thresh)))
+                            max_db_df_thresh: float = 20.0, enable: bool = True, slots=None) -> None:
+        """Stage gating of the Rust runtime (tract.rs:658-672, defaults tract.rs:180-185); off unless called.
+        ``slots`` None: the handle's setting, for every slot without one of its own.  Otherwise the listed slots' own
+        setting from the next call on, every frame of it included (the LADSPA plugin's per-instance thresholds; a group
+        lists all of its members; ``open`` and ``reset`` return a slot to the handle's; dfb_stream_set_lsnr_thresholds_slots).
+        ValueError for a NaN threshold while gating is on."""
+        th = (float(min_db_thresh), float(max_db_erb_thresh), float(max_db_df_thresh))
+        if slots is None:
+            check(_lib.lib().dfb_stream_set_lsnr_thresholds(self._h, int(enable), *th))
+            return
+        if enable and any(math.isnan(v) for v in th):
+            raise ValueError("an LSNR threshold is NaN")
+        a = slot_list(slots, self.batch)
+        check(_lib.lib().dfb_stream_set_lsnr_thresholds_slots(self._h, a.ctypes.data_as(C.POINTER(C.c_int64)), a.size,
+                                                              int(enable), *th))
 
     def reset(self) -> None:
         """Every slot open with a fresh stream, the clock back at 0."""

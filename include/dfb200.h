@@ -266,6 +266,53 @@ int dfb_enhance_ragged_rates_host(dfb_model *m, dfb_state *st, const float *h_au
 /* output length of a stream of T samples at `rate` in a rated batch: ceil(out48 rate / 48000), out48 =
  * dfb_enhance_out_len(st, ceil(T 48000 / rate), pad); -1 for a null state, T <= 0 or rate <= 0 */
 int64_t dfb_enhance_out_len_at(const dfb_state *st, int64_t T, int pad, int rate);
+/* Per-stream settings and LSNR rows of a ragged batch (DESIGN.md section 5k): dfb_enhance_ragged_rates(_host) with rates and
+ * group_sizes both optional (null: every stream at 48 kHz / no links), plus
+ *   settings / n_settings: one dfb_enhance_settings per stream, in the caller's order (n_settings == B), or null: every stream
+ *     takes atten_lim_db, the model's post filter and no gating, as in the other dfb_enhance_ragged* calls.  With a table,
+ *     atten_lim_db is ignored and stream b takes:
+ *       atten_lim_db       the rule of the other calls: <= 0 turns the limit off, else lim = 10^(-db / 20); NaN is invalid;
+ *       post_filter_beta   the DeepFilterNet3 post filter (deepfilternet3.py:448-454) with this beta, finite and >= 0,
+ *                          0 = off, in place of the model's option (dfb_model_set_options); DeepFilterNet2's own post filter
+ *                          on the ERB gains still follows the model's option;
+ *       lsnr_gating != 0   LSNR stage gating (tract.rs:658-672 apply_stages, as dfb_stream_set_lsnr_thresholds) with the
+ *                          three thresholds, none NaN.
+ *     The streams of a link group take one setting: their entries must be equal.  Stream b's result equals that of the
+ *     batch with stream b's entry given to every stream, bit for bit.
+ *   d_lsnr / h_lsnr, lsnr_numel, lsnr_offsets (HOST array): null for no LSNR output; else stream b's LSNR row,
+ *     dfb_enhance_lsnr_len(st, lengths[b], pad, rates[b]) floats in dB, goes to lsnr + lsnr_offsets[b].  Value j is the
+ *     LSNR of the 48 kHz STFT frame that 10 ms output hop j carries: DfNet.forward's lsnr[j + 1] of the stream alone with
+ *     pad != 0 (the output drops the first fft - hop = 480 samples, frame 0's head), lsnr[j] with pad == 0.  The frames
+ *     are those of the 48 kHz signal at every rate, so a stream at rate r has one value per 10 ms of its output, the last
+ *     one for the hop its output's last partial hop falls in.  This is the rule of dfb_stream_process_lsnr: hop j carries
+ *     frame f, and its value is that frame's LSNR, the one gating reads.
+ * Both run on the specialised apply kernel: a table needs df_order 5, nb_df 96 and 32 ERB bands (every shipped model);
+ * post_filter_beta > 0 and lsnr_gating need a DeepFilterNet3 topology; DeepFilterNet v1 takes neither a table nor LSNR
+ * rows.  Everything else is DFB_ERR_UNSUPPORTED.  DFB_ERR_INVALID for n_settings != B, a NaN limit or threshold, a beta
+ * < 0 or not finite, linked streams whose entries differ, LSNR rows without offsets or outside lsnr_numel, and everything
+ * the rated call refuses.  Gating selects what is applied to a frame, as on streaming handles: the network runs every
+ * frame (the Rust runtime skips its decoders on gated frames; see DESIGN.md section 5k).  A refused call changes nothing.
+ * With settings and d_lsnr both null this is the call it extends, launch for launch.  The _host variant copies the LSNR
+ * rows back chunk by chunk, next to the audio. */
+typedef struct {
+    float atten_lim_db;
+    float post_filter_beta;
+    int32_t lsnr_gating;
+    float min_db_thresh, max_db_erb_thresh, max_db_df_thresh;
+} dfb_enhance_settings;
+int dfb_enhance_ragged_ex(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
+                          const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
+                          const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
+                          const int32_t *rates, const dfb_enhance_settings *settings, int64_t n_settings, float *d_lsnr,
+                          int64_t lsnr_numel, const int64_t *lsnr_offsets, void *stream);
+int dfb_enhance_ragged_ex_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel, const int64_t *in_offsets,
+                               const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *h_out, int64_t out_numel,
+                               const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
+                               const int32_t *rates, const dfb_enhance_settings *settings, int64_t n_settings, float *h_lsnr,
+                               int64_t lsnr_numel, const int64_t *lsnr_offsets);
+/* LSNR values of a stream of T samples at `rate` in dfb_enhance_ragged_ex: ceil(out48 / 480), out48 =
+ * dfb_enhance_out_len(st, ceil(T 48000 / rate), pad) (T at 48 kHz); -1 for a null state, T <= 0 or rate <= 0 */
+int64_t dfb_enhance_lsnr_len(const dfb_state *st, int64_t T, int pad, int rate);
 /* Debug aid: one of a model's offline resamplers (up != 0: rate -> 48 kHz, else 48 kHz -> rate) alone over B rows (B <= 65535):
  * row b is in_lengths[b] samples at d_in + in_offsets[b] (at rates[b] going up, at 48 kHz going down; registered rates
  * only), and its resampled signal, io.resample's length, goes to d_out + out_offsets[b].  The launches are those of a chunk
@@ -298,6 +345,15 @@ int64_t dfb_stream_latency_frames(const dfb_stream *s);    /* hops the output tr
  * DeepFilterNet3 topologies only. */
 int dfb_stream_set_lsnr_thresholds(dfb_stream *s, int enable, float min_db_thresh, float max_db_erb_thresh,
                                    float max_db_df_thresh);
+/* Per-slot LSNR stage gating (the LADSPA plugin's per-instance thresholds): the listed slots gate with these thresholds
+ * (enable != 0) or not at all (enable == 0), in place of the handle's setting above, from the next process / flush call on,
+ * every frame of that call included.  `slots` as dfb_stream_set_atten_lim (a free slot or a partial group is
+ * DFB_ERR_INVALID; DFB_ERR_UNSUPPORTED on linked handles and for models whose apply step is not the specialised kernel).
+ * DeepFilterNet3 topologies only when enable != 0 (else DFB_ERR_UNSUPPORTED); a NaN threshold is DFB_ERR_INVALID; a
+ * spectral handle, which gates in one pass for all rows, is DFB_ERR_UNSUPPORTED.  Opening a slot and dfb_stream_reset
+ * return it to the handle's setting.  A refused call changes nothing. */
+int dfb_stream_set_lsnr_thresholds_slots(dfb_stream *s, const int64_t *slots, int64_t n, int enable, float min_db_thresh,
+                                         float max_db_erb_thresh, float max_db_df_thresh);
 /* Linked channels (see dfb_enhance_ragged_linked): streams g * channels + c form link group g; B % channels == 0.
  * Only on a new or reset handle (DFB_ERR_INVALID after the first frame: the frame re-synthesised for the overlap-add
  * tail would mix two settings) that has had no slot operation (DFB_ERR_UNSUPPORTED).  channels = 1 or DFB_REDUCE_NONE:
