@@ -1343,6 +1343,11 @@ static int forward_v1(dfb_model *m, Arena &arena, const float *d_feat_erb, const
     m->dbg["cemb"] = {f.cemb, M * H}; m->dbg["emb_in"] = {f.emb, M * H}; m->dbg["emb"] = {f.embo, M * H};
     m->dbg["dec_emb"] = {f.dec, M * H}; m->dbg["d3"] = {f.d3, M * (E / 4) * kCh}; m->dbg["d2"] = {f.d2, M * (E / 2) * kCh};
     m->dbg["d1"] = {f.d1, M * E * kCh}; m->dbg["dfc"] = {f.dfc, M * H}; m->dbg["y0"] = {f.y[0], M * H};
+    // every GRU layer's output (y: encoder, z: DF decoder) and the decoder pathways, for the layer-by-layer tests
+    for (int l = 1; l < c.enc_gru_layers && l < 3; l++) m->dbg["y" + std::to_string(l)] = {f.y[l], M * H};
+    for (int l = 0; l < c.df_gru_layers && l < 2; l++) m->dbg["z" + std::to_string(l)] = {f.z[l], M * H};
+    m->dbg["p3"] = {f.p3, M * (E / 4) * kCh}; m->dbg["p2"] = {f.p2, M * (E / 4) * kCh};
+    m->dbg["p1"] = {f.p1, M * (E / 2) * kCh}; m->dbg["p0"] = {f.p0, M * E * kCh};
     auto gather = [&](cudaStream_t st, int n, const float *const *src, const int64_t *ld, const int *const *idx, int K, int relu,
                       float *out, unsigned short *hi, unsigned short *lo) -> int {
         GatherParams g{};

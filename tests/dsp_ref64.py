@@ -219,13 +219,16 @@ def _deep_filter(S, bS, coefs, nb_df, order, lookahead, Tv):
 
 
 def apply(spec, m, coefs, widths, *, mode, nb_df, order, lookahead, post_filter=False, pf_beta=0.02, mask_only=False,
-          Tv=None):
+          Tv=None, alpha=None):
     """The enhanced spectrum of one model output (deepfilternet3.py:438-454 / deepfilternet2.py:481-505):
       mode 1 (DeepFilterNet3): k < nb_df: deep filter of the noisy spectrum; k >= nb_df (or mask_only): spec * erb_inv(m)
         (lib.rs:314-326 == Mask.forward modules.py:266-269); then the optional post filter on every bin.
       mode 2 (DeepFilterNet2): spec * erb_inv(m') first, m' = Mask.pf(m) with the post filter, then the deep filter of
         that masked spectrum for k < nb_df (unless mask_only).
+      mode 2 with alpha [B, T] (DeepFilterNet v1, DfOp real_unfold + assign_df, DeepFilterNet/df/modules.py:388-406,
+        470-478): the deep-filtered DF bins blended with the masked bins, Y a + X_masked (1 - a).
     spec [B, T, F] complex, m [B, T, E], coefs [B, T, nb_df, O] complex -> (spec_e, bound)."""
+    assert alpha is None or mode == 2, "the alpha blend filters the masked spectrum (mode 2)"
     spec = np.asarray(spec, np.complex128)
     m = np.asarray(m, np.float64)
     B, T, F = spec.shape
@@ -246,6 +249,13 @@ def apply(spec, m, coefs, widths, *, mode, nb_df, order, lookahead, post_filter=
         y[..., :nb_df], by[..., :nb_df] = Yd, bYd
     else:
         Yd, bYd = _deep_filter(xm, bxm, coefs, nb_df, order, lookahead, Tv)
+        if alpha is not None:
+            # the blend's roundings: 1 - a, the masked bin's products with g and (1 - a) in either association, Y a and
+            # the sum; the inputs' bounds carried through the weights a and 1 - a (both in [0, 1])
+            a = np.asarray(alpha, np.float64)[..., None]
+            xd, bxd = xm[..., :nb_df], bxm[..., :nb_df]
+            bYd = a * bYd + (1 - a) * bxd + gamma(4) * (a * np.abs(Yd) + (1 - a) * np.abs(xd))
+            Yd = Yd * a + xd * (1 - a)
         y, by = xm.copy(), bxm.copy()
         y[..., :nb_df], by[..., :nb_df] = Yd, bYd
     if post_filter and mode == 1:

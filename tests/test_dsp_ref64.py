@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+import dfnet1_oracle as O1
 import dfnet_oracle as O
 import dsp_ref64 as R
 import libdf_oracle as LO
@@ -111,6 +112,42 @@ def test_apply_stages(ost, mode, la, pf, mask_only):
     spec, m, c = random_apply_inputs(2, 19, 96, 5, seed=mode * 10 + la)
     ref, b = R.apply(spec, m, c, w, mode=mode, nb_df=96, order=5, lookahead=la, post_filter=pf, mask_only=mask_only)
     assert within(oracle_apply(spec, m, c, w, mode, 96, 5, la, pf, mask_only), ref, b) <= 1
+
+
+def oracle_df_alpha(spec, m, c, alpha, widths, nb_df, order, la, pf):
+    """DeepFilterNet v1's apply stages in fp32 torch: the (optionally post-filtered) mask, then dfnet1_oracle's DfOp
+    real_unfold blended by alpha with the masked bins."""
+    s = torch.view_as_real(torch.from_numpy(spec)).unsqueeze(1)
+    mt = torch.from_numpy(m).unsqueeze(1)
+    if pf:
+        beta = 0.02
+        m_sin = mt * torch.sin(np.pi * mt / 2)
+        mt = (1 + beta) * mt / (1 + beta * mt.div(m_sin.clamp_min(1e-12)).pow(2))
+    spec_m = O.apply_mask(s, mt, O.erb_inv_matrix(widths))
+    coefs = torch.view_as_real(torch.from_numpy(c)).permute(0, 1, 3, 2, 4)      # [B,T,O,Fd,2]
+    e = O1.df_op_real_unfold(spec_m, coefs, torch.from_numpy(alpha).unsqueeze(-1), nb_df, order, la)
+    return torch.view_as_complex(e.squeeze(1).contiguous()).numpy()
+
+
+def random_alpha(B, T, seed):
+    rng = np.random.default_rng(seed)
+    a = rng.random((B, T)).astype(np.float32)
+    a[:, ::5] = 0.0     # exact 0 and 1: only one of the blend's terms remains
+    a[:, 1::5] = 1.0
+    return a
+
+
+@pytest.mark.parametrize("la", [0, 1, 3])
+@pytest.mark.parametrize("pf", [False, True])
+def test_alpha_blend(ost, la, pf):
+    """DeepFilterNet v1's alpha blend (mode 2 with alpha) of the fp32 oracle within ref64's bound, with and without Mask.pf,
+    at look-aheads 0, 1 (shipped) and 3 (measured max err / bound: 0.99, a gain bin's single rounded product; 0.34 over
+    the blended DF bins)."""
+    w = ost.erb_widths()
+    spec, m, c = random_apply_inputs(2, 19, 96, 5, seed=70 + la)
+    alpha = random_alpha(2, 19, seed=la)
+    ref, b = R.apply(spec, m, c, w, mode=2, nb_df=96, order=5, lookahead=la, post_filter=pf, alpha=alpha)
+    assert within(oracle_df_alpha(spec, m, c, alpha, w, 96, 5, la, pf), ref, b) <= 1
 
 
 def test_bounds_see_small_formula_changes(ost):

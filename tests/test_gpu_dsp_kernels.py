@@ -4,7 +4,7 @@ Each test asserts |gpu - ref64| <= K * bound for every element, where bound is r
 same formula (the fp32 CPU oracle meets the same bounds with K = 1, tests/test_dsp_ref64.py), at the shapes where the kernels
 switch paths: the one-thread and the time-segmented normalisation scan, the analysis kernel's 8-frame CTA tiles, the apply
 kernel's 8 / 16-frame warp tiles with the re-synthesised frame before each and the preloaded deep-filter history, the
-specialised and the generic apply kernel.  Inputs come from seeds only."""
+specialised and the generic apply kernel, DeepFilterNet v1's alpha blend in both.  Inputs come from seeds only."""
 import ctypes as C
 import dataclasses
 
@@ -15,7 +15,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 import dsp_ref64 as R
-from test_gpu_parity import cfg_of
+from test_gpu_parity import cfg_of, cfg_v1
 from tests_common import synth_audio
 
 from deepfilternet_b200 import DfNet, _lib, enhance, libdf
@@ -95,6 +95,8 @@ KINDS = {   # name: (test_gpu_parity config, nb_df, apply mode, df look-ahead)
     "dfn3_df64": ("dfn3", 64, 1, 2), "dfn2_df64": ("dfn2", 64, 2, 2),
     # 24 ERB bands: the generic apply kernel at another band count
     "dfn3_e24": ("e24", 96, 1, 2),
+    # DeepFilterNet v1: the masked deep filter blended with the masked bins by alpha (specialised / generic kernel)
+    "v1": ("v1", 96, 2, 1), "v1_df64": ("v1", 64, 2, 1),
 }
 OPTS = {"plain": (False, False), "pf": (True, False), "mask_only": (False, True)}
 
@@ -103,7 +105,7 @@ OPTS = {"plain": (False, False), "pf": (True, False), "mask_only": (False, True)
 def models(st):
     out = {}
     for name, (kind, nb_df, _, _) in KINDS.items():
-        cfg = dataclasses.replace(cfg_of(kind), nb_df=nb_df)
+        cfg = dataclasses.replace(cfg_v1() if kind == "v1" else cfg_of(kind), nb_df=nb_df)
         out[name] = DfNet(cfg, random_state_dict(cfg, seed=3), st if cfg.nb_erb == 32 else libdf.DF(48000, 960, HOP, cfg.nb_erb, 2))
     return out
 
@@ -160,6 +162,47 @@ def test_apply_against_ref64(st, models, kind, opt, Tf):
     run_apply_case(st, models, kind, opt, 3, Tf, seed=Tf)
 
 
+def forward_full(model, st, sp, fe, fs, pf, mask_only):
+    """dfb_model_forward_full with every output pointer (DeepFilterNet v1 has no dfb_apply): spec_e, m, coefs (complex
+    [B,T,nb_df,O]) and alpha of one call"""
+    L = _lib.lib()
+    B, _, T, E = fe.shape
+    d_sp, d_fe, d_fs = (t.cuda().contiguous() for t in (sp, fe, fs))
+    nan = lambda *s: torch.full(s, float("nan"), device="cuda")
+    spec_e, m, lsnr, c, a = nan(*d_sp.shape), nan(B, T, E), nan(B, T), nan(B, T, model.nb_df, 10), nan(B, T)
+    check(L.dfb_model_set_options(model.handle, int(pf), C.c_float(0.02), int(mask_only)))
+    try:
+        check(L.dfb_model_forward_full(model.handle, st.handle, d_sp.data_ptr(), d_fe.data_ptr(), d_fs.data_ptr(), B, T,
+                                       spec_e.data_ptr(), m.data_ptr(), lsnr.data_ptr(), c.data_ptr(), a.data_ptr(),
+                                       torch.cuda.current_stream().cuda_stream))
+        torch.cuda.synchronize()
+    finally:
+        check(L.dfb_model_set_options(model.handle, int(model.post_filter), C.c_float(model.post_filter_beta), int(not model.run_df)))
+    return (complex_of(spec_e.cpu()[:, 0]), m.cpu().numpy(), complex_of(c.cpu().reshape(B, T, model.nb_df, 5, 2)),
+            a.cpu().numpy())
+
+
+@pytest.mark.parametrize("Tf", [1, 2, 3, 8, 9, 16, 17, 31, 32, 33, 63, 64, 65])
+@pytest.mark.parametrize("opt", list(OPTS))
+@pytest.mark.parametrize("kind", ["v1", "v1_df64"])
+def test_alpha_blend_against_ref64(st, models, kind, opt, Tf):
+    """DeepFilterNet v1's apply stage (mode 2 with alpha: the deep filter of the masked spectrum blended with the masked
+    bins by alpha), with and without Mask.pf and with mask_only: the specialised kernel at nb_df = 96, the generic one
+    at 64.  dfb_apply refuses v1, so dfb_model_forward_full runs the whole model and spec_e is compared with ref64's apply
+    of that call's own m, coefs and alpha, at frame counts around the 8-frame warp tile and the 32-frame CTA.  K = 1 (worst
+    err / bound on an H100 80GB HBM3: 0.995 plain, 0.997 with mask_only, 0.65 with the post filter, at either nb_df)."""
+    _, nb_df, mode, la = KINDS[kind]
+    pf, mask_only = OPTS[opt]
+    model = models[kind]
+    x = torch.from_numpy(noisy(2, Tf * HOP + 131, seed=300 + Tf))
+    sp, fe, fs = df_features(x, st, nb_df, alpha=model.cfg.norm_alpha)
+    got, m, c, a = forward_full(model, st, sp, fe, fs, pf, mask_only)
+    assert np.isfinite(a).all() and ((a >= 0) & (a <= 1)).all()
+    ref, b = R.apply(complex_of(sp[:, 0]), m, c, st.erb_widths(), mode=mode, nb_df=nb_df, order=5, lookahead=la,
+                     post_filter=pf, mask_only=mask_only, alpha=a)
+    assert_within(f"{kind} {opt} Tf={Tf}", got, ref, b, 1)
+
+
 @pytest.mark.parametrize("opt", ["plain", "pf"])
 @pytest.mark.parametrize("kind", ["dfn3", "dfn2"])
 def test_apply_16_frame_warps(st, models, kind, opt):
@@ -179,13 +222,13 @@ def test_generic_apply_against_ref64(st, models, kind, opt, Tf):
 
 
 # ------------------------------------------------------------------ fused synthesis ----
-@pytest.mark.parametrize("kind", ["dfn3", "ll", "dfn2"])
+@pytest.mark.parametrize("kind", ["dfn3", "ll", "dfn2", "v1"])
 def test_fused_synthesis_against_ref64(st, models, kind):
     """enhance(pad=False) in one time chunk against the float64 ISTFT of the spec_e that DfNet.forward returns for the same
     df_features: the irFFT, window and overlap-add of k_apply_synthesis, including the tail of each warp's frame t0 - 1,
     at lengths that end inside and on a warp / CTA tile; and the attenuation limit mixed in before the ISTFT.  One-chunk
     enhance and forward compute the same model outputs, so the bound is ref64's ISTFT bound alone.  K = 1 (worst
-    err / bound on an H100 80GB HBM3: 0.10, with the limit 0.05)."""
+    err / bound on an H100 80GB HBM3: 0.10, with the limit 0.05; DeepFilterNet v1 0.05, with the limit 0.04)."""
     model = models[kind]
     model.set_chunking(1, 1, 1)
     lim_db = 12.0

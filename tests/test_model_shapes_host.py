@@ -1,16 +1,19 @@
 """CPU: the element-wise bounds of tests/model_ref64.py, which tests/test_gpu_model_shapes.py holds the DNN's layers to, reject
 plausible kernel mistakes.  Each mistake is applied to the float64 reference on the same inputs; its worst err / bound
 must exceed 1, while the reference rounded to fp32 stays within the bound.  Shipped baseline (32 ERB bands, kt = 1) and
-one non-32 row (24 bands, NF = 5 / 10 / 21 tiles)."""
+one non-32 row (24 bands, NF = 5 / 10 / 21 tiles); DeepFilterNet v1's shipped shape (model_ref64's v1 section)."""
+import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+import dfnet1_oracle as O1
 import dfnet_oracle as O
 import dsp_ref64 as R
 import model_ref64 as M
 from deepfilternet_b200.config import ModelConfig, check_model_shape
 from deepfilternet_b200.weights import random_state_dict
+from test_gpu_gru_tc import C1, C2    # the GRU recurrence bound's constants
 
 B, T = 2, 33
 
@@ -141,3 +144,110 @@ def test_look_ahead_refused_before_the_library(model, change):
     with pytest.raises(NotImplementedError, match="look-ahead"):
         check_model_shape(ModelConfig(model=model, **change), {})
     check_model_shape(ModelConfig(model=model, conv_lookahead=2), {})
+
+
+# ------------------------------------------------------------------------------------------- DeepFilterNet v1 ----
+# The bounds of model_ref64's v1 section (tests/test_gpu_v1_layers.py) against the mistakes a v1 kernel or its packing
+# could make: same rule, each mistake above 1, the fp32 rounding of the reference within 1.
+@pytest.fixture(scope="module")
+def v1():
+    cfg = ModelConfig(model="deepfilternet", conv_lookahead=2, df_lookahead=1, conv_ch=64, conv_kernel=(2, 3),
+                      convt_kernel=(2, 3), conv_kernel_inp=(2, 3), conv_k_enc=2, conv_k_dec=2, emb_hidden_dim=512,
+                      df_hidden_dim=512, emb_num_layers=3, df_num_layers=2, gru_groups=8, lin_groups=8, group_shuffle=True)
+    sd64, ab = M.state64(random_state_dict(cfg, seed=31))
+    g = torch.Generator().manual_seed(1)
+    E, Fd, H = cfg.nb_erb, cfg.nb_df, cfg.emb_hidden_dim
+    act = lambda f: torch.relu(torch.randn(B, 64, T, f, generator=g, dtype=torch.float64))
+    sym = lambda *s: torch.rand(*s, generator=g, dtype=torch.float64) * 2 - 1
+    x = dict(fe=torch.randn(B, 1, T, E, generator=g, dtype=torch.float64), fs=torch.randn(B, 2, T, Fd, generator=g, dtype=torch.float64),
+             e0=act(E), c0=act(Fd), c1=act(Fd // 2), d3=act(E // 4), d2=act(E // 2), p2=act(E // 4), p1=act(E // 2), d1=act(E), p0=act(E),
+             e3=act(E // 4).float(), cemb=torch.randn(B, T, H, generator=g), y0=sym(B, T, H), y1=sym(B, T, H), dfc=sym(B, T, H))
+    return cfg, sd64, ab, x
+
+
+def test_v1_fp32_rounding_of_reference_meets_bounds(v1):
+    cfg, sd, ab, x = v1
+    prev = torch.cat([torch.zeros(B, 1, 512, dtype=torch.float64), x["y1"][:, :-1]], 1)
+    for rb in (M.v1_input_conv(sd, ab, "enc.erb_conv0", x["fe"], 1), M.v1_input_conv(sd, ab, "enc.df_conv0", x["fs"], 2),
+               M.v1_block(sd, ab, "enc.erb_conv1", x["e0"], lookahead=1, ffma=True), M.v1_block(sd, ab, "enc.df_conv1", x["c0"]),
+               M.v1_block(sd, ab, "erb_dec.convt2", x["d3"], transposed=True, path=x["p2"], ffma=True),
+               M.v1_cemb(sd, ab, x["c1"], cfg.lin_groups),
+               M.v1_gru_layer(sd, ab, "enc.emb_gru.grus.1", 8, M.v1_gru_input(x["y0"], 8, True), prev, C1, C2),
+               M.v1_dec_emb(sd, ab, x["dfc"], cfg.lin_groups, True, 8), M.v1_mask(sd, ab, x["p0"], x["d1"]),
+               M.v1_coefs(sd, ab, cfg, x["dfc"], x["c0"], gemm=False), M.v1_coefs(sd, ab, cfg, x["dfc"], x["c0"], gemm=True)):
+        assert ratio(rb[0].float().double(), rb) <= 1
+
+
+def test_v1_look_ahead_padding_off_by_one_frame(v1):
+    """erb_conv1's look-ahead 1 and df_conv0's 2 (which crops the first frame), each taken one frame short or long."""
+    cfg, sd, ab, x = v1
+    ref = M.v1_block(sd, ab, "enc.erb_conv1", x["e0"], lookahead=1, ffma=True)
+    for la in (0, 2):
+        assert ratio(M.v1_block(sd, ab, "enc.erb_conv1", x["e0"], lookahead=la)[0], ref) > 1
+    ref = M.v1_input_conv(sd, ab, "enc.df_conv0", x["fs"], 2)
+    for la in (1, 3):
+        assert ratio(M.v1_input_conv(sd, ab, "enc.df_conv0", x["fs"], la)[0], ref) > 1
+
+
+def test_v1_transposed_taps_not_reversed(v1):
+    """convt2 / convt1 (two time taps, FFMA k_dwpw) with the ConvTranspose2d's time taps used in causal order."""
+    cfg, sd, ab, x = v1
+    for name, inp, path in (("erb_dec.convt2", x["d3"], x["p2"]), ("erb_dec.convt1", x["d2"], x["p1"])):
+        ref = M.v1_block(sd, ab, name, inp, transposed=True, path=path, ffma=True)
+        bad = mutated(sd, name + ".sconvt.weight", lambda w: w.flip(2))
+        assert ratio(M.v1_block(bad, ab, name, inp, transposed=True, path=path)[0], ref) > 1
+
+
+def test_v1_emb_in_order(v1):
+    """The GRU input e3 + shuffle(cemb), exact: e3 flattened channel-last instead of channel-major (a wrong idx_e3), or
+    df_fc_emb's shuffle dropped (a wrong idx_shuf)."""
+    cfg, sd, ab, x = v1
+    e3 = x["e3"].permute(0, 2, 3, 1).numpy()            # device layout [B,T,F8,C]
+    cemb = x["cemb"].numpy()
+    rb = M.v1_emb_in(e3, cemb, cfg.lin_groups)
+    assert ratio(torch.from_numpy(rb[0]), tuple(torch.from_numpy(v) for v in rb)) == 0
+    channel_last = e3.reshape(B, T, -1) + M.group_shuffle(cemb, cfg.lin_groups)
+    no_shuffle = np.ascontiguousarray(e3.swapaxes(-1, -2)).reshape(B, T, -1) + cemb
+    for bad in (channel_last, no_shuffle):
+        assert R.err_ratio(bad.astype(np.float64), *rb) > 1
+
+
+def test_v1_gru_input_shuffle_dropped(v1):
+    """Encoder GRU layer 1 fed the previous layer's output without the group shuffle that weights.py folds into W_ih."""
+    cfg, sd, ab, x = v1
+    prev = torch.cat([torch.zeros(B, 1, 512, dtype=torch.float64), x["y1"][:, :-1]], 1)
+    ref = M.v1_gru_layer(sd, ab, "enc.emb_gru.grus.1", 8, M.v1_gru_input(x["y0"], 8, True), prev, C1, C2)
+    assert ratio(M.v1_gru_layer(sd, ab, "enc.emb_gru.grus.1", 8, x["y0"], prev, C1, C2)[0], ref) > 1
+
+
+def test_v1_alpha_blend_with_unmasked_spectrum():
+    """The alpha blend taken with the noisy DF bins instead of the masked ones."""
+    rng = np.random.default_rng(3)
+    widths = np.full(32, 15)
+    widths[-1] += 1                                      # 481 bins
+    spec = ((rng.standard_normal((1, 12, 481)) + 1j * rng.standard_normal((1, 12, 481))) * 0.1)
+    m = rng.random((1, 12, len(widths)))
+    c = (rng.standard_normal((1, 12, 96, 5)) + 1j * rng.standard_normal((1, 12, 96, 5))) * 0.5
+    alpha = rng.random((1, 12))
+    ref, b = R.apply(spec, m, c, widths, mode=2, nb_df=96, order=5, lookahead=1, alpha=alpha)
+    yd, _ = R.apply(spec, m, c, widths, mode=2, nb_df=96, order=5, lookahead=1)
+    bad = ref.copy()
+    a = alpha[..., None]
+    bad[..., :96] = yd[..., :96] * a + spec[..., :96] * (1 - a)
+    assert R.err_ratio(bad, ref, b) > 1
+
+
+def test_v1_coefs_activation_dropped(v1):
+    """df_fc_out's tanh dropped, or df_convp's ReLU dropped, at both df_fc_out kernels' bounds."""
+    cfg, sd, ab, x = v1
+    B_, T_, H = x["dfc"].shape
+    lin = (x["dfc"] @ sd["df_dec.df_fc_out.0.weight"].T + sd["df_dec.df_fc_out.0.bias"]).view(B_, T_, 10, -1)
+    p = O1.convkxf(x["c0"], sd, "df_dec.df_convp", 1).permute(0, 2, 1, 3)
+    bn = "df_dec.df_convp.norm"
+    s = sd[bn + ".weight"] / torch.sqrt(sd[bn + ".running_var"] + 1e-5)
+    p_lin = F.conv2d(x["c0"], sd["df_dec.df_convp.sconv.weight"]) * s.view(1, -1, 1, 1) + (sd[bn + ".bias"] - sd[bn + ".running_mean"] * s).view(1, -1, 1, 1)
+    p_lin = p_lin.permute(0, 2, 1, 3)
+    for gemm in (False, True):
+        ref = M.v1_coefs(sd, ab, cfg, x["dfc"], x["c0"], gemm)
+        for bad in (lin + p, torch.tanh(lin) + p_lin):
+            assert ratio(bad.permute(0, 1, 3, 2), ref) > 1
