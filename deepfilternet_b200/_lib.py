@@ -84,18 +84,12 @@ SIGNATURES = {
     "dfb_enhance": (_I, [_VP, _VP, _VP, _I64, _I64, _I, _F, _VP, _VP]),
     "dfb_enhance_host": (_I, [_VP, _VP, _VP, _I64, _I64, _I, _F, _VP]),
     "dfb_enhance_out_len": (_I64, [_VP, _I64, _I]),
-    "dfb_enhance_ragged": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP]),
-    "dfb_enhance_ragged_host": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP]),
-    "dfb_enhance_ragged_linked": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I, _VP]),
-    "dfb_enhance_ragged_linked_host": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I]),
     "dfb_model_add_rate": (_I, [_VP, _I, _VP, _I, _I, _I, _VP, _I, _I, _I]),
-    "dfb_enhance_ragged_rates": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I, _VP, _VP]),
-    "dfb_enhance_ragged_rates_host": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I, _VP]),
+    "dfb_enhance_ragged": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I, _VP, _VP, _I64, _VP,
+                                _I64, _VP, _VP]),
+    "dfb_enhance_ragged_host": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I, _VP, _VP, _I64,
+                                     _VP, _I64, _VP]),
     "dfb_enhance_out_len_at": (_I64, [_VP, _I64, _I, _I]),
-    "dfb_enhance_ragged_ex": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I, _VP, _VP, _I64, _VP,
-                                   _I64, _VP, _VP]),
-    "dfb_enhance_ragged_ex_host": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I, _F, _VP, _I64, _VP, _VP, _I64, _I, _VP, _VP, _I64,
-                                        _VP, _I64, _VP]),
     "dfb_enhance_lsnr_len": (_I64, [_VP, _I64, _I, _I]),
     "dfb_debug_resample_rows": (_I, [_I, _VP, _VP, _VP, _VP, _VP, _I64, _VP, _VP, _VP, _I64, _VP]),
     "dfb_model_workspace_bytes": (_I64, [_VP]),

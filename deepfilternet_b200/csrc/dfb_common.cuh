@@ -126,7 +126,7 @@ struct DspTables {
 // common length.
 struct RaggedRow { int64_t in_off, len, out_off, out_len, Tf; };
 
-// Link group of one stream (linked channels, dfb_enhance_ragged_linked / dfb_stream_set_mask_reduce): the n streams
+// Link group of one stream (linked channels, dfb_enhance_ragged's link groups / dfb_stream_set_mask_reduce): the n streams
 // first .. first + n - 1 of the kernel's batch, which include this one, are the channels of one recording and share one
 // ERB mask.  A separate table rather than more RaggedRow fields: the analysis and input-conv kernels read RaggedRow.
 struct LinkRow { int first, n; };
@@ -160,7 +160,7 @@ struct ResampleIO {
 // [nw][K = 2 width + og] for the gcd-reduced rates og -> nw.  Output t of a stream is sum_k taps[t % nw][k] x[(t / nw) og -
 // width + k] over k = 0 .. K-1 in that order, taps outside the stream's input skipped: k_resample's sum, bit for bit.
 struct RateDir { const float *taps; int og, nw, K, width; };
-// A stream of a rated batch (dfb_enhance_ragged_rates) as a resampler launch sees it: in_len input samples at in + in_off,
+// A stream of a rated batch (dfb_enhance_ragged with rates) as a resampler launch sees it: in_len input samples at in + in_off,
 // out_len outputs at out + out_off, its direction (-1: a 48 kHz stream, which no resampler touches) and its 48 kHz frame
 // count tf (it has ended, every 48 kHz output written, once the chunk loop's DNN frames reach tf).
 struct RateRow { int64_t in_off, in_len, out_off, out_len, tf; int dir; };
@@ -202,7 +202,7 @@ __host__ __device__ __forceinline__ void rate_range(bool up, const RateDir &d, c
 // beta (0 = off) from absolute frame sw on, and the previous ones before it.  Only the frame before sw, re-synthesised
 // for its overlap-add tail, still reads the previous ones.  gate != 0: LSNR stage gating with the thresholds th_min /
 // th_erb / th_df (tract.rs:658-672), which apply to every frame of the row; it takes effect only in launches that run the
-// LSNR head (ApplyParams::lsnr).  Batch rows (dfb_enhance_ragged_ex) have sw = 0: one setting for the whole stream.
+// LSNR head (ApplyParams::lsnr).  Batch rows (dfb_enhance_ragged's settings) have sw = 0: one setting for the whole stream.
 struct SlotCtl { float lim, beta, lim0, beta0; int64_t sw; float th_min, th_erb, th_df; int gate; };
 
 // Streaming slots (dfb_stream_open_slots): `first` holds the absolute first frame of each stream of a launch, or is null.

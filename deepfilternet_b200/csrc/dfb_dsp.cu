@@ -372,7 +372,7 @@ __global__ void __launch_bounds__(256) k_resample_down(ResampleDirs dirs, const 
                  io.out + r.slot * io.out_pitch + io.out_col * d.hop_out, v * d.hop_out, fill_to(io, d));
 }
 
-// Offline resampler of a rated batch (dfb_enhance_ragged_rates; RateDir / RateRow / RateIO in dfb_common.cuh; DESIGN.md
+// Offline resampler of a rated batch (dfb_enhance_ragged with rates; RateDir / RateRow / RateIO in dfb_common.cuh; DESIGN.md
 // section 5i).  The whole input of a stream is on the device, so no history is carried: an output reads its taps straight
 // from the input, and an output is computed once, by the launch in whose range it falls.  Grid (tiles, rows): CTA (x, b)
 // writes row b's outputs [o0 + x kRateTile, o0 + (x + 1) kRateTile) of its range [o0, o1), so a row's outputs spread over
@@ -1155,7 +1155,7 @@ __global__ void __launch_bounds__(kGenThreads) k_synthesis_gen(const float2 *__r
 using namespace dfb;
 
 extern "C" const char *dfb_last_error(void) { return g_err.c_str(); }
-extern "C" const char *dfb_version(void) { return "dfb200 0.1.0 sm_90a"; }
+extern "C" const char *dfb_version(void) { return "dfb200 0.2.0 sm_90a"; }
 extern "C" int64_t dfb_kernel_launches(void) { return g_launches.load(); }
 
 extern "C" int dfb_profile_enable(int on, const char *only_kernel) {

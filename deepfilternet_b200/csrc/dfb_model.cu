@@ -1591,7 +1591,7 @@ extern "C" int64_t dfb_enhance_out_len_at(const dfb_state *st, int64_t T, int pa
     return len_from_48k(dfb_enhance_out_len(st, len_at_48k(T, rate), pad), rate);
 }
 
-// LSNR values of a stream in dfb_enhance_ragged_ex: one per 10 ms hop of its 48 kHz output, ceil(out48 / hop)
+// LSNR values of a stream in dfb_enhance_ragged: one per 10 ms hop of its 48 kHz output, ceil(out48 / hop)
 extern "C" int64_t dfb_enhance_lsnr_len(const dfb_state *st, int64_t T, int pad, int rate) {
     if (!st || T <= 0 || rate <= 0) return -1;
     const int64_t o48 = dfb_enhance_out_len(st, rate == kModelRate ? T : len_at_48k(T, rate), pad);
@@ -1777,7 +1777,7 @@ struct ChunkIO {
     // batches with a settings table), or null.  ctl_gate: some row gates, so the LSNR head runs.
     const SlotCtl *ctl = nullptr;
     bool ctl_gate = false;
-    // ragged batch LSNR rows (dfb_enhance_ragged_ex), or null: row b's value j, at lsnr_rows + lsnr_offs[b] (device table),
+    // ragged batch LSNR rows (dfb_enhance_ragged), or null: row b's value j, at lsnr_rows + lsnr_offs[b] (device table),
     // is the LSNR of the frame output hop j carries, frame j + out_sample0 / hop (k_lsnr_rows)
     float *lsnr_rows = nullptr;
     const int64_t *lsnr_offs = nullptr;
@@ -2128,7 +2128,7 @@ struct ChunkHooks {
     std::function<int(int64_t y0, int64_t y1, int64_t d1, int64_t na, cudaStream_t cs)> after;
 };
 
-// Per-row settings and LSNR rows of one stream group (dfb_enhance_ragged_ex), as device tables in the group's order, or
+// Per-row settings and LSNR rows of one stream group (dfb_enhance_ragged), as device tables in the group's order, or
 // nulls: ctl the settings (sw = 0), gate whether any row gates, lsnr / lsnr_offs the LSNR rows (ChunkIO::lsnr_rows).
 struct BatchOut {
     const SlotCtl *ctl = nullptr;
@@ -2649,7 +2649,7 @@ extern "C" int dfb_enhance_host(dfb_model *m, dfb_state *st, const float *h_audi
     return enhance_rows(m, st, rows, rr, h_audio, h_out, pad, atten_lim_db, true, nullptr);
 }
 
-// Validates the per-stream settings of dfb_enhance_ragged_ex (n of them, one per stream in the caller's order) and returns
+// Validates the per-stream settings of dfb_enhance_ragged (n of them, one per stream in the caller's order) and returns
 // them as apply-kernel rows with sw = 0 (*gate: some stream gates).  Linked streams (`links` non-empty) must agree within
 // their group.  The table runs the specialised CTL apply kernel, so it follows the slot path's model rules.
 static int settings_plan(const dfb_model *m, const dfb_enhance_settings *set, int64_t n, int64_t B, const std::vector<LinkRow> &links,
@@ -2683,14 +2683,14 @@ static int settings_plan(const dfb_model *m, const dfb_enhance_settings *set, in
     return DFB_OK;
 }
 
-// The body of every dfb_enhance_ragged* entry point: `group_sizes` null for a call without link groups, `rates` null for
-// one whose streams are all at 48 kHz, `settings` null for one setting (atten_lim_db, the model's post filter, no gating)
-// for every stream, `lsnr` null for no LSNR rows.
+// The body of dfb_enhance_ragged(_host): `group_sizes` null for a call without link groups, `rates` null for one whose
+// streams are all at 48 kHz, `settings` null for one setting (atten_lim_db, the model's post filter, no gating) for every
+// stream, `lsnr` null for no LSNR rows.
 static int enhance_ragged(dfb_model *m, dfb_state *st, const float *src, int64_t in_numel, const int64_t *in_offsets,
                           const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *dst, int64_t out_numel,
                           const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
-                          const int32_t *rates, bool host, cudaStream_t s, const dfb_enhance_settings *settings = nullptr,
-                          int64_t n_settings = 0, float *lsnr = nullptr, int64_t lsnr_numel = 0, const int64_t *lsnr_offsets = nullptr) {
+                          const int32_t *rates, const dfb_enhance_settings *settings, int64_t n_settings, float *lsnr,
+                          int64_t lsnr_numel, const int64_t *lsnr_offsets, bool host, cudaStream_t s) {
     if (!m || !st || !src || !dst) return fail(DFB_ERR_INVALID, "null argument");
     if (int rcs = check_state(m, st)) return rcs;
     std::vector<RaggedRow> rows;
@@ -2718,75 +2718,24 @@ static int enhance_ragged(dfb_model *m, dfb_state *st, const float *src, int64_t
                         settings ? &ctl : nullptr, gate, lsnr, lsnr_offsets);
 }
 
-extern "C" int dfb_enhance_ragged_ex(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
-                                     const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
-                                     const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
-                                     const int32_t *rates, const dfb_enhance_settings *settings, int64_t n_settings, float *d_lsnr,
-                                     int64_t lsnr_numel, const int64_t *lsnr_offsets, void *stream) {
-    return enhance_ragged(m, st, d_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, d_out, out_numel, out_offsets,
-                          group_sizes, n_groups, reduce_mask, rates, false, (cudaStream_t)stream, settings, n_settings, d_lsnr,
-                          lsnr_numel, lsnr_offsets);
-}
-
-extern "C" int dfb_enhance_ragged_ex_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel,
-                                          const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad, float atten_lim_db,
-                                          float *h_out, int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes,
-                                          int64_t n_groups, int reduce_mask, const int32_t *rates,
-                                          const dfb_enhance_settings *settings, int64_t n_settings, float *h_lsnr, int64_t lsnr_numel,
-                                          const int64_t *lsnr_offsets) {
-    return enhance_ragged(m, st, h_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, h_out, out_numel, out_offsets,
-                          group_sizes, n_groups, reduce_mask, rates, true, nullptr, settings, n_settings, h_lsnr, lsnr_numel,
-                          lsnr_offsets);
-}
-
 extern "C" int dfb_enhance_ragged(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
                                   const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
-                                  const int64_t *out_offsets, void *stream) {
+                                  const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
+                                  const int32_t *rates, const dfb_enhance_settings *settings, int64_t n_settings, float *d_lsnr,
+                                  int64_t lsnr_numel, const int64_t *lsnr_offsets, void *stream) {
     return enhance_ragged(m, st, d_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, d_out, out_numel, out_offsets,
-                          nullptr, 0, kReduceNone, nullptr, false, (cudaStream_t)stream);
+                          group_sizes, n_groups, reduce_mask, rates, settings, n_settings, d_lsnr, lsnr_numel, lsnr_offsets, false,
+                          (cudaStream_t)stream);
 }
 
 extern "C" int dfb_enhance_ragged_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel, const int64_t *in_offsets,
                                        const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *h_out, int64_t out_numel,
-                                       const int64_t *out_offsets) {
+                                       const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
+                                       const int32_t *rates, const dfb_enhance_settings *settings, int64_t n_settings, float *h_lsnr,
+                                       int64_t lsnr_numel, const int64_t *lsnr_offsets) {
     return enhance_ragged(m, st, h_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, h_out, out_numel, out_offsets,
-                          nullptr, 0, kReduceNone, nullptr, true, nullptr);
-}
-
-extern "C" int dfb_enhance_ragged_linked(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel,
-                                         const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad, float atten_lim_db,
-                                         float *d_out, int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes,
-                                         int64_t n_groups, int reduce_mask, void *stream) {
-    return !group_sizes ? fail(DFB_ERR_INVALID, "no link groups")
-                        : enhance_ragged(m, st, d_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, d_out, out_numel,
-                                         out_offsets, group_sizes, n_groups, reduce_mask, nullptr, false, (cudaStream_t)stream);
-}
-
-extern "C" int dfb_enhance_ragged_linked_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel,
-                                              const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad,
-                                              float atten_lim_db, float *h_out, int64_t out_numel, const int64_t *out_offsets,
-                                              const int64_t *group_sizes, int64_t n_groups, int reduce_mask) {
-    return !group_sizes ? fail(DFB_ERR_INVALID, "no link groups")
-                        : enhance_ragged(m, st, h_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, h_out, out_numel,
-                                         out_offsets, group_sizes, n_groups, reduce_mask, nullptr, true, nullptr);
-}
-
-extern "C" int dfb_enhance_ragged_rates(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
-                                        const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out,
-                                        int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups,
-                                        int reduce_mask, const int32_t *rates, void *stream) {
-    return !rates ? fail(DFB_ERR_INVALID, "null argument")
-                  : enhance_ragged(m, st, d_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, d_out, out_numel, out_offsets,
-                                   group_sizes, n_groups, reduce_mask, rates, false, (cudaStream_t)stream);
-}
-
-extern "C" int dfb_enhance_ragged_rates_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel,
-                                             const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad, float atten_lim_db,
-                                             float *h_out, int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes,
-                                             int64_t n_groups, int reduce_mask, const int32_t *rates) {
-    return !rates ? fail(DFB_ERR_INVALID, "null argument")
-                  : enhance_ragged(m, st, h_audio, in_numel, in_offsets, lengths, B, pad, atten_lim_db, h_out, out_numel, out_offsets,
-                                   group_sizes, n_groups, reduce_mask, rates, true, nullptr);
+                          group_sizes, n_groups, reduce_mask, rates, settings, n_settings, h_lsnr, lsnr_numel, lsnr_offsets, true,
+                          nullptr);
 }
 
 // Debug aid: one of the model's offline resamplers alone over a ragged batch, in the launches the chunk loop would make
@@ -3068,7 +3017,7 @@ extern "C" int dfb_stream_reset(dfb_stream *h) {
 }
 
 // Linked channels on a stream handle: streams g * channels + c (c < channels) are the channels of recording g and share one
-// ERB mask (reduce_mask max / mean, as dfb_enhance_ragged_linked): fixed slot groups, which survive a reset and take no
+// ERB mask (reduce_mask max / mean, as dfb_enhance_ragged's link groups): fixed slot groups, which survive a reset and take no
 // slot operations.  Only before the first frame of a new or reset handle: the frame re-synthesised for the overlap-add
 // tail at the next call would otherwise mix the two settings.  channels = 1 records the reduction of the slot groups
 // opened later (dfb_stream_open_linked).

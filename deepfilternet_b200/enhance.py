@@ -121,6 +121,11 @@ def _settings(model: DfNet, n: int, atten_lim_db, post_filter_beta, lsnr_thresho
     return tab
 
 
+def _ptr(a):
+    """The address of a numpy array or tensor for the library, or None (a null pointer) for None."""
+    return None if a is None else a.data_ptr() if isinstance(a, Tensor) else a.ctypes.data
+
+
 @torch.no_grad()
 def enhance(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
             atten_lim_db: Optional[float] = None, out: Optional[Tensor] = None, *, reduce_mask: Optional[str] = None,
@@ -130,7 +135,7 @@ def enhance(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
     (or [C, (T // hop) * hop], delayed by n_fft - hop, when ``pad`` is False).
     ``out`` (extension): optional preallocated (e.g. pinned) CPU tensor for the result.
     ``reduce_mask`` (extension): "max" or "mean" links the C channels as the Rust runtime does (tract.rs:868-902): they
-    share one ERB mask, the max or mean of their own (include/dfb200.h, dfb_enhance_ragged_linked); None / "none": every
+    share one ERB mask, the max or mean of their own (include/dfb200.h, dfb_enhance_ragged); None / "none": every
     channel on its own.
     ``sr`` (extension): the rate of ``audio`` when it is not the model's 48 kHz, as :func:`enhance_batch` takes it.
     ``post_filter_beta`` / ``lsnr_thresholds`` / ``return_lsnr`` (extensions): one value each, as :func:`enhance_batch`
@@ -169,9 +174,9 @@ def enhance(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
     lens = np.full(c, t, dtype=np.int64)
     in_off, out_off = np.arange(c, dtype=np.int64) * t, np.arange(c, dtype=np.int64) * out_len
     groups = np.array([c], dtype=np.int64)
-    check(_lib.lib().dfb_enhance_ragged_linked_host(model.handle, df_state.handle, x.data_ptr(), c * t, in_off.ctypes.data,
-                                                    lens.ctypes.data, c, 1 if pad else 0, lim, out.data_ptr(), c * out_len,
-                                                    out_off.ctypes.data, groups.ctypes.data, 1, reduce))
+    check(_lib.lib().dfb_enhance_ragged_host(model.handle, df_state.handle, x.data_ptr(), c * t, in_off.ctypes.data,
+                                             lens.ctypes.data, c, 1 if pad else 0, lim, out.data_ptr(), c * out_len,
+                                             out_off.ctypes.data, groups.ctypes.data, 1, reduce, None, None, 0, None, 0, None))
     return out
 
 
@@ -206,20 +211,20 @@ def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: boo
     """Several recordings of different lengths in one call: ``audios`` is a sequence of CPU [C_i, T_i] tensors as
     :func:`enhance` takes them, every channel one stream.  Entry i of the result equals
     ``enhance(model, df_state, audios[i], pad, atten_lim_db)``.  The batch is packed into one page-locked buffer and
-    enhanced by one ``dfb_enhance_ragged_rates_host`` call, which copies only the streams' own samples and computes only their
+    enhanced by one ``dfb_enhance_ragged_host`` call, which copies only the streams' own samples and computes only their
     own frames.  The results are views into one page-locked output buffer.  ``reduce_mask`` "max" / "mean": each entry's
     channels are linked, as ``enhance(..., reduce_mask=reduce_mask)`` links them.
     ``sr``: the entries' sample rate, one for all or one per entry (None: 48 kHz).  Entry i at rate r is then
     ``io.resample(enhance(model, df_state, io.resample(audios[i], r, 48000), ...), 48000, r)``, with both resamplers run
-    on the device per time chunk so that only rate-r samples cross PCIe (dfb_enhance_ragged_rates_host; any rate whose
+    on the device per time chunk so that only rate-r samples cross PCIe (any rate whose
     sinc_fast taps hold at most 2^18 floats, e.g. 8, 11.025, 16, 22.05, 44.1, 96 kHz).
-    Per-entry settings (dfb_enhance_ragged_ex_host): ``atten_lim_db`` one value or one per entry; ``post_filter_beta`` None
+    Per-entry settings: ``atten_lim_db`` one value or one per entry; ``post_filter_beta`` None
     (the model's DeepFilterNet3 post filter), one value or one per entry, 0 = off (DeepFilterNet3 topologies); and
     ``lsnr_thresholds`` None (no gating), one (min_db_thresh, max_db_erb_thresh, max_db_df_thresh) or one per entry (None:
     that entry does not gate) -- the Rust runtime's LSNR stage gating (DeepFilterNet3 topologies).  Entry i then equals
     the batch with entry i's settings given to every entry.  ``return_lsnr``: the result is ``(outputs, lsnrs)``, lsnrs[i]
     float32 [n_i] (a multi-channel entry [C_i, n_i]) with value j the LSNR in dB of the frame 10 ms output hop j carries
-    (include/dfb200.h, dfb_enhance_ragged_ex)."""
+    (include/dfb200.h, dfb_enhance_ragged)."""
     model.eval()
     xs = list(audios)
     for i, a in enumerate(xs):
@@ -237,24 +242,18 @@ def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: boo
     reduce = ragged.reduce_code(reduce_mask)
     groups = ragged.packed_groups(shapes) if reduce != 0 else None
     outs = [y[s:s + c * n].view(c, n) for s, c, n in slices]
-    if tab is None and not return_lsnr:
-        check(_lib.lib().dfb_enhance_ragged_rates_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
-                                                       lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
-                                                       out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
-                                                       groups.size if groups is not None else 0, reduce, srates.ctypes.data))
-        return outs
     chans = np.array([c for c, _ in shapes], dtype=np.int64)
     stab = np.ascontiguousarray(np.repeat(tab, chans)) if tab is not None else None   # every channel takes its entry's
-    ln = ragged.lsnr_lens(lens, srates, df_state.hop_size(), pad) if return_lsnr else None
-    l_off = np.concatenate(([0], np.cumsum(ln)[:-1])).astype(np.int64) if return_lsnr else None
-    lz = torch.empty(int(ln.sum()) if return_lsnr else 0, dtype=torch.float32, pin_memory=pin)
-    check(_lib.lib().dfb_enhance_ragged_ex_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
-                                                lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
-                                                out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
-                                                groups.size if groups is not None else 0, reduce, srates.ctypes.data,
-                                                stab.ctypes.data if stab is not None else None, lens.size,
-                                                lz.data_ptr() if return_lsnr else None, lz.numel(),
-                                                l_off.ctypes.data if return_lsnr else None))
+    ln = l_off = lz = None
+    if return_lsnr:
+        ln = ragged.lsnr_lens(lens, srates, df_state.hop_size(), pad)
+        l_off = np.concatenate(([0], np.cumsum(ln)[:-1])).astype(np.int64)
+        lz = torch.empty(int(ln.sum()), dtype=torch.float32, pin_memory=pin)
+    check(_lib.lib().dfb_enhance_ragged_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
+                                             lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
+                                             out_off.ctypes.data, _ptr(groups), groups.size if groups is not None else 0, reduce,
+                                             srates.ctypes.data, _ptr(stab), lens.size, _ptr(lz), lz.numel() if lz is not None else 0,
+                                             _ptr(l_off)))
     if not return_lsnr:
         return outs
     lsnrs, k = [], 0
@@ -278,7 +277,7 @@ def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pa
     one length, and they share one ERB mask; each group's rows equal :func:`enhance` of that recording with the same
     ``reduce_mask``.
     ``sr``: the rows' sample rate, one for all or one per row (a link group's rows at one rate), as :func:`enhance_batch`
-    takes it; lengths and the result are in each row's own samples (dfb_enhance_ragged_rates).
+    takes it; lengths and the result are in each row's own samples (dfb_enhance_ragged).
     ``atten_lim_db`` / ``post_filter_beta`` / ``lsnr_thresholds``: as :func:`enhance_batch` takes them, one per row where
     per entry (a link group's rows take one setting).  ``return_lsnr``: the result is ``(out, lsnr, lsnr_lengths)``, lsnr a
     [B, max n] float32 CUDA tensor whose row b holds lsnr_lengths[b] values (NaN after them), as enhance_batch's."""
@@ -308,27 +307,18 @@ def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pa
           or not out.is_contiguous()):
         raise ValueError(f"out must be a contiguous float32 CUDA tensor of shape {(b, ow)} on {audio.device}")
     lim = abs(float(atten_lim_db)) if atten_lim_db is not None and tab is None else 0.0
-    if tab is None and not return_lsnr:
-        with torch.cuda.device(audio.device):
-            stream = torch.cuda.current_stream(audio.device).cuda_stream
-            check(_lib.lib().dfb_enhance_ragged_rates(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
-                                                      lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow,
-                                                      out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
-                                                      groups.size if groups is not None else 0, reduce, rates.ctypes.data, stream))
-        return out
-    ln = ragged.lsnr_lens(lens, rates, df_state.hop_size(), pad)
-    nl = int(ln.max())
-    lz = torch.full((b, nl), float("nan"), dtype=torch.float32, device=audio.device) if return_lsnr else None
-    l_off = np.arange(b, dtype=np.int64) * nl
+    ln = l_off = lz = None
+    if return_lsnr:
+        ln = ragged.lsnr_lens(lens, rates, df_state.hop_size(), pad)
+        nl = int(ln.max())
+        lz = torch.full((b, nl), float("nan"), dtype=torch.float32, device=audio.device)
+        l_off = np.arange(b, dtype=np.int64) * nl
     with torch.cuda.device(audio.device):
         stream = torch.cuda.current_stream(audio.device).cuda_stream
-        check(_lib.lib().dfb_enhance_ragged_ex(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
-                                               lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow,
-                                               out_off.ctypes.data, groups.ctypes.data if groups is not None else None,
-                                               groups.size if groups is not None else 0, reduce, rates.ctypes.data,
-                                               tab.ctypes.data if tab is not None else None, b,
-                                               lz.data_ptr() if return_lsnr else None, b * nl,
-                                               l_off.ctypes.data if return_lsnr else None, stream))
+        check(_lib.lib().dfb_enhance_ragged(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
+                                            lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow, out_off.ctypes.data,
+                                            _ptr(groups), groups.size if groups is not None else 0, reduce, rates.ctypes.data,
+                                            _ptr(tab), b, _ptr(lz), lz.numel() if lz is not None else 0, _ptr(l_off), stream))
     return (out, lz, torch.from_numpy(ln)) if return_lsnr else out
 
 

@@ -66,7 +66,7 @@ def packed_layout(shapes: Sequence[Tuple[int, int]], hop: int, pad: bool, rates=
     return lens, in_off, out_off, int(lens.sum()), int(olens.sum()), slices, np.ascontiguousarray(np.array(srates, dtype=np.int32))
 
 
-# Linked channels (dfb_enhance_ragged_linked): the channels of one recording share one ERB mask, reduced over them.
+# Linked channels (dfb_enhance_ragged's link groups): the channels of one recording share one ERB mask, reduced over them.
 # Numbering of dfb_reduce_mask and of the Rust runtime's ReduceMask / --reduce-mask (libDF/src/tract.rs:95-99).
 REDUCE_MASK = {"none": 0, "max": 1, "mean": 2}
 
@@ -105,7 +105,7 @@ def packed_groups(shapes: Sequence[Tuple[int, int]]) -> np.ndarray:
     return np.ascontiguousarray(np.array([int(shp[0]) for shp in shapes], dtype=np.int64))
 
 
-# Rated batches (dfb_enhance_ragged_rates): every stream at its own sample rate, resampled to and from the model's 48 kHz
+# Rated batches (dfb_enhance_ragged's rates): every stream at its own sample rate, resampled to and from the model's 48 kHz
 # with io.resample's sinc_fast taps.  A rate is supported when its two gcd-reduced tap tables hold at most MAX_RATE_TAPS
 # floats together.
 MODEL_SR = 48000
@@ -182,7 +182,7 @@ def lsnr_lens(lens: np.ndarray, rates, hop: int, pad: bool) -> np.ndarray:
     return -(-o48 // hop)
 
 
-# Per-entry settings of the batch calls (dfb_enhance_ragged_ex): the layout of dfb_enhance_settings
+# Per-entry settings of the batch calls (dfb_enhance_ragged's settings): the layout of dfb_enhance_settings
 SETTINGS_DTYPE = np.dtype([("atten_lim_db", "<f4"), ("post_filter_beta", "<f4"), ("lsnr_gating", "<i4"),
                            ("min_db_thresh", "<f4"), ("max_db_erb_thresh", "<f4"), ("max_db_df_thresh", "<f4")])
 
@@ -250,7 +250,7 @@ def settings_table(n: int, atten_lim_db, post_filter_beta, lsnr_thresholds, defa
 
 
 def check_settings_model(model: str, nb_erb: int, nb_df: int, df_order: int, tab, return_lsnr: bool) -> None:
-    """The combinations dfb_enhance_ragged_ex refuses with DFB_ERR_UNSUPPORTED, refused before the library is called
+    """The combinations dfb_enhance_ragged refuses with DFB_ERR_UNSUPPORTED, refused before the library is called
     (DfbError): a settings table needs the specialised apply kernel (df_order 5, nb_df 96, 32 ERB bands) and not DeepFilterNet
     v1; a beta > 0 or gating needs a DeepFilterNet3 topology; DeepFilterNet v1 returns no LSNR rows."""
     from ._lib import DFB_ERR_UNSUPPORTED, DfbError

@@ -191,50 +191,6 @@ int dfb_enhance_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t 
                      float atten_lim_db, float *h_out);
 /* output length of dfb_enhance for a given input length */
 int64_t dfb_enhance_out_len(const dfb_state *st, int64_t T, int pad);
-/* A batch of B streams of different lengths: stream b is lengths[b] samples at audio + in_offsets[b]; its result,
- * dfb_enhance_out_len(st, lengths[b], pad) samples, goes to out + out_offsets[b].  Nothing else in `out` is written.
- * in_offsets / lengths / out_offsets are HOST arrays; in_numel / out_numel bound them (DFB_ERR_INVALID when a stream
- * reaches outside, has a length <= 0, or has no frame: shorter than one hop with pad == 0).  Every stream's output equals
- * dfb_enhance of that stream alone (fp32 reduction order aside) -- which zero-padding the batch to its longest stream
- * does not give: the padded frames would change the look-ahead of every shorter stream's last frames.
- * Offsets cover a padded [B, S] tensor (in_offsets[b] = b * S) as well as streams packed back to back.  The streams run
- * longest first; a time chunk computes only the streams that have frames left in it, so a batch of mixed lengths costs
- * about its true frame count, not B times the longest.  DeepFilterNet v1 (one window per signal) runs streams of the
- * same frame count together, so a batch of v1 streams saves no frames.
- * The _host variant takes host pointers (page-locked memory lets its copies overlap the compute), copies only the
- * streams' own samples and results, stages one stream group at a time on the device, and is synchronous. */
-int dfb_enhance_ragged(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
-                       const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
-                       const int64_t *out_offsets, void *stream);
-int dfb_enhance_ragged_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel, const int64_t *in_offsets,
-                            const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *h_out, int64_t out_numel,
-                            const int64_t *out_offsets);
-/* Linked channels: the Rust runtime's mask reduction over the channels of one recording (libDF/src/tract.rs:95-99,
- * 868-902; the default of its LADSPA plugin and, as --reduce-mask, of its deep-filter binary).  A link group is C >= 1
- * streams of one length, the channels of one recording.  Everything up to the model outputs stays per channel (STFT,
- * features and their normalisation, encoder, GRU states, m_c, coefs_c, lsnr_c).  The ERB mask is then shared:
- *   max:  m[t][e] = max_c m_c[t][e]
- *   mean: m[t][e] = (sum_c m_c[t][e], fp32 in channel order) * fl32(1 / C)
- * and every channel's apply stage uses it wherever it uses its own mask: the ERB gains (bins >= nb_df, or all bins with
- * mask_only), DeepFilterNet2's masked spectrum that feeds its deep filter, and DeepFilterNet2's post filter on the gains.
- * The deep-filter coefficients, DeepFilterNet3's post filter, the attenuation limit and the ISTFT stay per channel.
- * LSNR stage gating (streaming, DeepFilterNet3) makes one decision per group and frame, from the LSNR of the group's
- * FIRST channel: this library's reading of the single scalar the Rust runtime takes from its [ch] LSNR output.
- * With DFB_REDUCE_NONE, or groups of one stream, the result is the unlinked one.
- * DeepFilterNet3, DeepFilterNet3_ll and DeepFilterNet2; DeepFilterNet v1 with a group of C > 1 is DFB_ERR_UNSUPPORTED. */
-typedef enum { DFB_REDUCE_NONE = 0, DFB_REDUCE_MAX = 1, DFB_REDUCE_MEAN = 2 } dfb_reduce_mask;  /* tract.rs:95-99 */
-/* dfb_enhance_ragged(_host) with link groups: group g is the next group_sizes[g] streams in the caller's order
- * (group_sizes is a HOST array of n_groups entries summing to B; DFB_ERR_INVALID otherwise, or when a group's streams differ
- * in length).  A group is never split across stream groups: DFB_ERR_OOM when the workspace cap (dfb_model_set_max_workspace)
- * cannot hold the largest one. */
-int dfb_enhance_ragged_linked(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
-                              const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
-                              const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
-                              void *stream);
-int dfb_enhance_ragged_linked_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel,
-                                   const int64_t *in_offsets, const int64_t *lengths, int64_t B, int pad, float atten_lim_db,
-                                   float *h_out, int64_t out_numel, const int64_t *out_offsets, const int64_t *group_sizes,
-                                   int64_t n_groups, int reduce_mask);
 /* Rated batches: streams at their own sample rates, resampled to and from 48 kHz on the device (DESIGN.md section 5i).
  * dfb_model_add_rate registers rate r on the model, with the arguments of dfb_stream_add_slot_rate: up_taps / down_taps
  * [nw][2 width + og] (HOST arrays) are io.resample_kernel(r, 48000) / (48000, r) with the sinc_fast parameters, og / nw the
@@ -244,73 +200,105 @@ int dfb_enhance_ragged_linked_host(dfb_model *m, dfb_state *st, const float *h_a
  * Synchronises the model's device. */
 int dfb_model_add_rate(dfb_model *m, int rate, const float *up_taps, int up_og, int up_nw, int up_width,
                        const float *down_taps, int down_og, int down_nw, int down_width);
-/* dfb_enhance_ragged_linked(_host) with a HOST array rates[B]: stream b is lengths[b] samples at rates[b] Hz (48000 or a
- * registered rate), and lengths, offsets and in_numel / out_numel count each stream's own samples.  group_sizes may be null
- * (no links); a link group has one rate and one length.  Stream b's result, dfb_enhance_out_len_at(st, lengths[b], pad,
+/* Ragged batch: B streams of different lengths in one call, optionally linked, at their own rates, with per-stream
+ * settings and LSNR rows (DESIGN.md sections 5b, 5i, 5k).  group_sizes, rates, settings and d_lsnr / h_lsnr may each be
+ * null, which turns that part off.
+ *
+ * Layout.  Stream b is lengths[b] samples at audio + in_offsets[b]; its result, dfb_enhance_out_len(st, lengths[b], pad)
+ * samples, goes to out + out_offsets[b].  Nothing else in `out` is written.  in_offsets / lengths / out_offsets are HOST
+ * arrays; in_numel / out_numel bound them.  Every stream's output equals dfb_enhance of that stream alone (fp32 reduction
+ * order aside) -- which zero-padding the batch to its longest stream does not give: the padded frames would change the
+ * look-ahead of every shorter stream's last frames.  Offsets cover a padded [B, S] tensor (in_offsets[b] = b * S) as well as
+ * streams packed back to back.  The streams run longest first; a time chunk computes only the streams that have frames left
+ * in it, so a batch of mixed lengths costs about its true frame count, not B times the longest.  DeepFilterNet v1 (one
+ * window per signal) runs streams of the same frame count together, so a batch of v1 streams saves no frames.  The _host
+ * variant takes host pointers (page-locked memory lets its copies overlap the compute), copies only the streams' own samples
+ * and results, stages one stream group at a time on the device, and is synchronous.
+ *
+ * Link groups (group_sizes null: no links, and reduce_mask is ignored).  Linked channels: the Rust runtime's mask reduction
+ * over the channels of one recording (libDF/src/tract.rs:95-99, 868-902; the default of its LADSPA plugin and, as
+ * --reduce-mask, of its deep-filter binary).  A link group is C >= 1 streams of one length, the channels of one recording:
+ * group g is the next group_sizes[g] streams in the caller's order (group_sizes is a HOST array of n_groups entries summing
+ * to B).  Everything up to the model outputs stays per channel (STFT, features and their normalisation, encoder, GRU
+ * states, m_c, coefs_c, lsnr_c).  The ERB mask is then shared:
+ *   max:  m[t][e] = max_c m_c[t][e]
+ *   mean: m[t][e] = (sum_c m_c[t][e], fp32 in channel order) * fl32(1 / C)
+ * and every channel's apply stage uses it wherever it uses its own mask: the ERB gains (bins >= nb_df, or all bins with
+ * mask_only), DeepFilterNet2's masked spectrum that feeds its deep filter, and DeepFilterNet2's post filter on the gains.
+ * The deep-filter coefficients, DeepFilterNet3's post filter, the attenuation limit and the ISTFT stay per channel.
+ * LSNR stage gating (streaming, DeepFilterNet3) makes one decision per group and frame, from the LSNR of the group's
+ * FIRST channel: this library's reading of the single scalar the Rust runtime takes from its [ch] LSNR output.
+ * With DFB_REDUCE_NONE, or groups of one stream, the result is the unlinked one.  A group is never split across stream
+ * groups.  DeepFilterNet3, DeepFilterNet3_ll and DeepFilterNet2.
+ *
+ * Rates (rates null: every stream at 48 kHz).  With a HOST array rates[B], stream b is lengths[b] samples at rates[b] Hz
+ * (48000 or a registered rate, dfb_model_add_rate), and lengths, offsets and in_numel / out_numel count each stream's own
+ * samples.  A link group has one rate and one length.  Stream b's result, dfb_enhance_out_len_at(st, lengths[b], pad,
  * rates[b]) samples at out + out_offsets[b], is
  *     io.resample(enhance(io.resample(x_b, r_b, 48000), pad, atten_lim_db), 48000, r_b)
  * with io.resample's sinc_fast taps: the 48 kHz signal the analysis reads and the rate-r output are those of io.resample
  * (k_resample's sums) bit for bit, and the enhancement between them is that of the ragged batch (fp32 reduction order
- * aside).  A 48 kHz stream is enhanced as in dfb_enhance_ragged, untouched by any resampler.  Only rate-r samples cross
- * PCIe in the _host variant, whose copies overlap the compute as dfb_enhance_ragged_host's do.  DFB_ERR_INVALID for an
- * unregistered rate, mixed rates or lengths in a link group, a stream with no frame at 48 kHz when pad == 0, or a stream
- * that reaches outside in_numel / out_numel. */
-int dfb_enhance_ragged_rates(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
-                             const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
-                             const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
-                             const int32_t *rates, void *stream);
-int dfb_enhance_ragged_rates_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel, const int64_t *in_offsets,
-                                  const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *h_out, int64_t out_numel,
-                                  const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
-                                  const int32_t *rates);
-/* output length of a stream of T samples at `rate` in a rated batch: ceil(out48 rate / 48000), out48 =
- * dfb_enhance_out_len(st, ceil(T 48000 / rate), pad); -1 for a null state, T <= 0 or rate <= 0 */
-int64_t dfb_enhance_out_len_at(const dfb_state *st, int64_t T, int pad, int rate);
-/* Per-stream settings and LSNR rows of a ragged batch (DESIGN.md section 5k): dfb_enhance_ragged_rates(_host) with rates and
- * group_sizes both optional (null: every stream at 48 kHz / no links), plus
- *   settings / n_settings: one dfb_enhance_settings per stream, in the caller's order (n_settings == B), or null: every stream
- *     takes atten_lim_db, the model's post filter and no gating, as in the other dfb_enhance_ragged* calls.  With a table,
- *     atten_lim_db is ignored and stream b takes:
- *       atten_lim_db       the rule of the other calls: <= 0 turns the limit off, else lim = 10^(-db / 20); NaN is invalid;
- *       post_filter_beta   the DeepFilterNet3 post filter (deepfilternet3.py:448-454) with this beta, finite and >= 0,
- *                          0 = off, in place of the model's option (dfb_model_set_options); DeepFilterNet2's own post filter
- *                          on the ERB gains still follows the model's option;
- *       lsnr_gating != 0   LSNR stage gating (tract.rs:658-672 apply_stages, as dfb_stream_set_lsnr_thresholds) with the
- *                          three thresholds, none NaN.
- *     The streams of a link group take one setting: their entries must be equal.  Stream b's result equals that of the
- *     batch with stream b's entry given to every stream, bit for bit.
- *   d_lsnr / h_lsnr, lsnr_numel, lsnr_offsets (HOST array): null for no LSNR output; else stream b's LSNR row,
- *     dfb_enhance_lsnr_len(st, lengths[b], pad, rates[b]) floats in dB, goes to lsnr + lsnr_offsets[b].  Value j is the
- *     LSNR of the 48 kHz STFT frame that 10 ms output hop j carries: DfNet.forward's lsnr[j + 1] of the stream alone with
- *     pad != 0 (the output drops the first fft - hop = 480 samples, frame 0's head), lsnr[j] with pad == 0.  The frames
- *     are those of the 48 kHz signal at every rate, so a stream at rate r has one value per 10 ms of its output, the last
- *     one for the hop its output's last partial hop falls in.  This is the rule of dfb_stream_process_lsnr: hop j carries
- *     frame f, and its value is that frame's LSNR, the one gating reads.
- * Both run on the specialised apply kernel: a table needs df_order 5, nb_df 96 and 32 ERB bands (every shipped model);
- * post_filter_beta > 0 and lsnr_gating need a DeepFilterNet3 topology; DeepFilterNet v1 takes neither a table nor LSNR
- * rows.  Everything else is DFB_ERR_UNSUPPORTED.  DFB_ERR_INVALID for n_settings != B, a NaN limit or threshold, a beta
- * < 0 or not finite, linked streams whose entries differ, LSNR rows without offsets or outside lsnr_numel, and everything
- * the rated call refuses.  Gating selects what is applied to a frame, as on streaming handles: the network runs every
- * frame (the Rust runtime skips its decoders on gated frames; see DESIGN.md section 5k).  A refused call changes nothing.
- * With settings and d_lsnr both null this is the call it extends, launch for launch.  The _host variant copies the LSNR
- * rows back chunk by chunk, next to the audio. */
+ * aside).  A 48 kHz stream is enhanced as with rates null, untouched by any resampler.  Only rate-r samples cross PCIe in
+ * the _host variant, whose copies overlap the compute as they do at 48 kHz.
+ *
+ * Settings (settings null: every stream takes atten_lim_db, the model's post filter and no gating).  settings / n_settings:
+ * one dfb_enhance_settings per stream, in the caller's order (n_settings == B).  With a table, atten_lim_db is ignored and
+ * stream b takes:
+ *   atten_lim_db       the rule of the atten_lim_db argument: <= 0 turns the limit off, else lim = 10^(-db / 20); NaN is
+ *                      invalid;
+ *   post_filter_beta   the DeepFilterNet3 post filter (deepfilternet3.py:448-454) with this beta, finite and >= 0,
+ *                      0 = off, in place of the model's option (dfb_model_set_options); DeepFilterNet2's own post filter
+ *                      on the ERB gains still follows the model's option;
+ *   lsnr_gating != 0   LSNR stage gating (tract.rs:658-672 apply_stages, as dfb_stream_set_lsnr_thresholds) with the
+ *                      three thresholds, none NaN.
+ * The streams of a link group take one setting: their entries must be equal.  Stream b's result equals that of the batch
+ * with stream b's entry given to every stream, bit for bit.  Gating selects what is applied to a frame, as on streaming
+ * handles: the network runs every frame (the Rust runtime skips its decoders on gated frames; see DESIGN.md section 5k).
+ *
+ * LSNR rows (d_lsnr / h_lsnr null: no LSNR output).  lsnr_offsets is a HOST array: stream b's LSNR row,
+ * dfb_enhance_lsnr_len(st, lengths[b], pad, rates[b]) floats in dB, goes to lsnr + lsnr_offsets[b].  Value j is the LSNR of
+ * the 48 kHz STFT frame that 10 ms output hop j carries: DfNet.forward's lsnr[j + 1] of the stream alone with pad != 0 (the
+ * output drops the first fft - hop = 480 samples, frame 0's head), lsnr[j] with pad == 0.  The frames are those of the
+ * 48 kHz signal at every rate, so a stream at rate r has one value per 10 ms of its output, the last one for the hop its
+ * output's last partial hop falls in.  This is the rule of dfb_stream_process_lsnr: hop j carries frame f, and its value is
+ * that frame's LSNR, the one gating reads.  The _host variant copies the LSNR rows back chunk by chunk, next to the audio.
+ *
+ * A table and LSNR rows run on the specialised apply kernel: a table needs df_order 5, nb_df 96 and 32 ERB bands (every
+ * shipped model); post_filter_beta > 0 and lsnr_gating need a DeepFilterNet3 topology; DeepFilterNet v1 takes neither a
+ * table nor LSNR rows.
+ *
+ * Errors.  A refused call changes nothing.
+ *   DFB_ERR_INVALID      a null model, state, audio, out or layout array; a stream that reaches outside in_numel /
+ *                        out_numel, has a length <= 0, or has no frame at 48 kHz (shorter than one hop with pad == 0); an
+ *                        unregistered rate; group sizes < 1, above 65535 or not summing to B, a reduce_mask other than
+ *                        DFB_REDUCE_*, or a link group whose streams differ in rate or length; n_settings != B, a NaN limit
+ *                        or threshold, a beta < 0 or not finite, linked streams whose entries differ; LSNR rows without
+ *                        offsets or outside lsnr_numel.
+ *   DFB_ERR_UNSUPPORTED  a state other than 960 / 480; DeepFilterNet v1 with a link group of C > 1 (max / mean), a table
+ *                        or LSNR rows; a table on a model shape other than the one above; a beta > 0 or gating on a
+ *                        topology other than DeepFilterNet3.
+ *   DFB_ERR_OOM          the workspace cap (dfb_model_set_max_workspace) cannot hold the largest link group. */
+typedef enum { DFB_REDUCE_NONE = 0, DFB_REDUCE_MAX = 1, DFB_REDUCE_MEAN = 2 } dfb_reduce_mask;  /* tract.rs:95-99 */
 typedef struct {
     float atten_lim_db;
     float post_filter_beta;
     int32_t lsnr_gating;
     float min_db_thresh, max_db_erb_thresh, max_db_df_thresh;
 } dfb_enhance_settings;
-int dfb_enhance_ragged_ex(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
-                          const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
-                          const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
-                          const int32_t *rates, const dfb_enhance_settings *settings, int64_t n_settings, float *d_lsnr,
-                          int64_t lsnr_numel, const int64_t *lsnr_offsets, void *stream);
-int dfb_enhance_ragged_ex_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel, const int64_t *in_offsets,
-                               const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *h_out, int64_t out_numel,
-                               const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
-                               const int32_t *rates, const dfb_enhance_settings *settings, int64_t n_settings, float *h_lsnr,
-                               int64_t lsnr_numel, const int64_t *lsnr_offsets);
-/* LSNR values of a stream of T samples at `rate` in dfb_enhance_ragged_ex: ceil(out48 / 480), out48 =
+int dfb_enhance_ragged(dfb_model *m, dfb_state *st, const float *d_audio, int64_t in_numel, const int64_t *in_offsets,
+                       const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *d_out, int64_t out_numel,
+                       const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
+                       const int32_t *rates, const dfb_enhance_settings *settings, int64_t n_settings, float *d_lsnr,
+                       int64_t lsnr_numel, const int64_t *lsnr_offsets, void *stream);
+int dfb_enhance_ragged_host(dfb_model *m, dfb_state *st, const float *h_audio, int64_t in_numel, const int64_t *in_offsets,
+                            const int64_t *lengths, int64_t B, int pad, float atten_lim_db, float *h_out, int64_t out_numel,
+                            const int64_t *out_offsets, const int64_t *group_sizes, int64_t n_groups, int reduce_mask,
+                            const int32_t *rates, const dfb_enhance_settings *settings, int64_t n_settings, float *h_lsnr,
+                            int64_t lsnr_numel, const int64_t *lsnr_offsets);
+/* output length of a stream of T samples at `rate` in a rated batch: ceil(out48 rate / 48000), out48 =
+ * dfb_enhance_out_len(st, ceil(T 48000 / rate), pad); -1 for a null state, T <= 0 or rate <= 0 */
+int64_t dfb_enhance_out_len_at(const dfb_state *st, int64_t T, int pad, int rate);
+/* LSNR values of a stream of T samples at `rate` in dfb_enhance_ragged: ceil(out48 / 480), out48 =
  * dfb_enhance_out_len(st, ceil(T 48000 / rate), pad) (T at 48 kHz); -1 for a null state, T <= 0 or rate <= 0 */
 int64_t dfb_enhance_lsnr_len(const dfb_state *st, int64_t T, int pad, int rate);
 /* Debug aid: one of a model's offline resamplers (up != 0: rate -> 48 kHz, else 48 kHz -> rate) alone over B rows (B <= 65535):
@@ -354,7 +342,7 @@ int dfb_stream_set_lsnr_thresholds(dfb_stream *s, int enable, float min_db_thres
  * return it to the handle's setting.  A refused call changes nothing. */
 int dfb_stream_set_lsnr_thresholds_slots(dfb_stream *s, const int64_t *slots, int64_t n, int enable, float min_db_thresh,
                                          float max_db_erb_thresh, float max_db_df_thresh);
-/* Linked channels (see dfb_enhance_ragged_linked): streams g * channels + c form link group g; B % channels == 0.
+/* Linked channels (see dfb_enhance_ragged's link groups): streams g * channels + c form link group g; B % channels == 0.
  * Only on a new or reset handle (DFB_ERR_INVALID after the first frame: the frame re-synthesised for the overlap-add
  * tail would mix two settings) that has had no slot operation (DFB_ERR_UNSUPPORTED).  channels = 1 or DFB_REDUCE_NONE:
  * unlinked (the default); channels = 1 also records reduce_mask as the reduction of the slot groups that
@@ -556,7 +544,7 @@ int dfb_debug_resample_slots(int up, const dfb_stream *s, const int32_t *h_rates
  *   1  otherwise                   network gains and coefs
  * On a mask_only model stage 1 is stage 2.  Where the Rust runtime returns NULL for a skipped output, the values here are
  * defined, so a caller can apply every row as it comes.  Linked channels: each member's gains are the group's reduced mask
- * (max / mean as dfb_enhance_ragged_linked); coefs and LSNR stay per channel. */
+ * (max / mean as dfb_enhance_ragged's link groups); coefs and LSNR stay per channel. */
 int dfb_stream_create_spec(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B);
 int dfb_stream_process_spec(dfb_stream *s, const float *d_spec, int64_t n_frames, float *d_gains, float *d_coefs,
                             float *d_lsnr, int8_t *d_stage, void *stream);

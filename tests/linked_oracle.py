@@ -1,4 +1,4 @@
-"""CPU restatement of linked channels (include/dfb200.h, dfb_enhance_ragged_linked) on top of the oracle's building blocks
+"""CPU restatement of linked channels (include/dfb200.h, dfb_enhance_ragged's link groups) on top of the oracle's building blocks
 (oracle/dfnet_oracle.py, which itself stays the plain reference forward pass).
 
 The channels of one recording run through the network as a batch, each with its own features, states and outputs; the

@@ -1,4 +1,4 @@
-"""GPU: linked channels (dfb_enhance_ragged_linked, dfb_stream_set_mask_reduce).  The channels of a recording share one ERB
+"""GPU: linked channels (dfb_enhance_ragged's link groups, dfb_stream_set_mask_reduce).  The channels of a recording share one ERB
 mask, the max or mean of theirs; everything else stays per channel.  Checked against the CPU restatement
 (tests/linked_oracle.py), against the unlinked path where linking must change nothing, and against each recording
 enhanced alone, whatever the batch order, time chunking, lanes and stream groups."""
@@ -230,8 +230,9 @@ def test_host_device_and_batch_entry_points(states):
     stream = torch.cuda.current_stream().cuda_stream
     for g, red in (([2], 1), ([1, 2], 1), ([1, 1], 3)):
         g = np.array(g, np.int64)
-        rc = L.dfb_enhance_ragged_linked(model.handle, st.handle, src.data_ptr(), 9603, off.ctypes.data, lens.ctypes.data, 2, 1, 0.0,
-                                         dst.data_ptr(), 9603, off.ctypes.data, g.ctypes.data, g.size, red, stream)
+        rc = L.dfb_enhance_ragged(model.handle, st.handle, src.data_ptr(), 9603, off.ctypes.data, lens.ctypes.data, 2, 1, 0.0,
+                                  dst.data_ptr(), 9603, off.ctypes.data, g.ctypes.data, g.size, red, None, None, 0, None, 0, None,
+                                  stream)
         assert rc == _lib.DFB_ERR_INVALID, (g, red)
 
 

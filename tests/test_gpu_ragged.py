@@ -182,8 +182,9 @@ def test_layouts_order_and_untouched_output(states):
     out_off = np.array([7, 5000, 7000], np.int64)
     out_d = torch.full((40000,), 7.0, device="cuda")
     stream = torch.cuda.current_stream().cuda_stream
+    no_extras = (None, 0, 0, None, None, 0, None, 0, None)   # no link groups, rates, settings or LSNR rows
     _lib.check(L.dfb_enhance_ragged(model.handle, st.handle, src.data_ptr(), src.numel(), in_off.ctypes.data, lens.ctypes.data, 3, 1,
-                                    0.0, out_d.data_ptr(), out_d.numel(), out_off.ctypes.data, stream))
+                                    0.0, out_d.data_ptr(), out_d.numel(), out_off.ctypes.data, *no_extras, stream))
     out = out_d.cpu()
     mask = torch.ones(40000, dtype=torch.bool)
     for o, t, i in zip(out_off, lens, in_off):
@@ -195,7 +196,7 @@ def test_layouts_order_and_untouched_output(states):
     for io_, oo_, n_in, n_out in ((in_off, out_off, int(in_off[-1] + lens[-1] - 1), 40000), (in_off, out_off, src.numel(), 36999),
                                   (np.array([-1, 0, 0], np.int64), out_off, src.numel(), 40000)):
         rc = L.dfb_enhance_ragged(model.handle, st.handle, src.data_ptr(), n_in, io_.ctypes.data, lens.ctypes.data, 3, 1, 0.0,
-                                  out_d.data_ptr(), n_out, oo_.ctypes.data, stream)
+                                  out_d.data_ptr(), n_out, oo_.ctypes.data, *no_extras, stream)
         assert rc == _lib.DFB_ERR_INVALID
 
 

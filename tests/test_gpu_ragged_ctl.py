@@ -1,9 +1,7 @@
-"""GPU: per-entry settings and LSNR rows of ragged batches (dfb_enhance_ragged_ex, enhance_batch / enhance_device_ragged
+"""GPU: per-entry settings and LSNR rows of ragged batches (dfb_enhance_ragged, enhance_batch / enhance_device_ragged
 with per-entry atten_lim_db / post_filter_beta / lsnr_thresholds and return_lsnr) and per-slot LSNR thresholds
 (DfStream.set_lsnr_thresholds(slots=...)).
 
-* Without a table and LSNR rows the new entry point is each of the six existing ragged calls, bit for bit and launch for
-  launch.
 * Entry i of a batch with mixed settings equals entry i of the same batch with entry i's settings given to every entry
   (bit for bit), and the entry enhanced alone by enhance() with those settings (RMS, as the other ragged tests).
 * Gating: forced stages reproduce each stage's definition; mixed stages equal the float restatement of apply_stages on
@@ -78,61 +76,6 @@ def entries(seed):
     for i, (s, r, c) in enumerate(zip(secs, rates, chans)):
         out.append(synth_audio(c, int(s * r) + 7 * i, seed=seed + i, sr=r))
     return out, rates
-
-
-# ------------------------------------------------------------------ the new entry point without extras ----
-def _table_ptr(tab):
-    return tab.ctypes.data if tab is not None else None
-
-
-def test_ex_without_extras_equals_existing_calls(st):
-    """dfb_enhance_ragged_ex with no table and no LSNR output is each of the six dfb_enhance_ragged* calls, bit for bit and
-    with the same dfb_kernel_launches() count."""
-    L = _lib.lib()
-    model = model_of(st, "dfn3")
-    lens = np.array([48000 + 17, 9600, 24000 * 3 + 5, 4801], dtype=np.int64)
-    rates = np.array([48000, 16000, 48000, 16000], dtype=np.int32)
-    in_off = np.concatenate(([0], np.cumsum(lens)[:-1])).astype(np.int64)
-    olen = ragged._out_lens(lens, rates, HOP, True)
-    out_off = np.concatenate(([0], np.cumsum(olen)[:-1])).astype(np.int64)
-    n_in, n_out = int(lens.sum()), int(olen.sum())
-    groups = np.array([2, 1, 1], dtype=np.int64)
-    lens_l = lens.copy(); lens_l[1] = lens_l[0]           # a link group has one length
-    x = synth_audio(1, max(n_in, int(lens_l.sum())), seed=5)[0].contiguous()
-    in_off_l = np.concatenate(([0], np.cumsum(lens_l)[:-1])).astype(np.int64)
-    olen_l = ragged._out_lens(lens_l, 48000, HOP, True)
-    out_off_l = np.concatenate(([0], np.cumsum(olen_l)[:-1])).astype(np.int64)
-    model.add_rate(16000)
-    for host in (False, True):
-        for kind in ("ragged", "linked", "rates"):
-            lz, io_, oo, no = (lens_l, in_off_l, out_off_l, int(olen_l.sum())) if kind == "linked" else (lens, in_off, out_off, n_out)
-            ni = int(lz.sum()) if kind == "linked" else n_in
-            xin = x[:ni].contiguous() if host else x[:ni].cuda()
-            ys = [torch.zeros(no, device="cpu" if host else "cuda") for _ in range(2)]
-            g = groups.ctypes.data if kind == "linked" else None
-            ng = groups.size if kind == "linked" else 0
-            red = 2 if kind == "linked" else 0
-            r = rates.ctypes.data if kind == "rates" else None
-            counts = []
-            for i, y in enumerate(ys):
-                n0 = L.dfb_kernel_launches()
-                args = (model.handle, st.handle, xin.data_ptr(), ni, io_.ctypes.data, lz.ctypes.data, lz.size, 1, 6.0, y.data_ptr(), no,
-                        oo.ctypes.data)
-                if i == 0:
-                    if kind == "ragged":
-                        rc = (L.dfb_enhance_ragged_host(*args) if host else L.dfb_enhance_ragged(*args, None))
-                    elif kind == "linked":
-                        rc = (L.dfb_enhance_ragged_linked_host(*args, g, ng, red) if host else L.dfb_enhance_ragged_linked(*args, g, ng, red, None))
-                    else:
-                        rc = (L.dfb_enhance_ragged_rates_host(*args, None, 0, 0, r) if host else L.dfb_enhance_ragged_rates(*args, None, 0, 0, r, None))
-                else:
-                    ex = (g, ng, red, r, None, 0, None, 0, None)
-                    rc = L.dfb_enhance_ragged_ex_host(*args, *ex) if host else L.dfb_enhance_ragged_ex(*args, *ex, None)
-                _lib.check(rc)
-                torch.cuda.synchronize()
-                counts.append(L.dfb_kernel_launches() - n0)
-            assert torch.equal(ys[0].cpu(), ys[1].cpu()), (host, kind)
-            assert counts[0] == counts[1], (host, kind, counts)
 
 
 # ------------------------------------------------------------------ per-entry limit and beta ----
@@ -319,6 +262,10 @@ def test_per_slot_thresholds(st):
 
 
 # ------------------------------------------------------------------ refusals ----
+def _table_ptr(tab):
+    return tab.ctypes.data if tab is not None else None
+
+
 def test_refusals(st):
     """The combinations that are not built are refused with DFB_ERR_UNSUPPORTED, in Python and in the library, and a
     malformed table with DFB_ERR_INVALID; a refused call leaves the output untouched."""
@@ -351,10 +298,10 @@ def test_refusals(st):
 
     def call(model, tab, n_tab=2, groups=None, red=0, lsnr=False, lsnr_numel=60):
         g = np.asarray(groups, dtype=np.int64) if groups is not None else None
-        return L.dfb_enhance_ragged_ex_host(model.handle, st.handle, x.data_ptr(), 24000, in_off.ctypes.data, lens.ctypes.data, 2, 1,
-                                            0.0, y.data_ptr(), 24000, in_off.ctypes.data, g.ctypes.data if g is not None else None,
-                                            g.size if g is not None else 0, red, None, _table_ptr(tab), n_tab,
-                                            lz.data_ptr() if lsnr else None, lsnr_numel, lo.ctypes.data if lsnr else None)
+        return L.dfb_enhance_ragged_host(model.handle, st.handle, x.data_ptr(), 24000, in_off.ctypes.data, lens.ctypes.data, 2, 1,
+                                         0.0, y.data_ptr(), 24000, in_off.ctypes.data, g.ctypes.data if g is not None else None,
+                                         g.size if g is not None else 0, red, None, _table_ptr(tab), n_tab,
+                                         lz.data_ptr() if lsnr else None, lsnr_numel, lo.ctypes.data if lsnr else None)
 
     def tab_of(**kw):
         t = np.zeros(2, dtype=ragged.SETTINGS_DTYPE)

@@ -1,4 +1,4 @@
-"""GPU: rated ragged batches (enhance_batch / enhance_device_ragged with sr=, dfb_enhance_ragged_rates).  The offline
+"""GPU: rated ragged batches (enhance_batch / enhance_device_ragged with sr=, dfb_enhance_ragged with rates).  The offline
 resampler alone must be io.resample bit for bit over a ragged batch in any chunking, writing nothing outside its rows;
 every entry of a rated batch must equal io.resample(enhance(io.resample(a, r, 48000)), 48000, r) within the ragged
 path's bound; and the rated call must keep the batch path's invariants (device vs host, chunking, lanes, stream groups,
@@ -227,8 +227,8 @@ def test_48k_calls_are_unchanged(st, dfn3):
     d0 = enhance_device_ragged(model, st, x, lens)
     assert torch.equal(enhance_device_ragged(model, st, x, lens, sr=48000), d0)
     assert torch.equal(enhance(model, st, a[0], sr=48000), enhance(model, st, a[0]))
-    # every ragged entry point on one packed batch: a rated call at 48 kHz is the plain or linked call, and a linked call
-    # with groups of one the plain call, bit for bit and in as many launches
+    # one packed batch through dfb_enhance_ragged(_host): rates all 48 kHz are rates null, with or without link groups, and
+    # link groups of one are groups null, bit for bit and in as many launches
     L = _lib.lib()
     i64 = lambda v: np.ascontiguousarray(np.asarray(v, np.int64))   # noqa: E731
     lens = i64([30000, 30000, 4801, 12345, 12345, 12345])
@@ -237,21 +237,21 @@ def test_48k_calls_are_unchanged(st, dfn3):
     x = synth_audio(1, n, seed=642)[0].contiguous()
     stream = torch.cuda.current_stream().cuda_stream
 
-    def run(dev, name, *tail):
+    def run(dev, g=None, n_groups=0, reduce=0, rates=None):
         src, out = (x.cuda(), torch.zeros(n, device="cuda")) if dev else (x, torch.zeros(n))
         n0 = L.dfb_kernel_launches()
-        _lib.check(getattr(L, name if dev else name + "_host")(model.handle, st.handle, src.data_ptr(), n, off.ctypes.data,
-                                                             lens.ctypes.data, 6, 1, 0.0, out.data_ptr(), n, off.ctypes.data,
-                                                             *tail, *((stream,) if dev else ())))
+        args = (model.handle, st.handle, src.data_ptr(), n, off.ctypes.data, lens.ctypes.data, 6, 1, 0.0, out.data_ptr(), n,
+                off.ctypes.data, g, n_groups, reduce, rates, None, 0, None, 0, None)
+        _lib.check(L.dfb_enhance_ragged(*args, stream) if dev else L.dfb_enhance_ragged_host(*args))
         return out.cpu(), L.dfb_kernel_launches() - n0
 
     for dev in (True, False):
-        plain = run(dev, "dfb_enhance_ragged")
-        linked = run(dev, "dfb_enhance_ragged_linked", groups.ctypes.data, 3, 2)
+        plain = run(dev)
+        linked = run(dev, groups.ctypes.data, 3, 2)
         assert not torch.equal(linked[0], plain[0]), dev
-        for got, ref in ((run(dev, "dfb_enhance_ragged_rates", None, 0, 0, r48.ctypes.data), plain),
-                         (run(dev, "dfb_enhance_ragged_linked", ones.ctypes.data, 6, 2), plain),
-                         (run(dev, "dfb_enhance_ragged_rates", groups.ctypes.data, 3, 2, r48.ctypes.data), linked)):
+        for got, ref in ((run(dev, rates=r48.ctypes.data), plain),
+                         (run(dev, ones.ctypes.data, 6, 2), plain),
+                         (run(dev, groups.ctypes.data, 3, 2, r48.ctypes.data), linked)):
             assert torch.equal(got[0], ref[0]) and got[1] == ref[1], (dev, got[1], ref[1])
 
 
@@ -286,9 +286,9 @@ def test_errors(st, dfn3):
     for rates, groups in (([16000, 12345], None), ([16000, 8000], g)):
         model.add_rate(8000)
         r32 = np.ascontiguousarray(np.asarray(rates, np.int32))
-        rc = _lib.lib().dfb_enhance_ragged_rates(model.handle, st.handle, x.data_ptr(), x.numel(), off.ctypes.data, ln.ctypes.data,
-                                                 2, 1, 0.0, y.data_ptr(), y.numel(), oo.ctypes.data,
-                                                 groups.ctypes.data if groups is not None else None, 1 if groups is not None else 0,
-                                                 2 if groups is not None else 0, r32.ctypes.data,
-                                                 torch.cuda.current_stream().cuda_stream)
+        rc = _lib.lib().dfb_enhance_ragged(model.handle, st.handle, x.data_ptr(), x.numel(), off.ctypes.data, ln.ctypes.data,
+                                           2, 1, 0.0, y.data_ptr(), y.numel(), oo.ctypes.data,
+                                           groups.ctypes.data if groups is not None else None, 1 if groups is not None else 0,
+                                           2 if groups is not None else 0, r32.ctypes.data, None, 0, None, 0, None,
+                                           torch.cuda.current_stream().cuda_stream)
         assert rc == _lib.DFB_ERR_INVALID, rates

@@ -285,7 +285,7 @@ def test_refusals():
         "dfb_enhance": lambda: L.dfb_enhance(model.handle, st.handle, d, 1, 1600, 1, C.c_float(0.0), d, s),
         "dfb_enhance_host": lambda: L.dfb_enhance_host(model.handle, st.handle, h, 1, 1600, 1, C.c_float(0.0), h),
         "dfb_enhance_ragged_host": lambda: L.dfb_enhance_ragged_host(model.handle, st.handle, h, 1600, op, lp, 1, 1, C.c_float(0.0),
-                                                                     h, 1600, op),
+                                                                     h, 1600, op, None, 0, 0, None, None, 0, None, 0, None),
         "dfb_apply": lambda: L.dfb_apply(model.handle, st.handle, d, d, d, 1, 4, d, s),
         "dfb_model_forward_full": lambda: L.dfb_model_forward_full(model.handle, st.handle, d, d, d, 1, 4, d, d, d, d, None, s),
         "dfb_stream_create": lambda: L.dfb_stream_create(C.byref(handle), model.handle, st.handle, 1, C.c_float(0.0)),

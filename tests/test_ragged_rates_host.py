@@ -1,4 +1,4 @@
-"""CPU: rated ragged batches (enhance_batch / enhance_device_ragged with sr=, dfb_enhance_ragged_rates).  Output lengths
+"""CPU: rated ragged batches (enhance_batch / enhance_device_ragged with sr=, dfb_enhance_ragged with rates).  Output lengths
 against io.resample's composition, the supported-rate bound, the Python-side refusals, and the new C ABI's declarations,
 bindings and exports."""
 import ctypes
@@ -14,7 +14,7 @@ from deepfilternet_b200 import _lib, io, ragged
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HOP = 480
 RATES = (8000, 11025, 12000, 16000, 22050, 24000, 32000, 44100, 88200, 96000)
-NEW = {"dfb_model_add_rate": 10, "dfb_enhance_ragged_rates": 17, "dfb_enhance_ragged_rates_host": 16,
+NEW = {"dfb_model_add_rate": 10, "dfb_enhance_ragged": 22, "dfb_enhance_ragged_host": 21,
        "dfb_enhance_out_len_at": 4, "dfb_debug_resample_rows": 12}
 
 
