@@ -130,9 +130,12 @@ SIGNATURES = {
     "dfb_debug_spec_ingest": (_I, [_VP, _VP, _I64, _I64P, _I64P, _I64, _I, _VP, _VP, _VP]),
     "dfb_model_set_max_workspace": (_I, [_VP, _I64]),
     "dfb_model_set_options": (_I, [_VP, _I, _F, _I]),
+    "dfb_model_set_gating_mode": (_I, [_VP, _I]),
+    "dfb_stream_set_gating_mode": (_I, [_VP, _I]),
     "dfb_model_set_chunking": (_I, [_VP, _I, _I, _I]),
     "dfb_debug_gru_timing": (_I, [_VP, _I, _VP]),
     "dfb_debug_gru_tc": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _VP, _VP, _VP, _I64, _I, _I, _I, _I, _I, _I, _I, _VP]),
+    "dfb_debug_gru_tc_hold": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _VP, _VP, _VP, _I64, _VP, _I, _I, _I, _I, _I, _I, _I, _VP]),
     "dfb_debug_gemm_bf16x3": (_I, [_VP, _VP, _I64, _VP, _VP, _VP, _VP, _I64, _I64, _I, _I, _VP]),
     "dfb_debug_df_convp_tc": (_I, [_VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP, _I64, _VP]),
     "dfb_debug_gl_bx": (_I, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _I64, _VP, _VP, _I64, _I64, _I, _I, _I, _I, _F, _F, _VP]),

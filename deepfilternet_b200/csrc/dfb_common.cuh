@@ -312,7 +312,10 @@ int launch_resample_rows(cudaStream_t s, bool up, const RateDir *d_dirs, const R
                          int64_t max_out, int smem_floats);
 // time window of a recurrence launch: steps 0 .. T-1 are frames t0 .. of buffers holding Ts frames per stream; h0 (null:
 // zeros) / hT (null: not stored) are the carried hidden states [B][H]
-struct GruWindow { const float *h0; float *hT; int t0, Ts; const int64_t *first = nullptr; int64_t w0 = 0; /* stream_first */ };
+struct GruWindow {
+    const float *h0; float *hT; int t0, Ts; const int64_t *first = nullptr; int64_t w0 = 0; /* stream_first */
+    const unsigned char *run = nullptr;   /* or run flags [B][Ts]: a step whose flag is 0 keeps the state (k_gru_tc HOLD) */
+};
 // tensor-core GRU recurrence, H = 256 or 512 (dfb_tc.cu); hout may be null when the planes hout_hi / hout_lo are given.
 // ns = 0, xg = -1: the production choice of instance; otherwise the instance <ns, H, xg> (dfb_debug_gru_tc)
 int launch_gru_tc(cudaStream_t s, const float *xproj, const float *whh, const float *bhh, const float *res, float *hout,

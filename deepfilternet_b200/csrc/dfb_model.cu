@@ -464,7 +464,7 @@ using namespace dfb;
 // carried hidden states of one GRU stack between time chunks: h = [layers][Bs][H]; t0 = first frame the recurrences run.
 // Bs is the stream count the state was allocated for: a chunk may run only a prefix B <= Bs of the streams (ragged batch)
 // first / w0: streaming slots, each stream's first frame (stream_first) or null
-struct GruChunk { float *h; bool have_state; int t0; int Bs; const int64_t *first; int64_t w0; };
+struct GruChunk { float *h; bool have_state; int t0; int Bs; const int64_t *first; int64_t w0; const unsigned char *run = nullptr; };
 
 // Weight tables: device pointers into the weight slab, bound once by dfb_model_create for the layers the configured
 // forward pass runs.  A tensor that pass does not read stays null.
@@ -507,6 +507,7 @@ struct dfb_model {
     Arena arena;
     int dev_chunks = 0, host_chunks = 4, n_lanes = 2;   // chunk pipeline (dfb_model_set_chunking); dev_chunks 0 = auto
     int post_filter = 0, mask_only = 0;       // optional stages (dfb_model_set_options)
+    int gating_mode = 0;                      // DFB_GATING_APPLY / DFB_GATING_RUNTIME (dfb_model_set_gating_mode)
     float pf_beta = 0.02f;
     size_t max_workspace = size_t(40) << 30;  // dfb_enhance chunks / groups the batch so that the arena stays below this
                                               // (40 GB: room for the batch itself and its output on an 80 GB H100)
@@ -523,6 +524,8 @@ struct dfb_model {
         cudaStream_t main = nullptr, hi = nullptr, aux = nullptr, dhi = nullptr, daux = nullptr, low = nullptr;
         cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_fork_enc = nullptr, ev_join_enc = nullptr, ev_in = nullptr,
                     ev_out = nullptr, ev_c0 = nullptr, ev_convp = nullptr, ev_skip = nullptr, ev_done = nullptr;
+        unsigned char *rt = nullptr;   // runtime gating mode's run flags and compacted DF pathway rows (grow-only)
+        size_t rt_cap = 0;
     } lanes[2];
     Arena arena1;                           // lane 1's activations (lane 0 uses `arena`)
     // offline resamplers of rated batches (dfb_model_add_rate): the registered rates, their directions (rate_up[i] /
@@ -743,6 +746,7 @@ extern "C" void dfb_model_free(dfb_model *m) {
             if (st) cudaStreamDestroy(st);
         for (cudaEvent_t e : {L.ev_fork, L.ev_join, L.ev_fork_enc, L.ev_join_enc, L.ev_in, L.ev_out, L.ev_c0, L.ev_convp, L.ev_skip, L.ev_done})
             if (e) cudaEventDestroy(e);
+        if (L.rt) cudaFree(L.rt);
     }
     delete m;
 }
@@ -825,7 +829,7 @@ int run_gru(dfb_model *m, cudaStream_t s, const GruLayer *lw, int layers, int H,
         const bool last = l == layers - 1;
         float *dst = last ? y : nullptr;   // a middle layer's output feeds only the next projection, which reads its planes
         float *hs = ck && ck->h ? ck->h + (int64_t)l * ck->Bs * H : nullptr;   // carried state of this layer [Bs][H], rows [0, B)
-        GruWindow gw{ck && ck->have_state ? hs : nullptr, hs, t0, T, ck ? ck->first : nullptr, ck ? ck->w0 : 0};
+        GruWindow gw{ck && ck->have_state ? hs : nullptr, hs, t0, T, ck ? ck->first : nullptr, ck ? ck->w0 : 0, ck ? ck->run : nullptr};
         // the last layer's planes feed a grouped linear and include the residual; the others feed the next projection
         unsigned short *hi = last ? out_hi : pl_hi, *lo = last ? out_lo : pl_lo;
         if ((rc = launch_gru_tc(s, xproj, g.w_hh, g.b_hh, last ? res_last : nullptr, dst, hi, lo, B, Tn,
@@ -964,8 +968,187 @@ struct ChunkCtx {
     const RaggedRow *rows;         // ragged batch: per-stream frame counts (features end at rows[b].Tf), or null
     int64_t W0;                    // absolute frame of window row 0
     const int64_t *first;          // streaming slots: per-stream first frames (before them = padding), or null
+    const struct GateRun *gate = nullptr;   // runtime gating mode, or null (apply mode: the decoders run every frame)
 };
 constexpr int kHalo = 8;           // >= temporal receptive field of every feed-forward chain of the shipped models
+
+// ---- runtime gating mode (dfb_model_set_gating_mode, tract.rs:478-503): each decoder runs only on the frames the LSNR
+// stage rule lets through, as if run alone on that subsequence.  The ERB decoder runs on frame t iff min <= lsnr <= max_erb,
+// the DF decoder iff that holds and lsnr <= max_df (tract.rs:658-672), with the same comparisons as the apply kernel and
+// k_spec_emit, so the stages applied and the frames run always agree.  Recurrences hold their state through the other
+// frames (k_gru_tc HOLD); time-tap layers read the previous frames their decoder ran on: the DF pathway conv runs on each
+// row's compacted run frames after the carried c0 of its last kt - 1 run frames, and (conv_kt == 2) the inputs of convt3 and
+// of the mask head are filled forward from the ERB decoder's last run frame.
+struct GateRun {
+    const SlotCtl *ctl;            // per-row gating and thresholds, or null: every row gates with th when gate_all
+    const LinkRow *links;          // link groups (channel 0 decides), or null
+    float th[3];
+    int gate_all;
+    float *t_c0, *t_run;           // StreamState tails
+    bool valid;                    // the tails hold the last DNN chunk's run frames; else it ran in apply mode, where every
+                                   // frame ran: take them from the halo (frames before the window or a stream's start: zero)
+};
+
+struct GatePlan {
+    const float *ll; const SlotCtl *ctl; const LinkRow *links; const int64_t *first;
+    int64_t w0; float th[3]; int gate_all, T, Rc;
+    unsigned char *erb_run, *df_run;   // [B][T] run flags of the window's new frames (halo rows: 1)
+    int *erb_src;                      // [B][T] last ERB run frame <= t among the new frames, -1: none (the carried one)
+    int *df_pos, *df_n;                // [B][T] DF run frames among the new frames before t; [B] their number
+    // (conv_kt == 2) has_run [b * run_w]: the ERB decoder has run on a frame of stream b (carried; from_halo: every earlier
+    // frame of the stream ran); erb_first [B]: the first frame the kt = 2 layers may read -- the stream's first frame once
+    // the decoder has run, else its first run frame, so that the frames before it are padding, as tract's zero state is
+    float *has_run; int run_w, from_halo;
+    int64_t *erb_first;
+};
+
+// one CTA per row: flags in parallel over frame segments, then an exclusive scan of the segments' last ERB run frame and
+// DF run count
+__global__ void __launch_bounds__(256) k_gate_plan(GatePlan g) {
+    __shared__ int s_last[256], s_cnt[256];
+    const int b = blockIdx.x, tid = threadIdx.x, T = g.T;
+    const int lb = g.links ? g.links[b].first : b;
+    const bool gate = g.ctl ? g.ctl[b].gate != 0 : g.gate_all != 0;
+    const float th0 = g.ctl ? g.ctl[b].th_min : g.th[0], th1 = g.ctl ? g.ctl[b].th_erb : g.th[1], th2 = g.ctl ? g.ctl[b].th_df : g.th[2];
+    const int tf = stream_first(g.first, b, g.w0);
+    const int per = (T - g.Rc + 255) / 256;
+    const int t0 = g.Rc + tid * per, t1 = min(t0 + per, T);
+    const int64_t row = (int64_t)b * T;
+    for (int t = tid; t < g.Rc; t += 256) { g.erb_run[row + t] = 1; g.df_run[row + t] = 1; g.erb_src[row + t] = t; g.df_pos[row + t] = 0; }
+    int last = -1, cnt = 0;
+    for (int t = t0; t < t1; t++) {
+        bool e = t >= tf, d = e;
+        if (e && gate) {   // stage 2 or 3 of the apply kernel runs the ERB decoder, stage 3 also the DF decoder
+            const float l = g.ll[(int64_t)lb * T + t];
+            e = !(l < th0) && !(l > th1);
+            d = e && !(l > th2);
+        }
+        g.erb_run[row + t] = e; g.df_run[row + t] = d;
+        if (e) last = t;
+        cnt += d;
+    }
+    int first_run = T;
+    for (int t = t0; t < t1 && first_run == T; t++)
+        if (g.erb_run[row + t]) first_run = t;
+    s_last[tid] = last; s_cnt[tid] = cnt;
+    __syncthreads();
+    if (tid == 0) {
+        int m = -1, c = 0;
+        for (int i = 0; i < 256; i++) {
+            const int lm = s_last[i], lc = s_cnt[i];
+            s_last[i] = m; s_cnt[i] = c;
+            if (lm > m) m = lm;
+            c += lc;
+        }
+        g.df_n[b] = c;
+    }
+    __shared__ int s_first;
+    if (tid == 0) s_first = T;
+    __syncthreads();
+    if (first_run < T) atomicMin(&s_first, first_run);
+    __syncthreads();
+    if (g.has_run && tid == 0) {
+        float &h = g.has_run[(int64_t)b * g.run_w];
+        const int64_t f0 = g.first ? g.first[b] : 0;
+        const bool prev = g.from_halo ? g.Rc > 0 && g.w0 + g.Rc - 1 >= f0 : h != 0.f;
+        g.erb_first[b] = prev ? f0 : g.w0 + s_first;
+        h = prev || s_first < T ? 1.f : 0.f;
+    }
+    __syncthreads();
+    last = s_last[tid]; cnt = s_cnt[tid];
+    for (int t = t0; t < t1; t++) {
+        if (g.erb_run[row + t]) last = t;
+        g.erb_src[row + t] = last;
+        g.df_pos[row + t] = cnt;
+        cnt += g.df_run[row + t];
+    }
+}
+
+// DF pathway input of the run frames, compacted: row b of P [B][Tp][W] is the c0 of its last K - 1 run frames before the
+// window's new frames (the carried tail, or the halo), then c0 of its DF run frames among them.  grid (K - 1 + T - Rc, B)
+__global__ void __launch_bounds__(256) k_gate_gather(const float *__restrict__ c0, const float *__restrict__ tail, float *__restrict__ P,
+                                                     int T, int Rc, int K, int W, int Tp, const unsigned char *__restrict__ df_run,
+                                                     const int *__restrict__ df_pos, int from_halo, const int64_t *__restrict__ first,
+                                                     int64_t w0) {
+    const int b = blockIdx.y, x = blockIdx.x;
+    const float4 *src = nullptr;
+    int64_t dst;
+    if (x < K - 1) {
+        dst = (int64_t)b * Tp + x;
+        if (!from_halo) src = reinterpret_cast<const float4 *>(tail + ((int64_t)b * (K - 1) + x) * W);
+        else {
+            const int t = Rc - (K - 1) + x;
+            if (t >= 0 && t >= stream_first(first, b, w0)) src = reinterpret_cast<const float4 *>(c0 + ((int64_t)b * T + t) * W);
+        }
+    } else {
+        const int t = Rc + x - (K - 1);
+        if (!df_run[(int64_t)b * T + t]) return;
+        dst = (int64_t)b * Tp + K - 1 + df_pos[(int64_t)b * T + t];
+        src = reinterpret_cast<const float4 *>(c0 + ((int64_t)b * T + t) * W);
+    }
+    float4 *d = reinterpret_cast<float4 *>(P + dst * W);
+    for (int i = threadIdx.x; i < W / 4; i += blockDim.x) d[i] = src ? src[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+// the compacted pathway term back to its frames (other frames, whose coefficients no stage applies: 0); grid (T, B)
+__global__ void __launch_bounds__(256) k_gate_scatter(const float *__restrict__ Q, float *__restrict__ coefs, int T, int Rc, int K, int W,
+                                                      int Tp, const unsigned char *__restrict__ df_run, const int *__restrict__ df_pos) {
+    const int b = blockIdx.y, t = blockIdx.x;
+    const int64_t i = (int64_t)b * T + t;
+    const bool run = t >= Rc && df_run[i];
+    const float *src = Q + ((int64_t)b * Tp + K - 1 + (run ? df_pos[i] : 0)) * W;
+    float *dst = coefs + i * W;
+    for (int k = threadIdx.x; k < W; k += blockDim.x) dst[k] = run ? src[k] : 0.f;
+}
+
+// the last K - 1 compacted rows (run frames) become the carried tail; grid (K - 1, B)
+__global__ void __launch_bounds__(256) k_gate_tail(const float *__restrict__ P, float *__restrict__ tail, int K, int W, int Tp,
+                                                   const int *__restrict__ df_n) {
+    const int b = blockIdx.y, x = blockIdx.x;
+    const float4 *src = reinterpret_cast<const float4 *>(P + ((int64_t)b * Tp + df_n[b] + x) * W);
+    float4 *dst = reinterpret_cast<float4 *>(tail + ((int64_t)b * (K - 1) + x) * W);
+    for (int i = threadIdx.x; i < W / 4; i += blockDim.x) dst[i] = src[i];
+}
+
+// (conv_kt == 2) the frames before a run frame, as the kt = 2 layers read them, are the ERB decoder's last run frame: fill
+// rows [Rc - 1, T) of x [B][T][fs] (W values per frame) that are not run frames from the last run frame before them, or from
+// the carried one (tail + off; from_halo: row Rc - 1 as recomputed, zeros at a stream's start).  save: afterwards, copy row
+// T - 1 to the carried one.  grid (T - Rc + 1, B)
+struct FillSeg { float *x; int64_t fs; int W, off; };
+__global__ void __launch_bounds__(256) k_gate_fill(FillSeg sg, float *__restrict__ tail, int tail_w, int T, int Rc,
+                                                   const unsigned char *__restrict__ erb_run, const int *__restrict__ erb_src,
+                                                   int from_halo, int save) {
+    const int b = blockIdx.y;
+    float *trow = tail + (int64_t)b * tail_w + sg.off;
+    float *xb = sg.x + (int64_t)b * T * sg.fs;
+    if (save) {
+        for (int k = threadIdx.x; k < sg.W; k += blockDim.x) trow[k] = xb[(int64_t)(T - 1) * sg.fs + k];
+        return;
+    }
+    const int t = Rc - 1 + blockIdx.x;
+    if (t < 0) return;
+    const float *src;
+    if (t == Rc - 1) {
+        if (from_halo) return;
+        src = trow;
+    } else {
+        if (erb_run[(int64_t)b * T + t]) return;
+        const int j = erb_src[(int64_t)b * T + t];
+        src = j >= 0 ? xb + (int64_t)j * sg.fs : from_halo ? (Rc > 0 ? xb + (int64_t)(Rc - 1) * sg.fs : nullptr) : trow;
+    }
+    for (int k = threadIdx.x; k < sg.W; k += blockDim.x) xb[(int64_t)t * sg.fs + k] = src ? src[k] : 0.f;
+}
+
+// grow-only device buffer of a lane (run flags + compacted pathway rows); the lane's decoder phases are serialised
+static unsigned char *lane_rt(dfb_model::Lane &L, size_t bytes) {
+    if (L.rt_cap < bytes) {
+        if (L.rt) { cudaDeviceSynchronize(); cudaFree(L.rt); L.rt = nullptr; L.rt_cap = 0; }
+        const size_t want = (bytes + bytes / 4 + (1u << 20)) & ~size_t((1u << 20) - 1);
+        if (cudaMalloc(&L.rt, want) != cudaSuccess) { L.rt = nullptr; return nullptr; }
+        L.rt_cap = want;
+    }
+    return L.rt;
+}
 
 static int forward_impl(dfb_model *m, Arena &arena, const float *d_feat_erb, const float *d_feat_spec, int B, int T,
                         float *d_m, float *d_coefs, float *d_lsnr, float *d_alpha, cudaStream_t s, ChunkCtx *cx = nullptr);
@@ -1015,6 +1198,8 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
     GruChunk ck_enc{cx ? cx->h_enc : nullptr, cx && cx->have_state, cx ? cx->Rc : 0, cx ? cx->Bs : B, first, W0};
     GruChunk ck_erb{cx ? cx->h_erb : nullptr, cx && cx->have_state, cx ? cx->Rc : 0, cx ? cx->Bs : B, first, W0};
     GruChunk ck_df{cx ? cx->h_df : nullptr, cx && cx->have_state, cx ? cx->Rc : 0, cx ? cx->Bs : B, first, W0};
+    const GateRun *gate = cx ? cx->gate : nullptr;
+    const int Rc = cx ? cx->Rc : 0;
     // DFB_SERIAL=1: everything on the caller's stream (profiling: per-kernel times without overlap)
     static const bool serial = getenv("DFB_SERIAL") && atoi(getenv("DFB_SERIAL"));
     dfb_model::Lane &L = m->lanes[cx ? cx->lane : 0];
@@ -1151,16 +1336,18 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         // DF pathway conv (needs c0 only; its result is consumed by the very last DF-decoder kernel): on the
         // low-priority stream, so its CTAs only take SMs that the critical path -- the encoder convs now, the GRU
         // clusters later -- leaves idle (on the DF branch's own streams it delays df_fc_emb, which is on the critical path)
-        DFB_CUDA(cudaStreamWaitEvent(sl, L.ev_c0, 0));
         if (!df_convp_built(c.df_order, c.df_pathway_kt))
             return fail(DFB_ERR_UNSUPPORTED, "df_order %d / df_pathway_kernel_size_t %d (built kernels: df_order 5, kt 1-5)",
                         c.df_order, c.df_pathway_kt);
         if (Fd % 2) return fail(DFB_ERR_UNSUPPORTED, "df pathway conv: odd nb_df");
-        // channel contraction on the tensor cores (BF16x3), shifted adds + 1x1 conv in the epilogue
-        if ((rc = launch_df_convp_tc(sl, f.c0, w.df_convp.w_sw, w.df_convp.w2, w.df_convp.b, d_coefs, B, T, Fd, c.df_order,
-                                     c.df_pathway_kt, first, W0)))
-            return rc;
-        DFB_CUDA(cudaEventRecord(L.ev_convp, sl));
+        if (!gate) {   // (runtime gating mode: on the run frames only, after the gate plan below)
+            DFB_CUDA(cudaStreamWaitEvent(sl, L.ev_c0, 0));
+            // channel contraction on the tensor cores (BF16x3), shifted adds + 1x1 conv in the epilogue
+            if ((rc = launch_df_convp_tc(sl, f.c0, w.df_convp.w_sw, w.df_convp.w2, w.df_convp.b, d_coefs, B, T, Fd, c.df_order,
+                                         c.df_pathway_kt, first, W0)))
+                return rc;
+            DFB_CUDA(cudaEventRecord(L.ev_convp, sl));
+        }
     }
     {
         DwPwParams p = mk(w.erb_conv1, f.e0, E, (int64_t)E * kCh, f.e1, E / 2, (int64_t)E / 2 * kCh, c.conv_kt);
@@ -1206,6 +1393,58 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         if (d_lsnr && (rc = run_gl(s, f.emb, emb_dim, w.lsnr.w, w.lsnr.b, nullptr, 0, d_lsnr, 1, M, 1, emb_dim, 1, ACT_SIGMOID, c.lsnr_scale,
                                    c.lsnr_offset)))
             return rc;
+    }
+    // runtime gating mode: which frames each decoder runs on, from the LSNR just computed
+    const int Kp = c.df_pathway_kt, Wc = Fd * kCh, Wq = Fd * 2 * c.df_order, Tp = Kp - 1 + T - Rc;
+    unsigned char *erb_run = nullptr, *df_run = nullptr;
+    int *erb_src = nullptr, *df_pos = nullptr, *df_n = nullptr;
+    float *gP = nullptr, *gQ = nullptr;
+    const int tw_run = 2 * ED + 2 * E * kCh + 1;   // StreamState::t_run per row: dec_emb | e3 | d1 | e0 | has_run
+    const int64_t *kt_first = first;               // first frames the ERB decoder's kt = 2 layers read from
+    if (gate) {
+        if (!d_lsnr) return fail(DFB_ERR_INVALID, "runtime gating without the LSNR head");
+        auto al = [](size_t n) { return (n + 255) & ~size_t(255); };
+        const size_t nf = (size_t)M, o1 = al(nf), o2 = o1 + al(nf), o3 = o2 + al(nf * 4), o4 = o3 + al(nf * 4), o5 = o4 + al((size_t)B * 4),
+                     o6 = o5 + al((size_t)B * Tp * Wc * 4), o7 = o6 + al((size_t)B * Tp * Wq * 4), end = o7 + al((size_t)B * 8);
+        unsigned char *rt = lane_rt(L, end);
+        if (!rt) return fail(DFB_ERR_OOM, "runtime gating buffers (%zu bytes)", end);
+        erb_run = rt; df_run = rt + o1; erb_src = reinterpret_cast<int *>(rt + o2); df_pos = reinterpret_cast<int *>(rt + o3);
+        df_n = reinterpret_cast<int *>(rt + o4); gP = reinterpret_cast<float *>(rt + o5); gQ = reinterpret_cast<float *>(rt + o6);
+        int64_t *erb_first = reinterpret_cast<int64_t *>(rt + o7);
+        GatePlan gp{d_lsnr, gate->ctl, gate->links, first, W0, {gate->th[0], gate->th[1], gate->th[2]}, gate->gate_all, T, Rc,
+                    erb_run, df_run, erb_src, df_pos, df_n, c.conv_kt > 1 ? gate->t_run + tw_run - 1 : nullptr, tw_run,
+                    gate->valid ? 0 : 1, erb_first};
+        kt_first = erb_first;
+        {
+            dfb::ProfScope prof_scope__("k_gate_plan", s);   // (not on the enhancement path bench.py models: see launch_spec_ingest)
+            k_gate_plan<<<B, 256, 0, s>>>(gp);
+            DFB_LAUNCH_CHECK();
+        }
+        ck_erb.run = erb_run;
+        ck_df.run = df_run;
+        // the pathway conv over each row's compacted run frames, after the carried c0 of its last Kp - 1: on the
+        // low-priority stream, beside the decoders' recurrences (it reads the tail the previous chunk's decoder phase wrote)
+        DFB_CUDA(cudaEventRecord(L.ev_c0, s));
+        DFB_CUDA(cudaStreamWaitEvent(sl, L.ev_c0, 0));
+        if (cx->wait_dec) DFB_CUDA(cudaStreamWaitEvent(sl, cx->wait_dec, 0));
+        {
+            dfb::ProfScope prof_scope__("k_gate_gather", sl);   // (see k_gate_plan)
+            k_gate_gather<<<dim3((unsigned)(Tp), (unsigned)B), 256, 0, sl>>>(f.c0, gate->t_c0, gP, T, Rc, Kp, Wc, Tp, df_run, df_pos,
+                                                                           gate->valid ? 0 : 1, first, W0);
+            DFB_LAUNCH_CHECK();
+            if (Kp > 1) {
+                k_gate_tail<<<dim3((unsigned)(Kp - 1), (unsigned)B), 256, 0, sl>>>(gP, gate->t_c0, Kp, Wc, Tp, df_n);
+                DFB_LAUNCH_CHECK();
+            }
+        }
+        if ((rc = launch_df_convp_tc(sl, gP, w.df_convp.w_sw, w.df_convp.w2, w.df_convp.b, gQ, B, Tp, Fd, c.df_order, Kp, nullptr, 0)))
+            return rc;
+        {
+            dfb::ProfScope prof_scope__("k_gate_scatter", sl);   // (see k_gate_plan)
+            k_gate_scatter<<<dim3((unsigned)T, (unsigned)B), 256, 0, sl>>>(gQ, d_coefs, T, Rc, Kp, Wq, Tp, df_run, df_pos);
+            DFB_LAUNCH_CHECK();
+        }
+        DFB_CUDA(cudaEventRecord(L.ev_convp, sl));
     }
     // fork: the two decoders only share read-only encoder outputs
     // the encoder phase is done (ev_fork also tells the next time chunk that it may start); the decoder phase runs on the
@@ -1272,7 +1511,23 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
                                        fb * ns, B, cudaMemcpyDeviceToDevice, s));
             cx->dec_tail_n = ns;
         }
+        // (runtime gating, kt = 2) convt3 and the mask head read the ERB decoder's previous run frame
+        auto fill = [&](FillSeg sg, int save) -> int {
+            dfb::ProfScope prof_scope__("k_gate_fill", s);   // (see k_gate_plan)
+            k_gate_fill<<<dim3((unsigned)(save ? 1 : T - Rc + 1), (unsigned)B), 256, 0, s>>>(sg, gate->t_run, tw_run, T, Rc, erb_run, erb_src,
+                                                                                          gate->valid ? 0 : 1, save);
+            DFB_LAUNCH_CHECK();
+            return DFB_OK;
+        };
+        const bool fill_kt = gate && c.conv_kt > 1;
+        const FillSeg sg_dec{f.dec_emb, ED, ED, 0}, sg_e3{f.e3, e3_fs, ED, ED}, sg_d1{f.d1, (int64_t)E * kCh, E * kCh, 2 * ED},
+                      sg_e0{f.e0, (int64_t)E * kCh, E * kCh, 2 * ED + E * kCh};
+        if (fill_kt) {
+            for (const FillSeg &sg : {sg_dec, sg_e3}) if ((rc = fill(sg, 0))) return rc;
+            for (const FillSeg &sg : {sg_dec, sg_e3}) if ((rc = fill(sg, 1))) return rc;
+        }
         DwPwParams p = mk(w.convt3, f.dec_emb, E / 4, ED, f.d3, E / 4, ED, c.conv_kt);
+        p.first = kt_first;
         p.path = f.e3; p.path_fs = e3_fs; p.ps = w.conv3p.s; p.pb = w.conv3p.b;
         if ((rc = run_dwpw<DW_S1>(s, p, B, w.convt3.pw_sw))) return rc;
         p = mk(w.convt2, f.d3, E / 4, ED, f.d2, E / 2, (int64_t)E / 2 * kCh, 1);
@@ -1295,10 +1550,14 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
             DFB_CUDA(cudaFuncSetAttribute(k_mask_out, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           (kMaskWarps * 2 * (64 + 2) * kMaskLd + 2 * 3 * kCh) * 4));
         }
+        if (fill_kt) {
+            for (const FillSeg &sg : {sg_d1, sg_e0}) if ((rc = fill(sg, 0))) return rc;
+            for (const FillSeg &sg : {sg_d1, sg_e0}) if ((rc = fill(sg, 1))) return rc;
+        }
         int per_cta = kMaskWarps * kMaskChunk;
         dim3 grid((unsigned)((T + per_cta - 1) / per_cta), (unsigned)B);
         DFB_PROF("k_mask_out", s);
-        k_mask_out<<<grid, 32 * kMaskWarps, smem, s>>>(f.e0, f.d1, w.conv0p.s, w.conv0p.b, w.conv0_out.w, w.conv0_out.b, d_m, T, E, c.conv_kt, first, W0);
+        k_mask_out<<<grid, 32 * kMaskWarps, smem, s>>>(f.e0, f.d1, w.conv0p.s, w.conv0p.b, w.conv0_out.w, w.conv0_out.b, d_m, T, E, c.conv_kt, kt_first, W0);
         DFB_LAUNCH_CHECK();
     }
     return finish();
@@ -1514,6 +1773,13 @@ static void apply_options(const dfb_model *m, dfb::ApplyParams &p) {
 // init_df(post_filter=..., mask_only=...) (df/enhance.py:101-187): the post filter of deepfilternet3.py:448-454 (beta =
 // pf_beta) or, for DeepFilterNet2, Mask.pf on the ERB gains (modules.py:234-245, beta fixed at 0.02); mask_only = the
 // model built with run_df = False (checkpoint.py:32): no deep filtering stage.
+extern "C" int dfb_model_set_gating_mode(dfb_model *m, int mode) {
+    if (!m) return fail(DFB_ERR_INVALID, "null model");
+    if (mode != DFB_GATING_APPLY && mode != DFB_GATING_RUNTIME) return fail(DFB_ERR_INVALID, "gating mode %d", mode);
+    m->gating_mode = mode;
+    return DFB_OK;
+}
+
 extern "C" int dfb_model_set_options(dfb_model *m, int post_filter, float pf_beta, int mask_only) {
     if (!m) return fail(DFB_ERR_INVALID, "null model");
     m->post_filter = post_filter ? 1 : 0;
@@ -1679,6 +1945,10 @@ struct StreamState {
     float *t_l = nullptr;                                        // ... and of lsnr (stage gating)
     float *t_dec = nullptr;                                      // (conv_kt == 2) last kHalo frames of dec_emb
     int n_feat = 0, n_mc = 0, n_dec = 0;                         // valid frames in the tails
+    // runtime gating mode (GateRun): c0 of the DF decoder's last df_pathway_kt - 1 run frames, (conv_kt == 2) dec_emb | e3 |
+    // d1 | e0 of the ERB decoder's last run frame; rt_valid: the last DNN chunk kept them (else it ran in apply mode)
+    float *t_c0 = nullptr, *t_run = nullptr;
+    bool rt_valid = false;
 };
 constexpr int kMcTail = 6;   // >= df_order (DeepFilterNet2, see run_chunk)
 
@@ -1694,12 +1964,14 @@ static ChunkGeom chunk_geom(const dfb_model_config &c) {
 }
 
 // Every array of the state slab is `layers` x [B][per_row] floats; only the GRU states have more than one layer.
-// Arrays 13 / 14: the histories of a resampled handle's up / down resampler (dfb_stream_set_sample_rate), 0 floats otherwise.
-constexpr int kStateArrays = 15;
+// Arrays 13 / 14: the runtime gating mode's decoder tails (GateRun), 0 floats for DeepFilterNet v1 (14: for conv_kt == 1).
+// Arrays 15 / 16: the histories of a resampled handle's up / down resampler (dfb_stream_set_sample_rate), 0 floats otherwise.
+// The resampler histories stay last: handles that resample nothing move every array but those two (k_slot_rows).
+constexpr int kStateArrays = 17;
 // row_off / row_floats: one stream's row of every array, packed (the scratch rows of k_slot_rows)
 struct StateLayout { int64_t off[kStateArrays], row_off[kStateArrays], row_floats; int layers[kStateArrays], per_row[kStateArrays]; };
 
-static size_t state_floats(const dfb_model_config &c, const dfb_state *st, int B, size_t off[16], StateLayout *lay = nullptr,
+static size_t state_floats(const dfb_model_config &c, const dfb_state *st, int B, size_t off[kStateArrays], StateLayout *lay = nullptr,
                            int rs_up = 0, int rs_down = 0) {
     const ChunkGeom g = chunk_geom(c);
     const int E = c.nb_erb, Fd = c.nb_df, O2 = 2 * c.df_order, F = st->tb.F, ED = E / 4 * kCh;
@@ -1720,16 +1992,20 @@ static size_t state_floats(const dfb_model_config &c, const dfb_state *st, int B
     add(9, 1, kMcTail * E); add(10, 1, kMcTail * Fd * O2);
     add(11, 1, c.conv_kt > 1 ? kHalo * ED : 0);
     add(12, 1, kMcTail);
-    add(13, 1, rs_up); add(14, 1, rs_down);
+    add(13, 1, c.model_kind != 1 ? (c.df_pathway_kt - 1) * Fd * kCh : 0);
+    add(14, 1, c.model_kind != 1 && c.conv_kt > 1 ? 2 * ED + 2 * E * kCh + 1 : 0);
+    add(15, 1, rs_up); add(16, 1, rs_down);
     return n;
 }
-static void state_bind(StreamState &S, float *base, const size_t off[16], int B) {
+static void state_bind(StreamState &S, float *base, const size_t off[kStateArrays], int B) {
     S.B = B; S.slab = base;
     S.ana_mem = base + off[0]; S.erb_state = base + off[1]; S.unit_state = base + off[2];
     S.h_enc = base + off[3]; S.h_erb = base + off[4]; S.h_df = base + off[5];
     S.t_spec = base + off[6]; S.t_fe = base + off[7]; S.t_fs = base + off[8];
     S.t_m = base + off[9]; S.t_c = base + off[10]; S.t_dec = base + off[11]; S.t_l = base + off[12];
+    S.t_c0 = base + off[13]; S.t_run = base + off[14];
     S.a1 = S.d1 = S.e1 = 0; S.started = S.dnn_started = false; S.n_feat = S.n_mc = S.n_dec = 0;
+    S.rt_valid = false;
 }
 
 // last n frames of buf [B][T][fe] -> tail [B][cap][fe] (right aligned), and back into frames [dst_t, dst_t + n) of a buffer
@@ -1792,6 +2068,8 @@ struct ChunkIO {
     const float *spec_in = nullptr;
     int64_t spec_frames = 0;
     const struct SpecOut *spec_out = nullptr;
+    // runtime gating mode (GateRun): wherever a row gates, its decoders run only on the frames its stages let through
+    bool runtime = false;
 };
 
 // Outputs of a spectral call (k_spec_emit): caller row c, output row j of n_out carries frame f0 + j; slot_row maps caller
@@ -2031,7 +2309,16 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
     if (run_dnn) {
     ChunkCtx cx{Rc, Tsb, Tv, S.h_enc, S.h_erb, S.h_df, S.dnn_started, c.conv_kt > 1 ? S.t_dec : nullptr, S.n_dec, lane,
                 have_prev ? P.ev_done : nullptr, S.B, io.rows, W0, io.first};
+    // the rows gate as the apply kernel (io.ctl: each row's own entry) or k_spec_emit decides
+    const bool gates = io.ctl ? io.ctl_gate : (io.lsnr_th != nullptr || (spectral && io.spec_out->gating));
+    GateRun gr{io.ctl, io.links, {0.f, 0.f, 0.f}, 0, S.t_c0, S.t_run, S.rt_valid};
+    if (io.runtime && gates && c.model_kind != 1) {
+        const float *th = spectral ? io.spec_out->th : io.lsnr_th;
+        if (!io.ctl) { gr.gate_all = 1; gr.th[0] = th[0]; gr.th[1] = th[1]; gr.th[2] = th[2]; }
+        cx.gate = &gr;
+    }
     if ((rc = forward_impl(m, arena, fe, fs, B, Tw, mm, cc, ll, aa, s, &cx))) return rc;
+    S.rt_valid = cx.gate != nullptr;
     S.n_dec = cx.dec_tail_n;
     S.dnn_started = true;
     // the halo rows of m / coefs come from skipped recurrences: restore the last finished frames from the previous chunk
@@ -2146,7 +2433,7 @@ static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, float *d
     const ChunkGeom g = chunk_geom(c);
     const int hop = st->hop, fft = st->fft;
     const int64_t Tf = tfs[0];
-    size_t off[16];
+    size_t off[kStateArrays];
     const size_t nstate = state_floats(c, st, (int)nb, off);
     float *slab = m->aux_arena.take<float>(nstate);
     if (!slab) return fail(DFB_ERR_OOM, "stream state arena exhausted");
@@ -2185,6 +2472,7 @@ static int enhance_group(dfb_model *m, dfb_state *st, const float *d_x, float *d
         ChunkIO io{d_x, Tf * hop, 0, nullptr, d_out, 0, 0, delay, lim, nullptr, rows, (int)na, links, reduce};
         io.ctl = bo.ctl; io.ctl_gate = bo.gate;
         io.lsnr_rows = bo.lsnr; io.lsnr_offs = bo.lsnr_offs;
+        io.runtime = m->gating_mode == DFB_GATING_RUNTIME;
         if ((rc = run_chunk(m, st, S, io, a1n, d1n, e1n > S.e1 ? e1n : S.e1, cs, lane, pipelined))) break;
         if (hooks && (rc = hooks->after(e0 * hop > delay ? e0 * hop - delay : 0, S.e1 * hop - delay, d1n, na, cs))) break;
         // what the hook enqueued on the lane is part of the chunk: the caller's stream and the next chunk's decoder wait for it
@@ -2411,7 +2699,7 @@ static int enhance_rows(dfb_model *m, dfb_state *st, std::vector<RaggedRow> &row
     bool pipelined = false;
     int rc = enhance_plan(m, st, B, tfs[0], min_chunks, min_group, &group, &tc, &pipelined);
     if (rc) return rc;
-    size_t off[16];   // the aux arena holds one group's state slab and tables
+    size_t off[kStateArrays];   // the aux arena holds one group's state slab and tables
     if ((rc = m->aux_arena.reserve(state_floats(m->cfg, st, (int)group, off) * sizeof(float) +
                                    (size_t)group * (sizeof(RaggedRow) + sizeof(LinkRow) + (rated ? 2 * sizeof(RateRow) : 0) +
                                                     sizeof(SlotCtl) + sizeof(int64_t)) + 8192)))
@@ -2841,6 +3129,7 @@ struct dfb_stream {
     float *slab = nullptr;
     bool gating = false;
     float th[3] = {-10.f, 30.f, 20.f};                 // tract.rs:180-185 defaults
+    int gating_mode = -1;                              // dfb_stream_set_gating_mode, -1: the model's
     float *stage_in = nullptr, *stage_out = nullptr;   // device staging of the *_host entry point
     size_t stage_in_cap = 0, stage_out_cap = 0;
     bool fed = false;                                  // a frame has been processed since create / reset
@@ -2909,7 +3198,7 @@ static int rs_hist(const dfb_stream *h, const ResampleDirs &d) {
     for (size_t i = 0; i < h->rs_rates.size(); i++) S = std::max(S, d.d[i].S);
     return S;
 }
-static size_t stream_state_floats(const dfb_stream *h, size_t off[16], StateLayout *lay = nullptr) {
+static size_t stream_state_floats(const dfb_stream *h, size_t off[kStateArrays], StateLayout *lay = nullptr) {
     return state_floats(h->m->cfg, h->st, h->B, off, lay, rs_hist(h, h->rs_up), rs_hist(h, h->rs_down));
 }
 
@@ -2956,7 +3245,7 @@ static int stream_new(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B, 
     h->lim = (atten_lim_db > 0.f) ? powf(10.f, -atten_lim_db / 20.f) : 0.f;
     h->spectral = spectral;
     if (spectral) h->lsnr_from = 0;
-    size_t off[16];
+    size_t off[kStateArrays];
     const size_t n = state_floats(m->cfg, st, (int)B, off);
     auto dev = [](auto **p, size_t bytes) {
         if (cudaMalloc(p, bytes) == cudaSuccess) return true;
@@ -3007,7 +3296,7 @@ extern "C" void dfb_stream_free(dfb_stream *h) {
 
 extern "C" int dfb_stream_reset(dfb_stream *h) {
     if (!h) return fail(DFB_ERR_INVALID, "null stream");
-    size_t off[16];
+    size_t off[kStateArrays];
     stream_state_floats(h, off);
     state_bind(h->S, h->slab, off, h->B);
     h->fed = false;
@@ -3037,6 +3326,13 @@ extern "C" int dfb_stream_set_mask_reduce(dfb_stream *h, int channels, int reduc
 // LSNR stage gating of the Rust runtime (libDF/src/tract.rs:658-672; thresholds tract.rs:180-185, DfParams of
 // deep-filter / capi.rs).  Off by default: the Python path this library mirrors does not gate.  DeepFilterNet3 only on
 // audio handles (the apply kernel gates mode 1); a spectral handle gates in k_spec_emit, for DeepFilterNet2 too.
+extern "C" int dfb_stream_set_gating_mode(dfb_stream *h, int mode) {
+    if (!h) return fail(DFB_ERR_INVALID, "null stream");
+    if (mode != -1 && mode != DFB_GATING_APPLY && mode != DFB_GATING_RUNTIME) return fail(DFB_ERR_INVALID, "gating mode %d", mode);
+    h->gating_mode = mode;
+    return DFB_OK;
+}
+
 extern "C" int dfb_stream_set_lsnr_thresholds(dfb_stream *h, int enable, float min_db_thresh, float max_db_erb_thresh,
                                               float max_db_df_thresh) {
     if (!h) return fail(DFB_ERR_INVALID, "null stream");
@@ -3359,7 +3655,7 @@ static int slots_move_rows(dfb_stream *h, cudaStream_t s) {
     for (int r = 0; r < h->n_act; r++) h->row_src[(size_t)r] = r;
     if (ops.empty()) return DFB_OK;
     dfb_model *m = h->m;
-    size_t off[16];
+    size_t off[kStateArrays];
     StateLayout lay;
     stream_state_floats(h, off, &lay);
     if (int rc = m->arena.reserve(sizeof(int2) * ops.size() + sizeof(float) * (size_t)lay.row_floats * n_mv + 1024)) return rc;
@@ -3487,6 +3783,7 @@ static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, 
     if (h->ctl_on) { io.ctl = h->d_ctl; io.ctl_gate = h->ctl_gate; }
     io.lsnr_from = h->lsnr_from;
     io.lsnr_out = d_lsnr;
+    io.runtime = (h->gating_mode >= 0 ? h->gating_mode : m->gating_mode) == DFB_GATING_RUNTIME;
     rc = m->arena.reserve(chunk_bytes_per_stream(m->cfg, st, (int)(d1n - (S.d1 > kHalo ? S.d1 - kHalo : 0)) + 1) * (size_t)h->n_act +
                               (2 << 20));
     if (rc) return rc;
@@ -3578,12 +3875,12 @@ static int rate_pass(dfb_stream *h, const float *d_in, int64_t n, bool flush, fl
     // Free rows are zeroed over their whole width by a call's first pass.  A row live in it fills its own row past its
     // samples with zeros, and only such rows turn free before the call's next pass.
     if (nb < B && n_out > 0 && col == 0) DFB_CUDA(cudaMemset2DAsync(d_out, sizeof(float) * pitch, 0, sizeof(float) * pitch, B, s));
-    size_t off[16];
+    size_t off[kStateArrays];
     stream_state_floats(h, off);
-    const ResampleIO up{d_in, h->rs_in, h->slab + off[13], n * wide, n * hop, n * hop, rs_hist(h, h->rs_up), 0, 0, n, a0, 0};
+    const ResampleIO up{d_in, h->rs_in, h->slab + off[15], n * wide, n * hop, n * hop, rs_hist(h, h->rs_up), 0, 0, n, a0, 0};
     if (!flush && (rc = launch_resample_stream(s, true, h->rs_up, nd, h->d_rs, nb, up))) return rc;
     if ((rc = stream_step(h, flush ? nullptr : h->rs_in, n, flush, h->rs_out, d_lsnr, s))) return rc;
-    const ResampleIO down{h->rs_out, d_out, h->slab + off[14], n_out * hop, pitch, pitch, rs_hist(h, h->rs_down), 0, col, n_out, a0, L};
+    const ResampleIO down{h->rs_out, d_out, h->slab + off[16], n_out * hop, pitch, pitch, rs_hist(h, h->rs_down), 0, col, n_out, a0, L};
     return launch_resample_stream(s, false, h->rs_down, nd, h->d_rs, nb, down);
 }
 
@@ -3618,7 +3915,7 @@ static int audio_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, f
 
 // (Re)allocates the state slab of a new or reset handle for its current directions, zeroed.
 static int stream_slab(dfb_stream *h) {
-    size_t off[16];
+    size_t off[kStateArrays];
     const size_t n = stream_state_floats(h, off);
     float *p = nullptr;
     if (cudaMalloc(&p, n * sizeof(float)) != cudaSuccess) return fail(DFB_ERR_OOM, "stream state allocation failed");

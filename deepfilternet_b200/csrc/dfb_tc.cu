@@ -581,12 +581,15 @@ struct GruTcParams {
     // h = 0 through the steps before it: those frames do not exist for the stream.
     const int64_t *first;
     int64_t w0;
+    // (HOLD) run flags [B][Ts]: step t of stream b runs when run[b * Ts + t0 + t] != 0; a held step keeps the state as it
+    // was, exchanges it and writes it out as that step's output
+    const unsigned char *run;
 };
 
 // XG = 1: the new state travels through L2 instead of SM to SM -- every CTA stores its slice to a global scratch piece and
 // asks the TMA engine for ONE multicast bulk copy of that piece into all CTAs of the cluster (itself included) instead of
 // kC - 1 per-peer DSMEM copies.
-template <int NS, int HH, int XG>
+template <int NS, int HH, int XG, int HOLD>
 __global__ void __launch_bounds__(GtCfg<NS, HH>::kThreads, 1) k_gru_tc(GruTcParams p) {
     using Cfg = GtCfg<NS, HH>;
     constexpr int kGtThreads = Cfg::kThreads, kGtH = HH, kGtC = Cfg::kC, NT = NS / 8;
@@ -673,7 +676,9 @@ __global__ void __launch_bounds__(GtCfg<NS, HH>::kThreads, 1) k_gru_tc(GruTcPara
         if (dbg_on) p.dbg[t * 8 + 0] = clock64();
         if (tid == 0 && t + 1 < T) mbar_expect_tx(&sm.bar_h[cur ^ 1], step_bytes);
         float2 xr = make_float2(0.f, 0.f), xz = xr, xn = xr;
+        bool held = false;
         if (active) {
+            if (HOLD) held = p.run[(int64_t)(b0 + s) * p.Ts + p.t0 + t] == 0;
             const float *xp = p.xproj + ((int64_t)(b0 + s) * p.Ts + p.t0 + t) * (3 * H) + gu;
             xr = *reinterpret_cast<const float2 *>(xp);
             xz = *reinterpret_cast<const float2 *>(xp + H);
@@ -733,9 +738,11 @@ __global__ void __launch_bounds__(GtCfg<NS, HH>::kThreads, 1) k_gru_tc(GruTcPara
             const float r0 = gt_sigmoid(xr.x + a[0] + bhr.x), r1 = gt_sigmoid(xr.y + a[1] + bhr.y);
             const float z0 = gt_sigmoid(xz.x + a[2] + bhz.x), z1 = gt_sigmoid(xz.y + a[3] + bhz.y);
             const float n0 = gt_tanh(xn.x + r0 * (a[4] + bhn.x)), n1 = gt_tanh(xn.y + r1 * (a[5] + bhn.y));
+            const float k0 = hprev0, k1 = hprev1;
             hprev0 = (1.f - z0) * n0 + z0 * hprev0;
             hprev1 = (1.f - z1) * n1 + z1 * hprev1;
             if (t < t_first) hprev0 = hprev1 = 0.f;
+            if (HOLD && held) { hprev0 = k0; hprev1 = k1; }
             unsigned short h0, l0, h1, l1;
             bf16_split(hprev0, h0, l0);
             bf16_split(hprev1, h1, l1);
@@ -811,14 +818,14 @@ static unsigned char *gru_xbuf(cudaStream_t s, size_t bytes) {
 }
 
 // function attributes (once per device) and the launch configuration of one k_gru_tc instance; `at` backs cfg.attrs
-template <int NS, int HH, int XG>
+template <int NS, int HH, int XG, int HOLD = 0>
 static int gru_tc_config(cudaLaunchConfig_t &cfg, cudaLaunchAttribute (&at)[1]) {
     using Cfg = GtCfg<NS, HH>;
     static PerDeviceOnce attr_once;
     const int smem = (int)sizeof(GruTcSmem<NS, HH>) + 1024;
     if (auto once_guard = attr_once.first()) {
-        if (Cfg::kC > 8) DFB_CUDA(cudaFuncSetAttribute(k_gru_tc<NS, HH, XG>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-        DFB_CUDA(cudaFuncSetAttribute(k_gru_tc<NS, HH, XG>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        if (Cfg::kC > 8) DFB_CUDA(cudaFuncSetAttribute(k_gru_tc<NS, HH, XG, HOLD>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+        DFB_CUDA(cudaFuncSetAttribute(k_gru_tc<NS, HH, XG, HOLD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     }
     cfg = cudaLaunchConfig_t{};
     cfg.blockDim = dim3(Cfg::kThreads);
@@ -842,7 +849,7 @@ static int gru_tc_max_clusters(int *out) {
         int rc = gru_tc_config<NS, HH, XG>(cfg, at);
         if (rc) return rc;
         cfg.gridDim = dim3((unsigned)GtCfg<NS, HH>::kC);
-        DFB_CUDA(cudaOccupancyMaxActiveClusters(&n, k_gru_tc<NS, HH, XG>, &cfg));
+        DFB_CUDA(cudaOccupancyMaxActiveClusters(&n, k_gru_tc<NS, HH, XG, 0>, &cfg));
         cached[dev & 63].store(n, std::memory_order_relaxed);
     }
     *out = n;
@@ -854,7 +861,7 @@ static int launch_gru_tc_n(cudaStream_t s, GruTcParams p) {
     using Cfg = GtCfg<NS, HH>;
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute at[1];
-    int rc = gru_tc_config<NS, HH, XG>(cfg, at);
+    int rc = p.run ? gru_tc_config<NS, HH, XG, 1>(cfg, at) : gru_tc_config<NS, HH, XG, 0>(cfg, at);
     if (rc) return rc;
     p.Bc = NS;
     const int ngroups = (p.B + NS - 1) / NS;
@@ -865,7 +872,8 @@ static int launch_gru_tc_n(cudaStream_t s, GruTcParams p) {
         if (!p.xbuf) return fail(DFB_ERR_OOM, "GRU exchange scratch");
     }
     DFB_PROF(HH == 256 ? "k_gru_tc" : "k_gru_tc512", s);
-    DFB_CUDA(cudaLaunchKernelEx(&cfg, k_gru_tc<NS, HH, XG>, p));
+    if (p.run) DFB_CUDA(cudaLaunchKernelEx(&cfg, k_gru_tc<NS, HH, XG, 1>, p));
+    else DFB_CUDA(cudaLaunchKernelEx(&cfg, k_gru_tc<NS, HH, XG, 0>, p));
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return DFB_OK;
 }
@@ -904,6 +912,7 @@ int launch_gru_tc(cudaStream_t s, const float *xproj, const float *whh, const fl
                   w ? w->t0 : 0, w ? w->Ts : T, B, T, 0, dbg};
     p.first = w ? w->first : nullptr;
     p.w0 = w ? w->w0 : 0;
+    p.run = w ? w->run : nullptr;
     if (ns == 0 && xg == -1) {
         const int rc = gru_tc_select(B, H, wide, &ns, &xg);
         if (rc) return rc;
@@ -991,6 +1000,20 @@ extern "C" int dfb_debug_gru_tc(const float *xproj, const float *whh, const floa
     if (B <= 0 || T <= 0 || t0 < 0 || (int64_t)t0 + T > Ts)
         return dfb::fail(DFB_ERR_INVALID, "gru_tc: B %d, window [%d, %d + %d) of %d frames", B, t0, t0, T, Ts);
     const dfb::GruWindow w{h0, hT, t0, Ts, first, w0};
+    return dfb::launch_gru_tc((cudaStream_t)stream, xproj, whh, bhh, res, hout, (unsigned short *)hout_hi,
+                              (unsigned short *)hout_lo, B, T, nullptr, 0, planes_res, &w, H, ns, xg);
+}
+
+// Debug aid (tests/test_gpu_gating_runtime.py): dfb_debug_gru_tc with run flags run [B][Ts] (k_gru_tc's HOLD instances)
+extern "C" int dfb_debug_gru_tc_hold(const float *xproj, const float *whh, const float *bhh, const float *res, float *hout,
+                                     void *hout_hi, void *hout_lo, int planes_res, const float *h0, float *hT, const int64_t *first,
+                                     int64_t w0, const unsigned char *run, int t0, int Ts, int B, int T, int H, int ns, int xg,
+                                     void *stream) {
+    if (!xproj || !whh || !bhh || !run || (!hout && !hout_hi) || (!hout_hi != !hout_lo))
+        return dfb::fail(DFB_ERR_INVALID, "gru_tc_hold: null argument");
+    if (B <= 0 || T <= 0 || t0 < 0 || (int64_t)t0 + T > Ts)
+        return dfb::fail(DFB_ERR_INVALID, "gru_tc_hold: B %d, window [%d, %d + %d) of %d frames", B, t0, t0, T, Ts);
+    const dfb::GruWindow w{h0, hT, t0, Ts, first, w0, run};
     return dfb::launch_gru_tc((cudaStream_t)stream, xproj, whh, bhh, res, hout, (unsigned short *)hout_hi,
                               (unsigned short *)hout_lo, B, T, nullptr, 0, planes_res, &w, H, ns, xg);
 }

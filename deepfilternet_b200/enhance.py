@@ -130,7 +130,7 @@ def _ptr(a):
 def enhance(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
             atten_lim_db: Optional[float] = None, out: Optional[Tensor] = None, *, reduce_mask: Optional[str] = None,
             sr: Optional[int] = None, post_filter_beta: Optional[float] = None, lsnr_thresholds=None,
-            return_lsnr: bool = False):
+            return_lsnr: bool = False, gating_mode: Optional[str] = None):
     """enhance.py:206-250: audio f32 CPU [C,T] @ model sr -> enhanced f32 CPU [C,T]
     (or [C, (T // hop) * hop], delayed by n_fft - hop, when ``pad`` is False).
     ``out`` (extension): optional preallocated (e.g. pinned) CPU tensor for the result.
@@ -139,8 +139,10 @@ def enhance(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
     channel on its own.
     ``sr`` (extension): the rate of ``audio`` when it is not the model's 48 kHz, as :func:`enhance_batch` takes it.
     ``post_filter_beta`` / ``lsnr_thresholds`` / ``return_lsnr`` (extensions): one value each, as :func:`enhance_batch`
-    takes them; with ``return_lsnr`` the result is ``(enhanced, lsnr)``."""
+    takes them; with ``return_lsnr`` the result is ``(enhanced, lsnr)``.  ``gating_mode`` as :func:`enhance_batch` takes it."""
     model.eval()
+    if gating_mode is not None:
+        ragged.gating_mode_code(gating_mode)
     if audio.dim() != 2:
         raise ValueError("audio must have shape [C, T]")
     if isinstance(atten_lim_db, (list, tuple, np.ndarray, Tensor)):
@@ -151,7 +153,8 @@ def enhance(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
         if lsnr_thresholds is not None:
             lsnr_thresholds = ragged._thresholds(lsnr_thresholds, "lsnr_thresholds")
         r = enhance_batch(model, df_state, [audio], pad, atten_lim_db, reduce_mask, sr=None if sr is None else [sr],
-                          post_filter_beta=post_filter_beta, lsnr_thresholds=lsnr_thresholds, return_lsnr=return_lsnr)
+                          post_filter_beta=post_filter_beta, lsnr_thresholds=lsnr_thresholds, return_lsnr=return_lsnr,
+                          gating_mode=gating_mode)
         y = (r[0] if return_lsnr else r)[0]
         if out is not None:
             if out.shape != y.shape or out.dtype != torch.float32 or out.is_cuda or not out.is_contiguous():
@@ -207,7 +210,7 @@ def enhance_device(model: DfNet, df_state: DF, audio: Tensor, pad: bool = True,
 @torch.no_grad()
 def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: bool = True,
                   atten_lim_db=None, reduce_mask: Optional[str] = None, *, sr=None, post_filter_beta=None,
-                  lsnr_thresholds=None, return_lsnr: bool = False):
+                  lsnr_thresholds=None, return_lsnr: bool = False, gating_mode: Optional[str] = None):
     """Several recordings of different lengths in one call: ``audios`` is a sequence of CPU [C_i, T_i] tensors as
     :func:`enhance` takes them, every channel one stream.  Entry i of the result equals
     ``enhance(model, df_state, audios[i], pad, atten_lim_db)``.  The batch is packed into one page-locked buffer and
@@ -224,8 +227,13 @@ def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: boo
     that entry does not gate) -- the Rust runtime's LSNR stage gating (DeepFilterNet3 topologies).  Entry i then equals
     the batch with entry i's settings given to every entry.  ``return_lsnr``: the result is ``(outputs, lsnrs)``, lsnrs[i]
     float32 [n_i] (a multi-channel entry [C_i, n_i]) with value j the LSNR in dB of the frame 10 ms output hop j carries
-    (include/dfb200.h, dfb_enhance_ragged)."""
+    (include/dfb200.h, dfb_enhance_ragged).
+    ``gating_mode`` None (the model's, :meth:`DfNet.set_gating_mode`), "apply" or "runtime": with "runtime" a gating
+    entry's decoders run only on the frames its stages let through, as the Rust runtime's do (include/dfb200.h,
+    dfb_gating_mode); entries that do not gate are computed as in "apply"."""
     model.eval()
+    if gating_mode is not None:
+        ragged.gating_mode_code(gating_mode)
     xs = list(audios)
     for i, a in enumerate(xs):
         if not isinstance(a, Tensor) or a.dim() != 2:
@@ -249,11 +257,12 @@ def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: boo
         ln = ragged.lsnr_lens(lens, srates, df_state.hop_size(), pad)
         l_off = np.concatenate(([0], np.cumsum(ln)[:-1])).astype(np.int64)
         lz = torch.empty(int(ln.sum()), dtype=torch.float32, pin_memory=pin)
-    check(_lib.lib().dfb_enhance_ragged_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
-                                             lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
-                                             out_off.ctypes.data, _ptr(groups), groups.size if groups is not None else 0, reduce,
-                                             srates.ctypes.data, _ptr(stab), lens.size, _ptr(lz), lz.numel() if lz is not None else 0,
-                                             _ptr(l_off)))
+    with model._gating(gating_mode):
+        check(_lib.lib().dfb_enhance_ragged_host(model.handle, df_state.handle, x.data_ptr(), n_in, in_off.ctypes.data,
+                                                 lens.ctypes.data, lens.size, 1 if pad else 0, lim, y.data_ptr(), n_out,
+                                                 out_off.ctypes.data, _ptr(groups), groups.size if groups is not None else 0, reduce,
+                                                 srates.ctypes.data, _ptr(stab), lens.size, _ptr(lz), lz.numel() if lz is not None else 0,
+                                                 _ptr(l_off)))
     if not return_lsnr:
         return outs
     lsnrs, k = [], 0
@@ -268,7 +277,7 @@ def enhance_batch(model: DfNet, df_state: DF, audios: Sequence[Tensor], pad: boo
 def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pad: bool = True,
                           atten_lim_db=None, out: Optional[Tensor] = None, group_sizes=None,
                           reduce_mask: Optional[str] = None, *, sr=None, post_filter_beta=None, lsnr_thresholds=None,
-                          return_lsnr: bool = False):
+                          return_lsnr: bool = False, gating_mode: Optional[str] = None):
     """Device-resident ragged batch: ``audio`` is a padded CUDA tensor [B, S] whose row b holds ``lengths[b]`` real
     samples.  Returns [B, max out_len] (asynchronous on the current stream): row b equals :func:`enhance_device` of
     ``audio[b, :lengths[b]]`` alone, and is zero beyond its own output length.  With ``out`` given, only each row's own
@@ -280,7 +289,10 @@ def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pa
     takes it; lengths and the result are in each row's own samples (dfb_enhance_ragged).
     ``atten_lim_db`` / ``post_filter_beta`` / ``lsnr_thresholds``: as :func:`enhance_batch` takes them, one per row where
     per entry (a link group's rows take one setting).  ``return_lsnr``: the result is ``(out, lsnr, lsnr_lengths)``, lsnr a
-    [B, max n] float32 CUDA tensor whose row b holds lsnr_lengths[b] values (NaN after them), as enhance_batch's."""
+    [B, max n] float32 CUDA tensor whose row b holds lsnr_lengths[b] values (NaN after them), as enhance_batch's.
+    ``gating_mode`` as :func:`enhance_batch` takes it."""
+    if gating_mode is not None:
+        ragged.gating_mode_code(gating_mode)
     if not audio.is_cuda or audio.dtype != torch.float32 or not audio.is_contiguous() or audio.dim() != 2:
         raise ValueError("enhance_device_ragged expects a contiguous float32 CUDA tensor of shape [B, S]")
     if audio.device != model.cuda_device:
@@ -313,7 +325,7 @@ def enhance_device_ragged(model: DfNet, df_state: DF, audio: Tensor, lengths, pa
         nl = int(ln.max())
         lz = torch.full((b, nl), float("nan"), dtype=torch.float32, device=audio.device)
         l_off = np.arange(b, dtype=np.int64) * nl
-    with torch.cuda.device(audio.device):
+    with torch.cuda.device(audio.device), model._gating(gating_mode):
         stream = torch.cuda.current_stream(audio.device).cuda_stream
         check(_lib.lib().dfb_enhance_ragged(model.handle, df_state.handle, audio.data_ptr(), b * s, in_off.ctypes.data,
                                             lens.ctypes.data, b, 1 if pad else 0, lim, out.data_ptr(), b * ow, out_off.ctypes.data,
@@ -416,7 +428,8 @@ LSNR_THRESH_CLI = (("min_db_thresh", -15.0), ("max_db_erb_thresh", 35.0), ("max_
 def cli_settings(args, model: DfNet) -> dict:
     """The keyword arguments of enhance / enhance_batch that --pf-beta and the threshold flags ask for: with --pf, a
     DeepFilterNet3 model's post filter takes --pf-beta (where it differs from the model's pf_beta, the plain call runs);
-    any threshold flag turns LSNR stage gating on, the flags not given taking the deep-filter binary's defaults."""
+    any threshold flag turns LSNR stage gating on, the flags not given taking the deep-filter binary's defaults, and
+    --gating-mode runtime makes the decoders skip the gated frames."""
     kw = {}
     beta = getattr(args, "pf_beta", None)
     if getattr(args, "pf", False) and model.cfg.model == "deepfilternet3" and beta is not None and beta != model.post_filter_beta:
@@ -424,6 +437,8 @@ def cli_settings(args, model: DfNet) -> dict:
     th = [getattr(args, name, None) for name, _ in LSNR_THRESH_CLI]
     if any(v is not None for v in th):
         kw["lsnr_thresholds"] = tuple(d if v is None else v for v, (_, d) in zip(th, LSNR_THRESH_CLI))
+        if getattr(args, "gating_mode", "apply") != "apply":
+            kw["gating_mode"] = args.gating_mode
     return kw
 
 
@@ -451,6 +466,9 @@ def cli_parser():
         parser.add_argument("--" + name.replace("_", "-"), type=float, default=None,
                             help=f"LSNR stage gating threshold in dB (DeepFilterNet3; default {default:g} when any threshold "
                                  "flag is given). Without any of these flags every frame is processed (no gating).")
+    parser.add_argument("--gating-mode", choices=sorted(ragged.GATING_MODES), default="apply",
+                        help="With LSNR stage gating: 'apply' runs the network on every frame and applies each frame's stage; "
+                             "'runtime' runs each decoder only on the frames its stage lets through, as the deep-filter binary does.")
     return parser
 
 

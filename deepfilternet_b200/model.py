@@ -8,6 +8,7 @@ kernels of libdfb200.so (csrc/dfb_model.cu) through the C ABI.  torch is used fo
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import glob
 import os
@@ -111,6 +112,30 @@ class DfNet(nn.Module):
         self._h = h
         self._derived = derived
         check(_lib.lib().dfb_model_set_options(self._h, int(self.post_filter), self.post_filter_beta, int(not self.run_df)))
+        self.gating_mode = "apply"
+
+    def set_gating_mode(self, mode: str) -> None:
+        """What LSNR stage gating does to the network, for every call that gates and every stream handle that follows the
+        model: "apply" (the default) applies each frame's stage to a network that runs every frame; "runtime" runs each
+        decoder only on the frames its stage lets through, as the Rust runtime does (include/dfb200.h, dfb_gating_mode).
+        ValueError for any other value."""
+        from . import ragged
+        code = ragged.gating_mode_code(mode)
+        check(_lib.lib().dfb_model_set_gating_mode(self._h, code))
+        self.gating_mode = mode
+
+    @contextlib.contextmanager
+    def _gating(self, mode: Optional[str]):
+        """The model's gating mode is ``mode`` inside the block (None: as it is), and what it was afterwards."""
+        if mode is None or mode == self.gating_mode:
+            yield
+            return
+        prev = self.gating_mode
+        self.set_gating_mode(mode)
+        try:
+            yield
+        finally:
+            self.set_gating_mode(prev)
 
     def __del__(self):
         h = getattr(self, "_h", None)

@@ -71,6 +71,17 @@ def packed_layout(shapes: Sequence[Tuple[int, int]], hop: int, pad: bool, rates=
 REDUCE_MASK = {"none": 0, "max": 1, "mean": 2}
 
 
+# include/dfb200.h dfb_gating_mode: what LSNR stage gating does to the network
+GATING_MODES = {"apply": 0, "runtime": 1}
+
+
+def gating_mode_code(mode) -> int:
+    """"apply" or "runtime" -> DFB_GATING_APPLY / DFB_GATING_RUNTIME (ValueError otherwise)."""
+    if not isinstance(mode, str) or mode not in GATING_MODES:
+        raise ValueError(f"gating_mode must be one of {sorted(GATING_MODES)}, not {mode!r}")
+    return GATING_MODES[mode]
+
+
 def reduce_code(reduce_mask) -> int:
     """None, "none", "max" or "mean" -> 0, 0, 1, 2 (ValueError otherwise)."""
     if reduce_mask is None:

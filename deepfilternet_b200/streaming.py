@@ -195,8 +195,10 @@ def need_spectral(s) -> None:
 class DfStream:
     def __init__(self, model: DfNet, df_state: DF, batch: int = 1, atten_lim_db: Optional[float] = None, channels: int = 1,
                  reduce_mask: Optional[str] = None, spectral: bool = False, sr: Optional[int] = None,
-                 slot_rates=None):
+                 slot_rates=None, gating_mode: Optional[str] = None):
         self.model, self.df_state, self.batch = model, df_state, int(batch)
+        if gating_mode is not None:
+            ragged.gating_mode_code(gating_mode)
         self.registered_rates = ()
         self.spectral = bool(spectral)
         if self.spectral and atten_lim_db is not None:
@@ -217,6 +219,8 @@ class DfStream:
                 self.add_slot_rate(r)
             if channels != 1 or ragged.reduce_code(reduce_mask):
                 self.set_mask_reduce(channels, reduce_mask)
+            if gating_mode is not None:
+                self.set_gating_mode(gating_mode)
         except Exception:
             self.__del__()   # a constructor that fails leaves no handle behind
             raise
@@ -287,6 +291,13 @@ class DfStream:
             except Exception:
                 pass
             self._h = None
+
+    def set_gating_mode(self, mode: Optional[str]) -> None:
+        """What LSNR stage gating does to this handle's network from the next call's frames on: "apply", "runtime" (each
+        decoder runs only on the frames its stage lets through, as in the Rust runtime; the frames before the switch count
+        as run frames) or None, the model's (:meth:`DfNet.set_gating_mode`; the default).  ValueError for any other value
+        (dfb_stream_set_gating_mode)."""
+        check(_lib.lib().dfb_stream_set_gating_mode(self._h, -1 if mode is None else ragged.gating_mode_code(mode)))
 
     def set_lsnr_thresholds(self, min_db_thresh: float = -10.0, max_db_erb_thresh: float = 30.0,
                             max_db_df_thresh: float = 20.0, enable: bool = True, slots=None) -> None:

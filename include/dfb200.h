@@ -252,8 +252,9 @@ int dfb_model_add_rate(dfb_model *m, int rate, const float *up_taps, int up_og, 
  *   lsnr_gating != 0   LSNR stage gating (tract.rs:658-672 apply_stages, as dfb_stream_set_lsnr_thresholds) with the
  *                      three thresholds, none NaN.
  * The streams of a link group take one setting: their entries must be equal.  Stream b's result equals that of the batch
- * with stream b's entry given to every stream, bit for bit.  Gating selects what is applied to a frame, as on streaming
- * handles: the network runs every frame (the Rust runtime skips its decoders on gated frames; see DESIGN.md section 5k).
+ * with stream b's entry given to every stream, bit for bit.  What gating does to the network follows the model's gating mode
+ * (dfb_model_set_gating_mode): in DFB_GATING_RUNTIME a gating stream's decoders run only on the frames its stages let
+ * through, as in the Rust runtime; a stream that does not gate is computed as in DFB_GATING_APPLY.
  *
  * LSNR rows (d_lsnr / h_lsnr null: no LSNR output).  lsnr_offsets is a HOST array: stream b's LSNR row,
  * dfb_enhance_lsnr_len(st, lengths[b], pad, rates[b]) floats in dB, goes to lsnr + lsnr_offsets[b].  Value j is the LSNR of
@@ -279,6 +280,21 @@ int dfb_model_add_rate(dfb_model *m, int rate, const float *up_taps, int up_og, 
  *                        topology other than DeepFilterNet3.
  *   DFB_ERR_OOM          the workspace cap (dfb_model_set_max_workspace) cannot hold the largest link group. */
 typedef enum { DFB_REDUCE_NONE = 0, DFB_REDUCE_MAX = 1, DFB_REDUCE_MEAN = 2 } dfb_reduce_mask;  /* tract.rs:95-99 */
+/* What LSNR stage gating does to the network.  DFB_GATING_APPLY (the default): the stages select what is applied to a
+ * frame and the network runs every frame.  DFB_GATING_RUNTIME, as the Rust runtime (tract.rs:478-503): wherever a stream
+ * gates, the ERB decoder runs only on the frames with min <= lsnr <= max_erb (stages "gains" and "gains + deep filter"),
+ * the DF decoder only on those that also have lsnr <= max_df.  A decoder that does not run on a frame leaves no trace of
+ * it: its GRU layers keep their states, and its time-tap layers (the DF pathway conv; convt3 and the mask head of
+ * conv_kt = 2 models) read the previous frames it ran on.  Each decoder computes what it would compute run alone on its
+ * frames, from zero states, as tract's pulsed erb_dec / df_dec graphs.  The encoder and the LSNR are the same in both
+ * modes, and so are the stage rule, the attenuation limit, the post filter and the mask reduction of link groups.  Not
+ * built: the Rust runtime's skip of the network after silent hops (tract.rs:513-525) and its pass-through below an
+ * attenuation limit of 0.01 dB (tract.rs:543-546).  Gated frames still cost decoder compute. */
+typedef enum { DFB_GATING_APPLY = 0, DFB_GATING_RUNTIME = 1 } dfb_gating_mode;
+/* The model's gating mode, read by every call that gates (dfb_enhance_ragged with a settings table, streaming and spectral
+ * handles that follow the model); a mode other than DFB_GATING_* is DFB_ERR_INVALID and changes nothing.  DeepFilterNet v1
+ * takes the mode and still refuses gating. */
+int dfb_model_set_gating_mode(dfb_model *m, int mode);
 typedef struct {
     float atten_lim_db;
     float post_filter_beta;
@@ -319,7 +335,8 @@ int dfb_debug_resample_rows(int up, const dfb_model *m, const float *d_in, const
  * dfb_stream_latency_frames() hops (the model's look-ahead) on top of the STFT's fft - hop samples: the concatenated
  * output equals dfb_enhance(pad = 0) of the concatenated input, delayed by latency * hop samples.  dfb_enhance itself
  * runs on the same time-chunked executor.  Optional stages: the post filter (dfb_model_set_options) and the Rust
- * runtime's LSNR stage gating (dfb_stream_set_lsnr_thresholds); not built: its silent-frame skip (tract.rs:516-525). */
+ * runtime's LSNR stage gating (dfb_stream_set_lsnr_thresholds), with the decoders skipping gated frames as the runtime's do
+ * in DFB_GATING_RUNTIME (dfb_stream_set_gating_mode); not built: its silent-frame skip (tract.rs:516-525). */
 typedef struct dfb_stream dfb_stream;
 /* capi.rs df_create: B independent streams on the model's device; atten_lim_db <= 0 disables the limit */
 int dfb_stream_create(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B, float atten_lim_db);
@@ -327,6 +344,10 @@ void dfb_stream_free(dfb_stream *s);                       /* capi.rs df_free */
 int dfb_stream_reset(dfb_stream *s);                       /* back to the initial state (all memories zero) */
 int64_t dfb_stream_frame_length(const dfb_stream *s);      /* capi.rs df_get_frame_length: hop size in samples */
 int64_t dfb_stream_latency_frames(const dfb_stream *s);    /* hops the output trails the input by */
+/* The handle's gating mode (dfb_gating_mode), or -1 to follow the model's (dfb_model_set_gating_mode; the default).  It
+ * takes effect from the next call's DNN frames.  A handle that switches to DFB_GATING_RUNTIME continues as if every frame
+ * before the switch had been a run frame of both decoders.  Any other mode is DFB_ERR_INVALID and changes nothing. */
+int dfb_stream_set_gating_mode(dfb_stream *s, int mode);
 /* LSNR stage gating (libDF/src/tract.rs:658-672 apply_stages; defaults -10 / 30 / 20 dB, tract.rs:180-185): per frame,
  * lsnr < min_db_thresh -> zero gains, no deep filter; > max_db_erb_thresh -> the frame passes unprocessed;
  * > max_db_df_thresh -> ERB gains only; else gains + deep filter.  Off by default (the Python path never gates);
@@ -544,7 +565,9 @@ int dfb_debug_resample_slots(int up, const dfb_stream *s, const int32_t *h_rates
  *   1  otherwise                   network gains and coefs
  * On a mask_only model stage 1 is stage 2.  Where the Rust runtime returns NULL for a skipped output, the values here are
  * defined, so a caller can apply every row as it comes.  Linked channels: each member's gains are the group's reduced mask
- * (max / mean as dfb_enhance_ragged's link groups); coefs and LSNR stay per channel. */
+ * (max / mean as dfb_enhance_ragged's link groups); coefs and LSNR stay per channel.  In DFB_GATING_RUNTIME
+ * (dfb_stream_set_gating_mode) the network gains of stages 1 / 2 and the coefs of stage 1 come from decoders that ran
+ * only on such frames, as df_process_frame_raw's do; this holds for DeepFilterNet2 and DeepFilterNet2_ll too. */
 int dfb_stream_create_spec(dfb_stream **out, dfb_model *m, dfb_state *st, int64_t B);
 int dfb_stream_process_spec(dfb_stream *s, const float *d_spec, int64_t n_frames, float *d_gains, float *d_coefs,
                             float *d_lsnr, int8_t *d_stage, void *stream);
@@ -583,6 +606,11 @@ int dfb_debug_gru_timing(dfb_model *m, int steps, long long *h_out);
 int dfb_debug_gru_tc(const float *xproj, const float *whh, const float *bhh, const float *res, float *hout, void *hout_hi,
                      void *hout_lo, int planes_res, const float *h0, float *hT, const int64_t *first, int64_t w0, int t0,
                      int Ts, int B, int T, int H, int ns, int xg, void *stream);
+/* Debug aid: dfb_debug_gru_tc with run flags run [B][Ts] (bytes, not NULL), the recurrence of the runtime gating mode:
+ * at a step whose flag is 0 the state keeps its value, is carried on and is written out (plus res) as that step's output. */
+int dfb_debug_gru_tc_hold(const float *xproj, const float *whh, const float *bhh, const float *res, float *hout, void *hout_hi,
+                          void *hout_lo, int planes_res, const float *h0, float *hT, const int64_t *first, int64_t w0,
+                          const unsigned char *run, int t0, int Ts, int B, int T, int H, int ns, int xg, void *stream);
 /* Debug aid: one launch of the BF16x3 projection GEMM on device pointers: y [M][N] (pitch ldy) = x w^T + bias with x
  * given as BF16 hi / lo planes [M][K] (pitch ldx) and w as BF16 hi / lo planes [N][K]; bias may be NULL. */
 int dfb_debug_gemm_bf16x3(const void *x_hi, const void *x_lo, int64_t ldx, const void *w_hi, const void *w_lo,
