@@ -80,6 +80,8 @@ SIGNATURES = {
     "dfb_model_free": (None, [_VP]),
     "dfb_model_forward": (_I, [_VP, _VP, _VP, _I64, _I64, _VP, _VP, _VP, _VP, _VP]),
     "dfb_apply": (_I, [_VP, _VP, _VP, _VP, _VP, _I64, _I64, _VP, _VP]),
+    "dfb_debug_apply_rows": (_I, [_VP, _VP, _VP, _I, _I, _VP, _VP, _VP, _VP, _I, _I64, _I, _I, _I, _I64, _I64P, _I64P, _VP, _I,
+                                  _VP, _I64P, _VP, _F, _F, _F, _F, _I64, _I64, _VP, _VP, _VP]),
     "dfb_model_forward_full": (_I, [_VP, _VP, _VP, _VP, _VP, _I64, _I64, _VP, _VP, _VP, _VP, _VP, _VP]),
     "dfb_enhance": (_I, [_VP, _VP, _VP, _I64, _I64, _I, _F, _VP, _VP]),
     "dfb_enhance_host": (_I, [_VP, _VP, _VP, _I64, _I64, _I, _F, _VP]),

@@ -1809,6 +1809,72 @@ static int apply_impl(dfb_model *m, dfb_state *st, const float *d_spec, const fl
     return launch_apply_synthesis(st, p, B, (cudaStream_t)stream);
 }
 
+// Debug aid: one launch_apply_synthesis with every field of ApplyParams the batch and slot executors set, the tables copied
+// from the host; it picks the kernel instance exactly as those executors' launches do (include/dfb200.h).
+extern "C" int dfb_debug_apply_rows(dfb_model *m, dfb_state *st, const float *d_spec, int spec_T, int Tv, const float *d_m,
+                                    const float *d_coefs, const float *d_alpha, const float *d_lsnr, int mc_T, int64_t B, int Tf,
+                                    int t_first, int t_emit, int64_t w0, const int64_t *h_rows, const int64_t *h_first,
+                                    const int32_t *h_links, int reduce, const float *h_ctl, const int64_t *h_ctl_sw,
+                                    const int32_t *h_ctl_gate, float th_min, float th_erb, float th_df, float atten_lim,
+                                    int64_t out_offset, int64_t out_len, float *d_audio, float *d_spec_out, void *stream) {
+    if (!m || !st || !d_spec || !d_m || !d_coefs || (!d_audio && !d_spec_out)) return fail(DFB_ERR_INVALID, "null argument");
+    if (int rcs = check_state(m, st)) return rcs;
+    if (B <= 0 || B > 65535 || Tf <= 0 || spec_T < 0 || (spec_T && spec_T < Tf) || Tv < 0 || Tv > (spec_T ? spec_T : Tf) ||
+        mc_T < 0 || (mc_T && mc_T < Tf) || t_first < 0 || t_emit < 0 || t_emit > Tf || w0 < 0 || out_len < 0)
+        return fail(DFB_ERR_INVALID, "bad geometry");
+    if ((m->cfg.model_kind == 1) != (d_alpha != nullptr))
+        return fail(DFB_ERR_INVALID, "alpha is DeepFilterNet v1's, and v1 needs it");
+    if (!h_rows && (h_first || h_links || h_ctl)) return fail(DFB_ERR_INVALID, "first, links and settings need the row table");
+    if (h_ctl && (!h_ctl_sw || !h_ctl_gate)) return fail(DFB_ERR_INVALID, "settings need their switch frames and gate flags");
+    std::vector<RaggedRow> rows;
+    std::vector<LinkRow> links;
+    std::vector<SlotCtl> ctl;
+    for (int64_t b = 0; h_rows && b < B; b++) {
+        const int64_t *r = h_rows + 3 * b;
+        if (r[0] < 0 || r[1] < 0 || r[2] < w0 || r[2] - w0 > INT32_MAX) return fail(DFB_ERR_INVALID, "bad row %lld", (long long)b);
+        rows.push_back(RaggedRow{0, 0, r[0], r[1], r[2]});
+        if (h_links) {
+            const int32_t f = h_links[2 * b], n = h_links[2 * b + 1];
+            if (n < 1 || f < 0 || f > b || b >= (int64_t)f + n || (int64_t)f + n > B)
+                return fail(DFB_ERR_INVALID, "bad link group of row %lld", (long long)b);
+            links.push_back(LinkRow{f, n});
+        }
+        if (h_ctl) {
+            const float *c = h_ctl + 7 * b;
+            ctl.push_back(SlotCtl{c[0], c[1], c[2], c[3], h_ctl_sw[b], c[4], c[5], c[6], h_ctl_gate[b]});
+        }
+    }
+    DFB_CUDA(cudaSetDevice(m->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const size_t o_first = sizeof(RaggedRow) * rows.size(), o_links = o_first + (h_first ? sizeof(int64_t) * B : 0),
+                 o_ctl = o_links + sizeof(LinkRow) * links.size(), total = o_ctl + sizeof(SlotCtl) * ctl.size();
+    std::vector<char> slab(total);
+    if (!rows.empty()) memcpy(slab.data(), rows.data(), o_first);
+    if (h_first) memcpy(slab.data() + o_first, h_first, sizeof(int64_t) * B);
+    if (!links.empty()) memcpy(slab.data() + o_links, links.data(), sizeof(LinkRow) * links.size());
+    if (!ctl.empty()) memcpy(slab.data() + o_ctl, ctl.data(), sizeof(SlotCtl) * ctl.size());
+    char *d = nullptr;
+    if (total && (cudaMalloc(&d, total) != cudaSuccess || cudaMemcpyAsync(d, slab.data(), total, cudaMemcpyHostToDevice, s) != cudaSuccess)) {
+        if (d) cudaFree(d);
+        return fail(DFB_ERR_OOM, "debug tables");
+    }
+    dfb::ApplyParams p{};
+    p.spec = (const float2 *)d_spec; p.m = d_m; p.coefs = d_coefs; p.audio = d_audio; p.spec_out = (float2 *)d_spec_out;
+    p.out_stride = out_len; p.out_len = out_len; p.out_offset = out_offset;
+    p.Tf = Tf; p.spec_T = spec_T; p.Tv = Tv; p.mc_T = mc_T; p.t_first = t_first;
+    p.mode = apply_mode(m); p.nb_df = m->cfg.nb_df; p.order = m->cfg.df_order; p.lookahead = m->cfg.df_lookahead;
+    p.atten_lim = atten_lim; p.alpha = d_alpha;
+    apply_options(m, p);
+    p.lsnr = d_lsnr; p.th_min = th_min; p.th_erb = th_erb; p.th_df = th_df;
+    p.rows = h_rows ? (const RaggedRow *)d : nullptr; p.w0 = w0; p.t_emit = t_emit;
+    p.first = h_first ? (const int64_t *)(d + o_first) : nullptr;
+    if (h_links) { p.links = (const LinkRow *)(d + o_links); p.reduce = reduce; }
+    const int rc = launch_apply_synthesis(st, p, B, s, h_ctl ? (const SlotCtl *)(d + o_ctl) : nullptr);
+    cudaStreamSynchronize(s);
+    if (d) cudaFree(d);
+    return rc;
+}
+
 extern "C" int dfb_model_forward_full(dfb_model *m, dfb_state *st, const float *d_spec, const float *d_feat_erb,
                                       const float *d_feat_spec, int64_t B, int64_t T, float *d_spec_e, float *d_m,
                                       float *d_lsnr, float *d_coefs, float *d_alpha, void *stream) {

@@ -171,6 +171,27 @@ int dfb_model_forward(dfb_model *m, const float *d_feat_erb, const float *d_feat
 int dfb_apply(dfb_model *m, dfb_state *st, const float *d_spec, const float *d_m, const float *d_coefs,
               int64_t B, int64_t T, float *d_spec_e, void *stream);
 
+/* Debug aid: one launch of the apply + ISTFT kernel with the row-level arguments the batch and slot executors pass, the
+ * kernel instance chosen as they choose it.  Window frames t = 0 .. Tf-1 (absolute w0 + t) of B streams: spec c64[B][spec_T
+ * (0: Tf)][F] of which the first Tv (0: all) rows exist; m f32[B][mc_T (0: Tf)][E], coefs f32[B][mc_T][nb_df][2 order],
+ * alpha f32[B][mc_T] (DeepFilterNet v1 only, which needs it), lsnr f32[B][mc_T] or NULL (LSNR stage gating, DeepFilterNet3
+ * only).  Frame t's samples [t hop - out_offset, + hop) are written for t >= t_first, and spec_out c64[B][Tf][F] (or NULL)
+ * receives each synthesised frame's enhanced spectrum.  HOST tables, each NULL or B entries:
+ *   rows   int64 [B][3]  out_off, out_len, Tf: stream b's output row audio[out_off, out_off + out_len) and its end (absolute
+ *                        frame Tf; a stream that has not ended in the window synthesises up to t_emit).  NULL: row b is
+ *                        audio[b out_len, (b + 1) out_len) and every stream ends at Tf;
+ *   first  int64 [B]     streaming slots' first frames (absolute), frames before them synthesise to zero;
+ *   links  int32 [B][2]  link group (first stream, n) of stream b, mask reduction `reduce` (DFB_REDUCE_MAX / _MEAN);
+ *   ctl    f32 [B][7]    lim, beta, lim0, beta0, th_min, th_erb, th_df of stream b, with ctl_sw int64 [B] (absolute switch
+ *                        frame) and ctl_gate int32 [B] (gate flag).
+ * first, links and ctl need rows.  Without ctl the thresholds and atten_lim (a factor, 0 = off) apply to every row. */
+int dfb_debug_apply_rows(dfb_model *m, dfb_state *st, const float *d_spec, int spec_T, int Tv, const float *d_m,
+                         const float *d_coefs, const float *d_alpha, const float *d_lsnr, int mc_T, int64_t B, int Tf,
+                         int t_first, int t_emit, int64_t w0, const int64_t *h_rows, const int64_t *h_first,
+                         const int32_t *h_links, int reduce, const float *h_ctl, const int64_t *h_ctl_sw,
+                         const int32_t *h_ctl_gate, float th_min, float th_erb, float th_df, float atten_lim,
+                         int64_t out_offset, int64_t out_len, float *d_audio, float *d_spec_out, void *stream);
+
 /* DfNet.forward (deepfilternet3.py:389-456): (spec, feat_erb, feat_spec) -> (spec_e, m, lsnr, coefs);
  * any of d_m / d_lsnr / d_coefs / d_alpha may be NULL. */
 int dfb_model_forward_full(dfb_model *m, dfb_state *st, const float *d_spec, const float *d_feat_erb,

@@ -296,3 +296,138 @@ def istft(X, window, hop, bX=None):
     bout[:, 1:] += by[:, :-1, hop:]
     bout += U * np.abs(out)
     return out.reshape(C, Tf * hop), bout.reshape(C, Tf * hop)
+
+
+def stage_of(lsnr, th_min, th_erb, th_df):
+    """tract.rs:658-672 (DfTract::apply_stages), element-wise: 0 zero gains (lsnr < min), 1 unprocessed (> max_erb), 2 ERB
+    gains only (> max_df), 3 gains and deep filter."""
+    l = np.asarray(lsnr)
+    return np.where(l < th_min, 0, np.where(l > th_erb, 1, np.where(l > th_df, 2, 3)))
+
+
+def reduce_link_mask(m, links, reduce):
+    """The ERB mask each stream applies: its link group's (first, n) max, or the mean as the fp32 sum in channel order times
+    fl32(1 / n) (tract.rs:881-898), computed in numpy float32 and then exact.  m [B, T, E] fp32; links None: m itself."""
+    m = np.asarray(m, np.float32)
+    if links is None:
+        return m.astype(np.float64)
+    out = np.empty(m.shape, np.float64)
+    for b, (f, n) in enumerate(links):
+        v = m[f].copy()
+        for c in range(1, n):
+            v = np.maximum(v, m[f + c]) if reduce == "max" else (v + m[f + c]).astype(np.float32)
+        if reduce != "max":
+            v = (v * (F32(1) / F32(n))).astype(np.float32)
+        out[b] = v
+    return out
+
+
+def apply_rows(spec, m, coefs, widths, window, *, mode, nb_df, order, lookahead, Tf, n_audio, post_filter=False,
+               pf_beta=0.02, mask_only=False, alpha=None, Tv=None, lsnr=None, th=(-15.0, 35.0, 35.0), atten_lim=0.0,
+               rows=None, first=None, links=None, reduce="max", ctl=None, w0=0, t_first=0, t_emit=None, out_offset=0,
+               out_len=None, hop=480):
+    """The apply + synthesis step of one window of a ragged batch or of streaming slots, row by row (the contract of
+    include/dfb200.h dfb_debug_apply_rows).  spec [B, spec_T, F] with Tv (None: spec_T) existing rows, m [B, mc_T, E],
+    coefs [B, mc_T, nb_df, O] complex, alpha / lsnr [B, mc_T] or None.  Per stream b, window frames t = 0 .. Tf - 1 are
+    absolute frames w0 + t:
+      geometry   rows[b] = (out_off, out_len, row_Tf): the stream ends at tfb = row_Tf - w0; it synthesises frames
+                 [0, Te), Te = tfb if tfb <= Tf else t_emit, and its deep-filter taps read spectrum rows [0, min(Tv, tfb)).
+                 DeepFilterNet2's masked taps apply the mask only to rows below mc_T.  rows None: Te = Tf, output row
+                 b is audio[b out_len, (b + 1) out_len);
+      link       links[b] = (first, n): the mask is the group's reduction (reduce_link_mask) and the stage follows the LSNR
+                 of the group's first stream;
+      stage      stage_of its LSNR with ctl[b]'s thresholds (gating only where ctl[b]["gate"]) or th (every row), when lsnr
+                 is given; frames before the slot's first frame (first[b] - w0) are stage 0.  Stage 0: zeros; 1: the noisy
+                 bins; 2: ERB gains on every bin; 3: the model's apply (apply).  The DeepFilterNet3 post filter applies at
+                 stages 2 and 3 only (tract.rs:617), then the limit;
+      settings   ctl[b] = dict(lim, beta, lim0, beta0, sw, th_min, th_erb, th_df, gate): from absolute frame sw on the
+                 limit lim and DeepFilterNet3 post-filter beta (0: off) are lim / beta, before it lim0 / beta0.  ctl None:
+                 atten_lim and (post_filter, pf_beta) on every frame;
+      output     the ISTFT of frames [0, Te) from zero memory: frame t's samples t hop + i - out_offset for t >= t_first,
+                 those in [0, out_len) of the row.
+    -> (Y [B, Tf, F], bound, Y written [B, Tf] bool), (audio [n_audio], bound, written [n_audio] bool)."""
+    spec = np.asarray(spec, np.complex128)
+    B, spec_T, F = spec.shape
+    mc_T = m.shape[1]
+    Tv = spec_T if Tv is None else Tv
+    t_emit = Tf if t_emit is None else t_emit
+    ml = reduce_link_mask(m, links, reduce)
+    bob = band_of_bin(widths)
+    Y = np.zeros((B, Tf, F), np.complex128)
+    bY = np.zeros((B, Tf, F))
+    wY = np.zeros((B, Tf), bool)
+    audio, baudio, waudio = np.zeros(n_audio), np.zeros(n_audio), np.zeros(n_audio, bool)
+    for b in range(B):
+        if rows is not None:
+            off, olen, rtf = rows[b]
+            tfb = rtf - w0
+            Te = tfb if tfb <= Tf else t_emit
+            Tvb = min(Tv, tfb)
+        else:
+            off, olen, Te, Tvb = b * out_len, out_len, Tf, Tv
+        if Te <= 0:
+            continue
+        lb = links[b][0] if links is not None else b
+        tz = max(first[b] - w0, 0) if first is not None else 0
+        X = spec[b, :Te]
+        g, bg = ml[b], np.zeros(ml[b].shape)
+        if post_filter and mode == 2:
+            g, bg = pf_gain_mask(ml[b])
+        gb, bgb = g[:Te][:, bob], bg[:Te][:, bob]
+        ax = np.abs(X)
+        xm, bxm = X * gb, U * ax * gb + ax * bgb
+        y, by = xm.copy(), bxm.copy()
+        if not mask_only:
+            Tn = max(Te, Tvb)
+            src = np.zeros((Tn, F), np.complex128)
+            bsrc = np.zeros((Tn, F))
+            src[:Tvb] = spec[b, :Tvb]
+            if mode == 2:       # the masked spectrum below mc_T, the bare one above
+                k = min(Tvb, mc_T)
+                gk, bgk = g[:k][:, bob], bg[:k][:, bob]
+                a = np.abs(src[:k])
+                bsrc[:k] = U * a * gk + a * bgk
+                src[:k] = src[:k] * gk
+            c = np.zeros((Tn, nb_df, order), np.complex128)
+            c[:Te] = coefs[b, :Te]
+            Yd, bYd = _deep_filter(src[None], bsrc[None], c[None], nb_df, order, lookahead, Tvb)
+            Yd, bYd = Yd[0, :Te], bYd[0, :Te]
+            if mode == 2 and alpha is not None:
+                a = np.asarray(alpha[b, :Te], np.float64)[:, None]
+                xd, bxd = xm[:, :nb_df], bxm[:, :nb_df]
+                bYd = a * bYd + (1 - a) * bxd + gamma(4) * (a * np.abs(Yd) + (1 - a) * np.abs(xd))
+                Yd = Yd * a + xd * (1 - a)
+            y[:, :nb_df], by[:, :nb_df] = Yd, bYd
+        # stages, per frame
+        stage = np.full(Te, 3)
+        c = ctl[b] if ctl is not None else None
+        if lsnr is not None and (c is None or c["gate"]):
+            t3 = (c["th_min"], c["th_erb"], c["th_df"]) if c is not None else th
+            stage = stage_of(np.asarray(lsnr[lb, :Te], np.float64), *t3)
+        stage[:min(tz, Te)] = 0
+        s2 = (stage == 2)[:, None]
+        y, by = np.where(s2, xm, y), np.where(s2, bxm, by)
+        s1 = (stage == 1)[:, None]
+        y, by = np.where(s1, X, y), np.where(s1, 0.0, by)
+        s0 = (stage == 0)[:, None]
+        y, by = np.where(s0, 0.0, y), np.where(s0, 0.0, by)
+        now = (w0 + np.arange(Te) >= c["sw"]) if c is not None else np.ones(Te, bool)
+        for t in range(Te):
+            if c is not None:
+                lim, beta = (c["lim"], c["beta"]) if now[t] else (c["lim0"], c["beta0"])
+                pf1 = mode == 1 and beta > 0
+            else:
+                lim, beta, pf1 = atten_lim, pf_beta, post_filter and mode == 1
+            if pf1 and stage[t] >= 2:
+                y[t], by[t] = pf_gain_spec(y[t], X[t], by[t], beta)
+            if lim > 0:
+                y[t], by[t] = atten_limit(X[t], y[t], by[t], lim)
+        Y[b, :Te], bY[b, :Te], wY[b, :Te] = y, by, True
+        o, bo = istft(y[None], window, hop, by[None])
+        for t in range(max(t_first, 0), Te):
+            gpos = t * hop + np.arange(hop) - out_offset
+            ok = (gpos >= 0) & (gpos < olen)
+            audio[off + gpos[ok]] = o[0, t * hop:(t + 1) * hop][ok]
+            baudio[off + gpos[ok]] = bo[0, t * hop:(t + 1) * hop][ok]
+            waudio[off + gpos[ok]] = True
+    return (Y, bY, wY), (audio, baudio, waudio)

@@ -178,3 +178,92 @@ def test_istft_and_atten_limit(ost, Tf):
     got = torch.from_numpy(X) * lim + torch.from_numpy(Y) * (1 - lim)
     out, bo = R.atten_limit(X.astype(np.complex128), Y.astype(np.complex128), np.zeros(X.shape), lim)
     assert within(got.numpy(), out, bo) <= 1
+
+
+F32 = np.float32
+TH = (-10.0, 30.0, 20.0)        # tract's default min / max_erb / max_df thresholds (fp32-exact)
+
+
+def stage_lsnr(B, T, seed, th=TH):
+    """LSNR rows that visit every stage, with values exactly at each threshold and one fp32 ulp either side."""
+    rng = np.random.default_rng(seed)
+    pick = [x for v in th for x in (np.nextafter(F32(v), F32(-np.inf)), F32(v), np.nextafter(F32(v), F32(np.inf)))]
+    pick += [F32(th[0] - 5), F32((th[0] + th[2]) / 2), F32((th[1] + th[2]) / 2), F32(th[1] + 5)]
+    return np.asarray(rng.choice(pick, (B, T)), np.float32)
+
+
+def linked_oracle_rows(spec, m, c, lsnr, w, channels, reduce, la, lim):
+    """tests/linked_oracle.py's fp32 torch statement: the link reduction, the DeepFilterNet3 apply stages on the shared mask,
+    the stage gating from each group's first channel, then the limit."""
+    import linked_oracle as LK
+    s = torch.view_as_real(torch.from_numpy(spec)).unsqueeze(1)
+    ml = LK.reduce_mask(torch.from_numpy(m).unsqueeze(1), channels, reduce)
+    e = oracle_apply(spec, ml.squeeze(1).numpy(), c, w, 1, 96, 5, la, False, False)
+    e = torch.view_as_real(torch.from_numpy(e)).unsqueeze(1)
+    out = LK.apply_stages(s, e, ml, torch.from_numpy(lsnr)[..., None], w, channels, *TH)
+    out = torch.view_as_complex(out.squeeze(1).contiguous())
+    if lim:
+        out = torch.from_numpy(spec) * lim + out * (1 - lim)
+    return out.numpy()
+
+
+@pytest.mark.parametrize("lim", [0.0, float(F32(10 ** (-12 / 20)))])
+@pytest.mark.parametrize("channels,reduce", [(1, "max"), (2, "max"), (2, "mean"), (3, "mean"), (5, "mean"), (3, "max")])
+def test_apply_rows_against_linked_oracle(ost, channels, reduce, lim):
+    """ref64's row-level apply (stages, link reduction, limit, ISTFT) and linked_oracle's fp32 torch restatement of the same
+    step agree within the bounds with K = 1, at every stage, with LSNR values exactly at each threshold and one ulp either
+    side (measured max err / bound: spectrum 0.99, 0.54 with the limit; audio 0.012)."""
+    w = ost.erb_widths()
+    B, T = 2 * channels, 23
+    spec, m, c = random_apply_inputs(B, T, 96, 5, seed=channels * 7 + len(reduce))
+    lsnr = stage_lsnr(B, T, seed=channels)
+    links = [(b - b % channels, channels) for b in range(B)]
+    (Y, bY, wY), (a, ba, wa) = R.apply_rows(spec, m, c, w, ost.fft_window(), mode=1, nb_df=96, order=5, lookahead=2, Tf=T,
+                                            n_audio=B * T * HOP, lsnr=lsnr, th=TH, atten_lim=lim, links=links, reduce=reduce,
+                                            out_len=T * HOP)
+    assert wY.all() and wa.all()
+    st = R.stage_of(lsnr[::channels].repeat(channels, 0), *TH)
+    assert all((st == k).any() for k in range(4))
+    got = linked_oracle_rows(spec, m, c, lsnr, w, channels, reduce, 2, lim)
+    rs, ra = within(got, Y, bY), within(ost.synthesis(got.astype(np.complex64)).reshape(-1), a, ba)
+    print(f"err/bound spectrum {rs:.3g} audio {ra:.3g}")
+    assert rs <= 1 and ra <= 1
+
+
+def test_apply_rows_bounds_see_stage_and_switch_errors(ost):
+    """The row-level bounds are tight enough for the errors the GPU tests must catch: an LSNR exactly at a threshold taken
+    to the other side (a comparison written with <= / >=), a settings switch one frame late, a slot's first frame
+    zeroed, and a link mean summed in another order, each leave the bound of the correct reference."""
+    w, win = ost.erb_widths(), ost.fft_window()
+    B, T = 3, 20
+    spec, m, c = random_apply_inputs(B, T, 96, 5, seed=5)
+    lsnr = np.full((B, T), F32(0.0), np.float32)
+    kw = dict(mode=1, nb_df=96, order=5, lookahead=2, Tf=T, n_audio=B * T * HOP, th=TH, out_len=T * HOP)
+    ref = R.apply_rows(spec, m, c, w, win, lsnr=lsnr, **kw)
+    for th, side in zip(TH, (-np.inf, np.inf, np.inf)):
+        eq = lsnr.copy()
+        eq[:, 7] = F32(th)
+        (Y, bY, _), (a, ba, _) = R.apply_rows(spec, m, c, w, win, lsnr=eq, **kw)
+        moved = eq.copy()
+        moved[:, 7] = np.nextafter(F32(th), F32(side))      # what the flipped comparison computes at equality
+        (Ym, _, _), (am, _, _) = R.apply_rows(spec, m, c, w, win, lsnr=moved, **kw)
+        assert within(Ym, Y, bY) > 1e3 and within(am, a, ba) > 1e3
+    ctl = [dict(lim=0.25, beta=0.0, lim0=0.0, beta0=0.02, sw=9, th_min=0.0, th_erb=0.0, th_df=0.0, gate=0)] * B
+    rows = [(b * T * HOP, T * HOP, 100) for b in range(B)]
+    (Y, bY, _), (a, ba, _) = R.apply_rows(spec, m, c, w, win, ctl=ctl, rows=rows, **kw)
+    late = [dict(ctl[0], sw=10)] * B
+    (Ym, _, _), (am, _, _) = R.apply_rows(spec, m, c, w, win, ctl=late, rows=rows, **kw)
+    assert within(Ym, Y, bY) > 1e3 and within(am, a, ba) > 1e3
+    first = [4] * B
+    (Y, bY, _), _ = R.apply_rows(spec, m, c, w, win, rows=rows, first=first, **kw)
+    (Ym, _, _), _ = R.apply_rows(spec, m, c, w, win, rows=rows, first=[5] * B, **kw)
+    assert within(Ym, Y, bY) > 1e3
+    links = [(0, 3)] * 3
+    m = m.copy()
+    m[0, 1::4], m[1:, 1::4] = 1.0, F32(0.4 * 2.0 ** -23)      # the reordered sum rounds 1 up by one ulp
+    (Y, bY, _), _ = R.apply_rows(spec, m, c, w, win, links=links, reduce="mean", **kw)
+    rev = np.ascontiguousarray(m[::-1])
+    mean_rev = ((rev[0] + rev[1]).astype(np.float32) + rev[2]).astype(np.float32) * (F32(1) / F32(3))
+    assert (mean_rev != R.reduce_link_mask(m, links, "mean")[0]).any()
+    (Ym, _, _), _ = R.apply_rows(spec, np.broadcast_to(mean_rev, m.shape).copy(), c, w, win, **kw)
+    assert within(Ym, Y, bY) > 1.5
