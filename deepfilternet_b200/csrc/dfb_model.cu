@@ -1411,6 +1411,16 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         erb_run = rt; df_run = rt + o1; erb_src = reinterpret_cast<int *>(rt + o2); df_pos = reinterpret_cast<int *>(rt + o3);
         df_n = reinterpret_cast<int *>(rt + o4); gP = reinterpret_cast<float *>(rt + o5); gQ = reinterpret_cast<float *>(rt + o6);
         int64_t *erb_first = reinterpret_cast<int64_t *>(rt + o7);
+        // the window's gating buffers; bytes and integers fetched as the float words that hold them (lane_rt's 256-byte
+        // alignment keeps ceil(M / 4) words of the flag bytes in bounds)
+        auto word = [](const void *p) { return reinterpret_cast<const float *>(p); };
+        m->dbg["lsnr"] = {d_lsnr, M}; m->dbg["m"] = {d_m, M * E}; m->dbg["coefs"] = {d_coefs, (int64_t)M * Wq};
+        m->dbg["gate_erb_run"] = {word(erb_run), (M + 3) / 4}; m->dbg["gate_df_run"] = {word(df_run), (M + 3) / 4};
+        m->dbg["gate_erb_src"] = {word(erb_src), M}; m->dbg["gate_df_pos"] = {word(df_pos), M};
+        m->dbg["gate_df_n"] = {word(df_n), B}; m->dbg["gate_erb_first"] = {word(erb_first), 2 * (int64_t)B};
+        m->dbg["gate_P"] = {gP, (int64_t)B * Tp * Wc}; m->dbg["gate_Q"] = {gQ, (int64_t)B * Tp * Wq};
+        // the ERB recurrence's output, as the BF16 planes erb_out reads (its fp32 form, g_b, is not always written)
+        m->dbg["erb_gru_hi"] = {word(f.gb_hi), M * H / 2}; m->dbg["erb_gru_lo"] = {word(f.gb_lo), M * H / 2};
         GatePlan gp{d_lsnr, gate->ctl, gate->links, first, W0, {gate->th[0], gate->th[1], gate->th[2]}, gate->gate_all, T, Rc,
                     erb_run, df_run, erb_src, df_pos, df_n, c.conv_kt > 1 ? gate->t_run + tw_run - 1 : nullptr, tw_run,
                     gate->valid ? 0 : 1, erb_first};

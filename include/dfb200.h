@@ -661,7 +661,15 @@ int dfb_debug_spec_ingest(dfb_state *st, const float *d_spec, int64_t n, const i
                           int nb_df, float *d_erb_db, float *d_bins, void *stream);
 /* Debug aid for parity tests: copies the named activation of the LAST forward pass on this handle
  * (e0,e1,e2,e3,c0,c1,emb_in,emb,dec_emb,d3,d2,d1,dfc) to the host; returns the element count
- * (or a negative dfb_status).  Valid until the next call on the handle. */
+ * (or a negative dfb_status).  Valid until the next call on the handle.
+ * A window run in runtime gating mode (dfb_model_set_gating_mode) adds, for its B rows of T frames (M = B T):
+ *   lsnr [B][T], m [B][T][nb_erb], coefs [B][T][nb_df][2 df_order]: the window's outputs;
+ *   gate_erb_run, gate_df_run: run flags, one byte per frame [B][T], fetched as ceil(M / 4) floats;
+ *   gate_erb_src, gate_df_pos: int32 [B][T] (the last ERB run frame, -1: none; DF run frames before t);
+ *   gate_df_n: int32 [B];  gate_erb_first: int64 [B] (2 B floats), the first frame the kt = 2 layers read;
+ *   gate_P [B][Tp][nb_df * 64], gate_Q [B][Tp][nb_df][2 df_order]: the compacted DF pathway rows and their conv, with
+ *   Tp = df_pathway_kt - 1 + new frames;
+ *   erb_gru_hi, erb_gru_lo: the ERB recurrence's output [B][T][emb_hidden] as BF16 planes (M emb_hidden / 2 floats each). */
 int64_t dfb_model_debug_fetch(dfb_model *m, const char *name, float *h_out, int64_t max_numel);
 /* bytes of device workspace the model handle currently owns (grow-only arena) */
 int64_t dfb_model_workspace_bytes(const dfb_model *m);
