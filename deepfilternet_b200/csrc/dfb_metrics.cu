@@ -1,6 +1,7 @@
 // dfb_metrics.cu -- batched speech-quality metrics of a ragged batch (dfb_metrics* in include/dfb200.h; DESIGN.md section 5j):
 // SI-SDR (DeepFilterNet/df/evaluation_utils.py si_sdr_speechmetrics), STOI (df/stoi.py stoi, after io.resample to 10 kHz)
-// and segmental SNR (df/sepm.py SNRseg, after io.resample to 16 kHz).
+// segmental SNR (df/sepm.py SNRseg, after io.resample to 16 kHz), and the two spectral distances of df/sepm.py's composite
+// measure on the same 16 kHz rows: LLR (sepm.llr) and WSS (sepm.wss).
 //
 // One call is a fixed sequence of launches, with no host round trip between them:
 //   k_resample_rows (dfb_dsp.cu)  clean and degraded rows -> 10 kHz / 16 kHz, one launch per signal
@@ -11,8 +12,13 @@
 //                                 (never materialised): the 15 third-octave band magnitudes
 //   k_stoi_seg                    one warp per 30-frame segment: the sum over bands of the clipped, normalised correlations
 //   k_ssnr                        one warp per 480-sample frame at 16 kHz: the clipped segmental SNR (fp64)
+//   k_llr                         one warp per 480-sample frame at 16 kHz: the log-likelihood ratio of the order-16 LPC
+//                                 models of both signals (fp64)
+//   k_wss                         one CTA per 480-sample frame at 16 kHz: a 1024-point fp64 FFT of both signals, the 25
+//                                 critical-band energies and Klatt's weighted spectral slope distance (fp64)
 //   k_sisdr                       one CTA per 4096-sample chunk: fp64 sums r.r, r.e, e.e
-//   k_metrics_final               one CTA per entry: the per-entry means / SI-SDR from the frame, segment and chunk values
+//   k_metrics_final               one CTA per entry: the per-entry means / SI-SDR from the frame, segment and chunk values,
+//                                 and LLR / WSS as the mean of the round(0.95 T) smallest frame values (a radix select)
 // Every per-entry sum runs in an order fixed relative to the entry's start (per-thread strided sums, then a fixed shuffle
 // and shared-memory tree), with no atomics, so an entry's results are the same bits wherever and with whatever it is batched.
 #include <algorithm>
@@ -30,6 +36,9 @@ constexpr int kStoiFs = 10000, kSsnrFs = 16000;
 constexpr int kStoiFrame = 256, kStoiHop = 128, kStoiFft = 512, kStoiBands = 15, kStoiSeg = 30;
 constexpr int kSsnrWin = 480, kSsnrHop = 120;            // round(0.03 fs), floor(0.25 * 0.03 fs) at 16 kHz
 constexpr int kSisdrChunk = 4096;
+constexpr int kLpcOrder = 16;                            // sepm.llr's P at fs >= 10 kHz
+constexpr int kWssFft = 1024, kWssBins = 512, kWssBands = 25;   // 2^ceil(log2(2 * 480)); bins 0 .. 511 (the last is dropped)
+constexpr int kMaxCritTaps = 1024;                       // nonzero critical-band filter weights (about 600 are used)
 constexpr int kStftFrames = 4;                           // STFT frames per CTA of k_stoi_stft (two signals each)
 constexpr float kEps64f = 2.220446049250313e-16f;        // np.finfo(float).eps, as df/stoi.py adds it to float32 tensors
 constexpr double kEps64 = 2.220446049250313e-16;         // np.finfo(np.float64).eps (sepm.SNRseg)
@@ -37,6 +46,8 @@ constexpr double kEps32 = 1.1920928955078125e-07;        // np.finfo(np.float32)
 
 __constant__ float c_w256[kStoiFrame];   // torch.hann_window(258, periodic=False)[1:-1]
 __constant__ double c_wss[kSsnrWin];     // SNRseg's hannWin: 0.5 (1 - cos(2 pi n / 481)), n = 1 .. 480
+__constant__ double c_crit[kMaxCritTaps]; // critical-band filter weights of band i at bins [crit_lo[i], crit_lo[i] + crit_n[i])
+__constant__ int c_crit_lo[kWssBands], c_crit_n[kWssBands], c_crit_off[kWssBands];
 
 // One entry of a call, planned on the host.
 struct MetEntry {
@@ -46,7 +57,9 @@ struct MetEntry {
     int64_t fo;             // first STOI frame: energies en[fo ..], kept list kidx[fo ..], segments seg[fo ..], bands at 15 fo
     int64_t so;             // first SSNR frame value
     int64_t co;             // first SI-SDR chunk
+    int64_t cf;             // first LLR / WSS frame value
     int nfr, pad_front, pad_end, nfs, nch;
+    int nct, kct;           // LLR / WSS frames T = (t16 - 480) / 120 (0 when t16 < 480) and k = round(0.95 T)
 };
 // What the device finds out about an entry's STOI (dfb_debug_metrics_counts reads it back).
 struct MetState { int nk, s0, lc, nf; };
@@ -58,6 +71,8 @@ struct MetBufs {
     int *kidx;
     double *ss;
     double *ch;   // [3][chunks]
+    double *llr, *wss;   // per-frame distortions at cf
+    const double2 *fft_tw;   // e^(-2 pi i m / 1024), m = 0 .. 1023
     MetState *st;
     int64_t n_fr, n_ch;
 };
@@ -268,6 +283,219 @@ __global__ void __launch_bounds__(256) k_ssnr(const MetEntry *__restrict__ ents,
     }
 }
 
+// ---- df/sepm.py's composite measure: LLR and WSS on the 16 kHz rows (frame i: samples [120 i, 120 i + 480)) ----
+
+// sepm.lpcoeff's Levinson-Durbin on the fp64 lags r (the error floored at eps), returned as the reference returns it:
+// A = [1, -a_1 .. -a_16] in float32.  Fully unrolled, so every array stays in registers.
+__device__ __forceinline__ void levinson(const double (&r)[kLpcOrder + 1], float (&A)[kLpcOrder + 1]) {
+    double a[kLpcOrder];
+    double E = r[0];
+#pragma unroll
+    for (int i = 0; i < kLpcOrder; i++) {
+        double sum = 0.0;
+#pragma unroll
+        for (int j = 0; j < i; j++) sum += a[j] * r[i - j];
+        const double k = (r[i + 1] - sum) / fmax(E, kEps64);
+        double na[kLpcOrder];
+#pragma unroll
+        for (int j = 0; j < i; j++) na[j] = a[j] - k * a[i - 1 - j];
+#pragma unroll
+        for (int j = 0; j < i; j++) a[j] = na[j];
+        a[i] = k;
+        E = (1.0 - k * k) * E;
+    }
+    A[0] = 1.f;
+#pragma unroll
+    for (int j = 0; j < kLpcOrder; j++) A[j + 1] = (float)(-a[j]);
+}
+
+// A' toeplitz(R) A in fp64 from float32 operands.
+__device__ __forceinline__ double toeplitz_form(const float (&A)[kLpcOrder + 1], const float (&R)[kLpcOrder + 1]) {
+    double s = 0.0;
+#pragma unroll
+    for (int i = 0; i <= kLpcOrder; i++) {
+        double v = 0.0;
+#pragma unroll
+        for (int j = 0; j <= kLpcOrder; j++) v = fma((double)R[i > j ? i - j : j - i], (double)A[j], v);
+        s = fma((double)A[i], v, s);
+    }
+    return s;
+}
+
+// grid (ceil(max T / 4), B), 128 threads: warp w of CTA x is frame i = 4 x + w of entry blockIdx.y.  sepm.llr at 16 kHz:
+// the autocorrelation lags 0 .. 16 of each windowed frame (w_n x_n in fp64), its LPC model, then
+// llr[cf + i] = ln(A_d' toeplitz(R_c) A_d / (A_c' toeplitz(R_c) A_c + eps)), 1000 standing in for a ratio <= 0.
+__global__ void __launch_bounds__(128) k_llr(const MetEntry *__restrict__ ents, MetBufs b) {
+    constexpr int NP = kSsnrWin + kLpcOrder;   // the frame, then 16 zeros for the lags that run past it
+    __shared__ double s_x[4][NP];
+    const MetEntry e = ents[blockIdx.y];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int i = blockIdx.x * 4 + w;
+    if (i >= e.nct) return;
+    double *x = s_x[w];
+    float A[2][kLpcOrder + 1], Rc[kLpcOrder + 1];
+#pragma unroll
+    for (int sig = 0; sig < 2; sig++) {
+        const float *src = (sig ? b.y16 : b.x16) + e.o16 + (int64_t)i * kSsnrHop;
+        __syncwarp();
+        for (int n = lane; n < NP; n += 32) x[n] = n < kSsnrWin ? c_wss[n] * (double)__ldg(src + n) : 0.0;
+        __syncwarp();
+        double r[kLpcOrder + 1];
+#pragma unroll
+        for (int k = 0; k <= kLpcOrder; k++) r[k] = 0.0;
+        for (int n = lane; n < kSsnrWin; n += 32) {
+            const double xn = x[n];
+#pragma unroll
+            for (int k = 0; k <= kLpcOrder; k++) r[k] = fma(xn, x[n + k], r[k]);
+        }
+#pragma unroll
+        for (int k = 0; k <= kLpcOrder; k++) r[k] = warp_sum(r[k]);
+        levinson(r, A[sig]);
+        if (sig == 0) {
+#pragma unroll
+            for (int k = 0; k <= kLpcOrder; k++) Rc[k] = (float)r[k];
+        }
+    }
+    if (lane == 0) {
+        double frac = toeplitz_form(A[1], Rc) / (toeplitz_form(A[0], Rc) + kEps64);
+        if (frac <= 0.0) frac = 1000.0;
+        b.llr[e.cf + i] = log(frac);
+    }
+}
+
+__device__ __forceinline__ double2 cmul(double2 a, double2 b) { return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
+
+// In-place 1024-point complex FFT of z (shared) by the CTA's 256 threads: five Stockham radix-4 stages, one butterfly per
+// thread and stage; tw[m] = e^(-2 pi i m / 1024).
+__device__ __forceinline__ void fft1024(double2 *z, const double2 *__restrict__ tw) {
+    const int j = threadIdx.x;
+#pragma unroll 1
+    for (int ns = 1; ns < kWssFft; ns *= 4) {
+        const int jm = j & (ns - 1), step = kWssFft / (4 * ns);
+        double2 v[4];
+#pragma unroll
+        for (int r = 0; r < 4; r++) {
+            v[r] = z[j + r * (kWssFft / 4)];
+            if (r) v[r] = cmul(v[r], __ldg(tw + r * jm * step));
+        }
+        const double2 a0 = make_double2(v[0].x + v[2].x, v[0].y + v[2].y), a1 = make_double2(v[0].x - v[2].x, v[0].y - v[2].y);
+        const double2 a2 = make_double2(v[1].x + v[3].x, v[1].y + v[3].y), a3 = make_double2(v[1].x - v[3].x, v[1].y - v[3].y);
+        const int d = (j - jm) * 4 + jm;
+        __syncthreads();   // every thread has read its inputs
+        z[d] = make_double2(a0.x + a2.x, a0.y + a2.y);
+        z[d + ns] = make_double2(a1.x + a3.y, a1.y - a3.x);          // a1 - i a3
+        z[d + 2 * ns] = make_double2(a0.x - a2.x, a0.y - a2.y);
+        z[d + 3 * ns] = make_double2(a1.x - a3.y, a1.y + a3.x);      // a1 + i a3
+        __syncthreads();
+    }
+}
+
+// findLocPeaks for the band of this lane (slopes on lanes 0 .. 23, energies on lanes 0 .. 24), its exact rule: for a
+// rising slope, walk up while the slope rises (to band 24 at most) and take energy[n - 1]; otherwise walk down while it
+// does not rise and take energy[n + 1].  The walks are a ballot and a find-first-set.
+__device__ __forceinline__ double loc_peak(double slope, double en, int lane) {
+    const unsigned rise = __ballot_sync(0xffffffffu, lane < kWssBands - 1 && slope > 0.0);
+    int src;
+    if ((rise >> lane) & 1u) {
+        const unsigned m = ~rise & ((1u << (kWssBands - 1)) - 1u) & (~0u << lane);
+        src = (m ? __ffs(m) - 1 : kWssBands - 1) - 1;
+    } else {
+        const unsigned m = rise & (lane < 31 ? (2u << lane) - 1u : ~0u);
+        src = (m ? 31 - __clz(m) : -1) + 1;
+    }
+    return __shfl_sync(0xffffffffu, en, src & 31);
+}
+
+// grid (max T, B), 256 threads: frame i = blockIdx.x of entry blockIdx.y.  sepm.wss at 16 kHz: both windowed frames
+// w_n (x_n + eps) in fp64 as one complex 1024-point FFT (clean real, degraded imaginary), the power of bins 0 .. 511 of
+// each, the 25 critical-band energies in dB (clamped at -100), their 24 slopes, Klatt's weights (Kmax 20, Klocmax 1)
+// averaged over both signals, and wss[cf + i] = sum W (slope_c - slope_d)^2 / sum W.
+__global__ void __launch_bounds__(256) k_wss(const MetEntry *__restrict__ ents, MetBufs b) {
+    __shared__ double2 z[kWssFft];
+    const MetEntry e = ents[blockIdx.y];
+    const int i = blockIdx.x;
+    if (i >= e.nct) return;
+    const float *c = b.x16 + e.o16 + (int64_t)i * kSsnrHop, *d = b.y16 + e.o16 + (int64_t)i * kSsnrHop;
+    for (int n = threadIdx.x; n < kWssFft; n += blockDim.x) {
+        double2 v = make_double2(0.0, 0.0);
+        if (n < kSsnrWin) {
+            const double w = c_wss[n];
+            v.x = w * ((double)__ldg(c + n) + kEps64);
+            v.y = w * ((double)__ldg(d + n) + kEps64);
+        }
+        z[n] = v;
+    }
+    __syncthreads();
+    fft1024(z, b.fft_tw);
+    if (threadIdx.x >= 32) return;
+    const int lane = threadIdx.x;
+    double ec = 0.0, ed = 0.0;
+    if (lane < kWssBands) {
+        const int lo = c_crit_lo[lane], nb = c_crit_n[lane], off = c_crit_off[lane];
+        for (int t = 0; t < nb; t++) {
+            const int k = lo + t;
+            const double2 zk = z[k], zn = z[(kWssFft - k) & (kWssFft - 1)];
+            // X_k = (Z_k + conj Z_-k) / 2, Y_k = (Z_k - conj Z_-k) / 2i
+            const double xr = 0.5 * (zk.x + zn.x), xi = 0.5 * (zk.y - zn.y);
+            const double yr = 0.5 * (zk.y + zn.y), yi = 0.5 * (zn.x - zk.x);
+            const double g = c_crit[off + t];
+            ec = fma(g, xr * xr + xi * xi, ec);
+            ed = fma(g, yr * yr + yi * yi, ed);
+        }
+    }
+    double lc = 10.0 * log10(ec), ld = 10.0 * log10(ed);
+    if (!(lc >= -100.0)) lc = -100.0;   // log10(0) = -inf
+    if (!(ld >= -100.0)) ld = -100.0;
+    const double sc = __shfl_down_sync(0xffffffffu, lc, 1) - lc, sd = __shfl_down_sync(0xffffffffu, ld, 1) - ld;
+    double mc = lane < kWssBands ? lc : -INFINITY, md = lane < kWssBands ? ld : -INFINITY;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        mc = fmax(mc, __shfl_xor_sync(0xffffffffu, mc, o));
+        md = fmax(md, __shfl_xor_sync(0xffffffffu, md, o));
+    }
+    const double pc = loc_peak(sc, lc, lane), pd = loc_peak(sd, ld, lane);
+    double num = 0.0, den = 0.0;
+    if (lane < kWssBands - 1) {
+        const double wc = 20.0 / ((20.0 + mc) - lc) * (1.0 / ((1.0 + pc) - lc));
+        const double wd = 20.0 / ((20.0 + md) - ld) * (1.0 / ((1.0 + pd) - ld));
+        const double W = (wc + wd) / 2.0;
+        num = W * ((sc - sd) * (sc - sd));
+        den = W;
+    }
+    num = warp_sum(num);
+    den = warp_sum(den);
+    if (lane == 0) b.wss[e.cf + i] = num / den;
+}
+
+// Order-preserving key of a double: a larger value has a larger key.
+__device__ __forceinline__ unsigned long long okey(double v) {
+    const unsigned long long u = (unsigned long long)__double_as_longlong(v);
+    return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+}
+
+// The mean of the k smallest of v[0 .. n) (1 <= k <= n) by the CTA, independent of their order: a bitwise radix select of
+// the k-th smallest key t (64 counting passes), then (sum of the values below t in a fixed order + (k - their count) t) / k.
+__device__ double trimmed_mean(const double *__restrict__ v, int n, int k, double *sm) {
+    unsigned long long t = 0;
+    for (int bit = 63; bit >= 0; bit--) {
+        const unsigned long long hi = t | ((1ull << bit) - 1ull);   // the largest key with t's prefix and a 0 here
+        int c = 0;
+        for (int j = threadIdx.x; j < n; j += blockDim.x) c += okey(v[j]) <= hi;
+        c = block_sum(c, reinterpret_cast<int *>(sm));
+        if (c < k) t |= 1ull << bit;
+    }
+    double s = 0.0;
+    int c = 0;
+    for (int j = threadIdx.x; j < n; j += blockDim.x) {
+        const double x = v[j];
+        if (okey(x) < t) { s += x; c++; }
+    }
+    s = block_sum(s, sm);
+    c = block_sum(c, reinterpret_cast<int *>(sm));
+    const double tv = __longlong_as_double((long long)((t >> 63) ? (t & 0x7fffffffffffffffull) : ~t));
+    return (s + (double)(k - c) * tv) / (double)k;
+}
+
 // grid (ceil(max chunks), B), 256 threads: chunk k of entry blockIdx.y, samples [4096 k, 4096 k + 4096): fp64 sums of
 // r r, r e and e e (each product of two floats is exact in fp64).
 __global__ void __launch_bounds__(256) k_sisdr(const MetEntry *__restrict__ ents, MetBufs b) {
@@ -290,7 +518,7 @@ __global__ void __launch_bounds__(256) k_sisdr(const MetEntry *__restrict__ ents
     }
 }
 
-// grid B, 256 threads: out[row][b] for the metrics of `bits`, rows in the order SI-SDR, STOI, SSNR.
+// grid B, 256 threads: out[row][b] for the metrics of `bits`, rows in the order SI-SDR, STOI, SSNR, LLR, WSS.
 __global__ void __launch_bounds__(256) k_metrics_final(const MetEntry *__restrict__ ents, MetBufs b, int bits, float *out, int64_t B) {
     __shared__ double sm[32];
     const MetEntry e = ents[blockIdx.x];
@@ -326,6 +554,13 @@ __global__ void __launch_bounds__(256) k_metrics_final(const MetEntry *__restric
         for (int k = threadIdx.x; k < n; k += blockDim.x) s += b.ss[e.so + k];
         s = block_sum(s, sm);
         if (threadIdx.x == 0) out[row * B + blockIdx.x] = n > 0 ? (float)(s / n) : __int_as_float(0x7fc00000);
+        row++;
+    }
+    for (int m = 0; m < 2; m++) {
+        if (!(bits & (m ? DFB_METRIC_WSS : DFB_METRIC_LLR))) continue;
+        const double v = e.nct > 0 ? trimmed_mean((m ? b.wss : b.llr) + e.cf, e.nct, e.kct, sm) : 0.0;
+        if (threadIdx.x == 0) out[row * B + blockIdx.x] = e.nct > 0 ? (float)v : __int_as_float(0x7fc00000);
+        row++;
     }
 }
 
@@ -352,6 +587,44 @@ StoiBands stoi_bands() {
     return b;
 }
 
+// The 25 critical bands of D. H. Klatt, "Prediction of perceived phonetic distance from critical-band spectra: a first
+// step", Proc. IEEE ICASSP 1982, pp. 1278-1281: centre frequencies and bandwidths in Hz, as the weighted spectral slope
+// measure uses them (7 bands of 70 Hz, then each band starting where the previous one ends).
+constexpr double kCritCentre[kWssBands] = {50.0,    120.0,   190.0,   260.0,   330.0,   400.0,   470.0,   540.0,   617.372,
+                                           703.378, 798.717, 904.128, 1020.38, 1148.30, 1288.72, 1442.54, 1610.70, 1794.16,
+                                           1993.93, 2211.08, 2446.71, 2701.97, 2978.04, 3276.17, 3597.63};
+constexpr double kCritWidth[kWssBands] = {70.0,    70.0,    70.0,    70.0,    70.0,    70.0,    70.0,    77.3724, 86.0056,
+                                          95.3398, 105.411, 116.256, 127.914, 140.423, 153.823, 168.154, 183.457, 199.776,
+                                          217.153, 235.631, 255.255, 276.072, 298.126, 321.465, 346.136};
+
+// The critical-band filters over the 512 kept bins at 16 kHz: band i weighs bin j by
+// exp(-11 ((j - floor(f0)) / bw)^2 + ln(70 / width_i)), f0 and bw the centre and width in bins, where that exceeds the
+// filter's -30 dB point exp(-30 / (2 * 2.303)); each band's nonzero weights are one contiguous run of bins.
+struct CritFilters { double w[kMaxCritTaps]; int lo[kWssBands], n[kWssBands], off[kWssBands]; };
+bool crit_filters(CritFilters &f) {
+    const double min_factor = std::exp(-30.0 / (2.0 * 2.303));
+    int used = 0;
+    for (int i = 0; i < kWssBands; i++) {
+        const double f0 = std::floor(kCritCentre[i] / (kSsnrFs / 2.0) * kWssBins);
+        const double bw = kCritWidth[i] / (kSsnrFs / 2.0) * kWssBins;
+        const double norm = std::log(kCritWidth[0]) - std::log(kCritWidth[i]);
+        f.lo[i] = -1;
+        f.n[i] = 0;
+        f.off[i] = used;
+        for (int j = 0; j < kWssBins; j++) {
+            const double q = (j - f0) / bw;
+            const double w = std::exp(-11.0 * (q * q) + norm);
+            if (!(w > min_factor)) continue;
+            if (f.lo[i] < 0) f.lo[i] = j;
+            if (j != f.lo[i] + f.n[i] || used >= kMaxCritTaps) return false;
+            f.w[used++] = w;
+            f.n[i]++;
+        }
+        if (f.lo[i] < 0) f.lo[i] = 0;
+    }
+    return true;
+}
+
 }  // namespace
 }  // namespace dfb
 
@@ -369,6 +642,9 @@ struct dfb_metrics {
     Arena arena;                  // per-call workspace, grown when a call needs more
     int64_t last_b = 0;           // entries of the last call (dfb_debug_metrics_counts)
     MetState *last_st = nullptr;  // their STOI states, inside the arena
+    double2 *d_fft_tw = nullptr;  // twiddles of WSS's 1024-point fp64 FFT
+    std::vector<int64_t> last_nct;             // LLR / WSS frames of each entry of the last call (dfb_debug_metrics_frames)
+    double *last_llr = nullptr, *last_wss = nullptr;   // their per-frame values, inside the arena
 };
 
 namespace {
@@ -390,17 +666,17 @@ int check_taps(int sr, int to, const float *taps, int og, int nw, int width, int
 struct MetPlan {
     std::vector<MetEntry> ents;
     std::vector<RateRow> rows;
-    int64_t n10 = 0, n16 = 0, n_fr = 0, n_ss = 0, n_ch = 0, max_fr = 0, max_ss = 0, max_ch = 0, max_out = 0;
+    int64_t n10 = 0, n16 = 0, n_fr = 0, n_ss = 0, n_ch = 0, n_cf = 0, max_fr = 0, max_ss = 0, max_ch = 0, max_cf = 0, max_out = 0;
 };
 
 int plan_call(const dfb_metrics *h, int64_t in_numel, const int64_t *offsets, const int64_t *lengths, const int64_t *deg_lengths,
               int64_t B, int bits, MetPlan &p) {
     if (B <= 0 || B > 32767) return fail(DFB_ERR_INVALID, "batch of %lld entries: 1 .. 32767 per call", (long long)B);
-    if (bits <= 0 || (bits & ~(DFB_METRIC_SISDR | DFB_METRIC_STOI | DFB_METRIC_SSNR)))
-        return fail(DFB_ERR_INVALID, "unknown metric bits 0x%x (SI-SDR 1, STOI 2, SSNR 4)", bits);
+    if (bits <= 0 || (bits & ~(DFB_METRIC_SISDR | DFB_METRIC_STOI | DFB_METRIC_SSNR | DFB_METRIC_LLR | DFB_METRIC_WSS)))
+        return fail(DFB_ERR_INVALID, "unknown metric bits 0x%x (SI-SDR 1, STOI 2, SSNR 4, LLR 16, WSS 32)", bits);
     if (!offsets || !lengths || !deg_lengths) return fail(DFB_ERR_INVALID, "null layout");
-    const bool stoi = bits & DFB_METRIC_STOI, ssnr = bits & DFB_METRIC_SSNR;
-    const bool rs10 = stoi && h->dirs[0].taps, rs16 = ssnr && h->dirs[1].taps;
+    const bool stoi = bits & DFB_METRIC_STOI, ssnr = bits & DFB_METRIC_SSNR, comp = bits & (DFB_METRIC_LLR | DFB_METRIC_WSS);
+    const bool rs10 = stoi && h->dirs[0].taps, rs16 = (ssnr || comp) && h->dirs[1].taps;
     p.ents.resize(B);
     for (int64_t b = 0; b < B; b++) {
         const int64_t T = lengths[b];
@@ -432,7 +708,7 @@ int plan_call(const dfb_metrics *h, int64_t in_numel, const int64_t *offsets, co
             p.n_fr += nfr;
             p.max_fr = std::max(p.max_fr, nfr);
         }
-        if (ssnr) {
+        if (ssnr || comp) {
             e.t16 = rs16 ? resampled_len(T, h->dirs[1].og, h->dirs[1].nw) : T;
             e.o16 = rs16 ? 0 : e.in_off;   // (16 kHz rows follow the 10 kHz ones: offset set below)
             if (rs16) {
@@ -441,6 +717,17 @@ int plan_call(const dfb_metrics *h, int64_t in_numel, const int64_t *offsets, co
                 p.n16 += e.t16;
                 p.max_out = std::max(p.max_out, e.t16);
             }
+        }
+        if (comp) {
+            const int64_t nct = e.t16 >= kSsnrWin ? (e.t16 - kSsnrWin) / kSsnrHop : 0;
+            if (nct > (1 << 30)) return fail(DFB_ERR_INVALID, "entry %lld is too long", (long long)b);
+            e.nct = (int)nct;
+            e.kct = (int)std::nearbyint((double)nct * 0.95);   // Python's round(T * 0.95): half to even
+            e.cf = p.n_cf;
+            p.n_cf += nct;
+            p.max_cf = std::max(p.max_cf, nct);
+        }
+        if (ssnr) {
             const int64_t nfs = e.t16 >= kSsnrWin - kSsnrHop ? (e.t16 - kSsnrWin + kSsnrHop) / kSsnrHop : 0;
             e.nfs = (int)nfs;
             e.so = p.n_ss;
@@ -470,6 +757,7 @@ size_t call_bytes(const MetPlan &p, int64_t B, bool host, int64_t in_numel, int 
     s += a256(sizeof(float) * (p.n_fr + 1)) * 2 + a256(sizeof(int) * (p.n_fr + 1));   // energies, segments, kept list
     s += 2 * a256(sizeof(float) * (kStoiBands * p.n_fr + 1));            // band magnitudes
     s += a256(sizeof(double) * (p.n_ss + 1)) + a256(sizeof(double) * (3 * p.n_ch + 1));
+    s += 2 * a256(sizeof(double) * (p.n_cf + 1));                        // LLR / WSS frame values
     if (host) s += 2 * a256(sizeof(float) * in_numel) + a256(sizeof(float) * n_rows * B);
     return s;
 }
@@ -494,6 +782,9 @@ int run_call(dfb_metrics *h, const float *d_clean, const float *d_deg, const Met
     mb.by = a.take<float>(kStoiBands * p.n_fr + 1);
     mb.ss = a.take<double>(p.n_ss + 1);
     mb.ch = a.take<double>(3 * p.n_ch + 1);
+    mb.llr = a.take<double>(p.n_cf + 1);
+    mb.wss = a.take<double>(p.n_cf + 1);
+    mb.fft_tw = h->d_fft_tw;
     mb.n_fr = p.n_fr;
     mb.n_ch = p.n_ch;
     if (host) {
@@ -537,6 +828,14 @@ int run_call(dfb_metrics *h, const float *d_clean, const float *d_deg, const Met
         k_ssnr<<<dim3((unsigned)((p.max_ss + 7) / 8), ub), 256, 0, s>>>(d_ents, mb);
         DFB_LAUNCH_CHECK();
     }
+    if ((bits & DFB_METRIC_LLR) && p.max_cf > 0) {
+        k_llr<<<dim3((unsigned)((p.max_cf + 3) / 4), ub), 128, 0, s>>>(d_ents, mb);
+        DFB_LAUNCH_CHECK();
+    }
+    if ((bits & DFB_METRIC_WSS) && p.max_cf > 0) {
+        k_wss<<<dim3((unsigned)p.max_cf, ub), 256, 0, s>>>(d_ents, mb);
+        DFB_LAUNCH_CHECK();
+    }
     if (bits & DFB_METRIC_SISDR) {
         k_sisdr<<<dim3((unsigned)p.max_ch, ub), 256, 0, s>>>(d_ents, mb);
         DFB_LAUNCH_CHECK();
@@ -545,6 +844,11 @@ int run_call(dfb_metrics *h, const float *d_clean, const float *d_deg, const Met
     DFB_LAUNCH_CHECK();
     h->last_b = (bits & DFB_METRIC_STOI) ? B : 0;
     h->last_st = mb.st;
+    h->last_nct.clear();
+    if (bits & (DFB_METRIC_LLR | DFB_METRIC_WSS))
+        for (const MetEntry &e : p.ents) h->last_nct.push_back(e.nct);
+    h->last_llr = mb.llr;
+    h->last_wss = mb.wss;
     if (host) {
         DFB_CUDA(cudaMemcpyAsync(h_out, d_out, sizeof(float) * n_rows * B, cudaMemcpyDeviceToHost, s));
         DFB_CUDA(cudaStreamSynchronize(s));
@@ -577,7 +881,7 @@ extern "C" int dfb_metrics_create(dfb_metrics **out, int device, int sr, const f
     h->bands = stoi_bands();
     if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaMalloc(&h->d_tw, sizeof(float2) * tw.size()) != cudaSuccess ||
-        cudaMalloc(&h->d_dirs, sizeof(RateDir) * 2) != cudaSuccess ||
+        cudaMalloc(&h->d_dirs, sizeof(RateDir) * 2) != cudaSuccess || cudaMalloc(&h->d_fft_tw, sizeof(double2) * kWssFft) != cudaSuccess ||
         cudaMalloc(&h->d_taps, sizeof(float) * (size_t)(f10 + f16 + 1)) != cudaSuccess)
         return bail(fail(DFB_ERR_OOM, "metrics handle allocation failed"));
     if (f10) {
@@ -594,7 +898,14 @@ extern "C" int dfb_metrics_create(dfb_metrics **out, int device, int sr, const f
     for (int n = 0; n < kStoiFrame; n++) w256[n] = (float)(0.5 - 0.5 * std::cos(2.0 * M_PI * (n + 1) / (kStoiFrame + 1)));
     double wss[kSsnrWin];
     for (int n = 0; n < kSsnrWin; n++) wss[n] = 0.5 * (1.0 - std::cos(2.0 * M_PI * (n + 1) / (kSsnrWin + 1)));
+    std::vector<double2> tw64(kWssFft);
+    for (int m = 0; m < kWssFft; m++) tw64[m] = make_double2(std::cos(2.0 * M_PI * m / kWssFft), -std::sin(2.0 * M_PI * m / kWssFft));
+    static CritFilters crit;
+    if (!crit_filters(crit)) return bail(fail(DFB_ERR_UNSUPPORTED, "critical-band filter table overflow"));
     if (cudaMemcpy(h->d_tw, tw.data(), sizeof(float2) * tw.size(), cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaMemcpy(h->d_fft_tw, tw64.data(), sizeof(double2) * kWssFft, cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaMemcpyToSymbol(c_crit, crit.w, sizeof crit.w) != cudaSuccess || cudaMemcpyToSymbol(c_crit_lo, crit.lo, sizeof crit.lo) != cudaSuccess ||
+        cudaMemcpyToSymbol(c_crit_n, crit.n, sizeof crit.n) != cudaSuccess || cudaMemcpyToSymbol(c_crit_off, crit.off, sizeof crit.off) != cudaSuccess ||
         cudaMemcpy(h->d_dirs, h->dirs, sizeof(RateDir) * 2, cudaMemcpyHostToDevice) != cudaSuccess ||
         cudaMemcpyToSymbol(c_w256, w256, sizeof w256) != cudaSuccess || cudaMemcpyToSymbol(c_wss, wss, sizeof wss) != cudaSuccess)
         return bail(fail(DFB_ERR_CUDA, "metrics table upload failed"));
@@ -611,6 +922,7 @@ extern "C" void dfb_metrics_free(dfb_metrics *h) {
     cudaFree(h->d_taps);
     cudaFree(h->d_dirs);
     cudaFree(h->d_tw);
+    cudaFree(h->d_fft_tw);
     if (h->stream) cudaStreamDestroy(h->stream);
     delete h;
 }
@@ -652,5 +964,21 @@ extern "C" int dfb_debug_metrics_counts(dfb_metrics *h, const float *h_clean, co
         h_counts[3 * b + 1] = st[b].lc;
         h_counts[3 * b + 2] = st[b].nf;
     }
+    return DFB_OK;
+}
+
+extern "C" int dfb_debug_metrics_frames(dfb_metrics *h, const float *h_clean, const float *h_degraded, int64_t in_numel,
+                                        const int64_t *offsets, const int64_t *lengths, int64_t B, int64_t *h_frames,
+                                        double *h_llr, double *h_wss, int64_t capacity) {
+    if (!h || !h_frames || !h_llr || !h_wss) return fail(DFB_ERR_INVALID, "null argument");
+    std::vector<float> rows((size_t)(2 * (B > 0 ? B : 1)));
+    int rc = dfb_metrics_compute_host(h, h_clean, h_degraded, in_numel, offsets, lengths, lengths, B,
+                                      DFB_METRIC_LLR | DFB_METRIC_WSS, rows.data());
+    if (rc) return rc;
+    int64_t n = 0;
+    for (int64_t b = 0; b < B; b++) n += (h_frames[b] = h->last_nct[b]);
+    if (n > capacity) return fail(DFB_ERR_INVALID, "%lld frames, room for %lld", (long long)n, (long long)capacity);
+    DFB_CUDA(cudaMemcpy(h_llr, h->last_llr, sizeof(double) * n, cudaMemcpyDeviceToHost));
+    DFB_CUDA(cudaMemcpy(h_wss, h->last_wss, sizeof(double) * n, cudaMemcpyDeviceToHost));
     return DFB_OK;
 }

@@ -1,6 +1,7 @@
 """Speech-quality scoring on the device, after ``df.evaluation_utils`` (DeepFilterNet/df/evaluation_utils.py).
 
-Three metrics, each equal to the reference function applied to one entry alone (include/dfb200.h, DESIGN.md section 5j):
+Five metrics, each equal to the reference function applied to one entry alone (include/dfb200.h, DESIGN.md sections 5j
+and 5m):
 
 * ``"sisdr"``: ``si_sdr_speechmetrics(clean, degraded)`` at the input rate.
 * ``"stoi"``: ``df.stoi.stoi(clean[None], degraded[None], sr)[0]`` (:func:`deepfilternet_b200.stoi.stoi`), NaN for an
@@ -9,10 +10,15 @@ Three metrics, each equal to the reference function applied to one entry alone (
   signal differently.  How far the two differ is not measured.
 * ``"ssnr"``: ``df.sepm.SNRseg(c16, d16, 16000)`` after ``io.resample(x, sr, 16000)``, the fifth value of the reference's
   ``CompositeMetric``; NaN for an entry with no frame left.
+* ``"llr"`` / ``"wss"``: ``df.sepm.llr(c16, d16, 16000)`` / ``df.sepm.wss(c16, d16, 16000)`` on the same 16 kHz rows;
+  NaN for an entry with fewer than 600 samples at 16 kHz (no frame).
 
 A batch is scored by one library call (``dfb_metrics_compute(_host)``): resampling, silence removal, STFT, band
-envelopes, segment correlations and every per-entry mean run on the GPU.  PESQ (and with it CSIG / CBAK / COVL) and
-DNSMOS are not provided.
+envelopes, segment correlations, LPC models, critical-band spectra and every per-entry mean run on the GPU.
+
+``"composite"`` (``df.sepm.composite``: PESQ, CSIG, CBAK, COVL, SSNR) needs PESQ-WB, an external C package this
+library does not provide: it is available when the caller passes ``pesq=``, a callable scoring one 16 kHz pair, and
+the library computes the rest from the device's LLR, WSS and SSNR.  DNSMOS is not provided.
 
 ``python -m deepfilternet_b200.evaluation_utils DATASET_DIR -m MODEL`` scores a VoiceBank-DEMAND style test set as the
 reference's ``scripts/test_voicebank_demand.py`` does.
@@ -37,7 +43,11 @@ from ._lib import check
 logger = logging.getLogger("deepfilternet_b200")
 
 # metric name -> (bit of dfb_metrics_compute, name in results and CSV files); the output rows follow the bit order
-METRICS = {"sisdr": (1, "SISDR"), "stoi": (2, "STOI"), "ssnr": (4, "SSNR")}
+METRICS = {"sisdr": (1, "SISDR"), "stoi": (2, "STOI"), "ssnr": (4, "SSNR"), "llr": (16, "LLR"), "wss": (32, "WSS")}
+# "composite" with a caller's PESQ: its values, in the reference CompositeMetric's order, and the device rows it needs
+COMPOSITE_NAMES = ("PESQ", "CSIG", "CBAK", "COVL", "SSNR")
+COMPOSITE_BITS = 4 | 16 | 32
+COMPOSITE_MIN_LEN16 = 600   # the reference's wss raises below 600 samples at 16 kHz (no frame)
 UNSUPPORTED = {
     "composite": "needs PESQ (an external C package)",
     "composite-octave": "needs PESQ and Octave",
@@ -67,6 +77,34 @@ def metric_bits(metrics: Sequence[str]) -> int:
     if bits == 0:
         raise ValueError("no metric requested")
     return bits
+
+
+def _split_composite(metrics: Sequence[str], pesq) -> Tuple[List[str], int]:
+    """(lower-case names, bits of the device rows they need): "composite" counts as SSNR + LLR + WSS when ``pesq`` is
+    given, and raises as :func:`metric_bits` does without it."""
+    names = [str(m).lower() for m in ([metrics] if isinstance(metrics, str) else metrics)]
+    if pesq is None or "composite" not in names:
+        return names, metric_bits(names)
+    if not callable(pesq):
+        raise ValueError("pesq must be a callable (ref16, deg16) -> float")
+    rest = [m for m in names if m != "composite"]
+    return names, COMPOSITE_BITS | (metric_bits(rest) if rest else 0)
+
+
+def composite_values(pesq: Callable[[np.ndarray, np.ndarray], float], ref16: np.ndarray, deg16: np.ndarray, llr: float,
+                     wss: float, ssnr: float) -> np.ndarray:
+    """df.sepm.composite of one 16 kHz pair from its LLR, WSS and SSNR: float32 (PESQ, CSIG, CBAK, COVL, SSNR), CSIG / CBAK /
+    COVL being Hu & Loizou's regressions (IEEE TASLP 16(1), 2008) clipped to [1, 5] in fp64.  NaN for fewer than 600
+    samples, where ``pesq`` is not called."""
+    if ref16.size < COMPOSITE_MIN_LEN16:
+        return np.full(5, np.nan, dtype=np.float32)
+    p = float(pesq(ref16, deg16))
+    llr, wss, ssnr = float(llr), float(wss), float(ssnr)
+    csig = 3.093 - 1.029 * llr + 0.603 * p - 0.009 * wss
+    cbak = 1.634 + 0.478 * p - 0.007 * wss + 0.063 * ssnr
+    covl = 1.594 + 0.805 * p - 0.512 * llr - 0.007 * wss
+    clip = lambda v: min(5.0, max(1.0, v))  # noqa: E731
+    return np.asarray([p, clip(csig), clip(cbak), clip(covl), ssnr], dtype=np.float64).astype(np.float32)
 
 
 def bit_names(bits: int) -> List[str]:
@@ -170,17 +208,24 @@ def metrics_handle(sr: int, device: int = 0) -> _Metrics:
 
 def _rows_to_dict(out: Tensor, bits: int, metrics: Sequence[str]) -> Dict[str, Tensor]:
     rows = {k: out[i] for i, k in enumerate(bit_names(bits))}
-    return {str(m).lower(): rows[str(m).lower()] for m in metrics}
+    metrics = [metrics] if isinstance(metrics, str) else metrics
+    return {str(m).lower(): rows[str(m).lower()] for m in metrics if str(m).lower() != "composite"}
 
 
 @torch.no_grad()
 def evaluate_batch(clean: Sequence[Tensor], degraded: Sequence[Tensor], sr: int,
-                   metrics: Sequence[str] = ("sisdr", "stoi", "ssnr"), device: int = 0) -> Dict[str, Tensor]:
+                   metrics: Sequence[str] = ("sisdr", "stoi", "ssnr"), device: int = 0,
+                   pesq: Optional[Callable[[np.ndarray, np.ndarray], float]] = None) -> Dict[str, Tensor]:
     """Scores entries of different lengths in one call: ``clean[i]`` and ``degraded[i]`` are 1-D CPU tensors of one length
     at ``sr`` Hz.  Returns {metric: float32 CPU tensor [B]}, in the order of ``metrics``; entry i equals the reference
     function on entry i alone.  The batch is packed into page-locked buffers and scored by one ``dfb_metrics_compute_host``
-    call, which copies only the entries' samples."""
-    bits = metric_bits(metrics)
+    call, which copies only the entries' samples.
+
+    ``"composite"`` needs ``pesq``, a callable ``(ref16, deg16) -> float`` (PESQ-WB of one entry's 16 kHz float32 pair,
+    ``io.resample``'s output, which is what the device scores); it is then a float32 tensor [B, 5] of (PESQ, CSIG, CBAK,
+    COVL, SSNR) as ``df.sepm.composite``, NaN for entries with fewer than 600 samples at 16 kHz (``pesq`` is not called
+    for them).  Without ``pesq`` it raises ValueError; exceptions of ``pesq`` propagate."""
+    names, bits = _split_composite(metrics, pesq)
     cs, ds = list(clean), list(degraded)
     for i, t in enumerate(cs + ds):
         if not isinstance(t, Tensor) or t.dim() != 1:
@@ -196,7 +241,17 @@ def evaluate_batch(clean: Sequence[Tensor], degraded: Sequence[Tensor], sr: int,
     out = torch.empty((bin(bits).count("1"), lens.size), dtype=torch.float32)
     check(_lib.lib().dfb_metrics_compute_host(h.handle, xc.data_ptr(), xd.data_ptr(), n, off.ctypes.data, lens.ctypes.data,
                                               lens.ctypes.data, lens.size, bits, out.data_ptr()))
-    return _rows_to_dict(out, bits, metrics)
+    res = _rows_to_dict(out, bits, names)
+    if "composite" in names:
+        from .io import resample
+        rows = {k: out[i] for i, k in enumerate(bit_names(bits))}
+        comp = torch.empty((lens.size, 5), dtype=torch.float32)
+        for i, (c, d) in enumerate(zip(cs, ds)):
+            c16, d16 = (resample(t.detach().to("cpu", torch.float32).reshape(1, -1), h.sr, 16000, device=device)[0].numpy()
+                        for t in (c, d))
+            comp[i] = torch.from_numpy(composite_values(pesq, c16, d16, rows["llr"][i], rows["wss"][i], rows["ssnr"][i]))
+        res = {m: (comp if m == "composite" else res[m]) for m in names}
+    return res
 
 
 @torch.no_grad()
@@ -254,7 +309,8 @@ def evaluation_loop(df_state, model, clean_files: List[str], noisy_files: List[s
                     metrics: List[str] = ["stoi", "sisdr", "ssnr"],  # noqa: B006 (the reference's signature)
                     save_audio_callback: Optional[Callable[[str, Tensor], None]] = None, batch_size: int = 32,
                     log_percent: int = 25, csv_path_enh: Optional[str] = None, csv_path_noisy: Optional[str] = None,
-                    noisy_metric: bool = False) -> Dict[str, float]:
+                    noisy_metric: bool = False,
+                    pesq: Optional[Callable[[np.ndarray, np.ndarray], float]] = None) -> Dict[str, float]:
     """evaluation_utils.evaluation_loop: enhance each noisy file and score it against its clean file.
 
     Per file, as the reference: ``enh = enhance(model, df_state, noisy, pad=False)[0]`` and
@@ -262,18 +318,22 @@ def evaluation_loop(df_state, model, clean_files: List[str], noisy_files: List[s
     at the model's rate with sinc_fast resampling.  ``batch_size`` files are enhanced by one :func:`enhance_batch` call and
     scored by one metrics call (noisy entries included).  Returns the reference's means, ``"Noisy    STOI"`` (with
     ``noisy_metric``) and ``"Enhanced STOI"`` for each metric in ``metrics`` order; ``csv_path_enh`` / ``csv_path_noisy``
-    get the reference's per-file CSV layout.  Metrics other than "stoi", "sisdr" and "ssnr" raise ValueError."""
+    get the reference's per-file CSV layout.  "composite" needs ``pesq`` (see :func:`evaluate_batch`) and adds PESQ, CSIG,
+    CBAK, COVL and SSNR, as the reference's CompositeMetric; other metrics than those of :data:`METRICS` raise ValueError."""
     from .enhance import enhance_batch
     from .io import load_audio
 
-    names = [str(m).lower() for m in metrics]
-    metric_bits(names)
+    names, _ = _split_composite(metrics, pesq)
     if len(clean_files) != len(noisy_files):
         raise ValueError(f"{len(clean_files)} clean files, {len(noisy_files)} noisy")
     sr = df_state.sr()
     check_sr(sr)
-    enh_vals: Dict[str, List[Tuple[str, float]]] = {m: [] for m in names}
-    noisy_vals: Dict[str, List[Tuple[str, float]]] = {m: [] for m in names}
+    # metric -> its (label, column of the metric's values) pairs; "composite" has five
+    labels = {m: [(lab, q) for q, lab in enumerate(COMPOSITE_NAMES)] if m == "composite" else [(METRICS[m][1], None)]
+              for m in names}
+    cols = [lab for m in names for lab, _ in labels[m]]
+    enh_vals: Dict[str, List[Tuple[str, float]]] = {c: [] for c in cols}
+    noisy_vals: Dict[str, List[Tuple[str, float]]] = {c: [] for c in cols}
     pairs = list(zip(noisy_files, clean_files))
     batch_size = max(1, int(batch_size))
     batches = [pairs[i:i + batch_size] for i in range(0, len(pairs), batch_size)]
@@ -291,13 +351,15 @@ def evaluation_loop(df_state, model, clean_files: List[str], noisy_files: List[s
         if noisy_metric:
             degraded += [torch.from_numpy(df_state.synthesis(df_state.analysis(n.numpy()))[0]) for n in noisy]
             refs += clean
-        scores = evaluate_batch(refs, degraded, sr, names, device=model.cuda_device.index or 0)
+        scores = evaluate_batch(refs, degraded, sr, names, device=model.cuda_device.index or 0, pesq=pesq)
         for j, (nf, cf) in enumerate(batch):
             fn = os.path.basename(nf)
             for m in names:
-                enh_vals[m].append((fn, float(scores[m][j])))
-                if noisy_metric:
-                    noisy_vals[m].append((fn, float(scores[m][len(batch) + j])))
+                for lab, q in labels[m]:
+                    col = scores[m] if q is None else scores[m][:, q]
+                    enh_vals[lab].append((fn, float(col[j])))
+                    if noisy_metric:
+                        noisy_vals[lab].append((fn, float(col[len(batch) + j])))
             if save_audio_callback is not None:
                 save_audio_callback(cf, enh[j].to(torch.float32).view(1, -1))
         prev, done = done, done + len(batch)
@@ -305,13 +367,12 @@ def evaluation_loop(df_state, model, clean_files: List[str], noisy_files: List[s
             for p in range(int(100 * prev / len(pairs)) + 1, int(100 * done / len(pairs)) + 1):
                 if p % log_percent == 0:
                     logger.info("Progress: %2d%%", p)
-    label = {m: METRICS[m][1] for m in names}
 
     def flat(vals) -> Dict[str, Dict[str, float]]:
         out: Dict[str, Dict[str, float]] = defaultdict(dict)
-        for m in names:
-            for fn, v in vals[m]:
-                out[fn][label[m]] = v
+        for c in vals:
+            for fn, v in vals[c]:
+                out[fn][c] = v
         return out
 
     if csv_path_enh is not None:
@@ -319,10 +380,10 @@ def evaluation_loop(df_state, model, clean_files: List[str], noisy_files: List[s
     if csv_path_noisy is not None and noisy_metric:
         write_csv(csv_path_noisy, flat(noisy_vals))
     out_dict: Dict[str, float] = {}
-    for m in names:
+    for c in enh_vals:
         if noisy_metric:
-            out_dict[f"Noisy    {label[m]}"] = float(np.mean([v for _, v in noisy_vals[m]]))
-        out_dict[f"Enhanced {label[m]}"] = float(np.mean([v for _, v in enh_vals[m]]))
+            out_dict[f"Noisy    {c}"] = float(np.mean([v for _, v in noisy_vals[c]]))
+        out_dict[f"Enhanced {c}"] = float(np.mean([v for _, v in enh_vals[c]]))
     return out_dict
 
 
@@ -339,8 +400,17 @@ def cli_parser():
     parser.add_argument("--compute-noisy-metric", action="store_true")
     parser.add_argument("--batch-size", type=int, default=32, help="Files enhanced and scored per call.")
     parser.add_argument("--metrics", type=str, nargs="+", default=["stoi", "sisdr", "ssnr"],
-                        help=f"Metrics to compute, of {sorted(METRICS)}.")
+                        help=f"Metrics to compute, of {sorted(METRICS)}, and 'composite' when the pesq package is installed.")
     return parser
+
+
+def pesq_wb() -> Optional[Callable[[np.ndarray, np.ndarray], float]]:
+    """``pesq.pesq(16000, ref, deg, "wb")`` of the ``pesq`` package when it imports, else None."""
+    try:
+        import pesq as pesq_pkg
+    except ImportError:
+        return None
+    return lambda ref16, deg16: pesq_pkg.pesq(16000, ref16, deg16, "wb")
 
 
 def main(args) -> Dict[str, float]:
@@ -351,7 +421,8 @@ def main(args) -> Dict[str, float]:
     from .enhance import init_df
     from .io import save_audio
 
-    metric_bits(args.metrics)
+    pesq_fn = pesq_wb() if "composite" in [str(m).lower() for m in args.metrics] else None
+    _split_composite(args.metrics, pesq_fn)
     model, df_state, suffix, _ = init_df(args.model_base_dir, post_filter=args.pf, log_level=args.log_level,
                                          config_allow_defaults=True, epoch=args.epoch)
     if not os.path.isdir(args.dataset_dir):
@@ -372,7 +443,7 @@ def main(args) -> Dict[str, float]:
     metrics = evaluation_loop(df_state, model, clean_files, noisy_files, metrics=args.metrics,
                               save_audio_callback=save_audio_callback if args.output_dir is not None else None,
                               batch_size=args.batch_size, csv_path_enh=args.csv_path_enh, csv_path_noisy=args.csv_path_noisy,
-                              noisy_metric=args.compute_noisy_metric)
+                              noisy_metric=args.compute_noisy_metric, pesq=pesq_fn)
     for k, v in metrics.items():
         logger.info("%s: %s", k, v)
     print("".join(f"{m}," for k, m in metrics.items() if "SSNR" not in k)[:-1])

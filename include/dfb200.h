@@ -681,9 +681,15 @@ int64_t dfb_model_workspace_bytes(const dfb_model *m);
  *                     (fp64 sums, float32 eps);
  *   DFB_METRIC_STOI   df/stoi.py stoi(clean[None], degraded[None], sr)[0]: io.resample to 10 kHz (sinc_fast), silent
  *                     frames removed, 15 third-octave bands, 30-frame segments; NaN when fewer than 512 samples remain;
- *   DFB_METRIC_SSNR   df/sepm.py SNRseg(c16, d16, 16000) after io.resample to 16 kHz (sinc_fast); NaN when no frame is left.
+ *   DFB_METRIC_SSNR   df/sepm.py SNRseg(c16, d16, 16000) after io.resample to 16 kHz (sinc_fast); NaN when no frame is left;
+ *   DFB_METRIC_LLR    df/sepm.py llr(c16, d16, 16000): the log-likelihood ratio of order-16 LPC models of the T =
+ *                     (L16 - 480) / 120 frames of 480 samples at hop 120, averaged over the round(0.95 T) smallest;
+ *   DFB_METRIC_WSS    df/sepm.py wss(c16, d16, 16000): Klatt's weighted spectral slope over 25 critical bands on the same
+ *                     frames, averaged the same way.  LLR and WSS are NaN when T = 0.
+ * With PESQ-WB (not provided) they make df/sepm.py's composite measure: CSIG, CBAK and COVL are Hu & Loizou's (IEEE TASLP
+ * 16(1), 2008) linear regressions on PESQ, LLR, WSS and SSNR.  Bit 8 is not a metric.
  * This STOI is df/stoi.py's, not pystoi's, which removes silence and frames differently. */
-enum { DFB_METRIC_SISDR = 1, DFB_METRIC_STOI = 2, DFB_METRIC_SSNR = 4 };
+enum { DFB_METRIC_SISDR = 1, DFB_METRIC_STOI = 2, DFB_METRIC_SSNR = 4, DFB_METRIC_LLR = 16, DFB_METRIC_WSS = 32 };
 typedef struct dfb_metrics dfb_metrics;
 /* A metrics handle on `device` for inputs at `sr` Hz: taps10 / taps16 [nw][2 width + og] (HOST arrays) are
  * io.resample_kernel(sr, 10000) / (sr, 16000) with the sinc_fast parameters, og / nw the gcd-reduced rates (DFB_ERR_INVALID
@@ -694,7 +700,7 @@ int dfb_metrics_create(dfb_metrics **out, int device, int sr, const float *taps1
 void dfb_metrics_free(dfb_metrics *h);
 /* One call scores B <= 32767 entries: entry b is clean_lengths[b] samples of clean at d_clean + offsets[b] and as many of
  * degraded at d_degraded + offsets[b] (offsets / lengths HOST arrays, in_numel bounding both buffers).  d_out [n][B] fp32
- * gets one row per bit of `metrics`, in the order SI-SDR, STOI, SSNR.  DFB_ERR_INVALID for a length <= 0, different clean
+ * gets one row per bit of `metrics`, in the order SI-SDR, STOI, SSNR, LLR, WSS.  DFB_ERR_INVALID for a length <= 0, different clean
  * and degraded lengths, an entry outside in_numel, no metric or an unknown metric bit.  Asynchronous on `stream`; the
  * handle's workspace serves one call at a time. */
 int dfb_metrics_compute(dfb_metrics *h, const float *d_clean, const float *d_degraded, int64_t in_numel, const int64_t *offsets,
@@ -709,6 +715,12 @@ int64_t dfb_metrics_workspace_bytes(const dfb_metrics *h);
  * removal and its STFT frames (0 when that length is below 512). */
 int dfb_debug_metrics_counts(dfb_metrics *h, const float *h_clean, const float *h_degraded, int64_t in_numel,
                              const int64_t *offsets, const int64_t *lengths, int64_t B, int64_t *h_counts);
+/* Debug aid: the LLR and WSS of a dfb_metrics_host call, then h_frames [B] = each entry's frame count T and h_llr / h_wss
+ * = every entry's per-frame distortions before the 0.95 trim (fp64), entries back to back.  DFB_ERR_INVALID when the
+ * frames of all entries exceed `capacity` doubles. */
+int dfb_debug_metrics_frames(dfb_metrics *h, const float *h_clean, const float *h_degraded, int64_t in_numel,
+                             const int64_t *offsets, const int64_t *lengths, int64_t B, int64_t *h_frames, double *h_llr,
+                             double *h_wss, int64_t capacity);
 
 #ifdef __cplusplus
 }
