@@ -149,6 +149,7 @@ SIGNATURES = {
     "dfb_metrics_workspace_bytes": (_I64, [_VP]),
     "dfb_debug_metrics_counts": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _VP]),
     "dfb_debug_metrics_frames": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _VP, _I64]),
+    "dfb_debug_metrics_pystoi": (_I, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64]),
 }
 
 

@@ -1,7 +1,8 @@
 // dfb_metrics.cu -- batched speech-quality metrics of a ragged batch (dfb_metrics* in include/dfb200.h; DESIGN.md section 5j):
 // SI-SDR (DeepFilterNet/df/evaluation_utils.py si_sdr_speechmetrics), STOI (df/stoi.py stoi, after io.resample to 10 kHz)
 // segmental SNR (df/sepm.py SNRseg, after io.resample to 16 kHz), and the two spectral distances of df/sepm.py's composite
-// measure on the same 16 kHz rows: LLR (sepm.llr) and WSS (sepm.wss).
+// measure on the same 16 kHz rows: LLR (sepm.llr) and WSS (sepm.wss); and pystoi's STOI and extended STOI on the 10 kHz rows
+// (pystoi.stoi(x, y, 10000, extended), which df/evaluation_utils.py stoi reports; section 5n).
 //
 // One call is a fixed sequence of launches, with no host round trip between them:
 //   k_resample_rows (dfb_dsp.cu)  clean and degraded rows -> 10 kHz / 16 kHz, one launch per signal
@@ -16,15 +17,22 @@
 //                                 models of both signals (fp64)
 //   k_wss                         one CTA per 480-sample frame at 16 kHz: a 1024-point fp64 FFT of both signals, the 25
 //                                 critical-band energies and Klatt's weighted spectral slope distance (fp64)
+//   k_pystoi_energy               one warp per pystoi frame (256 samples at hop 128, unpadded): its energy in dB (fp64)
+//   k_stoi_mask<true>             one CTA per entry: the same mask and prefix count on those energies, pystoi's counts
+//   k_pystoi_stft                 one CTA per STFT frame: its samples from at most two kept frames, one fp64 512-point FFT
+//                                 of both signals, the 15 band magnitudes of each (fp64)
+//   k_pystoi_seg                  one warp per 30-frame segment: its STOI sum and its ESTOI sum (fp64)
 //   k_sisdr                       one CTA per 4096-sample chunk: fp64 sums r.r, r.e, e.e
 //   k_metrics_final               one CTA per entry: the per-entry means / SI-SDR from the frame, segment and chunk values,
-//                                 and LLR / WSS as the mean of the round(0.95 T) smallest frame values (a radix select)
+//                                 LLR / WSS as the mean of the round(0.95 T) smallest frame values (a radix select), and
+//                                 pystoi's STOI / ESTOI as segment means
 // Every per-entry sum runs in an order fixed relative to the entry's start (per-thread strided sums, then a fixed shuffle
 // and shared-memory tree), with no atomics, so an entry's results are the same bits wherever and with whatever it is batched.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <numeric>
+#include <type_traits>
 #include <vector>
 
 #include "dfb_common.cuh"
@@ -45,6 +53,7 @@ constexpr double kEps64 = 2.220446049250313e-16;         // np.finfo(np.float64)
 constexpr double kEps32 = 1.1920928955078125e-07;        // np.finfo(np.float32).eps (si_sdr_speechmetrics on float32)
 
 __constant__ float c_w256[kStoiFrame];   // torch.hann_window(258, periodic=False)[1:-1]
+__constant__ double c_w256d[kStoiFrame]; // np.hanning(258)[1:-1] (pystoi), fp64
 __constant__ double c_wss[kSsnrWin];     // SNRseg's hannWin: 0.5 (1 - cos(2 pi n / 481)), n = 1 .. 480
 __constant__ double c_crit[kMaxCritTaps]; // critical-band filter weights of band i at bins [crit_lo[i], crit_lo[i] + crit_n[i])
 __constant__ int c_crit_lo[kWssBands], c_crit_n[kWssBands], c_crit_off[kWssBands];
@@ -60,8 +69,11 @@ struct MetEntry {
     int64_t cf;             // first LLR / WSS frame value
     int nfr, pad_front, pad_end, nfs, nch;
     int nct, kct;           // LLR / WSS frames T = (t16 - 480) / 120 (0 when t16 < 480) and k = round(0.95 T)
+    int pnf;                // pystoi frames F = ceil((t10 - 256) / 128) (0 when t10 <= 256)
+    int64_t po;             // first pystoi frame: energies pen[po ..], kept list pkidx[po ..], segments at po, bands at 15 po
 };
-// What the device finds out about an entry's STOI (dfb_debug_metrics_counts reads it back).
+// What the device finds out about an entry's STOI (dfb_debug_metrics_counts reads it back) or, for pystoi, its kept
+// frames K, silence-free length lc and STFT frames nf = K - 1 (dfb_debug_metrics_pystoi).
 struct MetState { int nk, s0, lc, nf; };
 struct StoiBands { int lo[kStoiBands], hi[kStoiBands]; float inv_wsum; };
 
@@ -75,6 +87,10 @@ struct MetBufs {
     const double2 *fft_tw;   // e^(-2 pi i m / 1024), m = 0 .. 1023
     MetState *st;
     int64_t n_fr, n_ch;
+    double *pen, *pbx, *pby, *pseg;   // pystoi: frame energies, band magnitudes [15][F], segment sums [2][n_pf] at po
+    int *pkidx;
+    MetState *pst;
+    int64_t n_pf;
 };
 
 // ---- deterministic reductions ----
@@ -122,25 +138,35 @@ __global__ void __launch_bounds__(256) k_stoi_energy(const MetEntry *__restrict_
 // grid B, 1024 threads: frame i is kept when (max_j en_j - 40) - en_i < 0 (df/stoi.py remove_silent_frames, in float32);
 // kidx[fo + j] is the j-th kept frame.  The overlap-added kept frames have (nk - 1) 128 + 256 samples; the first pad_front
 // are dropped when frame 0 is kept, the last pad_end when the last frame is kept.  STOI needs at least 512 samples.
+// PY: pystoi's remove_silent_frames on the fp64 energies pen of its F unpadded frames, into pkidx / pst: nothing is
+// trimmed, and the nk - 1 STFT frames of the (nk - 1) 128 + 256 samples are all used (an entry without a frame has none).
+template <bool PY>
 __global__ void __launch_bounds__(1024) k_stoi_mask(const MetEntry *__restrict__ ents, MetBufs b) {
-    __shared__ float s_red[32];
+    using T = typename std::conditional<PY, double, float>::type;
+    __shared__ T s_red[32];
     __shared__ int s_cnt[33];
     const MetEntry e = ents[blockIdx.x];
-    const float *en = b.en + e.fo;
-    float mx = -INFINITY;
-    for (int i = threadIdx.x; i < e.nfr; i += blockDim.x) mx = fmaxf(mx, en[i]);
+    const int nfr = PY ? e.pnf : e.nfr;
+    if (PY && nfr == 0) {
+        if (threadIdx.x == 0) b.pst[blockIdx.x] = MetState{0, 0, 0, 0};
+        return;
+    }
+    const T *en = PY ? (const T *)(b.pen + e.po) : (const T *)(b.en + e.fo);
+    int *kidx = PY ? b.pkidx + e.po : b.kidx + e.fo;
+    T mx = -INFINITY;
+    for (int i = threadIdx.x; i < nfr; i += blockDim.x) mx = max(mx, en[i]);
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    for (int o = 16; o > 0; o >>= 1) mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
     if (lane == 0) s_red[w] = mx;
     __syncthreads();
     mx = s_red[0];
-    for (int k = 1; k < nw; k++) mx = fmaxf(mx, s_red[k]);
-    const float thr = mx - 40.f;
+    for (int k = 1; k < nw; k++) mx = max(mx, s_red[k]);
+    const T thr = mx - T(40);
     int base = 0;
-    for (int c0 = 0; c0 < e.nfr; c0 += blockDim.x) {
+    for (int c0 = 0; c0 < nfr; c0 += blockDim.x) {
         const int i = c0 + threadIdx.x;
-        const bool keep = i < e.nfr && (thr - en[i]) < 0.f;
+        const bool keep = i < nfr && (thr - en[i]) < T(0);
         const unsigned bal = __ballot_sync(0xffffffffu, keep);
         __syncthreads();   // s_cnt of the previous chunk is consumed
         if (lane == 0) s_cnt[w] = __popc(bal);
@@ -151,10 +177,12 @@ __global__ void __launch_bounds__(1024) k_stoi_mask(const MetEntry *__restrict__
             s_cnt[32] = a;
         }
         __syncthreads();
-        if (keep) b.kidx[e.fo + base + s_cnt[w] + __popc(bal & ((1u << lane) - 1u))] = i;
+        if (keep) kidx[base + s_cnt[w] + __popc(bal & ((1u << lane) - 1u))] = i;
         base += s_cnt[32];
     }
-    if (threadIdx.x == 0) {
+    if (PY) {
+        if (threadIdx.x == 0) b.pst[blockIdx.x] = MetState{base, 0, (base - 1) * kStoiHop + kStoiFrame, base - 1};
+    } else if (threadIdx.x == 0) {
         const int nk = base;
         const bool first = (thr - en[0]) < 0.f, last = (thr - en[e.nfr - 1]) < 0.f;
         MetState s;
@@ -262,6 +290,174 @@ __global__ void __launch_bounds__(256) k_stoi_seg(const MetEntry *__restrict__ e
     if (lane == 0) b.seg[e.fo + m] = corr;
 }
 
+__device__ __forceinline__ double2 cmul(double2 a, double2 b) { return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
+
+// ---- pystoi (0.4.1) on the 10 kHz rows, fp64 throughout as numpy computes it: frame i is samples [128 i, 128 i + 256)
+// of the unpadded row times np.hanning(258)[1:-1], i < F = ceil((t10 - 256) / 128) ----
+
+// grid (ceil(max F / 8), B), 256 threads: warp w of CTA x is frame i = 8 x + w of entry blockIdx.y:
+// pen[po + i] = 20 log10(|frame| + eps).
+__global__ void __launch_bounds__(256) k_pystoi_energy(const MetEntry *__restrict__ ents, MetBufs b) {
+    const MetEntry e = ents[blockIdx.y];
+    const int i = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (i >= e.pnf) return;
+    const float *x = b.x10 + e.o10 + (int64_t)i * kStoiHop;
+    double s = 0.0;
+#pragma unroll
+    for (int k = 0; k < kStoiFrame / 32; k++) {
+        const int n = lane + 32 * k;
+        const double v = c_w256d[n] * (double)__ldg(x + n);
+        s = fma(v, v, s);
+    }
+    s = warp_sum(s);
+    if (lane == 0) b.pen[e.po + i] = 20.0 * log10(sqrt(s) + kEps64);
+}
+
+// In-place 512-point complex FFT of z (shared) by the CTA's 128 threads: four Stockham radix-4 stages, then one radix-2
+// stage; tw[m] = e^(-2 pi i m / 1024) (the WSS table, every second entry).
+__device__ __forceinline__ void fft512(double2 *z, const double2 *__restrict__ tw) {
+    constexpr int N = kStoiFft, TS = kWssFft / kStoiFft;
+    const int j = threadIdx.x;
+#pragma unroll 1
+    for (int ns = 1; ns * 4 <= N; ns *= 4) {
+        const int jm = j & (ns - 1), step = N / (4 * ns);
+        double2 v[4];
+#pragma unroll
+        for (int r = 0; r < 4; r++) {
+            v[r] = z[j + r * (N / 4)];
+            if (r) v[r] = cmul(v[r], __ldg(tw + TS * r * jm * step));
+        }
+        const double2 a0 = make_double2(v[0].x + v[2].x, v[0].y + v[2].y), a1 = make_double2(v[0].x - v[2].x, v[0].y - v[2].y);
+        const double2 a2 = make_double2(v[1].x + v[3].x, v[1].y + v[3].y), a3 = make_double2(v[1].x - v[3].x, v[1].y - v[3].y);
+        const int d = (j - jm) * 4 + jm;
+        __syncthreads();
+        z[d] = make_double2(a0.x + a2.x, a0.y + a2.y);
+        z[d + ns] = make_double2(a1.x + a3.y, a1.y - a3.x);          // a1 - i a3
+        z[d + 2 * ns] = make_double2(a0.x - a2.x, a0.y - a2.y);
+        z[d + 3 * ns] = make_double2(a1.x - a3.y, a1.y + a3.x);      // a1 + i a3
+        __syncthreads();
+    }
+    // last stage, ns = 256: z[k] = v0 + w^k v1, z[k + 256] = v0 - w^k v1
+    double2 v0[2], v1[2];
+#pragma unroll
+    for (int r = 0; r < 2; r++) {
+        const int k = j + r * (N / 4);
+        v0[r] = z[k];
+        v1[r] = cmul(z[k + N / 2], __ldg(tw + TS * k));
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < 2; r++) {
+        const int k = j + r * (N / 4);
+        z[k] = make_double2(v0[r].x + v1[r].x, v0[r].y + v1[r].y);
+        z[k + N / 2] = make_double2(v0[r].x - v1[r].x, v0[r].y - v1[r].y);
+    }
+    __syncthreads();
+}
+
+// grid (max F, B), 128 threads: STFT frame f = blockIdx.x < nf of entry blockIdx.y.  Sample s = 128 f + n of the
+// silence-free signal is the overlap-add (no division) of the windowed kept frames j1 - 1 and j1 = s / 128 that cover
+// it; the frame is that times the window again, both signals as one complex 512-point FFT (clean real, degraded
+// imaginary), and pbx / pby [15 po + band F + f] = sqrt(sum over the band's bins of |X_k|^2).
+__global__ void __launch_bounds__(128) k_pystoi_stft(const MetEntry *__restrict__ ents, MetBufs b, StoiBands bands) {
+    __shared__ double2 z[kStoiFft];
+    const MetEntry e = ents[blockIdx.y];
+    const int f = blockIdx.x, nk = b.pst[blockIdx.y].nk;
+    if (f >= nk - 1) return;
+    const int *kidx = b.pkidx + e.po;
+    const float *x = b.x10 + e.o10, *y = b.y10 + e.o10;
+    for (int n = threadIdx.x; n < kStoiFft; n += blockDim.x) {
+        double2 v = make_double2(0.0, 0.0);
+        if (n < kStoiFrame) {
+            const int j1 = f + (n >> 7), q = n & 127;
+            const int64_t pa = (int64_t)__ldg(kidx + j1) * kStoiHop + q;   // j1 <= nk - 1: kept frame j1, first half
+            double xs = c_w256d[q] * (double)__ldg(x + pa), ys = c_w256d[q] * (double)__ldg(y + pa);
+            if (j1 >= 1) {   // kept frame j1 - 1, second half
+                const int64_t pb = (int64_t)__ldg(kidx + j1 - 1) * kStoiHop + q + kStoiHop;
+                xs += c_w256d[q + kStoiHop] * (double)__ldg(x + pb);
+                ys += c_w256d[q + kStoiHop] * (double)__ldg(y + pb);
+            }
+            v.x = c_w256d[n] * xs;
+            v.y = c_w256d[n] * ys;
+        }
+        z[n] = v;
+    }
+    __syncthreads();
+    fft512(z, b.fft_tw);
+    if (threadIdx.x >= 2 * kStoiBands) return;
+    const int band = threadIdx.x % kStoiBands, sig = threadIdx.x / kStoiBands;
+    double acc = 0.0;
+    for (int k = bands.lo[band]; k < bands.hi[band]; k++) {
+        const double2 zk = z[k], zn = z[(kStoiFft - k) & (kStoiFft - 1)];
+        // X_k = (Z_k + conj Z_-k) / 2, Y_k = (Z_k - conj Z_-k) / 2i
+        const double re = sig ? 0.5 * (zk.y + zn.y) : 0.5 * (zk.x + zn.x);
+        const double im = sig ? 0.5 * (zn.x - zk.x) : 0.5 * (zk.y - zn.y);
+        acc += re * re + im * im;
+    }
+    (sig ? b.pby : b.pbx)[kStoiBands * e.po + (int64_t)band * e.pnf + f] = sqrt(acc);
+}
+
+// grid (ceil(max F / 8), B), 256 threads: warp w of CTA x is segment m = 8 x + w < J = nf - 29 of entry blockIdx.y,
+// frames [m, m + 30), lane l < 30 holding frame m + l of all 15 bands of both signals.
+// pseg[po + m] = STOI's sum over the bands of the correlation of the scaled, clipped, centred and normalised rows;
+// pseg[n_pf + po + m] = ESTOI's sum of x_n y_n / 30 over the segment, the rows then the columns of both 15 x 30 matrices
+// centred and normalised (a centred row or column of norm 0 normalises to 0).
+__global__ void __launch_bounds__(256) k_pystoi_seg(const MetEntry *__restrict__ ents, MetBufs b) {
+    const MetEntry e = ents[blockIdx.y];
+    const int J = b.pst[blockIdx.y].nf - kStoiSeg + 1;
+    const int m = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (m >= J) return;
+    const double c1 = 1.0 + 5.623413251903491;   // 1 + 10^(15 / 20)
+    const bool in = lane < kStoiSeg;
+    const double inv_n = 1.0 / kStoiSeg;
+    double xr[kStoiBands], yr[kStoiBands];
+    double corr = 0.0;
+#pragma unroll
+    for (int band = 0; band < kStoiBands; band++) {
+        const int64_t o = kStoiBands * e.po + (int64_t)band * e.pnf + m + lane;
+        const double xv = in ? b.pbx[o] : 0.0, yv0 = in ? b.pby[o] : 0.0;
+        // STOI
+        const double nrm = sqrt(warp_sum(xv * xv)) / (sqrt(warp_sum(yv0 * yv0)) + kEps64);
+        const double yv = in ? fmin(yv0 * nrm, xv * c1) : 0.0;
+        const double xm = warp_sum(xv) / kStoiSeg, ym = warp_sum(yv) / kStoiSeg;
+        const double xd = in ? xv - xm : 0.0, yd = in ? yv - ym : 0.0;
+        const double xn = xd / (sqrt(warp_sum(xd * xd)) + kEps64), yn = yd / (sqrt(warp_sum(yd * yd)) + kEps64);
+        corr += warp_sum(xn * yn);
+        // ESTOI: the band's row centred and normalised
+        const double ym0 = warp_sum(yv0) / kStoiSeg;   // every lane shuffles: outside the conditionals
+        const double xc = in ? xv - xm : 0.0, yc = in ? yv0 - ym0 : 0.0;
+        const double nx = sqrt(warp_sum(xc * xc)), ny = sqrt(warp_sum(yc * yc));
+        xr[band] = nx > 0.0 ? xc / nx : 0.0;
+        yr[band] = ny > 0.0 ? yc / ny : 0.0;
+    }
+    // ESTOI: this lane's column centred and normalised
+    double sx = 0.0, sy = 0.0;
+#pragma unroll
+    for (int band = 0; band < kStoiBands; band++) { sx += xr[band]; sy += yr[band]; }
+    sx /= kStoiBands;
+    sy /= kStoiBands;
+    double qx = 0.0, qy = 0.0;
+#pragma unroll
+    for (int band = 0; band < kStoiBands; band++) {
+        xr[band] -= sx; yr[band] -= sy;
+        qx = fma(xr[band], xr[band], qx);
+        qy = fma(yr[band], yr[band], qy);
+    }
+    qx = sqrt(qx);
+    qy = sqrt(qy);
+    double es = 0.0;
+#pragma unroll
+    for (int band = 0; band < kStoiBands; band++) {
+        const double xn = qx > 0.0 ? xr[band] / qx : 0.0, yn = qy > 0.0 ? yr[band] / qy : 0.0;
+        es += xn * yn * inv_n;
+    }
+    es = warp_sum(in ? es : 0.0);
+    if (lane == 0) {
+        b.pseg[e.po + m] = corr;
+        b.pseg[b.n_pf + e.po + m] = es;
+    }
+}
+
 // grid (ceil(max nfs / 8), B), 256 threads: warp w of CTA x is SSNR frame i = 8 x + w (samples [120 i, 120 i + 480) at 16 kHz)
 // of entry blockIdx.y; the last frame is not computed (SNRseg drops it).  fp64, as SNRseg computes.
 __global__ void __launch_bounds__(256) k_ssnr(const MetEntry *__restrict__ ents, MetBufs b) {
@@ -362,8 +558,6 @@ __global__ void __launch_bounds__(128) k_llr(const MetEntry *__restrict__ ents, 
         b.llr[e.cf + i] = log(frac);
     }
 }
-
-__device__ __forceinline__ double2 cmul(double2 a, double2 b) { return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 
 // In-place 1024-point complex FFT of z (shared) by the CTA's 256 threads: five Stockham radix-4 stages, one butterfly per
 // thread and stage; tw[m] = e^(-2 pi i m / 1024).
@@ -518,7 +712,7 @@ __global__ void __launch_bounds__(256) k_sisdr(const MetEntry *__restrict__ ents
     }
 }
 
-// grid B, 256 threads: out[row][b] for the metrics of `bits`, rows in the order SI-SDR, STOI, SSNR, LLR, WSS.
+// grid B, 256 threads: out[row][b] for the metrics of `bits`, rows in the order SI-SDR, STOI, SSNR, LLR, WSS, PYSTOI, ESTOI.
 __global__ void __launch_bounds__(256) k_metrics_final(const MetEntry *__restrict__ ents, MetBufs b, int bits, float *out, int64_t B) {
     __shared__ double sm[32];
     const MetEntry e = ents[blockIdx.x];
@@ -560,6 +754,19 @@ __global__ void __launch_bounds__(256) k_metrics_final(const MetEntry *__restric
         if (!(bits & (m ? DFB_METRIC_WSS : DFB_METRIC_LLR))) continue;
         const double v = e.nct > 0 ? trimmed_mean((m ? b.wss : b.llr) + e.cf, e.nct, e.kct, sm) : 0.0;
         if (threadIdx.x == 0) out[row * B + blockIdx.x] = e.nct > 0 ? (float)v : __int_as_float(0x7fc00000);
+        row++;
+    }
+    // pystoi: NaN without a frame (pystoi raises), 1e-5 with fewer than 30 STFT frames (pystoi warns and returns it)
+    for (int m = 0; m < 2; m++) {
+        if (!(bits & (m ? DFB_METRIC_ESTOI : DFB_METRIC_PYSTOI))) continue;
+        const int nf = e.pnf > 0 ? b.pst[blockIdx.x].nf : 0, J = nf - kStoiSeg + 1;
+        double s = 0.0;
+        for (int k = threadIdx.x; k < J; k += blockDim.x) s += b.pseg[m * b.n_pf + e.po + k];
+        s = block_sum(s, sm);
+        if (threadIdx.x == 0)
+            out[row * B + blockIdx.x] = e.pnf == 0 ? __int_as_float(0x7fc00000)
+                                        : J <= 0   ? 1e-5f
+                                                   : (float)(m ? s / J : s / ((double)J * kStoiBands));
         row++;
     }
 }
@@ -645,6 +852,9 @@ struct dfb_metrics {
     double2 *d_fft_tw = nullptr;  // twiddles of WSS's 1024-point fp64 FFT
     std::vector<int64_t> last_nct;             // LLR / WSS frames of each entry of the last call (dfb_debug_metrics_frames)
     double *last_llr = nullptr, *last_wss = nullptr;   // their per-frame values, inside the arena
+    std::vector<int64_t> last_pnf, last_po;    // pystoi frames F and first frame of each entry of the last call
+    MetState *last_pst = nullptr;              // their pystoi states, inside the arena (dfb_debug_metrics_pystoi)
+    double *last_pbx = nullptr, *last_pby = nullptr;   // their band magnitudes, inside the arena
 };
 
 namespace {
@@ -667,16 +877,20 @@ struct MetPlan {
     std::vector<MetEntry> ents;
     std::vector<RateRow> rows;
     int64_t n10 = 0, n16 = 0, n_fr = 0, n_ss = 0, n_ch = 0, n_cf = 0, max_fr = 0, max_ss = 0, max_ch = 0, max_cf = 0, max_out = 0;
+    int64_t n_pf = 0, max_pf = 0;   // pystoi frames
 };
 
 int plan_call(const dfb_metrics *h, int64_t in_numel, const int64_t *offsets, const int64_t *lengths, const int64_t *deg_lengths,
               int64_t B, int bits, MetPlan &p) {
     if (B <= 0 || B > 32767) return fail(DFB_ERR_INVALID, "batch of %lld entries: 1 .. 32767 per call", (long long)B);
-    if (bits <= 0 || (bits & ~(DFB_METRIC_SISDR | DFB_METRIC_STOI | DFB_METRIC_SSNR | DFB_METRIC_LLR | DFB_METRIC_WSS)))
-        return fail(DFB_ERR_INVALID, "unknown metric bits 0x%x (SI-SDR 1, STOI 2, SSNR 4, LLR 16, WSS 32)", bits);
+    if (bits <= 0 || (bits & ~(DFB_METRIC_SISDR | DFB_METRIC_STOI | DFB_METRIC_SSNR | DFB_METRIC_LLR | DFB_METRIC_WSS |
+                               DFB_METRIC_PYSTOI | DFB_METRIC_ESTOI)))
+        return fail(DFB_ERR_INVALID, "unknown metric bits 0x%x (SI-SDR 1, STOI 2, SSNR 4, LLR 16, WSS 32, PYSTOI 128, ESTOI 256)",
+                    bits);
     if (!offsets || !lengths || !deg_lengths) return fail(DFB_ERR_INVALID, "null layout");
     const bool stoi = bits & DFB_METRIC_STOI, ssnr = bits & DFB_METRIC_SSNR, comp = bits & (DFB_METRIC_LLR | DFB_METRIC_WSS);
-    const bool rs10 = stoi && h->dirs[0].taps, rs16 = (ssnr || comp) && h->dirs[1].taps;
+    const bool py = bits & (DFB_METRIC_PYSTOI | DFB_METRIC_ESTOI);
+    const bool rs10 = (stoi || py) && h->dirs[0].taps, rs16 = (ssnr || comp) && h->dirs[1].taps;
     p.ents.resize(B);
     for (int64_t b = 0; b < B; b++) {
         const int64_t T = lengths[b];
@@ -690,7 +904,7 @@ int plan_call(const dfb_metrics *h, int64_t in_numel, const int64_t *offsets, co
         std::memset(&e, 0, sizeof e);
         e.in_off = offsets[b];
         e.len = T;
-        if (stoi) {
+        if (stoi || py) {
             e.t10 = rs10 ? resampled_len(T, h->dirs[0].og, h->dirs[0].nw) : T;
             e.o10 = rs10 ? p.n10 : e.in_off;
             if (rs10) {
@@ -698,6 +912,16 @@ int plan_call(const dfb_metrics *h, int64_t in_numel, const int64_t *offsets, co
                 p.n10 += e.t10;
                 p.max_out = std::max(p.max_out, e.t10);
             }
+        }
+        if (py) {
+            const int64_t pnf = e.t10 > kStoiFrame ? (e.t10 - kStoiFrame + kStoiHop - 1) / kStoiHop : 0;
+            if (pnf > (1 << 30)) return fail(DFB_ERR_INVALID, "entry %lld is too long", (long long)b);
+            e.pnf = (int)pnf;
+            e.po = p.n_pf;
+            p.n_pf += pnf;
+            p.max_pf = std::max(p.max_pf, pnf);
+        }
+        if (stoi) {
             const int64_t pad = kStoiFrame - e.t10 % kStoiFrame;
             e.pad_front = (int)(pad / 2);
             e.pad_end = (int)(pad - pad / 2);
@@ -758,6 +982,9 @@ size_t call_bytes(const MetPlan &p, int64_t B, bool host, int64_t in_numel, int 
     s += 2 * a256(sizeof(float) * (kStoiBands * p.n_fr + 1));            // band magnitudes
     s += a256(sizeof(double) * (p.n_ss + 1)) + a256(sizeof(double) * (3 * p.n_ch + 1));
     s += 2 * a256(sizeof(double) * (p.n_cf + 1));                        // LLR / WSS frame values
+    // pystoi: energies, kept list, band magnitudes of both signals, STOI / ESTOI segment sums, states
+    s += a256(sizeof(double) * (p.n_pf + 1)) + a256(sizeof(int) * (p.n_pf + 1)) + 2 * a256(sizeof(double) * (kStoiBands * p.n_pf + 1));
+    s += a256(sizeof(double) * (2 * p.n_pf + 1)) + a256(sizeof(MetState) * B);
     if (host) s += 2 * a256(sizeof(float) * in_numel) + a256(sizeof(float) * n_rows * B);
     return s;
 }
@@ -784,6 +1011,13 @@ int run_call(dfb_metrics *h, const float *d_clean, const float *d_deg, const Met
     mb.ch = a.take<double>(3 * p.n_ch + 1);
     mb.llr = a.take<double>(p.n_cf + 1);
     mb.wss = a.take<double>(p.n_cf + 1);
+    mb.pen = a.take<double>(p.n_pf + 1);
+    mb.pkidx = a.take<int>(p.n_pf + 1);
+    mb.pbx = a.take<double>(kStoiBands * p.n_pf + 1);
+    mb.pby = a.take<double>(kStoiBands * p.n_pf + 1);
+    mb.pseg = a.take<double>(2 * p.n_pf + 1);
+    mb.pst = a.take<MetState>(B);
+    mb.n_pf = p.n_pf;
     mb.fft_tw = h->d_fft_tw;
     mb.n_fr = p.n_fr;
     mb.n_ch = p.n_ch;
@@ -817,12 +1051,28 @@ int run_call(dfb_metrics *h, const float *d_clean, const float *d_deg, const Met
     if (bits & DFB_METRIC_STOI) {
         k_stoi_energy<<<dim3((unsigned)((p.max_fr + 7) / 8), ub), 256, 0, s>>>(d_ents, mb);
         DFB_LAUNCH_CHECK();
-        k_stoi_mask<<<ub, 1024, 0, s>>>(d_ents, mb);
+        k_stoi_mask<false><<<ub, 1024, 0, s>>>(d_ents, mb);
         DFB_LAUNCH_CHECK();
         k_stoi_stft<<<dim3((unsigned)((p.max_fr + kStftFrames - 1) / kStftFrames), ub), 256, 0, s>>>(d_ents, mb, h->plan, h->bands);
         DFB_LAUNCH_CHECK();
         k_stoi_seg<<<dim3((unsigned)((p.max_fr + 7) / 8), ub), 256, 0, s>>>(d_ents, mb);
         DFB_LAUNCH_CHECK();
+    }
+    if (bits & (DFB_METRIC_PYSTOI | DFB_METRIC_ESTOI)) {
+        if (p.max_pf > 0) {
+            k_pystoi_energy<<<dim3((unsigned)((p.max_pf + 7) / 8), ub), 256, 0, s>>>(d_ents, mb);
+            DFB_LAUNCH_CHECK();
+        }
+        k_stoi_mask<true><<<ub, 1024, 0, s>>>(d_ents, mb);
+        DFB_LAUNCH_CHECK();
+        if (p.max_pf > 1) {
+            k_pystoi_stft<<<dim3((unsigned)p.max_pf, ub), 128, 0, s>>>(d_ents, mb, h->bands);
+            DFB_LAUNCH_CHECK();
+        }
+        if (p.max_pf > kStoiSeg) {
+            k_pystoi_seg<<<dim3((unsigned)((p.max_pf + 7) / 8), ub), 256, 0, s>>>(d_ents, mb);
+            DFB_LAUNCH_CHECK();
+        }
     }
     if ((bits & DFB_METRIC_SSNR) && p.max_ss > 1) {
         k_ssnr<<<dim3((unsigned)((p.max_ss + 7) / 8), ub), 256, 0, s>>>(d_ents, mb);
@@ -849,6 +1099,13 @@ int run_call(dfb_metrics *h, const float *d_clean, const float *d_deg, const Met
         for (const MetEntry &e : p.ents) h->last_nct.push_back(e.nct);
     h->last_llr = mb.llr;
     h->last_wss = mb.wss;
+    h->last_pnf.clear();
+    h->last_po.clear();
+    if (bits & (DFB_METRIC_PYSTOI | DFB_METRIC_ESTOI))
+        for (const MetEntry &e : p.ents) { h->last_pnf.push_back(e.pnf); h->last_po.push_back(e.po); }
+    h->last_pst = mb.pst;
+    h->last_pbx = mb.pbx;
+    h->last_pby = mb.pby;
     if (host) {
         DFB_CUDA(cudaMemcpyAsync(h_out, d_out, sizeof(float) * n_rows * B, cudaMemcpyDeviceToHost, s));
         DFB_CUDA(cudaStreamSynchronize(s));
@@ -896,6 +1153,8 @@ extern "C" int dfb_metrics_create(dfb_metrics **out, int device, int sr, const f
     }
     float w256[kStoiFrame];
     for (int n = 0; n < kStoiFrame; n++) w256[n] = (float)(0.5 - 0.5 * std::cos(2.0 * M_PI * (n + 1) / (kStoiFrame + 1)));
+    double w256d[kStoiFrame];
+    for (int n = 0; n < kStoiFrame; n++) w256d[n] = 0.5 - 0.5 * std::cos(2.0 * M_PI * (n + 1) / (kStoiFrame + 1));
     double wss[kSsnrWin];
     for (int n = 0; n < kSsnrWin; n++) wss[n] = 0.5 * (1.0 - std::cos(2.0 * M_PI * (n + 1) / (kSsnrWin + 1)));
     std::vector<double2> tw64(kWssFft);
@@ -907,7 +1166,8 @@ extern "C" int dfb_metrics_create(dfb_metrics **out, int device, int sr, const f
         cudaMemcpyToSymbol(c_crit, crit.w, sizeof crit.w) != cudaSuccess || cudaMemcpyToSymbol(c_crit_lo, crit.lo, sizeof crit.lo) != cudaSuccess ||
         cudaMemcpyToSymbol(c_crit_n, crit.n, sizeof crit.n) != cudaSuccess || cudaMemcpyToSymbol(c_crit_off, crit.off, sizeof crit.off) != cudaSuccess ||
         cudaMemcpy(h->d_dirs, h->dirs, sizeof(RateDir) * 2, cudaMemcpyHostToDevice) != cudaSuccess ||
-        cudaMemcpyToSymbol(c_w256, w256, sizeof w256) != cudaSuccess || cudaMemcpyToSymbol(c_wss, wss, sizeof wss) != cudaSuccess)
+        cudaMemcpyToSymbol(c_w256, w256, sizeof w256) != cudaSuccess || cudaMemcpyToSymbol(c_wss, wss, sizeof wss) != cudaSuccess ||
+        cudaMemcpyToSymbol(c_w256d, w256d, sizeof w256d) != cudaSuccess)
         return bail(fail(DFB_ERR_CUDA, "metrics table upload failed"));
     h->plan.tw = h->d_tw;
     *out = h;
@@ -980,5 +1240,42 @@ extern "C" int dfb_debug_metrics_frames(dfb_metrics *h, const float *h_clean, co
     if (n > capacity) return fail(DFB_ERR_INVALID, "%lld frames, room for %lld", (long long)n, (long long)capacity);
     DFB_CUDA(cudaMemcpy(h_llr, h->last_llr, sizeof(double) * n, cudaMemcpyDeviceToHost));
     DFB_CUDA(cudaMemcpy(h_wss, h->last_wss, sizeof(double) * n, cudaMemcpyDeviceToHost));
+    return DFB_OK;
+}
+
+extern "C" int dfb_debug_metrics_pystoi(dfb_metrics *h, const float *h_clean, const float *h_degraded, int64_t in_numel,
+                                        const int64_t *offsets, const int64_t *lengths, int64_t B, int64_t *h_counts,
+                                        double *h_bands, int64_t capacity) {
+    if (!h || !h_counts) return fail(DFB_ERR_INVALID, "null argument");
+    std::vector<float> rows((size_t)(2 * (B > 0 ? B : 1)));
+    int rc = dfb_metrics_compute_host(h, h_clean, h_degraded, in_numel, offsets, lengths, lengths, B,
+                                      DFB_METRIC_PYSTOI | DFB_METRIC_ESTOI, rows.data());
+    if (rc) return rc;
+    std::vector<MetState> st(B);
+    DFB_CUDA(cudaMemcpy(st.data(), h->last_pst, sizeof(MetState) * B, cudaMemcpyDeviceToHost));
+    int64_t n = 0;
+    for (int64_t b = 0; b < B; b++) {
+        const int64_t F = h->last_pnf[b], nf = F > 0 ? st[b].nf : 0;
+        int64_t *c = h_counts + 5 * b;
+        c[0] = F;
+        c[1] = F > 0 ? st[b].nk : 0;
+        c[2] = F > 0 ? st[b].lc : 0;
+        c[3] = nf;
+        c[4] = nf >= kStoiSeg ? nf - kStoiSeg + 1 : 0;
+        n += 2 * kStoiBands * nf;
+    }
+    if (!h_bands) return DFB_OK;
+    if (n > capacity) return fail(DFB_ERR_INVALID, "%lld band magnitudes, room for %lld", (long long)n, (long long)capacity);
+    int64_t o = 0;
+    for (int64_t b = 0; b < B; b++) {
+        const int64_t F = h->last_pnf[b], nf = h_counts[5 * b + 3];
+        if (nf == 0) continue;
+        for (int sig = 0; sig < 2; sig++) {
+            const double *src = (sig ? h->last_pby : h->last_pbx) + kStoiBands * h->last_po[b];
+            DFB_CUDA(cudaMemcpy2D(h_bands + o, sizeof(double) * nf, src, sizeof(double) * F, sizeof(double) * nf, kStoiBands,
+                                  cudaMemcpyDeviceToHost));
+            o += kStoiBands * nf;
+        }
+    }
     return DFB_OK;
 }

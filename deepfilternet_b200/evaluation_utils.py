@@ -1,17 +1,21 @@
 """Speech-quality scoring on the device, after ``df.evaluation_utils`` (DeepFilterNet/df/evaluation_utils.py).
 
-Five metrics, each equal to the reference function applied to one entry alone (include/dfb200.h, DESIGN.md sections 5j
-and 5m):
+Seven metrics, each equal to the reference function applied to one entry alone (include/dfb200.h, DESIGN.md sections
+5j, 5m and 5n):
 
 * ``"sisdr"``: ``si_sdr_speechmetrics(clean, degraded)`` at the input rate.
 * ``"stoi"``: ``df.stoi.stoi(clean[None], degraded[None], sr)[0]`` (:func:`deepfilternet_b200.stoi.stoi`), NaN for an
   entry with fewer than 512 samples left at 10 kHz after silence removal (the reference leaves garbage there).  This is
-  df/stoi.py's STOI, not pystoi's, which the reference's ``StoiMetric`` reports: pystoi removes silence and frames the
-  signal differently.  How far the two differ is not measured.
+  df/stoi.py's STOI, the reference's training-validation STOI, not pystoi's, which its evaluation reports: pystoi removes
+  silence and frames the signal differently (DESIGN.md section 5n gives the measured difference).
 * ``"ssnr"``: ``df.sepm.SNRseg(c16, d16, 16000)`` after ``io.resample(x, sr, 16000)``, the fifth value of the reference's
   ``CompositeMetric``; NaN for an entry with no frame left.
 * ``"llr"`` / ``"wss"``: ``df.sepm.llr(c16, d16, 16000)`` / ``df.sepm.wss(c16, d16, 16000)`` on the same 16 kHz rows;
   NaN for an entry with fewer than 600 samples at 16 kHz (no frame).
+* ``"pystoi"`` / ``"estoi"``: ``df.evaluation_utils.stoi(clean, degraded, sr, extended)`` (:func:`stoi`), pystoi's STOI
+  and extended STOI after ``io.resample(x, sr, 10000)``, what the reference's ``StoiMetric`` and CI report; NaN for an
+  entry of at most 256 samples at 10 kHz (pystoi raises), 1e-5 when fewer than 30 STFT frames remain (pystoi's value).
+  ESTOI omits pystoi's eps-scaled random noise.
 
 A batch is scored by one library call (``dfb_metrics_compute(_host)``): resampling, silence removal, STFT, band
 envelopes, segment correlations, LPC models, critical-band spectra and every per-entry mean run on the GPU.
@@ -43,7 +47,8 @@ from ._lib import check
 logger = logging.getLogger("deepfilternet_b200")
 
 # metric name -> (bit of dfb_metrics_compute, name in results and CSV files); the output rows follow the bit order
-METRICS = {"sisdr": (1, "SISDR"), "stoi": (2, "STOI"), "ssnr": (4, "SSNR"), "llr": (16, "LLR"), "wss": (32, "WSS")}
+METRICS = {"sisdr": (1, "SISDR"), "stoi": (2, "STOI"), "ssnr": (4, "SSNR"), "llr": (16, "LLR"), "wss": (32, "WSS"),
+           "pystoi": (128, "PYSTOI"), "estoi": (256, "ESTOI")}
 # "composite" with a caller's PESQ: its values, in the reference CompositeMetric's order, and the device rows it needs
 COMPOSITE_NAMES = ("PESQ", "CSIG", "CBAK", "COVL", "SSNR")
 COMPOSITE_BITS = 4 | 16 | 32
@@ -291,6 +296,17 @@ def si_sdr_speechmetrics(reference, estimate) -> float:
     e = torch.as_tensor(np.asarray(estimate, dtype=np.float32).reshape(-1))
     # SI-SDR does not resample, so any supported rate serves
     return float(evaluate_batch([r], [e], 48000, ("sisdr",))["sisdr"][0])
+
+
+def stoi(clean, degraded, sr: int, extended: bool = False) -> float:
+    """df.evaluation_utils.stoi: pystoi's STOI (ESTOI with ``extended``) of one pair of equal-length 1-D signals at
+    ``sr`` Hz after ``io.resample`` to 10 kHz, on the device."""
+    c = np.asarray(clean, dtype=np.float32)
+    d = np.asarray(degraded, dtype=np.float32)
+    if c.ndim != 1 or d.ndim != 1:
+        raise ValueError("stoi expects 1-D signals")
+    m = "estoi" if extended else "pystoi"
+    return float(evaluate_batch([torch.from_numpy(c)], [torch.from_numpy(d)], sr, (m,))[m][0])
 
 
 # ----------------------------------------------------------------------------------- evaluation loop ----

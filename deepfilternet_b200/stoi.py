@@ -27,8 +27,9 @@ def stoi(x: Tensor, y: Tensor, fs_source: int) -> Tensor:
        mean-free and unit-norm; the result is the mean of their correlations over bands and segments.
 
     A row with fewer than 512 samples after step 2 gets NaN (df/stoi.py skips it and leaves garbage in its slot).
-    This is df/stoi.py's STOI, not pystoi's (which the reference uses for reporting): pystoi removes silence and frames
-    the signal differently, and the difference between the two is not measured."""
+    This is df/stoi.py's STOI, not pystoi's (which the reference uses for reporting, and
+    ``evaluation_utils.stoi`` computes): pystoi removes silence and frames the signal differently.  On the reference's
+    pretrained outputs for its CI asset the two differ by 3e-4 to 6e-4 (DESIGN.md section 5n)."""
     if x.shape != y.shape:
         raise ValueError("Inputs must have the same shape")
     if x.dim() != 2:

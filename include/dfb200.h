@@ -687,9 +687,19 @@ int64_t dfb_model_workspace_bytes(const dfb_model *m);
  *   DFB_METRIC_WSS    df/sepm.py wss(c16, d16, 16000): Klatt's weighted spectral slope over 25 critical bands on the same
  *                     frames, averaged the same way.  LLR and WSS are NaN when T = 0.
  * With PESQ-WB (not provided) they make df/sepm.py's composite measure: CSIG, CBAK and COVL are Hu & Loizou's (IEEE TASLP
- * 16(1), 2008) linear regressions on PESQ, LLR, WSS and SSNR.  Bit 8 is not a metric.
- * This STOI is df/stoi.py's, not pystoi's, which removes silence and frames differently. */
-enum { DFB_METRIC_SISDR = 1, DFB_METRIC_STOI = 2, DFB_METRIC_SSNR = 4, DFB_METRIC_LLR = 16, DFB_METRIC_WSS = 32 };
+ * 16(1), 2008) linear regressions on PESQ, LLR, WSS and SSNR.
+ *   DFB_METRIC_PYSTOI pystoi.stoi(x10, y10, 10000) (pystoi 0.4.1), which df/evaluation_utils.py stoi reports, on the
+ *                     same 10 kHz rows as STOI: F = ceil((L10 - 256) / 128) frames of 256 samples at hop 128, those
+ *                     within 40 dB of the loudest kept and overlap-added (K of them), K - 1 STFT frames, J = K - 30
+ *                     segments of 30 frames, all in fp64 (DESIGN.md section 5n);
+ *   DFB_METRIC_ESTOI  pystoi.stoi(x10, y10, 10000, extended=True) on the same segments, without pystoi's eps-scaled
+ *                     random noise: a centred row or column of norm 0 normalises to 0.
+ *                     Both are NaN when L10 <= 256 (no frame: pystoi raises) and 1e-5 when K - 1 < 30 (pystoi's value).
+ * Bits 8 and 64 are not metrics.  DFB_METRIC_STOI is df/stoi.py's STOI, which removes silence and frames differently from pystoi's. */
+enum {
+    DFB_METRIC_SISDR = 1, DFB_METRIC_STOI = 2, DFB_METRIC_SSNR = 4, DFB_METRIC_LLR = 16, DFB_METRIC_WSS = 32,
+    DFB_METRIC_PYSTOI = 128, DFB_METRIC_ESTOI = 256
+};
 typedef struct dfb_metrics dfb_metrics;
 /* A metrics handle on `device` for inputs at `sr` Hz: taps10 / taps16 [nw][2 width + og] (HOST arrays) are
  * io.resample_kernel(sr, 10000) / (sr, 16000) with the sinc_fast parameters, og / nw the gcd-reduced rates (DFB_ERR_INVALID
@@ -700,7 +710,7 @@ int dfb_metrics_create(dfb_metrics **out, int device, int sr, const float *taps1
 void dfb_metrics_free(dfb_metrics *h);
 /* One call scores B <= 32767 entries: entry b is clean_lengths[b] samples of clean at d_clean + offsets[b] and as many of
  * degraded at d_degraded + offsets[b] (offsets / lengths HOST arrays, in_numel bounding both buffers).  d_out [n][B] fp32
- * gets one row per bit of `metrics`, in the order SI-SDR, STOI, SSNR, LLR, WSS.  DFB_ERR_INVALID for a length <= 0, different clean
+ * gets one row per bit of `metrics`, in the order SI-SDR, STOI, SSNR, LLR, WSS, PYSTOI, ESTOI.  DFB_ERR_INVALID for a length <= 0, different clean
  * and degraded lengths, an entry outside in_numel, no metric or an unknown metric bit.  Asynchronous on `stream`; the
  * handle's workspace serves one call at a time. */
 int dfb_metrics_compute(dfb_metrics *h, const float *d_clean, const float *d_degraded, int64_t in_numel, const int64_t *offsets,
@@ -721,6 +731,13 @@ int dfb_debug_metrics_counts(dfb_metrics *h, const float *h_clean, const float *
 int dfb_debug_metrics_frames(dfb_metrics *h, const float *h_clean, const float *h_degraded, int64_t in_numel,
                              const int64_t *offsets, const int64_t *lengths, int64_t B, int64_t *h_frames, double *h_llr,
                              double *h_wss, int64_t capacity);
+/* Debug aid: the PYSTOI and ESTOI of a dfb_metrics_host call, then h_counts [B][5] = each entry's pystoi frames F, kept
+ * frames K, silence-free length, STFT frames nf and segments J (all 0 when F = 0).  When h_bands is not NULL it gets every
+ * entry's band magnitudes (fp64), entries back to back, each [2][15][nf] (clean, then degraded); DFB_ERR_INVALID when
+ * they exceed `capacity` doubles. */
+int dfb_debug_metrics_pystoi(dfb_metrics *h, const float *h_clean, const float *h_degraded, int64_t in_numel,
+                             const int64_t *offsets, const int64_t *lengths, int64_t B, int64_t *h_counts, double *h_bands,
+                             int64_t capacity);
 
 #ifdef __cplusplus
 }
