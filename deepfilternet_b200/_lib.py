@@ -124,6 +124,11 @@ SIGNATURES = {
     "dfb_stream_open_linked_at": (_I, [_VP, _I64P, _I64, _I]),
     "dfb_stream_slot_rates": (_I, [_VP, C.POINTER(C.c_int32)]),
     "dfb_debug_resample_slots": (_I, [_I, _VP, C.POINTER(C.c_int32), _VP, _I64, _I64P, _I64, _VP, _VP]),
+    "dfb_stream_session_bytes": (_I, [_VP, C.POINTER(C.c_int32), _I, _I64P]),
+    "dfb_stream_export_sessions": (_I, [_VP, C.POINTER(C.c_int32), _I, _I, _VP, _VP]),
+    "dfb_stream_export_sessions_host": (_I, [_VP, C.POINTER(C.c_int32), _I, _I, _VP]),
+    "dfb_stream_import_sessions": (_I, [_VP, C.POINTER(C.c_int32), _I, _VP, _VP]),
+    "dfb_stream_import_sessions_host": (_I, [_VP, C.POINTER(C.c_int32), _I, _VP]),
     "dfb_stream_create_spec": (_I, [C.POINTER(_VP), _VP, _VP, _I64]),
     "dfb_stream_process_spec": (_I, [_VP, _VP, _I64, _VP, _VP, _VP, _VP, _VP]),
     "dfb_stream_flush_spec": (_I, [_VP, _VP, _VP, _VP, _VP, _VP]),

@@ -534,7 +534,38 @@ struct dfb_model {
     std::vector<RateDir> rate_up, rate_down;
     std::vector<float *> rate_taps;
     RateDir *d_rate_dirs = nullptr;
+    uint64_t fingerprint = 0;               // the config and the weight bytes (model_fingerprint): what a session blob names
 };
+
+// A 64-bit fingerprint of a model: its config, its ERB band widths, then every tensor's name, size and bytes in name order (the order the
+// caller lists them in does not matter).  It tells session blobs (dfb_stream_export_sessions) of different models apart;
+// it is not a cryptographic hash.
+static uint64_t fp_mix(uint64_t h, const void *p, size_t n) {
+    const unsigned char *b = static_cast<const unsigned char *>(p);
+    size_t i = 0;
+    for (; i + 8 <= n; i += 8) {
+        uint64_t w;
+        memcpy(&w, b + i, 8);
+        h = (h ^ w) * 0x9E3779B97F4A7C15ull;
+        h ^= h >> 29;
+    }
+    uint64_t w = n;
+    for (size_t k = 0; i < n; i++, k++) w ^= (uint64_t)b[i] << (8 * (k % 8));
+    h = (h ^ w) * 0xBF58476D1CE4E5B9ull;
+    return h ^ (h >> 31);
+}
+static uint64_t model_fingerprint(const dfb_model_config &c, const int64_t *erb_widths, const dfb_tensor *tensors, int n_tensors) {
+    uint64_t h = fp_mix(0x6466623230307366ull, &c, sizeof c);
+    if (erb_widths) h = fp_mix(h, erb_widths, sizeof(int64_t) * (size_t)c.nb_erb);   // the ERB bands the model was built for
+    std::map<std::string, int> order;
+    for (int i = 0; i < n_tensors; i++) order[tensors[i].name] = i;
+    for (const auto &kv : order) {
+        const dfb_tensor &t = tensors[kv.second];
+        h = fp_mix(h, kv.first.data(), kv.first.size());
+        h = fp_mix(h, t.data, (size_t)t.numel * sizeof(float));
+    }
+    return h;
+}
 
 // Looks the uploaded tensors up by name.  The first missing or wrong-sized one (numel < 0: any size) becomes the bind's
 // error; lookups after it return null.
@@ -697,6 +728,7 @@ extern "C" int dfb_model_create(dfb_model **out, int device, const dfb_model_con
         t[tt.name] = {dst, tt.numel};
         off += ((size_t)tt.numel * 4 + 255) & ~size_t(255);
     }
+    m->fingerprint = model_fingerprint(*cfg, erb_widths, tensors, n_tensors);
     Binder b{t};
     if ((rc = cfg->model_kind == 1 ? bind_v1(*cfg, b, m->net1) : bind_net(*cfg, b, m->net))) {
         dfb_model_free(m);
@@ -2046,6 +2078,20 @@ static ChunkGeom chunk_geom(const dfb_model_config &c) {
 constexpr int kStateArrays = 17;
 // row_off / row_floats: one stream's row of every array, packed (the scratch rows of k_slot_rows)
 struct StateLayout { int64_t off[kStateArrays], row_off[kStateArrays], row_floats; int layers[kStateArrays], per_row[kStateArrays]; };
+constexpr int kRsArray = kStateArrays - 2;   // the first resampler history (15: up, 16: down)
+
+// Element e (layer-major, as row_off packs a row) of slab row `row` of array a, in a slab of Bs rows.  Every kernel that
+// moves state rows addresses them here: k_slot_rows, k_sessions_pack, k_sessions_unpack.
+__device__ __forceinline__ int64_t state_elem(const StateLayout &lay, int Bs, int a, int row, int64_t e) {
+    const int per = lay.per_row[a];
+    const int l = (int)(e / per), j = (int)(e - (int64_t)l * per);
+    return lay.off[a] + ((int64_t)l * Bs + row) * per + j;
+}
+// element e of array a in a fresh stream's row: zeros, and the normalisation EMA states at the values launch_feat_norm
+// starts from without a state (arrays 1 and 2 have one layer)
+__device__ __forceinline__ float state_init(int a, int64_t e, int E, int Fd) {
+    return a == 1 ? erb_norm_init((int)e, E) : a == 2 ? unit_norm_init((int)e, Fd) : 0.f;
+}
 
 static size_t state_floats(const dfb_model_config &c, const dfb_state *st, int B, size_t off[kStateArrays], StateLayout *lay = nullptr,
                            int rs_up = 0, int rs_down = 0) {
@@ -3169,22 +3215,16 @@ constexpr int64_t kOpenEnd = 0x7fffffff;   // rows[b].Tf of an open slot: kernel
 // Two launches whatever the number of rows.  grid (x, ops of the pass, kStateArrays).
 __global__ void k_slot_rows(float *__restrict__ slab, StateLayout lay, int Bs, const int2 *__restrict__ ops, float *__restrict__ scratch,
                             int pass, int E, int Fd) {
-    const int i = blockIdx.y, a = blockIdx.z, per = lay.per_row[a];
+    const int i = blockIdx.y, a = blockIdx.z;
     const int2 op = ops[i];
-    const int64_t n = (int64_t)lay.layers[a] * per;
+    const int64_t n = (int64_t)lay.layers[a] * lay.per_row[a];
     float *sc = scratch + (int64_t)i * lay.row_floats + lay.row_off[a];
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
-        const int l = (int)(e / per), j = (int)(e - (int64_t)l * per);
-        float *base = slab + lay.off[a] + (int64_t)l * Bs * per + j;
         if (pass == 0) {
-            sc[e] = base[(int64_t)op.y * per];
+            sc[e] = slab[state_elem(lay, Bs, a, op.y, e)];
             continue;
         }
-        float v = 0.f;
-        if (op.y >= 0) v = sc[e];
-        else if (a == 1) v = erb_norm_init(j, E);
-        else if (a == 2) v = unit_norm_init(j, Fd);
-        base[(int64_t)op.x * per] = v;
+        slab[state_elem(lay, Bs, a, op.x, e)] = op.y >= 0 ? sc[e] : state_init(a, e, E, Fd);
     }
 }
 
@@ -3261,6 +3301,8 @@ struct dfb_stream {
     size_t rs_in_cap = 0, rs_out_cap = 0;
     float *rs_lsnr = nullptr;                          // flush: the LSNR of its two passes
     size_t rs_lsnr_cap = 0;
+    float *sess_stage = nullptr;                       // device staging of dfb_stream_export / import_sessions_host
+    size_t sess_stage_cap = 0;
     std::vector<ResampleRow> rs_rows;                  // the live rows' table on the device
     ResampleRow *d_rs = nullptr;
 };
@@ -3363,7 +3405,7 @@ extern "C" void dfb_stream_free(dfb_stream *h) {
     if (h->d_slotmap) cudaFree(h->d_slotmap);
     if (h->spec_stage_in) cudaFree(h->spec_stage_in);
     if (h->spec_stage_out) cudaFree(h->spec_stage_out);
-    for (float *p : {h->rs_in, h->rs_out, h->rs_lsnr})
+    for (float *p : {h->rs_in, h->rs_out, h->rs_lsnr, h->sess_stage})
         if (p) cudaFree(p);
     for (float *p : h->rs_taps) cudaFree(p);
     if (h->d_rs) cudaFree(h->d_rs);
@@ -3605,27 +3647,31 @@ static int ctl_check(const dfb_stream *h, const int64_t *slots, int64_t n) {
     return DFB_OK;
 }
 
+// The per-row settings table from now on (the device table allocated once).
+static int ctl_enable(dfb_stream *h) {
+    if (h->ctl_on) return DFB_OK;
+    if (!h->d_ctl) {
+        DFB_CUDA(cudaSetDevice(h->m->device));
+        if (cudaMalloc(&h->d_ctl, sizeof(SlotCtl) * (size_t)h->B) != cudaSuccess) {
+            h->d_ctl = nullptr;
+            return fail(DFB_ERR_OOM, "slot settings allocation failed");
+        }
+    }
+    // every slot has run with the handle's settings so far
+    for (int b = 0; b < h->B; b++) h->slot_ctl[(size_t)b] = SlotCtl{h->lim, h->beta_run, h->lim, h->beta_run, 0};
+    std::fill(h->slot_fresh.begin(), h->slot_fresh.end(), (char)0);
+    h->ctl_up.clear();
+    h->ctl_on = true;
+    return DFB_OK;
+}
+
 // After the value's checks: naming a free slot is refused; otherwise the per-row table is on from now on.
 static int ctl_begin(dfb_stream *h, const int64_t *slots, int64_t n) {
     for (int64_t i = 0; i < n; i++)
         if (h->slot_state[(size_t)slots[i]] == kSlotFree) return fail(DFB_ERR_INVALID, "slot %lld is free", (long long)slots[i]);
     if (n == 0) return DFB_OK;
     h->slot_ops = true;
-    if (!h->ctl_on) {
-        if (!h->d_ctl) {
-            DFB_CUDA(cudaSetDevice(h->m->device));
-            if (cudaMalloc(&h->d_ctl, sizeof(SlotCtl) * (size_t)h->B) != cudaSuccess) {
-                h->d_ctl = nullptr;
-                return fail(DFB_ERR_OOM, "slot settings allocation failed");
-            }
-        }
-        // every slot has run with the handle's settings so far
-        for (int b = 0; b < h->B; b++) h->slot_ctl[(size_t)b] = SlotCtl{h->lim, h->beta_run, h->lim, h->beta_run, 0};
-        std::fill(h->slot_fresh.begin(), h->slot_fresh.end(), (char)0);
-        h->ctl_up.clear();
-        h->ctl_on = true;
-    }
-    return DFB_OK;
+    return ctl_enable(h);
 }
 
 static int ctl_set(dfb_stream *h, const int64_t *slots, int64_t n, bool beta, float v) {
@@ -4235,6 +4281,476 @@ extern "C" int dfb_stream_process_host_lsnr(dfb_stream *h, const float *h_in, in
 }
 extern "C" int dfb_stream_process_host(dfb_stream *h, const float *h_in, int64_t n_frames, float *h_out) {
     return dfb_stream_process_host_lsnr(h, h_in, n_frames, h_out, nullptr);
+}
+
+// ---- session export / import (dfb_stream_export_sessions / dfb_stream_import_sessions; DESIGN.md section 5o).  A session
+// is its rows of the 17 state arrays plus the host bookkeeping of its slots; its outputs depend on the handle only through
+// the handle's clock, which the blob replaces by the session's age.  The rows move in one kernel launch per direction.
+constexpr uint32_t kBlobMagic = 0x53424644u;   // "DFBS", little-endian
+constexpr uint32_t kBlobVersion = 1;
+constexpr int64_t kNoLsnr = INT64_MIN;         // BlobSession::lsnr_start of a session whose LSNR head never ran
+struct BlobHeader {
+    uint32_t magic, version;
+    uint64_t fingerprint;
+    int32_t sr, fft_size, hop_size, nb_erb;
+    int32_t gating_mode, gate_tails, n_sessions, n_rows;
+    int64_t total_bytes;
+    int64_t row_floats[kStateArrays];
+};
+struct BlobSession {
+    int64_t age, lsnr_start, ctl_switch;
+    int32_t rate, channels, reduce, reserved;
+    float lim, beta;
+    int32_t gate;
+    float th[3];
+    float last_lim, last_beta, prev_lim, prev_beta;
+    int32_t last_gate;
+    float last_th[3];
+    int32_t up_hist, down_hist;
+    int64_t data_offset;
+};
+static_assert(sizeof(BlobHeader) == 192 && sizeof(BlobSession) == 112, "the blob layout of include/dfb200.h");
+
+// One row (channel) of a blob: its slab row (-1 on export: a fresh stream's initial state), its floats' offset in the
+// data area, its session's own resampler history widths and (import) the leading entries of its LSNR tail read as NaN.
+struct SessionRow { int64_t blob; int slab, up, down, nan_l; };
+
+// Offset of array a in a blob row: arrays 0 .. 14 as the slab's row_off packs them, then the row's own histories.
+__device__ __forceinline__ int64_t blob_elem0(const StateLayout &lay, const SessionRow &r, int a) {
+    return r.blob + (a < kRsArray ? lay.row_off[a] : lay.row_off[kRsArray] + (a > kRsArray ? r.up : 0));
+}
+
+// Every listed row of every state array into the blob, read where the row's state lives at the last call (a pending
+// move's source) or as a fresh stream's initial state.  grid (x, rows, kStateArrays).
+__global__ void k_sessions_pack(const float *__restrict__ slab, StateLayout lay, int Bs, const SessionRow *__restrict__ rows,
+                                float *__restrict__ blob, int E, int Fd) {
+    const int a = blockIdx.z;
+    const SessionRow r = rows[blockIdx.y];
+    const int64_t n = a < kRsArray ? (int64_t)lay.layers[a] * lay.per_row[a] : a == kRsArray ? r.up : r.down;
+    float *dst = blob + blob_elem0(lay, r, a);
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x)
+        dst[e] = r.slab >= 0 ? slab[state_elem(lay, Bs, a, r.slab, e)] : state_init(a, e, E, Fd);
+}
+
+// The blob's rows into slab rows: a resampler history padded with zeros to the handle's width, the first nan_l entries
+// of the LSNR tail (array 12) NaN.  grid (x, rows, kStateArrays).
+__global__ void k_sessions_unpack(float *__restrict__ slab, StateLayout lay, int Bs, const SessionRow *__restrict__ rows,
+                                  const float *__restrict__ blob) {
+    const int a = blockIdx.z;
+    const SessionRow r = rows[blockIdx.y];
+    const int64_t n = (int64_t)lay.layers[a] * lay.per_row[a], own = a < kRsArray ? n : a == kRsArray ? r.up : r.down;
+    const float *src = blob + blob_elem0(lay, r, a);
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+        float v = e < own ? src[e] : 0.f;
+        if (a == 12 && e < r.nan_l) v = __int_as_float(0x7fffffff);
+        slab[state_elem(lay, Bs, a, r.slab, e)] = v;
+    }
+}
+
+// One launch of the pack (export) or unpack kernel over the rows, their table in the model arena.
+static int sessions_launch(dfb_stream *h, bool pack, const std::vector<SessionRow> &rows, float *blob_data, cudaStream_t s) {
+    if (rows.empty()) return DFB_OK;
+    dfb_model *m = h->m;
+    size_t off[kStateArrays];
+    StateLayout lay;
+    stream_state_floats(h, off, &lay);
+    if (int rc = m->arena.reserve(sizeof(SessionRow) * rows.size() + 1024)) return rc;
+    m->arena.reset();
+    SessionRow *d_rows = m->arena.take<SessionRow>(rows.size());
+    DFB_CUDA(cudaMemcpyAsync(d_rows, rows.data(), sizeof(SessionRow) * rows.size(), cudaMemcpyHostToDevice, s));
+    const dim3 grid(4, (unsigned)rows.size(), kStateArrays);
+    if (pack)
+        k_sessions_pack<<<grid, 256, 0, s>>>(h->slab, lay, h->B, d_rows, blob_data, m->cfg.nb_erb, m->cfg.nb_df);
+    else
+        k_sessions_unpack<<<grid, 256, 0, s>>>(h->slab, lay, h->B, d_rows, blob_data);
+    DFB_LAUNCH_CHECK();
+    m->arena.reset();
+    return DFB_OK;
+}
+
+// what session export and import refuse on any handle
+static int sessions_handle(const dfb_stream *h) {
+    if (!h) return fail(DFB_ERR_INVALID, "null stream");
+    if (h->spectral) return fail(DFB_ERR_UNSUPPORTED, "session export / import: audio handles only (a spectral handle's sessions do not move)");
+    if (h->m->cfg.model_kind == 1) return fail(DFB_ERR_UNSUPPORTED, "DeepFilterNet v1 has no streaming sessions");
+    return DFB_OK;
+}
+static int eff_gating_mode(const dfb_stream *h) { return h->gating_mode >= 0 ? h->gating_mode : h->m->gating_mode; }
+static int slot_rate_of(const dfb_stream *h, int b) { return resampled(h) ? h->rs_rates[(size_t)h->slot_dir[(size_t)b]] : kModelRate; }
+static int rs_own(const dfb_stream *h, int dir, bool up) { return resampled(h) ? (up ? h->rs_up : h->rs_down).d[dir].S : 0; }
+static bool ctl_shape(const dfb_model_config &c) { return c.df_order == 5 && c.nb_df == 96 && c.nb_erb == 32; }
+
+// A handle whose clock has settled: its DNN and output frames trail the input by the model's look-ahead and lag, a full
+// halo lies behind them and every tail is full.  A session's state means the same in every such handle.
+static bool clock_settled(const dfb_stream *h) {
+    const StreamState &S = h->S;
+    const dfb_model_config &c = h->m->cfg;
+    const ChunkGeom g = chunk_geom(c);
+    return S.started && S.dnn_started && S.d1 == S.a1 - g.Lmax && S.e1 == S.d1 - g.lag && S.d1 >= kHalo && S.n_feat == g.Hf &&
+           S.n_mc == kMcTail && (c.conv_kt == 1 || S.n_dec == kHalo);
+}
+// An idle handle (no live row) moves its clock to the first settled frame, as a call with nothing to compute would.
+static void clock_settle(dfb_stream *h) {
+    StreamState &S = h->S;
+    const ChunkGeom g = chunk_geom(h->m->cfg);
+    S.a1 = std::max<int64_t>(S.a1, kHalo + g.Lmax);
+    S.d1 = S.a1 - g.Lmax; S.e1 = S.d1 - g.lag;
+    S.started = S.dnn_started = true;
+    S.n_feat = g.Hf; S.n_mc = kMcTail; S.n_dec = kHalo;
+}
+
+// An export's slots: open, each linked group whole, from its channel 0 and in channel order.  The blob's header, its
+// session records and the rows to pack.
+static int export_plan(const dfb_stream *h, const int32_t *slots, int n, BlobHeader *hd, std::vector<BlobSession> *ses,
+                       std::vector<SessionRow> *rows) {
+    if (int rc = sessions_handle(h)) return rc;
+    if (n <= 0 || !slots) return fail(DFB_ERR_INVALID, "bad argument");
+    std::vector<int64_t> s64(slots, slots + n);
+    if (int rc = slot_list_check(h, s64.data(), n)) return rc;
+    for (int i = 0; i < n; i++)
+        if (h->slot_state[(size_t)slots[i]] != kSlotOpen)
+            return fail(DFB_ERR_INVALID, "slot %d is %s: only open sessions are exported", slots[i],
+                        h->slot_state[(size_t)slots[i]] == kSlotFree ? "free" : "closing");
+    size_t off[kStateArrays];
+    StateLayout lay;
+    stream_state_floats(h, off, &lay);
+    *hd = BlobHeader{kBlobMagic, kBlobVersion, h->m->fingerprint, h->st->sr, h->st->fft, h->st->hop, h->st->nb_erb,
+                     eff_gating_mode(h), eff_gating_mode(h) == DFB_GATING_RUNTIME && h->S.rt_valid ? 1 : 0, 0, n, 0, {}};
+    for (int a = 0; a < kStateArrays; a++) hd->row_floats[a] = (int64_t)lay.layers[a] * lay.per_row[a];
+    ses->clear(); rows->clear();
+    int64_t data = 0;   // floats
+    for (int i = 0; i < n;) {
+        const int b = slots[i], g = h->slot_grp[(size_t)b], nch = h->slot_nch[(size_t)b], dir = h->slot_dir[(size_t)b];
+        if (b != g)
+            return fail(DFB_ERR_INVALID, "slot %d is a channel of the group of slot %d: list a group from its channel 0, in channel order", b, g);
+        for (int c = 0; c < nch; c++)
+            if (i + c >= n || h->slot_row[(size_t)slots[i + c]] != h->slot_row[(size_t)g] + c)
+                return fail(DFB_ERR_INVALID, "the group of slot %d: list its %d channels in channel order", g, nch);
+        const size_t sb = (size_t)b;
+        const int64_t first = h->slot_first[sb];
+        BlobSession r{};
+        r.age = h->S.a1 - first;
+        r.lsnr_start = h->lsnr_from >= 0 ? h->lsnr_from - first : kNoLsnr;
+        r.rate = slot_rate_of(h, b); r.channels = nch; r.reduce = nch > 1 ? h->group_reduce : kReduceNone;
+        // the settings the session's next call resolves, pinned: its own, or the handle's at this time
+        r.lim = std::isnan(h->slot_lim[sb]) ? h->lim : h->slot_lim[sb];
+        r.beta = std::isnan(h->slot_beta[sb]) ? default_beta(h->m) : h->slot_beta[sb];
+        const bool own = h->slot_gate[sb] >= 0;
+        r.gate = own ? h->slot_gate[sb] : (h->gating ? 1 : 0);
+        for (int k = 0; k < 3; k++) r.th[k] = own ? h->slot_th[3 * sb + k] : h->th[k];
+        // the last call's settings and the switch to them; without a per-row table (or before its first call) the
+        // session has one setting for all of its frames
+        if (h->ctl_on && !h->slot_fresh[sb]) {
+            const SlotCtl &c = h->slot_ctl[sb];
+            r.last_lim = c.lim; r.last_beta = c.beta; r.prev_lim = c.lim0; r.prev_beta = c.beta0; r.ctl_switch = c.sw - first;
+            r.last_gate = c.gate; r.last_th[0] = c.th_min; r.last_th[1] = c.th_erb; r.last_th[2] = c.th_df;
+        } else {
+            r.last_lim = r.prev_lim = r.lim; r.last_beta = r.prev_beta = r.beta; r.ctl_switch = 0;
+            r.last_gate = r.gate; for (int k = 0; k < 3; k++) r.last_th[k] = r.th[k];
+        }
+        r.up_hist = rs_own(h, dir, true); r.down_hist = rs_own(h, dir, false);
+        r.data_offset = data;   // floats into the data area for now
+        const int64_t per = lay.row_off[kRsArray] + r.up_hist + r.down_hist;
+        for (int c = 0; c < nch; c++, data += per)
+            rows->push_back(SessionRow{data, h->row_src[(size_t)h->slot_row[(size_t)slots[i + c]]], r.up_hist, r.down_hist, 0});
+        ses->push_back(r);
+        i += nch;
+    }
+    hd->n_sessions = (int32_t)ses->size();
+    const int64_t data0 = (int64_t)sizeof(BlobHeader) + (int64_t)sizeof(BlobSession) * (int64_t)ses->size();
+    for (BlobSession &r : *ses) r.data_offset = data0 + r.data_offset * (int64_t)sizeof(float);
+    hd->total_bytes = data0 + data * (int64_t)sizeof(float);
+    return DFB_OK;
+}
+
+static void header_bytes(const BlobHeader &hd, const std::vector<BlobSession> &ses, unsigned char *dst) {
+    memcpy(dst, &hd, sizeof hd);
+    if (!ses.empty()) memcpy(dst + sizeof hd, ses.data(), sizeof(BlobSession) * ses.size());
+}
+
+// A released export frees its slots at once, without a tail: the sessions live only in the blob.
+static void export_release(dfb_stream *h, const int32_t *slots, int n) {
+    for (int i = 0; i < n; i++) slot_release(h, slots[i]);
+    rows_compact(h);
+    h->slot_ops = true;
+}
+
+extern "C" int dfb_stream_session_bytes(const dfb_stream *h, const int32_t *slots, int n, int64_t *bytes) {
+    if (!bytes) return fail(DFB_ERR_INVALID, "bad argument");
+    BlobHeader hd;
+    std::vector<BlobSession> ses;
+    std::vector<SessionRow> rows;
+    if (int rc = export_plan(h, slots, n, &hd, &ses, &rows)) return rc;
+    *bytes = hd.total_bytes;
+    return DFB_OK;
+}
+
+// a device blob: its rows are read and written as floats
+static int blob_pointer(const void *d_blob) {
+    if (!d_blob) return fail(DFB_ERR_INVALID, "bad argument");
+    if ((uintptr_t)d_blob % alignof(float)) return fail(DFB_ERR_INVALID, "a device session blob must be 4-byte aligned");
+    return DFB_OK;
+}
+
+extern "C" int dfb_stream_export_sessions(dfb_stream *h, const int32_t *slots, int n, int release, void *d_blob, void *stream) {
+    BlobHeader hd;
+    std::vector<BlobSession> ses;
+    std::vector<SessionRow> rows;
+    if (int rc = export_plan(h, slots, n, &hd, &ses, &rows)) return rc;
+    if (int rc = blob_pointer(d_blob)) return rc;
+    DFB_CUDA(cudaSetDevice(h->m->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const size_t head = sizeof(BlobHeader) + sizeof(BlobSession) * ses.size();
+    std::vector<unsigned char> hb(head);
+    header_bytes(hd, ses, hb.data());
+    DFB_CUDA(cudaMemcpyAsync(d_blob, hb.data(), head, cudaMemcpyHostToDevice, s));
+    if (int rc = sessions_launch(h, true, rows, (float *)((char *)d_blob + head), s)) return rc;
+    // the pack has read the slab rows (a released session's may be reused by the next call on any stream) and the blob is
+    // complete when this returns; the kernel's row table in the model arena is free again
+    DFB_CUDA(cudaStreamSynchronize(s));
+    if (release) export_release(h, slots, n);
+    return DFB_OK;
+}
+
+extern "C" int dfb_stream_export_sessions_host(dfb_stream *h, const int32_t *slots, int n, int release, void *h_blob) {
+    BlobHeader hd;
+    std::vector<BlobSession> ses;
+    std::vector<SessionRow> rows;
+    if (int rc = export_plan(h, slots, n, &hd, &ses, &rows)) return rc;
+    if (!h_blob) return fail(DFB_ERR_INVALID, "bad argument");
+    DFB_CUDA(cudaSetDevice(h->m->device));
+    const size_t head = sizeof(BlobHeader) + sizeof(BlobSession) * ses.size(), data = (size_t)hd.total_bytes - head;
+    if (int rc = stage_grow(&h->sess_stage, &h->sess_stage_cap, data)) return rc;
+    cudaStream_t s = h->m->stream;
+    if (int rc = sessions_launch(h, true, rows, h->sess_stage, s)) return rc;
+    DFB_CUDA(cudaMemcpyAsync((char *)h_blob + head, h->sess_stage, data, cudaMemcpyDeviceToHost, s));
+    header_bytes(hd, ses, (unsigned char *)h_blob);
+    DFB_CUDA(cudaStreamSynchronize(s));
+    if (release) export_release(h, slots, n);
+    return DFB_OK;
+}
+
+// The header of a blob, checked on its own: magic, version, counts against the n listed slots, and a size that holds its
+// records (read only after this check).
+static int import_header(const BlobHeader &hd, int n) {
+    if (hd.magic != kBlobMagic) return fail(DFB_ERR_INVALID, "not a session blob (magic 0x%08x)", hd.magic);
+    if (hd.version != kBlobVersion) return fail(DFB_ERR_INVALID, "session blob version %u (this library reads %u)", hd.version, kBlobVersion);
+    if (hd.n_sessions < 1 || hd.n_rows < hd.n_sessions || hd.n_rows > 65535)
+        return fail(DFB_ERR_INVALID, "session blob with %d sessions in %d rows", hd.n_sessions, hd.n_rows);
+    if (hd.n_rows != n) return fail(DFB_ERR_INVALID, "the blob holds %d channels: list %d slots, not %d", hd.n_rows, hd.n_rows, n);
+    if (hd.total_bytes < (int64_t)sizeof(BlobHeader) + (int64_t)sizeof(BlobSession) * hd.n_sessions)
+        return fail(DFB_ERR_INVALID, "session blob of %lld bytes: shorter than its %d session records", (long long)hd.total_bytes,
+                    hd.n_sessions);
+    return DFB_OK;
+}
+
+// Everything an import checks before it changes anything, and its plan: per blob row its slot and session, the slab
+// rows it lands in and its table row for the unpack kernel.
+struct ImportPlan {
+    std::vector<int> dir;            // per session: its direction in this handle
+    std::vector<SessionRow> rows;    // per blob row
+    bool idle = false;               // the handle has no live row: its clock settles and it takes the blob's gating tails
+};
+static int import_plan(dfb_stream *h, const int32_t *slots, int n, const BlobHeader &hd, const std::vector<BlobSession> &ses,
+                       ImportPlan *p) {
+    const dfb_model_config &c = h->m->cfg;
+    size_t off[kStateArrays];
+    StateLayout lay;
+    stream_state_floats(h, off, &lay);
+    // the blob's own consistency: its records and size
+    int64_t data = (int64_t)sizeof(BlobHeader) + (int64_t)sizeof(BlobSession) * hd.n_sessions, rows = 0;
+    for (int k = 0; k < kRsArray; k++)
+        if (hd.row_floats[k] != (int64_t)lay.layers[k] * lay.per_row[k])
+            return fail(DFB_ERR_INVALID, "state array %d: the blob's rows hold %lld floats, this handle's %lld", k,
+                        (long long)hd.row_floats[k], (long long)lay.layers[k] * lay.per_row[k]);
+    for (const BlobSession &r : ses) {
+        if (r.channels < 1 || r.up_hist < 0 || r.down_hist < 0 || r.up_hist > 4096 || r.down_hist > 4096 || r.age < 0 ||
+            r.age > kOpenEnd || r.data_offset != data)
+            return fail(DFB_ERR_INVALID, "session blob: a malformed session record");
+        data += (int64_t)r.channels * (lay.row_off[kRsArray] + r.up_hist + r.down_hist) * (int64_t)sizeof(float);
+        rows += r.channels;
+    }
+    if (rows != hd.n_rows || data != hd.total_bytes)
+        return fail(DFB_ERR_INVALID, "session blob: its records describe %lld bytes in %lld rows, its header %lld in %d",
+                    (long long)data, (long long)rows, (long long)hd.total_bytes, hd.n_rows);
+    // compatibility with this handle
+    if (hd.fingerprint != h->m->fingerprint)
+        return fail(DFB_ERR_INVALID, "the sessions ran another model (fingerprint %016llx, this handle's model %016llx)",
+                    (unsigned long long)hd.fingerprint, (unsigned long long)h->m->fingerprint);
+    if (hd.sr != h->st->sr || hd.fft_size != h->st->fft || hd.hop_size != h->st->hop || hd.nb_erb != h->st->nb_erb)
+        return fail(DFB_ERR_INVALID, "the sessions ran another DSP state (sr %d, fft %d, hop %d, %d ERB bands; this handle's: %d, %d, %d, %d)",
+                    hd.sr, hd.fft_size, hd.hop_size, hd.nb_erb, h->st->sr, h->st->fft, h->st->hop, h->st->nb_erb);
+    if (hd.gating_mode != eff_gating_mode(h))
+        return fail(DFB_ERR_INVALID, "the sessions ran in gating mode %d, this handle runs %d", hd.gating_mode, eff_gating_mode(h));
+    std::vector<int64_t> s64(slots, slots + n);
+    if (int rc = slot_list_check(h, s64.data(), n)) return rc;
+    for (int i = 0; i < n; i++)
+        if (h->slot_state[(size_t)slots[i]] != kSlotFree) return fail(DFB_ERR_INVALID, "slot %d is not free", slots[i]);
+    p->idle = h->n_act == 0;
+    if (!p->idle && !clock_settled(h))
+        return fail(DFB_ERR_INVALID, "this handle's clock has not settled since its start or flush: it settles after %d frames "
+                    "of calls (8 of halo, %d of look-ahead); import into it then, or into a handle with no live session",
+                    kHalo + chunk_geom(c).Lmax, chunk_geom(c).Lmax);
+    if (!p->idle && hd.gating_mode == DFB_GATING_RUNTIME && (hd.gate_tails != 0) != h->S.rt_valid)
+        return fail(DFB_ERR_INVALID, "runtime gating: the sessions' decoder tails %s kept by their last call, this handle's live "
+                    "sessions' %s: import into a handle whose last call gated %s, or into one with no live session",
+                    hd.gate_tails ? "were" : "were not", h->S.rt_valid ? "were" : "were not", hd.gate_tails ? "too" : "nothing either");
+    const bool ctl = ctl_shape(c);
+    p->dir.clear();
+    for (const BlobSession &r : ses) {
+        int dir = -1;
+        if (mixed_rate(h)) {
+            for (size_t k = 0; k < h->rs_rates.size(); k++)
+                if (h->rs_rates[k] == r.rate) dir = (int)k;
+        } else if (r.rate == (h->rate ? h->rate : kModelRate)) {
+            dir = 0;
+        }
+        if (dir < 0) {
+            std::string runs = mixed_rate(h) ? "" : std::to_string(h->rate ? h->rate : kModelRate);
+            for (int rr : mixed_rate(h) ? h->rs_rates : std::vector<int>{}) runs += (runs.empty() ? "" : ", ") + std::to_string(rr);
+            return fail(DFB_ERR_INVALID, "a session at %d Hz: this handle runs %s", r.rate, runs.c_str());
+        }
+        if (r.up_hist != rs_own(h, dir, true) || r.down_hist != rs_own(h, dir, false))
+            return fail(DFB_ERR_INVALID, "a session at %d Hz with resampler histories of %d / %d samples: this handle's are %d / %d",
+                        r.rate, r.up_hist, r.down_hist, rs_own(h, dir, true), rs_own(h, dir, false));
+        if (r.channels > 1 && r.reduce != h->group_reduce)
+            return fail(DFB_ERR_INVALID, "a group of %d channels with mask reduction %d: this handle's groups reduce by %d",
+                        r.channels, r.reduce, h->group_reduce);
+        if (!ctl && (r.lim != h->lim || r.beta != default_beta(h->m) || r.gate != (h->gating ? 1 : 0) ||
+                     (r.gate && memcmp(r.th, h->th, sizeof r.th))))
+            return fail(DFB_ERR_UNSUPPORTED, "per-session settings are built for df_order 5, nb_df 96 and 32 ERB bands: the "
+                        "sessions' settings differ from this handle's");
+        p->dir.push_back(dir);
+    }
+    // slab rows: a new row lands in its own slab row unless a pending move still reads that one
+    std::vector<char> used((size_t)h->B, 0);
+    for (int r = 0; r < h->n_act; r++)
+        if (h->row_src[(size_t)r] >= 0) used[(size_t)h->row_src[(size_t)r]] = 1;
+    const ChunkGeom g = chunk_geom(c);
+    p->rows.clear();
+    int next = 0;
+    int64_t boff = 0;
+    for (const BlobSession &r : ses) {
+        // DeepFilterNet2's output trails its DNN: the LSNR tail's frames [d1 - kMcTail, d1) may still be output, and the
+        // ones before the session's LSNR start have none
+        int nan_l = 0;
+        if (g.lag > 0) {
+            const int64_t t0 = r.age - g.Lmax - kMcTail;   // the session's frame of tail entry 0
+            nan_l = r.lsnr_start == kNoLsnr ? kMcTail : (int)std::min<int64_t>(kMcTail, std::max<int64_t>(0, r.lsnr_start - t0));
+        }
+        for (int ch = 0; ch < r.channels; ch++) {
+            const int row = h->n_act + (int)p->rows.size();
+            int q = row;
+            if (used[(size_t)q]) {
+                while (used[(size_t)next]) next++;
+                q = next;
+            }
+            used[(size_t)q] = 1;
+            p->rows.push_back(SessionRow{boff, q, r.up_hist, r.down_hist, nan_l});
+            boff += lay.row_off[kRsArray] + r.up_hist + r.down_hist;
+        }
+    }
+    return ctl ? ctl_enable(h) : DFB_OK;   // the sessions' own settings go to the per-row table (it changes no output)
+}
+
+// The blob's sessions in the listed slots, as the source left them: rebased onto this handle's clock, settings pinned.
+static void import_slots(dfb_stream *h, const int32_t *slots, const BlobHeader &hd, const std::vector<BlobSession> &ses,
+                         const ImportPlan &p) {
+    if (p.idle) {
+        clock_settle(h);
+        h->S.rt_valid = hd.gate_tails != 0;
+    }
+    const bool ctl = h->ctl_on;
+    int i = 0;
+    for (size_t k = 0; k < ses.size(); k++) {
+        const BlobSession &r = ses[k];
+        const int64_t first = h->S.a1 - r.age;
+        if (p.idle && r.lsnr_start != kNoLsnr) h->lsnr_from = std::max<int64_t>(0, std::min(h->S.d1, first + r.lsnr_start));
+        for (int ch = 0; ch < r.channels; ch++, i++) {
+            const size_t b = (size_t)slots[i];
+            const int row = h->n_act++;
+            h->slot_row[b] = row;
+            h->row_slot[(size_t)row] = (int)b;
+            h->row_src[(size_t)row] = p.rows[(size_t)i].slab;
+            h->slot_grp[b] = slots[i - ch];
+            h->slot_nch[b] = r.channels;
+            h->slot_state[b] = kSlotOpen;
+            h->slot_first[b] = first;
+            h->slot_end[b] = kOpenEnd;
+            h->slot_dir[b] = p.dir[k];
+            if (ctl) {
+                h->slot_lim[b] = r.lim; h->slot_beta[b] = r.beta;
+                h->slot_gate[b] = (signed char)(r.gate ? 1 : 0);
+                for (int j = 0; j < 3; j++) h->slot_th[3 * b + j] = r.th[j];
+                h->slot_fresh[b] = 0;
+                h->slot_ctl[b] = SlotCtl{r.last_lim, r.last_beta, r.prev_lim, r.prev_beta, first + r.ctl_switch, r.last_th[0],
+                                         r.last_th[1], r.last_th[2], r.last_gate};
+            } else {   // the handle's settings, which the plan found equal to the session's
+                h->slot_lim[b] = h->slot_beta[b] = NAN;
+                h->slot_gate[b] = -1;
+                h->slot_fresh[b] = 1;
+            }
+        }
+    }
+    // clock_settle moves d1 back to a1 - Lmax on a handle that was flushed (a flush leaves d1 = a1), and an LSNR request
+    // after the flush set lsnr_from to that d1: the LSNR head must start no later than the imported sessions' next frame
+    if (p.idle && ses.size() && ses[0].lsnr_start == kNoLsnr && h->lsnr_from > h->S.d1) h->lsnr_from = h->S.d1;
+    h->tab_dirty = true;
+    h->slot_ops = true;
+}
+
+// the header and session records of a host blob
+static int host_records(const void *h_blob, int n, BlobHeader *hd, std::vector<BlobSession> *ses) {
+    if (!h_blob) return fail(DFB_ERR_INVALID, "bad argument");
+    memcpy(hd, h_blob, sizeof *hd);
+    if (int rc = import_header(*hd, n)) return rc;
+    ses->resize((size_t)hd->n_sessions);
+    memcpy(ses->data(), (const char *)h_blob + sizeof *hd, sizeof(BlobSession) * ses->size());
+    return DFB_OK;
+}
+
+extern "C" int dfb_stream_import_sessions(dfb_stream *h, const int32_t *slots, int n, const void *d_blob, void *stream) {
+    if (int rc = sessions_handle(h)) return rc;
+    if (n <= 0 || !slots) return fail(DFB_ERR_INVALID, "bad argument");
+    if (int rc = blob_pointer(d_blob)) return rc;
+    DFB_CUDA(cudaSetDevice(h->m->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    // the header first; its records only once the header says the blob holds them
+    BlobHeader hd;
+    DFB_CUDA(cudaMemcpyAsync(&hd, d_blob, sizeof hd, cudaMemcpyDeviceToHost, s));
+    DFB_CUDA(cudaStreamSynchronize(s));
+    if (int rc = import_header(hd, n)) return rc;
+    std::vector<BlobSession> ses((size_t)hd.n_sessions);
+    DFB_CUDA(cudaMemcpyAsync(ses.data(), (const char *)d_blob + sizeof hd, sizeof(BlobSession) * ses.size(), cudaMemcpyDeviceToHost, s));
+    DFB_CUDA(cudaStreamSynchronize(s));
+    ImportPlan p;
+    if (int rc = import_plan(h, slots, n, hd, ses, &p)) return rc;
+    const size_t head = sizeof(BlobHeader) + sizeof(BlobSession) * ses.size();
+    if (int rc = sessions_launch(h, false, p.rows, (float *)((const char *)d_blob + head), s)) return rc;
+    // the rows are in place, and the kernel's row table in the model arena is free again, before the handle's next call
+    // on any stream
+    DFB_CUDA(cudaStreamSynchronize(s));
+    import_slots(h, slots, hd, ses, p);
+    return DFB_OK;
+}
+
+extern "C" int dfb_stream_import_sessions_host(dfb_stream *h, const int32_t *slots, int n, const void *h_blob) {
+    if (int rc = sessions_handle(h)) return rc;
+    if (n <= 0 || !slots) return fail(DFB_ERR_INVALID, "bad argument");
+    BlobHeader hd;
+    std::vector<BlobSession> ses;
+    if (int rc = host_records(h_blob, n, &hd, &ses)) return rc;
+    DFB_CUDA(cudaSetDevice(h->m->device));
+    ImportPlan p;
+    if (int rc = import_plan(h, slots, n, hd, ses, &p)) return rc;
+    const size_t head = sizeof(BlobHeader) + sizeof(BlobSession) * ses.size(), data = (size_t)hd.total_bytes - head;
+    if (int rc = stage_grow(&h->sess_stage, &h->sess_stage_cap, data)) return rc;
+    cudaStream_t s = h->m->stream;
+    DFB_CUDA(cudaMemcpyAsync(h->sess_stage, (const char *)h_blob + head, data, cudaMemcpyHostToDevice, s));
+    if (int rc = sessions_launch(h, false, p.rows, h->sess_stage, s)) return rc;
+    DFB_CUDA(cudaStreamSynchronize(s));
+    import_slots(h, slots, hd, ses, p);
+    return DFB_OK;
 }
 
 // ---- spectral handle (dfb_stream_create_spec): capi.rs df_process_frame_raw, batched and for n_frames frames at once.

@@ -46,6 +46,13 @@ different rates share one pass through the slot path.  Rows stay 480 samples per
     s.open([3, 9], sr=16000)
     s.open([7])                          # 48 kHz
     out = s.process(chunk)               # chunk: float32 [256, n * 480]
+
+``export`` takes live sessions out of a handle as one ``uint8`` blob and ``resume`` continues them in free slots of any
+compatible handle -- another one, in another process or on another GPU -- with the outputs the source would have given
+next (dfb_stream_export_sessions in include/dfb200.h; ``session_info`` reads a blob's header)::
+
+    blob = s.export([3, 9], release=True)        # the sessions leave s
+    d.resume(blob, [0, 1])                       # and continue in slots 0 and 1 of d
 """
 from __future__ import annotations
 
@@ -154,6 +161,110 @@ def pf_beta_arg(beta: float) -> float:
     if not math.isfinite(v) or v < 0:
         raise ValueError(f"post-filter beta must be finite and >= 0, got {beta}")
     return v
+
+
+BLOB_MAGIC, BLOB_VERSION = 0x53424644, 1
+_BLOB_HEADER = np.dtype([("magic", "<u4"), ("version", "<u4"), ("fingerprint", "<u8"), ("sr", "<i4"), ("fft_size", "<i4"),
+                         ("hop_size", "<i4"), ("nb_erb", "<i4"), ("gating_mode", "<i4"), ("gate_tails", "<i4"),
+                         ("n_sessions", "<i4"), ("n_rows", "<i4"), ("total_bytes", "<i8"), ("row_floats", "<i8", (17,))])
+_BLOB_SESSION = np.dtype([("age", "<i8"), ("lsnr_start", "<i8"), ("ctl_switch", "<i8"), ("rate", "<i4"), ("channels", "<i4"),
+                          ("reduce", "<i4"), ("reserved", "<i4"), ("lim", "<f4"), ("beta", "<f4"), ("gate", "<i4"),
+                          ("th", "<f4", (3,)), ("last_lim", "<f4"), ("last_beta", "<f4"), ("prev_lim", "<f4"),
+                          ("prev_beta", "<f4"), ("last_gate", "<i4"), ("last_th", "<f4", (3,)), ("up_hist", "<i4"),
+                          ("down_hist", "<i4"), ("data_offset", "<i8")])
+assert _BLOB_HEADER.itemsize == 192 and _BLOB_SESSION.itemsize == 112
+_NO_LSNR = np.iinfo(np.int64).min
+_REDUCE_NAMES = {0: None, 1: "max", 2: "mean"}
+
+
+class SessionInfo(NamedTuple):
+    """One session of a blob: its age in hops since it opened, its rate, its channels (a linked group when > 1) and their
+    mask reduction, the settings it resumes with (attenuation limit as a linear factor, 0 = off; post-filter beta; LSNR
+    gating and its thresholds) and the frame its LSNR output starts at, relative to its frame 0 (None: never asked for)."""
+    age: int
+    sr: int
+    channels: int
+    reduce_mask: Optional[str]
+    atten_lim: float
+    post_filter_beta: float
+    lsnr_gating: bool
+    thresholds: tuple
+    lsnr_start: Optional[int]
+
+
+class BlobInfo(NamedTuple):
+    """The header of a session blob (DfStream.export): the model fingerprint, the DSP state's sr / fft_size / hop_size /
+    nb_erb, the gating mode ("apply" / "runtime"), its size in bytes and its sessions in blob order."""
+    fingerprint: int
+    sr: int
+    fft_size: int
+    hop_size: int
+    nb_erb: int
+    gating_mode: str
+    nbytes: int
+    sessions: tuple
+
+    @property
+    def rows(self) -> int:
+        """the slots the blob resumes in: one per channel"""
+        return sum(x.channels for x in self.sessions)
+
+
+def blob_arg(blob) -> Tensor:
+    """``blob`` of DfStream.resume / session_info: a flat uint8 tensor (CPU or CUDA), else ValueError.  A view that does
+    not start on a 16-byte boundary (a slice of blobs stored back to back) is copied: the library reads the rows as
+    floats."""
+    if not isinstance(blob, Tensor) or blob.dtype != torch.uint8 or blob.dim() != 1:
+        raise ValueError(f"a session blob is a flat uint8 tensor, got {getattr(blob, 'dtype', type(blob).__name__)}")
+    blob = blob.contiguous()
+    return blob.clone() if blob.data_ptr() % 16 else blob
+
+
+def _blob_error(msg):
+    return DfbError(DFB_ERR_INVALID, f"session blob: {msg}")
+
+
+def blob_header(blob: Tensor):
+    """The checked header of a blob_arg: DfbError (DFB_ERR_INVALID) for a bad magic number or version, or a size other
+    than the header's."""
+    if blob.numel() < _BLOB_HEADER.itemsize:
+        raise _blob_error(f"{blob.numel()} bytes, shorter than its header")
+    head = blob[:_BLOB_HEADER.itemsize].cpu().numpy().view(_BLOB_HEADER)[0]
+    if int(head["magic"]) != BLOB_MAGIC:
+        raise _blob_error(f"magic 0x{int(head['magic']):08x}")
+    if int(head["version"]) != BLOB_VERSION:
+        raise _blob_error(f"version {int(head['version'])} (this library reads {BLOB_VERSION})")
+    ns, total = int(head["n_sessions"]), int(head["total_bytes"])
+    if ns < 1 or total != blob.numel():
+        raise _blob_error(f"{blob.numel()} bytes, its header says {total} in {ns} sessions")
+    return head
+
+
+def session_info(blob) -> BlobInfo:
+    """Parses a blob's header on the host (include/dfb200.h, dfb_stream_export_sessions).  DfbError (DFB_ERR_INVALID, as the
+    C ABI refuses it) for a blob that is not one: a bad magic number or version, a truncated blob or one whose size is not
+    what its header says."""
+    blob = blob_arg(blob)
+    head = blob_header(blob)
+    ns, total = int(head["n_sessions"]), int(head["total_bytes"])
+    bad = _blob_error
+    end = _BLOB_HEADER.itemsize + ns * _BLOB_SESSION.itemsize
+    if end > total:
+        raise bad(f"{ns} session records do not fit in {total} bytes")
+    recs = blob[_BLOB_HEADER.itemsize:end].cpu().numpy().view(_BLOB_SESSION)
+    sessions = []
+    for r in recs:
+        red = int(r["reduce"])
+        if int(r["channels"]) < 1 or red not in _REDUCE_NAMES:
+            raise bad("a malformed session record")
+        ls = int(r["lsnr_start"])
+        sessions.append(SessionInfo(int(r["age"]), int(r["rate"]), int(r["channels"]), _REDUCE_NAMES[red], float(r["lim"]),
+                                    float(r["beta"]), bool(r["gate"]), tuple(float(v) for v in r["th"]),
+                                    None if ls == _NO_LSNR else ls))
+    if sum(x.channels for x in sessions) != int(head["n_rows"]):
+        raise bad(f"its sessions hold {sum(x.channels for x in sessions)} channels, its header says {int(head['n_rows'])}")
+    return BlobInfo(int(head["fingerprint"]), int(head["sr"]), int(head["fft_size"]), int(head["hop_size"]), int(head["nb_erb"]),
+                    "runtime" if int(head["gating_mode"]) == 1 else "apply", total, tuple(sessions))
 
 
 class SpecFrames(NamedTuple):
@@ -397,6 +508,58 @@ class DfStream:
         out = np.zeros(self.batch, np.int64)
         check(_lib.lib().dfb_stream_slot_groups(self._h, out.ctypes.data_as(C.POINTER(C.c_int64))))
         return out
+
+    def export(self, slots, release: bool = False, device=None) -> Tensor:
+        """The sessions of the listed open slots as one uint8 blob, on the handle's device (``device`` None or that CUDA
+        device) or on the host (``device="cpu"``).  A linked group is listed whole, from its channel 0 in channel order.
+        ``release=False``: a snapshot, the sessions and their neighbours continue unchanged.  ``release=True``: the slots
+        are free at once, without a look-ahead tail; the sessions live on in the blob, for ``resume`` on this or another
+        handle (dfb_stream_export_sessions).  ValueError for a malformed slot list; DfbError for a free or closing slot,
+        part of a group, a spectral handle."""
+        a = np.ascontiguousarray(group_list(slots, self.batch), dtype=np.int32)
+        ptr = a.ctypes.data_as(C.POINTER(C.c_int32))
+        nbytes = C.c_int64()
+        check(_lib.lib().dfb_stream_session_bytes(self._h, ptr, a.size, C.byref(nbytes)))
+        dev = torch.device(device) if device is not None else self.model.cuda_device
+        if dev.type == "cpu":   # page-locked: the one device-to-host copy runs at full speed
+            out = torch.empty(nbytes.value, dtype=torch.uint8, pin_memory=True)
+            self._finish_device_calls()
+            check(_lib.lib().dfb_stream_export_sessions_host(self._h, ptr, a.size, int(bool(release)), out.data_ptr()))
+            return out
+        if dev.type != "cuda" or (dev.index is not None and dev != self.model.cuda_device):
+            raise ValueError(f"a blob goes to the handle's device {self.model.cuda_device} or to the cpu, not {dev}")
+        out = torch.empty(nbytes.value, dtype=torch.uint8, device=self.model.cuda_device)
+        with torch.cuda.device(out.device):
+            check(_lib.lib().dfb_stream_export_sessions(self._h, ptr, a.size, int(bool(release)), out.data_ptr(),
+                                                        torch.cuda.current_stream(out.device).cuda_stream))
+        return out
+
+    def _finish_device_calls(self) -> None:
+        """The _host session entry points run on the handle's own stream: let this handle's calls with CUDA tensors, on
+        torch's current stream, finish first (the device-pointer entry points run on that stream and synchronise it)."""
+        torch.cuda.current_stream(self.model.cuda_device).synchronize()
+
+    def resume(self, blob, slots) -> None:
+        """Continue the sessions of ``blob`` (``export``'s, a CPU or CUDA uint8 tensor) in the listed free slots, one per
+        channel in blob order; a group lands as a linked group.  The next ``process`` / ``flush`` calls return what the
+        source would have returned next, and ``close`` / ``flush`` end them as any session.  Their settings come with them.
+        ValueError for a malformed slot list or blob argument; DfbError (DFB_ERR_INVALID) for a blob that is not one, for
+        another model, DSP state or gating mode, a rate or group reduction this handle does not run, a slot that is not
+        free (dfb_stream_import_sessions)."""
+        blob = blob_arg(blob)
+        a = np.ascontiguousarray(group_list(slots, self.batch), dtype=np.int32)
+        rows = int(blob_header(blob)["n_rows"])   # (the library checks the session records)
+        if a.size != rows:
+            raise ValueError(f"the blob holds {rows} channels: list {rows} slots, not {a.size}")
+        ptr = a.ctypes.data_as(C.POINTER(C.c_int32))
+        if not blob.is_cuda:
+            self._finish_device_calls()
+            check(_lib.lib().dfb_stream_import_sessions_host(self._h, ptr, a.size, blob.data_ptr()))
+            return
+        blob = blob.to(self.model.cuda_device)
+        with torch.cuda.device(blob.device):
+            check(_lib.lib().dfb_stream_import_sessions(self._h, ptr, a.size, blob.data_ptr(),
+                                                        torch.cuda.current_stream(blob.device).cuda_stream))
 
     @torch.no_grad()
     def process(self, audio: Tensor, return_lsnr: bool = False):

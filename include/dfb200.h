@@ -557,6 +557,66 @@ int dfb_stream_slot_rates(const dfb_stream *s, int32_t *h_rates);
 int dfb_debug_resample_slots(int up, const dfb_stream *s, const int32_t *h_rates, const float *d_in, int64_t C,
                              const int64_t *h_calls, int64_t n_calls, float *d_out, void *stream);
 
+/* Session export / import (DESIGN.md section 5o): take live sessions out of an audio handle as one blob and resume them in
+ * free slots of any compatible handle -- the same one, another one with other neighbours, batch size and clock, one in
+ * another process or on another GPU.  A resumed session's next process / flush calls return exactly the hops the source
+ * would have returned next, bit for bit for the same neighbour counts (the kernels' fp32 reduction order can follow the
+ * number of live rows, as for every session of a slot handle), then it closes and drains as any session does.
+ *
+ * `slots` is a HOST array of n slot indices (each in [0, B), listed once).  Export lists open sessions only (a free or
+ * closing slot is DFB_ERR_INVALID), each linked group whole, from its channel 0 and in channel order (else
+ * DFB_ERR_INVALID).  Import lists n free slots (else DFB_ERR_INVALID), one per channel of the blob in blob order; a group
+ * lands as a linked group.  A refused call changes nothing.  Spectral handles: DFB_ERR_UNSUPPORTED (DeepFilterNet v1 has
+ * no streaming handle).
+ *   dfb_stream_session_bytes      the blob's size in bytes for these sessions (checks `slots` as export does).
+ *   dfb_stream_export_sessions    packs the sessions into d_blob (device, 4-byte aligned, >= session_bytes) on `stream`
+ *                                 and synchronises it: the blob is complete when the call returns.
+ *                                 release = 0: a snapshot, the sessions and every other slot continue unchanged, bit for
+ *                                 bit.  release != 0: the slots are free at once, without a look-ahead tail: the sessions
+ *                                 now live only in the blob.  One kernel launch, whatever the number of sessions.
+ *   dfb_stream_import_sessions    resumes the blob at d_blob (device, 4-byte aligned, the whole blob) in free slots of
+ *                                 this handle: reads the header, then its records, then one kernel launch, each on
+ *                                 `stream`, which it synchronises before returning.  The blob may come from another
+ *                                 device: copy it to this handle's first.
+ *   _host variants                the blob in host memory: one device copy of the rows per call, on the handle's own
+ *                                 stream, synchronised, as dfb_stream_process_host.
+ * Every variant returns with its device work done, so the handle's next call may run on any stream.  Work of earlier
+ * calls on another stream than the export's / import's must have finished first (synchronise that stream), as for the
+ * handle's other calls.
+ * Import refuses with DFB_ERR_INVALID, naming the mismatch: another model (fingerprint of dfb_model_create's config, ERB
+ * band widths and weight bytes) or DSP state; another gating mode (dfb_stream_set_gating_mode / the model's); a session rate this handle
+ * does not run (its rate on a handle at one rate, 48000 and its registered rates on a mixed-rate one); a group whose mask
+ * reduction is not the handle's (dfb_stream_set_mask_reduce); a bad magic or version, a size too small for its records,
+ * records that do not describe the header's size, or a device blob that is not 4-byte aligned; and, on a handle with live sessions, a clock that has not settled (fewer than 8 + look-ahead
+ * frames since its creation, reset or flush) or, in DFB_GATING_RUNTIME, decoder tails kept by the blob's last call where
+ * this handle's last call kept none or the reverse.  A handle with no live session takes any blob: its clock moves ahead
+ * to where it has settled, as calls with no live slot would move it.
+ * What travels: each session's age (frames since its open), rate, group, its settings pinned (the limit, post-filter beta
+ * and LSNR gating its next call would resolve, own or the source handle's; the destination's defaults do not reach it;
+ * change them with the per-slot setters) with the previous call's settings and switch frame, and the frame its LSNR
+ * output starts at.  LSNR rows of DeepFilterNet2 (whose audio trails its DNN by df_lookahead frames): the first LSNR call
+ * after an import where exactly one of the two handles had computed LSNR before may differ from the source's in its
+ * first df_lookahead hops (NaN for a value or the reverse); every other LSNR value, and the audio, is exact.
+ *
+ * Blob layout (little-endian, version 1): a header of 192 bytes, n_sessions records of 112 bytes, then the rows.
+ *   header   0 u32 magic 0x53424644 ("DFBS")  4 u32 version  8 u64 model fingerprint
+ *           16 i32 sr, fft_size, hop_size, nb_erb (the DSP state)  32 i32 gating mode (0 apply, 1 runtime)
+ *           36 i32 gate tails (runtime gating: the decoder tails were kept by the last call)  40 i32 n_sessions
+ *           44 i32 n_rows (channels)  48 i64 total bytes  56 i64 floats per row of each of the 17 state arrays
+ *           (arrays 15 / 16, the resampler histories: the source handle's width)
+ *   session  0 i64 age  8 i64 LSNR start frame relative to the session's frame 0 (INT64_MIN: none)  16 i64 switch frame
+ *           of the last call's settings (relative)  24 i32 rate  28 i32 channels  32 i32 mask reduction  36 i32 0
+ *           40 f32 atten limit (linear, 0 off)  44 f32 beta  48 i32 gate  52 f32 thresholds[3] (min, max erb, max df)
+ *           64 f32 last call's limit, beta, previous limit, previous beta  80 i32 last gate  84 f32 last thresholds[3]
+ *           96 i32 own up / 100 down resampler history floats  104 i64 byte offset of its rows
+ *   rows     per channel: arrays 0 .. 14 (layer-major, as many floats as the header says), then its own up and down
+ *           histories (an import pads them with zeros to the handle's width). */
+int dfb_stream_session_bytes(const dfb_stream *s, const int32_t *slots, int n, int64_t *bytes);
+int dfb_stream_export_sessions(dfb_stream *s, const int32_t *slots, int n, int release, void *d_blob, void *stream);
+int dfb_stream_export_sessions_host(dfb_stream *s, const int32_t *slots, int n, int release, void *h_blob);
+int dfb_stream_import_sessions(dfb_stream *s, const int32_t *slots, int n, const void *d_blob, void *stream);
+int dfb_stream_import_sessions_host(dfb_stream *s, const int32_t *slots, int n, const void *h_blob);
+
 /* Spectral streaming handle (capi.rs df_process_frame_raw, DfTract::process_raw, tract.rs:441-506): the caller runs its own
  * filter bank, passes spectrum frames in and gets the network's outputs back -- ERB gains, deep-filter coefficients, LSNR
  * and the stage LSNR gating picks -- with the features' normalisation, the GRU, conv and norm states carried between
