@@ -109,6 +109,9 @@ SIGNATURES = {
     "dfb_stream_open_slots": (_I, [_VP, _I64P, _I64]),
     "dfb_stream_close_slots": (_I, [_VP, _I64P, _I64]),
     "dfb_stream_slot_states": (_I, [_VP, C.POINTER(C.c_int32)]),
+    "dfb_stream_hold_slots": (_I, [_VP, _I64P, _I64, _I]),
+    "dfb_stream_held_slots": (_I, [_VP, C.POINTER(C.c_int8)]),
+    "dfb_debug_stream_rows_moved": (_I, [_VP, _I64P]),
     "dfb_stream_open_linked": (_I, [_VP, _I64P, _I64]),
     "dfb_stream_slot_groups": (_I, [_VP, _I64P]),
     "dfb_stream_set_atten_lim": (_I, [_VP, _I64P, _I64, _F]),

@@ -1019,6 +1019,7 @@ struct GateRun {
     float *t_c0, *t_run;           // StreamState tails
     bool valid;                    // the tails hold the last DNN chunk's run frames; else it ran in apply mode, where every
                                    // frame ran: take them from the halo (frames before the window or a stream's start: zero)
+    const unsigned char *halo;     // per row: 1 takes that row's tails from the halo, 0 from the tails; or null: !valid for all
 };
 
 struct GatePlan {
@@ -1032,6 +1033,7 @@ struct GatePlan {
     // the decoder has run, else its first run frame, so that the frames before it are padding, as tract's zero state is
     float *has_run; int run_w, from_halo;
     int64_t *erb_first;
+    const unsigned char *halo;         // per-row from_halo (GateRun::halo), or null: from_halo for every row
 };
 
 // one CTA per row: flags in parallel over frame segments, then an exclusive scan of the segments' last ERB run frame and
@@ -1082,7 +1084,7 @@ __global__ void __launch_bounds__(256) k_gate_plan(GatePlan g) {
     if (g.has_run && tid == 0) {
         float &h = g.has_run[(int64_t)b * g.run_w];
         const int64_t f0 = g.first ? g.first[b] : 0;
-        const bool prev = g.from_halo ? g.Rc > 0 && g.w0 + g.Rc - 1 >= f0 : h != 0.f;
+        const bool prev = (g.halo ? g.halo[b] : g.from_halo) ? g.Rc > 0 && g.w0 + g.Rc - 1 >= f0 : h != 0.f;
         g.erb_first[b] = prev ? f0 : g.w0 + s_first;
         h = prev || s_first < T ? 1.f : 0.f;
     }
@@ -1097,12 +1099,14 @@ __global__ void __launch_bounds__(256) k_gate_plan(GatePlan g) {
 }
 
 // DF pathway input of the run frames, compacted: row b of P [B][Tp][W] is the c0 of its last K - 1 run frames before the
-// window's new frames (the carried tail, or the halo), then c0 of its DF run frames among them.  grid (K - 1 + T - Rc, B)
+// window's new frames (the carried tail, or the halo: from_halo, or per row halo[b]), then c0 of its DF run frames among
+// them.  grid (K - 1 + T - Rc, B)
 __global__ void __launch_bounds__(256) k_gate_gather(const float *__restrict__ c0, const float *__restrict__ tail, float *__restrict__ P,
                                                      int T, int Rc, int K, int W, int Tp, const unsigned char *__restrict__ df_run,
-                                                     const int *__restrict__ df_pos, int from_halo, const int64_t *__restrict__ first,
-                                                     int64_t w0) {
+                                                     const int *__restrict__ df_pos, int from_halo, const unsigned char *__restrict__ halo,
+                                                     const int64_t *__restrict__ first, int64_t w0) {
     const int b = blockIdx.y, x = blockIdx.x;
+    if (halo) from_halo = halo[b];
     const float4 *src = nullptr;
     int64_t dst;
     if (x < K - 1) {
@@ -1144,13 +1148,14 @@ __global__ void __launch_bounds__(256) k_gate_tail(const float *__restrict__ P, 
 
 // (conv_kt == 2) the frames before a run frame, as the kt = 2 layers read them, are the ERB decoder's last run frame: fill
 // rows [Rc - 1, T) of x [B][T][fs] (W values per frame) that are not run frames from the last run frame before them, or from
-// the carried one (tail + off; from_halo: row Rc - 1 as recomputed, zeros at a stream's start).  save: afterwards, copy row
-// T - 1 to the carried one.  grid (T - Rc + 1, B)
+// the carried one (tail + off; from_halo, or per row halo[b]: row Rc - 1 as recomputed, zeros at a stream's start).  save:
+// afterwards, copy row T - 1 to the carried one.  grid (T - Rc + 1, B)
 struct FillSeg { float *x; int64_t fs; int W, off; };
 __global__ void __launch_bounds__(256) k_gate_fill(FillSeg sg, float *__restrict__ tail, int tail_w, int T, int Rc,
                                                    const unsigned char *__restrict__ erb_run, const int *__restrict__ erb_src,
-                                                   int from_halo, int save) {
+                                                   int from_halo, const unsigned char *__restrict__ halo, int save) {
     const int b = blockIdx.y;
+    if (halo) from_halo = halo[b];
     float *trow = tail + (int64_t)b * tail_w + sg.off;
     float *xb = sg.x + (int64_t)b * T * sg.fs;
     if (save) {
@@ -1455,7 +1460,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         m->dbg["erb_gru_hi"] = {word(f.gb_hi), M * H / 2}; m->dbg["erb_gru_lo"] = {word(f.gb_lo), M * H / 2};
         GatePlan gp{d_lsnr, gate->ctl, gate->links, first, W0, {gate->th[0], gate->th[1], gate->th[2]}, gate->gate_all, T, Rc,
                     erb_run, df_run, erb_src, df_pos, df_n, c.conv_kt > 1 ? gate->t_run + tw_run - 1 : nullptr, tw_run,
-                    gate->valid ? 0 : 1, erb_first};
+                    gate->valid ? 0 : 1, erb_first, gate->halo};
         kt_first = erb_first;
         {
             dfb::ProfScope prof_scope__("k_gate_plan", s);   // (not on the enhancement path bench.py models: see launch_spec_ingest)
@@ -1472,7 +1477,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         {
             dfb::ProfScope prof_scope__("k_gate_gather", sl);   // (see k_gate_plan)
             k_gate_gather<<<dim3((unsigned)(Tp), (unsigned)B), 256, 0, sl>>>(f.c0, gate->t_c0, gP, T, Rc, Kp, Wc, Tp, df_run, df_pos,
-                                                                           gate->valid ? 0 : 1, first, W0);
+                                                                           gate->valid ? 0 : 1, gate->halo, first, W0);
             DFB_LAUNCH_CHECK();
             if (Kp > 1) {
                 k_gate_tail<<<dim3((unsigned)(Kp - 1), (unsigned)B), 256, 0, sl>>>(gP, gate->t_c0, Kp, Wc, Tp, df_n);
@@ -1557,7 +1562,7 @@ static int forward_body(dfb_model *m, Arena &arena, const float *d_feat_erb, con
         auto fill = [&](FillSeg sg, int save) -> int {
             dfb::ProfScope prof_scope__("k_gate_fill", s);   // (see k_gate_plan)
             k_gate_fill<<<dim3((unsigned)(save ? 1 : T - Rc + 1), (unsigned)B), 256, 0, s>>>(sg, gate->t_run, tw_run, T, Rc, erb_run, erb_src,
-                                                                                          gate->valid ? 0 : 1, save);
+                                                                                          gate->valid ? 0 : 1, gate->halo, save);
             DFB_LAUNCH_CHECK();
             return DFB_OK;
         };
@@ -2192,6 +2197,7 @@ struct ChunkIO {
     const struct SpecOut *spec_out = nullptr;
     // runtime gating mode (GateRun): wherever a row gates, its decoders run only on the frames its stages let through
     bool runtime = false;
+    const unsigned char *rt_halo = nullptr;   // per-row GateRun::halo, or null: every row as S.rt_valid says
 };
 
 // Outputs of a spectral call (k_spec_emit): caller row c, output row j of n_out carries frame f0 + j; slot_row maps caller
@@ -2433,7 +2439,7 @@ static int run_chunk(dfb_model *m, dfb_state *st, StreamState &S, const ChunkIO 
                 have_prev ? P.ev_done : nullptr, S.B, io.rows, W0, io.first};
     // the rows gate as the apply kernel (io.ctl: each row's own entry) or k_spec_emit decides
     const bool gates = io.ctl ? io.ctl_gate : (io.lsnr_th != nullptr || (spectral && io.spec_out->gating));
-    GateRun gr{io.ctl, io.links, {0.f, 0.f, 0.f}, 0, S.t_c0, S.t_run, S.rt_valid};
+    GateRun gr{io.ctl, io.links, {0.f, 0.f, 0.f}, 0, S.t_c0, S.t_run, S.rt_valid, io.rt_halo};
     if (io.runtime && gates && c.model_kind != 1) {
         const float *th = spectral ? io.spec_out->th : io.lsnr_th;
         if (!io.ctl) { gr.gate_all = 1; gr.th[0] = th[0]; gr.th[1] = th[1]; gr.th[2] = th[2]; }
@@ -3255,6 +3261,14 @@ struct dfb_stream {
     std::vector<int64_t> slot_first, slot_end;         // absolute first frame; end frame of a closing slot
     int n_act = 0;
     std::vector<int> row_src;                          // per row: its state-slab row at the last call, or -1: a fresh stream
+    // held sessions (dfb_stream_hold_slots; DESIGN.md section 5p): live rows [n_act, n_live) that no call computes
+    std::vector<char> slot_held;
+    std::vector<int64_t> slot_held_frames;             // per slot: frames held since the LSNR head started (its LSNR start)
+    int n_live = 0;
+    int64_t rows_moved = 0;                            // rows k_slot_rows wrote at the last call (dfb_debug_stream_rows_moved)
+    // runtime gating: per slot, whether its decoder tails were kept by its own last DNN call (S.rt_valid of that call)
+    std::vector<char> slot_rt;
+    unsigned char *d_halo = nullptr;                   // per row: take the tails from the halo (GateRun::halo)
     // slot groups (dfb_stream_open_linked, or the fixed channel groups of dfb_stream_set_mask_reduce): per slot the slot of
     // its group's channel 0 (-1 free) and the group's channel count.  A group's rows are contiguous in the active prefix,
     // in channel order.
@@ -3339,7 +3353,10 @@ static void slots_init(dfb_stream *h) {
     h->slot_first.assign(B, 0);
     h->slot_end.assign(B, kOpenEnd);
     h->slot_dir.assign(B, 0);
-    h->n_act = h->B;
+    h->n_act = h->n_live = h->B;
+    h->slot_held.assign(B, 0);
+    h->slot_held_frames.assign(B, 0);
+    h->slot_rt.assign(B, 0);
     h->tab_dirty = true;
     h->slot_lim.assign(B, NAN);
     h->slot_beta.assign(B, NAN);
@@ -3401,6 +3418,7 @@ extern "C" void dfb_stream_free(dfb_stream *h) {
     if (h->d_first) cudaFree(h->d_first);
     if (h->d_grp) cudaFree(h->d_grp);
     if (h->d_ctl) cudaFree(h->d_ctl);
+    if (h->d_halo) cudaFree(h->d_halo);
     if (h->stage_lsnr) cudaFree(h->stage_lsnr);
     if (h->d_slotmap) cudaFree(h->d_slotmap);
     if (h->spec_stage_in) cudaFree(h->spec_stage_in);
@@ -3481,36 +3499,88 @@ extern "C" int64_t dfb_stream_latency_samples(const dfb_stream *h) {
 }
 
 // ---- streaming slots: host bookkeeping.  Device rows follow at the next call (stream_step moves them first, by row_src).
-// the slot becomes free; its row stays in the active prefix until rows_compact
+// the slot becomes free (and not held); its row stays among the live rows until rows_layout
 static void slot_release(dfb_stream *h, int slot) {
     h->slot_row[(size_t)slot] = -1;
     h->slot_grp[(size_t)slot] = -1;
     h->slot_nch[(size_t)slot] = 0;
     h->slot_state[(size_t)slot] = kSlotFree;
+    h->slot_held[(size_t)slot] = 0;
 }
 
-// The rows of freed slots leave the active prefix and the rows behind them close up in order, so every group stays
-// contiguous and in channel order.  A row that moves carries its source row (row_src) along: the next call moves the
-// state-slab rows in one pass (k_slot_rows), however many rows moved.
-static void rows_compact(dfb_stream *h) {
-    int n = 0;
-    for (int r = 0; r < h->n_act; r++) {
+// The live rows' layout: the advancing groups (open or closing, not held) are the prefix [0, n_act), the held groups the
+// rows [n_act, n_live) behind it, each group contiguous and in channel order; the rows of freed slots leave.  A group
+// that lies inside its region keeps its row; the others fill the holes first fit, so a row that leaves the prefix is
+// replaced by one from its end instead of the prefix closing up (the region falls back to packing its groups in order
+// when linked groups fragment the holes).  A row that moves carries its source row (row_src) along: the next call moves
+// the state-slab rows in one pass (k_slot_rows), however many rows moved.
+static void rows_layout(dfb_stream *h) {
+    struct Grp { int row, n; bool held; };
+    std::vector<Grp> grps;
+    int n_adv = 0, n_live = 0;
+    for (int r = 0; r < h->n_live;) {
         const int b = h->row_slot[(size_t)r];
-        if (h->slot_state[(size_t)b] == kSlotFree) continue;
-        h->row_slot[(size_t)n] = b;
-        h->row_src[(size_t)n] = h->row_src[(size_t)r];
-        h->slot_row[(size_t)b] = n++;
+        if (h->slot_state[(size_t)b] == kSlotFree) { r++; continue; }
+        const int n = h->slot_nch[(size_t)b];   // r holds the group's channel 0
+        const bool held = h->slot_held[(size_t)b] != 0;
+        grps.push_back(Grp{r, n, held});
+        if (!held) n_adv += n;
+        n_live += n;
+        r += n;
     }
-    if (n != h->n_act) h->tab_dirty = true;
-    h->n_act = n;
+    std::vector<int> to(grps.size(), -1);   // per group its new first row
+    for (int region = 0; region < 2; region++) {
+        const bool held = region == 1;
+        const int lo = held ? n_adv : 0, hi = held ? n_live : n_adv;
+        std::vector<char> taken((size_t)(hi - lo), 0);
+        for (size_t k = 0; k < grps.size(); k++) {
+            const Grp &g = grps[k];
+            if (g.held != held || g.row < lo || g.row + g.n > hi) continue;
+            to[k] = g.row;
+            std::fill(taken.begin() + (g.row - lo), taken.begin() + (g.row - lo + g.n), (char)1);
+        }
+        bool fits = true;
+        for (size_t k = 0; k < grps.size() && fits; k++) {
+            if (grps[k].held != held || to[k] >= 0) continue;
+            const int n = grps[k].n;
+            int at = -1;
+            for (int q = 0, run = 0; q < hi - lo && at < 0; q++) {
+                run = taken[(size_t)q] ? 0 : run + 1;
+                if (run == n) at = q - n + 1;
+            }
+            if (at < 0) { fits = false; break; }
+            to[k] = lo + at;
+            std::fill(taken.begin() + at, taken.begin() + at + n, (char)1);
+        }
+        if (!fits)
+            for (size_t k = 0, q = (size_t)lo; k < grps.size(); k++)
+                if (grps[k].held == held) { to[k] = (int)q; q += (size_t)grps[k].n; }
+    }
+    const std::vector<int> slot_of(h->row_slot), src_of(h->row_src);
+    bool moved = n_live != h->n_live || n_adv != h->n_act;
+    for (size_t k = 0; k < grps.size(); k++)
+        for (int c = 0; c < grps[k].n; c++) {
+            const int from = grps[k].row + c, r = to[k] + c, b = slot_of[(size_t)from];
+            moved |= r != from;
+            h->row_slot[(size_t)r] = b;
+            h->row_src[(size_t)r] = src_of[(size_t)from];
+            h->slot_row[(size_t)b] = r;
+        }
+    if (moved) h->tab_dirty = true;
+    h->n_act = n_adv;
+    h->n_live = n_live;
 }
 
 // closing slots whose last frame has been output become free: `out_end` is the frame after the last output hop so far
 // (a1 - latency after a process call, a1 after a flush).  The members of a group share their end frame: they leave together.
 static void slots_retire(dfb_stream *h, int64_t out_end) {
+    bool freed = false;
     for (int b = 0; b < h->B; b++)
-        if (h->slot_state[(size_t)b] == kSlotClosing && h->slot_end[(size_t)b] <= out_end) slot_release(h, b);
-    rows_compact(h);
+        if (h->slot_state[(size_t)b] == kSlotClosing && h->slot_end[(size_t)b] <= out_end) {
+            slot_release(h, b);
+            freed = true;
+        }
+    if (freed) rows_layout(h);   // (no row leaves: the layout stands)
 }
 
 static void slot_close(dfb_stream *h, int slot) {
@@ -3521,9 +3591,12 @@ static void slot_close(dfb_stream *h, int slot) {
     h->tab_dirty = true;
 }
 
+static void holds_lift_all(dfb_stream *h);
+
 // After a flush every stream has ended: all slots are free once their tails are out.  Without look-ahead a flush computes
 // nothing and only closes the slots.
 static void slots_close_all(dfb_stream *h) {
+    holds_lift_all(h);
     for (int b = 0; b < h->B; b++) slot_close(h, b);
     slots_retire(h, h->S.a1 - path_latency(h));
     h->slot_ops = true;
@@ -3560,15 +3633,15 @@ static int slot_list(dfb_stream *h, const int64_t *slots, int64_t n) {
 }
 
 // Opens one group per `nch` consecutive listed slots (channel c of a group in its c-th slot), each a fresh stream in rows
-// appended to the active prefix.  The listed slots' old streams (whole groups, by slot_list_check) are dropped without
+// of the active prefix.  The listed slots' old streams (whole groups, by slot_list_check) are dropped without
 // their tails first.  dir: the sessions' direction of the resamplers (0: the handle's rate, 48 kHz on a mixed-rate handle).
 static int slots_open(dfb_stream *h, const int64_t *slots, int64_t n, int64_t nch, int dir = 0) {
     if (int rc = slot_list(h, slots, n)) return rc;
     for (int64_t i = 0; i < n; i++)
         if (h->slot_state[(size_t)slots[i]] != kSlotFree) slot_release(h, (int)slots[i]);
-    rows_compact(h);
+    rows_layout(h);
     for (int64_t i = 0; i < n; i++) {
-        const int b = (int)slots[i], r = h->n_act++;
+        const int b = (int)slots[i], r = h->n_live++;
         h->slot_row[(size_t)b] = r;
         h->row_slot[(size_t)r] = b;
         h->row_src[(size_t)r] = -1;
@@ -3581,7 +3654,10 @@ static int slots_open(dfb_stream *h, const int64_t *slots, int64_t n, int64_t nc
         h->slot_lim[(size_t)b] = h->slot_beta[(size_t)b] = NAN;   // back to the handle's settings
         h->slot_gate[(size_t)b] = -1;
         h->slot_fresh[(size_t)b] = 1;
+        h->slot_rt[(size_t)b] = h->S.rt_valid;
+        h->slot_held_frames[(size_t)b] = 0;
     }
+    rows_layout(h);
     h->tab_dirty = true;
     return DFB_OK;
 }
@@ -3631,6 +3707,50 @@ extern "C" int dfb_stream_close_slots(dfb_stream *h, const int64_t *slots, int64
     for (int64_t i = 0; i < n; i++) slot_close(h, (int)slots[i]);
     slots_retire(h, h->S.a1 - path_latency(h));   // without look-ahead (latency 0) a closed slot is free at once
     return DFB_OK;
+}
+
+// ---- held sessions (DESIGN.md section 5p).  A held session sits in a live row behind the active prefix, which no call
+// computes or writes; after every call its bookkeeping moves forward by the frames the clock advanced (holds_rebase), so
+// that, relative to the clock, its state is what its last advancing call left.
+extern "C" int dfb_stream_hold_slots(dfb_stream *h, const int64_t *slots, int64_t n, int hold) {
+    if (int rc = slot_list_check(h, slots, n)) return rc;
+    for (int64_t i = 0; i < n; i++)
+        if (h->slot_state[(size_t)slots[i]] == kSlotFree) return fail(DFB_ERR_INVALID, "slot %lld is free", (long long)slots[i]);
+    h->slot_ops = true;
+    for (int64_t i = 0; i < n; i++) {
+        const size_t b = (size_t)slots[i];
+        h->slot_held[b] = hold ? 1 : 0;
+        // before a handle's first frame its rows start from a state the first call implies (S.started): a row that sits
+        // that call out gets it written instead, as a freshly opened row
+        if (hold && !h->S.started) h->row_src[(size_t)h->slot_row[b]] = -1;
+    }
+    rows_layout(h);
+    return DFB_OK;
+}
+
+extern "C" int dfb_stream_held_slots(const dfb_stream *h, int8_t *h_held) {
+    if (!h || !h_held) return fail(DFB_ERR_INVALID, "null argument");
+    for (int b = 0; b < h->B; b++) h_held[b] = h->slot_held[(size_t)b] ? 1 : 0;
+    return DFB_OK;
+}
+
+// every hold lifted (a flush ends every session, held ones included)
+static void holds_lift_all(dfb_stream *h) {
+    if (h->n_live == h->n_act) return;
+    std::fill(h->slot_held.begin(), h->slot_held.end(), (char)0);
+    rows_layout(h);
+}
+
+// after a call that moved the clock d frames on: the held sessions' first frame, end frame and settings switch with it
+static void holds_rebase(dfb_stream *h, int64_t d) {
+    if (d == 0 || h->n_live == h->n_act) return;
+    for (int r = h->n_act; r < h->n_live; r++) {
+        const size_t b = (size_t)h->row_slot[(size_t)r];
+        h->slot_first[b] += d;
+        h->slot_held_frames[b] += d;
+        if (h->slot_state[b] == kSlotClosing) h->slot_end[b] += d;
+        h->slot_ctl[b].sw += d;
+    }
 }
 
 // ---- per-slot settings.  A setting is stored per slot; each call resolves every live slot's setting (its own, or the
@@ -3762,19 +3882,20 @@ extern "C" int dfb_stream_slot_groups(const dfb_stream *h, int64_t *h_first) {
     return DFB_OK;
 }
 
-// Row moves of a call: row r takes its state from row_src[r] as the last call left it, or starts fresh (-1).  Two
-// launches of k_slot_rows whatever the number of rows, the scratch rows in the model arena (the chunk that follows reuses
-// it in stream order).
+// Row moves of a call: live row r (held rows included) takes its state from row_src[r] as the last call left it, or starts
+// fresh (-1).  Two launches of k_slot_rows whatever the number of rows, the scratch rows in the model arena (the chunk
+// that follows reuses it in stream order).
 static int slots_move_rows(dfb_stream *h, cudaStream_t s) {
     std::vector<int2> ops;
     int n_mv = 0;
     for (int pass = 0; pass < 2; pass++)   // the moves first, then the fresh rows
-        for (int r = 0; r < h->n_act; r++) {
+        for (int r = 0; r < h->n_live; r++) {
             const int src = h->row_src[(size_t)r];
             if (src != r && (src >= 0) == (pass == 0)) ops.push_back(make_int2(r, src));
         }
     for (const int2 &op : ops) n_mv += op.y >= 0;
-    for (int r = 0; r < h->n_act; r++) h->row_src[(size_t)r] = r;
+    for (int r = 0; r < h->n_live; r++) h->row_src[(size_t)r] = r;
+    h->rows_moved = (int64_t)ops.size();
     if (ops.empty()) return DFB_OK;
     dfb_model *m = h->m;
     size_t off[kStateArrays];
@@ -3847,7 +3968,9 @@ static int stream_tables(dfb_stream *h, int64_t n, bool flush, bool spec, cudaSt
                 h->d_slotmap = nullptr;
                 return fail(DFB_ERR_OOM, "slot table allocation failed");
             }
-            DFB_CUDA(cudaMemcpyAsync(h->d_slotmap, h->slot_row.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, s));
+            std::vector<int> map(h->slot_row);   // held rows carry no frame
+            for (int &r : map) r = r < h->n_act ? r : -1;
+            DFB_CUDA(cudaMemcpyAsync(h->d_slotmap, map.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, s));
         }
         h->tab_dirty = pending;   // such a row reads nothing from the next call on
         h->tab_n = n;
@@ -3860,7 +3983,11 @@ static int stream_tables(dfb_stream *h, int64_t n, bool flush, bool spec, cudaSt
 // Spectral handle (so != null): d_in is [B][n][F] complex, the outputs go to so's buffers, d_out / d_lsnr are null.
 static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, float *d_out, float *d_lsnr, cudaStream_t s,
                        SpecOut *so = nullptr) {
-    if (d_lsnr && h->lsnr_from < 0) h->lsnr_from = h->S.d1;   // from now on every call runs the LSNR head
+    if (d_lsnr && h->lsnr_from < 0) {   // from now on every call runs the LSNR head
+        h->lsnr_from = h->S.d1;
+        // a session's LSNR start is relative to its frames as of now: only the frames it is held from here on shift it
+        std::fill(h->slot_held_frames.begin(), h->slot_held_frames.end(), (int64_t)0);
+    }
     dfb_model *m = h->m;
     dfb_state *st = h->st;
     StreamState &S = h->S;
@@ -3894,6 +4021,7 @@ static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, 
         if (a1n > 0) S.started = true;
         if (d1n > 0) S.dnn_started = true;
         S.n_feat = g.Hf; S.n_mc = kMcTail; S.n_dec = kHalo;
+        holds_rebase(h, a1n - a0);
         slots_retire(h, flush ? a1n : a1n - Ltot);
         return DFB_OK;
     }
@@ -3906,19 +4034,42 @@ static int stream_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, 
     io.lsnr_from = h->lsnr_from;
     io.lsnr_out = d_lsnr;
     io.runtime = (h->gating_mode >= 0 ? h->gating_mode : m->gating_mode) == DFB_GATING_RUNTIME;
+    // a row whose own tails' validity differs from the last DNN call's (a session held since another mode's call) switches
+    // alone: per-row halo flags
+    if (io.runtime) {
+        std::vector<unsigned char> halo((size_t)h->n_act);
+        bool mixed = false;
+        for (int r = 0; r < h->n_act; r++) {
+            const bool v = h->slot_rt[(size_t)h->row_slot[(size_t)r]] != 0;
+            halo[(size_t)r] = v ? 0 : 1;
+            mixed |= v != S.rt_valid;
+        }
+        if (mixed) {
+            if (!h->d_halo && cudaMalloc(&h->d_halo, (size_t)B) != cudaSuccess) {
+                h->d_halo = nullptr;
+                return fail(DFB_ERR_OOM, "gating table allocation failed");
+            }
+            DFB_CUDA(cudaMemcpyAsync(h->d_halo, halo.data(), halo.size(), cudaMemcpyHostToDevice, s));
+            io.rt_halo = h->d_halo;
+        }
+    }
     rc = m->arena.reserve(chunk_bytes_per_stream(m->cfg, st, (int)(d1n - (S.d1 > kHalo ? S.d1 - kHalo : 0)) + 1) * (size_t)h->n_act +
                               (2 << 20));
     if (rc) return rc;
     if (!flush && a1n > a0 && !so) {
-        if (!S.started) DFB_CUDA(cudaMemsetAsync(S.ana_mem, 0, sizeof(float) * B * hop, s));
+        if (!S.started) DFB_CUDA(cudaMemsetAsync(S.ana_mem, 0, sizeof(float) * h->n_act * hop, s));
         io.init_mem = S.ana_mem;
     }
+    const int64_t d1_was = S.d1;
     if ((rc = run_chunk(m, st, S, io, a1n, d1n, e1n, s))) return rc;
     if (!flush && !so) {
         k_carry_hop<<<h->n_act, 128, 0, s>>>(S.ana_mem, d_in, h->d_rows, (n - 1) * hop, hop);
         DFB_LAUNCH_CHECK();
     }
     m->arena.reset();
+    if (S.d1 > d1_was)   // a DNN chunk ran: the advancing rows' tails are as it left them
+        for (int r = 0; r < h->n_act; r++) h->slot_rt[(size_t)h->row_slot[(size_t)r]] = S.rt_valid;
+    holds_rebase(h, a1n - a0);
     slots_retire(h, flush ? a1n : a1n - Ltot);
     return DFB_OK;
 }
@@ -4012,6 +4163,7 @@ static int rate_step(dfb_stream *h, const float *d_in, int64_t n, bool flush, fl
     const int64_t wide = dfb_stream_frame_length(h), B = h->B;
     if (!flush) return rate_pass(h, d_in, n, false, d_out, n * wide, 0, d_lsnr, s);
     const int64_t L = path_latency(h), w = L + 1;
+    holds_lift_all(h);
     for (int b = 0; b < h->B; b++) slot_close(h, b);
     h->slot_ops = true;
     int rc;
@@ -4411,11 +4563,17 @@ static int export_plan(const dfb_stream *h, const int32_t *slots, int n, BlobHea
         if (h->slot_state[(size_t)slots[i]] != kSlotOpen)
             return fail(DFB_ERR_INVALID, "slot %d is %s: only open sessions are exported", slots[i],
                         h->slot_state[(size_t)slots[i]] == kSlotFree ? "free" : "closing");
+    // runtime gating: the sessions' own decoder tails (a held session keeps those of its last advancing call)
+    const bool tails = h->slot_rt[(size_t)slots[0]] != 0;
+    for (int i = 1; i < n; i++)
+        if (eff_gating_mode(h) == DFB_GATING_RUNTIME && (h->slot_rt[(size_t)slots[i]] != 0) != tails)
+            return fail(DFB_ERR_INVALID, "runtime gating: the decoder tails of slot %d %s kept by its last call, those of slot %d %s: "
+                        "export them apart", slots[0], tails ? "were" : "were not", slots[i], tails ? "were not" : "were");
     size_t off[kStateArrays];
     StateLayout lay;
     stream_state_floats(h, off, &lay);
     *hd = BlobHeader{kBlobMagic, kBlobVersion, h->m->fingerprint, h->st->sr, h->st->fft, h->st->hop, h->st->nb_erb,
-                     eff_gating_mode(h), eff_gating_mode(h) == DFB_GATING_RUNTIME && h->S.rt_valid ? 1 : 0, 0, n, 0, {}};
+                     eff_gating_mode(h), eff_gating_mode(h) == DFB_GATING_RUNTIME && tails ? 1 : 0, 0, n, 0, {}};
     for (int a = 0; a < kStateArrays; a++) hd->row_floats[a] = (int64_t)lay.layers[a] * lay.per_row[a];
     ses->clear(); rows->clear();
     int64_t data = 0;   // floats
@@ -4430,7 +4588,9 @@ static int export_plan(const dfb_stream *h, const int32_t *slots, int n, BlobHea
         const int64_t first = h->slot_first[sb];
         BlobSession r{};
         r.age = h->S.a1 - first;
-        r.lsnr_start = h->lsnr_from >= 0 ? h->lsnr_from - first : kNoLsnr;
+        // relative to the session's own frames: lsnr_from is on the handle's clock, which has moved on by the frames the
+        // session was held since then
+        r.lsnr_start = h->lsnr_from >= 0 ? h->lsnr_from - (first - h->slot_held_frames[sb]) : kNoLsnr;
         r.rate = slot_rate_of(h, b); r.channels = nch; r.reduce = nch > 1 ? h->group_reduce : kReduceNone;
         // the settings the session's next call resolves, pinned: its own, or the handle's at this time
         r.lim = std::isnan(h->slot_lim[sb]) ? h->lim : h->slot_lim[sb];
@@ -4471,7 +4631,7 @@ static void header_bytes(const BlobHeader &hd, const std::vector<BlobSession> &s
 // A released export frees its slots at once, without a tail: the sessions live only in the blob.
 static void export_release(dfb_stream *h, const int32_t *slots, int n) {
     for (int i = 0; i < n; i++) slot_release(h, slots[i]);
-    rows_compact(h);
+    rows_layout(h);
     h->slot_ops = true;
 }
 
@@ -4586,7 +4746,7 @@ static int import_plan(dfb_stream *h, const int32_t *slots, int n, const BlobHea
     if (int rc = slot_list_check(h, s64.data(), n)) return rc;
     for (int i = 0; i < n; i++)
         if (h->slot_state[(size_t)slots[i]] != kSlotFree) return fail(DFB_ERR_INVALID, "slot %d is not free", slots[i]);
-    p->idle = h->n_act == 0;
+    p->idle = h->n_live == 0;
     if (!p->idle && !clock_settled(h))
         return fail(DFB_ERR_INVALID, "this handle's clock has not settled since its start or flush: it settles after %d frames "
                     "of calls (8 of halo, %d of look-ahead); import into it then, or into a handle with no live session",
@@ -4624,7 +4784,7 @@ static int import_plan(dfb_stream *h, const int32_t *slots, int n, const BlobHea
     }
     // slab rows: a new row lands in its own slab row unless a pending move still reads that one
     std::vector<char> used((size_t)h->B, 0);
-    for (int r = 0; r < h->n_act; r++)
+    for (int r = 0; r < h->n_live; r++)
         if (h->row_src[(size_t)r] >= 0) used[(size_t)h->row_src[(size_t)r]] = 1;
     const ChunkGeom g = chunk_geom(c);
     p->rows.clear();
@@ -4639,7 +4799,7 @@ static int import_plan(dfb_stream *h, const int32_t *slots, int n, const BlobHea
             nan_l = r.lsnr_start == kNoLsnr ? kMcTail : (int)std::min<int64_t>(kMcTail, std::max<int64_t>(0, r.lsnr_start - t0));
         }
         for (int ch = 0; ch < r.channels; ch++) {
-            const int row = h->n_act + (int)p->rows.size();
+            const int row = h->n_live + (int)p->rows.size();
             int q = row;
             if (used[(size_t)q]) {
                 while (used[(size_t)next]) next++;
@@ -4668,7 +4828,7 @@ static void import_slots(dfb_stream *h, const int32_t *slots, const BlobHeader &
         if (p.idle && r.lsnr_start != kNoLsnr) h->lsnr_from = std::max<int64_t>(0, std::min(h->S.d1, first + r.lsnr_start));
         for (int ch = 0; ch < r.channels; ch++, i++) {
             const size_t b = (size_t)slots[i];
-            const int row = h->n_act++;
+            const int row = h->n_live++;
             h->slot_row[b] = row;
             h->row_slot[(size_t)row] = (int)b;
             h->row_src[(size_t)row] = p.rows[(size_t)i].slab;
@@ -4678,6 +4838,8 @@ static void import_slots(dfb_stream *h, const int32_t *slots, const BlobHeader &
             h->slot_first[b] = first;
             h->slot_end[b] = kOpenEnd;
             h->slot_dir[b] = p.dir[k];
+            h->slot_rt[b] = hd.gate_tails != 0;
+            h->slot_held_frames[b] = 0;
             if (ctl) {
                 h->slot_lim[b] = r.lim; h->slot_beta[b] = r.beta;
                 h->slot_gate[b] = (signed char)(r.gate ? 1 : 0);
@@ -4695,6 +4857,7 @@ static void import_slots(dfb_stream *h, const int32_t *slots, const BlobHeader &
     // clock_settle moves d1 back to a1 - Lmax on a handle that was flushed (a flush leaves d1 = a1), and an LSNR request
     // after the flush set lsnr_from to that d1: the LSNR head must start no later than the imported sessions' next frame
     if (p.idle && ses.size() && ses[0].lsnr_start == kNoLsnr && h->lsnr_from > h->S.d1) h->lsnr_from = h->S.d1;
+    rows_layout(h);   // behind held rows, the new rows move into the active prefix
     h->tab_dirty = true;
     h->slot_ops = true;
 }
@@ -4811,6 +4974,13 @@ extern "C" int dfb_stream_process_spec_host(dfb_stream *h, const float *h_spec, 
     if (h_stage) DFB_CUDA(cudaMemcpyAsync(h_stage, sg, rows, cudaMemcpyDeviceToHost, s));
     DFB_CUDA(cudaStreamSynchronize(s));
     if (flush) slots_close_all(h);
+    return DFB_OK;
+}
+
+// debug aid: the state-slab rows k_slot_rows wrote at the handle's last call (moved or started fresh)
+extern "C" int dfb_debug_stream_rows_moved(const dfb_stream *h, int64_t *n) {
+    if (!h || !n) return fail(DFB_ERR_INVALID, "null argument");
+    *n = h->rows_moved;
     return DFB_OK;
 }
 

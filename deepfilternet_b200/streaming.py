@@ -502,6 +502,23 @@ class DfStream:
         check(_lib.lib().dfb_stream_slot_states(self._h, out.ctypes.data_as(C.POINTER(C.c_int32))))
         return out
 
+    def hold(self, slots, held: bool = True) -> None:
+        """Hold the listed live slots (``held=False``: lift their hold) from the next call on: a held session sits out every
+        call, as if the call had not happened.  Its input rows are ignored, its output rows are zeros and its LSNR NaN; it
+        keeps its slot, state, settings and age, and continues bit for bit in the first call after the hold is lifted, so
+        that its outputs over the calls it advanced in equal ``DfStream(batch=1)`` fed the same audio in those calls' sizes.
+        ``open``, ``reset``, ``export(release=True)`` and ``flush`` lift holds; ``flush`` ends held sessions as their own
+        flush would.  A group is held as a unit: list all of its members (dfb_stream_hold_slots).  ValueError for a
+        malformed slot list; DfbError for a free slot, part of a group or a handle with fixed channel groups."""
+        a = slot_list(slots, self.batch)
+        check(_lib.lib().dfb_stream_hold_slots(self._h, a.ctypes.data_as(C.POINTER(C.c_int64)), a.size, int(bool(held))))
+
+    def held_slots(self) -> np.ndarray:
+        """bool [batch]: True per held slot (``hold``)."""
+        out = np.zeros(self.batch, np.int8)
+        check(_lib.lib().dfb_stream_held_slots(self._h, out.ctypes.data_as(C.POINTER(C.c_int8))))
+        return out.astype(bool)
+
     def slot_groups(self) -> np.ndarray:
         """int64 [batch]: per slot, the slot holding channel 0 of its group (the slot itself for a one-channel session),
         -1 for a free slot."""

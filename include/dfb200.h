@@ -433,6 +433,37 @@ int dfb_stream_open_linked(dfb_stream *s, const int64_t *slots, int64_t n);
 /* h_first i64[B] (host): per slot, the slot holding channel 0 of its group (the slot itself for one channel), -1 if free */
 int dfb_stream_slot_groups(const dfb_stream *s, int64_t *h_first);
 
+/* Held sessions (DESIGN.md section 5p): a session that has no audio for a call (jitter, discontinuous transmission, a
+ * participant on hold) sits the call out, as a libdeepfilter stream that df_process_frame is not called on.  A held
+ * session behaves, for every call it is held through, as if that call had not happened: its state, age, settings, LSNR
+ * start and drain do not change, its input rows are ignored, its output rows are zeros and its LSNR entries NaN (on a
+ * spectral handle NaN rows with stage -1), as a free slot's.  It stays live: dfb_stream_slot_states reports it open or
+ * closing, and it keeps its slot.  A session's outputs over the calls it advanced in, followed by its drain or flush,
+ * equal a single-stream handle fed the same audio in those calls' sizes, bit for bit.
+ *   dfb_stream_hold_slots   hold != 0 holds the listed live slots from the next call on, until hold == 0 lifts it.
+ *                           Holding a held slot or lifting an unheld one does nothing.  `slots` as for
+ *                           dfb_stream_open_slots; a free slot, or part of a linked group, is DFB_ERR_INVALID; a handle
+ *                           with fixed channel groups DFB_ERR_UNSUPPORTED.  A refused call changes nothing.  Holding is a
+ *                           slot operation (dfb_stream_set_sample_rate, dfb_stream_add_slot_rate, dfb_stream_set_mask_reduce).
+ *   dfb_stream_held_slots   h_held i8[B] (host): 1 per held slot, else 0.
+ * Every process entry point respects holds: device, host, _lsnr, spectral, resampled and mixed-rate.
+ * Close while held: the session closes at the end of the input it has been fed and drains only in calls it advances in.
+ * Settings made while held (dfb_stream_set_atten_lim, _post_filter_beta, _lsnr_thresholds_slots) take effect from the first
+ * frame whose output starts in the first call the session advances in.  Holds are lifted by open / open_linked over the
+ * slot, dfb_stream_reset, a released export and flush, which ends every session, held ones included, each exactly as its
+ * own flush would; an import lands its sessions not held.  Export of a held session (snapshot or release) gives the blob
+ * it would have given just before the hold.  DFB_GATING_RUNTIME: a held session keeps its decoder tails and whether its
+ * last call kept them; if that call ran in the other gating mode it switches alone, as a handle does (DESIGN.md 5l).  An
+ * export lists sessions whose tails agree (else DFB_ERR_INVALID).  DeepFilterNet2 LSNR rows: when the handle's LSNR output
+ * first starts while a session is held, that session's first LSNR call after the hold may differ in its first df_lookahead
+ * hops (NaN for a value), as after an import; its audio is exact.  Only the advancing rows are computed, so a held session
+ * costs no compute; a change of hold state moves at most the rows whose state changed plus as many others, in the same two
+ * row-move launches as open and close, at the next call. */
+int dfb_stream_hold_slots(dfb_stream *s, const int64_t *slots, int64_t n, int hold);
+int dfb_stream_held_slots(const dfb_stream *s, int8_t *h_held);
+/* Debug aid: the state-slab rows the handle's last call moved or started fresh before computing (its row-move kernel) */
+int dfb_debug_stream_rows_moved(const dfb_stream *s, int64_t *n);
+
 /* Per-slot settings (capi.rs df_set_atten_lim / df_set_post_filter_beta, which each change one stream between two frames).
  * `slots` is validated as for dfb_stream_open_slots; naming a free slot is DFB_ERR_INVALID, an open or closing one is fine
  * (a closing slot's setting covers the rest of its tail).  A refused call changes nothing.  Linked handles:
